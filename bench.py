@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/sec of Llama-3.1-8B bf16 on B200 (BASELINE.json metric).
+"""bench.py -- decode tokens/sec of Llama-3.1-8B bf16 on one H100 (BASELINE.json metric).
 
 Default workload (SURVEY.md 8d, BASELINE.json configs[1]): random-init weights of the 8B architecture, the
 fixed 8-token synthetic prompt, SequenceLength 136 -> one prefill call (S=8) that yields token #1 plus 127
@@ -22,9 +22,13 @@ evaluated in the matching order: the reference's order at N=1, per-shard referen
 shards under tensor parallelism); LNB_ACC_FAST is timed and parity-checked beside it under `other_acc_mode` at
 every N.  --acc fast swaps the two roles.
 
-Other BASELINE configs (not driver-run; results are committed under profiles/):
-  --config prefill2048   configs[2]: one S=2048 prompt-processing call on the tcgen05 GEMM path (tokens/s)
+Other BASELINE configs:
+  --config prefill2048   configs[2]: one S=2048 prompt-processing call on the tensor-core (wgmma) GEMM path (tokens/s)
   --config batch8        configs[4]: 8 concurrent prompts, 128-token decode, one pass over the weights per step
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (the generated token ids; prefill2048: the next
+token and the last row's logits) as DIR/<name>.npy (float64), so that two builds can be compared output for output: the inputs
+are fixed by seeds and do not change run to run.
 
 `--impl reference` times only the CPU restatement (the Go toolchain does not exist in this image, so the reference
 binary itself cannot run; see DESIGN.md).  Multi-GPU (torchrun, one rank per GPU): tensor parallel, "strong".
@@ -48,11 +52,13 @@ METRIC = "decode tokens/sec Llama-3.1-8B bf16"
 
 
 def load_peaks():
+    """peak HBM GB/s and dense bf16 TFLOP/s: MEASURED_PEAKS.json when a measurement of this card exists, else NVIDIA's data
+    sheet for the H100 SXM (3.35 TB/s, 989 TFLOP/s at up to 700 W)"""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return float(d["hbm_gbs"]), float(d.get("bf16_tflops", 1590.0)), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return float(d["hbm_gbs"]), float(d.get("bf16_tflops", 989.0)), "measured"
+    return 3350.0, 989.0, "H100 SXM data sheet"
 
 
 class ClockSampler(threading.Thread):
@@ -310,6 +316,16 @@ class Env:
             self.dist.destroy_process_group()
 
 
+def dump_outputs(a, **arrays):
+    """--dump-outputs: the arrays the timed path returned in its last timed step, DIR/<name>.npy in float64 (at most 1 MB)"""
+    if not a.dump_outputs:
+        return
+    import numpy as np
+    os.makedirs(a.dump_outputs, exist_ok=True)
+    for name, arr in arrays.items():
+        np.save(os.path.join(a.dump_outputs, name + ".npy"), np.ascontiguousarray(arr, np.float64))
+
+
 def acc_code(L, name):
     return L._capi.LNB_ACC_FAST if name == "fast" else L._capi.LNB_ACC_STRICT
 
@@ -366,7 +382,7 @@ def run_decode(a):
         launches = ctx.launch_count() - launches0
         assert gen_k == gen, "generation is not reproducible run to run"
         dec_ms, wall = env.max_over_ranks(dec_ms, wall)
-        return dict(ctx=ctx, tokens=gen, dec_ms=dec_ms, wall=wall, pre_s=pre_s, graphed=graphed, clocks=clocks, launches=launches,
+        return dict(ctx=ctx, tokens=gen_k, dec_ms=dec_ms, wall=wall, pre_s=pre_s, graphed=graphed, clocks=clocks, launches=launches,
                     value=n_steps * N_DECODE / (dec_ms / 1e3), engine=ctx.uses_engine())
 
     try:
@@ -380,6 +396,8 @@ def run_decode(a):
             raise
     ctx = arm["ctx"]
     gen_tokens, value = arm["tokens"], arm["value"]
+    if rank == 0:
+        dump_outputs(a, tokens=np.array(gen_tokens, np.float64))
     stop_hit = any(t in L.synth.STOP_IDS for t in gen_tokens)
 
     # ---- roofline of the dominant kernel (w1|w3 GEMV), timed alone ----------------------------
@@ -403,7 +421,7 @@ def run_decode(a):
            "kernel chain: one launch per projection, the w1|w3 GEMV launched back to back over all 32 layers' weights"
     roofline = {"bound": "hbm", "kernel": "w1|w3 GEMV (rmsnorm prologue, SwiGLU epilogue), acc=%s" % head, "measured_as": path,
                 "achieved": dom["gbs"], "peak": env.peak_hbm, "unit": "GB/s", "frac": round(dom["gbs"] / env.peak_hbm, 4),
-                "traffic": traffic, "traffic_source": traffic_src, "peak_kind": env.peak_kind + " (burst copy bandwidth)",
+                "traffic": traffic, "traffic_source": traffic_src, "peak_kind": env.peak_kind + (" (burst copy bandwidth)" if env.peak_kind == "measured" else ""),
                 "bytes_per_launch": dom["bytes"], "us_per_launch": dom["us"]}
     per_gpu_bytes = (13_958_643_712 + 1_050_673_152) / world + 524_288 + 16_384 + 131_072 / world * 72
     step_s = arm["dec_ms"] / 1e3 / (a.steps * N_DECODE)
@@ -529,7 +547,7 @@ def run_decode(a):
                        "parallelism": "tp%d" % world, "acc": head, "decode_path": "engine" if arm["engine"] else "kernel chain",
                        "cuda_graph": bool(arm["graphed"]) and not arm["engine"],
                        "collective": collective,
-                       "l2": "working set 15 GB per token >> 126 MB L2 (no flush needed)",
+                       "l2": "working set 15 GB per token >> 50 MB L2 (no flush needed)",
                        "stop_id_generated": stop_hit, "notes": notes},
             "decode_ms_per_token": round(arm["dec_ms"] / (a.steps * N_DECODE), 4),
             "prefill_ms": round(1e3 * arm["pre_s"] / a.steps, 3),
@@ -544,7 +562,7 @@ def run_decode(a):
 
 
 def run_prefill(a):
-    """BASELINE configs[2]: one Forward of S=2048 prompt tokens on 1xB200 (tcgen05 GEMM path, LNB_ACC_FAST)."""
+    """BASELINE configs[2]: one Forward of S=2048 prompt tokens on one H100 (tensor-core GEMM path, LNB_ACC_FAST)."""
     env = Env(a)
     np, torch, L = env.np, env.torch, env.L
     if env.world != 1:
@@ -569,6 +587,11 @@ def run_prefill(a):
     clocks = sampler.summary()
     launches = ctx.launch_count() - l0
     per = wall / a.steps
+    if a.dump_outputs:
+        # the timed call hands back only the token; the same call once more, with the same inputs, also returns its logits
+        nxt2, lg = env.tf.forward_argmax(ctx, toks, 0, want_logits="last")
+        assert int(nxt2) == int(nxt), "prefill is not reproducible call to call"
+        dump_outputs(a, next_token=np.array([nxt], np.float64), last_row_logits=np.asarray(lg[0], np.float64))
     # algorithmic flops of what this call computes: every projection for all S rows, the LM head for the last row only,
     # causal attention (QK^T and PV over the S(S+1)/2 visible (query, key) pairs of 32 heads x 32 layers, 128 MACs each)
     flops = 2 * 6_979_321_856 * S + 2 * 128256 * 4096 + 32 * 32 * (S * (S + 1) // 2) * 128 * 2 * 2
@@ -591,7 +614,7 @@ def run_prefill(a):
             "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
             "config": {"workload": "Llama-3.1-8B bf16 random-init, one prefill call of S=2048 random token ids at position 0, "
                                    "last-row LM head + greedy argmax (BASELINE.json configs[2])", "acc": "fast (tensor-core order)",
-                       "l2": "weights 15 GB >> 126 MB L2"},
+                       "l2": "weights 15 GB >> 50 MB L2"},
             "gpu_launches": int(launches), "clocks": clocks,
             "roofline": {"bound": "tensor", "achieved": round(flops / per / 1e12, 1), "peak": env.peak_tf, "unit": "TFLOP/s",
                          "frac": round(flops / per / 1e12 / env.peak_tf, 4), "traffic": None,
@@ -643,6 +666,8 @@ def run_batch8(a):
             tot += dt
         env.barrier()
         (tot,) = env.max_over_ranks(tot)
+        if name == a.acc and env.rank == 0:
+            dump_outputs(a, tokens=np.array(toks, np.float64))
         res[name] = dict(value=B * N_DECODE * a.steps / tot, ms=1e3 * tot / (a.steps * N_DECODE), toks=toks,
                          clocks=sampler.summary() if sampler else None, launches=ctx.launch_count() - l0)
         ctx.close()
@@ -697,6 +722,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline / parity legs")
     ap.add_argument("--parity-tokens", type=int, default=128, help="generated tokens compared with the oracle (teacher-forced)")
     ap.add_argument("--parity", action="store_true", help="prefill2048: also run the oracle's S=2048 prefill (minutes of CPU)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float64)")
     a = ap.parse_args()
     if a.impl == "reference":
         return run_reference(a)

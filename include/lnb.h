@@ -1,5 +1,5 @@
 /*
- * lnb.h -- C-ABI of liblnb.so: the B200 (sm_100a) forward path that sits under the
+ * lnb.h -- C-ABI of liblnb.so: the H100 (sm_90a) forward path that sits under the
  * Go API of adalkiran/llama-nuts-and-bolts.
  *
  * The reference has no FFI or plugin interface (it is pure Go, CPU only); the

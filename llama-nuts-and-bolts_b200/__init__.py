@@ -1,4 +1,4 @@
-"""llama-nuts-and-bolts_b200 -- B200 (sm_100a) forward path behind the Go API of
+"""llama-nuts-and-bolts_b200 -- H100 (sm_90a) forward path behind the Go API of
 adalkiran/llama-nuts-and-bolts.
 
 Layout

@@ -136,7 +136,7 @@ struct lnb_model {
   ncclComm_t comm = nullptr;
   void* staging = nullptr;
   size_t staging_bytes = 0;
-  int sm_count = 148;
+  int sm_count = 132;
 };
 
 static int parse_name(const lnb_model* m, const char* name, int* kind, int* layer) {
@@ -795,8 +795,8 @@ extern "C" int lnb_model_finalize(lnb_model* m) {
 // itself: ONE CTA per SM (>113 KB of shared memory each) holding 1, 2 or 4 chain warps (warps 1..4
 // sit on SMSPs 1,2,3,0; the producer warp 0 sleeps on its mbarrier), picked from N so that the grid
 // stays close to one wave.  Two chain warps on one scheduler run at half speed each.
-using CfgS1 = GemvCfg<32, 1, 1, 512, 3>;    // N <= 32*148 rows
-using CfgS1M = GemvCfg<64, 1, 1, 512, 3>;   // N <= 64*148
+using CfgS1 = GemvCfg<32, 1, 1, 512, 3>;    // N <= 32*kWaveSMs rows
+using CfgS1M = GemvCfg<64, 1, 1, 512, 3>;   // N <= 64*kWaveSMs
 using CfgS1W = GemvCfg<128, 1, 1, 256, 3>;  // larger N (w1|w3, LM head): several waves, HBM-bound
 using CfgS2 = GemvCfg<32, 1, 2, 256, 4>;
 using CfgS8 = GemvCfg<32, 1, 8, 256, 4>;
@@ -806,6 +806,7 @@ using CfgF2 = GemvCfg<32, 8, 2, 256, 4>;
 using CfgF8 = GemvCfg<32, 8, 8, 256, 4>;
 
 static const size_t kMaxSmem = 227 * 1024;
+static const int kWaveSMs = 132;   // H100 SXM: one wave of one-CTA-per-SM GEMV blocks
 
 struct Launcher {
   cudaStream_t stream;
@@ -879,15 +880,15 @@ static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total) {
     }
     int rc;
     if (strict) {
-      if (mb == 1 && p.N > 64 * 148 && p.N % 128 == 0 && CfgS1W::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgS1W, PRO, EPI>(L, p);
-      else if (mb == 1 && p.N > 32 * 148 && p.N % 64 == 0 && CfgS1M::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgS1M, PRO, EPI>(L, p);
+      if (mb == 1 && p.N > 64 * kWaveSMs && p.N % 128 == 0 && CfgS1W::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgS1W, PRO, EPI>(L, p);
+      else if (mb == 1 && p.N > 32 * kWaveSMs && p.N % 64 == 0 && CfgS1M::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgS1M, PRO, EPI>(L, p);
       else if (mb == 1) rc = launch_gemv_cfg<CfgS1, PRO, EPI>(L, p);
       else if (mb == 8) rc = launch_gemv_cfg<CfgS8, PRO, EPI>(L, p);
       else rc = launch_gemv_cfg<CfgS2, PRO, EPI>(L, p);
     } else {
       if (mb == 8) rc = launch_gemv_cfg<CfgF8, PRO, EPI>(L, p);
       else if (mb == 2) rc = launch_gemv_cfg<CfgF2, PRO, EPI>(L, p);
-      else if (p.N <= 32 * 148 && CfgF1L::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgF1L, PRO, EPI>(L, p);
+      else if (p.N <= 32 * kWaveSMs && CfgF1L::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgF1L, PRO, EPI>(L, p);
       else rc = launch_gemv_cfg<CfgF1, PRO, EPI>(L, p);
     }
     if (rc) return rc;
@@ -917,7 +918,7 @@ static int launch_simple(const Launcher& L, void (*kern)(Args...), dim3 grid, di
 // scan, 3 = one-pass predict / fold / walk (both seqsum.cuh; need a row length that fits seq_scan_shape).
 // algo 0 = the model path's choice: LNB_RMS_ALGO=chain|scan|seg, else kRmsDefaultAlgo.
 enum { RMS_AUTO = 0, RMS_CHAIN = 1, RMS_SCAN = 2, RMS_SEG = 3, RMS_ENGINE = 4 };   // 4 = the decode engine's in-CTA variant (engine.cuh)
-static const int kRmsDefaultAlgo = RMS_SEG;  // measured: 209 tok/s vs 195 (chain) vs 171 (iterative scan), STRICT 8B decode
+static const int kRmsDefaultAlgo = RMS_SEG;  // the fewest dependent steps of the three
 static int rms_default_algo() {
   static const int a = [] {
     const char* e = getenv("LNB_RMS_ALGO");
@@ -1106,7 +1107,6 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
   CU(cudaFuncSetAttribute(sdpa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   CU(cudaFuncSetAttribute(sdpa_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SP_SMEM));
   CU(cudaFuncSetAttribute(sdpa_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM));
-  CU(cudaFuncSetAttribute(sdpa_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SX_SMEM));
   lnb_session* s = new lnb_session();
   s->m = m;
   s->seq_len = seq_len;
@@ -1343,10 +1343,9 @@ static bool engine_probe(lnb_session* s) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   auto no = [&](const char* why) { s->eng_state = -1; s->eng_why = why; return false; };
-  // Default (measured on B200, profiles/r02_*): the engine wins wherever launch count or the serial order dominates --
-  // LNB_ACC_STRICT at every N (213 vs 207, 325 vs 282, 449 vs 352 tokens/s at 1 / 2 / 8 GPUs) and every host-driven loop --
-  // and ties with the kernel chain in LNB_ACC_FAST (308 vs 330 at 1 GPU, 501 vs 484 at 2, 774 vs 800 at 8).  It is the
-  // default except for single-GPU FAST sessions; LNB_ENGINE=1 / 0 forces it on / off.
+  // Default: the engine is meant for where launch count or the serial order dominates -- LNB_ACC_STRICT at every N and
+  // every host-driven loop; in LNB_ACC_FAST it competes with the kernel chain.  It is the default except for single-GPU
+  // FAST sessions; LNB_ENGINE=1 / 0 forces it on / off.
   const char* e = getenv("LNB_ENGINE");
   if (e && !strcmp(e, "0")) return no("LNB_ENGINE=0");
   // single-sequence steps of single-GPU FAST sessions stay on the kernel chain by default (the batch engine does not care)
@@ -1416,11 +1415,6 @@ static const double* exp_table_device() {
 static bool sdpa_tc_enabled() {
   const char* e = getenv("LNB_SDPA_TC");
   return !(e && !strcmp(e, "0"));
-}
-// default: the software-pipelined form (sdpa_tc2_kernel); LNB_SDPA_TC=1: the serial form (sdpa_tc_kernel)
-static bool sdpa_tc_pipelined() {
-  const char* e = getenv("LNB_SDPA_TC");
-  return !(e && !strcmp(e, "1"));
 }
 static int eng_kt(int mode, int N, int K, int G) {
   const int per = (N / 8 + G - 1) / G;                      // most panels one CTA owns
@@ -1562,7 +1556,7 @@ static int engine_launch(lnb_session* s, int n_steps, bool advance) {
   }
   P.err_host = s->h_err;
   {
-    // L2 prefetch per CTA and projection beyond the ring: 148 x 256 KB = 37 MB of the 126 MB L2 by default (LNB_ENGINE_PF_KB, 0 = off)
+    // L2 prefetch per CTA and projection beyond the ring: 132 x 256 KB = 33 MB of the 50 MB L2 when enabled (LNB_ENGINE_PF_KB, 0 = off)
     static const int pf_kb = [] { const char* e = getenv("LNB_ENGINE_PF_KB"); return e ? atoi(e) : 0; }();
     P.pf_window = pf_kb > 0 ? (unsigned int)pf_kb * 1024u : 0u;
   }
@@ -1642,10 +1636,12 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
     CU(cudaMemset(s->bx, 0, (size_t)a.dim * 16)); CU(cudaMemset(s->bh1, 0, (size_t)a.dim * 16));
     CU(cudaMemset(s->bq, 0, (size_t)m->q_l * 16)); CU(cudaMemset(s->bo, 0, (size_t)m->q_l * 16));
     CU(cudaMemset(s->bm, 0, (size_t)m->ffn_l * 16)); CU(cudaMemset(s->bxn, 0, (size_t)a.dim * 16));
-    // FAST: the tensor-core form (every K a multiple of 16; LNB_BATCH_TC=0 keeps the FMA-pipe kernel)
+    // FAST: the FMA-pipe kernel by default -- on an H100 (3.35 TB/s) it keeps up with the weight stream at 8 rows and beat
+    // the tensor-core form, 880 vs 602 tokens/s (bench.py --config batch8 --acc fast, H100 SXM 700 W); LNB_BATCH_TC=1 selects
+    // the tensor-core form (every K a multiple of 16)
     {
       const char* e2 = getenv("LNB_BATCH_TC");
-      s->batch_tc = s->mode != LNB_ACC_STRICT && !(e2 && !strcmp(e2, "0")) && a.dim % 16 == 0 && m->q_l % 16 == 0 && m->ffn_l % 16 == 0;
+      s->batch_tc = s->mode != LNB_ACC_STRICT && (e2 && !strcmp(e2, "1")) && a.dim % 16 == 0 && m->q_l % 16 == 0 && m->ffn_l % 16 == 0;
     }
     if (s->mode == LNB_ACC_STRICT) CU(cudaFuncSetAttribute(batch_engine_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, ENG_SMEM));
     else if (s->batch_tc) CU(cudaFuncSetAttribute(batch_engine_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, BT_SMEM));
@@ -1855,7 +1851,7 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
           p.out_f32 = s->part;
           if ((rc = launch_gemv<PRO_PLAIN, EPI_F32RAW>(L, mode, p, S))) return rc;
           NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
-          if ((rc = launch_simple(L, resid_from_f32_kernel, dim3(std::min(148, (S * a.dim + 255) / 256)), dim3(256), 0,
+          if ((rc = launch_simple(L, resid_from_f32_kernel, dim3(std::min(kWaveSMs, (S * a.dim + 255) / 256)), dim3(256), 0,
                                   (const float*)s->part, (const uint16_t*)s->x, s->h1, (int64_t)S * a.dim)))
             return rc;
         }
@@ -1886,7 +1882,7 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
           p.out_f32 = s->part;
           if ((rc = launch_gemv<PRO_PLAIN, EPI_F32RAW>(L, mode, p, S))) return rc;
           NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
-          if ((rc = launch_simple(L, resid_from_f32_kernel, dim3(std::min(148, (S * a.dim + 255) / 256)), dim3(256), 0,
+          if ((rc = launch_simple(L, resid_from_f32_kernel, dim3(std::min(kWaveSMs, (S * a.dim + 255) / 256)), dim3(256), 0,
                                   (const float*)s->part, (const uint16_t*)s->h1, s->x, (int64_t)S * a.dim)))
             return rc;
         }
@@ -1934,7 +1930,7 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
 }
 
 // Prompt processing on the tensor cores (LNB_ACC_FAST, S >= 32): the same forward pass as
-// enqueue_forward with every projection as a tcgen05 GEMM (gemm_tc.cuh) and the elementwise steps
+// enqueue_forward with every projection as a tensor-core GEMM (gemm_tc.cuh) and the elementwise steps
 // as separate memory-bound kernels that write the next GEMM's X8 operand directly.
 static bool forward_tc_ok(const lnb_session* s, int S) {
   const lnb_model* m = s->m;
@@ -1978,13 +1974,7 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
     if ((rc = launch_simple(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
                             a.head_dim, s->ck[l] + tc_cache_off, s->cv[l] + tc_cache_off, (const float*)m->cis, pos_ptr, S)))
       return rc;
-    if (a.head_dim == SP_HD && exp_tab && sdpa_tc_pipelined()) {
-      if ((rc = launch_simple(L, sdpa_tc2_kernel, dim3(m->q_l / a.head_dim, (S + 127) / 128), dim3(256), (size_t)SX_SMEM,
-                              (const uint16_t*)s->q, m->q_l, (const uint16_t*)(s->ck[l] + tc_cache_off),
-                              (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l, a.n_heads / a.n_kv_heads, s->o8, m->q_l, pos_ptr, S, scale,
-                              exp_tab)))
-        return rc;
-    } else if (a.head_dim == SP_HD && exp_tab) {
+    if (a.head_dim == SP_HD && exp_tab) {
       if ((rc = launch_simple(L, sdpa_tc_kernel, dim3(m->q_l / a.head_dim, (S + 127) / 128), dim3(256), (size_t)ST_SMEM,
                               (const uint16_t*)s->q, m->q_l, (const uint16_t*)(s->ck[l] + tc_cache_off),
                               (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l, a.n_heads / a.n_kv_heads, s->o8, m->q_l, pos_ptr, S, scale,
@@ -2637,7 +2627,7 @@ static int op_finish() {
   CU(cudaDeviceSynchronize());
   return 0;
 }
-static int grid_for(int64_t n) { return (int)std::min<int64_t>(148 * 8, (n + 255) / 256); }
+static int grid_for(int64_t n) { return (int)std::min<int64_t>(kWaveSMs * 8, (n + 255) / 256); }
 
 extern "C" int lnb_op_linear_bf16(const uint16_t* x, const uint16_t* w, uint16_t* out, int S, int K, int N, int acc_mode) {
   OpScope scope_;
@@ -2649,7 +2639,7 @@ extern "C" int lnb_op_linear_bf16(const uint16_t* x, const uint16_t* w, uint16_t
   H2D(dx, x, xb); H2D(dw, w, wb);
   const bool tileable = (N % 16 == 0) && (K % 8 == 0) && (CfgF1::smem_bytes(K) <= kMaxSmem);
   if (acc_mode == LNB_ACC_FAST && tc_eligible(S, N, K)) {
-    // prompt-sized inputs: tcgen05 tensor-core tiles (hardware accumulation order)
+    // prompt-sized inputs: wgmma tensor-core tiles (hardware accumulation order)
     const int Mpad = (S + TC_BM - 1) / TC_BM * TC_BM;
     OPBUF(dwp, wb); OPBUF(dx8, (size_t)Mpad * K * 2);
     retile_kernel<<<grid_for((int64_t)N * K / 8), 256>>>(dw.as<uint16_t>(), K, 0, 0, N, K, dwp.as<uint16_t>(), 0, 1);
@@ -2803,12 +2793,7 @@ extern "C" int lnb_op_attention_bf16(const uint16_t* q, const uint16_t* cache_k,
     OPBUF(d8, (size_t)Mpad * n_heads * hd * 2); OPBUF(dpos, 16);
     CU(cudaMemset(dpos.p, 0, 16));
     const double* exp_tab = (sdpa_tc_enabled() && S >= 32) ? exp_table_device() : nullptr;
-    if (exp_tab && sdpa_tc_pipelined()) {
-      CU(cudaFuncSetAttribute(sdpa_tc2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SX_SMEM));
-      sdpa_tc2_kernel<<<dim3(n_heads, (S + 127) / 128), 256, SX_SMEM>>>(dq.as<uint16_t>(), n_heads * hd, dk.as<uint16_t>(), dv.as<uint16_t>(),
-                                                                        n_kv * hd, n_heads / n_kv, d8.as<uint16_t>(), n_heads * hd,
-                                                                        dpos.as<int32_t>(), S, f, exp_tab);
-    } else if (exp_tab) {
+    if (exp_tab) {
       CU(cudaFuncSetAttribute(sdpa_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM));
       sdpa_tc_kernel<<<dim3(n_heads, (S + 127) / 128), 256, ST_SMEM>>>(dq.as<uint16_t>(), n_heads * hd, dk.as<uint16_t>(), dv.as<uint16_t>(),
                                                                        n_kv * hd, n_heads / n_kv, d8.as<uint16_t>(), n_heads * hd,

@@ -1,4 +1,4 @@
-// common.cuh -- shared device helpers for liblnb.so (sm_100a only).
+// common.cuh -- shared device helpers for liblnb.so (sm_90a only).
 //
 // bf16 <-> f32 follow the reference exactly: widening is a 16-bit shift, narrowing
 // is TRUNCATION (src/dtype/bfloat16.go:19-21,59-61), never round-to-nearest.

@@ -11,7 +11,7 @@
 //   * the step is a PHASE LIST in device memory (EnginePhase[]: projection, attention, all-reduce, argmax exchange);
 //     every CTA walks the same list, phases are separated by a grid barrier (one atomic + one spin per CTA);
 //   * every projection's rows are split STATICALLY and evenly over the CTAs at 8-row panel granularity
-//     (3584 panels of w1|w3 over 148 CTAs = 24 or 25 each: balance 0.97 instead of 0.76);
+//     (3584 panels of w1|w3 over 132 CTAs = 27 or 28 each: balance 0.97);
 //   * warp 0 of every CTA is a bulk-copy producer that walks the phase list AHEAD of the consumers: weights do not
 //     depend on activations, so while the consumers wait at a grid barrier (or for a peer GPU) the ring already
 //     fills with the next projection's first tiles -- no ramp;
@@ -120,7 +120,7 @@ __host__ __device__ inline void eng_split(int P, int b, int G, int* lo, int* hi)
 // tile of 1 panel at kt = 256 would move 4 KB per stage and crawl at the ring's latency (4 stages x 4 KB per ~1.2 us).
 // FAST only: the STRICT chain tiles are compile-time unrolled for kt <= 512.
 __host__ __device__ inline int eng_tile_kt(int ks, int np, int K, int kt, int stage_bytes) {
-  if (ks == 1 || true) return kt;   // (scaling measured slower on B200: kept for the record, disabled)
+  if (ks == 1 || true) return kt;   // (k-tile scaling: kept for the record, disabled)
   while (kt * 2 <= K && kt * 2 <= 2048 && np * (kt * 2) * 16 <= stage_bytes && K % (kt * 2) == 0) kt *= 2;
   return kt;
 }

@@ -21,17 +21,15 @@
 // Per sequence the arithmetic is that of its own S=1 Forward (src/model/llamatransformer.go:145-180), expression for
 // expression: STRICT results are bit-identical to independent oracle contexts (tests/test_gpu_model.py, tools/tp_check.py).
 //
-// LNB_ACC_FAST, tensor-core form (batch_engine_kernel<0>, the FAST default): the FMA pipes cannot keep up with the weight
-// stream at 8 rows (an SM issues 64 three-register FFMA lanes per clock, and every broadcast LDS.128 of the activation tile
-// costs four LSU cycles: profiles/r02_batch_engine_profile.txt), so the FAST projections run on the 5th-gen tensor cores:
-//   D[128 x N] (TMEM, fp32)  +=  X[128 x 16k] (TMEM, bf16; lane m = sequence m, lanes >= 8 don't matter)  .  W[N x 16k]^T
-// with the weight tile of a ring stage as the B operand -- it IS a K-major, no-swizzle UMMA operand already (8-row x 16-byte
-// core matrices = the panels, as in gemm_tc.cuh), N = 8 x the panels the CTA owns (rounded to 16), so a CTA with 3 panels
-// spends 3 panels' worth of tensor-core time -- and the activations as the A operand IN TENSOR MEMORY (the `.ts` form: an A
-// operand in shared memory would cost a 4 KB read per k16 step whatever N is).  Warp roles: 0 = weight producer (as
-// before); 9 = activation blocks global -> shared (bulk copies of 128 k x 8 rows = 2 KB, after the phase's grid barrier);
-// 8 = activation blocks shared -> TMEM (tcgen05.st, lane m <- sequence m); 5 = MMA issuer (one lane) + TMEM owner;
-// 4 = accumulators TMEM -> shared (tcgen05.ld, 8 lanes x 128 columns); 1..4 = the per-row epilogue (gemv_epilogue).
+// LNB_ACC_FAST, tensor-core form (batch_engine_kernel<0>, LNB_BATCH_TC=1; the FMA-pipe form batch_engine_kernel<8> is the FAST
+// default, it measured faster on an H100): the FAST projections run on the tensor cores as warpgroup MMAs (wgmma.cuh):
+//   D[64 x 32] (registers, fp32)  +=  X[64 x 16k] (registers, bf16; row m = sequence m, rows >= 8 are zero)  .  W[32 x 16k]^T
+// with the weight tile of a ring stage as the B operand -- it IS a K-major, no-swizzle operand already (8-row x 16-byte core
+// matrices = the panels, as in gemm_tc.cuh); a tile of np panels takes ceil(np / 4) such 32-row slices, so a CTA with 3
+// panels spends 4 panels' worth of tensor-core time.  Warp roles: 0 = weight producer (as before); 9 = activation blocks
+// global -> shared (bulk copies of 128 k x 8 rows = 2 KB, after the phase's grid barrier); 4..7 = the MMA warpgroup (it loads
+// the activation fragments from the shared block, issues the MMAs and hands the 8 accumulator rows over through shared
+// memory); 1, 2, 3 and 8 = the per-row epilogue (bt_epilogue).
 // RMSNorm moves into the SCALE phase, which stores the normalised row t(t(x * r) * w) next to r.  The accumulation order
 // is the tensor core's: FAST only (documented reorder); STRICT stays on the FMA pipes in the reference's order.
 #pragma once
@@ -90,23 +88,15 @@ constexpr int BE_PART_OFF = 48 * 1024;       // FAST stream partials [8 streams]
 constexpr int BE_SCAN_OFF = 64 * 1024;       // binade-scan scratch 4 KB
 constexpr int BE_R_OFF = 68 * 1024;          // r[8]
 // tensor-core form: activation blocks of 128 k (2 KB) in a ring inside the work area; a block of mbarriers behind the work
-// area; tensor memory: columns 0..255 two accumulators of 128, 256..511 four activation blocks of 64
+// area; the accumulators of a row tile reach the epilogue warps through a double-buffered hand-over area
 constexpr int BT_NXS = 8;                    // activation blocks in shared memory
-constexpr int BT_NXT = 4;                    // activation blocks in tensor memory
 constexpr int BT_KT_MAX = 512;
 constexpr int BT_XB = 128 * 16;              // one block: 128 k x 8 rows x 2 B
 constexpr int BT_X_OFF = 16 * 1024;          // 8 x 2 KB in the work area
 constexpr int BT_D_OFF = 48 * 1024;          // accumulator hand-over [2][8][129] f32
 constexpr int BT_SMEM = ENG_SMEM + 512;      // + the mbarriers of this form
+constexpr int BT_NEPI = 128;                 // epilogue threads (consumer warps 0, 1, 2 and 7)
 static_assert(BT_SMEM <= 227 * 1024, "shared memory per CTA");
-LNB_DEVINL void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-LNB_DEVINL void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // ---- one k-tile of the activations: this thread's 16-byte pieces of the chunk-major block [k0, k0 + kt) ------------------
 // piece i (i < kt): chunk i >> 3 of the tile, row i & 7  ->  consecutive threads read consecutive 16 bytes
@@ -253,11 +243,8 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
   uint64_t* empty_bar = full_bar + NST;
   uint64_t* fullxs_bar = reinterpret_cast<uint64_t*>(smem + ENG_SMEM);   // (tensor-core form) activation blocks, shared
   uint64_t* emptyxs_bar = fullxs_bar + BT_NXS;
-  uint64_t* fullxt_bar = emptyxs_bar + BT_NXS;     // activation blocks, tensor memory
-  uint64_t* emptyxt_bar = fullxt_bar + BT_NXT;
-  uint64_t* accfull_bar = emptyxt_bar + BT_NXT;    // two accumulators of 128 TMEM columns
+  uint64_t* accfull_bar = emptyxs_bar + BT_NXS;    // the two accumulator hand-over buffers
   uint64_t* accempty_bar = accfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(accempty_bar + 2);
   float* s_scalar = reinterpret_cast<float*>(smem + 256);
   GemvParams* gp = reinterpret_cast<GemvParams*>(smem + 512);
   uint8_t* s_ring = smem + 1024;
@@ -277,21 +264,11 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
     }
     if (TC) {
       for (int s = 0; s < BT_NXS; s++) { mbar_init(&fullxs_bar[s], 1); mbar_init(&emptyxs_bar[s], 1); }
-      for (int s = 0; s < BT_NXT; s++) { mbar_init(&fullxt_bar[s], 1); mbar_init(&emptyxt_bar[s], 1); }
-      for (int b = 0; b < 2; b++) { mbar_init(&accfull_bar[b], 1); mbar_init(&accempty_bar[b], 1); }
+      for (int b = 0; b < 2; b++) { mbar_init(&accfull_bar[b], 1); mbar_init(&accempty_bar[b], BT_NEPI); }
     }
     mbar_fence_init();
   }
-  uint32_t tmem_base = 0;
-  if (TC) {
-    if ((tid >> 5) == 5) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
-  }
   __syncthreads();
-  if (TC) {
-    tc_fence_after();
-    tmem_base = *tmem_slot;
-  }
 
   if (tid < 32) {
     // =========================== producer: the weights of every projection, ahead of the consumers ================
@@ -467,13 +444,11 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
       // ---- tensor-core projection: D[seq, weight row] += X[seq, 16k] . W[weight row, 16k] per k16 step ------------------
       const int K = E->K, kt = E->kt;
       const int n_tiles = (K + kt - 1) / kt;
-      const int n_blk = (K + 127) / 128;
       int p0, p1;
       eng_split(E->N / 8, bid, G, &p0, &p1);
       if (p1 > p0) {
-        if (cw_u < 4) {
-          // -- epilogue warps (hardware warps 1..4): thread = weight row of the 128-row tile; hardware warp 4 (TMEM lane
-          //    quarter 0 = the sequences) first moves the accumulator through shared memory
+        if (cw_u < 3 || cw_u == 7) {
+          // -- epilogue warps (hardware warps 1, 2, 3, 8): thread ec = (panel of the tile, sequence)
           if (c == 0) {
             GemvParams g{};
             g.W = E->W; g.N = E->N; g.K = K; g.M = n; g.eps = P.eps;
@@ -487,59 +462,46 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
             if (E->epi == EPI_P2P) g.st = P.st;
             *gp = g;
           }
-          float* s_d = reinterpret_cast<float*>(s_work + BT_D_OFF);
-          const int pp = c >> 3, m = c & 7;              // (c < 128 here) thread = (panel of the tile, sequence)
+          const float* s_d = reinterpret_cast<const float*>(s_work + BT_D_OFF);
+          const int ec = (cw_u == 7) ? c - 128 : c;
+          const int pp = ec >> 3, m = ec & 7;
           const int epi = E->epi;
-          named_bar_sync(2, 128);
+          named_bar_sync(2, BT_NEPI);
           const GemvParams& g = *gp;
           BE_PROF(1);
           for (int rt = p0; rt < p1; rt += PT) {
             const int np = min(PT, p1 - rt);
-            float* sd = s_d + (size_t)(acc_cnt & 1u) * (8 * 129);
-            if (cw == 3) {
-              const int buf = acc_cnt & 1;
-              eng_mbar_wait(&accfull_bar[buf], (acc_cnt >> 1) & 1u, P.err_host, P.timeout_ns, false, acc_cnt);
-              tc_fence_after();
-              const int ncol = ((np + 1) >> 1) * 16;
-              for (int cb = 0; cb < ncol; cb += 16) {
-                uint32_t acc[16];
-                tmem_ld16(tmem_base + (uint32_t)(buf * 128 + cb), acc);
-                if (lane < 8) {
-#pragma unroll
-                  for (int e = 0; e < 16; e++) sd[lane * 129 + cb + e] = __uint_as_float(acc[e]);
-                }
-              }
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(&accempty_bar[buf]);    // the issuer may start the tile after next in this buffer
-            }
+            const int buf = acc_cnt & 1;
+            eng_mbar_wait(&accfull_bar[buf], (acc_cnt >> 1) & 1u, P.err_host, P.timeout_ns, false, acc_cnt);
             acc_cnt++;
-            named_bar_sync(2, 128);
             BE_PROF(3);
+            const float* sd = s_d + (size_t)buf * (8 * 129);
             float v[8];
 #pragma unroll
             for (int e = 0; e < 8; e++) v[e] = sd[m * 129 + pp * 8 + e];
+            mbar_arrive(&accempty_bar[buf]);              // the MMA warpgroup may hand the tile after next over in this buffer
             bt_epilogue(g, epi, v, rt + pp, m, pp < np && m < n, lane);
             BE_PROF(5);
           }
           fence_proxy_async();      // these stores are read by the next projection's bulk copies (after the grid barrier)
-        } else if (cw_u == 4) {
-          // -- MMA issuer (hardware warp 5).  The whole warp runs the loop and one elected lane issues: every operand is then
-          //    warp-uniform for the compiler and lives in uniform registers (issued from a one-lane branch, each MMA cost
-          //    ~120 cycles of R2UR transfers -- more than the MMA itself)
-          const bool pm = P.prof != nullptr && lane == 0;
-          const bool lead = elect_one();
+        } else {
+          // -- the MMA warpgroup (hardware warps 4..7).  Warp 4 holds accumulator rows 0..7 = the sequences (fragment row
+          //    l / 4 of lane l); it alone loads activations (the other warps' rows of A are zero) and hands the results over
+          const int wl = cw_u - 3;                       // warp of the warpgroup
+          const int g8 = lane >> 2, cq = 2 * (lane & 3);
+          const bool pm = P.prof != nullptr && wl == 0 && lane == 0;
           long long tm = pm ? clock64() : 0;
 #define BT_MARK(var) do { if (pm) { const long long n_ = clock64(); var += (unsigned int)(n_ - tm); tm = n_; } } while (0)
+          const uint8_t* xring = s_work + BT_X_OFF;
+          float* s_d = reinterpret_cast<float*>(s_work + BT_D_OFF);
           for (int rt = p0; rt < p1; rt += PT) {
             const int np = min(PT, p1 - rt);
-            const uint32_t idesc = umma_idesc_bf16(128, ((np + 1) >> 1) * 16);
-            const int buf = acc_cnt & 1;
-            eng_mbar_wait(&accempty_bar[buf], ((acc_cnt >> 1) & 1u) ^ 1u, P.err_host, P.timeout_ns, false, acc_cnt);
-            BT_MARK(mma_acc);
-            acc_cnt++;
-            tc_fence_after();
-            const uint32_t d_tmem = tmem_base + (uint32_t)(buf * 128);
+            const int nsl = (np + 3) >> 2;               // 32-row slices of the tile
+            float d[4][16];
+#pragma unroll
+            for (int q = 0; q < 4; q++)
+#pragma unroll
+              for (int i = 0; i < 16; i++) d[q][i] = 0.f;
             uint32_t accum = 0u;
             for (int t = 0; t < n_tiles; t++) {
               const int ktt = min(kt, K - t * kt);
@@ -549,69 +511,63 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
               seq++;
               const uint32_t w_base = smem_u32(s_ring + (size_t)sw * STAGE);
               for (int kb0 = 0; kb0 < ktt; kb0 += 128) {
-                const int sx = seqx % BT_NXT;
-                eng_mbar_wait(&fullxt_bar[sx], (seqx / BT_NXT) & 1u, P.err_host, P.timeout_ns, false, seqx);
+                const int ss = seqx % BT_NXS;
+                if (wl == 0) eng_mbar_wait(&fullxs_bar[ss], (seqx / BT_NXS) & 1u, P.err_host, P.timeout_ns, false, seqx);
                 BT_MARK(mma_x);
                 seqx++;
-                tc_fence_after();
-                // B: next k-chunk 128 B, next panel kt * 16 B, next k16 step 256 B (= 16 in the descriptor's address field);
-                // A: 8 columns (16 bf16) per lane and k16 step
-                uint64_t b_desc = umma_desc(w_base + (uint32_t)kb0 * 16u, 128, (uint32_t)kt * 16u);
-                uint32_t a_tmem = tmem_base + 256u + (uint32_t)(sx * 64);
+                // A fragments of the (up to) 8 k16 steps of this block: chunk-major [16 chunks][8 rows][8] = core matrices
                 const int nk16 = min(128, ktt - kb0) / 16;
-                if (nk16 == 8) {
+                uint32_t a[8][4];
 #pragma unroll
-                  for (int j = 0; j < 8; j++) {
-                    if (lead) umma_bf16_ts(d_tmem, a_tmem, b_desc, idesc, accum);
-                    accum = 1u; b_desc += 16; a_tmem += 8;
-                  }
-                } else {
-                  for (int j = 0; j < nk16; j++) {
-                    if (lead) umma_bf16_ts(d_tmem, a_tmem, b_desc, idesc, accum);
-                    accum = 1u; b_desc += 16; a_tmem += 8;
+                for (int j = 0; j < 8; j++) {
+                  a[j][0] = a[j][1] = a[j][2] = a[j][3] = 0u;
+                  if (wl == 0 && j < nk16) {
+                    const uint8_t* xs = xring + (size_t)ss * BT_XB + g8 * 16 + cq * 2;
+                    a[j][0] = *reinterpret_cast<const uint32_t*>(xs + (2 * j) * 128);
+                    a[j][2] = *reinterpret_cast<const uint32_t*>(xs + (2 * j + 1) * 128);
                   }
                 }
-                if (lead) umma_commit(&emptyxt_bar[sx]);   // the activation block may be overwritten once these MMAs have read it
+                __syncwarp();
+                if (wl == 0 && lane == 0) mbar_arrive(&emptyxs_bar[ss]);   // the block is in registers: it may be overwritten
+                // B: next k-chunk 128 B, next panel kt * 16 B, next k16 step 256 B (= 16 in the descriptor's address field);
+                // slice q = panels 4q .. 4q+3
+                const uint64_t b0 = gmma_desc(w_base + (uint32_t)kb0 * 16u, 128, (uint32_t)kt * 16u);
+                const uint64_t slice = (uint64_t)(((uint32_t)kt * 64u) >> 4);
+                wgmma_fence();
+#pragma unroll
+                for (int j = 0; j < 8; j++) {
+                  if (j < nk16) {
+#pragma unroll
+                    for (int q = 0; q < 4; q++)
+                      if (q < nsl) wgmma_rs_n32(d[q], a[j], b0 + (uint64_t)q * slice + (uint64_t)(16 * j), accum);
+                    accum = 1u;
+                  }
+                }
+                wgmma_commit();
                 BT_MARK(mma_issue);
               }
-              if (lead) umma_commit(&empty_bar[sw]);       // and the weight stage
+              wgmma_wait<0>();                             // this stage's MMAs have read the weights
+              if (wl == 0 && lane == 0) mbar_arrive(&empty_bar[sw]);
             }
-            if (lead) umma_commit(&accfull_bar[buf]);
-            __syncwarp();
+#pragma unroll
+            for (int q = 0; q < 4; q++) wgmma_fence_regs(d[q]);
+            if (wl == 0) {
+              const int buf = acc_cnt & 1;
+              eng_mbar_wait(&accempty_bar[buf], ((acc_cnt >> 1) & 1u) ^ 1u, P.err_host, P.timeout_ns, false, acc_cnt);
+              BT_MARK(mma_acc);
+              float* sd = s_d + (size_t)buf * (8 * 129) + g8 * 129 + cq;
+#pragma unroll
+              for (int q = 0; q < 4; q++)
+                if (q < nsl) {
+#pragma unroll
+                  for (int cb = 0; cb < 4; cb++) { sd[q * 32 + cb * 8] = d[q][4 * cb]; sd[q * 32 + cb * 8 + 1] = d[q][4 * cb + 1]; }
+                }
+              __syncwarp();
+              if (lane == 0) mbar_arrive(&accfull_bar[buf]);
+            }
+            acc_cnt++;
           }
 #undef BT_MARK
-        } else if (cw_u == 7) {
-          // -- activation blocks shared -> tensor memory (hardware warp 8 = TMEM lane quarter 0): lane m <- sequence m
-          const uint8_t* xring = s_work + BT_X_OFF;
-          for (int rt = p0; rt < p1; rt += PT) {
-            for (int b = 0; b < n_blk; b++, seqx++) {
-              const int ss = seqx % BT_NXS, sx = seqx % BT_NXT;
-              eng_mbar_wait(&fullxs_bar[ss], (seqx / BT_NXS) & 1u, P.err_host, P.timeout_ns, false, seqx);
-              eng_mbar_wait(&emptyxt_bar[sx], ((seqx / BT_NXT) & 1u) ^ 1u, P.err_host, P.timeout_ns, false, seqx);
-              tc_fence_after();
-              const int nch = min(128, K - b * 128) / 8;
-              const uint8_t* src = xring + (size_t)ss * BT_XB + lane * 16;
-#pragma unroll
-              for (int g = 0; g < 4; g++) {
-                uint32_t v[16];
-#pragma unroll
-                for (int q = 0; q < 4; q++) {
-                  const int ch = g * 4 + q;
-                  uint4 w = make_uint4(0u, 0u, 0u, 0u);
-                  if (lane < 8 && ch < nch) w = *reinterpret_cast<const uint4*>(src + ch * 128);
-                  v[q * 4 + 0] = w.x; v[q * 4 + 1] = w.y; v[q * 4 + 2] = w.z; v[q * 4 + 3] = w.w;
-                }
-                tmem_st16(tmem_base + 256u + (uint32_t)(sx * 64 + g * 16), v);
-              }
-              tmem_wait_st();
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) {
-                mbar_arrive(&fullxt_bar[sx]);
-                mbar_arrive(&emptyxs_bar[ss]);
-              }
-            }
-          }
         }
       }
     } else if (!TC && type == BP_GEMV) {
@@ -914,15 +870,11 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
 #pragma unroll
     for (int k = 0; k < ENG_NPROF; k++) pr[k] += (unsigned long long)pacc[k];
   }
-  if (TC && P.prof && cw == 4 && lane == 0) {         // (slots 2, 4, 10, 11 are free in the tensor-core form)
+  if (TC && P.prof && cw == 3 && lane == 0) {         // (slots 2, 4, 10, 11 are free in the tensor-core form)
     unsigned long long* q = P.prof + (size_t)bid * ENG_NPROF;
     q[2] += mma_acc; q[4] += mma_w; q[10] += mma_x; q[11] += mma_issue;
   }
   if (bid == 0 && c == 0 && P.tp > 1) P.st->ar_epoch = epoch;
-  if (TC && cw == 4) {                      // (every tcgen05 operation of this CTA completed before the last grid barrier)
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 }  // namespace lnb

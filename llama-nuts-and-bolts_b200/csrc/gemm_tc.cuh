@@ -1,25 +1,24 @@
-// gemm_tc.cuh -- the prompt-processing projection: C[M,N] = X[M,K] . W[N,K]^T on the 5th-generation
-// tensor cores (tcgen05.mma, bf16 in, fp32 accumulate in TMEM), operands staged into shared memory by
-// the TMA engine's bulk-async copies.  Replaces ml.LinearTransformation
-// (src/ml/operations_impl.go:427-447 -> operations_lineartransform.go:145-207) when S is large
+// gemm_tc.cuh -- the prompt-processing projection: C[M,N] = X[M,K] . W[N,K]^T on the Hopper tensor cores (wgmma, bf16 in,
+// fp32 accumulate in registers), operands staged into shared memory by the TMA engine's bulk-async copies.  Replaces
+// ml.LinearTransformation (src/ml/operations_impl.go:427-447 -> operations_lineartransform.go:145-207) when S is large
 // (prefill); the decode path (S = 1..8) uses gemv.cuh.
 //
 // Numerics: products are exact, accumulation is fp32 in the tensor core's own order, the result is
 // truncated to bf16 exactly like the reference's ToBFloat16 (:205).  The accumulation ORDER is the
 // hardware's, so this path belongs to LNB_ACC_FAST; LNB_ACC_STRICT keeps the sequential GEMV.
 //
-// Operand layouts (both "K-major, no swizzle" in UMMA terms: 8-row x 16-byte core matrices):
+// Operand layouts (both K-major, no swizzle: 8-row x 16-byte core matrices, wgmma.cuh):
 //   W  : the same panel-major HBM layout the GEMV streams (8-row panels = core matrices, gemv.cuh): the 16
 //        panels of a 128-row tile are copied panel by panel (KT*16 B each) and form ONE N=128 B operand:
 //        LBO = 128 B (next k-chunk), SBO = KT*16 B (next panel).
 //   X  : "X8" activations written by the preceding kernel, tile-major: [M/128][K/128] tiles of
 //        [16 row-groups][16 k-chunks][8 rows][8 elems] = 32 KB contiguous -> ONE bulk copy per stage;
 //        LBO = 128 B (next k-chunk), SBO = 2048 B (next 8 rows).
-// One CTA computes a 128 x 128 tile: 8 accumulators of 128 lanes x 16 columns in TMEM (128 columns).
-// Warp roles: 0, 2, 3 = bulk-copy producers (one thread each), 1 = MMA issuer (one elected lane), 2 also allocates TMEM,
-// 4..7 = epilogue (tcgen05.ld -> truncate -> global).
+// One CTA computes a 128 x 128 tile.  Warps 0..7 = two consumer warpgroups, warpgroup g owns rows 64g .. 64g+63 of the
+// tile (64 fp32 accumulators per thread) and runs the epilogue from its registers; warp 8 = bulk-copy producer (a stage is
+// 17 copies: lanes 0..15 copy one weight panel each, lane 16 the activation tile, so the copies are issued in parallel).
 #pragma once
-#include "common.cuh"
+#include "wgmma.cuh"
 
 namespace lnb {
 
@@ -43,79 +42,9 @@ constexpr int TC_BM = 128, TC_BN = 128, TC_KT = 128, TC_NS = 3;
 constexpr int TC_A_STAGE = TC_BM * TC_KT * 2;  // 32 KB
 constexpr int TC_B_STAGE = TC_BN * TC_KT * 2;  // 32 KB
 constexpr int TC_SMEM = 1024 + TC_NS * (TC_A_STAGE + TC_B_STAGE);
-constexpr int TC_THREADS = 256;
-
-// ---- tcgen05 wrappers (PTX as in /opt/skills/guides/blackwell_cuda_programming.md) ---------------
-LNB_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-LNB_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-LNB_DEVINL void tmem_alloc(uint32_t* slot_in_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-LNB_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// shared-memory matrix descriptor, SWIZZLE_NONE, K-major (cute/arch/mma_sm100_desc.hpp bit layout)
-LNB_DEVINL uint64_t umma_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3fffu);            // start address  [0,14)
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;  // leading byte offset [16,30)
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;  // stride byte offset  [32,46)
-  d |= (uint64_t)1 << 46;                             // descriptor version (sm_100)
-  return d;                                           // base_offset 0, lbo_mode 0, layout_type 0 = SWIZZLE_NONE
-}
-// instruction descriptor, kind::f16: D = f32, A = B = bf16, both K-major, M x N
-LNB_DEVINL constexpr uint32_t umma_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-LNB_DEVINL void umma_bf16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Optional A operand from TMEM (".ts" form, -DLNB_TC_A_IN_TMEM=1): the 128 x 16 activation slice of a k16
-// step is copied shared -> tensor memory (tcgen05.cp, 128 lanes x 256 bit) and the MMA reads it from there.
-// Verified correct on B200; not faster than the SS form for this tile shape, so it is off by default.
-LNB_DEVINL void tmem_cp_128x256b(uint32_t taddr, uint64_t s_desc) {
-  asm volatile("tcgen05.cp.cta_group::1.128x256b [%0], %1;" ::"r"(taddr), "l"(s_desc) : "memory");
-}
-LNB_DEVINL void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// generic-proxy writes (st.shared / st.global by threads) before async-proxy reads (tcgen05.mma operands, bulk copies)
-LNB_DEVINL void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
-LNB_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// one lane of the (converged) warp, chosen by the hardware: ptxas then knows a single lane issues the tcgen05 instructions
-// under this predicate and moves their operands to uniform registers once, without a loop over possibly distinct values
-LNB_DEVINL bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0u;
-}
-#ifndef LNB_TC_A_IN_TMEM
-#define LNB_TC_A_IN_TMEM 0
-#endif
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-LNB_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-LNB_DEVINL void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+constexpr int TC_CONSUMERS = 256;
+constexpr int TC_THREADS = TC_CONSUMERS + 32;
+static_assert(TC_SMEM <= 227 * 1024, "shared memory per CTA");
 
 // ---- layout helpers for the tensor-core path (X8 = tile-major activations, see the header comment)
 // X8 address of element (row, col) of a [*, K] activation matrix
@@ -128,10 +57,8 @@ LNB_DEVINL size_t x8_index(int row, int col, int K) {
 template <int EPI>
 __global__ void __launch_bounds__(TC_THREADS, 1) gemm_tc_kernel(const GemmTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem);  // [NS]
-  uint64_t* empty_bar = full_bar + TC_NS;                  // [NS]
-  uint64_t* acc_bar = empty_bar + TC_NS;                   // accumulators complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem);  // [NS] stage loaded
+  uint64_t* empty_bar = full_bar + TC_NS;                  // [NS] stage read by every consumer's MMAs
   uint8_t* sA = smem + 1024;
   uint8_t* sB = sA + TC_NS * TC_A_STAGE;
 
@@ -142,140 +69,104 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gemm_tc_kernel(const GemmTcPara
   const int n_kt = p.K / TC_KT;
 
   if (tid == 0) {
-    for (int s = 0; s < TC_NS; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(acc_bar, 1);
+    for (int s = 0; s < TC_NS; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], TC_CONSUMERS); }
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc(tmem_slot, LNB_TC_A_IN_TMEM ? 256 : 128);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_launch_dependents();
 
-  if (warp == 0 || warp == 2 || warp == 3) {
-    // Three producer threads (warps 0, 2, 3): a stage is 1 + 16 bulk copies, and ONE thread needs ~50 cycles per copy -- 850
-    // cycles per stage against the 512 cycles its eight MMAs occupy the tensor pipe (ncu: tensor pipe 34 % active, L2 -> SM
-    // traffic at a third of what the SM can take: the pipe was waiting for the copy ISSUE, not for bandwidth).  Warp 0 announces
-    // the stage's bytes and copies the activation tile and 4 weight panels, warps 2 and 3 copy 6 panels each; a copy that
-    // completes before the announcement only makes the barrier's pending-byte count transiently negative.
-    if (lane == 0) {
-      pdl_wait();  // the activations come from the previous kernel (weights alone could go earlier)
-      const int part = (warp == 0) ? 0 : warp - 1;
-      const int j0 = (part == 0) ? 0 : (part == 1 ? 4 : 10), j1 = (part == 0) ? 4 : (part == 1 ? 10 : 16);
-      const uint64_t pol_w = l2_policy_evict_first();
-      const uint64_t pol_x = l2_policy_evict_last();   // every N-tile re-reads the same activations
-      const uint8_t* xb = reinterpret_cast<const uint8_t*>(p.X8);
-      const uint8_t* wb = reinterpret_cast<const uint8_t*>(p.W);
-      for (int t = 0; t < n_kt; t++) {
-        const int s = t % TC_NS;
-        mbar_wait(&empty_bar[s], (((uint32_t)(t / TC_NS)) & 1u) ^ 1u);
-        const size_t k0 = (size_t)t * TC_KT;
-        if (part == 0) {
-          mbar_expect_tx(&full_bar[s], TC_A_STAGE + TC_B_STAGE);
-          // A: one contiguous 128 x 128 tile of the tile-major X8 layout
-          bulk_g2s(sA + (size_t)s * TC_A_STAGE, xb + ((size_t)(m0 / TC_BM) * (p.K / TC_KT) + t) * TC_A_STAGE, TC_A_STAGE,
-                   &full_bar[s], pol_x);
-        }
-        // B: 16 panels of 8 rows, each (8 rows x KT) = KT*16 contiguous bytes
-        for (int j = j0; j < j1; j++)
-          bulk_g2s(sB + (size_t)s * TC_B_STAGE + (size_t)j * (TC_KT * 16),
-                   wb + ((size_t)(n0 / 8 + j) * p.K + k0) * 16, TC_KT * 16, &full_bar[s], pol_w);
-      }
-    }
-  } else if (warp == 1) {
-    // the whole warp runs the loop, one elected lane issues: the operands are then warp-uniform for ptxas and sit in uniform
-    // registers (from a `lane == 0` branch every MMA was preceded by a loop of R2UR transfers, ~120 cycles -- twice the
-    // 64 cycles a 128 x 128 x 16 MMA occupies the tensor pipe)
-    const bool lead = elect_one();
-    constexpr uint32_t idesc = umma_idesc_bf16(TC_BM, TC_BN);
+  if (warp == TC_CONSUMERS / 32) {
+    // ===================== producer: lane j < 16 copies weight panel j, lane 16 the activation tile ==================
+    pdl_wait();  // the activations come from the previous kernel (weights alone could go earlier)
+    const uint64_t pol_w = l2_policy_evict_first();
+    const uint64_t pol_x = l2_policy_evict_last();   // every N-tile re-reads the same activations
+    const uint8_t* xb = reinterpret_cast<const uint8_t*>(p.X8);
+    const uint8_t* wb = reinterpret_cast<const uint8_t*>(p.W);
     for (int t = 0; t < n_kt; t++) {
       const int s = t % TC_NS;
-      mbar_wait(&full_bar[s], ((uint32_t)(t / TC_NS)) & 1u);
-      tc_fence_after();
-      const uint32_t a_base = smem_u32(sA + (size_t)s * TC_A_STAGE);
-      const uint32_t b_base = smem_u32(sB + (size_t)s * TC_B_STAGE);
-      uint64_t a_desc = umma_desc(a_base, 128, TC_KT * 16);  // SBO = 16 chunks * 128 B; next k16 step = +256 B = +16 in the address field
-      uint64_t b_desc = umma_desc(b_base, 128, TC_KT * 16);
-#pragma unroll
-      for (int k16 = 0; k16 < TC_KT / 16; k16++) {
-#if LNB_TC_A_IN_TMEM
-        const uint32_t a_tmem = tmem_base + 128 + (uint32_t)(k16 & 1) * 8;   // 8 columns = 16 bf16 per lane, double-buffered
-        if (lead) {
-          tmem_cp_128x256b(a_tmem, a_desc);
-          umma_bf16_ts(tmem_base, a_tmem, b_desc, idesc, (t > 0 || k16 > 0) ? 1u : 0u);
-        }
-#else
-        if (lead) umma_bf16(tmem_base, a_desc, b_desc, idesc, (t > 0 || k16 > 0) ? 1u : 0u);   // 128 x 128 x 16 per instruction
-#endif
-        a_desc += 16; b_desc += 16;
-      }
-      if (lead) umma_commit(&empty_bar[s]);  // frees the stage once these MMAs have read it
+      mbar_wait(&empty_bar[s], (((uint32_t)(t / TC_NS)) & 1u) ^ 1u);
+      if (lane == 0) mbar_expect_tx(&full_bar[s], TC_A_STAGE + TC_B_STAGE);
+      __syncwarp();
+      const size_t k0 = (size_t)t * TC_KT;
+      if (lane < 16)   // B: 16 panels of 8 rows, each (8 rows x KT) = KT*16 contiguous bytes
+        bulk_g2s(sB + (size_t)s * TC_B_STAGE + (size_t)lane * (TC_KT * 16), wb + ((size_t)(n0 / 8 + lane) * p.K + k0) * 16, TC_KT * 16,
+                 &full_bar[s], pol_w);
+      else if (lane == 16)   // A: one contiguous 128 x 128 tile of the tile-major X8 layout
+        bulk_g2s(sA + (size_t)s * TC_A_STAGE, xb + ((size_t)(m0 / TC_BM) * (p.K / TC_KT) + t) * TC_A_STAGE, TC_A_STAGE,
+                 &full_bar[s], pol_x);
     }
-    if (lead) umma_commit(acc_bar);
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ===================== epilogue: TMEM -> registers -> global ================================
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int row = m0 + q * 32 + lane;     // activation row == TMEM lane
-    mbar_wait(acc_bar, 0);
-    tc_fence_after();
-    if (EPI == TC_EPI_RESID) pdl_wait();    // residual operand is written by an earlier kernel
-#pragma unroll 1
-    for (int j = 0; j < TC_BN / 16; j++) {
-      uint32_t r[16];
-      tmem_ld16(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(j * 16), r);
-      if (EPI == TC_EPI_SWIGLU) {
-        uint16_t sg[8];
-#pragma unroll
-        for (int e = 0; e < 8; e++) sg[e] = p.silu_tab[r[(e >> 2) * 8 + (e & 3)] >> 16];          // t(TABLE_SILU[t(gate)])
-        uint32_t o[4];
-#pragma unroll
-        for (int e = 0; e < 8; e += 2) {
-          const float lo = __fmul_rn(bf2f(sg[e]), __uint_as_float(r[(e >> 2) * 8 + 4 + (e & 3)] & 0xffff0000u));
-          const float hi = __fmul_rn(bf2f(sg[e + 1]), __uint_as_float(r[((e + 1) >> 2) * 8 + 4 + ((e + 1) & 3)] & 0xffff0000u));
-          o[e >> 1] = (__float_as_uint(lo) >> 16) | (__float_as_uint(hi) & 0xffff0000u);
-        }
-        *reinterpret_cast<uint4*>(p.out_bf16 + x8_index(row, (n0 + j * 16) >> 1, p.ldo)) = make_uint4(o[0], o[1], o[2], o[3]);
-      } else if (row < p.M) {
-        const size_t o = (size_t)row * p.ldo + n0 + j * 16;
-        if (EPI == TC_EPI_BF16 || EPI == TC_EPI_RESID) {
-          uint32_t packed[8];
-#pragma unroll
-          for (int e = 0; e < 8; e++) {
-            float a = __uint_as_float(r[2 * e]), b = __uint_as_float(r[2 * e + 1]);
-            if (EPI == TC_EPI_RESID) {
-              const uint32_t rw = *reinterpret_cast<const uint32_t*>(p.res + o + 2 * e);
-              a = __fadd_rn(bf_lo(rw), trunc_bf(a));   // ml.Add(x, t(linear))  llamatransformer.go:232,248
-              b = __fadd_rn(bf_hi(rw), trunc_bf(b));
-            }
-            packed[e] = (uint32_t)f2bf(a) | ((uint32_t)f2bf(b) << 16);
-          }
-          uint4* dst = reinterpret_cast<uint4*>(p.out_bf16 + o);
-          dst[0] = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-          dst[1] = make_uint4(packed[4], packed[5], packed[6], packed[7]);
-        } else {
-          float4* dst = reinterpret_cast<float4*>(p.out_f32 + o);
-#pragma unroll
-          for (int e = 0; e < 4; e++) {
-            float4 v;
-            v.x = __uint_as_float(r[4 * e]); v.y = __uint_as_float(r[4 * e + 1]);
-            v.z = __uint_as_float(r[4 * e + 2]); v.w = __uint_as_float(r[4 * e + 3]);
-            if (EPI == TC_EPI_F32TRUNC) { v.x = trunc_bf(v.x); v.y = trunc_bf(v.y); v.z = trunc_bf(v.z); v.w = trunc_bf(v.w); }
-            dst[e] = v;
-          }
-        }
-      }
-    }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, LNB_TC_A_IN_TMEM ? 256 : 128);
+
+  // ===================== consumers: warpgroup wg computes rows 64 wg .. 64 wg + 63 of the tile ===========================
+  const int wg = warp >> 2;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; i++) acc[i] = 0.f;
+  for (int t = 0; t < n_kt; t++) {
+    const int s = t % TC_NS;
+    mbar_wait(&full_bar[s], ((uint32_t)(t / TC_NS)) & 1u);
+    // A: this warpgroup's 8 row groups start 8 x 2048 B into the stage; next k16 step = +256 B = +16 in the address field
+    uint64_t a_desc = gmma_desc(smem_u32(sA + (size_t)s * TC_A_STAGE + (size_t)wg * 8 * (TC_KT * 16)), 128, TC_KT * 16);
+    uint64_t b_desc = gmma_desc(smem_u32(sB + (size_t)s * TC_B_STAGE), 128, TC_KT * 16);
+    wgmma_fence();
+#pragma unroll
+    for (int k16 = 0; k16 < TC_KT / 16; k16++) {
+      wgmma_ss_n128(acc, a_desc, b_desc, (t > 0 || k16 > 0) ? 1u : 0u);   // 64 x 128 x 16 per instruction
+      a_desc += 16; b_desc += 16;
+    }
+    wgmma_commit();
+    // the previous stage's MMAs are complete once at most this stage's group is in flight: hand that stage back
+    wgmma_wait<1>();
+    if (t > 0) mbar_arrive(&empty_bar[(t - 1) % TC_NS]);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+
+  // ===================== epilogue: registers -> global ========================================================
+  const int row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);   // rows row0 (acc[4c], acc[4c+1]) and row0 + 8 (acc[4c+2..3])
+  const int cq = 2 * (lane & 3);                                    // columns 8c + cq, 8c + cq + 1
+  if (EPI == TC_EPI_RESID) pdl_wait();    // residual operand is written by an earlier kernel
+#pragma unroll
+  for (int c = 0; c < TC_BN / 8; c++) {
+    if (EPI == TC_EPI_SWIGLU) {
+      // columns 8c..8c+3 are gates, 8c+4..8c+7 the up values of the same hidden units: the lane two to the right holds them
+      float up[4];
+#pragma unroll
+      for (int e = 0; e < 4; e++) up[e] = __shfl_xor_sync(0xffffffffu, acc[4 * c + e], 2);
+      if (cq < 4) {
+#pragma unroll
+        for (int hr = 0; hr < 2; hr++) {
+          const float g0 = acc[4 * c + 2 * hr], g1 = acc[4 * c + 2 * hr + 1];
+          const uint16_t s0 = p.silu_tab[__float_as_uint(g0) >> 16], s1 = p.silu_tab[__float_as_uint(g1) >> 16];   // t(TABLE_SILU[t(gate)])
+          const float lo = __fmul_rn(bf2f(s0), trunc_bf(up[2 * hr]));
+          const float hi = __fmul_rn(bf2f(s1), trunc_bf(up[2 * hr + 1]));
+          *reinterpret_cast<uint32_t*>(p.out_bf16 + x8_index(row0 + 8 * hr, (n0 >> 1) + 4 * c + cq, p.ldo)) =
+              (__float_as_uint(lo) >> 16) | (__float_as_uint(hi) & 0xffff0000u);
+        }
+      }
+    } else {
+#pragma unroll
+      for (int hr = 0; hr < 2; hr++) {
+        const int row = row0 + 8 * hr;
+        if (row >= p.M) continue;
+        const size_t o = (size_t)row * p.ldo + n0 + 8 * c + cq;
+        float a = acc[4 * c + 2 * hr], b = acc[4 * c + 2 * hr + 1];
+        if (EPI == TC_EPI_BF16 || EPI == TC_EPI_RESID) {
+          if (EPI == TC_EPI_RESID) {
+            const uint32_t rw = *reinterpret_cast<const uint32_t*>(p.res + o);
+            a = __fadd_rn(bf_lo(rw), trunc_bf(a));   // ml.Add(x, t(linear))  llamatransformer.go:232,248
+            b = __fadd_rn(bf_hi(rw), trunc_bf(b));
+          }
+          *reinterpret_cast<uint32_t*>(p.out_bf16 + o) = (uint32_t)f2bf(a) | ((uint32_t)f2bf(b) << 16);
+        } else {
+          if (EPI == TC_EPI_F32TRUNC) { a = trunc_bf(a); b = trunc_bf(b); }
+          *reinterpret_cast<float2*>(p.out_f32 + o) = make_float2(a, b);
+        }
+      }
+    }
   }
 }
-
 
 // ---- -----------------------------------------------------
 // row-major [M, K] bf16 -> X8 ([Mpad/8][K/8][8][8]); rows >= M are written as zeros

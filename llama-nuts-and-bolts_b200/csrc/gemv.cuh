@@ -14,7 +14,7 @@
 // back to back.  A (panel, k-range) block is ONE contiguous byte range -> a single bulk-async copy
 // (TMA engine, cp.async.bulk + mbarrier complete_tx) per panel per stage; in shared memory the 8 rows
 // of a chunk are 128 contiguous bytes -> conflict-free 128-bit LDS for "one thread = one output row"
-// (each quarter-warp reads one core matrix), and any number of consecutive panels forms a tcgen05
+// (each quarter-warp reads one core matrix), and any number of consecutive panels forms a wgmma
 // K-major / no-swizzle operand with a uniform 8-row-group stride (gemm_tc.cuh reads the SAME bytes).
 //
 // Thread roles: warp 0 = producer (one lane issues bulk copies into an NST-stage ring);

@@ -1,34 +1,35 @@
-// sdpa_tc.cuh -- the attention core of a prompt call on the 5th-generation tensor cores (LNB_ACC_FAST prefill, head_dim 128).
+// sdpa_tc.cuh -- the attention core of a prompt call on the Hopper tensor cores (LNB_ACC_FAST prefill, head_dim 128).
 // Replaces, for S >= 32 rows, the scaled-dot-product block of LlamaAttention.Forward (src/model/llamatransformer.go:402-514):
 //   sc_st = t( t(sum_d q_sd * k_td) / t(sqrt(hd)) )                MatMul :459, DivToScalar :464
 //   masked entries (t > pos0 + s) contribute nothing               :471
 //   e_st = exp_f64(sc_st);  Z_s = sum_t e_st (f64);  p_st = t(f32(e_st / Z_s))     Softmax :484-495  (here e_st * (1 / Z_s))
 //   o_sd = t( sum_t p_st * v_td )                                  MatMul :504
 // Truncation points, the f64 exponentials and the f64 division are the reference's; the two inner sums (over d for the
-// scores, over t for the output) run in the tensor core's order and Z is added per thread and then across the two threads
+// scores, over t for the output) run in the tensor core's order and Z is added per thread and then across the four threads
 // of a row -- a documented reorder, which is why this kernel belongs to LNB_ACC_FAST (STRICT keeps sdpa_kernel).
 //
-// One CTA = (query head H, 128 query rows).  Per 128-key tile:
-//   S[128 x 128] = Q . K^T      8 x tcgen05.mma (128 x 128 x 16), A = Q tile, B = K tile, both K-major core-matrix tiles in
-//                               shared memory ([16 row groups][16 chunks][8 rows][8 elems], the X8 tile of gemm_tc.cuh)
-//   pass 1: every thread reads half a row of S from TMEM and adds exp_f64 of its entries (row sums Z)
-//   pass 2: S again (recomputing 8 MMAs is cheaper than keeping 2048 columns), p = t(f32(e / Z)) written as the bf16 A tile
-//           P[128 x 128 keys];  O[128 x 128] += P . V   with B = V^T staged by the threads (V rows are key-major in the
-//           cache; the transposing copy is 64 two-byte stores per thread and tile)
+// One CTA = (query head H, 128 query rows), 256 threads = two warpgroups; warpgroup g owns query rows 64g .. 64g+63 and
+// keeps its scores and its output rows in registers (wgmma.cuh fragment layout).  Per 64-key tile:
+//   S[64 x 64] = Q . K^T      8 x wgmma m64n64k16, A = Q tile, B = K tile, both K-major core-matrix tiles in shared memory
+//                             ([row groups][16 chunks][8 rows][8 elems], the X8 tile of gemm_tc.cuh)
+//   pass 1: every thread adds exp_f64 of its entries (row sums Z)
+//   pass 2: S again (recomputing 8 MMAs is cheaper than keeping every tile), p = t(f32(e / Z)) packed straight into the bf16
+//           A fragments of O[64 x 128] += P . V (4 x wgmma m64n128k16, A from registers), B = V^T staged by the threads
+//           (V rows are key-major in the cache; the transposing copy is 32 two-byte stores per thread and tile)
+// K tiles are double-buffered and arrive with cp.async one tile ahead (zero-filled past the last key).
 // exp_f64 of a score is a TABLE LOOKUP: the score is a bf16 value, so exp_tab[bits] = exp((double)bf16(bits)), filled once per
 // device by the same device exp() the other attention kernels call (exp_tab_kernel), has exactly the bits an inline call
-// would produce; the live part of the table (|score| of a few units: a few thousand entries) stays in L1.  Computing the
-// 2 x 64 exponentials per thread and tile on the FP64 pipe took three times as long as everything else in the kernel.
-// The P tile reuses the K tile's shared memory (K is dead once S is complete), so a CTA needs 3 operand tiles = 100 KB and
-// two CTAs share an SM (2 x 256 TMEM columns): one CTA's loads and MMA round trips hide behind the other's softmax.
-// 256 threads: warp w reads TMEM lane quarter w % 4 (row = 32 * (w % 4) + lane), column half w / 4.
+// would produce; the live part of the table (|score| of a few units: a few thousand entries) stays in L1.
 #pragma once
 #include "gemm_tc.cuh"
 
 namespace lnb {
 
-constexpr int ST_TILE = 128 * 128 * 2;                 // one 128 x 128 bf16 operand tile
-constexpr int ST_SMEM = 1024 + 3 * ST_TILE + 128 * 8 * 3;   // Q, K (then P), V^T tiles + Z halves + Z
+constexpr int ST_BK = 64;                            // keys per tile
+constexpr int ST_QTILE = 128 * 128 * 2;              // 32 KB: [128 rows][128 d], A operand of S (SBO 2048)
+constexpr int ST_KTILE = ST_BK * 128 * 2;            // 16 KB: [64 keys][128 d], B operand of S (N = 64, K = 128): SBO 2048
+constexpr int ST_VTILE = 128 * ST_BK * 2;            // 16 KB: [128 d][64 keys], B operand of O (N = 128, K = 64): SBO 1024
+constexpr int ST_SMEM = ST_QTILE + 2 * ST_KTILE + ST_VTILE;
 
 // exp_tab[b] = exp((double)bf16(b)) for all 65536 bit patterns
 __global__ void exp_tab_kernel(double* __restrict__ tab) {
@@ -36,280 +37,51 @@ __global__ void exp_tab_kernel(double* __restrict__ tab) {
   if (i < 65536) tab[i] = exp((double)bf2f((uint16_t)i));
 }
 
-// element (r, c) of a K-major 128 x 128 operand tile: core matrix (r / 8, c / 8) = 128 contiguous bytes
+// element (r, c) of a K-major operand tile with 128 columns: core matrix (r / 8, c / 8) = 128 contiguous bytes
 LNB_DEVINL uint32_t st_off(int r, int c) { return (uint32_t)((((r >> 3) * 16 + (c >> 3)) * 8 + (r & 7)) * 16 + (c & 7) * 2); }
-
-
-// exp_f64 of 8 scores at once: the table loads are issued unconditionally and together (a masked entry reads exp(-inf) = 0,
-// which adds nothing to Z and gives p = 0), so their L1 latencies overlap -- with one conditional load per score the warps sat
-// on the long scoreboard for 12.5 of every 13 stall cycles (profiles/r02_tensor_kernels_ncu.txt)
-LNB_DEVINL void st_exp8(const uint32_t* __restrict__ acc8, int t_first, int qpos, int t_end, float scale, const double* __restrict__ tab,
-                        double (&ev)[8]) {
-  uint32_t idx[8];
-#pragma unroll
-  for (int e = 0; e < 8; e++) {
-    float sc = trunc_bf(__uint_as_float(acc8[e]));
-    sc = trunc_bf(__fdiv_rn(sc, scale));
-    const int t = t_first + e;
-    idx[e] = (t <= qpos && t < t_end) ? (__float_as_uint(sc) >> 16) : 0xff80u;      // 0xff80 = bf16 -inf
-  }
-#pragma unroll
-  for (int e = 0; e < 8; e++) ev[e] = __ldg(tab + idx[e]);
-}
-
-__global__ void __launch_bounds__(256, 2) sdpa_tc_kernel(const uint16_t* __restrict__ q, int ldq, const uint16_t* __restrict__ cache_k,
-                                                         const uint16_t* __restrict__ cache_v, int kv_dim, int n_rep,
-                                                         uint16_t* __restrict__ out_x8, int ldo, const int32_t* __restrict__ pos_ptr,
-                                                         int S, float scale_bf16_as_f32, const double* __restrict__ exp_tab) {
-  pdl_launch_dependents();
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* mma_bar = reinterpret_cast<uint64_t*>(smem);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + 16);
-  uint8_t* sQ = smem + 1024;
-  uint8_t* sK = sQ + ST_TILE;
-  uint8_t* sV = sK + ST_TILE;      // V^T: row = d, column = key
-  uint8_t* sP = sK;                // P replaces K once S = Q.K^T is complete
-  double* sZh = reinterpret_cast<double*>(sV + ST_TILE);   // [2][128] per column half
-  double* sZ = sZh + 256;                                  // [128]
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int H = blockIdx.x, h = H / n_rep;
-  const int qt = (int)gridDim.y - 1 - (int)blockIdx.y;     // the long (late) query tiles start first
-  const int s0 = qt * 128;
-  if (tid == 0) {
-    mbar_init(mma_bar, 1);
-    mbar_fence_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tS = tmem_base, tO = tmem_base + 128;
-  pdl_wait();
-  const int pos0 = *pos_ptr;
-  const int t_end = min(pos0 + S, pos0 + s0 + 128);        // keys this row block can see
-  const int n_tiles = (t_end + 127) / 128;
-  const bool lead = (warp == 0) && elect_one();
-  uint32_t mma_phase = 0;
-
-  // Q tile: 2048 pieces of 16 bytes (row r, chunk c8)
-  for (int i = tid; i < 2048; i += 256) {
-    const int r = i >> 4, c8 = i & 15;
-    uint4 v = make_uint4(0u, 0u, 0u, 0u);
-    if (s0 + r < S) v = *reinterpret_cast<const uint4*>(q + (size_t)(s0 + r) * ldq + (size_t)H * 128 + c8 * 8);
-    *reinterpret_cast<uint4*>(sQ + st_off(r, c8 * 8)) = v;
-  }
-  auto load_k = [&](int tile) {
-    const int t0 = tile * 128;
-    for (int i = tid; i < 2048; i += 256) {
-      const int r = i >> 4, c8 = i & 15;
-      uint4 v = make_uint4(0u, 0u, 0u, 0u);
-      if (t0 + r < t_end) v = *reinterpret_cast<const uint4*>(cache_k + (size_t)(t0 + r) * kv_dim + (size_t)h * 128 + c8 * 8);
-      *reinterpret_cast<uint4*>(sK + st_off(r, c8 * 8)) = v;
-    }
-  };
-  auto load_vt = [&](int tile) {
-    const int t0 = tile * 128;
-    for (int i = tid; i < 2048; i += 256) {
-      const int tl = i & 127, c8 = i >> 7;                 // consecutive lanes = consecutive keys
-      uint4 v = make_uint4(0u, 0u, 0u, 0u);
-      if (t0 + tl < t_end) v = *reinterpret_cast<const uint4*>(cache_v + (size_t)(t0 + tl) * kv_dim + (size_t)h * 128 + c8 * 8);
-      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-      for (int e = 0; e < 8; e++)
-        *reinterpret_cast<uint16_t*>(sV + st_off(c8 * 8 + e, tl)) = (uint16_t)((e & 1) ? (w[e >> 1] >> 16) : (w[e >> 1] & 0xffffu));
-    }
-  };
-  // D[128 x 128] (+)= A . B^T over the 128-wide k extent of two operand tiles
-  auto mma_tile = [&](uint32_t d_tmem, const uint8_t* a, const uint8_t* b, bool accumulate) {
-    if (lead) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, 128);
-      uint64_t a_desc = umma_desc(smem_u32(a), 128, 2048);   // next chunk 128 B, next 8 rows 2048 B, next k16 step 256 B
-      uint64_t b_desc = umma_desc(smem_u32(b), 128, 2048);
-#pragma unroll
-      for (int k16 = 0; k16 < 8; k16++) {
-        umma_bf16(d_tmem, a_desc, b_desc, idesc, (accumulate || k16 > 0) ? 1u : 0u);
-        a_desc += 16; b_desc += 16;
-      }
-      umma_commit(mma_bar);
-    }
-    __syncwarp();
-  };
-  auto mma_wait = [&]() {
-    mbar_wait(mma_bar, mma_phase);
-    mma_phase ^= 1u;
-    tc_fence_after();
-  };
-
-  const int row = (warp & 3) * 32 + lane;                  // TMEM lane = query row of the tile
-  const int half = warp >> 2;                              // columns [64 * half, 64 * half + 64)
-  const int qpos = pos0 + s0 + row;                        // keys t <= qpos are visible to this row
-  const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-
-  // ---------------- pass 1: row sums of exp ------------------------------------------------------------------------
-  double z = 0.0;
-  for (int tile = 0; tile < n_tiles; tile++) {
-    load_k(tile);
-    fence_proxy_async_smem();
-    __syncthreads();
-    mma_tile(tS, sQ, sK, false);
-    mma_wait();
-    const int t0 = tile * 128 + half * 64;
-#pragma unroll 1
-    for (int cb = 0; cb < 64; cb += 16) {
-      uint32_t acc[16];
-      tmem_ld16(tS + lane_sel + (uint32_t)(half * 64 + cb), acc);
-#pragma unroll
-      for (int g8 = 0; g8 < 16; g8 += 8) {
-        double ev[8];
-        st_exp8(acc + g8, t0 + cb + g8, qpos, t_end, scale_bf16_as_f32, exp_tab, ev);
-#pragma unroll
-        for (int e = 0; e < 8; e++) z = __dadd_rn(z, ev[e]);
-      }
-    }
-    tc_fence_before();
-    __syncthreads();                                       // S and the K tile are free again
-  }
-  sZh[half * 128 + row] = z;
-  __syncthreads();
-  if (tid < 128) sZ[tid] = __dadd_rn(sZh[tid], sZh[128 + tid]);
-  __syncthreads();
-  // p = t(f32(e * (1/Z))): the reference divides (e / Z); multiplying by the f64 reciprocal differs from the quotient by at most
-  // one f64 ulp, which survives the rounding to f32 AND the truncation to bf16 with probability ~2^-45 per element -- and an
-  // f64 division per score is ~30 FP64 instructions against one (this kernel is LNB_ACC_FAST only)
-  const double rZ = __ddiv_rn(1.0, sZ[row]);
-
-  // ---------------- pass 2: p = t(f32(e / Z)), O += P . V -----------------------------------------------------------
-  for (int tile = 0; tile < n_tiles; tile++) {
-    load_k(tile);
-    load_vt(tile);
-    fence_proxy_async_smem();
-    __syncthreads();
-    mma_tile(tS, sQ, sK, false);
-    mma_wait();
-    const int t0 = tile * 128 + half * 64;
-#pragma unroll 1
-    for (int cb = 0; cb < 64; cb += 16) {
-      uint32_t acc[16];
-      tmem_ld16(tS + lane_sel + (uint32_t)(half * 64 + cb), acc);
-      uint32_t pk[8];
-#pragma unroll
-      for (int g8 = 0; g8 < 16; g8 += 8) {
-        double ev[8];
-        st_exp8(acc + g8, t0 + cb + g8, qpos, t_end, scale_bf16_as_f32, exp_tab, ev);
-#pragma unroll
-        for (int e = 0; e < 8; e += 2) {
-          const float p0 = (float)__dmul_rn(ev[e], rZ), p1 = (float)__dmul_rn(ev[e + 1], rZ);
-          pk[(g8 + e) >> 1] = (__float_as_uint(p0) >> 16) | (__float_as_uint(p1) & 0xffff0000u);
-        }
-      }
-      uint8_t* dst = sP + st_off(row, half * 64 + cb);
-      *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);          // columns cb .. cb+7 of this row
-      *reinterpret_cast<uint4*>(dst + 128) = make_uint4(pk[4], pk[5], pk[6], pk[7]);    // the next chunk
-    }
-    tc_fence_before();
-    fence_proxy_async_smem();
-    __syncthreads();
-    mma_tile(tO, sP, sV, tile > 0);
-    mma_wait();                                            // P, V^T, K and S are free again
-    tc_fence_before();
-    __syncthreads();
-  }
-
-  // ---------------- O -> t(.) -> the X8 operand of the Wo GEMM ------------------------------------------------------
-  const int srow = s0 + row;
-#pragma unroll 1
-  for (int cb = 0; cb < 64; cb += 16) {
-    uint32_t acc[16];
-    tmem_ld16(tO + lane_sel + (uint32_t)(half * 64 + cb), acc);
-    if (srow < S) {
-#pragma unroll
-      for (int g = 0; g < 2; g++) {
-        uint4 w;
-        w.x = (acc[g * 8 + 0] >> 16) | (acc[g * 8 + 1] & 0xffff0000u);
-        w.y = (acc[g * 8 + 2] >> 16) | (acc[g * 8 + 3] & 0xffff0000u);
-        w.z = (acc[g * 8 + 4] >> 16) | (acc[g * 8 + 5] & 0xffff0000u);
-        w.w = (acc[g * 8 + 6] >> 16) | (acc[g * 8 + 7] & 0xffff0000u);
-        *reinterpret_cast<uint4*>(out_x8 + x8_index(srow, H * 128 + half * 64 + cb + g * 8, ldo)) = w;   // 8 columns = one chunk
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
-  }
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------------
-// sdpa_tc2_kernel -- the same arithmetic, software-pipelined.  ncu of sdpa_tc_kernel (profiles/r02_tensor_kernels_ncu.txt):
-// 0.19 instructions per cycle and scheduler, tensor pipe 4 % active -- every tile pays the latency of its serial chain
-// load K/V -> barrier -> MMA -> wait -> softmax -> barrier -> MMA -> wait.  Here (64-key tiles):
-//   * K tiles are double-buffered and arrive with cp.async two tiles ahead (no registers, zero-filled past the last key);
-//   * S is double-buffered in TMEM (2 x 64 columns): S_{j+1} = Q . K_{j+1}^T is issued BEFORE the softmax of tile j and runs
-//     on the tensor pipe meanwhile;
-//   * V rows of tile j are fetched into 16 registers before the softmax and transposed into shared memory after it;
-//   * O += P_j . V_j is waited for one tile later, just before P and V^T are overwritten.
-// Shared memory: Q 32 KB + 2 x K 16 KB + V^T 16 KB + P 16 KB = 100 KB (two CTAs per SM, as before); TMEM 256 columns.
-constexpr int SX_BK = 64;
-constexpr int SX_KTILE = SX_BK * 128 * 2;       // 16 KB: [64 keys][128 d], B operand of S (N = 64, K = 128): SBO 2048
-constexpr int SX_VTILE = 128 * SX_BK * 2;       // 16 KB: [128 d][64 keys], B operand of O (N = 128, K = 64): SBO 1024
-constexpr int SX_PTILE = 128 * SX_BK * 2;       // 16 KB: [128 rows][64 keys], A operand of O (M = 128, K = 64): SBO 1024
-constexpr int SX_SMEM = 1024 + ST_TILE + 2 * SX_KTILE + SX_VTILE + SX_PTILE + 128 * 8 * 3;
-
-// element (r, c) of a K-major operand tile with 64 columns: core matrix (r / 8, c / 8)
+// element (r, c) of a K-major operand tile with 64 columns
 LNB_DEVINL uint32_t sx_off64(int r, int c) { return (uint32_t)((((r >> 3) * 8 + (c >> 3)) * 8 + (r & 7)) * 16 + (c & 7) * 2); }
 LNB_DEVINL void cp_async16_zfill(void* smem_dst, const void* gsrc, bool valid) {
   const uint32_t n = valid ? 16u : 0u;          // src-size 0: the 16 bytes are written as zeros, nothing is read
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(n) : "memory");
 }
-LNB_DEVINL void cp_async_commit_wait_all() {
-  asm volatile("cp.async.commit_group;" ::: "memory");
-  asm volatile("cp.async.wait_group 0;" ::: "memory");
-}
 LNB_DEVINL void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 LNB_DEVINL void cp_async_wait0() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
-__global__ void __launch_bounds__(256, 2) sdpa_tc2_kernel(const uint16_t* __restrict__ q, int ldq, const uint16_t* __restrict__ cache_k,
-                                                          const uint16_t* __restrict__ cache_v, int kv_dim, int n_rep,
-                                                          uint16_t* __restrict__ out_x8, int ldo, const int32_t* __restrict__ pos_ptr,
-                                                          int S, float scale_bf16_as_f32, const double* __restrict__ exp_tab) {
+// exp_f64 of the scores of one row: two consecutive keys t, t + 1 (a masked entry reads exp(-inf) = 0, which adds nothing to Z
+// and gives p = 0); both table loads are issued before either is used
+LNB_DEVINL void st_exp2(float a0, float a1, int t, int qpos, int t_end, float scale, const double* __restrict__ tab, double& e0,
+                        double& e1) {
+  float s0 = trunc_bf(__fdiv_rn(trunc_bf(a0), scale)), s1 = trunc_bf(__fdiv_rn(trunc_bf(a1), scale));
+  const uint32_t i0 = (t <= qpos && t < t_end) ? (__float_as_uint(s0) >> 16) : 0xff80u;        // 0xff80 = bf16 -inf
+  const uint32_t i1 = (t + 1 <= qpos && t + 1 < t_end) ? (__float_as_uint(s1) >> 16) : 0xff80u;
+  e0 = __ldg(tab + i0);
+  e1 = __ldg(tab + i1);
+}
+
+__global__ void __launch_bounds__(256, 1) sdpa_tc_kernel(const uint16_t* __restrict__ q, int ldq, const uint16_t* __restrict__ cache_k,
+                                                         const uint16_t* __restrict__ cache_v, int kv_dim, int n_rep,
+                                                         uint16_t* __restrict__ out_x8, int ldo, const int32_t* __restrict__ pos_ptr,
+                                                         int S, float scale_bf16_as_f32, const double* __restrict__ exp_tab) {
   pdl_launch_dependents();
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* s_bar = reinterpret_cast<uint64_t*>(smem);          // [2] S buffers complete
-  uint64_t* pv_bar = s_bar + 2;                                 // O += P . V of a tile complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem + 32);
-  uint8_t* sQ = smem + 1024;
-  uint8_t* sK = sQ + ST_TILE;                                   // [2] K tiles
-  uint8_t* sV = sK + 2 * SX_KTILE;                              // V^T: row = d, column = key
-  uint8_t* sP = sV + SX_VTILE;
-  double* sZh = reinterpret_cast<double*>(sP + SX_PTILE);       // [2][128] per column half
-  double* sZ = sZh + 256;                                       // [128]
+  uint8_t* sQ = smem;
+  uint8_t* sK = sQ + ST_QTILE;                                  // [2] K tiles
+  uint8_t* sV = sK + 2 * ST_KTILE;                              // V^T: row = d, column = key
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int wg = warp >> 2;
   const int H = blockIdx.x, h = H / n_rep;
   const int qt = (int)gridDim.y - 1 - (int)blockIdx.y;          // the long (late) query tiles start first
   const int s0 = qt * 128;
-  if (tid == 0) {
-    mbar_init(&s_bar[0], 1);
-    mbar_init(&s_bar[1], 1);
-    mbar_init(pv_bar, 1);
-    mbar_fence_init();
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tO = tmem_base + 128;
   pdl_wait();
   const int pos0 = *pos_ptr;
   const int t_end = min(pos0 + S, pos0 + s0 + 128);             // keys this row block can see
-  const int n_tiles = (t_end + SX_BK - 1) / SX_BK;
-  const bool lead = (warp == 0) && elect_one();
+  const int n_tiles = (t_end + ST_BK - 1) / ST_BK;
+  // this thread's rows of the tile (fragment layout: row r_lo for accumulators 4c, 4c+1; r_lo + 8 for 4c+2, 4c+3) and columns
+  const int r_lo = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const int qpos_lo = pos0 + s0 + r_lo, qpos_hi = qpos_lo + 8;  // keys t <= qpos are visible to a row
 
   // Q tile: 2048 pieces of 16 bytes (row r, chunk c8)
   for (int i = tid; i < 2048; i += 256) {
@@ -320,116 +92,76 @@ __global__ void __launch_bounds__(256, 2) sdpa_tc2_kernel(const uint16_t* __rest
   }
   // K tile j -> buffer j & 1, asynchronously (4 pieces of 16 bytes per thread)
   auto prefetch_k = [&](int tile) {
-    const int t0 = tile * SX_BK;
-    uint8_t* dst = sK + (size_t)(tile & 1) * SX_KTILE;
+    const int t0 = tile * ST_BK;
+    uint8_t* dst = sK + (size_t)(tile & 1) * ST_KTILE;
 #pragma unroll
     for (int u = 0; u < 4; u++) {
       const int i = tid + u * 256, r = i >> 4, c8 = i & 15;
       const bool ok = t0 + r < t_end;
       const uint16_t* src = cache_k + (size_t)(ok ? t0 + r : 0) * kv_dim + (size_t)h * 128 + c8 * 8;
-      cp_async16_zfill(dst + st_off(r, c8 * 8), src, ok);        // (st_off: 16 chunks per row group, as in the 128-row tiles)
+      cp_async16_zfill(dst + st_off(r, c8 * 8), src, ok);
     }
     cp_async_commit();
   };
-  // S[tile & 1] = Q . K_tile^T   (M 128, N 64, K 128: 8 MMAs)
-  auto issue_s = [&](int tile) {
-    if (lead) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, SX_BK);
-      uint64_t a_desc = umma_desc(smem_u32(sQ), 128, 2048);
-      uint64_t b_desc = umma_desc(smem_u32(sK + (size_t)(tile & 1) * SX_KTILE), 128, 2048);
-      const uint32_t d = tmem_base + (uint32_t)((tile & 1) * SX_BK);
+  // S = Q . K_tile^T for this warpgroup's 64 rows (M 64, N 64, K 128: 8 MMAs), complete on return
+  auto scores = [&](int tile, float (&sacc)[32]) {
+    uint64_t a_desc = gmma_desc(smem_u32(sQ) + (uint32_t)wg * 8u * 2048u, 128, 2048);
+    uint64_t b_desc = gmma_desc(smem_u32(sK + (size_t)(tile & 1) * ST_KTILE), 128, 2048);
+    wgmma_fence();
 #pragma unroll
-      for (int k16 = 0; k16 < 8; k16++) {
-        umma_bf16(d, a_desc, b_desc, idesc, k16 > 0 ? 1u : 0u);
-        a_desc += 16; b_desc += 16;
-      }
-      umma_commit(&s_bar[tile & 1]);
+    for (int k16 = 0; k16 < 8; k16++) {
+      wgmma_ss_n64(sacc, a_desc, b_desc, k16 > 0 ? 1u : 0u);
+      a_desc += 16; b_desc += 16;
     }
-    __syncwarp();
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sacc);
   };
-  auto wait_s = [&](int tile) {
-    mbar_wait(&s_bar[tile & 1], (uint32_t)(tile >> 1) & 1u);
-    tc_fence_after();
-  };
-
-  const int row = (warp & 3) * 32 + lane;                       // TMEM lane = query row of the tile
-  const int half = warp >> 2;                                   // S: columns [32 half, +32); O: columns [64 half, +64)
-  const int qpos = pos0 + s0 + row;                             // keys t <= qpos are visible to this row
-  const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
 
   // ---------------- pass 1: row sums of exp ------------------------------------------------------------------------
-  double z = 0.0;
+  double z_lo = 0.0, z_hi = 0.0;
+  float sacc[32];
+#pragma unroll
+  for (int i = 0; i < 32; i++) sacc[i] = 0.f;
   prefetch_k(0);
-  cp_async_wait0();
-  fence_proxy_async_smem();
-  __syncthreads();
-  issue_s(0);
-  if (n_tiles > 1) prefetch_k(1);
   for (int tile = 0; tile < n_tiles; tile++) {
-    if (tile + 1 < n_tiles) {
-      cp_async_wait0();                                         // K_{tile+1} (issued one iteration ago) has landed
-      fence_proxy_async_smem();
-      __syncthreads();                                          // ... for everybody; and S[(tile+1) & 1] has been read out
-      issue_s(tile + 1);                                        // runs during this tile's softmax
-    }
-    wait_s(tile);
-    if (tile + 2 < n_tiles) prefetch_k(tile + 2);               // buffer tile & 1 is free: S_tile is complete
-    const int t0 = tile * SX_BK + half * 32;
-#pragma unroll 1
-    for (int cb = 0; cb < 32; cb += 16) {
-      uint32_t acc[16];
-      tmem_ld16(tmem_base + lane_sel + (uint32_t)((tile & 1) * SX_BK + half * 32 + cb), acc);
+    cp_async_wait0();                                           // this thread's pieces of K_tile have landed
+    fence_proxy_async_smem();
+    __syncthreads();                                            // ... everybody's; and the other buffer's MMAs are complete
+    if (tile + 1 < n_tiles) prefetch_k(tile + 1);
+    scores(tile, sacc);
+    const int t0 = tile * ST_BK + cq;
 #pragma unroll
-      for (int g8 = 0; g8 < 16; g8 += 8) {
-        double ev[8];
-        st_exp8(acc + g8, t0 + cb + g8, qpos, t_end, scale_bf16_as_f32, exp_tab, ev);
-#pragma unroll
-        for (int e = 0; e < 8; e++) z = __dadd_rn(z, ev[e]);
-      }
+    for (int c = 0; c < 8; c++) {
+      double e0, e1, e2, e3;
+      st_exp2(sacc[4 * c], sacc[4 * c + 1], t0 + 8 * c, qpos_lo, t_end, scale_bf16_as_f32, exp_tab, e0, e1);
+      st_exp2(sacc[4 * c + 2], sacc[4 * c + 3], t0 + 8 * c, qpos_hi, t_end, scale_bf16_as_f32, exp_tab, e2, e3);
+      z_lo = __dadd_rn(__dadd_rn(z_lo, e0), e1);
+      z_hi = __dadd_rn(__dadd_rn(z_hi, e2), e3);
     }
-    tc_fence_before();
   }
-  sZh[half * 128 + row] = z;
-  __syncthreads();
-  if (tid < 128) sZ[tid] = __dadd_rn(sZh[tid], sZh[128 + tid]);
-  __syncthreads();
-  const double rZ = __ddiv_rn(1.0, sZ[row]);                    // p = t(f32(e * (1/Z))), see sdpa_tc_kernel
+  // the four threads of a row: (z0 + z1) + (z2 + z3), the same bits in all four
+#pragma unroll
+  for (int o = 1; o <= 2; o <<= 1) {
+    z_lo = __dadd_rn(z_lo, __shfl_xor_sync(0xffffffffu, z_lo, o));
+    z_hi = __dadd_rn(z_hi, __shfl_xor_sync(0xffffffffu, z_hi, o));
+  }
+  // p = t(f32(e * (1/Z))): the reference divides (e / Z); multiplying by the f64 reciprocal differs from the quotient by at most
+  // one f64 ulp, which survives the rounding to f32 AND the truncation to bf16 with probability ~2^-45 per element -- and an
+  // f64 division per score is ~30 FP64 instructions against one (this kernel is LNB_ACC_FAST only)
+  const double rz_lo = __ddiv_rn(1.0, z_lo), rz_hi = __ddiv_rn(1.0, z_hi);
 
   // ---------------- pass 2: p = t(f32(e / Z)), O += P . V -----------------------------------------------------------
-  // (all MMAs of pass 1 are complete: every S tile was waited for)
-  prefetch_k(0);
-  cp_async_wait0();
-  fence_proxy_async_smem();
-  __syncthreads();
-  // barrier uses continue to count from pass 1: S buffer b has been used ceil((n_tiles - b) / 2) times
-  const int used0 = (n_tiles + 1) >> 1, used1 = n_tiles >> 1;
-  auto issue_s2 = [&](int tile) {
-    if (lead) {
-      constexpr uint32_t idesc = umma_idesc_bf16(128, SX_BK);
-      uint64_t a_desc = umma_desc(smem_u32(sQ), 128, 2048);
-      uint64_t b_desc = umma_desc(smem_u32(sK + (size_t)(tile & 1) * SX_KTILE), 128, 2048);
-      const uint32_t d = tmem_base + (uint32_t)((tile & 1) * SX_BK);
+  float oacc[64];
 #pragma unroll
-      for (int k16 = 0; k16 < 8; k16++) {
-        umma_bf16(d, a_desc, b_desc, idesc, k16 > 0 ? 1u : 0u);
-        a_desc += 16; b_desc += 16;
-      }
-      umma_commit(&s_bar[tile & 1]);
-    }
-    __syncwarp();
-  };
-  auto wait_s2 = [&](int tile) {
-    const int k = (tile >> 1) + ((tile & 1) ? used1 : used0);
-    mbar_wait(&s_bar[tile & 1], (uint32_t)k & 1u);
-    tc_fence_after();
-  };
-  issue_s2(0);
-  if (n_tiles > 1) prefetch_k(1);
+  for (int i = 0; i < 64; i++) oacc[i] = 0.f;
+  __syncthreads();                                              // every pass-1 MMA is complete: both K buffers are free
+  prefetch_k(0);
   for (int tile = 0; tile < n_tiles; tile++) {
-    // V rows of this tile: 4 pieces of 16 bytes per thread, in flight during the softmax (consecutive lanes = consecutive keys)
+    // V rows of this tile: 4 pieces of 16 bytes per thread (consecutive lanes = consecutive keys)
     uint4 vreg[4];
     {
-      const int t0v = tile * SX_BK;
+      const int t0v = tile * ST_BK;
 #pragma unroll
       for (int u = 0; u < 4; u++) {
         const int i = tid + u * 256, tl = i & 63, c8 = i >> 6;
@@ -437,91 +169,56 @@ __global__ void __launch_bounds__(256, 2) sdpa_tc2_kernel(const uint16_t* __rest
         if (t0v + tl < t_end) vreg[u] = *reinterpret_cast<const uint4*>(cache_v + (size_t)(t0v + tl) * kv_dim + (size_t)h * 128 + c8 * 8);
       }
     }
-    if (tile + 1 < n_tiles) {
-      cp_async_wait0();
-      fence_proxy_async_smem();
-      __syncthreads();
-      issue_s2(tile + 1);
+    cp_async_wait0();
+    __syncthreads();                                            // the previous tile's O MMAs are complete: V^T is free
+#pragma unroll
+    for (int u = 0; u < 4; u++) {
+      const int i = tid + u * 256, tl = i & 63, c8 = i >> 6;
+      const uint32_t w[4] = {vreg[u].x, vreg[u].y, vreg[u].z, vreg[u].w};
+#pragma unroll
+      for (int e = 0; e < 8; e++)
+        *reinterpret_cast<uint16_t*>(sV + sx_off64(c8 * 8 + e, tl)) = (uint16_t)((e & 1) ? (w[e >> 1] >> 16) : (w[e >> 1] & 0xffffu));
     }
-    wait_s2(tile);
-    if (tile + 2 < n_tiles) prefetch_k(tile + 2);
-    const int t0 = tile * SX_BK + half * 32;
-    uint32_t pk[16];
-#pragma unroll
-    for (int cb = 0; cb < 32; cb += 16) {
-      uint32_t acc[16];
-      tmem_ld16(tmem_base + lane_sel + (uint32_t)((tile & 1) * SX_BK + half * 32 + cb), acc);
-#pragma unroll
-      for (int g8 = 0; g8 < 16; g8 += 8) {
-        double ev[8];
-        st_exp8(acc + g8, t0 + cb + g8, qpos, t_end, scale_bf16_as_f32, exp_tab, ev);
-#pragma unroll
-        for (int e = 0; e < 8; e += 2) {
-          const float p0 = (float)__dmul_rn(ev[e], rZ), p1 = (float)__dmul_rn(ev[e + 1], rZ);
-          pk[(cb >> 1) + ((g8 + e) >> 1)] = (__float_as_uint(p0) >> 16) | (__float_as_uint(p1) & 0xffff0000u);
-        }
-      }
-    }
-    tc_fence_before();
-    if (tile > 0) {                                             // O += P_{tile-1} . V_{tile-1} is complete: P and V^T are free
-      mbar_wait(pv_bar, (uint32_t)(tile - 1) & 1u);
-      tc_fence_after();
-    }
-    {
-      uint8_t* dst = sP + sx_off64(row, half * 32);             // 4 chunks of 8 columns, 128 bytes apart
-#pragma unroll
-      for (int g = 0; g < 4; g++) *reinterpret_cast<uint4*>(dst + g * 128) = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-#pragma unroll
-      for (int u = 0; u < 4; u++) {
-        const int i = tid + u * 256, tl = i & 63, c8 = i >> 6;
-        const uint32_t w[4] = {vreg[u].x, vreg[u].y, vreg[u].z, vreg[u].w};
-#pragma unroll
-        for (int e = 0; e < 8; e++)
-          *reinterpret_cast<uint16_t*>(sV + sx_off64(c8 * 8 + e, tl)) = (uint16_t)((e & 1) ? (w[e >> 1] >> 16) : (w[e >> 1] & 0xffffu));
-      }
-    }
-    tc_fence_before();
     fence_proxy_async_smem();
     __syncthreads();
-    if (lead) {                                                 // O (+)= P . V   (M 128, N 128, K 64: 4 MMAs)
-      constexpr uint32_t idesc = umma_idesc_bf16(128, 128);
-      uint64_t a_desc = umma_desc(smem_u32(sP), 128, 1024);
-      uint64_t b_desc = umma_desc(smem_u32(sV), 128, 1024);
+    if (tile + 1 < n_tiles) prefetch_k(tile + 1);
+    scores(tile, sacc);
+    // P as the A fragments of 4 k16 steps: step j covers keys 16j .. 16j+15 = score blocks 2j and 2j+1; fragment registers
+    // 0, 1, 2, 3 = (row r_lo, block 2j), (r_lo + 8, 2j), (r_lo, 2j+1), (r_lo + 8, 2j+1)
+    uint32_t pa[4][4];
+    const int t0 = tile * ST_BK + cq;
 #pragma unroll
-      for (int k16 = 0; k16 < 4; k16++) {
-        umma_bf16(tO, a_desc, b_desc, idesc, (tile > 0 || k16 > 0) ? 1u : 0u);
-        a_desc += 16; b_desc += 16;
-      }
-      umma_commit(pv_bar);
+    for (int c = 0; c < 8; c++) {
+      double e0, e1, e2, e3;
+      st_exp2(sacc[4 * c], sacc[4 * c + 1], t0 + 8 * c, qpos_lo, t_end, scale_bf16_as_f32, exp_tab, e0, e1);
+      st_exp2(sacc[4 * c + 2], sacc[4 * c + 3], t0 + 8 * c, qpos_hi, t_end, scale_bf16_as_f32, exp_tab, e2, e3);
+      const float p0 = (float)__dmul_rn(e0, rz_lo), p1 = (float)__dmul_rn(e1, rz_lo);
+      const float p2 = (float)__dmul_rn(e2, rz_hi), p3 = (float)__dmul_rn(e3, rz_hi);
+      pa[c >> 1][(c & 1) * 2 + 0] = (__float_as_uint(p0) >> 16) | (__float_as_uint(p1) & 0xffff0000u);
+      pa[c >> 1][(c & 1) * 2 + 1] = (__float_as_uint(p2) >> 16) | (__float_as_uint(p3) & 0xffff0000u);
     }
-    __syncwarp();
+    uint64_t b_desc = gmma_desc(smem_u32(sV), 128, 1024);
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 4; j++) {                               // O += P . V   (M 64, N 128, K 64: 4 MMAs)
+      wgmma_rs_n128(oacc, pa[j], b_desc, 1u);
+      b_desc += 16;
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(oacc);
   }
-  mbar_wait(pv_bar, (uint32_t)(n_tiles - 1) & 1u);
-  tc_fence_after();
 
   // ---------------- O -> t(.) -> the X8 operand of the Wo GEMM ------------------------------------------------------
-  const int srow = s0 + row;
-#pragma unroll 1
-  for (int cb = 0; cb < 64; cb += 16) {
-    uint32_t acc[16];
-    tmem_ld16(tO + lane_sel + (uint32_t)(half * 64 + cb), acc);
+#pragma unroll
+  for (int hr = 0; hr < 2; hr++) {
+    const int srow = s0 + r_lo + 8 * hr;
     if (srow < S) {
 #pragma unroll
-      for (int g = 0; g < 2; g++) {
-        uint4 w;
-        w.x = (acc[g * 8 + 0] >> 16) | (acc[g * 8 + 1] & 0xffff0000u);
-        w.y = (acc[g * 8 + 2] >> 16) | (acc[g * 8 + 3] & 0xffff0000u);
-        w.z = (acc[g * 8 + 4] >> 16) | (acc[g * 8 + 5] & 0xffff0000u);
-        w.w = (acc[g * 8 + 6] >> 16) | (acc[g * 8 + 7] & 0xffff0000u);
-        *reinterpret_cast<uint4*>(out_x8 + x8_index(srow, H * 128 + half * 64 + cb + g * 8, ldo)) = w;   // 8 columns = one chunk
-      }
+      for (int c = 0; c < 16; c++)
+        *reinterpret_cast<uint32_t*>(out_x8 + x8_index(srow, H * 128 + 8 * c + cq, ldo)) =
+            (__float_as_uint(oacc[4 * c + 2 * hr]) >> 16) | (__float_as_uint(oacc[4 * c + 2 * hr + 1]) & 0xffff0000u);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 256);
   }
 }
 

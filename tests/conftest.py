@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (sm_90a); run with -m gpu")
     config.addinivalue_line("markers", "slow: full-size 8B oracle runs (minutes of CPU)")
 
 

@@ -3,9 +3,10 @@ writes tests/golden/reference_vectors.json.
 
 The reference is Go (no toolchain in the image), so it cannot be imported or run to generate fixtures; its tests
 however hold literal known answers for this path (SURVEY 8c).  This script parses those literals where they lie
-under /root/reference (read-only) and records file:line for each, so the committed fixture is provably the
-reference's data and not a transcription.  Run here:  python tests/golden/extract_reference_vectors.py
-(/root/reference does not exist on the GPU box; tests only read the committed JSON.)"""
+in a checkout of the reference (LNB_REFERENCE_DIR) and records file:line for each, so the committed fixture is provably
+the reference's data and not a transcription.  Run: LNB_REFERENCE_DIR=<checkout> python tests/golden/extract_reference_vectors.py
+It also writes reference_vectors.sha256, the digest tests/test_oracle_golden.py checks the fixture against; the tests
+only read the committed files."""
 import json
 import os
 import re
@@ -179,6 +180,10 @@ def main():
     with open(OUT, "w") as f:
         json.dump(out, f, indent=1, sort_keys=True)
         f.write("\n")
+    import hashlib
+    canon = json.dumps(out, sort_keys=True, separators=(",", ":")).encode()
+    with open(os.path.splitext(OUT)[0] + ".sha256", "w") as f:
+        f.write(hashlib.sha256(canon).hexdigest() + "\n")
     print("wrote", OUT)
 
 

@@ -1,7 +1,7 @@
 """GPU parity at the BASELINE size: the synthetic Llama-3.1-8B checkpoint (random-init weights of the 8B architecture,
 the same bits in HBM and in the oracle's host copy) through the model-level C-ABI, teacher-forced against the CPU
 oracle; and the op-level linear at the two largest projection shapes of the model.  The oracle costs about 0.1 s per
-S=1 step on the GPU box's cores, so a dozen positions fit a test run; bench.py compares all 128 generated tokens.
+S=1 step on the host cores of a GPU machine, so a dozen positions fit a test run; bench.py compares all 128 generated tokens.
 
 STRICT must reproduce the oracle bit for bit (north_star: logits within 1e-2, greedy ids identical -- met with 0.0).
 FAST is a documented reorder of the long fp32 sums: every logit stays within a few bf16 ulps, and the test pins the

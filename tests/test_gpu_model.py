@@ -185,7 +185,7 @@ def test_device_resident_decode_equals_host_loop(L, tiny, use_graph):
 
 
 def test_prefill_tensor_core_path(L, tiny):
-    """LNB_ACC_FAST with a prompt of >= 32 tokens runs the tcgen05 prefill path (gemm_tc.cuh + X8
+    """LNB_ACC_FAST with a prompt of >= 32 tokens runs the tensor-core prefill path (gemm_tc.cuh + X8
     elementwise kernels); it must agree with the oracle up to fp32 summation order, and the KV cache it
     leaves must drive the ordinary decode path."""
     args, _, om, gm = tiny
@@ -272,11 +272,42 @@ def test_cpp_host_mirror_generates_the_oracle_tokens(L):
     om.close()
 
 
-@pytest.mark.parametrize("mode", ["strict", "fast"])
-def test_batched_decode_equals_independent_contexts(L, tiny, mode):
+@pytest.mark.parametrize("mode", ["strict", "fast", "fast_tc"])
+def test_batched_decode_equals_independent_contexts(L, tiny, mode, monkeypatch):
     """config 5: n_seq sequences stepped together through one pass over the weights; STRICT: every sequence is
-    bit-identical to its own oracle InferenceContext (different prompt lengths, different positions)."""
-    args, _, om, gm = tiny
+    bit-identical to its own oracle InferenceContext (different prompt lengths, different positions).  fast_tc: the
+    batch engine's tensor-core form (LNB_BATCH_TC=1)."""
+    if mode == "fast_tc":
+        monkeypatch.setenv("LNB_BATCH_TC", "1")
+    check_batched_decode(L, tiny, mode)
+
+
+@pytest.fixture(scope="module")
+def wide(L):
+    """TINY with a 4096-wide FFN and a 16384-entry vocabulary: on any GPU with at most 256 SMs a CTA of the batch engine owns
+    more than 4 panels (32 rows) of w1|w3 and of the LM head, so the tensor-core form issues several 32-row slices per tile"""
+    args = dict(L.synth.TINY, ffn_dim=4096, vocab_size=16384)
+    tensors = host_tensors(args, SEED)
+    om = oracle_model(args, tensors)
+    gm = L.model.LoadModelFromTensors(args, tensors)
+    yield args, tensors, om, gm
+    gm.Free()
+    om.close()
+
+
+def test_batch_engine_tensor_core_form_on_wide_projections(L, wide, monkeypatch):
+    """the tensor-core form of the batch engine (LNB_BATCH_TC=1) with several 32-row slices per row tile: every sequence's
+    logits stay within FAST's tolerance of its own oracle context"""
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    args = wide[0]
+    assert -(-(2 * args["ffn_dim"] // 8) // sms) > 4 and -(-(args["vocab_size"] // 8) // sms) > 4
+    monkeypatch.setenv("LNB_BATCH_TC", "1")
+    check_batched_decode(L, wide, "fast_tc")
+
+
+def check_batched_decode(L, model, mode):
+    args, _, om, gm = model
     acc = L._capi.LNB_ACC_STRICT if mode == "strict" else L._capi.LNB_ACC_FAST
     rng = np.random.default_rng(55)
     seq, nseq = 32, 5

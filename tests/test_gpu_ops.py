@@ -189,8 +189,8 @@ def test_attention_strict_bit_exact(L, S, T, causal):
                                         S, T, nh, nkv, hd, causal, c.LNB_ACC_FAST))
     if S >= 32 and causal:
         # prompt-sized FAST attention runs sdpa_tc_kernel: q.k and p.v accumulate in the tensor core's order, so a score or an
-        # output can land on the other side of a bf16 truncation boundary (measured on B200: 0.05 % of the outputs differ,
-        # max-abs 0.0024 = a third of a bf16 ulp at 1.0; tools/sdpa_tc_check.py)
+        # output can land on the other side of a bf16 truncation boundary (a small fraction of the outputs, by at most one
+        # bf16 ulp; tools/sdpa_tc_check.py measures it)
         d = np.abs(O.bf16_to_f32(out).astype(np.float64) - O.bf16_to_f32(exp).astype(np.float64))
         assert d.max() <= 2.0 ** -7 and (out != exp).mean() < 5e-3
     else:
@@ -237,7 +237,7 @@ def test_softmax_argmax_getrows(L):
         ml.Fwd_Get_Rows(ml.Tensor(emb, ml.DT_BF16), ml.Tensor(np.array([64], np.int32), ml.DT_INT32))
 
 
-# ---- tensor-core prefill GEMM (tcgen05) behind ml.LinearTransformation ------------------------
+# ---- tensor-core prefill GEMM (wgmma) behind ml.LinearTransformation -------------------------
 
 @pytest.mark.parametrize("S,K,N", [(32, 64, 128), (128, 128, 128), (200, 4096, 256), (256, 1024, 1024), (130, 14336, 128)])
 def test_linear_tensor_core_prefill(L, S, K, N):

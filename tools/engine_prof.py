@@ -1,5 +1,5 @@
 """Where the persistent decode engine spends its time (LNB_ENGINE_PROF=1): cycles of consumer thread 0 per section, mean
-and max over the 148 CTAs, for a full decode run and for every projection phase alone.  Usage: python tools/engine_prof.py [fast,strict]"""
+and max over the CTAs, for a full decode run and for every projection phase alone.  Usage: python tools/engine_prof.py [fast,strict]"""
 import os
 import sys
 

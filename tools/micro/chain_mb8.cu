@@ -3,7 +3,7 @@
 // latency-bound.  How many such warps does an SM need before the FFMA pipe saturates, and what does one k cost?
 // Expectation: ~11 instructions per k per warp (8 FFMA + 1 cvt + 2 LDS.128 of x + 1/8 LDS.128 of w); with W warps per
 // scheduler the SM should approach 128 FFMA / clk.  Today's CfgS8 runs ONE warp per SM.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 --fmad=false -o chain_mb8 tools/micro/chain_mb8.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 --fmad=false -o chain_mb8 tools/micro/chain_mb8.cu
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -52,7 +52,7 @@ __global__ void __launch_bounds__(WARPS * 32) mb8(float* out, long long* cyc, in
 
 template <int WARPS>
 static void run(int K) {
-  const int NB = 148;
+  const int NB = 132;
   float* o;
   long long* c;
   cudaMalloc(&o, (size_t)NB * WARPS * 32 * 4);

@@ -4,7 +4,7 @@
 //   warp 0 (helper): bf16 core-matrix tile in smem -> f32 sub-tiles [k/4][row][4] in a ring (full/empty mbarriers)
 //   warp 1 (chain) : acc = fma(x[k], wf[k][row], acc), k strictly increasing -- the reference's order
 // Kernel `direct` is today's inner loop (conversion inside the chain warp) on the same data; both must print the same
-// checksum.  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 --fmad=false -o chain_pipe tools/micro/chain_pipe.cu
+// checksum.  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 --fmad=false -o chain_pipe tools/micro/chain_pipe.cu
 // Run under a timeout (mbarrier protocol untested on hardware): timeout 20 ./chain_pipe
 #include <cstdint>
 #include <cstdio>
@@ -115,7 +115,7 @@ __global__ void __launch_bounds__(32) direct(float* out, long long* cyc, int K) 
 }
 
 int main() {
-  const int K = 14336, NB = 148;
+  const int K = 14336, NB = 132;
   float *o1, *o2;
   long long *c1, *c2;
   cudaMalloc(&o1, NB * ROWS * 4); cudaMalloc(&o2, NB * ROWS * 4); cudaMalloc(&c1, NB * 8); cudaMalloc(&c2, NB * 8);

@@ -1,4 +1,4 @@
-"""Config 3 of BASELINE.json: prefill of S=2048 tokens on one B200 (tcgen05 GEMM path, LNB_ACC_FAST).
+"""Config 3 of BASELINE.json: prefill of S=2048 tokens on one H100 (tensor-core GEMM path, LNB_ACC_FAST).
 Prints prompt-processing tokens/s and the tensor-core throughput of the projections.
 Usage: python tools/prefill_bench.py [S] [reps]"""
 import os

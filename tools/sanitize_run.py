@@ -2,7 +2,7 @@
 paths once, on the TINY miniature, checked against the oracle so that the run is also a correctness run.
   compute-sanitizer --tool memcheck  python tools/sanitize_run.py
   compute-sanitizer --tool racecheck python tools/sanitize_run.py
-(tools/sanitize.sh runs both under gpurun and writes profiles/r02_sanitizer_*.txt)"""
+(tools/sanitize.sh runs both under compute-sanitizer)"""
 import os
 import sys
 
@@ -31,7 +31,7 @@ for mode, acc in (("strict", L._capi.LNB_ACC_STRICT), ("fast", L._capi.LNB_ACC_F
     graph, _, g = ctx.decode_run(first, 8, 6, use_graph=True)                                   # the same as CUDA-graph replays
     good = good and list(eager) == list(graph)
     ctx.set_active_sequence(1)
-    long_prompt = np.arange(3, 43, dtype=np.int32)                                              # S=40: tcgen05 prefill in FAST, 8-row blocks in STRICT
+    long_prompt = np.arange(3, 43, dtype=np.int32)                                              # S=40: tensor-core prefill in FAST, 8-row blocks in STRICT
     lo = osess.forward(long_prompt[:1], 0)                                                      # (oracle session reused only for shapes)
     nxt, lg = gm.Transformer.forward_argmax(ctx, long_prompt, 0, want_logits="last")
     o2 = om.new_session(48)

@@ -22,7 +22,7 @@ for S in [int(a) for a in sys.argv[1:]] or [70, 200, 513]:
     exp = O.attention(q, ck, cv, S, 1)
     t1 = time.time()
     res = {}
-    for tag, env in (("tc2", "2"), ("tc", "1"), ("fma", "0")):
+    for tag, env in (("tc", "1"), ("fma", "0")):
         os.environ["LNB_SDPA_TC"] = env
         c.check(c.lib.lnb_op_attention_bf16(c.ptr(q, c.u16p), c.ptr(ck, c.u16p), c.ptr(cv, c.u16p), c.ptr(out, c.u16p), S, S, nh, nkv, hd, 1,
                                             c.LNB_ACC_FAST))
