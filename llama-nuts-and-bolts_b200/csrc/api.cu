@@ -808,41 +808,57 @@ using CfgF8 = GemvCfg<32, 8, 8, 256, 4>;
 static const size_t kMaxSmem = 227 * 1024;
 static const int kWaveSMs = 132;   // H100 SXM: one wave of one-CTA-per-SM GEMV blocks
 
+// LAUNCH_PDL: programmatic stream serialization -- the kernel may start while its predecessor drains and waits for it in
+// pdl_wait().  LAUNCH_COOP: all CTAs co-resident (they wait for each other), or the launch fails.
+enum LaunchAttr { LAUNCH_PLAIN, LAUNCH_PDL, LAUNCH_COOP };
 struct Launcher {
   cudaStream_t stream;
-  bool pdl;
-  int64_t* counter;
+  LaunchAttr attr;
+  int64_t* counter;   // the session's launch count, or NULL
 };
 
-template <class Cfg, int PRO, int EPI>
-static int launch_gemv_cfg(const Launcher& L, const GemvParams& p) {
-  auto kern = gemv_kernel<Cfg, PRO, EPI>;
-  const size_t smem = Cfg::smem_bytes(p.K);
-  // the opt-in is per function AND per device (context): track it per instantiation per device
-  static std::atomic<uint64_t> attr_mask{0};
-  {
-    int dev = 0;
-    CU(cudaGetDevice(&dev));
-    const uint64_t bit = 1ull << (dev & 63);
-    if (!(attr_mask.load(std::memory_order_relaxed) & bit)) {
-      CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMaxSmem));
-      attr_mask.fetch_or(bit, std::memory_order_relaxed);
-    }
-  }
+template <typename... Args>
+static int launch_kernel(const Launcher& L, void (*kern)(Args...), dim3 grid, dim3 block, size_t smem, Args... args) {
   cudaLaunchConfig_t cfg{};
-  const int n_panels = p.N / 8;
-  cfg.gridDim = dim3((n_panels + Cfg::kP - 1) / Cfg::kP);
-  cfg.blockDim = dim3(Cfg::kThreads);
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = L.stream;
   cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
+  if (L.attr == LAUNCH_COOP) {
+    at[0].id = cudaLaunchAttributeCooperative;
+    at[0].val.cooperative = 1;
+  } else {
+    at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[0].val.programmaticStreamSerializationAllowed = 1;
+  }
   cfg.attrs = at;
-  cfg.numAttrs = L.pdl ? 1 : 0;
-  CU(cudaLaunchKernelEx(&cfg, kern, p));
+  cfg.numAttrs = L.attr == LAUNCH_PLAIN ? 0 : 1;
+  CU(cudaLaunchKernelEx(&cfg, kern, args...));
   if (L.counter) (*L.counter)++;
   return 0;
+}
+
+// The opt-in to large dynamic shared memory is per kernel AND per device (context): one mask of devices per kernel,
+// which is why the kernel itself is the template argument.
+template <auto Kern>
+static int smem_opt_in(int bytes) {
+  static std::atomic<uint64_t> done{0};
+  int dev = 0;
+  CU(cudaGetDevice(&dev));
+  const uint64_t bit = 1ull << (dev & 63);
+  if (!(done.load(std::memory_order_relaxed) & bit)) {
+    CU(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    done.fetch_or(bit, std::memory_order_relaxed);
+  }
+  return 0;
+}
+
+template <class Cfg, int PRO, int EPI>
+static int launch_gemv_cfg(const Launcher& L, const GemvParams& p) {
+  if (int rc = smem_opt_in<gemv_kernel<Cfg, PRO, EPI>>((int)kMaxSmem)) return rc;
+  return launch_kernel(L, gemv_kernel<Cfg, PRO, EPI>, dim3((p.N / 8 + Cfg::kP - 1) / Cfg::kP), dim3(Cfg::kThreads),
+                       Cfg::smem_bytes(p.K), p);
 }
 
 // picks the row-block size: largest MB in {8,2,1} that is useful for M and whose smem fits
@@ -896,23 +912,6 @@ static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total) {
   return 0;
 }
 
-template <typename... Args>
-static int launch_simple(const Launcher& L, void (*kern)(Args...), dim3 grid, dim3 block, size_t smem, Args... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = L.stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = L.pdl ? 1 : 0;
-  CU(cudaLaunchKernelEx(&cfg, kern, args...));
-  if (L.counter) (*L.counter)++;
-  return 0;
-}
-
 // LNB_ACC_STRICT RMSNorm scale r[row] (the reference's sequential fp32 sum of squares, bit-exact).  Three
 // interchangeable kernels, identical bits: 1 = one-thread FADD chain (rms_scale_kernel), 2 = iterative binade
 // scan, 3 = one-pass predict / fold / walk (both seqsum.cuh; need a row length that fits seq_scan_shape).
@@ -935,51 +934,29 @@ static int launch_rms_scale(const Launcher& L, const uint16_t* x, int ldx, float
   if (algo != RMS_CHAIN && !seq_scan_shape(D, &ch, &nt)) algo = RMS_CHAIN;
   if (algo == RMS_SCAN) {
     switch (ch) {
-      case 2: return launch_simple(L, rms_scale_scan_kernel<2>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
-      case 4: return launch_simple(L, rms_scale_scan_kernel<4>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
-      case 8: return launch_simple(L, rms_scale_scan_kernel<8>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
-      default: return launch_simple(L, rms_scale_scan_kernel<16>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
+      case 2: return launch_kernel(L, rms_scale_scan_kernel<2>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
+      case 4: return launch_kernel(L, rms_scale_scan_kernel<4>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
+      case 8: return launch_kernel(L, rms_scale_scan_kernel<8>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
+      default: return launch_kernel(L, rms_scale_scan_kernel<16>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
     }
   }
   if (algo == RMS_SEG) {
     switch (ch) {
-      case 2: return launch_simple(L, rms_scale_seg_kernel<2>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
-      case 4: return launch_simple(L, rms_scale_seg_kernel<4>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
-      case 8: return launch_simple(L, rms_scale_seg_kernel<8>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
-      default: return launch_simple(L, rms_scale_seg_kernel<16>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
+      case 2: return launch_kernel(L, rms_scale_seg_kernel<2>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
+      case 4: return launch_kernel(L, rms_scale_seg_kernel<4>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
+      case 8: return launch_kernel(L, rms_scale_seg_kernel<8>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
+      default: return launch_kernel(L, rms_scale_seg_kernel<16>, dim3(rows), dim3(nt), 0, x, ldx, r, D, eps);
     }
   }
-  return launch_simple(L, rms_scale_kernel, dim3(rows), dim3(128), (size_t)D * 4, x, ldx, r, D, eps);
+  return launch_kernel(L, rms_scale_kernel, dim3(rows), dim3(128), (size_t)D * 4, x, ldx, r, D, eps);
 }
 
 // tensor-core GEMM launcher (prefill): grid = (N/128, ceil(M/128))
 template <int EPI>
 static int launch_gemm_tc(const Launcher& L, const GemmTcParams& p) {
   if (p.N % TC_BN || p.K % TC_KT) return fail(LNB_EINVAL, "gemm_tc: N %d and K %d must be multiples of 128", p.N, p.K);
-  auto kern = gemm_tc_kernel<EPI>;
-  static std::atomic<uint64_t> attr_mask{0};   // per device, see launch_gemv_cfg
-  {
-    int dev = 0;
-    CU(cudaGetDevice(&dev));
-    const uint64_t bit = 1ull << (dev & 63);
-    if (!(attr_mask.load(std::memory_order_relaxed) & bit)) {
-      CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
-      attr_mask.fetch_or(bit, std::memory_order_relaxed);
-    }
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((p.M + TC_BM - 1) / TC_BM, p.N / TC_BN);
-  cfg.blockDim = dim3(TC_THREADS);
-  cfg.dynamicSmemBytes = TC_SMEM;
-  cfg.stream = L.stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = L.pdl ? 1 : 0;
-  CU(cudaLaunchKernelEx(&cfg, kern, p));
-  if (L.counter) (*L.counter)++;
-  return 0;
+  if (int rc = smem_opt_in<gemm_tc_kernel<EPI>>(TC_SMEM)) return rc;
+  return launch_kernel(L, gemm_tc_kernel<EPI>, dim3((p.M + TC_BM - 1) / TC_BM, p.N / TC_BN), dim3(TC_THREADS), TC_SMEM, p);
 }
 static bool tc_eligible(int M, int N, int K) { return M >= 32 && N % TC_BN == 0 && K % TC_KT == 0; }
 
@@ -1081,11 +1058,29 @@ struct lnb_session {
   int eng_key_seq = -1, eng_key_layers = -1, eng_key_kind = -2;
   const float* eng_key_logits = nullptr;
   cudaGraphExec_t graph = nullptr;
+  int64_t graph_launches = 0;    // kernels one replay of `graph` launches (counted while it was captured)
   bool graph_tried = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::mutex mu;
   int last_rows = 0;
 };
+
+static int set_state(lnb_session* s, int pos, int n_rows, int next_token, bool reset_step) {
+  return launch_kernel(Launcher{s->stream, LAUNCH_PLAIN, &s->launches}, set_state_kernel, dim3(1), dim3(1), 0, s->st, pos, n_rows,
+                       next_token, reset_step ? 1 : 0);
+}
+// layers a forward runs (lnb_session_set_layer_limit; <= 0: all)
+static int active_layers(const lnb_session* s) {
+  const int n = s->m->a.n_layers;
+  return (s->layer_limit > 0 && s->layer_limit < n) ? s->layer_limit : n;
+}
+// budget of one in-kernel wait for a peer (a late or dead rank yields LNB_ETIMEOUT instead of a hung GPU):
+// LNB_P2P_TIMEOUT_MS, default 1500; <= 0 waits forever (0 ns)
+static unsigned long long p2p_timeout_ns() {
+  const char* e = getenv("LNB_P2P_TIMEOUT_MS");
+  const long ms = e ? atol(e) : 1500;
+  return ms > 0 ? (unsigned long long)ms * 1000000ull : 0ull;
+}
 
 static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, lnb_session** out);
 extern "C" int lnb_session_create(lnb_model* m, int seq_len, int max_rows, int acc_mode, lnb_session** out) {
@@ -1242,13 +1237,10 @@ extern "C" int lnb_session_p2p_import(lnb_session* s, const void* handles, int n
   s->p2p.rank = m->tp_rank;
   s->p2p.n = n;
   s->p2p.slot_elems = s->max_rows * m->a.dim;
-  {  // budget of one in-kernel wait for a peer (a late or dead rank yields LNB_ETIMEOUT instead of a hung GPU)
-    const char* e = getenv("LNB_P2P_TIMEOUT_MS");
-    const long ms = e ? atol(e) : 1500;
-    s->p2p.timeout_ns = ms > 0 ? (unsigned long long)ms * 1000000ull : 0ull;
-  }
+  s->p2p.timeout_ns = p2p_timeout_ns();
   // epochs start at 1 (the region is zero-initialised, so no word carries a live epoch)
-  set_p2p_epoch_kernel<<<1, 1, 0, s->stream>>>(s->st, 1u);
+  int rc = launch_kernel(Launcher{s->stream, LAUNCH_PLAIN, &s->launches}, set_p2p_epoch_kernel, dim3(1), dim3(1), 0, s->st, 1u);
+  if (rc) return rc;
   CU(cudaStreamSynchronize(s->stream));
   if (s->graph) { cudaGraphExecDestroy(s->graph); s->graph = nullptr; }
   s->graph_tried = false;
@@ -1326,6 +1318,20 @@ static int ensure_logits(lnb_session* s, size_t rows) {
   if (s->m->tp_size > 1) CU(cudaMalloc((void**)&s->logits_full, rows * (size_t)s->m->a.vocab_size * 4));
   s->logits_rows = rows;
   return 0;
+}
+// tensor-parallel: rows [row0, row0 + rows) of every rank's logits shard -> the same rows of logits_full (a collective)
+static int gather_logits(lnb_session* s, int row0, int rows) {
+  lnb_model* m = s->m;
+  if (m->tp_size == 1) return 0;
+  for (int r = row0; r < row0 + rows; r++)
+    NC(g_nccl.AllGather(s->logits + (size_t)r * m->vocab_l, s->logits_full + (size_t)r * m->a.vocab_size, m->vocab_l, ncclFloat32_,
+                        m->comm, s->stream));
+  return 0;
+}
+// tensor-parallel LM head over NCCL: max-reduce the ranks' argmax keys, then publish the token (publish_kernel)
+static int reduce_argmax_publish(const Launcher& L, lnb_session* s, bool advance) {
+  NC(g_nccl.AllReduce(&s->st->amax_key, &s->st->amax_key, 1, ncclUint64_, ncclMax_, s->m->comm, s->stream));
+  return launch_kernel(L, publish_kernel, dim3(1), dim3(1), 0, s->st, advance ? 1 : 0, s->d_tok_out);
 }
 
 // ---- persistent decode engine (engine.cuh) ---------------------------------------------------------------------
@@ -1430,7 +1436,7 @@ static int eng_kt(int mode, int N, int K, int G) {
 static int engine_build(lnb_session* s, int kind, const float* logits_out) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
-  const int n_layers = (s->layer_limit > 0 && s->layer_limit < a.n_layers) ? s->layer_limit : a.n_layers;
+  const int n_layers = active_layers(s);
   if (s->d_phases && s->eng_key_seq == s->active_seq && s->eng_key_layers == n_layers && s->eng_key_kind == kind &&
       s->eng_key_logits == logits_out)
     return 0;
@@ -1549,11 +1555,7 @@ static int engine_launch(lnb_session* s, int n_steps, bool advance) {
   P.strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
   P.tok_out = s->d_tok_out; P.bar_ctr = s->d_bar;
   P.p2p = s->p2p; P.tp = m->tp_size;
-  P.timeout_ns = s->p2p.timeout_ns ? s->p2p.timeout_ns : 1500000000ull;
-  {
-    const char* e = getenv("LNB_P2P_TIMEOUT_MS");
-    if (e) P.timeout_ns = atol(e) > 0 ? (unsigned long long)atol(e) * 1000000ull : 0ull;
-  }
+  P.timeout_ns = p2p_timeout_ns();
   P.err_host = s->h_err;
   {
     // L2 prefetch per CTA and projection beyond the ring: 132 x 256 KB = 33 MB of the 50 MB L2 when enabled (LNB_ENGINE_PF_KB, 0 = off)
@@ -1579,19 +1581,10 @@ static int engine_launch(lnb_session* s, int n_steps, bool advance) {
     P.tag_base = s->eng_tag;
     s->eng_tag += (uint32_t)n * (uint32_t)s->n_phases;
     CU(cudaMemsetAsync(s->d_bar, 0, 4, s->stream));
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(m->sm_count);
-    cfg.blockDim = dim3(ENG_THREADS);
-    cfg.dynamicSmemBytes = ENG_SMEM;
-    cfg.stream = s->stream;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeCooperative;   // all CTAs co-resident (they wait for each other), or the launch fails
-    at[0].val.cooperative = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
-    if (s->mode == LNB_ACC_STRICT) CU(cudaLaunchKernelEx(&cfg, decode_engine_kernel<1>, P));
-    else CU(cudaLaunchKernelEx(&cfg, decode_engine_kernel<8>, P));
-    s->launches++;
+    const int rc = launch_kernel(Launcher{s->stream, LAUNCH_COOP, &s->launches},
+                                 s->mode == LNB_ACC_STRICT ? decode_engine_kernel<1> : decode_engine_kernel<8>, dim3(m->sm_count),
+                                 dim3(ENG_THREADS), ENG_SMEM, P);
+    if (rc) return rc;
     done += n;
   }
   s->last_was_engine = true;
@@ -1622,7 +1615,7 @@ static bool batch_engine_ok(lnb_session* s) {
 static int batch_engine_build(lnb_session* s, const float* logits_out) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
-  const int n_layers = (s->layer_limit > 0 && s->layer_limit < a.n_layers) ? s->layer_limit : a.n_layers;
+  const int n_layers = active_layers(s);
   if (s->d_bphases && s->bkey_layers == n_layers && s->bkey_logits == logits_out) return 0;
   if (!s->bx) {
     cudaError_t e = cudaMalloc((void**)&s->bx, (size_t)a.dim * 16);
@@ -1730,30 +1723,16 @@ static int batch_engine_launch(lnb_session* s, int n) {
   P.tokens = s->d_tokens; P.pos_arr = s->d_pos_arr; P.cache_seq_stride = (long long)s->seq_len * m->kv_l;
   P.rscale = s->rs; P.keys = s->d_bkeys; P.next_arr = s->d_next_arr; P.bar_ctr = s->d_bar;
   P.p2p = s->p2p; P.tp = m->tp_size;
-  P.timeout_ns = s->p2p.timeout_ns ? s->p2p.timeout_ns : 1500000000ull;
-  {
-    const char* e = getenv("LNB_P2P_TIMEOUT_MS");
-    if (e) P.timeout_ns = atol(e) > 0 ? (unsigned long long)atol(e) * 1000000ull : 0ull;
-  }
+  P.timeout_ns = p2p_timeout_ns();
   P.err_host = s->h_err;
   P.prof = s->d_prof;
   *s->h_err = 0;
   CU(cudaMemsetAsync(s->d_bar, 0, 4, s->stream));
   CU(cudaMemsetAsync(s->d_bkeys, 0, 64, s->stream));
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(m->sm_count);
-  cfg.blockDim = dim3(ENG_THREADS);
-  cfg.dynamicSmemBytes = s->batch_tc ? BT_SMEM : ENG_SMEM;
-  cfg.stream = s->stream;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeCooperative;
-  at[0].val.cooperative = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  if (s->mode == LNB_ACC_STRICT) CU(cudaLaunchKernelEx(&cfg, batch_engine_kernel<1>, P));
-  else if (s->batch_tc) CU(cudaLaunchKernelEx(&cfg, batch_engine_kernel<0>, P));
-  else CU(cudaLaunchKernelEx(&cfg, batch_engine_kernel<8>, P));
-  s->launches++;
+  const auto kern = s->mode == LNB_ACC_STRICT ? batch_engine_kernel<1> : s->batch_tc ? batch_engine_kernel<0> : batch_engine_kernel<8>;
+  const int rc = launch_kernel(Launcher{s->stream, LAUNCH_COOP, &s->launches}, kern, dim3(m->sm_count), dim3(ENG_THREADS),
+                               s->batch_tc ? BT_SMEM : ENG_SMEM, P);
+  if (rc) return rc;
   s->last_was_engine = false;
   return 0;
 }
@@ -1768,8 +1747,7 @@ static int sync_stream(lnb_session* s) {
 static int enqueue_decode_engine(lnb_session* s, int32_t token, int start_pos, int n_steps, bool advance, bool reset_step, const float* logits_out) {
   int rc = engine_build(s, -1, logits_out);
   if (rc) return rc;
-  set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, start_pos, 1, token, reset_step ? 1 : 0);
-  s->launches++;
+  if ((rc = set_state(s, start_pos, 1, token, reset_step))) return rc;
   *s->h_err = 0;
   return engine_launch(s, n_steps, advance);
 }
@@ -1777,11 +1755,11 @@ static int enqueue_decode_engine(lnb_session* s, int32_t token, int start_pos, i
 // Enqueue one LlamaTransformer.Forward (llamatransformer.go:145-180) for S rows on the
 // session stream.  from_state_token: row 0's token is st->next_token (device-driven decode).
 // logits_rows: 0 = none stored, 1 = last row, S = all rows.  advance: decode-loop bookkeeping.
-static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int logits_rows, bool advance, bool pdl, bool batch = false,
-                           bool gather_logits = true) {
+static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int logits_rows, bool advance, bool batch = false,
+                           bool gather = true) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
-  Launcher L{s->stream, pdl, &s->launches};
+  const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
   const int mode = s->mode;
   const int32_t* pos_ptr = &s->st->pos;
   // single-sequence calls work on the cache of the active sequence; a batched step addresses all of them
@@ -1789,23 +1767,37 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
   const size_t cache_off = batch ? 0 : (size_t)s->active_seq * seq_stride;
   if (batch && !s->sdpa_smem_decode) return fail(LNB_EINVAL, "batched decode needs SequenceLength small enough for the shared-memory attention kernel");
   int rc;
-  rc = launch_simple(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd,
+  rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd,
                      (const int32_t*)(from_state_token ? nullptr : s->d_tokens), (const LnbDevState*)s->st, s->x, a.dim);
   if (rc) return rc;
-  const int n_layers = (s->layer_limit > 0 && s->layer_limit < a.n_layers) ? s->layer_limit : a.n_layers;
-  const float scale = [&] {  // dtype.BFloat16fromFloat32(float32(math.Sqrt(float64(HeadDim)))) :464
-    float f = (float)sqrt((double)a.head_dim);
-    uint32_t u;
-    memcpy(&u, &f, 4);
-    u &= 0xffff0000u;
-    memcpy(&f, &u, 4);
-    return f;
-  }();
+  const int n_layers = active_layers(s);
+  const float scale = attn_scale_bf16(a.head_dim);
   const size_t sdpa_smem = (size_t)s->seq_len * 12 + (size_t)a.head_dim * 4;
   const bool strict = (mode == LNB_ACC_STRICT);
   auto strict_scale = [&](const uint16_t* xin, int rows) -> int {
     if (!strict) return 0;
     return launch_rms_scale(L, xin, a.dim, s->rs, rows, a.dim, a.norm_eps);
+  };
+  // wo / w2 + residual: out = res + x W^T; tensor-parallel ranks sum their partials first (peer all-reduce or NCCL)
+  auto proj_resid = [&](const uint16_t* W, int K, const uint16_t* x, const uint16_t* res, uint16_t* out) -> int {
+    GemvParams p{};
+    p.W = W; p.N = a.dim; p.K = K; p.x = x; p.ldx = K; p.ldo = a.dim;
+    if (m->tp_size == 1) {
+      p.out_bf16 = out; p.res = res;
+      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S);
+    }
+    int rc2;
+    if (s->p2p_ready) {
+      p.p2p = s->p2p; p.st = s->st;
+      if ((rc2 = launch_gemv<PRO_PLAIN, EPI_P2P>(L, mode, p, S))) return rc2;
+      return launch_kernel(L, p2p_reduce_resid_kernel, dim3(std::min(16, (S * a.dim + 255) / 256)), dim3(256), 0, s->p2p, s->st, res, out,
+                           S * a.dim);
+    }
+    p.out_f32 = s->part;
+    if ((rc2 = launch_gemv<PRO_PLAIN, EPI_F32RAW>(L, mode, p, S))) return rc2;
+    NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
+    return launch_kernel(L, resid_from_f32_kernel, dim3(std::min(kWaveSMs, (S * a.dim + 255) / 256)), dim3(256), 0, (const float*)s->part,
+                         res, out, (int64_t)S * a.dim);
   };
   for (int l = 0; l < n_layers; l++) {
     LayerW& W = m->layers[l];
@@ -1823,40 +1815,18 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
     }
     if ((S == 1 || batch) && s->sdpa_smem_decode) {
       const int n_rep = a.n_heads / a.n_kv_heads;
-      rc = launch_simple(L, sdpa_decode_kernel, dim3(m->kv_l / a.head_dim, batch ? S : 1), dim3(128 * n_rep), s->sdpa_decode_smem,
+      rc = launch_kernel(L, sdpa_decode_kernel, dim3(m->kv_l / a.head_dim, batch ? S : 1), dim3(128 * n_rep), s->sdpa_decode_smem,
                          (const uint16_t*)s->q, (const uint16_t*)(s->ck[l] + cache_off), (const uint16_t*)(s->cv[l] + cache_off), m->kv_l,
                          n_rep, a.head_dim, s->o, pos_ptr, s->seq_len, mode == LNB_ACC_STRICT ? 1 : 0, scale,
                          (const int32_t*)(batch ? s->d_pos_arr : nullptr), (long long)seq_stride, m->q_l, (const LnbDevState*)s->st);
     } else {
-      rc = launch_simple(L, sdpa_kernel, dim3(m->q_l / a.head_dim, S), dim3(128), sdpa_smem, (const uint16_t*)s->q, m->q_l,
+      rc = launch_kernel(L, sdpa_kernel, dim3(m->q_l / a.head_dim, S), dim3(128), sdpa_smem, (const uint16_t*)s->q, m->q_l,
                          (const uint16_t*)(s->ck[l] + cache_off), (const uint16_t*)(s->cv[l] + cache_off), m->kv_l,
                          a.n_heads / a.n_kv_heads, a.head_dim, s->o, m->q_l, pos_ptr, 0, S, S > 1 ? 1 : 0,
                          mode == LNB_ACC_STRICT ? 1 : 0, scale, 0);
     }
     if (rc) return rc;
-    {  // wo + residual                                             (:522, :232)
-      GemvParams p{};
-      p.W = W.wo; p.N = a.dim; p.K = m->q_l; p.x = s->o; p.ldx = m->q_l; p.ldo = a.dim;
-      if (m->tp_size == 1) {
-        p.out_bf16 = s->h1; p.res = s->x;
-        if ((rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S))) return rc;
-      } else {
-        if (s->p2p_ready) {
-          p.p2p = s->p2p; p.st = s->st;
-          if ((rc = launch_gemv<PRO_PLAIN, EPI_P2P>(L, mode, p, S))) return rc;
-          if ((rc = launch_simple(L, p2p_reduce_resid_kernel, dim3(std::min(16, (S * a.dim + 255) / 256)), dim3(256), 0, s->p2p, s->st,
-                                  (const uint16_t*)s->x, s->h1, S * a.dim)))
-            return rc;
-        } else {
-          p.out_f32 = s->part;
-          if ((rc = launch_gemv<PRO_PLAIN, EPI_F32RAW>(L, mode, p, S))) return rc;
-          NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
-          if ((rc = launch_simple(L, resid_from_f32_kernel, dim3(std::min(kWaveSMs, (S * a.dim + 255) / 256)), dim3(256), 0,
-                                  (const float*)s->part, (const uint16_t*)s->x, s->h1, (int64_t)S * a.dim)))
-            return rc;
-        }
-      }
-    }
+    if ((rc = proj_resid(W.wo, m->q_l, s->o, s->x, s->h1))) return rc;            // wo + residual (:522, :232)
     if ((rc = strict_scale(s->h1, S))) return rc;
     {  // ffn_norm -> w1|w3 -> SiLU * up                             (:237, :601-614)
       GemvParams p{};
@@ -1865,29 +1835,7 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
       p.out_bf16 = s->mbuf; p.ldo = m->ffn_l; p.silu_tab = m->silu_tab;
       if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, S))) return rc;
     }
-    {  // w2 + residual                                             (:619, :248)
-      GemvParams p{};
-      p.W = W.w2; p.N = a.dim; p.K = m->ffn_l; p.x = s->mbuf; p.ldx = m->ffn_l; p.ldo = a.dim;
-      if (m->tp_size == 1) {
-        p.out_bf16 = s->x; p.res = s->h1;
-        if ((rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S))) return rc;
-      } else {
-        if (s->p2p_ready) {
-          p.p2p = s->p2p; p.st = s->st;
-          if ((rc = launch_gemv<PRO_PLAIN, EPI_P2P>(L, mode, p, S))) return rc;
-          if ((rc = launch_simple(L, p2p_reduce_resid_kernel, dim3(std::min(16, (S * a.dim + 255) / 256)), dim3(256), 0, s->p2p, s->st,
-                                  (const uint16_t*)s->h1, s->x, S * a.dim)))
-            return rc;
-        } else {
-          p.out_f32 = s->part;
-          if ((rc = launch_gemv<PRO_PLAIN, EPI_F32RAW>(L, mode, p, S))) return rc;
-          NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
-          if ((rc = launch_simple(L, resid_from_f32_kernel, dim3(std::min(kWaveSMs, (S * a.dim + 255) / 256)), dim3(256), 0,
-                                  (const float*)s->part, (const uint16_t*)s->h1, s->x, (int64_t)S * a.dim)))
-            return rc;
-        }
-      }
-    }
+    if ((rc = proj_resid(W.w2, m->ffn_l, s->mbuf, s->h1, s->x))) return rc;        // w2 + residual (:619, :248)
   }
   {  // output_norm -> output -> f32 logits (+ greedy argmax of the last row)   (:166-175; inference.go:207-216)
     const int rows = (logits_rows > 1) ? S : 1;  // rows of the head actually computed
@@ -1905,23 +1853,14 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
     if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, rows))) return rc;
     if (batch) {
       // every row is the last row of its own sequence: one greedy argmax per row on the (gathered) logits
-      if (m->tp_size > 1)
-        for (int r = 0; r < rows; r++)
-          NC(g_nccl.AllGather(s->logits + (size_t)r * m->vocab_l, s->logits_full + (size_t)r * a.vocab_size, m->vocab_l, ncclFloat32_,
-                              m->comm, s->stream));
+      if ((rc = gather_logits(s, 0, rows))) return rc;
       const float* lg = (m->tp_size > 1) ? s->logits_full : s->logits;
-      if ((rc = launch_simple(L, argmax_f32_kernel, dim3(rows), dim3(256), 0, lg, a.vocab_size, s->d_next_arr))) return rc;
+      if ((rc = launch_kernel(L, argmax_f32_kernel, dim3(rows), dim3(256), 0, lg, a.vocab_size, s->d_next_arr))) return rc;
     } else if (m->tp_size > 1) {
-      if (s->p2p_ready) {
-        if ((rc = launch_simple(L, p2p_argmax_kernel, dim3(1), dim3(32), 0, s->p2p, s->st, advance ? 1 : 0, s->d_tok_out))) return rc;
-      } else {
-        NC(g_nccl.AllReduce(&s->st->amax_key, &s->st->amax_key, 1, ncclUint64_, ncclMax_, m->comm, s->stream));
-        if ((rc = launch_simple(L, publish_kernel, dim3(1), dim3(1), 0, s->st, advance ? 1 : 0, s->d_tok_out))) return rc;
-      }
-      if (logits_rows > 0 && gather_logits)
-        for (int r = 0; r < rows; r++)
-          NC(g_nccl.AllGather(s->logits + (size_t)r * m->vocab_l, s->logits_full + (size_t)r * a.vocab_size, m->vocab_l,
-                              ncclFloat32_, m->comm, s->stream));
+      if (s->p2p_ready) rc = launch_kernel(L, p2p_argmax_kernel, dim3(1), dim3(32), 0, s->p2p, s->st, advance ? 1 : 0, s->d_tok_out);
+      else rc = reduce_argmax_publish(L, s, advance);
+      if (rc) return rc;
+      if (logits_rows > 0 && gather && (rc = gather_logits(s, 0, rows))) return rc;
     }
   }
   s->last_rows = S;
@@ -1938,32 +1877,39 @@ static bool forward_tc_ok(const lnb_session* s, int S) {
   return s->mode == LNB_ACC_FAST && s->xn8 && S >= 32 && (m->q_l + 2 * m->kv_l) % TC_BN == 0 && a.dim % TC_BN == 0 &&
          (2 * m->ffn_l) % TC_BN == 0 && a.dim % TC_KT == 0 && m->q_l % TC_KT == 0 && m->ffn_l % TC_KT == 0;
 }
-static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gather_logits = true) {
+static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gather = true) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
-  Launcher L{s->stream, true, &s->launches};
+  const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
   const int32_t* pos_ptr = &s->st->pos;
   const int Mpad = (S + TC_BM - 1) / TC_BM * TC_BM;
   const int qkv_n = m->q_l + 2 * m->kv_l;
   const size_t tc_cache_off = (size_t)s->active_seq * s->seq_len * m->kv_l;
   int rc;
-  if ((rc = launch_simple(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd, (const int32_t*)s->d_tokens,
+  if ((rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd, (const int32_t*)s->d_tokens,
                           (const LnbDevState*)s->st, s->x, a.dim)))
     return rc;
-  const int n_layers = (s->layer_limit > 0 && s->layer_limit < a.n_layers) ? s->layer_limit : a.n_layers;
-  float scale = (float)sqrt((double)a.head_dim);
-  {
-    uint32_t u;
-    memcpy(&u, &scale, 4);
-    u &= 0xffff0000u;
-    memcpy(&scale, &u, 4);
-  }
+  const int n_layers = active_layers(s);
+  const float scale = attn_scale_bf16(a.head_dim);
   const size_t sdpa_smem = (size_t)s->seq_len * 12 + (size_t)a.head_dim * 4;
   const double* exp_tab = sdpa_tc_enabled() ? exp_table_device() : nullptr;
   const int ew_grid = m->sm_count * 8;
+  // wo / w2 + residual: out = res + X W^T; tensor-parallel ranks sum their partials over NCCL first
+  auto proj_resid = [&](const uint16_t* X8, const uint16_t* W, int K, const uint16_t* res, uint16_t* out) -> int {
+    GemmTcParams g{};
+    g.X8 = X8; g.W = W; g.M = S; g.N = a.dim; g.K = K; g.ldo = a.dim;
+    if (m->tp_size == 1) {
+      g.out_bf16 = out; g.res = res;
+      return launch_gemm_tc<TC_EPI_RESID>(L, g);
+    }
+    g.out_f32 = s->part;
+    if (int rc2 = launch_gemm_tc<TC_EPI_F32RAW>(L, g)) return rc2;
+    NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
+    return launch_kernel(L, resid_from_f32_kernel, dim3(ew_grid), dim3(256), 0, (const float*)s->part, res, out, (int64_t)S * a.dim);
+  };
   for (int l = 0; l < n_layers; l++) {
     LayerW& W = m->layers[l];
-    if ((rc = launch_simple(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->x, a.dim, (const uint16_t*)W.attn_norm,
+    if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->x, a.dim, (const uint16_t*)W.attn_norm,
                             s->xn8, S, a.dim, a.norm_eps)))
       return rc;
     {
@@ -1971,40 +1917,26 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
       g.X8 = s->xn8; g.W = W.wqkv; g.M = S; g.N = qkv_n; g.K = a.dim; g.out_bf16 = s->qkv_raw; g.ldo = qkv_n;
       if ((rc = launch_gemm_tc<TC_EPI_BF16>(L, g))) return rc;
     }
-    if ((rc = launch_simple(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
+    if ((rc = launch_kernel(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
                             a.head_dim, s->ck[l] + tc_cache_off, s->cv[l] + tc_cache_off, (const float*)m->cis, pos_ptr, S)))
       return rc;
     if (a.head_dim == SP_HD && exp_tab) {
-      if ((rc = launch_simple(L, sdpa_tc_kernel, dim3(m->q_l / a.head_dim, (S + 127) / 128), dim3(256), (size_t)ST_SMEM,
+      if ((rc = launch_kernel(L, sdpa_tc_kernel, dim3(m->q_l / a.head_dim, (S + 127) / 128), dim3(256), (size_t)ST_SMEM,
                               (const uint16_t*)s->q, m->q_l, (const uint16_t*)(s->ck[l] + tc_cache_off),
                               (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l, a.n_heads / a.n_kv_heads, s->o8, m->q_l, pos_ptr, S, scale,
                               exp_tab)))
         return rc;
     } else if (a.head_dim == SP_HD) {
-      if ((rc = launch_simple(L, sdpa_prefill_kernel, dim3(m->q_l / a.head_dim, (S + SP_QB - 1) / SP_QB), dim3(256), (size_t)SP_SMEM,
+      if ((rc = launch_kernel(L, sdpa_prefill_kernel, dim3(m->q_l / a.head_dim, (S + SP_QB - 1) / SP_QB), dim3(256), (size_t)SP_SMEM,
                               (const uint16_t*)s->q, m->q_l, (const uint16_t*)(s->ck[l] + tc_cache_off),
                               (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l, a.n_heads / a.n_kv_heads, s->o8, m->q_l, pos_ptr, S, scale)))
         return rc;
-    } else if ((rc = launch_simple(L, sdpa_kernel, dim3(m->q_l / a.head_dim, S), dim3(128), sdpa_smem, (const uint16_t*)s->q, m->q_l,
+    } else if ((rc = launch_kernel(L, sdpa_kernel, dim3(m->q_l / a.head_dim, S), dim3(128), sdpa_smem, (const uint16_t*)s->q, m->q_l,
                                    (const uint16_t*)(s->ck[l] + tc_cache_off), (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l,
                                    a.n_heads / a.n_kv_heads, a.head_dim, s->o8, m->q_l, pos_ptr, 0, S, 1, 0, scale, 1)))
       return rc;
-    {
-      GemmTcParams g{};
-      g.X8 = s->o8; g.W = W.wo; g.M = S; g.N = a.dim; g.K = m->q_l; g.ldo = a.dim;
-      if (m->tp_size == 1) {
-        g.out_bf16 = s->h1; g.res = s->x;
-        if ((rc = launch_gemm_tc<TC_EPI_RESID>(L, g))) return rc;
-      } else {
-        g.out_f32 = s->part;
-        if ((rc = launch_gemm_tc<TC_EPI_F32RAW>(L, g))) return rc;
-        NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
-        if ((rc = launch_simple(L, resid_from_f32_kernel, dim3(ew_grid), dim3(256), 0, (const float*)s->part, (const uint16_t*)s->x, s->h1,
-                                (int64_t)S * a.dim)))
-          return rc;
-      }
-    }
-    if ((rc = launch_simple(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->h1, a.dim, (const uint16_t*)W.ffn_norm,
+    if ((rc = proj_resid(s->o8, W.wo, m->q_l, s->x, s->h1))) return rc;
+    if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->h1, a.dim, (const uint16_t*)W.ffn_norm,
                             s->xn8, S, a.dim, a.norm_eps)))
       return rc;
     {
@@ -2013,26 +1945,12 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
       g.X8 = s->xn8; g.W = W.w13; g.M = S; g.N = 2 * m->ffn_l; g.K = a.dim; g.out_bf16 = s->m8; g.ldo = m->ffn_l; g.silu_tab = m->silu_tab;
       if ((rc = launch_gemm_tc<TC_EPI_SWIGLU>(L, g))) return rc;
     }
-    {
-      GemmTcParams g{};
-      g.X8 = s->m8; g.W = W.w2; g.M = S; g.N = a.dim; g.K = m->ffn_l; g.ldo = a.dim;
-      if (m->tp_size == 1) {
-        g.out_bf16 = s->x; g.res = s->h1;
-        if ((rc = launch_gemm_tc<TC_EPI_RESID>(L, g))) return rc;
-      } else {
-        g.out_f32 = s->part;
-        if ((rc = launch_gemm_tc<TC_EPI_F32RAW>(L, g))) return rc;
-        NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
-        if ((rc = launch_simple(L, resid_from_f32_kernel, dim3(ew_grid), dim3(256), 0, (const float*)s->part, (const uint16_t*)s->h1, s->x,
-                                (int64_t)S * a.dim)))
-          return rc;
-      }
-    }
+    if ((rc = proj_resid(s->m8, W.w2, m->ffn_l, s->h1, s->x))) return rc;
   }
   // LM head: all rows on the tensor cores when asked for (and the vocabulary shard tiles), then the
   // last row through the GEMV, which also owns the greedy argmax (identical to the decode path)
   if (logits_rows > 1 && m->vocab_l % TC_BN == 0) {
-    if ((rc = launch_simple(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->x, a.dim, (const uint16_t*)m->norm, s->xn8, S,
+    if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->x, a.dim, (const uint16_t*)m->norm, s->xn8, S,
                             a.dim, a.norm_eps)))
       return rc;
     GemmTcParams g{};
@@ -2053,23 +1971,20 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
     p.st = s->st; p.argmax_row = 0; p.publish = (m->tp_size == 1) ? 1 : 0; p.advance = 0; p.tok_out = s->d_tok_out;
     if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1))) return rc;
     if (m->tp_size > 1) {
-      NC(g_nccl.AllReduce(&s->st->amax_key, &s->st->amax_key, 1, ncclUint64_, ncclMax_, m->comm, s->stream));
-      if ((rc = launch_simple(L, publish_kernel, dim3(1), dim3(1), 0, s->st, 0, s->d_tok_out))) return rc;
-      if (logits_rows > 0 && gather_logits) {
-        const int rows = logits_rows > 1 ? S : 1;
-        for (int r = 0; r < rows; r++)
-          NC(g_nccl.AllGather(s->logits + (size_t)r * m->vocab_l, s->logits_full + (size_t)r * a.vocab_size, m->vocab_l, ncclFloat32_,
-                              m->comm, s->stream));
-      }
+      if ((rc = reduce_argmax_publish(L, s, false))) return rc;
+      if (logits_rows > 0 && gather && (rc = gather_logits(s, 0, logits_rows > 1 ? S : 1))) return rc;
     }
   }
   s->last_rows = S;
   return 0;
 }
 
-extern "C" int lnb_forward(lnb_session* s, const int32_t* tokens, int S, int start_pos, float* logits, int all_rows,
-                           int32_t* argmax_last) {
-  if (!s || !tokens) return fail(LNB_EINVAL, "NULL argument");
+// The forward of lnb_forward and lnb_forward_device; the caller holds s->mu.  keep_logits: the logits of the last row, or
+// of all S rows (all_rows), stay in s->logits.  host_logits: NULL, or where those rows are copied (tensor-parallel:
+// gathered from the ranks first).  next_token: NULL, or receives the greedy token of the last row.
+static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int start_pos, bool keep_logits, bool all_rows,
+                          float* host_logits, int32_t* next_token) {
+  if (!tokens) return fail(LNB_EINVAL, "NULL argument");
   if (S <= 0) return fail(LNB_EINVAL, "empty token array");  // llamatransformer.go:146-148
   if (S > s->max_rows) return fail(LNB_EINVAL, "S %d exceeds the session's max_rows %d", S, s->max_rows);
   if (start_pos < 0 || start_pos + S > s->seq_len)
@@ -2079,39 +1994,42 @@ extern "C" int lnb_forward(lnb_session* s, const int32_t* tokens, int S, int sta
                 "lnb_session_set_chunked_prefill enables the [S,T]-mask extension");
   for (int i = 0; i < S; i++)
     if (tokens[i] < 0 || tokens[i] >= s->m->a.vocab_size) return fail(LNB_EINVAL, "token id %d out of range", tokens[i]);
-  std::lock_guard<std::mutex> lk(s->mu);
   lnb_model* m = s->m;
   CU(cudaSetDevice(m->device));
-  const int lrows = logits ? (all_rows ? S : 1) : 0;
-  if (lrows) {
-    int rc = ensure_logits(s, (size_t)(all_rows ? s->max_rows : 1));
-    if (rc) return rc;
-  }
+  s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
+  const int lrows = keep_logits ? (all_rows ? S : 1) : 0;
   int rc;
+  if (lrows && (rc = ensure_logits(s, (size_t)(all_rows ? s->max_rows : 1)))) return rc;
   if (S == 1 && engine_ok(s)) {
     // decode step: ONE persistent kernel; the token id rides in the launch of set_state_kernel (4 bytes of kernel arguments)
     if ((rc = enqueue_decode_engine(s, tokens[0], start_pos, 1, false, false, lrows ? s->logits : nullptr))) return rc;
-    if (lrows && m->tp_size > 1)
-      NC(g_nccl.AllGather(s->logits, s->logits_full, m->vocab_l, ncclFloat32_, m->comm, s->stream));
+    if (host_logits && (rc = gather_logits(s, 0, 1))) return rc;
   } else {
     memcpy(s->h_pin, tokens, (size_t)S * 4);
     CU(cudaMemcpyAsync(s->d_tokens, s->h_pin, (size_t)S * 4, cudaMemcpyHostToDevice, s->stream));
-    set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, start_pos, S, -1, 0);
-    s->launches++;
-    rc = forward_tc_ok(s, S) ? enqueue_forward_tc(s, S, lrows) : enqueue_forward(s, S, false, lrows, false, true);
+    if ((rc = set_state(s, start_pos, S, -1, false))) return rc;
+    const bool gather = host_logits != nullptr;
+    rc = forward_tc_ok(s, S) ? enqueue_forward_tc(s, S, lrows, gather) : enqueue_forward(s, S, false, lrows, false, false, gather);
     if (rc) return rc;
   }
-  if (lrows) {
+  if (host_logits) {
     const float* src = (m->tp_size > 1) ? s->logits_full : s->logits;
-    CU(cudaMemcpyAsync(logits, src, (size_t)lrows * m->a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
+    CU(cudaMemcpyAsync(host_logits, src, (size_t)lrows * m->a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
   }
   int32_t* tokpin = s->h_pin + s->max_rows;
-  if (argmax_last) CU(cudaMemcpyAsync(tokpin, &s->st->next_token, 4, cudaMemcpyDeviceToHost, s->stream));
+  if (next_token) CU(cudaMemcpyAsync(tokpin, &s->st->next_token, 4, cudaMemcpyDeviceToHost, s->stream));
   if ((rc = p2p_err_enqueue(s))) return rc;
   if ((rc = sync_stream(s))) return rc;
   if ((rc = p2p_err_check(s))) return rc;
-  if (argmax_last) *argmax_last = *tokpin;
+  if (next_token) *next_token = *tokpin;
   return 0;
+}
+
+extern "C" int lnb_forward(lnb_session* s, const int32_t* tokens, int S, int start_pos, float* logits, int all_rows,
+                           int32_t* argmax_last) {
+  if (!s) return fail(LNB_EINVAL, "NULL argument");
+  std::lock_guard<std::mutex> lk(s->mu);
+  return forward_locked(s, tokens, S, start_pos, logits != nullptr, all_rows != 0, logits, argmax_last);
 }
 
 // Forward whose logits stay on the device: the host mirror of LlamaTransformer.Forward hands the caller a tensor
@@ -2121,41 +2039,14 @@ extern "C" int lnb_forward(lnb_session* s, const int32_t* tokens, int S, int sta
 // rows_kept: 1 = last row, S = all rows.  generation_out identifies the call (handles of older calls are stale).
 extern "C" int lnb_forward_device(lnb_session* s, const int32_t* tokens, int S, int start_pos, int rows_kept,
                                   int32_t* argmax_last, int64_t* generation_out) {
-  if (!s || !tokens) return fail(LNB_EINVAL, "NULL argument");
-  if (S <= 0) return fail(LNB_EINVAL, "empty token array");
+  if (!s) return fail(LNB_EINVAL, "NULL argument");
   if (rows_kept != 1 && rows_kept != S) return fail(LNB_EINVAL, "rows_kept must be 1 or S");
-  // same checks and the same enqueue as lnb_forward; only the D2H of the logits is left out
-  if (S > s->max_rows) return fail(LNB_EINVAL, "S %d exceeds the session's max_rows %d", S, s->max_rows);
-  if (start_pos < 0 || start_pos + S > s->seq_len)
-    return fail(LNB_EINVAL, "positions [%d, %d) exceed SequenceLength %d", start_pos, start_pos + S, s->seq_len);
-  if (S > 1 && start_pos != 0 && !s->allow_chunked)
-    return fail(LNB_EINVAL, "S>1 requires startPos 0 (the reference's [S,S] mask does not broadcast to [S,T]); "
-                "lnb_session_set_chunked_prefill enables the [S,T]-mask extension");
-  for (int i = 0; i < S; i++)
-    if (tokens[i] < 0 || tokens[i] >= s->m->a.vocab_size) return fail(LNB_EINVAL, "token id %d out of range", tokens[i]);
   std::lock_guard<std::mutex> lk(s->mu);
-  lnb_model* m = s->m;
-  CU(cudaSetDevice(m->device));
-  int rc = ensure_logits(s, (size_t)(rows_kept > 1 ? s->max_rows : 1));
+  int32_t tok = -1;
+  const int rc = forward_locked(s, tokens, S, start_pos, true, rows_kept > 1, nullptr, &tok);
   if (rc) return rc;
-  s->kept_rows = 0;
-  if (S == 1 && engine_ok(s)) {
-    if ((rc = enqueue_decode_engine(s, tokens[0], start_pos, 1, false, false, s->logits))) return rc;
-  } else {
-    memcpy(s->h_pin, tokens, (size_t)S * 4);
-    CU(cudaMemcpyAsync(s->d_tokens, s->h_pin, (size_t)S * 4, cudaMemcpyHostToDevice, s->stream));
-    set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, start_pos, S, -1, 0);
-    s->launches++;
-    rc = forward_tc_ok(s, S) ? enqueue_forward_tc(s, S, rows_kept, false) : enqueue_forward(s, S, false, rows_kept, false, true, false, false);
-    if (rc) return rc;
-  }
-  int32_t* tokpin = s->h_pin + s->max_rows;
-  CU(cudaMemcpyAsync(tokpin, &s->st->next_token, 4, cudaMemcpyDeviceToHost, s->stream));
-  if ((rc = p2p_err_enqueue(s))) return rc;
-  if ((rc = sync_stream(s))) return rc;
-  if ((rc = p2p_err_check(s))) return rc;
-  if (argmax_last) *argmax_last = *tokpin;
-  s->kept_last_token = *tokpin;
+  if (argmax_last) *argmax_last = tok;
+  s->kept_last_token = tok;
   s->kept_rows = rows_kept;
   s->generation++;
   if (generation_out) *generation_out = s->generation;
@@ -2179,9 +2070,7 @@ extern "C" int lnb_session_logits_read(lnb_session* s, int64_t generation, int r
   const size_t V = (size_t)m->a.vocab_size, bytes = (size_t)rows * V * 4;
   const float* src = s->logits + (size_t)row0 * m->vocab_l;
   if (m->tp_size > 1) {
-    for (int r = 0; r < rows; r++)
-      NC(g_nccl.AllGather(s->logits + (size_t)(row0 + r) * m->vocab_l, s->logits_full + (size_t)(row0 + r) * V, m->vocab_l, ncclFloat32_,
-                          m->comm, s->stream));
+    if ((rc = gather_logits(s, row0, rows))) return rc;
     src = s->logits_full + (size_t)row0 * V;
   }
   if (bytes <= ((size_t)16 << 20)) {
@@ -2279,6 +2168,7 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
   std::lock_guard<std::mutex> lk(s->mu);
   lnb_model* m = s->m;
   CU(cudaSetDevice(m->device));
+  s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
   int rc = ensure_logits(s, (size_t)s->max_rows);
   if (rc) return rc;
   memcpy(s->h_pin, tokens, (size_t)n * 4);
@@ -2290,15 +2180,10 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
     // ONE launch of the batch engine: every weight matrix streamed once for all n sequences
     if ((rc = batch_engine_build(s, logits ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, n))) return rc;
-    if (logits && m->tp_size > 1)
-      for (int r = 0; r < n; r++)
-        NC(g_nccl.AllGather(s->logits + (size_t)r * m->vocab_l, s->logits_full + (size_t)r * m->a.vocab_size, m->vocab_l, ncclFloat32_,
-                            m->comm, s->stream));
+    if (logits && (rc = gather_logits(s, 0, n))) return rc;
   } else {
-    set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, 0, n, -1, 0);
-    s->launches++;
-    rc = enqueue_forward(s, n, false, n > 1 ? n : 2, false, true, true);
-    if (rc) return rc;
+    if ((rc = set_state(s, 0, n, -1, false))) return rc;
+    if ((rc = enqueue_forward(s, n, false, n > 1 ? n : 2, false, true))) return rc;
   }
   if (logits) {
     const float* src = (m->tp_size > 1) ? s->logits_full : s->logits;
@@ -2321,12 +2206,12 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
   if (first_token < 0 || first_token >= s->m->a.vocab_size) return fail(LNB_EINVAL, "token id %d out of range", first_token);
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(s->m->device));
+  s->kept_rows = 0;   // a logits handle is valid until the session's next forward
+  int rc;
   if (engine_ok(s)) {
     // the whole run is ONE launch of the persistent engine: n_steps forwards, the greedy token fed back on the device
-    int rc = engine_build(s, -1, nullptr);
-    if (rc) return rc;
-    set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, start_pos, 1, first_token, 1);
-    s->launches++;
+    if ((rc = engine_build(s, -1, nullptr))) return rc;
+    if ((rc = set_state(s, start_pos, 1, first_token, true))) return rc;
     *s->h_err = 0;
     CU(cudaEventRecord(s->ev0, s->stream));
     if ((rc = engine_launch(s, n_steps, true))) return rc;
@@ -2344,9 +2229,9 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     cudaGraph_t g = nullptr;
     const int64_t saved = s->launches;
     cudaError_t e = cudaStreamBeginCapture(s->stream, cudaStreamCaptureModeThreadLocal);
-    int rc = 0;
+    rc = 0;
     if (e == cudaSuccess) {
-      rc = enqueue_forward(s, 1, true, 0, true, true);
+      rc = enqueue_forward(s, 1, true, 0, true);
       e = cudaStreamEndCapture(s->stream, &g);
     }
     if (e == cudaSuccess && rc == 0 && g) {
@@ -2355,36 +2240,26 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     }
     if (g) cudaGraphDestroy(g);
     cudaGetLastError();
+    s->graph_launches = s->launches - saved;   // the capture launched nothing: count it per replay
     s->launches = saved;
   }
   const bool graph = use_graph && s->graph;
-  set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, start_pos, 1, first_token, 1);
+  if ((rc = set_state(s, start_pos, 1, first_token, true))) return rc;
   CU(cudaEventRecord(s->ev0, s->stream));
-  const int64_t per_step_before = s->launches;
   for (int i = 0; i < n_steps; i++) {
     if (graph) {
       CU(cudaGraphLaunch(s->graph, s->stream));
-    } else {
-      int rc = enqueue_forward(s, 1, true, 0, true, true);
-      if (rc) return rc;
+      s->launches += s->graph_launches;
+    } else if ((rc = enqueue_forward(s, 1, true, 0, true))) {
+      return rc;
     }
-  }
-  if (graph) {
-    // count what the graph replays launch: one forward's worth per step
-    int64_t per_step = 0;
-    {
-      const lnb_model_args& a = s->m->a;
-      per_step = 2 + (int64_t)a.n_layers * (s->m->tp_size == 1 ? 5 : 7) + (s->m->tp_size == 1 ? 0 : 1) +
-                 (s->mode == LNB_ACC_STRICT ? 2 * (int64_t)a.n_layers + 1 : 0);
-    }
-    s->launches = per_step_before + per_step * n_steps;
   }
   CU(cudaEventRecord(s->ev1, s->stream));
   CU(cudaMemcpyAsync(s->h_pin + s->max_rows + 8, s->d_tok_out, (size_t)n_steps * 4, cudaMemcpyDeviceToHost, s->stream));
-  { int rce = p2p_err_enqueue(s); if (rce) return rce; }
+  if ((rc = p2p_err_enqueue(s))) return rc;
   CU(cudaStreamSynchronize(s->stream));
   CU(cudaGetLastError());
-  { int rce = p2p_err_check(s); if (rce) return rce; }
+  if ((rc = p2p_err_check(s))) return rc;
   float ms = 0.f;
   CU(cudaEventElapsedTime(&ms, s->ev0, s->ev1));
   if (ms_out) *ms_out = ms;
@@ -2408,10 +2283,10 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
     // prefetched across the grid barrier).  One launch walks all layers' copies `reps` times; time per phase.
     int rc = engine_build(s, kind, nullptr);
     if (rc) return rc;
-    set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, 0, 1, 0, 0);
+    if ((rc = set_state(s, 0, 1, 0, false))) return rc;
     *s->h_err = 0;
     if ((rc = engine_launch(s, 1, false))) return rc;     // warm-up sweep
-    set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, 0, 1, 0, 0);
+    if ((rc = set_state(s, 0, 1, 0, false))) return rc;
     CU(cudaEventRecord(s->ev0, s->stream));
     if ((rc = engine_launch(s, reps, false))) return rc;
     CU(cudaEventRecord(s->ev1, s->stream));
@@ -2433,8 +2308,8 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
     s->eng_key_kind = -2;   // the next decode call rebuilds the step's phase list
     return 0;
   }
-  Launcher L{s->stream, true, &s->launches};
-  set_state_kernel<<<1, 1, 0, s->stream>>>(s->st, 0, 1, 0, 0);
+  const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
+  if (int rc0 = set_state(s, 0, 1, 0, false)) return rc0;
   int n_launch = 0;
   int64_t bytes = 0;
   auto sweep = [&]() -> int {
@@ -2646,7 +2521,7 @@ extern "C" int lnb_op_linear_bf16(const uint16_t* x, const uint16_t* w, uint16_t
     pack_x8_kernel<<<grid_for((int64_t)Mpad * K / 8), 256>>>(dx.as<uint16_t>(), K, S, Mpad, K, dx8.as<uint16_t>());
     GemmTcParams g{};
     g.X8 = dx8.as<uint16_t>(); g.W = dwp.as<uint16_t>(); g.M = S; g.N = N; g.K = K; g.out_bf16 = dout.as<uint16_t>(); g.ldo = N;
-    Launcher L{nullptr, false, nullptr};
+    Launcher L{nullptr, LAUNCH_PLAIN, nullptr};
     int rc = launch_gemm_tc<TC_EPI_BF16>(L, g);
     if (rc) return rc;
     rc = op_finish();
@@ -2662,7 +2537,7 @@ extern "C" int lnb_op_linear_bf16(const uint16_t* x, const uint16_t* w, uint16_t
     retile_kernel<<<grid_for((int64_t)N * K / 8), 256>>>(dw.as<uint16_t>(), K, 0, 0, N, K, dwp.as<uint16_t>(), 0, 1);
     GemvParams p{};
     p.W = dwp.as<uint16_t>(); p.N = N; p.K = K; p.x = dx.as<uint16_t>(); p.ldx = K; p.out_bf16 = dout.as<uint16_t>(); p.ldo = N;
-    Launcher L{nullptr, false, nullptr};
+    Launcher L{nullptr, LAUNCH_PLAIN, nullptr};
     int rc = launch_gemv<PRO_PLAIN, EPI_BF16>(L, acc_mode, p, S);
     if (rc) return rc;
     rc = op_finish();
@@ -2701,7 +2576,7 @@ extern "C" int lnb_op_rmsnorm_bf16(const uint16_t* x, const uint16_t* w, uint16_
   const float* rs = nullptr;
   OPBUF(drs, (size_t)S * 4);
   if (strict && D % 2 == 0 && (size_t)D * 4 <= 48 * 1024) {  // the model path's own scale kernel
-    const Launcher L{nullptr, false, nullptr};
+    const Launcher L{nullptr, LAUNCH_PLAIN, nullptr};
     int rc0 = launch_rms_scale(L, dx.as<uint16_t>(), D, drs.as<float>(), S, D, eps);
     if (rc0) return rc0;
     rs = drs.as<float>();
@@ -2725,17 +2600,15 @@ extern "C" int lnb_op_rms_scale_f32(const uint16_t* x, float* r, int S, int D, f
     OPBUF(dx2, xb2); OPBUF(dr2, (size_t)S * 4);
     H2D(dx2, x, xb2);
     const size_t smem = (size_t)D * 4 + 4096;
-    switch (ech) {
-      case 16: CU(cudaFuncSetAttribute(eng_rms_scale_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-               eng_rms_scale_kernel<16><<<S, ENG_NCONS, smem>>>(dx2.as<uint16_t>(), D, dr2.as<float>(), D, eps); break;
-      case 8: CU(cudaFuncSetAttribute(eng_rms_scale_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-              eng_rms_scale_kernel<8><<<S, ENG_NCONS, smem>>>(dx2.as<uint16_t>(), D, dr2.as<float>(), D, eps); break;
-      case 4: CU(cudaFuncSetAttribute(eng_rms_scale_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-              eng_rms_scale_kernel<4><<<S, ENG_NCONS, smem>>>(dx2.as<uint16_t>(), D, dr2.as<float>(), D, eps); break;
-      default: CU(cudaFuncSetAttribute(eng_rms_scale_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-               eng_rms_scale_kernel<2><<<S, ENG_NCONS, smem>>>(dx2.as<uint16_t>(), D, dr2.as<float>(), D, eps); break;
-    }
-    int rc2 = op_finish();
+    const auto kern = ech == 16 ? eng_rms_scale_kernel<16>
+                    : ech == 8  ? eng_rms_scale_kernel<8>
+                    : ech == 4  ? eng_rms_scale_kernel<4>
+                                : eng_rms_scale_kernel<2>;
+    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const Launcher L{nullptr, LAUNCH_PLAIN, nullptr};
+    int rc2 = launch_kernel(L, kern, dim3(S), dim3(ENG_NCONS), smem, (const uint16_t*)dx2.as<uint16_t>(), D, dr2.as<float>(), D, eps);
+    if (rc2) return rc2;
+    rc2 = op_finish();
     if (rc2) return rc2;
     D2H(r, dr2, (size_t)S * 4);
     return 0;
@@ -2747,7 +2620,7 @@ extern "C" int lnb_op_rms_scale_f32(const uint16_t* x, float* r, int S, int D, f
   const size_t xb = (size_t)S * D * 2;
   OPBUF(dx, xb); OPBUF(dr, (size_t)S * 4);
   H2D(dx, x, xb);
-  const Launcher L{nullptr, false, nullptr};
+  const Launcher L{nullptr, LAUNCH_PLAIN, nullptr};
   int rc = launch_rms_scale(L, dx.as<uint16_t>(), D, dr.as<float>(), S, D, eps, algo);
   if (rc) return rc;
   rc = op_finish();
@@ -2782,11 +2655,7 @@ extern "C" int lnb_op_attention_bf16(const uint16_t* q, const uint16_t* cache_k,
   OPBUF(dq, qb); OPBUF(dk, cb); OPBUF(dv, cb); OPBUF(dout, qb);
   H2D(dq, q, qb); H2D(dk, cache_k, cb); H2D(dv, cache_v, cb);
   CU(cudaFuncSetAttribute(sdpa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  float f = (float)sqrt((double)hd);
-  uint32_t u;
-  memcpy(&u, &f, 4);
-  u &= 0xffff0000u;
-  memcpy(&f, &u, 4);
+  const float f = attn_scale_bf16(hd);
   if (acc_mode == LNB_ACC_FAST && S > 1 && causal_mask && hd == SP_HD && (n_heads * hd) % 128 == 0) {
     // the prefill path's tiled two-pass kernel (writes the X8 operand of the Wo GEMM; unpacked here)
     const int Mpad = (S + 127) / 128 * 128;

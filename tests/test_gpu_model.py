@@ -464,6 +464,21 @@ def test_captured_decode_graph_follows_active_sequence_and_layer_limit(L, tiny):
         assert [firsts[0]] + list(c) == list(om.generate(prompts[0], len(prompts[0]) + 9, stop_ids=(10**9,)))
     finally:
         ctx.close()
+    # single-GPU FAST sessions decode on the kernel chain, so decode_run replays the captured graph: under a layer limit
+    # the replays must count the kernels the eager steps launch
+    fast = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(seq), acc_mode=L._capi.LNB_ACC_FAST)
+    try:
+        first, _ = gm.Transformer.forward_argmax(fast, np.array(prompts[0], np.int32), 0)
+        assert not fast.uses_engine()
+        fast.set_layer_limit(1)
+        n0 = fast.launch_count()
+        a, _, graphed = fast.decode_run(first, len(prompts[0]), 4, use_graph=True)
+        n1 = fast.launch_count()
+        b, _, _ = fast.decode_run(first, len(prompts[0]), 4, use_graph=False)
+        assert graphed and list(a) == list(b)
+        assert n1 - n0 == fast.launch_count() - n1
+    finally:
+        fast.close()
 
 
 def test_forward_returns_a_device_handle_that_reads_like_the_host_tensor(L, tiny):
@@ -491,6 +506,9 @@ def test_forward_returns_a_device_handle_that_reads_like_the_host_tensor(L, tiny
         with pytest.raises(L.ml.MlError):
             lg2.RawData                                                           # never read, and a newer Forward ran
         assert lg3.Size == [1, args["vocab_size"]]
+        gm.Transformer.forward_argmax(ctx, toks[:1] + 3, 7, want_logits="last")  # any forward ends the handle
+        c, out = L._capi, np.empty((1, args["vocab_size"]), np.float32)
+        assert c.lib.lnb_session_logits_read(ctx.h, lg3.generation, 0, 1, c.ptr(out, c.f32p)) == -4    # LNB_ESTATE
     finally:
         ctx.close()
         osess.close()
