@@ -295,7 +295,10 @@ int lnb_op_rms_scale_f32(const uint16_t* x, float* r, int S, int D, float eps, i
 /* applyRotaryEmbeddings for one tensor (llamatransformer.go:753-790): x[S,H,hd] */
 int lnb_op_rope_bf16(const uint16_t* x, const float* cis, uint16_t* out, int S, int H, int hd, int start_pos);
 /* the attention core of LlamaAttention.Forward (llamatransformer.go:402-514):
- * q[S,n_heads,hd] rotated, cache_k/v[T,n_kv,hd] -> out[S,n_heads*hd] */
+ * q[S,n_heads,hd] rotated, cache_k/v[T,n_kv,hd] -> out[S,n_heads*hd].
+ * causal_mask: 0 = none; 1 = the reference's [S,S] mask (T must equal S, LNB_EINVAL otherwise); 2 = EXTENSION, the
+ * [S,T] mask of a chunked prefill: query row s sits at position T - S + s and sees the keys t <= T - S + s (the
+ * kernels a session's chunked prefill runs for this mode and S) */
 int lnb_op_attention_bf16(const uint16_t* q, const uint16_t* cache_k, const uint16_t* cache_v, uint16_t* out,
                           int S, int T, int n_heads, int n_kv, int hd, int causal_mask, int acc_mode);
 /* ml.Silu (activations.go:27-50), ml.Add / ml.MultiplyElementwise same-shape bf16

@@ -2648,7 +2648,8 @@ extern "C" int lnb_op_attention_bf16(const uint16_t* q, const uint16_t* cache_k,
   OpScope scope_;
   if (!q || !cache_k || !cache_v || !out) return fail(LNB_EINVAL, "NULL argument");
   if (S <= 0 || T < S || n_heads <= 0 || n_kv <= 0 || n_heads % n_kv || hd <= 0 || hd % 8) return fail(LNB_EINVAL, "bad shape");
-  if (causal_mask && T != S) return fail(LNB_EINVAL, "causal mask needs T == S (reference mask is [S,S])");
+  if (causal_mask < 0 || causal_mask > 2) return fail(LNB_EINVAL, "bad causal_mask %d", causal_mask);
+  if (causal_mask == 1 && T != S) return fail(LNB_EINVAL, "causal mask needs T == S (reference mask is [S,S])");
   const size_t smem = (size_t)T * 12 + (size_t)hd * 4;
   if (smem > 200 * 1024) return fail(LNB_EINVAL, "T %d too long", T);
   const size_t qb = (size_t)S * n_heads * hd * 2, cb = (size_t)T * n_kv * hd * 2;
@@ -2657,10 +2658,12 @@ extern "C" int lnb_op_attention_bf16(const uint16_t* q, const uint16_t* cache_k,
   CU(cudaFuncSetAttribute(sdpa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   const float f = attn_scale_bf16(hd);
   if (acc_mode == LNB_ACC_FAST && S > 1 && causal_mask && hd == SP_HD && (n_heads * hd) % 128 == 0) {
-    // the prefill path's tiled two-pass kernel (writes the X8 operand of the Wo GEMM; unpacked here)
+    // the prefill path's tiled two-pass kernel (writes the X8 operand of the Wo GEMM; unpacked here); query row s sits at
+    // position (T - S) + s, as in a session's chunked prefill
     const int Mpad = (S + 127) / 128 * 128;
+    const int32_t pos0 = T - S;
     OPBUF(d8, (size_t)Mpad * n_heads * hd * 2); OPBUF(dpos, 16);
-    CU(cudaMemset(dpos.p, 0, 16));
+    H2D(dpos, &pos0, sizeof(pos0));
     const double* exp_tab = (sdpa_tc_enabled() && S >= 32) ? exp_table_device() : nullptr;
     if (exp_tab) {
       CU(cudaFuncSetAttribute(sdpa_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ST_SMEM));

@@ -24,6 +24,11 @@ LLAMA31_8B = dict(dim=4096, n_layers=32, n_heads=32, n_kv_heads=8, head_dim=128,
 TINY = dict(dim=256, n_layers=2, n_heads=8, n_kv_heads=2, head_dim=32, ffn_dim=512,
             vocab_size=1024, max_seq_len=64, norm_eps=1e-5, rope_theta=500000.0, use_scaled_rope=1)
 
+# the same with the 8B model's head_dim of 128: FAST prompts of >= 32 tokens run the tensor-core prefill with its
+# wgmma attention kernel (sdpa_tc_kernel), which only serves head_dim 128
+TINY128 = dict(dim=1024, n_layers=2, n_heads=8, n_kv_heads=2, head_dim=128, ffn_dim=1024,
+               vocab_size=2048, max_seq_len=512, norm_eps=1e-5, rope_theta=500000.0, use_scaled_rope=1)
+
 # 8 fixed prompt ids (first = <|begin_of_text|>) and the reference's stop ids
 # (src/tiktoken/tiktokenreader.go:81)
 PROMPT_8 = [128000, 9906, 11, 856, 836, 374, 220, 16]

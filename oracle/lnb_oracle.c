@@ -421,6 +421,11 @@ void orc_attention(const uint16_t* q, const uint16_t* cacheK, const uint16_t* ca
   attention_impl(q, cacheK, cacheV, out, S, T, n_heads, n_kv, hd, causal_mask, 0);
 }
 
+void orc_attention_pos(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out, int S, int T,
+                       int n_heads, int n_kv, int hd, int causal_mask, int q_pos0) {
+  attention_impl(q, cacheK, cacheV, out, S, T, n_heads, n_kv, hd, causal_mask, q_pos0);
+}
+
 /* ------------------------------------------------------------ whole model */
 
 struct orc_model {

@@ -80,6 +80,10 @@ void orc_rope_apply(const uint16_t* x, const float* cis, uint16_t* out, int S, i
  * q[S,n_heads,hd] (already rotated), cacheK/V [>=T, n_kv, hd]; out [S, n_heads*hd]. */
 void orc_attention(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out,
                    int S, int T, int n_heads, int n_kv, int hd, int causal_mask);
+/* extension (beyond the reference): the same with query row s at absolute position q_pos0 + s, so a causal row sees the
+ * keys t <= q_pos0 + s -- the [S,T] mask of a chunked prefill (q_pos0 = T - S) */
+void orc_attention_pos(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out,
+                       int S, int T, int n_heads, int n_kv, int hd, int causal_mask, int q_pos0);
 
 /* ---- whole model ---- */
 typedef struct {

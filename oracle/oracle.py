@@ -99,6 +99,7 @@ def _declare(L):
     L.orc_rope_table.argtypes = [C.c_int, C.c_int, C.c_double, C.c_int, _u16p, _f32p]
     L.orc_rope_apply.argtypes = [_u16p, _f32p, _u16p, C.c_int, C.c_int, C.c_int, C.c_int]
     L.orc_attention.argtypes = [_u16p, _u16p, _u16p, _u16p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    L.orc_attention_pos.argtypes = [_u16p, _u16p, _u16p, _u16p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     L.orc_model_new.restype = C.c_void_p
     L.orc_model_new.argtypes = [C.POINTER(OrcArgs)]
     L.orc_model_free.argtypes = [C.c_void_p]
@@ -271,12 +272,18 @@ def rope_apply(x, cis, start_pos):
     return out
 
 
-def attention(q, cache_k, cache_v, T, causal_mask):
+def attention(q, cache_k, cache_v, T, causal_mask, q_pos0=0):
+    """q_pos0 > 0 (EXTENSION, beyond the reference): query row s sits at position q_pos0 + s, so a causal row sees the
+    keys t <= q_pos0 + s -- the [S,T] mask of a chunked prefill"""
     S, nh, hd = q.shape
     nkv = cache_k.shape[1]
     out = np.empty((S, nh * hd), np.uint16)
-    lib().orc_attention(_p(q, _u16p), _p(cache_k, _u16p), _p(cache_v, _u16p), _p(out, _u16p),
-                        S, T, nh, nkv, hd, int(causal_mask))
+    if q_pos0:
+        lib().orc_attention_pos(_p(q, _u16p), _p(cache_k, _u16p), _p(cache_v, _u16p), _p(out, _u16p),
+                                S, T, nh, nkv, hd, int(causal_mask), int(q_pos0))
+    else:
+        lib().orc_attention(_p(q, _u16p), _p(cache_k, _u16p), _p(cache_v, _u16p), _p(out, _u16p),
+                            S, T, nh, nkv, hd, int(causal_mask))
     return out
 
 

@@ -126,3 +126,34 @@ def test_full_size_linear_strict_bit_exact(L, N, K):
     e, f = O.bf16_to_f32(exp).astype(np.float64), O.bf16_to_f32(fast).astype(np.float64)
     ulp = 2.0 ** (np.floor(np.log2(np.maximum(np.abs(e), 1e-30))) - 7)
     assert (np.abs(f - e) <= np.maximum(ulp, 1e-5)).all()
+
+
+# largest |logit| distance of any row: measured 0.0273 (median row 0.0230) on an H100 SXM (80 GB), pinned at 0.05
+PREFILL_136_MAX_ABS = 0.05
+
+
+def test_8b_fast_tensor_core_prefill_all_rows(L, big):
+    """a FAST prefill of 136 synthetic tokens (max_rows 136, every row's logits) runs the tensor-core path at the real shapes:
+    sdpa_tc_kernel with 32 heads over 8 KV heads, gemm_tc_kernel at K = 14336 (w2), and the TC_EPI_F32TRUNC LM head at
+    N = 128256 for rows 0..134.  Every row is compared with the oracle's all-rows forward (13 s of CPU on the GPU machine's
+    host; the whole test took 14 s)."""
+    import time
+    args, om, gm, _, _, _, _ = big
+    S = 136
+    toks = np.random.default_rng(136).integers(0, args["vocab_size"], size=S).astype(np.int32)
+    t0 = time.perf_counter()
+    sess = om.new_session(S)
+    try:
+        exp = sess.forward(toks, 0, all_rows=True)
+    finally:
+        sess.close()
+    t_oracle = time.perf_counter() - t0
+    ctx = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(S), max_rows=S, acc_mode=L._capi.LNB_ACC_FAST)
+    try:
+        nxt, got = gm.Transformer.forward_argmax(ctx, toks, 0, want_logits="all")
+    finally:
+        ctx.close()
+    per_row = np.abs(got - exp).max(1)
+    print(f"8B prefill S={S}: oracle {t_oracle:.1f} s, max-abs per row: max {per_row.max():.4f}, median {np.median(per_row):.4f}")
+    assert nxt == int(np.argmax(got[-1]))
+    assert per_row.max() <= PREFILL_136_MAX_ABS, (int(per_row.argmax()), float(per_row.max()))

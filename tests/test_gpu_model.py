@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 
 from oracle import oracle as O
-from tests.helpers import bf16_ulp_diff, host_tensors, oracle_model
+from tests.helpers import bf16_ulp_diff, f32, host_tensors, oracle_model
 
 pytestmark = pytest.mark.gpu
 
@@ -56,7 +56,11 @@ def test_device_generator_equals_host_generator(L, tiny):
 
 @pytest.mark.parametrize("prompt_len", [1, 5, 8])
 def test_forward_strict_bit_exact(L, tiny, prompt_len):
-    args, _, om, gm = tiny
+    check_forward_strict(L, tiny, prompt_len)
+
+
+def check_forward_strict(L, model, prompt_len):
+    args, _, om, gm = model
     rng = np.random.default_rng(prompt_len)
     seq = 24
     toks = rng.integers(0, args["vocab_size"], size=seq).astype(np.int32)
@@ -519,7 +523,11 @@ def test_chunked_prefill_extension_equals_one_shot_prefill(L, tiny, mode):
     """SURVEY 8f-4 (beyond the reference): S > 1 at startPos > 0 with the [S,T] causal mask.  The library refuses it by
     default exactly like the reference's [S,S] mask would fail; with the switch on, a prompt fed in chunks leaves the caches
     and logits of the one-shot prefill (bit-identical in STRICT, and equal to the oracle's extension)."""
-    args, _, om, gm = tiny
+    check_chunked_prefill(L, tiny, mode)
+
+
+def check_chunked_prefill(L, model, mode):
+    args, _, om, gm = model
     acc = L._capi.LNB_ACC_STRICT if mode == "strict" else L._capi.LNB_ACC_FAST
     rng = np.random.default_rng(8)
     prompt = rng.integers(0, args["vocab_size"], size=19).astype(np.int32)
@@ -554,3 +562,184 @@ def test_chunked_prefill_extension_equals_one_shot_prefill(L, tiny, mode):
             assert got == list(om.generate(prompt, seq, stop_ids=gm.Vocabulary.StopTokenIds))
     finally:
         one.close(); chk.close(); o1.close(); o2.close()
+
+
+# ---- the tensor-core prefill on a head_dim-128 miniature: gemm_tc_kernel + sdpa_tc_kernel inside a model forward --------
+
+@pytest.fixture(scope="module")
+def tiny128(L):
+    """synth.TINY128: head_dim 128 and every tensor-core tiling condition of the prefill path (forward_tc_ok) hold, so a FAST
+    prompt of >= 32 tokens runs gemm_tc_kernel for every projection and sdpa_tc_kernel for attention"""
+    args = dict(L.synth.TINY128)
+    tensors = host_tensors(args, SEED)
+    om = oracle_model(args, tensors)
+    gm = L.model.LoadModelFromTensors(args, tensors)
+    yield args, tensors, om, gm
+    gm.Free()
+    om.close()
+
+
+# Largest distance from the oracle of a FAST tensor-core prefill of tiny128, per element, in bf16 ulps of the element
+# (of 2^-6 of the tensor's largest magnitude for smaller elements, where cancellation makes an ulp meaningless).
+# The reorder noise is close to absolute (a few ulps of the tensor's large entries), so small elements show the most ulps.
+# Pinned at about 1.5x the largest of S = 32, 129, 300 and both attention kernels, measured on an H100 SXM (80 GB):
+# logits 105.5 (chunked prefill: 66), residual after layer 1 32, after the last layer 64, K/V caches 58, decode steps 86.25.
+TC_ULPS = dict(logits=160, residual1=48, residual=96, cache=88, decode=128)
+
+
+def _ulps(got, exp):
+    g, e = np.asarray(got, np.float64), np.asarray(exp, np.float64)
+    floor = 2.0 ** -6 * max(np.abs(e).max(), 2.0 ** -100)
+    return np.abs(g - e) / 2.0 ** (np.floor(np.log2(np.maximum(np.abs(e), floor))) - 7)
+
+
+def _tc_launches(n_layers, S, all_rows):
+    """kernels enqueue_forward_tc launches for one forward on one GPU, plus the set_state_kernel of the call: gather_rows,
+    then per layer rmsnorm_x8, gemm_tc (wq|wk|wv), rope_kv, the attention kernel, gemm_tc (wo + residual), rmsnorm_x8,
+    gemm_tc (w1|w3 + SwiGLU), gemm_tc (w2 + residual); all-rows logits add rmsnorm_x8 + gemm_tc for rows < S - 1; the last
+    row's LM head GEMV"""
+    return 1 + 1 + 8 * n_layers + (2 if all_rows and S > 1 else 0) + 1
+
+
+def _kernel_env(monkeypatch, kernel):
+    if kernel == "sdpa_prefill":
+        monkeypatch.setenv("LNB_SDPA_TC", "0")
+    else:
+        monkeypatch.delenv("LNB_SDPA_TC", raising=False)
+
+
+def test_tiny128_prefill_runs_the_tensor_core_path(L, tiny128, monkeypatch):
+    """the path the other tiny128 tests claim to cover is the one that runs: head_dim 128 selects the sdpa_tc_kernel branch
+    of enqueue_forward_tc, the launch count of one forward is that function's, and LNB_SDPA_TC=0 (sdpa_prefill_kernel) gives
+    different bits"""
+    args, _, _, gm = tiny128
+    monkeypatch.delenv("LNB_SDPA_TC", raising=False)
+    assert args["head_dim"] == 128
+    q_l, kv_l = args["n_heads"] * 128, args["n_kv_heads"] * 128
+    assert (q_l + 2 * kv_l) % 128 == 0 and args["dim"] % 128 == 0 and (2 * args["ffn_dim"]) % 128 == 0 and args["ffn_dim"] % 128 == 0
+    toks = np.random.default_rng(3).integers(0, args["vocab_size"], size=300).astype(np.int32)
+    ctx = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(320), max_rows=300, acc_mode=L._capi.LNB_ACC_FAST)
+    try:
+        for S, want in ((32, "all"), (129, "last"), (300, "all"), (200, "none")):
+            n0 = ctx.launch_count()
+            gm.Transformer.forward_argmax(ctx, toks[:S], 0, want_logits=want)
+            assert ctx.launch_count() - n0 == _tc_launches(args["n_layers"], S, want == "all"), (S, want)
+        ctx.set_layer_limit(1)
+        n0 = ctx.launch_count()
+        gm.Transformer.forward_argmax(ctx, toks[:64], 0, want_logits="all")
+        assert ctx.launch_count() - n0 == _tc_launches(1, 64, True)
+        ctx.set_layer_limit(0)
+        _, a = gm.Transformer.forward_argmax(ctx, toks[:129], 0, want_logits="all")
+        monkeypatch.setenv("LNB_SDPA_TC", "0")
+        _, b = gm.Transformer.forward_argmax(ctx, toks[:129], 0, want_logits="all")
+        assert not np.array_equal(a, b)
+    finally:
+        ctx.close()
+
+
+@pytest.mark.parametrize("kernel", ["sdpa_tc", "sdpa_prefill"])
+@pytest.mark.parametrize("S", [32, 129, 300])
+def test_tiny128_fast_prefill_within_pinned_ulps_of_the_oracle(L, tiny128, S, kernel, monkeypatch):
+    """one-shot FAST prefill at S = 32 (one tile of everything), 129 (one row past a 128-row tile) and 300 (three query
+    tiles, five key tiles) against the oracle: logits of every row, the residual stream after layer 1 and after the last
+    layer, both caches of every layer, and four decode steps on the caches the prefill wrote -- every element within
+    TC_ULPS.  Measured on an H100 SXM, largest over both kernels (ulps): S = 32: logits 105.5, residual1 24, residual 50,
+    cache 58, decode 86.25; S = 129: 52.5, 24, 64, 33, 64; S = 300: 70.1, 32, 64, 43, 79."""
+    _kernel_env(monkeypatch, kernel)
+    args, _, om, gm = tiny128
+    rng = np.random.default_rng(S + 128)
+    toks = rng.integers(0, args["vocab_size"], size=S + 4).astype(np.int32)
+    osess = om.new_session(S + 4)
+    ctx = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(S + 4), max_rows=S, acc_mode=L._capi.LNB_ACC_FAST)
+    one = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(S + 4), max_rows=S, acc_mode=L._capi.LNB_ACC_FAST)
+    try:
+        exp, tr = osess.forward(toks[:S], 0, all_rows=True, trace=True)
+        nxt, got = gm.Transformer.forward_argmax(ctx, toks[:S], 0, want_logits="all")
+        assert nxt == int(np.argmax(got[-1]))
+        m = dict(logits=_ulps(got, exp).max(), residual=_ulps(f32(ctx.residual(S)), f32(tr[-1])).max(), cache=0.0, decode=0.0)
+        for layer in range(args["n_layers"]):
+            ok, ov = osess.cache(layer)
+            m["cache"] = max(m["cache"], _ulps(f32(ctx.CacheK(layer).RawData[:S]), f32(ok[:S])).max(),
+                             _ulps(f32(ctx.CacheV(layer).RawData[:S]), f32(ov[:S])).max())
+        one.set_layer_limit(1)
+        gm.Transformer.forward_argmax(one, toks[:S], 0)
+        m["residual1"] = _ulps(f32(one.residual(S)), f32(tr[1])).max()
+        for pos in range(S, S + 4):
+            e = osess.forward(toks[pos:pos + 1], pos)
+            g = gm.Transformer.Forward(ctx, L.ml.Tensor(toks[pos:pos + 1], L.ml.DT_INT32), pos).RawData
+            m["decode"] = max(m["decode"], _ulps(g, e).max())
+        print(f"tiny128 S={S} {kernel}: " + ", ".join(f"{k} {v:.2f}" for k, v in sorted(m.items())))
+        for k, v in m.items():
+            assert v <= TC_ULPS[k], (k, v)
+    finally:
+        ctx.close(); one.close(); osess.close()
+
+
+@pytest.mark.parametrize("kernel", ["sdpa_tc", "sdpa_prefill"])
+@pytest.mark.parametrize("S1,S2", [(40, 300), (129, 200)])
+def test_tiny128_prefill_rows_do_not_depend_on_later_rows(L, tiny128, S1, S2, kernel, monkeypatch):
+    """prefill prompt[:S1] and prompt[:S2]: each row's GEMM and attention arithmetic is independent of the other rows (masked
+    keys add exact zeros; Z is split over threads by absolute key index), so every layer's K/V rows < S1, the residual rows
+    < S1 and the logits rows < S1 - 1 are bit-identical (row S1 - 1 of the shorter run comes from the LM-head GEMV)"""
+    _kernel_env(monkeypatch, kernel)
+    args, _, _, gm = tiny128
+    toks = np.random.default_rng(S1 * S2).integers(0, args["vocab_size"], size=S2).astype(np.int32)
+    a = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(S2), max_rows=S1, acc_mode=L._capi.LNB_ACC_FAST)
+    b = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(S2), max_rows=S2, acc_mode=L._capi.LNB_ACC_FAST)
+    try:
+        _, la = gm.Transformer.forward_argmax(a, toks[:S1], 0, want_logits="all")
+        _, lb = gm.Transformer.forward_argmax(b, toks, 0, want_logits="all")
+        for layer in range(args["n_layers"]):
+            assert np.array_equal(a.CacheK(layer).RawData[:S1], b.CacheK(layer).RawData[:S1]), f"K cache, layer {layer}"
+            assert np.array_equal(a.CacheV(layer).RawData[:S1], b.CacheV(layer).RawData[:S1]), f"V cache, layer {layer}"
+        assert np.array_equal(a.residual(S1), b.residual(S2)[:S1])
+        assert np.array_equal(la[:S1 - 1], lb[:S1 - 1])
+    finally:
+        a.close(); b.close()
+
+
+@pytest.mark.parametrize("kernel", ["sdpa_tc", "sdpa_prefill"])
+def test_tiny128_chunked_fast_prefill_equals_one_shot(L, tiny128, kernel, monkeypatch):
+    """a 300-token prompt in chunks of 40 + 100 + 33 + 127 (starts 0, 40, 140, 173: on and off multiples of 64 and 128, so
+    the query tiles no longer line up with the key tiles) on the tensor-core path: caches and the residual are bit-identical
+    to the one-shot prefill, and so are the logits except each earlier chunk's last row (GEMV there, GEMM in the one-shot
+    run); every chunk is within TC_ULPS of the oracle's chunk extension"""
+    _kernel_env(monkeypatch, kernel)
+    args, _, om, gm = tiny128
+    n = 300
+    prompt = np.random.default_rng(77).integers(0, args["vocab_size"], size=n).astype(np.int32)
+    one = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(n + 4), max_rows=n, acc_mode=L._capi.LNB_ACC_FAST)
+    chk = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(n + 4), max_rows=127, acc_mode=L._capi.LNB_ACC_FAST)
+    osess = om.new_session(n + 4)
+    try:
+        chk.allow_chunked_prefill(True)
+        n1, l1 = gm.Transformer.forward_argmax(one, prompt, 0, want_logits="all")
+        r1 = one.residual(n)
+        pos, worst = 0, 0.0
+        chunks = (40, 100, 33, 127)
+        for i, size in enumerate(chunks):
+            n2, l2 = gm.Transformer.forward_argmax(chk, prompt[pos:pos + size], pos, want_logits="all")
+            last = i == len(chunks) - 1
+            assert np.array_equal(l2 if last else l2[:-1], l1[pos:pos + size] if last else l1[pos:pos + size - 1]), f"chunk at {pos}"
+            e2 = osess.forward(prompt[:size], 0, all_rows=True) if pos == 0 else osess.forward_chunk(prompt[pos:pos + size], pos)
+            worst = max(worst, _ulps(l2, e2).max())
+            pos += size
+        assert n2 == n1
+        assert np.array_equal(chk.residual(127), r1[n - 127:])
+        for layer in range(args["n_layers"]):
+            assert np.array_equal(chk.CacheK(layer).RawData[:n], one.CacheK(layer).RawData[:n]), f"K cache, layer {layer}"
+            assert np.array_equal(chk.CacheV(layer).RawData[:n], one.CacheV(layer).RawData[:n]), f"V cache, layer {layer}"
+        print(f"tiny128 chunked {kernel}: logits {worst:.2f} ulps from the oracle")
+        assert worst <= TC_ULPS["logits"]
+    finally:
+        one.close(); chk.close(); osess.close()
+
+
+@pytest.mark.parametrize("prompt_len", [1, 8])
+def test_forward_strict_bit_exact_head_dim_128(L, tiny128, prompt_len):
+    """test_forward_strict_bit_exact on tiny128: the persistent decode engine's head_dim-128 attention, bit for bit"""
+    check_forward_strict(L, tiny128, prompt_len)
+
+
+def test_chunked_prefill_strict_head_dim_128(L, tiny128):
+    check_chunked_prefill(L, tiny128, "strict")

@@ -190,7 +190,8 @@ def test_attention_strict_bit_exact(L, S, T, causal):
     if S >= 32 and causal:
         # prompt-sized FAST attention runs sdpa_tc_kernel: q.k and p.v accumulate in the tensor core's order, so a score or an
         # output can land on the other side of a bf16 truncation boundary (a small fraction of the outputs, by at most one
-        # bf16 ulp; tools/sdpa_tc_check.py measures it)
+        # bf16 ulp).  The order-free checks of both FAST prompt kernels are test_attention_fast_prompt_within_order_free_bounds
+        # and test_attention_mask_probes below
         d = np.abs(O.bf16_to_f32(out).astype(np.float64) - O.bf16_to_f32(exp).astype(np.float64))
         assert d.max() <= 2.0 ** -7 and (out != exp).mean() < 5e-3
     else:
@@ -266,3 +267,174 @@ def test_linear_tensor_core_prefill(L, S, K, N):
     finally:
         ml.ACC_MODE = L._capi.LNB_ACC_STRICT
     assert np.array_equal(got, O.linear_bf16(xi, wi))
+
+
+# ---- gemm_tc_kernel at its tile edges: exact data, order-free bounds, row independence --------------------------------
+
+def _linear(L, x, w, acc):
+    ml = L.ml
+    ml.ACC_MODE = acc
+    try:
+        return ml.LinearTransformation(ml.Tensor(x, ml.DT_BF16), ml.Tensor(w, ml.DT_BF16)).RawData
+    finally:
+        ml.ACC_MODE = L._capi.LNB_ACC_STRICT
+
+
+# M: one partial M tile, one row short of / exactly / one row past a 128-row tile, 16 tiles.  K in 128-wide k-tiles: 1, 2,
+# 3 (= TC_NS, the ring fills exactly), 4 (first reuse of stage 0), 32 and 112 (the mbarrier phase flips many times).
+# N: one, two and twelve 128-column tiles, and the stacked w1|w3 width.
+TC_EDGES = [(32, 128, 128), (127, 256, 256), (128, 384, 128), (129, 512, 1536), (255, 4096, 256), (2048, 512, 256),
+            (129, 14336, 128), (32, 4096, 28672), (128, 128, 1536), (255, 256, 128)]
+
+
+@pytest.mark.parametrize("M,K,N", TC_EDGES)
+def test_gemm_tc_edges_exact_bounded_and_row_independent(L, M, K, N):
+    """lnb_op_linear_bf16 in FAST mode at M >= 32 runs gemm_tc_kernel (tc_eligible: N % 128 == 0, K % 128 == 0).
+    (1) exact data: integers |x|, |w| <= 15, every row of X and every row of W scaled by its own power of two, so each
+    output's partial sums are integers of one common unit below 2^22 -- exact in fp32 in any order: the result must be
+    bit-identical to the oracle and to the f64 value truncated to bf16.  (2) random data: every output inside
+    tests.precise.linear_bounds.  (3) a row's result does not depend on the other rows: a prefix of X gives the prefix of
+    the output, and permuting X's rows permutes the output rows, bit for bit."""
+    from tests import precise as P
+    assert M >= 32 and N % 128 == 0 and K % 128 == 0
+    fast = L._capi.LNB_ACC_FAST
+    rng = np.random.default_rng(M * 31 + K * 7 + N)
+    rs = rng.integers(-6, 7, M).astype(np.float64)
+    cs = rng.integers(-6, 7, N).astype(np.float64)
+    xv = rng.integers(-15, 16, (M, K)) * 2.0 ** rs[:, None]
+    wv = rng.integers(-15, 16, (N, K)) * 2.0 ** cs[:, None]
+    xi, wi = bf(xv).reshape(M, K), bf(wv).reshape(N, K)
+    assert np.array_equal(f32(xi).reshape(M, K), xv) and np.array_equal(f32(wi).reshape(N, K), wv)
+    got = _linear(L, xi, wi, fast)
+    exact = xv @ wv.T
+    assert np.abs(exact / (2.0 ** (rs[:, None] + cs[None, :]))).max() < 2 ** 22
+    assert np.array_equal(got, bf(exact).reshape(M, N)), f"{(got != bf(exact).reshape(M, N)).sum()} of {got.size} differ"
+    assert np.array_equal(got, O.linear_bf16(xi, wi))
+
+    x = rand_bf16(rng, (M, K))
+    w = rand_bf16(rng, (N, K), 1.0 / math.sqrt(K))
+    got = _linear(L, x, w, fast)
+    lo, hi = P.linear_bounds(x, w)
+    assert P.within(got, lo, hi).all(), P.outside_report(got, lo, hi)
+    if M > 32:
+        m1 = max(32, M // 2 + 1)
+        assert np.array_equal(_linear(L, np.ascontiguousarray(x[:m1]), w, fast), got[:m1]), f"prefix of {m1} rows"
+    perm = rng.permutation(M)
+    assert np.array_equal(_linear(L, np.ascontiguousarray(x[perm]), w, fast), got[perm]), "permuted rows"
+
+
+# ---- prompt attention: STRICT sdpa_kernel, FAST sdpa_tc_kernel and sdpa_prefill_kernel, with a start position ---------
+
+def _attention(L, q, ck, cv, S, T, causal, acc):
+    nh, hd = q.shape[1], q.shape[2]
+    nkv = ck.shape[1]
+    out = np.empty((S, nh * hd), np.uint16)
+    c = L._capi
+    c.check(c.lib.lnb_op_attention_bf16(c.ptr(q, c.u16p), c.ptr(ck, c.u16p), c.ptr(cv, c.u16p), c.ptr(out, c.u16p),
+                                        S, T, nh, nkv, hd, causal, acc))
+    return out
+
+
+# (S, T - S, n_heads, n_kv): S on both sides of the 64-key tile, the 128-row query tile and the 32-row FMA tile; starts that
+# are 0, 1, and multiples and non-multiples of 64; n_rep 1, 4 and 8
+ATTN_CASES = [(32, 0, 8, 8), (63, 1, 32, 8), (64, 40, 32, 4), (65, 64, 8, 8), (127, 100, 32, 8), (128, 1, 8, 8),
+              (129, 0, 32, 4), (200, 64, 8, 8), (513, 100, 32, 8), (129, 40, 8, 8), (64, 0, 32, 8), (200, 1, 32, 4)]
+FAST_KERNELS = ["sdpa_tc", "sdpa_prefill"]
+
+
+@pytest.mark.parametrize("S,dpos,nh,nkv", ATTN_CASES)
+def test_attention_chunk_mask_strict_bit_exact(L, S, dpos, nh, nkv):
+    """causal_mask = 2 (query row s at position T - S + s) in STRICT runs sdpa_kernel: the oracle's bits"""
+    T, hd = S + dpos, 128
+    rng = np.random.default_rng(S * 131 + dpos)
+    q = rand_bf16(rng, (S, nh, hd))
+    ck, cv = rand_bf16(rng, (T, nkv, hd)), rand_bf16(rng, (T, nkv, hd))
+    exp = O.attention(q, ck, cv, T, 1, q_pos0=dpos)
+    got = _attention(L, q, ck, cv, S, T, 2, L._capi.LNB_ACC_STRICT)
+    assert np.array_equal(got, exp), f"{(got != exp).sum()} of {got.size} differ"
+    if dpos == 0:
+        assert np.array_equal(_attention(L, q, ck, cv, S, T, 1, L._capi.LNB_ACC_STRICT), exp)
+
+
+@pytest.mark.parametrize("kernel", FAST_KERNELS)
+@pytest.mark.parametrize("S,dpos,nh,nkv", ATTN_CASES)
+def test_attention_fast_prompt_within_order_free_bounds(L, S, dpos, nh, nkv, kernel, monkeypatch):
+    """FAST prompt attention (S >= 32, causal_mask = 2) on sdpa_tc_kernel, and on sdpa_prefill_kernel with LNB_SDPA_TC=0.
+    Exact-score inputs: every output inside tests.precise.attention_bounds (a statement about the exact softmax weights,
+    not about the STRICT summation order).  Random inputs: the reorder statistics against the STRICT oracle."""
+    from tests import precise as P
+    if kernel == "sdpa_prefill":
+        monkeypatch.setenv("LNB_SDPA_TC", "0")
+    T, hd = S + dpos, 128
+    fast = L._capi.LNB_ACC_FAST
+    rng = np.random.default_rng(S * 17 + dpos + nh)
+    q, ck = P.exact_score_qk(rng, S, T, nh, nkv, hd)
+    cv = rand_bf16(rng, (T, nkv, hd))
+    got = _attention(L, q, ck, cv, S, T, 2, fast)
+    lo, hi = P.attention_bounds(q, ck, cv, T, dpos)
+    assert P.within(got, lo, hi).all(), P.outside_report(got, lo, hi)
+    if dpos == 0:
+        assert np.array_equal(_attention(L, q, ck, cv, S, T, 1, fast), got)
+    q = rand_bf16(rng, (S, nh, hd))
+    ck, cv = rand_bf16(rng, (T, nkv, hd)), rand_bf16(rng, (T, nkv, hd))
+    got = _attention(L, q, ck, cv, S, T, 2, fast)
+    exp = O.attention(q, ck, cv, T, 1, q_pos0=dpos)
+    d = np.abs(f32(got).astype(np.float64) - f32(exp).astype(np.float64))
+    assert d.max() <= 2.0 ** -7 and (got != exp).mean() < 5e-3, (d.max(), (got != exp).mean())
+
+
+def _mask_probe(T, nh, nkv, S, pos0, hd=128):
+    """q, k, v for which the diagonal key (t = qpos) and the first masked key (t = qpos + 1) of every row score 512 / t(sqrt(128))
+    and every other key at most half of that: key t is 16 at dimension t % 64 and 16 at 64 + t // 64; row qpos asks for
+    both coordinates of qpos and of qpos + 1.  (Across a 64-key block boundary key qpos - 63 scores high too.)  v row t
+    carries the bits of t as +-2 in dimensions 0..9, so the output names the keys a row attends to."""
+    def onehot(t):
+        e = np.zeros(hd, np.float32)
+        e[t % 64] = 16
+        e[64 + t // 64] = 16
+        return e
+    k1 = np.stack([onehot(t) for t in range(T)])
+    q1 = np.stack([np.maximum(onehot(p), onehot(p + 1)) for p in range(pos0, pos0 + S)])
+    v1 = np.zeros((T, hd), np.float32)
+    for j in range(10):
+        v1[:, j] = 4 * ((np.arange(T) >> j) & 1) - 2
+    q = bf(np.repeat(q1[:, None, :], nh, 1)).reshape(S, nh, hd)
+    k = bf(np.repeat(k1[:, None, :], nkv, 1)).reshape(T, nkv, hd)
+    v = bf(np.repeat(v1[:, None, :], nkv, 1)).reshape(T, nkv, hd)
+    return q, k, v
+
+
+@pytest.mark.parametrize("kernel", FAST_KERNELS + ["strict"])
+@pytest.mark.parametrize("S,pos0", [(200, 0), (129, 64), (129, 128), (150, 40), (96, 100), (64, 1), (40, 191)])
+def test_attention_mask_probes(L, S, pos0, kernel, monkeypatch):
+    """the causal boundary itself: with these inputs a leaked first future key, or a lost diagonal key, moves each row's
+    output by at least 0.25 (shown on the exact softmax below), so any such row fails; starts on and off multiples of 64
+    and 128"""
+    from tests import precise as P
+    if kernel == "sdpa_prefill":
+        monkeypatch.setenv("LNB_SDPA_TC", "0")
+    nh, nkv, T = 8, 2, S + pos0
+    q, k, v = _mask_probe(T, nh, nkv, S, pos0)
+    assert P.exact_score_inputs(q, k)
+    acc = L._capi.LNB_ACC_STRICT if kernel == "strict" else L._capi.LNB_ACC_FAST
+    got = f32(_attention(L, q, k, v, S, T, 2, acc)).reshape(S, nh, 128)[:, :, :10].astype(np.float64)
+    vis = P.visible_keys(S, T, pos0)
+    rows = np.arange(S)
+    vf = f32(v).reshape(T, nkv, 128)[:, :1, :10].astype(np.float64)
+
+    def out(visible):
+        p = P.attention_probs(q[:, :1], k[:, :1], T, visible)
+        return np.einsum("sht,thd->shd", p, vf)[:, 0]
+
+    ok = out(vis)
+    leak = vis.copy()
+    fut = rows[pos0 + rows + 1 < T]
+    leak[fut, pos0 + fut + 1] = True
+    assert (np.abs(out(leak) - ok).max(1)[fut] >= 0.25).all()
+    nodiag = vis.copy()
+    nodiag[rows, pos0 + rows] = False
+    probed = rows[pos0 + rows > 0]                                  # row at position 0 sees only its diagonal
+    with np.errstate(invalid="ignore"):
+        assert (np.abs(out(nodiag) - ok).max(1)[probed] >= 0.25).all()
+    err = np.abs(got - ok[:, None, :]).max((1, 2))
+    assert (err < 0.125).all(), f"rows {np.nonzero(err >= 0.125)[0][:10]} attend to the wrong keys (max err {err.max()})"
