@@ -186,7 +186,12 @@ int lnb_model_destroy(lnb_model* m); /* hook for model.Model.Free (src/model/mod
 
 /* model.NewInferenceContext (src/model/inferencecontext.go:17-46): KV cache of seq_len rows
  * per layer, zero-filled.  max_rows = largest S a forward call may carry (>=1).
- * acc_mode = LNB_ACC_STRICT / LNB_ACC_FAST. */
+ * acc_mode = LNB_ACC_STRICT / LNB_ACC_FAST.
+ * seq_len may be anything up to the model's max_seq_len (the RoPE table; LNB_EINVAL above it).  Sessions
+ * whose seq_len the shared-memory attention kernel cannot hold (17 024 positions at head_dim 128) run every
+ * row on the streamed attention kernels, which need head_dim <= 128 and n_heads / n_kv_heads <= 8.
+ * LNB_ENOMEM when the caches and scratch do not fit the GPU (the message gives the bytes asked for);
+ * nothing stays allocated then. */
 int lnb_session_create(lnb_model* m, int seq_len, int max_rows, int acc_mode, lnb_session** out);
 int lnb_session_destroy(lnb_session* s);
 
@@ -204,7 +209,9 @@ int lnb_forward(lnb_session* s, const int32_t* tokens, int S, int start_pos,
  * dimension, SURVEY F10).  lnb_session_set_active_sequence selects which sequence lnb_forward /
  * lnb_decode_run / lnb_session_read address (e.g. to prefill each prompt); lnb_forward_batch then advances
  * all sequences by one token in ONE pass over the weights: row i = sequence i, token tokens[i] at position
- * positions[i].  Every row gets exactly the arithmetic of its own S=1 Forward. */
+ * positions[i].  Every row gets exactly the arithmetic of its own S=1 Forward.  Any seq_len works: beyond
+ * the shared-memory decode kernel's fit (351 positions at head_dim 128) the batched attention streams the
+ * caches from HBM.  n_seq * seq_len positions of caches must fit the GPU, or creation is LNB_ENOMEM. */
 int lnb_session_create_batch(lnb_model* m, int seq_len, int n_seq, int max_rows, int acc_mode, lnb_session** out);
 int lnb_session_set_active_sequence(lnb_session* s, int seq);
 int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const int32_t* positions, int n,

@@ -18,6 +18,7 @@
 #include "../../include/lnb.h"
 #include "gemm_tc.cuh"
 #include "sdpa_tc.cuh"
+#include "sdpa_stream.cuh"
 #include "gemv.cuh"
 #include "kernels.cuh"
 #include "seqsum.cuh"
@@ -854,6 +855,53 @@ static int smem_opt_in(int bytes) {
   return 0;
 }
 
+// ---- streamed attention (sdpa_stream.cuh) ---------------------------------------------------------------------
+// Scratch of one launch group of `rows` rows over keys [0, t_stride): bf16 scores, FAST chunk row sums and chunk
+// outputs.  The rows of a call are processed in groups of `rows`, so the score scratch stays within kSsScoreBudget
+// however many rows a prompt has.
+static const size_t kSsScoreBudget = (size_t)64 << 20;
+struct SsScratch {
+  uint16_t* sc = nullptr;
+  double* z = nullptr;
+  float* op = nullptr;
+  int rows = 0, t_stride = 0, n_chunks = 0;
+};
+static bool ss_shape_ok(int hd, int n_rep) { return hd % 8 == 0 && hd <= 128 && n_rep >= 1 && n_rep <= 8; }
+// sizes for keys [0, T) and at most max_rows rows per call (bytes per buffer)
+static void ss_plan(SsScratch& x, int T, int max_rows, int n_heads, int hd, size_t* sc_b, size_t* z_b, size_t* op_b) {
+  x.t_stride = (T + SS_VT - 1) / SS_VT * SS_VT;
+  x.n_chunks = (x.t_stride + SS_CH - 1) / SS_CH;
+  const size_t row = (size_t)n_heads * x.t_stride * 2;
+  x.rows = (int)std::max<size_t>(1, std::min<size_t>({kSsScoreBudget / row, (size_t)max_rows, (size_t)65535}));
+  *sc_b = (size_t)x.rows * row;
+  *z_b = (size_t)x.rows * n_heads * x.n_chunks * 8;
+  *op_b = (size_t)x.rows * n_heads * x.n_chunks * hd * 4;
+}
+// STRICT output chains: the d-range of one CTA (more CTAs per KV head; each chain still runs t = 0..p in order)
+static int ss_dsplit(int hd) { return hd % 32 == 0 ? 4 : hd % 16 == 0 ? 2 : 1; }
+// all `rows` rows of P (P.q, P.out, positions and caches set by the caller)
+static int launch_stream_attn(const Launcher& L, StreamAttn P, int rows, int n_kv, const SsScratch& x) {
+  const int dsplit = P.strict ? ss_dsplit(P.hd) : 1;
+  const size_t s_scores = ss_scores_smem(P.hd, P.n_rep), s_out = ss_out_smem(P.hd, P.n_rep, dsplit);
+  // the largest shape ss_shape_ok admits (head_dim 128, n_rep 8, FAST); the kernel's static shared memory comes on top
+  if (int rc = smem_opt_in<ss_out_kernel>((int)ss_out_smem(128, 8, 1))) return rc;
+  P.sc = x.sc; P.zpart = x.z; P.opart = x.op; P.t_stride = x.t_stride; P.n_chunks = x.n_chunks;
+  for (int r0 = 0; r0 < rows; r0 += x.rows) {
+    const int n = std::min(x.rows, rows - r0);
+    P.row0 = r0;
+    int rc;
+    if ((rc = launch_kernel(L, ss_scores_kernel, dim3(n_kv, n, x.n_chunks), dim3(SS_KT), s_scores, P))) return rc;
+    if (P.strict) {
+      if ((rc = launch_kernel(L, ss_zsum_kernel, dim3(P.n_heads, n), dim3(128), 0, P))) return rc;
+      if ((rc = launch_kernel(L, ss_out_kernel, dim3(n_kv * dsplit, n), dim3(P.n_rep * P.hd / dsplit), s_out, P, dsplit))) return rc;
+    } else {
+      if ((rc = launch_kernel(L, ss_out_kernel, dim3(n_kv, n, x.n_chunks), dim3(P.n_rep * P.hd), s_out, P, 1))) return rc;
+      if ((rc = launch_kernel(L, ss_combine_kernel, dim3(P.n_heads, n), dim3(P.hd), 0, P))) return rc;
+    }
+  }
+  return 0;
+}
+
 template <class Cfg, int PRO, int EPI>
 static int launch_gemv_cfg(const Launcher& L, const GemvParams& p) {
   if (int rc = smem_opt_in<gemv_kernel<Cfg, PRO, EPI>>((int)kMaxSmem)) return rc;
@@ -1033,6 +1081,10 @@ struct lnb_session {
   int32_t* d_next_arr = nullptr;  // [n_seq] greedy tokens of the current batched step
   bool sdpa_smem_decode = false;  // the whole K/V history of one KV head fits in shared memory
   size_t sdpa_decode_smem = 0;
+  // streamed attention (sdpa_stream.cuh): every row of the session runs it when sdpa_kernel cannot hold seq_len keys
+  // (stream_attn); batched steps run it when sdpa_decode_kernel cannot.  Scratch for ss.rows rows per launch group.
+  bool stream_attn = false;
+  SsScratch ss{};
   int64_t launches = 0;
   // persistent decode engine (engine.cuh): the phase list of one S=1 step in device memory
   EnginePhase* d_phases = nullptr;
@@ -1096,8 +1148,10 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
   if (seq_len <= 0 || max_rows <= 0) return fail(LNB_EINVAL, "seq_len and max_rows must be positive");
   if (seq_len > m->cis_rows) return fail(LNB_EINVAL, "seq_len %d exceeds the RoPE table (%d rows)", seq_len, m->cis_rows);
   if (acc_mode != LNB_ACC_STRICT && acc_mode != LNB_ACC_FAST) return fail(LNB_EINVAL, "bad acc_mode %d", acc_mode);
-  if ((size_t)seq_len * 12 + (size_t)m->a.head_dim * 4 > 200 * 1024)
-    return fail(LNB_EINVAL, "seq_len %d too long for the decode attention kernel", seq_len);
+  // sdpa_kernel holds a row's seq_len scores in shared memory; beyond that every row of the session streams
+  const bool stream_attn = (size_t)seq_len * 12 + (size_t)m->a.head_dim * 4 > 200 * 1024;
+  if (stream_attn && !ss_shape_ok(m->a.head_dim, m->a.n_heads / m->a.n_kv_heads))
+    return fail(LNB_EINVAL, "seq_len %d needs the streamed attention kernel, which serves head_dim <= 128 and n_rep <= 8", seq_len);
   CU(cudaSetDevice(m->device));
   CU(cudaFuncSetAttribute(sdpa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   CU(cudaFuncSetAttribute(sdpa_prefill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SP_SMEM));
@@ -1118,8 +1172,24 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
       CU(cudaFuncSetAttribute(sdpa_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     }
   }
+  s->stream_attn = stream_attn;
   cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-  auto al = [&](void** p, size_t bytes) { if (e == cudaSuccess) e = cudaMalloc(p, bytes); };
+  // every allocation is counted, so a failure can say how much the session asked for
+  size_t asked = 0, failed_bytes = 0;
+  auto al = [&](void** p, size_t bytes) {
+    asked += bytes;
+    if (e != cudaSuccess) return;
+    e = cudaMalloc(p, bytes);
+    if (e != cudaSuccess) { failed_bytes = bytes; *p = nullptr; }
+  };
+  if (stream_attn || (!s->sdpa_smem_decode && ss_shape_ok(a.head_dim, a.n_heads / a.n_kv_heads))) {
+    // streamed rows: every row of a long session, or the n_seq rows of a batched step
+    size_t sc_b, z_b, op_b;
+    ss_plan(s->ss, seq_len, stream_attn ? max_rows : n_seq, m->q_l / a.head_dim, a.head_dim, &sc_b, &z_b, &op_b);
+    al((void**)&s->ss.sc, sc_b);
+    al((void**)&s->ss.z, z_b);
+    al((void**)&s->ss.op, op_b);
+  }
   al((void**)&s->x, (size_t)max_rows * a.dim * 2);
   al((void**)&s->h1, (size_t)max_rows * a.dim * 2);
   al((void**)&s->q, (size_t)max_rows * m->q_l * 2);
@@ -1157,8 +1227,11 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
   if (e == cudaSuccess) e = cudaEventCreate(&s->ev1);
   if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
   if (e != cudaSuccess) {
+    cudaGetLastError();
     lnb_session_destroy(s);
-    return fail(LNB_ENOMEM, "session allocation failed: %s", cudaGetErrorString(e));
+    cudaGetLastError();
+    return fail(LNB_ENOMEM, "session allocation failed: %zu bytes of device memory asked for (KV cache %zu bytes), %zu-byte allocation: %s",
+                asked, (size_t)2 * a.n_layers * cbytes, failed_bytes, cudaGetErrorString(e));
   }
   *out = s;
   return 0;
@@ -1178,6 +1251,7 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->x_t); cudaFree(s->h1_t); cudaFree(s->qkv_t); cudaFree(s->o_t); cudaFree(s->m_t);
   cudaFree(s->bx); cudaFree(s->bh1); cudaFree(s->bq); cudaFree(s->bo); cudaFree(s->bm); cudaFree(s->bxn); cudaFree(s->d_bphases); cudaFree(s->d_bkeys);
   cudaFree(s->logits); cudaFree(s->logits_full); cudaFree(s->d_tokens); cudaFree(s->st); cudaFree(s->d_tok_out); cudaFree(s->d_pos_arr); cudaFree(s->d_next_arr);
+  cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
   for (auto p : s->ck) cudaFree(p);
   for (auto p : s->cv) cudaFree(p);
   if (s->h_pin) cudaFreeHost(s->h_pin);
@@ -1752,6 +1826,23 @@ static int enqueue_decode_engine(lnb_session* s, int32_t token, int start_pos, i
   return engine_launch(s, n_steps, advance);
 }
 
+// streamed attention of layer l: rows of the call at st->pos + r (batched: sequence r at d_pos_arr[r] on its own cache)
+static StreamAttn stream_params(lnb_session* s, int l, size_t cache_off, bool batch, uint16_t* out, int out_x8) {
+  const lnb_model* m = s->m;
+  const lnb_model_args& a = m->a;
+  StreamAttn P{};
+  P.q = s->q; P.ldq = m->q_l;
+  P.cache_k = s->ck[l] + cache_off; P.cache_v = s->cv[l] + cache_off; P.kv_dim = m->kv_l;
+  P.row_cache_stride = batch ? (long long)s->seq_len * m->kv_l : 0;
+  P.n_rep = a.n_heads / a.n_kv_heads; P.hd = a.head_dim; P.n_heads = m->q_l / a.head_dim;
+  P.pos_arr = batch ? s->d_pos_arr : nullptr;
+  P.pos_ptr = &s->st->pos; P.pos_step = 1;
+  P.out = out; P.ldo = m->q_l; P.out_x8 = out_x8;
+  P.scale = attn_scale_bf16(a.head_dim);
+  P.strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
+  return P;
+}
+
 // Enqueue one LlamaTransformer.Forward (llamatransformer.go:145-180) for S rows on the
 // session stream.  from_state_token: row 0's token is st->next_token (device-driven decode).
 // logits_rows: 0 = none stored, 1 = last row, S = all rows.  advance: decode-loop bookkeeping.
@@ -1765,7 +1856,8 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
   // single-sequence calls work on the cache of the active sequence; a batched step addresses all of them
   const size_t seq_stride = (size_t)s->seq_len * m->kv_l;
   const size_t cache_off = batch ? 0 : (size_t)s->active_seq * seq_stride;
-  if (batch && !s->sdpa_smem_decode) return fail(LNB_EINVAL, "batched decode needs SequenceLength small enough for the shared-memory attention kernel");
+  if (batch && !s->sdpa_smem_decode && !s->ss.sc)
+    return fail(LNB_EINVAL, "batched decode beyond the shared-memory attention kernel needs head_dim <= 128 and n_rep <= 8");
   int rc;
   rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd,
                      (const int32_t*)(from_state_token ? nullptr : s->d_tokens), (const LnbDevState*)s->st, s->x, a.dim);
@@ -1819,6 +1911,8 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
                          (const uint16_t*)s->q, (const uint16_t*)(s->ck[l] + cache_off), (const uint16_t*)(s->cv[l] + cache_off), m->kv_l,
                          n_rep, a.head_dim, s->o, pos_ptr, s->seq_len, mode == LNB_ACC_STRICT ? 1 : 0, scale,
                          (const int32_t*)(batch ? s->d_pos_arr : nullptr), (long long)seq_stride, m->q_l, (const LnbDevState*)s->st);
+    } else if (batch || s->stream_attn) {
+      rc = launch_stream_attn(L, stream_params(s, l, cache_off, batch, s->o, 0), S, m->kv_l / a.head_dim, s->ss);
     } else {
       rc = launch_kernel(L, sdpa_kernel, dim3(m->q_l / a.head_dim, S), dim3(128), sdpa_smem, (const uint16_t*)s->q, m->q_l,
                          (const uint16_t*)(s->ck[l] + cache_off), (const uint16_t*)(s->cv[l] + cache_off), m->kv_l,
@@ -1931,6 +2025,8 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
                               (const uint16_t*)s->q, m->q_l, (const uint16_t*)(s->ck[l] + tc_cache_off),
                               (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l, a.n_heads / a.n_kv_heads, s->o8, m->q_l, pos_ptr, S, scale)))
         return rc;
+    } else if (s->stream_attn) {
+      if ((rc = launch_stream_attn(L, stream_params(s, l, tc_cache_off, false, s->o8, 1), S, m->kv_l / a.head_dim, s->ss))) return rc;
     } else if ((rc = launch_kernel(L, sdpa_kernel, dim3(m->q_l / a.head_dim, S), dim3(128), sdpa_smem, (const uint16_t*)s->q, m->q_l,
                                    (const uint16_t*)(s->ck[l] + tc_cache_off), (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l,
                                    a.n_heads / a.n_kv_heads, a.head_dim, s->o8, m->q_l, pos_ptr, 0, S, 1, 0, scale, 1)))
@@ -2651,13 +2747,37 @@ extern "C" int lnb_op_attention_bf16(const uint16_t* q, const uint16_t* cache_k,
   if (causal_mask < 0 || causal_mask > 2) return fail(LNB_EINVAL, "bad causal_mask %d", causal_mask);
   if (causal_mask == 1 && T != S) return fail(LNB_EINVAL, "causal mask needs T == S (reference mask is [S,S])");
   const size_t smem = (size_t)T * 12 + (size_t)hd * 4;
-  if (smem > 200 * 1024) return fail(LNB_EINVAL, "T %d too long", T);
+  // beyond sdpa_kernel's T limit the op routes as a long session does: FAST prompts of >= 32 rows keep the tiled prompt
+  // kernels (they stream key tiles), every other case runs the streamed kernel
+  const bool fits = smem <= 200 * 1024;
+  const bool tiled = acc_mode == LNB_ACC_FAST && S > 1 && causal_mask && hd == SP_HD && (n_heads * hd) % 128 == 0 && (fits || S >= 32);
+  if (!fits && !tiled && !ss_shape_ok(hd, n_heads / n_kv)) return fail(LNB_EINVAL, "T %d too long", T);
   const size_t qb = (size_t)S * n_heads * hd * 2, cb = (size_t)T * n_kv * hd * 2;
   OPBUF(dq, qb); OPBUF(dk, cb); OPBUF(dv, cb); OPBUF(dout, qb);
   H2D(dq, q, qb); H2D(dk, cache_k, cb); H2D(dv, cache_v, cb);
   CU(cudaFuncSetAttribute(sdpa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   const float f = attn_scale_bf16(hd);
-  if (acc_mode == LNB_ACC_FAST && S > 1 && causal_mask && hd == SP_HD && (n_heads * hd) % 128 == 0) {
+  if (!fits && !tiled) {
+    SsScratch x;
+    size_t sc_b, z_b, op_b;
+    ss_plan(x, T, S, n_heads, hd, &sc_b, &z_b, &op_b);
+    OPBUF(dsc, sc_b); OPBUF(dz, z_b); OPBUF(dop, op_b);
+    x.sc = dsc.as<uint16_t>(); x.z = dz.as<double>(); x.op = dop.as<float>();
+    StreamAttn P{};
+    P.q = dq.as<uint16_t>(); P.ldq = n_heads * hd;
+    P.cache_k = dk.as<uint16_t>(); P.cache_v = dv.as<uint16_t>(); P.kv_dim = n_kv * hd;
+    P.n_rep = n_heads / n_kv; P.hd = hd; P.n_heads = n_heads;
+    P.pos_fixed = causal_mask ? T - S : T - 1; P.pos_step = causal_mask ? 1 : 0;   // query row s at T - S + s
+    P.out = dout.as<uint16_t>(); P.ldo = n_heads * hd;
+    P.scale = f;
+    P.strict = acc_mode == LNB_ACC_STRICT ? 1 : 0;
+    int rc2 = launch_stream_attn(Launcher{nullptr, LAUNCH_PLAIN, nullptr}, P, S, n_kv, x);
+    if (!rc2) rc2 = op_finish();
+    if (rc2) return rc2;
+    D2H(out, dout, qb);
+    return 0;
+  }
+  if (tiled) {
     // the prefill path's tiled two-pass kernel (writes the X8 operand of the Wo GEMM; unpacked here); query row s sits at
     // position (T - S) + s, as in a session's chunked prefill
     const int Mpad = (S + 127) / 128 * 128;
