@@ -3,6 +3,7 @@
 // 8-token prompt and prints the generated token ids and the decode rate.
 // Build: make -C host      Run: host/lnb_generate [seq_len=136] [strict|fast] [tiny | <modelDir>] [batch=N]
 // batch=N: N prompts (SURVEY 8d: prompt b = ids[1:] + 977 b) generated together, one pass over the weights per step.
+// batch=N slots=K: the same N prompts through K live sequences with continuous batching (inference::GenerateTokensContinuous).
 // prompt=TEXT (with <modelDir>/tokenizer.model): TEXT goes through the chat template and the BPE tokenizer, the
 // generated ids come back as text (cmd/main.go's flow without the console UI).
 // <modelDir> holds params.json + consolidated.00.pth (model.LoadModel, src/model/loader.go:18-70);
@@ -100,10 +101,11 @@ int main(int argc, char** argv) {
     model::LlamaTransformer& transformer = *loaded;
     model::Vocabulary vocab;
     if (tiny || transformer.args.vocab_size < 128256) vocab.StopTokenIds = {1000000000};
-    int batch = 0;
+    int batch = 0, slots = 0;
     const char* prompt_text = nullptr;
     for (int i = 1; i < argc; i++) {
       if (!strncmp(argv[i], "batch=", 6)) batch = atoi(argv[i] + 6);
+      if (!strncmp(argv[i], "slots=", 6)) slots = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "prompt=", 7)) prompt_text = argv[i] + 7;
     }
     std::unique_ptr<model::Tokenizer> tokenizer;
@@ -123,8 +125,9 @@ int main(int argc, char** argv) {
         for (size_t j = 1; j < prompt.size(); j++) prompts[b][j] = (prompt[j] + 977 * b) % mod;
       std::vector<std::vector<int32_t>> outs(batch);
       auto b0 = std::chrono::steady_clock::now();
-      inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts,
-                                     [&](int seq, inference::GenerationState, int32_t tok) { outs[seq].push_back(tok); });
+      auto collect = [&](int seq, inference::GenerationState, int32_t tok) { outs[seq].push_back(tok); };
+      if (slots > 0) inference::GenerateTokensContinuous(transformer, vocab, seq_len, acc, prompts, slots, std::max(slots, 64), collect);
+      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect);
       const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - b0).count();
       size_t total = 0;
       for (int b = 0; b < batch; b++) {

@@ -281,12 +281,13 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
  public:
   int SequenceLength;
   InferenceContext(LlamaTransformer& t, int sequenceLength, int accMode = LNB_ACC_STRICT, int maxRows = 8)
-      : SequenceLength(sequenceLength > 0 ? sequenceLength : t.args.max_seq_len), vocab_(t.args.vocab_size) {
+      : SequenceLength(sequenceLength > 0 ? sequenceLength : t.args.max_seq_len), vocab_(t.args.vocab_size), maxRows_(maxRows) {
     check(lnb_session_create(t.handle(), SequenceLength, maxRows, accMode, &h_));
   }
   // n reference InferenceContexts that share the weights (batched decode): own KV cache and position each
   InferenceContext(LlamaTransformer& t, int sequenceLength, int accMode, int maxRows, int nSeq)
-      : SequenceLength(sequenceLength > 0 ? sequenceLength : t.args.max_seq_len), vocab_(t.args.vocab_size) {
+      : SequenceLength(sequenceLength > 0 ? sequenceLength : t.args.max_seq_len), vocab_(t.args.vocab_size),
+        maxRows_(std::max(maxRows, nSeq)) {
     check(lnb_session_create_batch(t.handle(), SequenceLength, nSeq, maxRows, accMode, &h_));
   }
   ~InferenceContext() { lnb_session_destroy(h_); }
@@ -303,6 +304,21 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
     check(lnb_forward_batch(h_, tokens.data(), positions.data(), (int)tokens.size(), nullptr, next.data()));
     return next;
   }
+  // EXTENSION (continuous batching, lnb_forward_ragged): ONE forward over segments of different sequences, each with the
+  // arithmetic of its own Forward -> greedy token of each segment's last row
+  struct Segment { int seq, startPos; std::vector<int32_t> tokens; };
+  std::vector<int32_t> ForwardRagged(const std::vector<Segment>& segs) {
+    std::vector<int32_t> seq, start, len, flat, next(segs.size(), -1);
+    for (const Segment& s : segs) {
+      seq.push_back(s.seq);
+      start.push_back(s.startPos);
+      len.push_back((int32_t)s.tokens.size());
+      flat.insert(flat.end(), s.tokens.begin(), s.tokens.end());
+    }
+    check(lnb_forward_ragged(h_, (int)segs.size(), seq.data(), start.data(), len.data(), flat.data(), nullptr, next.data()));
+    return next;
+  }
+  int MaxRows() const { return maxRows_; }
   InferenceContext(const InferenceContext&) = delete;
   // LlamaTransformer.Forward (llamatransformer.go:145-180): tokens [S] -> f32 logits [S, vocab]
   ml::Tensor Forward(const ml::Tensor& inputTokens, int startPos) {
@@ -344,6 +360,7 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
  private:
   lnb_session* h_ = nullptr;
   int vocab_;
+  int maxRows_;
 };
 }  // namespace model
 
@@ -415,6 +432,80 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
     const std::vector<int32_t> next = infContext.ForwardBatch(cur, pos);
     for (int i = 0; i < n; i++)
       if (!done[i]) record(i, next[i], pos[i] + 1);
+  }
+}
+
+// Continuous batching (EXTENSION, lnb_forward_ragged): any number of prompts through at most `slots` live sequences, the
+// scheduler of the Python mirror's GenerateTokensContinuous.  Every step is ONE forward: each decoding sequence gets its
+// row, the rest of the stepTokens-row budget goes to prompt chunks first in first out, a prompt whose last chunk is in the
+// step emits its first token, a finished slot takes the next waiting prompt at position 0; steps without prompt rows run
+// lnb_forward_batch.  emit(prompt index, state, token); per prompt the stream is GenerateTokens' own.
+inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength,
+                                     int accMode, const std::vector<std::vector<int32_t>>& prompts, int slots, int stepTokens,
+                                     const std::function<void(int, GenerationState, int32_t)>& emit) {
+  if (slots < 1 || slots > 8) throw Error("slots must be in [1, 8]");
+  if (stepTokens < slots) throw Error("stepTokens must be at least slots (every decoding sequence gets a row)");
+  model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, stepTokens), slots);
+  const int seqLen = infContext.SequenceLength, budget = std::min(stepTokens, infContext.MaxRows());
+  for (const auto& p : prompts)
+    if (p.empty() || (int)p.size() >= seqLen)
+      throw Error("context SequenceLength " + std::to_string(seqLen) + " must be higher than prompt tokens length " + std::to_string(p.size()) +
+                  " (and prompts must not be empty)");
+  struct Slot { int i = -1, fed = 0, order = 0; int32_t cur = -1; int pos = 0; bool decoding = false; };
+  std::vector<Slot> slot((size_t)slots);
+  size_t next_prompt = 0;
+  int admitted = 0, live = 0;
+  while (next_prompt < prompts.size() || live > 0) {
+    for (Slot& s : slot)
+      if (s.i < 0 && next_prompt < prompts.size()) { s = Slot(); s.i = (int)next_prompt++; s.order = admitted++; live++; }
+    std::vector<int> decoding, prefilling;
+    for (int k = 0; k < slots; k++)
+      if (slot[k].i >= 0) (slot[k].decoding ? decoding : prefilling).push_back(k);
+    std::sort(prefilling.begin(), prefilling.end(), [&](int a, int b) { return slot[a].order < slot[b].order; });
+    std::vector<model::InferenceContext::Segment> segs;
+    std::vector<int> seg_slot;
+    for (int k : decoding) { segs.push_back({k, slot[k].pos, {slot[k].cur}}); seg_slot.push_back(k); }
+    int left = budget - (int)decoding.size();
+    for (int k : prefilling) {
+      if (left <= 0) break;
+      const std::vector<int32_t>& p = prompts[(size_t)slot[k].i];
+      const int n = std::min(left, (int)p.size() - slot[k].fed);
+      segs.push_back({k, slot[k].fed, std::vector<int32_t>(p.begin() + slot[k].fed, p.begin() + slot[k].fed + n)});
+      seg_slot.push_back(k);
+      left -= n;
+    }
+    std::vector<int32_t> out((size_t)slots, -1);
+    if (prefilling.empty()) {   // decode rows only: one batch-engine launch, row k = slot k (free slots: token 0 at 0)
+      const int n = decoding.back() + 1;
+      std::vector<int32_t> toks((size_t)n, 0), poss((size_t)n, 0);
+      for (int k : decoding) { toks[(size_t)k] = slot[k].cur; poss[(size_t)k] = slot[k].pos; }
+      const std::vector<int32_t> next = infContext.ForwardBatch(toks, poss);
+      for (int k : decoding) out[(size_t)k] = next[(size_t)k];
+    } else {
+      const std::vector<int32_t> next = infContext.ForwardRagged(segs);
+      for (size_t j = 0; j < segs.size(); j++) out[(size_t)seg_slot[j]] = next[j];
+    }
+    for (size_t j = 0; j < segs.size(); j++) {
+      Slot& s = slot[(size_t)seg_slot[j]];
+      int curPos;
+      if (!s.decoding) {
+        s.fed += (int)segs[j].tokens.size();
+        if (s.fed < (int)prompts[(size_t)s.i].size()) continue;
+        curPos = s.fed;
+        s.decoding = true;
+      } else {
+        curPos = s.pos + 1;
+      }
+      const int32_t tok = out[(size_t)seg_slot[j]];
+      s.cur = tok;
+      s.pos = curPos;
+      bool eos = false;
+      for (int32_t st : vocab.StopTokenIds) eos |= (st == tok);
+      const GenerationState state = eos ? GSFinishedByReachingEOS : (curPos + 1 == seqLen ? GSFinishedByReachingSeqLen : GSInProgress);
+      const int i = s.i;
+      if (state != GSInProgress) { s.i = -1; live--; }
+      emit(i, state, tok);
+    }
   }
 }
 }  // namespace inference

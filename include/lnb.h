@@ -235,6 +235,25 @@ int lnb_session_logits_argmax(lnb_session* s, int64_t generation, int row0, int 
  * bit-identical caches and logits in LNB_ACC_STRICT. */
 int lnb_session_set_chunked_prefill(lnb_session* s, int on);
 
+/* EXTENSION (continuous batching): one forward over n_segs segments; segment i = len[i] tokens of sequence seq[i] at
+ * positions start_pos[i] .. start_pos[i]+len[i]-1, rows laid out segment after segment in `tokens`.  Each segment gets the
+ * arithmetic of its own Forward on its own InferenceContext (llamatransformer.go:145-180) under the [S,T] mask (row s sees
+ * keys t <= start_pos + s; at start_pos 0 this is the reference's mask, :128-136), so prompts, prompt chunks and decode rows
+ * of different sequences share one pass over the weights.
+ *   valid: any session (single or batch); 1 <= n_segs <= n_seq; seq[] distinct, in [0, n_seq); len[i] >= 1,
+ *   sum(len) <= max_rows; 0 <= start_pos[i], start_pos[i] + len[i] <= seq_len; token ids in range.  Anything else, and
+ *   tp_size > 1 (not built), is LNB_EINVAL with nothing enqueued.  No lnb_session_set_chunked_prefill needed.
+ *   logits: NULL or host [n_segs, vocab] f32, the LAST row of each segment; argmax_out: NULL or [n_segs], the greedy token
+ *   of that row (inference.go:207-216).
+ * Every ragged row's attention runs on the streamed kernels (csrc/sdpa_stream.cuh); LNB_ACC_FAST calls of >= 32 rows run
+ * the projections on the tensor cores (one pass over the weights), all others the GEMV chain (one pass per 8 rows).
+ * LNB_ACC_STRICT: every segment is bit-identical to its own Forward.  The first call allocates the row map and, if needed,
+ * stream-attention scratch (LNB_ENOMEM with the bytes on failure; the session stays usable).  Afterwards a
+ * lnb_forward_device handle is stale, the active sequence and a captured decode graph are unchanged, and
+ * lnb_session_read(LNB_BUF_RESIDUAL) returns the call's [sum(len), dim] rows. */
+int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq, const int32_t* start_pos, const int32_t* len,
+                       const int32_t* tokens, float* logits, int32_t* argmax_out);
+
 /* Device-resident greedy decode: runs n_steps consecutive S=1 forwards starting with
  * `first_token` at position start_pos, feeding each argmax back on the device (no host
  * sync inside), optionally as CUDA-graph replays.  tokens_out[n_steps]; ms_out = device

@@ -65,6 +65,7 @@ SIGNATURES = {
     "lnb_session_engine_profile": (C.c_int, [vp, C.POINTER(C.c_double)]),
     "lnb_session_decode_engine": (C.c_int, [vp]),
     "lnb_session_set_chunked_prefill": (C.c_int, [vp, C.c_int]),
+    "lnb_forward_ragged": (C.c_int, [vp, C.c_int, i32p, i32p, i32p, i32p, f32p, i32p]),
     "lnb_session_read": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64]),
     "lnb_session_set_layer_limit": (C.c_int, [vp, C.c_int]),
     "lnb_session_launch_count": (C.c_int64, [vp]),

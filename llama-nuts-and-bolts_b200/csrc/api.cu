@@ -909,16 +909,19 @@ static int launch_gemv_cfg(const Launcher& L, const GemvParams& p) {
                        Cfg::smem_bytes(p.K), p);
 }
 
-// picks the row-block size: largest MB in {8,2,1} that is useful for M and whose smem fits
+// picks the row-block size: largest MB in {8,2,1} that is useful for M and whose smem fits.  mb_rows > 0 chooses it for
+// that many rows instead of M_total (ragged calls pass 8: the block size, and with it a row's FAST summation order, then
+// depends on K alone, not on how many rows share the call)
 template <int PRO, int EPI>
-static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total) {
+static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total, int mb_rows = 0) {
   if (p.N % 16 || p.K % 8) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 16 and K %d of 8", p.N, p.K);  // 16: panel pairs
   if ((EPI == EPI_QKV_ROPE || EPI == EPI_SWIGLU) && p.N % 32) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 32", p.N);
   const bool strict = (mode == LNB_ACC_STRICT);
   p.strict_norm = strict ? 1 : 0;
+  const int mb_for = mb_rows > 0 ? mb_rows : M_total;
   int mb = 1;
-  if (M_total >= 3 && (strict ? CfgS8::smem_bytes(p.K) : CfgF8::smem_bytes(p.K)) <= kMaxSmem) mb = 8;
-  else if (M_total >= 2 && (strict ? CfgS2::smem_bytes(p.K) : CfgF2::smem_bytes(p.K)) <= kMaxSmem) mb = 2;
+  if (mb_for >= 3 && (strict ? CfgS8::smem_bytes(p.K) : CfgF8::smem_bytes(p.K)) <= kMaxSmem) mb = 8;
+  else if (mb_for >= 2 && (strict ? CfgS2::smem_bytes(p.K) : CfgF2::smem_bytes(p.K)) <= kMaxSmem) mb = 2;
   if ((strict ? CfgS1::smem_bytes(p.K) : CfgF1::smem_bytes(p.K)) > kMaxSmem)
     return fail(LNB_EINVAL, "gemv: K %d too large for shared memory", p.K);
   const uint16_t* x0 = p.x;
@@ -1085,6 +1088,10 @@ struct lnb_session {
   // (stream_attn); batched steps run it when sdpa_decode_kernel cannot.  Scratch for ss.rows rows per launch group.
   bool stream_attn = false;
   SsScratch ss{};
+  // ragged calls (lnb_forward_ragged), allocated by the first one: [tokens | row_seq | row_pos | last row of each segment]
+  // of one call, max_rows * 3 + 8 words on the device and in pinned staging (ONE host-to-device copy per call)
+  int32_t* d_rag = nullptr;
+  int32_t* h_rag = nullptr;
   int64_t launches = 0;
   // persistent decode engine (engine.cuh): the phase list of one S=1 step in device memory
   EnginePhase* d_phases = nullptr;
@@ -1252,6 +1259,8 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->bx); cudaFree(s->bh1); cudaFree(s->bq); cudaFree(s->bo); cudaFree(s->bm); cudaFree(s->bxn); cudaFree(s->d_bphases); cudaFree(s->d_bkeys);
   cudaFree(s->logits); cudaFree(s->logits_full); cudaFree(s->d_tokens); cudaFree(s->st); cudaFree(s->d_tok_out); cudaFree(s->d_pos_arr); cudaFree(s->d_next_arr);
   cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
+  cudaFree(s->d_rag);
+  if (s->h_rag) cudaFreeHost(s->h_rag);
   for (auto p : s->ck) cudaFree(p);
   for (auto p : s->cv) cudaFree(p);
   if (s->h_pin) cudaFreeHost(s->h_pin);
@@ -1826,16 +1835,26 @@ static int enqueue_decode_engine(lnb_session* s, int32_t token, int start_pos, i
   return engine_launch(s, n_steps, advance);
 }
 
-// streamed attention of layer l: rows of the call at st->pos + r (batched: sequence r at d_pos_arr[r] on its own cache)
-static StreamAttn stream_params(lnb_session* s, int l, size_t cache_off, bool batch, uint16_t* out, int out_x8) {
+// Row map of a ragged call (lnb_forward_ragged), device pointers: row r holds token tokens[r] of sequence seq[r] at position
+// pos[r]; segment i's last row is last[i].  Rows of one segment are consecutive.
+struct RowMap {
+  const int32_t *tokens, *seq, *pos, *last;
+  int n_segs;
+};
+
+// streamed attention of layer l: rows of the call at st->pos + r (batched: sequence r at d_pos_arr[r] on its own cache;
+// ragged: sequence rm->seq[r] at rm->pos[r])
+static StreamAttn stream_params(lnb_session* s, int l, size_t cache_off, bool batch, uint16_t* out, int out_x8,
+                                const RowMap* rm = nullptr) {
   const lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   StreamAttn P{};
   P.q = s->q; P.ldq = m->q_l;
   P.cache_k = s->ck[l] + cache_off; P.cache_v = s->cv[l] + cache_off; P.kv_dim = m->kv_l;
-  P.row_cache_stride = batch ? (long long)s->seq_len * m->kv_l : 0;
+  P.row_cache_stride = (batch || rm) ? (long long)s->seq_len * m->kv_l : 0;
+  P.row_seq = rm ? rm->seq : nullptr;
   P.n_rep = a.n_heads / a.n_kv_heads; P.hd = a.head_dim; P.n_heads = m->q_l / a.head_dim;
-  P.pos_arr = batch ? s->d_pos_arr : nullptr;
+  P.pos_arr = rm ? rm->pos : batch ? s->d_pos_arr : nullptr;
   P.pos_ptr = &s->st->pos; P.pos_step = 1;
   P.out = out; P.ldo = m->q_l; P.out_x8 = out_x8;
   P.scale = attn_scale_bf16(a.head_dim);
@@ -1843,24 +1862,46 @@ static StreamAttn stream_params(lnb_session* s, int l, size_t cache_off, bool ba
   return P;
 }
 
+// LM head of a ragged call: the last row of each segment is compacted into h1 (dead after the last layer), ONE EPI_LOGITS
+// GEMV runs over those n_segs rows, then one greedy argmax per row into d_next_arr, as in a batched decode step
+static int ragged_head(const Launcher& L, lnb_session* s, const RowMap& rm) {
+  lnb_model* m = s->m;
+  const lnb_model_args& a = m->a;
+  const bool strict = (s->mode == LNB_ACC_STRICT);
+  int rc;
+  if ((rc = launch_kernel(L, gather_rows_kernel, dim3(rm.n_segs), dim3(256), 0, (const uint16_t*)s->x, rm.last, (const LnbDevState*)s->st,
+                          s->h1, a.dim)))
+    return rc;
+  if (strict && (rc = launch_rms_scale(L, s->h1, a.dim, s->rs, rm.n_segs, a.dim, a.norm_eps))) return rc;
+  GemvParams p{};
+  p.rscale = strict ? s->rs : nullptr;
+  p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
+  p.out_f32 = s->logits; p.ldo = m->vocab_l; p.st = nullptr; p.argmax_row = -1;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, rm.n_segs, 8))) return rc;
+  return launch_kernel(L, argmax_f32_kernel, dim3(rm.n_segs), dim3(256), 0, (const float*)s->logits, a.vocab_size, s->d_next_arr);
+}
+
 // Enqueue one LlamaTransformer.Forward (llamatransformer.go:145-180) for S rows on the
 // session stream.  from_state_token: row 0's token is st->next_token (device-driven decode).
 // logits_rows: 0 = none stored, 1 = last row, S = all rows.  advance: decode-loop bookkeeping.
+// rm: a ragged call -- rows of several sequences at their own positions (tokens, positions and caches from the row map,
+// attention on the streamed kernels, the LM head of ragged_head; logits_rows, advance and batch are unused).
 static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int logits_rows, bool advance, bool batch = false,
-                           bool gather = true) {
+                           bool gather = true, const RowMap* rm = nullptr) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
   const int mode = s->mode;
   const int32_t* pos_ptr = &s->st->pos;
-  // single-sequence calls work on the cache of the active sequence; a batched step addresses all of them
+  // single-sequence calls work on the cache of the active sequence; a batched step or a ragged call addresses all of them
   const size_t seq_stride = (size_t)s->seq_len * m->kv_l;
-  const size_t cache_off = batch ? 0 : (size_t)s->active_seq * seq_stride;
+  const size_t cache_off = (batch || rm) ? 0 : (size_t)s->active_seq * seq_stride;
+  const int mb_rows = rm ? 8 : 0;
   if (batch && !s->sdpa_smem_decode && !s->ss.sc)
     return fail(LNB_EINVAL, "batched decode beyond the shared-memory attention kernel needs head_dim <= 128 and n_rep <= 8");
   int rc;
   rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd,
-                     (const int32_t*)(from_state_token ? nullptr : s->d_tokens), (const LnbDevState*)s->st, s->x, a.dim);
+                     (const int32_t*)(rm ? rm->tokens : from_state_token ? nullptr : s->d_tokens), (const LnbDevState*)s->st, s->x, a.dim);
   if (rc) return rc;
   const int n_layers = active_layers(s);
   const float scale = attn_scale_bf16(a.head_dim);
@@ -1876,7 +1917,7 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
     p.W = W; p.N = a.dim; p.K = K; p.x = x; p.ldx = K; p.ldo = a.dim;
     if (m->tp_size == 1) {
       p.out_bf16 = out; p.res = res;
-      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S);
+      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S, mb_rows);
     }
     int rc2;
     if (s->p2p_ready) {
@@ -1903,9 +1944,12 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
       p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
       p.cache_k = s->ck[l] + cache_off; p.cache_v = s->cv[l] + cache_off; p.cis = m->cis; p.pos_ptr = pos_ptr;
       if (batch) { p.pos_arr = s->d_pos_arr; p.cache_seq_stride = (long long)seq_stride; }
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, S))) return rc;
+      if (rm) { p.pos_arr = rm->pos; p.row_seq = rm->seq; p.cache_seq_stride = (long long)seq_stride; }
+      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, S, mb_rows))) return rc;
     }
-    if ((S == 1 || batch) && s->sdpa_smem_decode) {
+    if (rm) {   // one attention path for every ragged row, whatever the session's other calls use
+      rc = launch_stream_attn(L, stream_params(s, l, 0, false, s->o, 0, rm), S, m->kv_l / a.head_dim, s->ss);
+    } else if ((S == 1 || batch) && s->sdpa_smem_decode) {
       const int n_rep = a.n_heads / a.n_kv_heads;
       rc = launch_kernel(L, sdpa_decode_kernel, dim3(m->kv_l / a.head_dim, batch ? S : 1), dim3(128 * n_rep), s->sdpa_decode_smem,
                          (const uint16_t*)s->q, (const uint16_t*)(s->ck[l] + cache_off), (const uint16_t*)(s->cv[l] + cache_off), m->kv_l,
@@ -1927,11 +1971,13 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
       p.rscale = strict ? s->rs : nullptr;
       p.W = W.w13; p.N = 2 * m->ffn_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm; p.eps = a.norm_eps;
       p.out_bf16 = s->mbuf; p.ldo = m->ffn_l; p.silu_tab = m->silu_tab;
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, S))) return rc;
+      if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, S, mb_rows))) return rc;
     }
     if ((rc = proj_resid(W.w2, m->ffn_l, s->mbuf, s->h1, s->x))) return rc;        // w2 + residual (:619, :248)
   }
-  {  // output_norm -> output -> f32 logits (+ greedy argmax of the last row)   (:166-175; inference.go:207-216)
+  if (rm) {
+    if ((rc = ragged_head(L, s, *rm))) return rc;
+  } else {  // output_norm -> output -> f32 logits (+ greedy argmax of the last row)   (:166-175; inference.go:207-216)
     const int rows = (logits_rows > 1) ? S : 1;  // rows of the head actually computed
     const int row0 = S - rows;
     if ((rc = strict_scale(s->x + (size_t)row0 * a.dim, rows))) return rc;
@@ -1971,16 +2017,19 @@ static bool forward_tc_ok(const lnb_session* s, int S) {
   return s->mode == LNB_ACC_FAST && s->xn8 && S >= 32 && (m->q_l + 2 * m->kv_l) % TC_BN == 0 && a.dim % TC_BN == 0 &&
          (2 * m->ffn_l) % TC_BN == 0 && a.dim % TC_KT == 0 && m->q_l % TC_KT == 0 && m->ffn_l % TC_KT == 0;
 }
-static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gather = true) {
+// rm: a ragged call (see enqueue_forward): projections stay on the tensor cores, RoPE / KV append follow the row map, and
+// attention runs on the streamed kernels
+static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gather = true, const RowMap* rm = nullptr) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
   const int32_t* pos_ptr = &s->st->pos;
   const int Mpad = (S + TC_BM - 1) / TC_BM * TC_BM;
   const int qkv_n = m->q_l + 2 * m->kv_l;
-  const size_t tc_cache_off = (size_t)s->active_seq * s->seq_len * m->kv_l;
+  const size_t seq_stride = (size_t)s->seq_len * m->kv_l;
+  const size_t tc_cache_off = rm ? 0 : (size_t)s->active_seq * seq_stride;
   int rc;
-  if ((rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd, (const int32_t*)s->d_tokens,
+  if ((rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd, (const int32_t*)(rm ? rm->tokens : s->d_tokens),
                           (const LnbDevState*)s->st, s->x, a.dim)))
     return rc;
   const int n_layers = active_layers(s);
@@ -2012,9 +2061,12 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
       if ((rc = launch_gemm_tc<TC_EPI_BF16>(L, g))) return rc;
     }
     if ((rc = launch_kernel(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
-                            a.head_dim, s->ck[l] + tc_cache_off, s->cv[l] + tc_cache_off, (const float*)m->cis, pos_ptr, S)))
+                            a.head_dim, s->ck[l] + tc_cache_off, s->cv[l] + tc_cache_off, (const float*)m->cis, pos_ptr, S,
+                            (const int32_t*)(rm ? rm->pos : nullptr), (const int32_t*)(rm ? rm->seq : nullptr), (long long)seq_stride)))
       return rc;
-    if (a.head_dim == SP_HD && exp_tab) {
+    if (rm) {
+      if ((rc = launch_stream_attn(L, stream_params(s, l, 0, false, s->o8, 1, rm), S, m->kv_l / a.head_dim, s->ss))) return rc;
+    } else if (a.head_dim == SP_HD && exp_tab) {
       if ((rc = launch_kernel(L, sdpa_tc_kernel, dim3(m->q_l / a.head_dim, (S + 127) / 128), dim3(256), (size_t)ST_SMEM,
                               (const uint16_t*)s->q, m->q_l, (const uint16_t*)(s->ck[l] + tc_cache_off),
                               (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l, a.n_heads / a.n_kv_heads, s->o8, m->q_l, pos_ptr, S, scale,
@@ -2045,6 +2097,11 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
   }
   // LM head: all rows on the tensor cores when asked for (and the vocabulary shard tiles), then the
   // last row through the GEMV, which also owns the greedy argmax (identical to the decode path)
+  if (rm) {
+    if ((rc = ragged_head(L, s, *rm))) return rc;
+    s->last_rows = S;
+    return 0;
+  }
   if (logits_rows > 1 && m->vocab_l % TC_BN == 0) {
     if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->x, a.dim, (const uint16_t*)m->norm, s->xn8, S,
                             a.dim, a.norm_eps)))
@@ -2291,6 +2348,102 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
   if ((rc = sync_stream(s))) return rc;
   if ((rc = p2p_err_check(s))) return rc;
   if (argmax_out) memcpy(argmax_out, npin, (size_t)n * 4);
+  return 0;
+}
+
+// ---- ragged calls (continuous batching): segments of several sequences at their own positions in ONE forward ----------
+// Buffers of the first ragged call: the row map (device + pinned staging) and, when the session has none or a smaller one,
+// stream-attention scratch for max_rows rows per launch group.  Nothing is replaced unless every allocation succeeded, so a
+// failure (LNB_ENOMEM) leaves the session as it was.
+static int ragged_alloc(lnb_session* s) {
+  lnb_model* m = s->m;
+  const lnb_model_args& a = m->a;
+  const size_t words = (size_t)s->max_rows * 3 + 16;   // + 8 segment last rows + 8 greedy tokens (host side)
+  SsScratch x{};
+  size_t sc_b, z_b, op_b;
+  ss_plan(x, s->seq_len, s->max_rows, m->q_l / a.head_dim, a.head_dim, &sc_b, &z_b, &op_b);
+  const bool need_ss = !s->ss.sc || s->ss.rows < x.rows;
+  if (s->d_rag && !need_ss) return 0;
+  const size_t asked = (s->d_rag ? 0 : words * 4) + (need_ss ? sc_b + z_b + op_b : 0);
+  int32_t* d_rag = nullptr;
+  int32_t* h_rag = nullptr;
+  cudaError_t e = cudaSuccess;
+  if (!s->d_rag) {
+    e = cudaMalloc((void**)&d_rag, words * 4);
+    if (e == cudaSuccess) e = cudaMallocHost((void**)&h_rag, words * 4);
+  }
+  if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.sc, sc_b);
+  if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.z, z_b);
+  if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.op, op_b);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(d_rag); cudaFreeHost(h_rag); cudaFree(x.sc); cudaFree(x.z); cudaFree(x.op);
+    cudaGetLastError();
+    return fail(LNB_ENOMEM, "ragged-call buffers: %zu bytes of device memory asked for (stream-attention scratch for %d rows: %zu): %s", asked,
+                x.rows, need_ss ? sc_b + z_b + op_b : (size_t)0, cudaGetErrorString(e));
+  }
+  if (!s->d_rag) { s->d_rag = d_rag; s->h_rag = h_rag; }
+  if (need_ss) {
+    CU(cudaStreamSynchronize(s->stream));   // batched steps may still read the old scratch
+    cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
+    s->ss = x;
+  }
+  return 0;
+}
+
+extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq, const int32_t* start_pos, const int32_t* len,
+                                  const int32_t* tokens, float* logits, int32_t* argmax_out) {
+  if (!s || !seq || !start_pos || !len || !tokens) return fail(LNB_EINVAL, "NULL argument");
+  lnb_model* m = s->m;
+  const lnb_model_args& a = m->a;
+  if (m->tp_size > 1) return fail(LNB_EINVAL, "lnb_forward_ragged is not built for tensor parallelism (tp_size %d)", m->tp_size);
+  if (!ss_shape_ok(a.head_dim, a.n_heads / a.n_kv_heads))
+    return fail(LNB_EINVAL, "ragged calls run the streamed attention kernels, which serve head_dim <= 128 and n_rep <= 8");
+  if (n_segs < 1 || n_segs > s->n_seq) return fail(LNB_EINVAL, "n_segs %d must be in [1, %d] (the session's sequences)", n_segs, s->n_seq);
+  bool used[8] = {false, false, false, false, false, false, false, false};
+  int64_t rows64 = 0;
+  for (int i = 0; i < n_segs; i++) {
+    if (seq[i] < 0 || seq[i] >= s->n_seq) return fail(LNB_EINVAL, "segment %d: sequence %d out of range (session has %d)", i, seq[i], s->n_seq);
+    if (used[seq[i]]) return fail(LNB_EINVAL, "segment %d: sequence %d has a segment already (one per sequence per call)", i, seq[i]);
+    used[seq[i]] = true;
+    if (len[i] < 1) return fail(LNB_EINVAL, "segment %d: len %d must be >= 1", i, len[i]);
+    if (start_pos[i] < 0 || (int64_t)start_pos[i] + len[i] > s->seq_len)
+      return fail(LNB_EINVAL, "segment %d: positions [%d, %lld) exceed SequenceLength %d", i, start_pos[i], (long long)start_pos[i] + len[i],
+                  s->seq_len);
+    rows64 += len[i];
+  }
+  if (rows64 > s->max_rows) return fail(LNB_EINVAL, "the segments carry %lld rows, more than the session's max_rows %d", (long long)rows64, s->max_rows);
+  const int rows = (int)rows64;
+  for (int r = 0; r < rows; r++)
+    if (tokens[r] < 0 || tokens[r] >= a.vocab_size) return fail(LNB_EINVAL, "token id %d (row %d) out of range", tokens[r], r);
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(m->device));
+  int rc;
+  if ((rc = ragged_alloc(s))) return rc;
+  if ((rc = ensure_logits(s, (size_t)n_segs))) return rc;
+  s->kept_rows = 0;   // a logits handle is valid until the session's next forward
+  // [tokens | row_seq | row_pos | last row of each segment]: one pinned staging copy
+  int32_t* h = s->h_rag;
+  memcpy(h, tokens, (size_t)rows * 4);
+  for (int i = 0, r = 0; i < n_segs; i++) {
+    for (int k = 0; k < len[i]; k++, r++) {
+      h[rows + r] = seq[i];
+      h[2 * rows + r] = start_pos[i] + k;
+    }
+    h[3 * rows + i] = r - 1;
+  }
+  CU(cudaMemcpyAsync(s->d_rag, h, (size_t)(3 * rows + n_segs) * 4, cudaMemcpyHostToDevice, s->stream));
+  const RowMap rm{s->d_rag, s->d_rag + rows, s->d_rag + 2 * rows, s->d_rag + 3 * rows, n_segs};
+  // FAST prompts of >= 32 rows: one pass over the weights on the tensor cores; everything else: the GEMV chain
+  rc = (s->mode == LNB_ACC_FAST && forward_tc_ok(s, rows)) ? enqueue_forward_tc(s, rows, 0, false, &rm)
+                                                          : enqueue_forward(s, rows, false, 0, false, false, false, &rm);
+  if (rc) return rc;
+  s->last_was_engine = false;
+  if (logits) CU(cudaMemcpyAsync(logits, s->logits, (size_t)n_segs * a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
+  int32_t* npin = s->h_rag + (size_t)s->max_rows * 3 + 8;
+  if (argmax_out) CU(cudaMemcpyAsync(npin, s->d_next_arr, (size_t)n_segs * 4, cudaMemcpyDeviceToHost, s->stream));
+  if ((rc = sync_stream(s))) return rc;
+  if (argmax_out) memcpy(argmax_out, npin, (size_t)n_segs * 4);
   return 0;
 }
 

@@ -232,19 +232,22 @@ __global__ void __launch_bounds__(256) rmsnorm_x8_kernel(const uint16_t* __restr
 
 // After the fused wq|wk|wv GEMM of the prefill path: RoPE on q and k (f64 intermediates, see
 // gemv.cuh EPI_QKV_ROPE), q -> q_out [S, q_dim], k -> cacheK[pos0+s], v -> cacheV[pos0+s]
-// (llamatransformer.go:374-403).  One thread per (row, pair of columns).
+// (llamatransformer.go:374-403).  One thread per (row, pair of columns).  Ragged calls (rows of several sequences):
+// row s sits at row_pos[s] of the cache of sequence row_seq[s] (+ row_seq[s] * seq_stride); both NULL otherwise.
 __global__ void rope_kv_kernel(const uint16_t* __restrict__ qkv, int ld, uint16_t* __restrict__ q_out, int q_dim, int kv_dim,
                                int head_dim, uint16_t* __restrict__ cache_k, uint16_t* __restrict__ cache_v,
-                               const float* __restrict__ cis, const int32_t* __restrict__ pos_ptr, int S) {
+                               const float* __restrict__ cis, const int32_t* __restrict__ pos_ptr, int S,
+                               const int32_t* __restrict__ row_pos, const int32_t* __restrict__ row_seq, long long seq_stride) {
   pdl_launch_dependents();
   pdl_wait();
   const int pairs = (q_dim + 2 * kv_dim) / 2;
   const int64_t total = (int64_t)S * pairs;
-  const int pos0 = *pos_ptr;
+  const int pos0 = row_pos ? 0 : *pos_ptr;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int s = (int)(i / pairs), n = (int)(i % pairs) * 2;
     const uint32_t w = *reinterpret_cast<const uint32_t*>(qkv + (size_t)s * ld + n);
-    const int pos = pos0 + s;
+    const int pos = row_pos ? row_pos[s] : pos0 + s;
+    const size_t cb = row_seq ? (size_t)row_seq[s] * (size_t)seq_stride : 0;
     if (n < q_dim + kv_dim) {
       const int nn = (n < q_dim) ? n : n - q_dim;
       const int ii = (nn % head_dim) >> 1;
@@ -252,9 +255,9 @@ __global__ void rope_kv_kernel(const uint16_t* __restrict__ qkv, int ld, uint16_
       const double a = (double)bf_lo(w), b = (double)bf_hi(w), c = (double)fc.x, d = (double)fc.y;
       const uint32_t o = (uint32_t)f2bf((float)(a * c - b * d)) | ((uint32_t)f2bf((float)(a * d + b * c)) << 16);
       if (n < q_dim) *reinterpret_cast<uint32_t*>(q_out + (size_t)s * q_dim + n) = o;
-      else *reinterpret_cast<uint32_t*>(cache_k + (size_t)pos * kv_dim + nn) = o;
+      else *reinterpret_cast<uint32_t*>(cache_k + cb + (size_t)pos * kv_dim + nn) = o;
     } else {
-      *reinterpret_cast<uint32_t*>(cache_v + (size_t)pos * kv_dim + (n - q_dim - kv_dim)) = w;
+      *reinterpret_cast<uint32_t*>(cache_v + cb + (size_t)pos * kv_dim + (n - q_dim - kv_dim)) = w;
     }
   }
 }

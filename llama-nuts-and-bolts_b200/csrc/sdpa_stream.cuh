@@ -3,7 +3,8 @@
 // fit, and lnb_op_attention_bf16 beyond sdpa_kernel's T limit.
 //
 // One description covers every caller: query row r (global index r of the call) has its own cache base
-// (cache + r * row_cache_stride: batched decode) and its own position p_r (pos_arr[r], or base + pos_step * r: S = 1
+// (cache + r * row_cache_stride: batched decode; cache + row_seq[r] * row_cache_stride: ragged calls, where rows of one
+// sequence follow each other) and its own position p_r (pos_arr[r], or base + pos_step * r: S = 1
 // decode, a prompt or chunked prefill under the [S,T] mask, or pos_step = 0 for the op's unmasked form) and sees keys
 // 0..p_r.  The arithmetic is sdpa_kernel's (llamatransformer.go:459-514):
 //   sc_t = t( t(sum_seq_d q_d k_td) / t(sqrt(hd)) );  e_t = exp_f64(sc_t);  p_t = t(f32(e_t / Z));  o_d = t(sum_t p_t v_td)
@@ -38,6 +39,7 @@ struct StreamAttn {
   const uint16_t* cache_v;
   int kv_dim;
   long long row_cache_stride;   // elements between the caches of consecutive rows (batched decode), else 0
+  const int32_t* row_seq;       // ragged calls: row r reads the cache of sequence row_seq[r] (+ row_seq[r] * row_cache_stride)
   int n_rep, hd, n_heads;       // n_heads: query heads of this rank
   const int32_t* pos_arr;       // per-row positions, or NULL:
   const int32_t* pos_ptr;       //   p_r = (pos_ptr ? *pos_ptr : pos_fixed) + pos_step * r
@@ -57,6 +59,9 @@ struct StreamAttn {
 LNB_DEVINL int ss_keys(const StreamAttn& P, int r) {   // keys row r sees (call only after pdl_wait)
   const int p = P.pos_arr ? __ldcg(P.pos_arr + r) : (P.pos_ptr ? __ldcg(P.pos_ptr) : P.pos_fixed) + P.pos_step * r;
   return p + 1;
+}
+LNB_DEVINL size_t ss_cache_base(const StreamAttn& P, int r) {   // (call only after pdl_wait)
+  return (size_t)(P.row_seq ? __ldcg(P.row_seq + r) : r) * (size_t)P.row_cache_stride;
 }
 LNB_DEVINL uint16_t* ss_score_row(const StreamAttn& P, int rl, int H) {
   return P.sc + ((size_t)rl * P.n_heads + H) * (size_t)P.t_stride;
@@ -89,7 +94,7 @@ __global__ void __launch_bounds__(SS_KT) ss_scores_kernel(const StreamAttn P) {
   const int hd = P.hd, n_rep = P.n_rep, ks = hd + 8, cpr = hd / 8;
   uint16_t* sK = reinterpret_cast<uint16_t*>(sm);                     // [SS_KT][hd + 8]
   float* sQ = reinterpret_cast<float*>(sK + (size_t)SS_KT * ks);      // [n_rep][hd]
-  const uint16_t* kb = P.cache_k + (size_t)r * P.row_cache_stride + (size_t)h * hd;
+  const uint16_t* kb = P.cache_k + ss_cache_base(P, r) + (size_t)h * hd;
   for (int i = tid; i < n_rep * hd; i += SS_KT) sQ[i] = bf2f(P.q[(size_t)r * P.ldq + (size_t)h * n_rep * hd + i]);
   double z[8];
 #pragma unroll
@@ -218,7 +223,7 @@ __global__ void __launch_bounds__(1024) ss_out_kernel(const StreamAttn P, int ds
     for (int k = 0; k < nch; k++) z = __dadd_rn(z, zp[k]);
     sZ[tid] = z;
   }
-  const uint16_t* vb = P.cache_v + (size_t)r * P.row_cache_stride + (size_t)h * P.hd + (size_t)g * dw;
+  const uint16_t* vb = P.cache_v + ss_cache_base(P, r) + (size_t)h * P.hd + (size_t)g * dw;
   auto issue = [&](int k0, int stage) {
     const int n = min(SS_VT, t1 - k0);
     uint16_t* v = sV + (size_t)stage * SS_VT * dw;

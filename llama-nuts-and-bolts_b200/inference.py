@@ -5,6 +5,7 @@ the Go original; each iteration is one call through the C-ABI.
 """
 from __future__ import annotations
 
+import collections
 import time
 
 import numpy as np
@@ -12,6 +13,14 @@ import numpy as np
 from . import ml, model as model_mod
 
 GSInProgress, GSFinishedByReachingEOS, GSFinishedByReachingSeqLen = 0, 1, 2
+
+# Row budget of one GenerateTokensContinuous step.  FAST ragged steps of >= 32 rows run on the tensor cores (one pass over
+# the weights); steps of 9..31 rows run the GEMV chain, which streams the weights once per 8 rows (up to 4 passes), and
+# STRICT steps always do.  64 leaves 56 prompt rows beside 8 decode rows, so a step that admits prompt tokens is normally
+# above the 32-row cliff.  tools/continuous_bench.py (8B, 32 prompts of 8..512 tokens, SequenceLength 1024, 8 slots, FAST,
+# H100 80GB HBM3 at 700 W) measured 460 / 462 / 469 tokens/s at step_tokens 32 / 64 / 256: within run-to-run spread, so the
+# budget was chosen from the cliff above, and kept small so that a long prompt delays decoding sequences by short steps.
+DEFAULT_STEP_TOKENS = 64
 
 
 class InferenceEngine:
@@ -144,6 +153,98 @@ class InferenceEngine:
                 yield GSInProgress, nextTokenId
         finally:
             infContext.close()
+
+    def GenerateTokensContinuous(self, prompts, slots: int = 8, step_tokens: int | None = None,
+                                 step_times: list | None = None):
+        """Continuous batching (EXTENSION, lnb_forward_ragged): any number of prompts through at most `slots` live
+        sequences.  Every step is ONE forward whose rows may belong to different sequences: each decoding sequence gets
+        its one row, the rest of the step's row budget (min(step_tokens, max_rows)) goes to prompt chunks, first in first
+        out; a prompt whose last chunk is in the step emits its first token from that step; a finished sequence's slot
+        is refilled at position 0 by the next waiting prompt.  Steps without prompt rows run lnb_forward_batch (the
+        batch engine: one launch per step).  Yields (prompt index, state, token id); per prompt the stream is exactly
+        what GenerateTokens(prompts[i]) yields (the bookkeeping of generateTokensInternal, inference.go:173-254)."""
+        if step_tokens is None:
+            step_tokens = DEFAULT_STEP_TOKENS
+        if not 1 <= slots <= 8:
+            raise ml.MlError(f"slots {slots} must be in [1, 8]")
+        if step_tokens < slots:
+            raise ml.MlError(f"step_tokens {step_tokens} must be at least slots {slots} (every decoding sequence gets a row)")
+        prompts = [[int(t) for t in p] for p in prompts]
+        infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
+                                                max_rows=max(self.max_rows, step_tokens), acc_mode=self.acc_mode, n_seq=slots)
+        if self.context_hook is not None:
+            self.context_hook(infContext)
+        try:
+            yield from self._generate_continuous(infContext, prompts, slots, min(step_tokens, infContext.max_rows), step_times)
+        finally:
+            infContext.close()
+
+    def _generate_continuous(self, infContext, prompts, slots: int, budget: int, step_times: list | None = None):
+        """the scheduler of GenerateTokensContinuous on a given context (anything with SequenceLength, forward_ragged and
+        forward_batch)"""
+        seqLen = infContext.SequenceLength
+        stop = self.model.Vocabulary.StopTokenIds
+        for p in prompts:
+            if len(p) >= seqLen:  # :176-179
+                raise ml.MlError(f"context SequenceLength {seqLen} must be higher than prompt tokens length {len(p)}")
+            if len(p) < 1:
+                raise ml.MlError("empty prompt")
+        waiting = collections.deque(range(len(prompts)))
+        # per slot: prompt index, prompt tokens already in the cache, token fed next and its position (cur None: prefilling),
+        # admission number (first in, first out among the prefilling slots)
+        slot: list[dict | None] = [None] * slots
+        admitted = 0
+        while waiting or any(sl is not None for sl in slot):
+            for k in range(slots):
+                if slot[k] is None and waiting:
+                    slot[k] = dict(i=waiting.popleft(), fed=0, cur=None, pos=0, order=admitted)
+                    admitted += 1
+            decoding = [k for k in range(slots) if slot[k] is not None and slot[k]["cur"] is not None]
+            prefilling = sorted((k for k in range(slots) if slot[k] is not None and slot[k]["cur"] is None),
+                                key=lambda k: slot[k]["order"])
+            segs = [(k, slot[k]["pos"], [slot[k]["cur"]]) for k in decoding]
+            left = budget - len(decoding)
+            for k in prefilling:
+                if left <= 0:
+                    break
+                sl = slot[k]
+                n = min(left, len(prompts[sl["i"]]) - sl["fed"])
+                segs.append((k, sl["fed"], prompts[sl["i"]][sl["fed"]:sl["fed"] + n]))
+                left -= n
+            t0 = time.perf_counter()
+            if not prefilling:
+                # decode rows only: one batch-engine launch; row k = slot k (free slots below the last decoding one are
+                # fed token 0 at position 0 of their own cache -- they hold no sequence, and a refill overwrites it)
+                n = max(decoding) + 1
+                toks = [slot[k]["cur"] if slot[k] is not None else 0 for k in range(n)]
+                poss = [slot[k]["pos"] if slot[k] is not None else 0 for k in range(n)]
+                nxt, _ = infContext.forward_batch(toks, poss)
+                out = {k: int(nxt[k]) for k in decoding}
+            else:
+                nxt, _ = infContext.forward_ragged(segs)
+                out = {k: int(nxt[j]) for j, (k, _, _) in enumerate(segs)}
+            if step_times is not None:
+                step_times.append(time.perf_counter() - t0)
+            for k, _, chunk in segs:
+                sl = slot[k]
+                if sl["cur"] is None:
+                    sl["fed"] += len(chunk)
+                    if sl["fed"] < len(prompts[sl["i"]]):
+                        continue
+                    curPos = sl["fed"]                    # first generated token (:194-216)
+                else:
+                    curPos = sl["pos"] + 1
+                tok = out[k]
+                sl["cur"], sl["pos"] = tok, curPos
+                if tok in stop:
+                    state = GSFinishedByReachingEOS
+                elif curPos + 1 == seqLen:
+                    state = GSFinishedByReachingSeqLen
+                else:
+                    state = GSInProgress
+                if state != GSInProgress:
+                    slot[k] = None
+                yield sl["i"], state, tok
 
     def GenerateTokensBatch(self, prompts, step_times: list | None = None):
         """The consumer `InferenceEngine.TokenizeBatch` (src/inference/tokenize.go:97-107) never got in the

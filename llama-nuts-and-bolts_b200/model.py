@@ -200,6 +200,23 @@ class InferenceContext:
                                     ptr(logits, _capi.f32p) if want_logits else None, ptr(nxt, _capi.i32p)))
         return nxt, logits
 
+    def forward_ragged(self, segments, want_logits: bool = False):
+        """EXTENSION (continuous batching, lnb_forward_ragged): ONE forward over segments (seq, start_pos, tokens) of
+        different sequences -- prompts, prompt chunks and decode rows -- each with the arithmetic of its own Forward.
+        Returns (greedy token of each segment's last row [n_segs], logits [n_segs, vocab] of those rows or None)."""
+        n = len(segments)
+        seq = np.array([s for s, _, _ in segments], np.int32)
+        start = np.array([p for _, p, _ in segments], np.int32)
+        toks = [np.asarray(t, np.int32).reshape(-1) for _, _, t in segments]
+        lens = np.array([len(t) for t in toks], np.int32)
+        flat = np.ascontiguousarray(np.concatenate(toks) if toks else np.zeros(0, np.int32), np.int32)
+        nxt = np.empty(n, np.int32)
+        logits = np.empty((n, self.transformer.args.VocabSize), np.float32) if want_logits else None
+        check(lib.lnb_forward_ragged(self.h, n, ptr(seq, _capi.i32p), ptr(start, _capi.i32p), ptr(lens, _capi.i32p),
+                                     ptr(flat, _capi.i32p), ptr(logits, _capi.f32p) if want_logits else None,
+                                     ptr(nxt, _capi.i32p)))
+        return nxt, logits
+
     def allow_chunked_prefill(self, on: bool = True):
         """EXTENSION (not in the reference): accept S > 1 at startPos > 0 with the [S,T] causal mask"""
         check(lib.lnb_session_set_chunked_prefill(self.h, int(on)))
