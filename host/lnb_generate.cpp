@@ -4,6 +4,8 @@
 // Build: make -C host      Run: host/lnb_generate [seq_len=136] [strict|fast] [tiny | <modelDir>] [batch=N]
 // batch=N: N prompts (SURVEY 8d: prompt b = ids[1:] + 977 b) generated together, one pass over the weights per step.
 // batch=N slots=K: the same N prompts through K live sequences with continuous batching (inference::GenerateTokensContinuous).
+// temp=T [top_k=K] [top_p=P] [seed=S]: seeded sampling instead of the greedy argmax (lnb_session_set_sampling); prompt b of a
+// batch samples with seed S + b.
 // prompt=TEXT (with <modelDir>/tokenizer.model): TEXT goes through the chat template and the BPE tokenizer, the
 // generated ids come back as text (cmd/main.go's flow without the console UI).
 // <modelDir> holds params.json + consolidated.00.pth (model.LoadModel, src/model/loader.go:18-70);
@@ -103,10 +105,15 @@ int main(int argc, char** argv) {
     if (tiny || transformer.args.vocab_size < 128256) vocab.StopTokenIds = {1000000000};
     int batch = 0, slots = 0;
     const char* prompt_text = nullptr;
+    model::SamplingArgs sampling;   // temp= top_k= top_p= seed= (temp 0, the default: greedy)
     for (int i = 1; i < argc; i++) {
       if (!strncmp(argv[i], "batch=", 6)) batch = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "slots=", 6)) slots = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "prompt=", 7)) prompt_text = argv[i] + 7;
+      if (!strncmp(argv[i], "temp=", 5)) sampling.Temperature = (float)atof(argv[i] + 5);
+      if (!strncmp(argv[i], "top_k=", 6)) sampling.TopK = atoi(argv[i] + 6);
+      if (!strncmp(argv[i], "top_p=", 6)) sampling.TopP = (float)atof(argv[i] + 6);
+      if (!strncmp(argv[i], "seed=", 5)) sampling.Seed = strtoull(argv[i] + 5, nullptr, 10);
     }
     std::unique_ptr<model::Tokenizer> tokenizer;
     if (prompt_text) {
@@ -126,8 +133,8 @@ int main(int argc, char** argv) {
       std::vector<std::vector<int32_t>> outs(batch);
       auto b0 = std::chrono::steady_clock::now();
       auto collect = [&](int seq, inference::GenerationState, int32_t tok) { outs[seq].push_back(tok); };
-      if (slots > 0) inference::GenerateTokensContinuous(transformer, vocab, seq_len, acc, prompts, slots, std::max(slots, 64), collect);
-      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect);
+      if (slots > 0) inference::GenerateTokensContinuous(transformer, vocab, seq_len, acc, prompts, slots, std::max(slots, 64), collect, &sampling);
+      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling);
       const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - b0).count();
       size_t total = 0;
       for (int b = 0; b < batch; b++) {
@@ -145,7 +152,7 @@ int main(int argc, char** argv) {
     inference::GenerateTokens(transformer, vocab, seq_len, acc, prompt, [&](inference::GenerationState, int32_t tok) {
       if (out.empty()) t_first = std::chrono::steady_clock::now();
       out.push_back(tok);
-    });
+    }, &sampling);
     auto t1 = std::chrono::steady_clock::now();
     if (tokenizer) printf("text: %s\n", tokenizer->TokenBatchToString(out).c_str());
     printf("tokens:");

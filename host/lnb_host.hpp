@@ -277,6 +277,18 @@ inline std::unique_ptr<LlamaTransformer> LoadModel(const std::string& modelDir, 
   return t;
 }
 
+// EXTENSION (the reference only has the greedy ml.Argmax): seeded sampling of the next token (lnb_session_set_sampling).
+// Temperature 0 is greedy; TopK 0 is the whole vocabulary; TopP in (0, 1].
+struct SamplingArgs {
+  float Temperature = 0.0f;
+  int32_t TopK = 0;
+  float TopP = 1.0f;
+  uint64_t Seed = 0;
+  bool Samples() const { return Temperature != 0.0f; }
+  // prompt i of a batch or continuous run samples with Seed + i (its stream is GenerateTokens' with that seed)
+  SamplingArgs ForPrompt(int i) const { SamplingArgs a = *this; a.Seed += (uint64_t)i; return a; }
+};
+
 class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
  public:
   int SequenceLength;
@@ -292,6 +304,12 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
   }
   ~InferenceContext() { lnb_session_destroy(h_); }
   void SetActiveSequence(int seq) { check(lnb_session_set_active_sequence(h_, seq)); }
+  // sequence seq samples its next tokens with *a (nullptr or Temperature 0: greedy); the token outputs below then carry them
+  void SetSampling(int seq, const SamplingArgs* a) {
+    if (!a || !a->Samples()) { check(lnb_session_set_sampling(h_, seq, nullptr)); return; }
+    const lnb_sampling p{a->Temperature, a->TopK, a->TopP, a->Seed};
+    check(lnb_session_set_sampling(h_, seq, &p));
+  }
   // Forward + last-row ml.Argmax in one call (inference.go:202-216), 4-byte read-back
   int32_t ForwardArgmax(const std::vector<int32_t>& tokens, int startPos) {
     int32_t next = -1;
@@ -369,9 +387,12 @@ enum GenerationState { GSInProgress = 0, GSFinishedByReachingEOS = 1, GSFinished
 
 // generateTokensInternal (inference.go:173-254); `emit` plays generatedTokensCh
 inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
-                           const std::vector<int32_t>& promptTokens, const std::function<void(GenerationState, int32_t)>& emit) {
+                           const std::vector<int32_t>& promptTokens, const std::function<void(GenerationState, int32_t)>& emit,
+                           const model::SamplingArgs* sampling = nullptr) {
   // the prefill call carries the whole prompt: size the session's row buffers for it
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max<int>(8, (int)promptTokens.size()));
+  const bool samples = sampling && sampling->Samples();
+  if (samples) infContext.SetSampling(0, sampling);   // the sampled token instead of Slice + ml.Argmax
   const int promptLength = (int)promptTokens.size();
   if (promptLength >= infContext.SequenceLength)
     throw Error("context SequenceLength " + std::to_string(infContext.SequenceLength) + " must be higher than prompt tokens length " +
@@ -380,13 +401,18 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
   std::copy(promptTokens.begin(), promptTokens.end(), tokens.begin());
   int prevPos = 0;
   for (int curPos = promptLength; curPos < infContext.SequenceLength; curPos++) {  // :194
-    ml::Tensor slice({curPos - prevPos}, ml::DataType::INT32);                     // tokens.Slice([prevPos],[curPos]) :195
-    std::memcpy(slice.RawData.data(), tokens.data() + prevPos, (size_t)(curPos - prevPos) * 4);
-    ml::Tensor logits = infContext.Forward(slice, prevPos);                        // :202
-    const int rows = logits.Size[0], V = logits.Size[1];
-    ml::Tensor last({1, V}, ml::DataType::F32);                                    // logits.Slice(last row) :207
-    std::memcpy(last.RawData.data(), logits.data<float>() + (size_t)(rows - 1) * V, (size_t)V * 4);
-    int32_t nextTokenId = ml::Argmax(last).data<int32_t>()[0];                     // :211
+    int32_t nextTokenId;
+    if (samples) {
+      nextTokenId = infContext.ForwardArgmax(std::vector<int32_t>(tokens.begin() + prevPos, tokens.begin() + curPos), prevPos);
+    } else {
+      ml::Tensor slice({curPos - prevPos}, ml::DataType::INT32);                   // tokens.Slice([prevPos],[curPos]) :195
+      std::memcpy(slice.RawData.data(), tokens.data() + prevPos, (size_t)(curPos - prevPos) * 4);
+      ml::Tensor logits = infContext.Forward(slice, prevPos);                      // :202
+      const int rows = logits.Size[0], V = logits.Size[1];
+      ml::Tensor last({1, V}, ml::DataType::F32);                                  // logits.Slice(last row) :207
+      std::memcpy(last.RawData.data(), logits.data<float>() + (size_t)(rows - 1) * V, (size_t)V * 4);
+      nextTokenId = ml::Argmax(last).data<int32_t>()[0];                           // :211
+    }
     if (tokens[curPos] != vocab.PadId) nextTokenId = tokens[curPos];               // :218-226
     tokens[curPos] = nextTokenId;
     bool eos = false;
@@ -403,10 +429,16 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
 // sequences advance together, one pass over the weights per step.  emit(sequence, state, token).
 inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                                 const std::vector<std::vector<int32_t>>& prompts,
-                                const std::function<void(int, GenerationState, int32_t)>& emit) {
+                                const std::function<void(int, GenerationState, int32_t)>& emit,
+                                const model::SamplingArgs* sampling = nullptr) {
   const int n = (int)prompts.size();
   if (n < 1) throw Error("empty prompt batch");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, n), n);
+  if (sampling && sampling->Samples())
+    for (int i = 0; i < n; i++) {
+      const model::SamplingArgs a = sampling->ForPrompt(i);
+      infContext.SetSampling(i, &a);
+    }
   const int seqLen = infContext.SequenceLength;
   for (const auto& p : prompts)
     if ((int)p.size() >= seqLen)
@@ -442,7 +474,8 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
 // lnb_forward_batch.  emit(prompt index, state, token); per prompt the stream is GenerateTokens' own.
 inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength,
                                      int accMode, const std::vector<std::vector<int32_t>>& prompts, int slots, int stepTokens,
-                                     const std::function<void(int, GenerationState, int32_t)>& emit) {
+                                     const std::function<void(int, GenerationState, int32_t)>& emit,
+                                     const model::SamplingArgs* sampling = nullptr) {
   if (slots < 1 || slots > 8) throw Error("slots must be in [1, 8]");
   if (stepTokens < slots) throw Error("stepTokens must be at least slots (every decoding sequence gets a row)");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, stepTokens), slots);
@@ -457,7 +490,13 @@ inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const
   int admitted = 0, live = 0;
   while (next_prompt < prompts.size() || live > 0) {
     for (Slot& s : slot)
-      if (s.i < 0 && next_prompt < prompts.size()) { s = Slot(); s.i = (int)next_prompt++; s.order = admitted++; live++; }
+      if (s.i < 0 && next_prompt < prompts.size()) {
+        s = Slot(); s.i = (int)next_prompt++; s.order = admitted++; live++;
+        if (sampling && sampling->Samples()) {   // before the prompt's first segment
+          const model::SamplingArgs a = sampling->ForPrompt(s.i);
+          infContext.SetSampling((int)(&s - slot.data()), &a);
+        }
+      }
     std::vector<int> decoding, prefilling;
     for (int k = 0; k < slots; k++)
       if (slot[k].i >= 0) (slot[k].decoding ? decoding : prefilling).push_back(k);

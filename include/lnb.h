@@ -199,7 +199,8 @@ int lnb_session_destroy(lnb_session* s);
  * ml.Argmax of the generate loop (src/inference/inference.go:207-216).
  *   tokens[S] int32, start_pos as in the reference (S>1 requires start_pos==0, F11).
  *   logits : NULL, or host [S, vocab] f32 if all_rows, host [1, vocab] (last row) otherwise
- *   argmax_last : NULL, or receives the greedy token of the last row.
+ *   argmax_last : NULL, or receives the next token of the last row (greedy unless the sequence samples,
+ *                 lnb_session_set_sampling).
  * One call = one H2D of tokens, the whole forward on the device, one D2H of what was asked. */
 int lnb_forward(lnb_session* s, const int32_t* tokens, int S, int start_pos,
                 float* logits, int all_rows, int32_t* argmax_last);
@@ -215,7 +216,8 @@ int lnb_forward(lnb_session* s, const int32_t* tokens, int S, int start_pos,
 int lnb_session_create_batch(lnb_model* m, int seq_len, int n_seq, int max_rows, int acc_mode, lnb_session** out);
 int lnb_session_set_active_sequence(lnb_session* s, int seq);
 int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const int32_t* positions, int n,
-                      float* logits /* NULL or [n, vocab] */, int32_t* argmax_out /* [n] */);
+                      float* logits /* NULL or [n, vocab] */,
+                      int32_t* argmax_out /* [n]: next token (greedy unless the sequence samples) */);
 
 /* LlamaTransformer.Forward whose result stays in HBM: the host mirror returns an ml.Tensor that carries a handle
  * (session, generation) instead of S x vocab floats, Tensor.Slice keeps the handle, and ml.Argmax on it runs on the
@@ -224,7 +226,9 @@ int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const int32_t* posi
  * rows_kept: 1 (last row) or S.  A handle is valid until the session's next forward (LNB_ESTATE afterwards).
  * Tensor-parallel: logits_read / logits_argmax are collectives (every rank makes the same call). */
 int lnb_forward_device(lnb_session* s, const int32_t* tokens, int S, int start_pos, int rows_kept,
-                       int32_t* argmax_last /* may be NULL */, int64_t* generation_out);
+                       int32_t* argmax_last /* may be NULL; next token (greedy unless the sequence samples) */,
+                       int64_t* generation_out);
+/* lnb_session_logits_argmax is the greedy ml.Argmax of every row, sampled forward or not */
 int lnb_session_logits_read(lnb_session* s, int64_t generation, int row0, int rows, float* host /* [rows, vocab] */);
 int lnb_session_logits_argmax(lnb_session* s, int64_t generation, int row0, int rows, int32_t* out /* [rows] */);
 
@@ -243,8 +247,8 @@ int lnb_session_set_chunked_prefill(lnb_session* s, int on);
  *   valid: any session (single or batch); 1 <= n_segs <= n_seq; seq[] distinct, in [0, n_seq); len[i] >= 1,
  *   sum(len) <= max_rows; 0 <= start_pos[i], start_pos[i] + len[i] <= seq_len; token ids in range.  Anything else, and
  *   tp_size > 1 (not built), is LNB_EINVAL with nothing enqueued.  No lnb_session_set_chunked_prefill needed.
- *   logits: NULL or host [n_segs, vocab] f32, the LAST row of each segment; argmax_out: NULL or [n_segs], the greedy token
- *   of that row (inference.go:207-216).
+ *   logits: NULL or host [n_segs, vocab] f32, the LAST row of each segment; argmax_out: NULL or [n_segs], the next token
+ *   of that row (greedy unless the sequence samples; greedy is inference.go:207-216).
  * Every ragged row's attention runs on the streamed kernels (csrc/sdpa_stream.cuh); LNB_ACC_FAST calls of >= 32 rows run
  * the projections on the tensor cores (one pass over the weights), all others the GEMV chain (one pass per 8 rows).
  * LNB_ACC_STRICT: every segment is bit-identical to its own Forward.  The first call allocates the row map and, if needed,
@@ -258,9 +262,33 @@ int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq, const int
  * `first_token` at position start_pos, feeding each argmax back on the device (no host
  * sync inside), optionally as CUDA-graph replays.  tokens_out[n_steps]; ms_out = device
  * time of the n_steps steps measured with CUDA events on the session stream.
- * This is the timed region of bench.py's `value`. */
+ * This is the timed region of bench.py's `value`.  tokens_out: next token of each step (greedy unless the active sequence
+ * samples; a sampled sequence decodes on the kernel chain with the sampler after each step, and lnb_last_error() says so
+ * on a session whose S=1 steps otherwise run the persistent engine). */
 int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos, int n_steps, int use_graph,
                    int32_t* tokens_out, float* ms_out);
+
+/* EXTENSION (the reference's generate loop only has the greedy ml.Argmax, inference.go:207-216): seeded temperature,
+ * top-k and top-p sampling, computed on the device (csrc/sample.cuh) with integer-exact arithmetic (DESIGN.md §9b).
+ * For one row of logits l: the rank order is (l descending, index ascending); the candidates are the top_k first ranks
+ * (0 or >= vocab: all); each gets the integer weight floor(2^40 exp(z)), z = f32(f32(l - max) / temperature), 0 for
+ * z < -28; top_p keeps the shortest rank prefix of the candidates with at least ceil(top_p * their mass); the token is
+ * drawn with 64 bits of splitmix64(seed, p_next), p_next = the position the token will occupy.  The draw depends only on
+ * (row, parameters, p_next): a sequence's sampled stream does not depend on how it was batched, chunked or scheduled. */
+typedef struct {
+  float temperature;   /* 0: greedy; else finite, > 0 */
+  int32_t top_k;       /* >= 0; 0: the whole vocabulary */
+  float top_p;         /* (0, 1]; 1: no top-p cut */
+  uint64_t seed;
+} lnb_sampling;
+/* Sequence `seq` of the session samples with *p from its next forward on; NULL or temperature 0: greedy (the default).
+ * Every token output of the session's forwards for that sequence then carries the sampled token (lnb_forward /
+ * lnb_forward_device argmax_last, lnb_forward_batch argmax_out, lnb_forward_ragged argmax_out, lnb_decode_run
+ * tokens_out).  LNB_EINVAL with nothing changed: seq outside [0, n_seq), temperature not finite or < 0, top_k < 0,
+ * top_p outside (0, 1], tp_size > 1 (not built).  The first sampler set allocates n_seq parameter slots and the weights
+ * of n_seq rows (LNB_ENOMEM with the bytes; the session stays as it was).  Setting parameters does not synchronise the
+ * stream or invalidate a captured decode graph; switching the active sequence between greedy and sampled re-captures it. */
+int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampling* p);
 
 /* Fused collective for tensor-parallel decode: instead of ncclAllReduce after Wo / w2, every rank's GEMV
  * epilogue stores its fp32 partials straight into all peers' memory over NVLink and a small kernel
@@ -335,6 +363,9 @@ int lnb_op_mul_bf16(const uint16_t* a, const uint16_t* b, uint16_t* out, int64_t
 /* ml.Softmax on f32 rows (operations_impl.go:478-511), ml.Argmax (:513-548) */
 int lnb_op_softmax_f32(const float* x, float* out, int rows, int cols);
 int lnb_op_argmax_f32(const float* x, int rows, int cols, int32_t* out);
+/* EXTENSION: the sampler of lnb_session_set_sampling alone on host rows (1..8 rows): logits[rows, vocab], parameters
+ * p[rows], pos_next[rows] (the p_next of each draw) -> out[rows]; temperature 0 gives the greedy ml.Argmax (:513-548) */
+int lnb_op_sample_f32(const float* logits, int rows, int vocab, const lnb_sampling* p, const int32_t* pos_next, int32_t* out);
 /* ml.Fwd_Get_Rows (operations_impl.go:142-173) */
 int lnb_op_get_rows_bf16(const uint16_t* emb, const int32_t* tokens, uint16_t* out, int S, int vocab, int dim);
 

@@ -25,6 +25,10 @@ class ModelArgsC(C.Structure):
     ]
 
 
+class SamplingC(C.Structure):   # lnb_sampling
+    _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("seed", C.c_uint64)]
+
+
 u16p = C.POINTER(C.c_uint16)
 f32p = C.POINTER(C.c_float)
 i32p = C.POINTER(C.c_int32)
@@ -66,6 +70,7 @@ SIGNATURES = {
     "lnb_session_decode_engine": (C.c_int, [vp]),
     "lnb_session_set_chunked_prefill": (C.c_int, [vp, C.c_int]),
     "lnb_forward_ragged": (C.c_int, [vp, C.c_int, i32p, i32p, i32p, i32p, f32p, i32p]),
+    "lnb_session_set_sampling": (C.c_int, [vp, C.c_int, C.POINTER(SamplingC)]),
     "lnb_session_read": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64]),
     "lnb_session_set_layer_limit": (C.c_int, [vp, C.c_int]),
     "lnb_session_launch_count": (C.c_int64, [vp]),
@@ -105,6 +110,7 @@ SIGNATURES = {
     "lnb_op_mul_bf16": (C.c_int, [u16p, u16p, u16p, C.c_int64]),
     "lnb_op_softmax_f32": (C.c_int, [f32p, f32p, C.c_int, C.c_int]),
     "lnb_op_argmax_f32": (C.c_int, [f32p, C.c_int, C.c_int, i32p]),
+    "lnb_op_sample_f32": (C.c_int, [f32p, C.c_int, C.c_int, C.POINTER(SamplingC), i32p, i32p]),
     "lnb_op_get_rows_bf16": (C.c_int, [u16p, i32p, u16p, C.c_int, C.c_int, C.c_int]),
 }
 

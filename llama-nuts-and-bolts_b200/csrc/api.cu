@@ -24,6 +24,7 @@
 #include "seqsum.cuh"
 #include "engine.cuh"
 #include "engine_batch.cuh"
+#include "sample.cuh"
 #include "pth.hpp"
 #include "tokenizer.hpp"
 
@@ -1122,6 +1123,16 @@ struct lnb_session {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::mutex mu;
   int last_rows = 0;
+  // seeded sampling (sample.cuh, lnb_session_set_sampling), allocated by the first sampler set: the parameters of each
+  // sequence in device memory (a captured graph reads them there), the weights of up to n_seq rows, the sampled token of
+  // a single-sequence forward (st->next_token keeps the greedy one)
+  lnb_sampling* d_samp = nullptr;           // [n_seq]
+  unsigned long long* d_samp_w = nullptr;   // [n_seq][vocab]
+  unsigned long long* d_samp_cand = nullptr;   // [n_seq][SMP_MERGE] split-sampler candidates, then [n_seq] u32 counters
+  int32_t* d_samp_tok = nullptr;
+  bool samp_on[8] = {false, false, false, false, false, false, false, false};
+  bool graph_sampled = false;               // the captured decode graph ends in the sampler ...
+  const float* graph_logits = nullptr;      // ... which reads this logits buffer
 };
 
 static int set_state(lnb_session* s, int pos, int n_rows, int next_token, bool reset_step) {
@@ -1260,6 +1271,7 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->logits); cudaFree(s->logits_full); cudaFree(s->d_tokens); cudaFree(s->st); cudaFree(s->d_tok_out); cudaFree(s->d_pos_arr); cudaFree(s->d_next_arr);
   cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
   cudaFree(s->d_rag);
+  cudaFree(s->d_samp); cudaFree(s->d_samp_w); cudaFree(s->d_samp_tok); cudaFree(s->d_samp_cand);
   if (s->h_rag) cudaFreeHost(s->h_rag);
   for (auto p : s->ck) cudaFree(p);
   for (auto p : s->cv) cudaFree(p);
@@ -2132,11 +2144,35 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
   return 0;
 }
 
+// ---- seeded sampling (sample.cuh, DESIGN.md §9b) ----------------------------------------------------------------
+// both sampler kernels; each row is served by the one its parameters select (on the device: they may change between replays)
+static int launch_sample_job(const Launcher& L, const SampleJob& J) {
+  int rc = launch_kernel(L, sample_split_kernel, dim3((J.V + SMP_SLICE - 1) / SMP_SLICE, J.n), dim3(SMP_THREADS), 0, J);
+  if (rc) return rc;
+  return launch_kernel(L, sample_kernel, dim3(J.n), dim3(SMP_THREADS), 0, J);
+}
+// One sampler launch over n rows of s->logits: row[i] of sequence seq[i] draws with p_next[i] (-1: st->pos, for a decode
+// run whose step has advanced) into out[out_idx[i]]; decode: the token also feeds the next step (st->next_token) and
+// lands in d_tok_out.  Only calls with a sampled row launch it.
+static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_t* seq, const int32_t* p_next, const int32_t* out_idx,
+                         int32_t* out, bool decode) {
+  SampleJob J{};
+  J.logits = s->logits; J.ld = s->m->vocab_l; J.V = s->m->a.vocab_size; J.n = n;
+  J.params = s->d_samp; J.wbuf = s->d_samp_w; J.pos_ptr = &s->st->pos; J.out = out;
+  J.cand = s->d_samp_cand; J.cnt = reinterpret_cast<unsigned int*>(s->d_samp_cand + (size_t)s->n_seq * SMP_MERGE);
+  J.st = decode ? s->st : nullptr; J.tok_out = decode ? s->d_tok_out : nullptr;
+  for (int i = 0; i < n; i++) {
+    J.row[i] = row[i]; J.slot[i] = seq[i]; J.p_next[i] = p_next[i]; J.out_idx[i] = out_idx ? out_idx[i] : 0;
+  }
+  return launch_sample_job(Launcher{s->stream, LAUNCH_PDL, &s->launches}, J);
+}
+
 // The forward of lnb_forward and lnb_forward_device; the caller holds s->mu.  keep_logits: the logits of the last row, or
 // of all S rows (all_rows), stay in s->logits.  host_logits: NULL, or where those rows are copied (tensor-parallel:
-// gathered from the ranks first).  next_token: NULL, or receives the greedy token of the last row.
+// gathered from the ranks first).  next_token: NULL, or receives the next token of the last row (greedy unless the active
+// sequence samples); greedy_token: NULL, or receives the greedy token of the last row.
 static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int start_pos, bool keep_logits, bool all_rows,
-                          float* host_logits, int32_t* next_token) {
+                          float* host_logits, int32_t* next_token, int32_t* greedy_token = nullptr) {
   if (!tokens) return fail(LNB_EINVAL, "NULL argument");
   if (S <= 0) return fail(LNB_EINVAL, "empty token array");  // llamatransformer.go:146-148
   if (S > s->max_rows) return fail(LNB_EINVAL, "S %d exceeds the session's max_rows %d", S, s->max_rows);
@@ -2150,9 +2186,10 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
   lnb_model* m = s->m;
   CU(cudaSetDevice(m->device));
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
-  const int lrows = keep_logits ? (all_rows ? S : 1) : 0;
+  const bool samp = s->samp_on[s->active_seq];   // the sampler reads the last row's logits
+  const int lrows = keep_logits ? (all_rows ? S : 1) : (samp ? 1 : 0);
   int rc;
-  if (lrows && (rc = ensure_logits(s, (size_t)(all_rows ? s->max_rows : 1)))) return rc;
+  if (lrows && (rc = ensure_logits(s, (size_t)(keep_logits && all_rows ? s->max_rows : 1)))) return rc;
   if (S == 1 && engine_ok(s)) {
     // decode step: ONE persistent kernel; the token id rides in the launch of set_state_kernel (4 bytes of kernel arguments)
     if ((rc = enqueue_decode_engine(s, tokens[0], start_pos, 1, false, false, lrows ? s->logits : nullptr))) return rc;
@@ -2165,16 +2202,22 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
     rc = forward_tc_ok(s, S) ? enqueue_forward_tc(s, S, lrows, gather) : enqueue_forward(s, S, false, lrows, false, false, gather);
     if (rc) return rc;
   }
+  if (samp) {   // the sampled token goes to d_samp_tok; st->next_token keeps the greedy one (lnb_session_logits_argmax)
+    const int32_t row = lrows - 1, seq = s->active_seq, pn = start_pos + S;
+    if ((rc = launch_sample(s, 1, &row, &seq, &pn, nullptr, s->d_samp_tok, false))) return rc;
+  }
   if (host_logits) {
     const float* src = (m->tp_size > 1) ? s->logits_full : s->logits;
     CU(cudaMemcpyAsync(host_logits, src, (size_t)lrows * m->a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
   }
   int32_t* tokpin = s->h_pin + s->max_rows;
-  if (next_token) CU(cudaMemcpyAsync(tokpin, &s->st->next_token, 4, cudaMemcpyDeviceToHost, s->stream));
+  if (next_token || greedy_token) CU(cudaMemcpyAsync(tokpin, &s->st->next_token, 4, cudaMemcpyDeviceToHost, s->stream));
+  if (samp && next_token) CU(cudaMemcpyAsync(tokpin + 1, s->d_samp_tok, 4, cudaMemcpyDeviceToHost, s->stream));
   if ((rc = p2p_err_enqueue(s))) return rc;
   if ((rc = sync_stream(s))) return rc;
   if ((rc = p2p_err_check(s))) return rc;
-  if (next_token) *next_token = *tokpin;
+  if (next_token) *next_token = samp ? tokpin[1] : tokpin[0];
+  if (greedy_token) *greedy_token = tokpin[0];
   return 0;
 }
 
@@ -2195,11 +2238,11 @@ extern "C" int lnb_forward_device(lnb_session* s, const int32_t* tokens, int S, 
   if (!s) return fail(LNB_EINVAL, "NULL argument");
   if (rows_kept != 1 && rows_kept != S) return fail(LNB_EINVAL, "rows_kept must be 1 or S");
   std::lock_guard<std::mutex> lk(s->mu);
-  int32_t tok = -1;
-  const int rc = forward_locked(s, tokens, S, start_pos, true, rows_kept > 1, nullptr, &tok);
+  int32_t tok = -1, greedy = -1;
+  const int rc = forward_locked(s, tokens, S, start_pos, true, rows_kept > 1, nullptr, &tok, &greedy);
   if (rc) return rc;
   if (argmax_last) *argmax_last = tok;
-  s->kept_last_token = tok;
+  s->kept_last_token = greedy;
   s->kept_rows = rows_kept;
   s->generation++;
   if (generation_out) *generation_out = s->generation;
@@ -2306,6 +2349,51 @@ extern "C" int lnb_session_set_active_sequence(lnb_session* s, int seq) {
   s->active_seq = seq;
   return 0;
 }
+// ---- seeded sampling: parameters of one sequence (sample.cuh, DESIGN.md §9b) ----------------------------------------
+static int sampling_check(const lnb_sampling* p) {
+  if (!std::isfinite(p->temperature) || p->temperature < 0.0f) return fail(LNB_EINVAL, "temperature %g must be finite and >= 0", (double)p->temperature);
+  if (p->temperature == 0.0f) return 0;   // greedy: the other fields are unused
+  if (p->top_k < 0) return fail(LNB_EINVAL, "top_k %d must be >= 0 (0: the whole vocabulary)", p->top_k);
+  if (!(p->top_p > 0.0f && p->top_p <= 1.0f)) return fail(LNB_EINVAL, "top_p %g must be in (0, 1]", (double)p->top_p);
+  return 0;
+}
+extern "C" int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampling* p) {
+  if (!s) return fail(LNB_EINVAL, "session is NULL");
+  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  if (s->m->tp_size > 1)
+    return fail(LNB_EINVAL, "sampling is not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", s->m->tp_size);
+  int rc;
+  if (p && (rc = sampling_check(p))) return rc;
+  const bool on = p && p->temperature > 0.0f;
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(s->m->device));
+  if (on && !s->d_samp) {   // parameter slots, weights of n_seq rows, one token; all or nothing
+    const size_t b_par = (size_t)s->n_seq * sizeof(lnb_sampling), b_w = (size_t)s->n_seq * s->m->a.vocab_size * 8;
+    const size_t b_cand = (size_t)s->n_seq * (SMP_MERGE * 8 + 4);
+    lnb_sampling* d_par = nullptr;
+    unsigned long long *d_w = nullptr, *d_cand = nullptr;
+    int32_t* d_tok = nullptr;
+    cudaError_t e = cudaMalloc((void**)&d_par, b_par);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_w, b_w);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_tok, 16);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_cand, b_cand);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_cand, 0, b_cand, s->stream);   // the split sampler's counters start at 0
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      cudaFree(d_par); cudaFree(d_w); cudaFree(d_tok); cudaFree(d_cand);
+      cudaGetLastError();
+      return fail(LNB_ENOMEM, "sampler buffers: %zu bytes of device memory asked for: %s", b_par + b_w + 16 + b_cand, cudaGetErrorString(e));
+    }
+    s->d_samp = d_par; s->d_samp_w = d_w; s->d_samp_tok = d_tok; s->d_samp_cand = d_cand;
+  }
+  if (on) {   // stream-ordered, no host synchronisation; a captured decode graph reads the slot when it replays
+    sample_set_params_kernel<<<1, 1, 0, s->stream>>>(s->d_samp + seq, *p);
+    CU(cudaGetLastError());
+  }
+  s->samp_on[seq] = on;
+  return 0;
+}
+
 // One decode step for n independent sequences (rows 0..n-1 = sequences 0..n-1): tokens[i] is fed at
 // positions[i] of sequence i.  The weights are streamed ONCE for all rows (the reference would run n
 // separate Forward calls on n InferenceContexts, SURVEY F10; every row sees exactly the arithmetic of its
@@ -2329,15 +2417,20 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
   memcpy(ppin, positions, (size_t)n * 4);
   CU(cudaMemcpyAsync(s->d_tokens, s->h_pin, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
   CU(cudaMemcpyAsync(s->d_pos_arr, ppin, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
+  int32_t srow[8], sseq[8], spn[8];
+  int ns = 0;
+  for (int i = 0; i < n; i++)
+    if (s->samp_on[i]) { srow[ns] = i; sseq[ns] = i; spn[ns] = positions[i] + 1; ns++; }
   if (batch_engine_ok(s)) {
     // ONE launch of the batch engine: every weight matrix streamed once for all n sequences
-    if ((rc = batch_engine_build(s, logits ? s->logits : nullptr))) return rc;
+    if ((rc = batch_engine_build(s, (logits || ns) ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, n))) return rc;
     if (logits && (rc = gather_logits(s, 0, n))) return rc;
   } else {
     if ((rc = set_state(s, 0, n, -1, false))) return rc;
     if ((rc = enqueue_forward(s, n, false, n > 1 ? n : 2, false, true))) return rc;
   }
+  if (ns && (rc = launch_sample(s, ns, srow, sseq, spn, srow, s->d_next_arr, false))) return rc;
   if (logits) {
     const float* src = (m->tp_size > 1) ? s->logits_full : s->logits;
     CU(cudaMemcpyAsync(logits, src, (size_t)n * m->a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
@@ -2439,6 +2532,13 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
                                                           : enqueue_forward(s, rows, false, 0, false, false, false, &rm);
   if (rc) return rc;
   s->last_was_engine = false;
+  {   // segments of sampled sequences: the sampler over their rows of s->logits, into d_next_arr
+    int32_t srow[8], sseq[8], spn[8];
+    int ns = 0;
+    for (int i = 0; i < n_segs; i++)
+      if (s->samp_on[seq[i]]) { srow[ns] = i; sseq[ns] = seq[i]; spn[ns] = start_pos[i] + len[i]; ns++; }
+    if (ns && (rc = launch_sample(s, ns, srow, sseq, spn, srow, s->d_next_arr, false))) return rc;
+  }
   if (logits) CU(cudaMemcpyAsync(logits, s->logits, (size_t)n_segs * a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
   int32_t* npin = s->h_rag + (size_t)s->max_rows * 3 + 8;
   if (argmax_out) CU(cudaMemcpyAsync(npin, s->d_next_arr, (size_t)n_segs * 4, cudaMemcpyDeviceToHost, s->stream));
@@ -2457,7 +2557,11 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
   CU(cudaSetDevice(s->m->device));
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward
   int rc;
-  if (engine_ok(s)) {
+  // a sampled sequence decodes on the kernel chain (the persistent engine feeds back the greedy token inside the kernel):
+  // each step keeps its logits row and ends in the sampler, whose token is the next step's input
+  const bool samp = s->samp_on[s->active_seq];
+  if (samp && engine_ok(s)) g_err = "the active sequence samples: lnb_decode_run runs the kernel chain (the decode engine has no sampler)";
+  if (!samp && engine_ok(s)) {
     // the whole run is ONE launch of the persistent engine: n_steps forwards, the greedy token fed back on the device
     if ((rc = engine_build(s, -1, nullptr))) return rc;
     if ((rc = set_state(s, start_pos, 1, first_token, true))) return rc;
@@ -2473,14 +2577,24 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     if (tokens_out) memcpy(tokens_out, s->h_pin + s->max_rows + 8, (size_t)n_steps * 4);
     return use_graph ? 1 : 0;   // (no graph is needed: there is nothing left to replay)
   }
+  if (samp && (rc = ensure_logits(s, 1))) return rc;
+  if (s->graph_tried && (s->graph_sampled != samp || (samp && s->graph_logits != s->logits))) drop_graph(s);
+  auto step = [&]() -> int {
+    const int r = enqueue_forward(s, 1, true, samp ? 1 : 0, true);
+    if (r || !samp) return r;
+    const int32_t row = 0, seq = s->active_seq, pn = -1;
+    return launch_sample(s, 1, &row, &seq, &pn, nullptr, nullptr, true);
+  };
   if (use_graph && !s->graph && !s->graph_tried) {
     s->graph_tried = true;
+    s->graph_sampled = samp;
+    s->graph_logits = s->logits;
     cudaGraph_t g = nullptr;
     const int64_t saved = s->launches;
     cudaError_t e = cudaStreamBeginCapture(s->stream, cudaStreamCaptureModeThreadLocal);
     rc = 0;
     if (e == cudaSuccess) {
-      rc = enqueue_forward(s, 1, true, 0, true);
+      rc = step();
       e = cudaStreamEndCapture(s->stream, &g);
     }
     if (e == cudaSuccess && rc == 0 && g) {
@@ -2499,7 +2613,7 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     if (graph) {
       CU(cudaGraphLaunch(s->graph, s->stream));
       s->launches += s->graph_launches;
-    } else if ((rc = enqueue_forward(s, 1, true, 0, true))) {
+    } else if ((rc = step())) {
       return rc;
     }
   }
@@ -3034,6 +3148,33 @@ extern "C" int lnb_op_argmax_f32(const float* x, int rows, int cols, int32_t* ou
   argmax_f32_kernel<<<rows, 256>>>(dx.as<float>(), cols, dout.as<int32_t>());
   int rc = op_finish();
   if (rc) return rc;
+  D2H(out, dout, (size_t)rows * 4);
+  return 0;
+}
+
+// the sampler alone on host rows: logits[rows, vocab], parameters p[rows], p_next pos_next[rows] -> out[rows]
+extern "C" int lnb_op_sample_f32(const float* logits, int rows, int vocab, const lnb_sampling* p, const int32_t* pos_next, int32_t* out) {
+  OpScope scope_;
+  if (!logits || !p || !pos_next || !out) return fail(LNB_EINVAL, "NULL argument");
+  if (rows < 1 || rows > SMP_MAX_ROWS || vocab < 1) return fail(LNB_EINVAL, "rows %d must be in [1, %d] and vocab %d positive", rows, SMP_MAX_ROWS, vocab);
+  int rc;
+  for (int r = 0; r < rows; r++) {
+    if ((rc = sampling_check(p + r))) return rc;
+    if (pos_next[r] < 0) return fail(LNB_EINVAL, "pos_next[%d] = %d must be >= 0", r, pos_next[r]);
+  }
+  const size_t b = (size_t)rows * vocab * 4;
+  OPBUF(dx, b); OPBUF(dp, (size_t)rows * sizeof(lnb_sampling)); OPBUF(dw, (size_t)rows * vocab * 8); OPBUF(dout, (size_t)rows * 4);
+  OPBUF(dc, (size_t)rows * (SMP_MERGE * 8 + 4));
+  H2D(dx, logits, b);
+  H2D(dp, p, (size_t)rows * sizeof(lnb_sampling));
+  CU(cudaMemset(dc.p, 0, (size_t)rows * (SMP_MERGE * 8 + 4)));
+  SampleJob J{};
+  J.logits = dx.as<float>(); J.ld = vocab; J.V = vocab; J.n = rows;
+  J.params = dp.as<lnb_sampling>(); J.wbuf = dw.as<unsigned long long>(); J.out = dout.as<int32_t>();
+  J.cand = dc.as<unsigned long long>(); J.cnt = reinterpret_cast<unsigned int*>(J.cand + (size_t)rows * SMP_MERGE);
+  for (int r = 0; r < rows; r++) { J.row[r] = r; J.slot[r] = r; J.p_next[r] = pos_next[r]; J.out_idx[r] = r; }
+  if ((rc = launch_sample_job(Launcher{nullptr, LAUNCH_PLAIN, nullptr}, J))) return rc;
+  if ((rc = op_finish())) return rc;
   D2H(out, dout, (size_t)rows * 4);
   return 0;
 }

@@ -3,6 +3,7 @@
 // programmatic-dependent-launch chain.
 #pragma once
 #include "common.cuh"
+#include "sample_det.h"
 
 namespace lnb {
 
@@ -49,12 +50,7 @@ __global__ void untile_kernel(const uint16_t* __restrict__ src, int rows, int K,
 // Synthetic checkpoint generator (DESIGN.md "Synthetic weights"): element i of the FULL
 // row-major tensor `name` is t((2u-1)*scale + offset), u = top 24 bits of
 // splitmix64(seed ^ fnv1a(name), i).  Writes either row-major (panel_major=0) or panel-major.
-LNB_DEVINL uint64_t splitmix64_at(uint64_t seed, uint64_t i) {
-  uint64_t z = seed + (i + 1) * 0x9E3779B97F4A7C15ULL;
-  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
-  z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
-  return z ^ (z >> 31);
-}
+LNB_DEVINL uint64_t splitmix64_at(uint64_t seed, uint64_t i) { return lnb_splitmix64_at(seed, i); }
 LNB_DEVINL uint16_t synth_value(uint64_t seed, uint64_t i, float scale, float offset) {
   const uint64_t z = splitmix64_at(seed, i);
   const float u = __fmul_rn((float)(z >> 40), 1.0f / 16777216.0f);

@@ -13,6 +13,14 @@ import numpy as np
 from . import ml, model as model_mod
 
 GSInProgress, GSFinishedByReachingEOS, GSFinishedByReachingSeqLen = 0, 1, 2
+SamplingArgs = model_mod.SamplingArgs
+
+
+def _sampling_for(sampling, i: int):
+    """prompt i of a batch or continuous run samples with Seed + i: its stream is GenerateTokens(prompts[i]) with that seed"""
+    if sampling is None or sampling.Temperature == 0:
+        return None
+    return SamplingArgs(sampling.Temperature, sampling.TopK, sampling.TopP, (sampling.Seed + i) & (2**64 - 1))
 
 # Row budget of one GenerateTokensContinuous step.  FAST ragged steps of >= 32 rows run on the tensor cores (one pass over
 # the weights); steps of 9..31 rows run the GEMV chain, which streams the weights once per 8 rows (up to 4 passes), and
@@ -97,7 +105,7 @@ class InferenceEngine:
                        IsResendOfWaiting=True, GenerationState=last_state if i + 1 == len(waiting) else GSInProgress)
 
     def GenerateTokens(self, promptTokens, use_reference_api: bool = False, step_times: list | None = None,
-                       prefill_chunk: int = 0):
+                       prefill_chunk: int = 0, sampling: "SamplingArgs | None" = None):
         """Generator over (state, token id) exactly like generatedTokensCh.
 
         use_reference_api=True goes through the reference-shaped calls of every iteration
@@ -106,9 +114,17 @@ class InferenceEngine:
 
         prefill_chunk > 0 (EXTENSION, SURVEY 8f-4): the prompt is fed in chunks of that many tokens (Forward at
         startPos > 0 with S > 1, lnb_session_set_chunked_prefill) instead of one call; prompts longer than the context's
-        max_rows become possible, and the generated stream is the same."""
+        max_rows become possible, and the generated stream is the same.
+
+        sampling (EXTENSION): SamplingArgs of a seeded sampler in place of the greedy argmax (None / Temperature 0: greedy).
+        The reference call sequence ends in ml.Argmax, so use_reference_api=True with a sampler is an error."""
+        sampling = _sampling_for(sampling, 0)
+        if sampling is not None and use_reference_api:
+            raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax (inference.go:207-216); it cannot sample")
         infContext = self.CreateInferenceContext()
         try:
+            if sampling is not None:
+                infContext.set_sampling(0, sampling)
             promptLength = len(promptTokens)
             if prefill_chunk > 0:
                 infContext.allow_chunked_prefill(True)
@@ -155,14 +171,15 @@ class InferenceEngine:
             infContext.close()
 
     def GenerateTokensContinuous(self, prompts, slots: int = 8, step_tokens: int | None = None,
-                                 step_times: list | None = None):
+                                 step_times: list | None = None, sampling: "SamplingArgs | None" = None):
         """Continuous batching (EXTENSION, lnb_forward_ragged): any number of prompts through at most `slots` live
         sequences.  Every step is ONE forward whose rows may belong to different sequences: each decoding sequence gets
         its one row, the rest of the step's row budget (min(step_tokens, max_rows)) goes to prompt chunks, first in first
         out; a prompt whose last chunk is in the step emits its first token from that step; a finished sequence's slot
         is refilled at position 0 by the next waiting prompt.  Steps without prompt rows run lnb_forward_batch (the
         batch engine: one launch per step).  Yields (prompt index, state, token id); per prompt the stream is exactly
-        what GenerateTokens(prompts[i]) yields (the bookkeeping of generateTokensInternal, inference.go:173-254)."""
+        what GenerateTokens(prompts[i]) yields (the bookkeeping of generateTokensInternal, inference.go:173-254).
+        sampling: prompt i samples with Seed + i (the stream of GenerateTokens(prompts[i]) with that seed)."""
         if step_tokens is None:
             step_tokens = DEFAULT_STEP_TOKENS
         if not 1 <= slots <= 8:
@@ -175,13 +192,15 @@ class InferenceEngine:
         if self.context_hook is not None:
             self.context_hook(infContext)
         try:
-            yield from self._generate_continuous(infContext, prompts, slots, min(step_tokens, infContext.max_rows), step_times)
+            yield from self._generate_continuous(infContext, prompts, slots, min(step_tokens, infContext.max_rows), step_times,
+                                                 sampling)
         finally:
             infContext.close()
 
-    def _generate_continuous(self, infContext, prompts, slots: int, budget: int, step_times: list | None = None):
+    def _generate_continuous(self, infContext, prompts, slots: int, budget: int, step_times: list | None = None,
+                             sampling: "SamplingArgs | None" = None):
         """the scheduler of GenerateTokensContinuous on a given context (anything with SequenceLength, forward_ragged and
-        forward_batch)"""
+        forward_batch, and set_sampling when `sampling` samples)"""
         seqLen = infContext.SequenceLength
         stop = self.model.Vocabulary.StopTokenIds
         for p in prompts:
@@ -199,6 +218,9 @@ class InferenceEngine:
                 if slot[k] is None and waiting:
                     slot[k] = dict(i=waiting.popleft(), fed=0, cur=None, pos=0, order=admitted)
                     admitted += 1
+                    sp = _sampling_for(sampling, slot[k]["i"])
+                    if sp is not None:   # before the prompt's first segment (the slot's previous prompt had another seed)
+                        infContext.set_sampling(k, sp)
             decoding = [k for k in range(slots) if slot[k] is not None and slot[k]["cur"] is not None]
             prefilling = sorted((k for k in range(slots) if slot[k] is not None and slot[k]["cur"] is None),
                                 key=lambda k: slot[k]["order"])
@@ -246,17 +268,18 @@ class InferenceEngine:
                     slot[k] = None
                 yield sl["i"], state, tok
 
-    def GenerateTokensBatch(self, prompts, step_times: list | None = None):
+    def GenerateTokensBatch(self, prompts, step_times: list | None = None, sampling: "SamplingArgs | None" = None):
         """The consumer `InferenceEngine.TokenizeBatch` (src/inference/tokenize.go:97-107) never got in the
         reference (SURVEY 8f-4): every prompt runs the loop of generateTokensInternal (:173-254) -- own
         InferenceContext / KV cache, own positions, own stop condition -- but all sequences advance together,
         one pass over the weights per step (lnb_forward_batch).  Yields (sequence index, state, token id);
-        per sequence the stream is exactly what GenerateTokens(prompts[i]) yields."""
+        per sequence the stream is exactly what GenerateTokens(prompts[i]) yields.  sampling: sequence i samples with
+        Seed + i (the stream of GenerateTokens(prompts[i]) with that seed)."""
         n = len(prompts)
         if n < 1:
             raise ml.MlError("empty prompt batch")
         if n == 1:
-            for state, tok in self.GenerateTokens(prompts[0]):
+            for state, tok in self.GenerateTokens(prompts[0], sampling=sampling):
                 yield 0, state, tok
             return
         infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
@@ -271,6 +294,10 @@ class InferenceEngine:
                     raise ml.MlError(f"context SequenceLength {seqLen} must be higher than prompt tokens length {len(p)}")
                 if len(p) < 1 or len(p) > infContext.max_rows:
                     raise ml.MlError(f"prompt length {len(p)} must be in [1, {infContext.max_rows}]")
+            for i in range(n):
+                sp = _sampling_for(sampling, i)
+                if sp is not None:
+                    infContext.set_sampling(i, sp)
             cur = [0] * n                                  # token fed next / position it is fed at
             pos = [0] * n
             done = [False] * n

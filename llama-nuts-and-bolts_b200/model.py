@@ -142,6 +142,20 @@ class InferenceArgs:  # src/common/inferenceargs.go:3-11
     SequenceLength: int = 0
 
 
+@dataclass
+class SamplingArgs:
+    """EXTENSION (the reference only has the greedy ml.Argmax): seeded sampling of the next token, lnb_session_set_sampling.
+    Temperature 0 is greedy; TopK 0 is the whole vocabulary; TopP in (0, 1], 1 is no top-p cut.  The draw for the token at
+    position p uses splitmix64(Seed, p), so a stream depends only on the model, the prompt and these values."""
+    Temperature: float = 0.0
+    TopK: int = 0
+    TopP: float = 1.0
+    Seed: int = 0
+
+    def c(self) -> "_capi.SamplingC":
+        return _capi.SamplingC(float(self.Temperature), int(self.TopK), float(self.TopP), int(self.Seed) & (2**64 - 1))
+
+
 class InferenceContext:
     """model.InferenceContext (inferencecontext.go:8-46): the KV cache (here: in HBM)."""
 
@@ -217,6 +231,16 @@ class InferenceContext:
                                      ptr(nxt, _capi.i32p)))
         return nxt, logits
 
+    def set_sampling(self, seq: int, args: "SamplingArgs | None"):
+        """EXTENSION: sequence `seq` samples its next tokens with `args` (None or Temperature 0: greedy) from its next
+        forward on; every token output of forward_argmax / forward_batch / forward_ragged / decode_run then carries the
+        sampled token for it"""
+        if args is None:
+            check(lib.lnb_session_set_sampling(self.h, seq, None))
+        else:
+            c = args.c()
+            check(lib.lnb_session_set_sampling(self.h, seq, C.byref(c)))
+
     def allow_chunked_prefill(self, on: bool = True):
         """EXTENSION (not in the reference): accept S > 1 at startPos > 0 with the [S,T] causal mask"""
         check(lib.lnb_session_set_chunked_prefill(self.h, int(on)))
@@ -228,7 +252,8 @@ class InferenceContext:
         return int(lib.lnb_session_launch_count(self.h))
 
     def decode_run(self, first_token: int, start_pos: int, n_steps: int, use_graph: bool = True):
-        """device-resident greedy decode (lnb_decode_run): returns (tokens, ms, used_graph)"""
+        """device-resident decode (lnb_decode_run; greedy unless the active sequence samples): returns (tokens, ms,
+        used_graph)"""
         toks = np.empty(n_steps, np.int32)
         ms = C.c_float(0)
         rc = check(lib.lnb_decode_run(self.h, first_token, start_pos, n_steps, int(use_graph),

@@ -1,0 +1,90 @@
+"""ctypes binding of the sampler's sequential C statement (TEST INFRASTRUCTURE, NOT PRODUCT CODE; DESIGN.md §9b).
+
+Only tests/ and tools/ may import this module.  See lnb_sample_ref.c.
+"""
+from __future__ import annotations
+
+import ctypes as C
+import os
+import subprocess
+import sys
+
+import numpy as np
+
+_HERE = os.path.dirname(os.path.abspath(__file__))
+_ROOT = os.path.dirname(_HERE)
+_SO = os.path.join(_HERE, "liblnb_sample_ref.so")
+if _ROOT not in sys.path:
+    sys.path.insert(0, _ROOT)
+
+from oracle import oracle as _oracle  # noqa: E402
+
+_f32p, _i32p, _i64p, _u64p, _f64p = (C.POINTER(C.c_float), C.POINTER(C.c_int32), C.POINTER(C.c_int64), C.POINTER(C.c_uint64),
+                                     C.POINTER(C.c_double))
+_lib = None
+
+
+def build(force: bool = False) -> str:
+    _oracle.build()
+    src = [os.path.join(_HERE, f) for f in ("lnb_sample_ref.c", "Makefile")] + \
+          [os.path.join(_ROOT, "llama-nuts-and-bolts_b200", "csrc", "sample_det.h")]
+    stale = (not os.path.exists(_SO)) or any(os.path.getmtime(s) > os.path.getmtime(_SO) for s in src)
+    if force or stale:
+        subprocess.check_call(["make", "-C", _HERE, "-s"])
+    return _SO
+
+
+def lib():
+    global _lib
+    if _lib is None:
+        build()
+        _oracle.lib()
+        L = C.CDLL(_SO)
+        L.orc_exp_det.restype, L.orc_exp_det.argtypes = C.c_double, [C.c_double]
+        L.orc_exp_det_n.restype, L.orc_exp_det_n.argtypes = None, [_f64p, _f64p, C.c_int64]
+        L.orc_exp_det_max_ulp_f32.restype, L.orc_exp_det_max_ulp_f32.argtypes = C.c_int64, [C.c_uint32, C.c_uint32]
+        L.orc_sample_weight.restype, L.orc_sample_weight.argtypes = C.c_uint64, [C.c_float, C.c_float, C.c_float]
+        L.orc_sample_row.restype = C.c_int32
+        L.orc_sample_row.argtypes = [_f32p, C.c_int, C.c_float, C.c_int32, C.c_float, C.c_uint64, C.c_int64]
+        L.orc_sample_rows.restype = None
+        L.orc_sample_rows.argtypes = [_f32p, C.c_int, C.c_int, _f32p, _i32p, _f32p, _u64p, _i64p, _i32p]
+        L.orc_generate_sampled.restype = C.c_int
+        L.orc_generate_sampled.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
+                                           C.c_float, C.c_uint64, _i32p]
+        _lib = L
+    return _lib
+
+
+def exp_det(z) -> np.ndarray | float:
+    """lnb_exp_det (csrc/sample_det.h) of a float or an f64 array"""
+    if np.isscalar(z):
+        return lib().orc_exp_det(float(z))
+    z = np.ascontiguousarray(z, np.float64)
+    out = np.empty_like(z)
+    lib().orc_exp_det_n(z.ctypes.data_as(_f64p), out.ctypes.data_as(_f64p), z.size)
+    return out
+
+
+def exp_det_max_ulp_f32(lo_bits: int, hi_bits: int) -> int:
+    return int(lib().orc_exp_det_max_ulp_f32(lo_bits, hi_bits))
+
+
+def sample_weight(l: float, m: float, T: float) -> int:
+    return int(lib().orc_sample_weight(l, m, T))
+
+
+def sample_row(logits, T: float, K: int, P: float, seed: int, p_next: int) -> int:
+    row = np.ascontiguousarray(logits, np.float32).reshape(-1)
+    return int(lib().orc_sample_row(row.ctypes.data_as(_f32p), row.size, T, K, P, seed & (2**64 - 1), p_next))
+
+
+def generate_sampled(om, prompt, seq_len: int, T: float, K: int, P: float, seed: int, stop_ids=(128008, 128009)) -> np.ndarray:
+    """orc_generate with the sampler in place of the argmax (om: oracle.OracleModel)"""
+    prompt = np.ascontiguousarray(prompt, np.int32)
+    stop = np.ascontiguousarray(stop_ids, np.int32)
+    out = np.empty(seq_len, np.int32)
+    n = lib().orc_generate_sampled(om.h, om.args.vocab, prompt.ctypes.data_as(_i32p), len(prompt), seq_len,
+                                   stop.ctypes.data_as(_i32p), len(stop), T, K, P, seed & (2**64 - 1), out.ctypes.data_as(_i32p))
+    if n < 0:
+        raise RuntimeError("orc_generate_sampled failed")
+    return out[:n].copy()
