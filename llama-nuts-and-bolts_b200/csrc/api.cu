@@ -1044,6 +1044,9 @@ __global__ void publish_kernel(LnbDevState* st, int advance, int32_t* tok_out) {
   }
 }
 
+// words of a ragged call's row map [tokens | row_seq | row_pos | last row of each segment]: `rows` words each, <= 8 segments
+static size_t row_map_words(int max_rows) { return (size_t)max_rows * 3 + 8; }
+
 struct lnb_session {
   lnb_model* m = nullptr;
   int seq_len = 0, max_rows = 1, mode = LNB_ACC_FAST;
@@ -1067,7 +1070,10 @@ struct lnb_session {
   int32_t* d_tokens = nullptr;
   LnbDevState* st = nullptr;
   int32_t* d_tok_out = nullptr;
-  int32_t* h_pin = nullptr;
+  // pinned staging, one allocation (at h_tok) carved into three views: token ids on their way to d_tokens, or a ragged
+  // call's row map on its way to d_rag [row_map_words]; the positions of a batched step on their way to d_pos_arr [8]; the
+  // tokens a call hands back [seq_len + 8]
+  int32_t *h_tok = nullptr, *h_pos = nullptr, *h_out = nullptr;
   uint32_t* h_err = nullptr;     // pinned mirror of st->ar_error (peer all-reduce timeout flag)
   // logits of the last forward stay in HBM (lnb_forward_device); the host reads rows / argmaxes on demand
   int kept_rows = 0;             // rows of s->logits that belong to the last forward (0: none)
@@ -1089,10 +1095,7 @@ struct lnb_session {
   // (stream_attn); batched steps run it when sdpa_decode_kernel cannot.  Scratch for ss.rows rows per launch group.
   bool stream_attn = false;
   SsScratch ss{};
-  // ragged calls (lnb_forward_ragged), allocated by the first one: [tokens | row_seq | row_pos | last row of each segment]
-  // of one call, max_rows * 3 + 8 words on the device and in pinned staging (ONE host-to-device copy per call)
-  int32_t* d_rag = nullptr;
-  int32_t* h_rag = nullptr;
+  int32_t* d_rag = nullptr;       // the row map of a ragged call, allocated by the first one (ONE host-to-device copy per call)
   int64_t launches = 0;
   // persistent decode engine (engine.cuh): the phase list of one S=1 step in device memory
   EnginePhase* d_phases = nullptr;
@@ -1122,7 +1125,6 @@ struct lnb_session {
   bool graph_tried = false;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::mutex mu;
-  int last_rows = 0;
   // seeded sampling (sample.cuh, lnb_session_set_sampling), allocated by the first sampler set: the parameters of each
   // sequence in device memory (a captured graph reads them there), the weights of up to n_seq rows, the sampled token of
   // a single-sequence forward (st->next_token keeps the greedy one)
@@ -1238,7 +1240,9 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
     if (e == cudaSuccess) e = cudaMemsetAsync(s->cv[l], 0, cbytes, s->stream);
   }
   if (e == cudaSuccess) e = cudaMemsetAsync(s->st, 0, sizeof(LnbDevState), s->stream);
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_pin, (size_t)(max_rows + seq_len + 16) * 4);
+  const size_t in_words = row_map_words(max_rows);
+  if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_tok, (in_words + 8 + seq_len + 8) * 4);
+  if (e == cudaSuccess) { s->h_pos = s->h_tok + in_words; s->h_out = s->h_tok + in_words + 8; }
   if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_err, 64);
   if (e == cudaSuccess) *s->h_err = 0;
   if (e == cudaSuccess) e = cudaEventCreate(&s->ev0);
@@ -1272,10 +1276,9 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
   cudaFree(s->d_rag);
   cudaFree(s->d_samp); cudaFree(s->d_samp_w); cudaFree(s->d_samp_tok); cudaFree(s->d_samp_cand);
-  if (s->h_rag) cudaFreeHost(s->h_rag);
   for (auto p : s->ck) cudaFree(p);
   for (auto p : s->cv) cudaFree(p);
-  if (s->h_pin) cudaFreeHost(s->h_pin);
+  if (s->h_tok) cudaFreeHost(s->h_tok);
   if (s->h_err) cudaFreeHost(s->h_err);
   if (s->h_logits_pin) cudaFreeHost(s->h_logits_pin);
   cudaFree(s->d_keys);
@@ -1847,77 +1850,149 @@ static int enqueue_decode_engine(lnb_session* s, int32_t token, int start_pos, i
   return engine_launch(s, n_steps, advance);
 }
 
-// Row map of a ragged call (lnb_forward_ragged), device pointers: row r holds token tokens[r] of sequence seq[r] at position
-// pos[r]; segment i's last row is last[i].  Rows of one segment are consecutive.
-struct RowMap {
-  const int32_t *tokens, *seq, *pos, *last;
-  int n_segs;
+// The rows of one forward: where row r's token, position and KV cache come from, and what the LM head makes of them.
+// rows_single, rows_batch and rows_ragged are the only places that decide this; the forward builders read it from here.
+enum RowsKind { ROWS_SINGLE, ROWS_BATCH, ROWS_RAGGED };
+// what the LM head produces: the last row's greedy token with no logits kept, the last row's or every row's (NONE, LAST,
+// ALL); or, for output rows that each end their own sequence, the logits and a greedy token in d_next_arr per row (PER_ROW)
+enum RowsHead { HEAD_NONE, HEAD_LAST, HEAD_ALL, HEAD_PER_ROW };
+struct Rows {
+  RowsKind kind;
+  int S;
+  const int32_t* tokens;    // device token id of each row, or NULL: st->next_token (a device-driven decode step)
+  const int32_t* pos_arr;   // device position of each row, or NULL: st->pos + r
+  const int32_t* row_seq;   // ragged: the sequence of each row
+  size_t cache_off;         // elements to the cache every row addresses (the active sequence's), or 0
+  long long seq_stride;     // rows on several caches: elements between consecutive sequences' caches, else 0
+  int mb_rows;              // launch_gemv's mb_rows: ragged 8, else 0
+  const int32_t* seg_last;  // ragged: the last row of each segment
+  RowsHead head;
+  int head_rows;            // rows the LM head computes
+  bool advance;             // the LM head advances st->pos and appends the token to d_tok_out (device-driven decode)
+  bool gather;              // tensor-parallel: the kept logits are all-gathered for the host
 };
-
-// streamed attention of layer l: rows of the call at st->pos + r (batched: sequence r at d_pos_arr[r] on its own cache;
-// ragged: sequence rm->seq[r] at rm->pos[r])
-static StreamAttn stream_params(lnb_session* s, int l, size_t cache_off, bool batch, uint16_t* out, int out_x8,
-                                const RowMap* rm = nullptr) {
-  const lnb_model* m = s->m;
-  const lnb_model_args& a = m->a;
-  StreamAttn P{};
-  P.q = s->q; P.ldq = m->q_l;
-  P.cache_k = s->ck[l] + cache_off; P.cache_v = s->cv[l] + cache_off; P.kv_dim = m->kv_l;
-  P.row_cache_stride = (batch || rm) ? (long long)s->seq_len * m->kv_l : 0;
-  P.row_seq = rm ? rm->seq : nullptr;
-  P.n_rep = a.n_heads / a.n_kv_heads; P.hd = a.head_dim; P.n_heads = m->q_l / a.head_dim;
-  P.pos_arr = rm ? rm->pos : batch ? s->d_pos_arr : nullptr;
-  P.pos_ptr = &s->st->pos; P.pos_step = 1;
-  P.out = out; P.ldo = m->q_l; P.out_x8 = out_x8;
-  P.scale = attn_scale_bf16(a.head_dim);
-  P.strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
-  return P;
+// rows 0..S-1 of the active sequence at st->pos + r.  tokens: device ids, or NULL for st->next_token.  logits_rows: logits
+// kept, 0 = none, 1 = the last row, S = all rows.
+static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int logits_rows, bool advance, bool gather) {
+  Rows R{};
+  R.kind = ROWS_SINGLE; R.S = S; R.tokens = tokens;
+  R.cache_off = (size_t)s->active_seq * s->seq_len * s->m->kv_l;
+  R.head = logits_rows == 0 ? HEAD_NONE : logits_rows == 1 ? HEAD_LAST : HEAD_ALL;
+  R.head_rows = logits_rows > 1 ? S : 1;
+  R.advance = advance; R.gather = gather;
+  return R;
+}
+// a batched step: row r is sequence r, token d_tokens[r] at position d_pos_arr[r]
+static Rows rows_batch(const lnb_session* s, int n) {
+  Rows R{};
+  R.kind = ROWS_BATCH; R.S = n; R.tokens = s->d_tokens; R.pos_arr = s->d_pos_arr;
+  R.seq_stride = (long long)s->seq_len * s->m->kv_l;
+  R.head = HEAD_PER_ROW; R.head_rows = n;
+  return R;
+}
+// a ragged call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each, then the last row of each segment
+static Rows rows_ragged(const lnb_session* s, int rows, int n_segs) {
+  Rows R{};
+  R.kind = ROWS_RAGGED; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
+  R.seq_stride = (long long)s->seq_len * s->m->kv_l;
+  R.mb_rows = 8;
+  R.seg_last = s->d_rag + 3 * rows;
+  R.head = HEAD_PER_ROW; R.head_rows = n_segs;
+  return R;
 }
 
-// LM head of a ragged call: the last row of each segment is compacted into h1 (dead after the last layer), ONE EPI_LOGITS
-// GEMV runs over those n_segs rows, then one greedy argmax per row into d_next_arr, as in a batched decode step
-static int ragged_head(const Launcher& L, lnb_session* s, const RowMap& rm) {
+// Attention of layer l for the rows R (queries in s->q), written to out: plain rows, or the X8 operand of the tensor-core
+// Wo GEMM (out_x8).  Ragged rows always stream, so a ragged call has one attention path whatever the session's other calls
+// use.  sdpa_tc_kernel and sdpa_prefill_kernel write X8 only; sdpa_decode_kernel writes plain rows only.
+static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows& R, uint16_t* out, int out_x8) {
+  const lnb_model* m = s->m;
+  const lnb_model_args& a = m->a;
+  const int S = R.S, n_rep = a.n_heads / a.n_kv_heads, n_q = m->q_l / a.head_dim, n_kv = m->kv_l / a.head_dim;
+  const uint16_t *ck = s->ck[l] + R.cache_off, *cv = s->cv[l] + R.cache_off;
+  const int32_t* pos_ptr = &s->st->pos;
+  const float scale = attn_scale_bf16(a.head_dim);
+  const int strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
+  const bool batched = R.kind == ROWS_BATCH;
+  auto streamed = [&]() {
+    StreamAttn P{};
+    P.q = s->q; P.ldq = m->q_l;
+    P.cache_k = ck; P.cache_v = cv; P.kv_dim = m->kv_l;
+    P.row_cache_stride = R.seq_stride; P.row_seq = R.row_seq; P.pos_arr = R.pos_arr;
+    P.n_rep = n_rep; P.hd = a.head_dim; P.n_heads = n_q;
+    P.pos_ptr = pos_ptr; P.pos_step = 1;
+    P.out = out; P.ldo = m->q_l; P.out_x8 = out_x8;
+    P.scale = scale; P.strict = strict;
+    return launch_stream_attn(L, P, S, n_kv, s->ss);
+  };
+  if (R.kind == ROWS_RAGGED) return streamed();
+  if (!out_x8 && (S == 1 || batched) && s->sdpa_smem_decode)
+    return launch_kernel(L, sdpa_decode_kernel, dim3(n_kv, S), dim3(128 * n_rep), s->sdpa_decode_smem, (const uint16_t*)s->q, ck, cv,
+                         m->kv_l, n_rep, a.head_dim, out, pos_ptr, s->seq_len, strict, scale, R.pos_arr,
+                         (long long)s->seq_len * m->kv_l, m->q_l, (const LnbDevState*)s->st);
+  if (out_x8 && a.head_dim == SP_HD) {
+    const double* exp_tab = sdpa_tc_enabled() ? exp_table_device() : nullptr;
+    if (exp_tab)
+      return launch_kernel(L, sdpa_tc_kernel, dim3(n_q, (S + 127) / 128), dim3(256), (size_t)ST_SMEM, (const uint16_t*)s->q, m->q_l, ck,
+                           cv, m->kv_l, n_rep, out, m->q_l, pos_ptr, S, scale, exp_tab);
+    return launch_kernel(L, sdpa_prefill_kernel, dim3(n_q, (S + SP_QB - 1) / SP_QB), dim3(256), (size_t)SP_SMEM, (const uint16_t*)s->q,
+                         m->q_l, ck, cv, m->kv_l, n_rep, out, m->q_l, pos_ptr, S, scale);
+  }
+  if (batched || s->stream_attn) return streamed();
+  return launch_kernel(L, sdpa_kernel, dim3(n_q, S), dim3(128), (size_t)s->seq_len * 12 + (size_t)a.head_dim * 4, (const uint16_t*)s->q,
+                       m->q_l, ck, cv, m->kv_l, n_rep, a.head_dim, out, m->q_l, pos_ptr, 0, S, S > 1 ? 1 : 0, strict, scale, out_x8);
+}
+
+// LM head of a batched step or a ragged call, where every output row is the last row of its own sequence: ragged calls
+// first compact the last row of each segment into h1 (dead after the last layer); then ONE EPI_LOGITS GEMV over the
+// head_rows rows and one greedy argmax per row into d_next_arr (tensor-parallel: on the gathered logits)
+static int per_row_head(const Launcher& L, lnb_session* s, const Rows& R) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   const bool strict = (s->mode == LNB_ACC_STRICT);
+  const int n = R.head_rows;
+  const uint16_t* x = R.seg_last ? s->h1 : s->x;
   int rc;
-  if ((rc = launch_kernel(L, gather_rows_kernel, dim3(rm.n_segs), dim3(256), 0, (const uint16_t*)s->x, rm.last, (const LnbDevState*)s->st,
-                          s->h1, a.dim)))
+  if (R.seg_last && (rc = launch_kernel(L, gather_rows_kernel, dim3(n), dim3(256), 0, (const uint16_t*)s->x, R.seg_last,
+                                        (const LnbDevState*)s->st, s->h1, a.dim)))
     return rc;
-  if (strict && (rc = launch_rms_scale(L, s->h1, a.dim, s->rs, rm.n_segs, a.dim, a.norm_eps))) return rc;
+  if (strict && (rc = launch_rms_scale(L, x, a.dim, s->rs, n, a.dim, a.norm_eps))) return rc;
   GemvParams p{};
   p.rscale = strict ? s->rs : nullptr;
-  p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
-  p.out_f32 = s->logits; p.ldo = m->vocab_l; p.st = nullptr; p.argmax_row = -1;
-  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, rm.n_segs, 8))) return rc;
-  return launch_kernel(L, argmax_f32_kernel, dim3(rm.n_segs), dim3(256), 0, (const float*)s->logits, a.vocab_size, s->d_next_arr);
+  p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
+  p.out_f32 = s->logits; p.ldo = m->vocab_l; p.n_offset = m->tp_rank * m->vocab_l; p.st = nullptr; p.argmax_row = -1;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, n, R.mb_rows))) return rc;
+  if ((rc = gather_logits(s, 0, n))) return rc;
+  const float* lg = (m->tp_size > 1) ? s->logits_full : s->logits;
+  return launch_kernel(L, argmax_f32_kernel, dim3(n), dim3(256), 0, lg, a.vocab_size, s->d_next_arr);
 }
 
-// Enqueue one LlamaTransformer.Forward (llamatransformer.go:145-180) for S rows on the
-// session stream.  from_state_token: row 0's token is st->next_token (device-driven decode).
-// logits_rows: 0 = none stored, 1 = last row, S = all rows.  advance: decode-loop bookkeeping.
-// rm: a ragged call -- rows of several sequences at their own positions (tokens, positions and caches from the row map,
-// attention on the streamed kernels, the LM head of ragged_head; logits_rows, advance and batch are unused).
-static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int logits_rows, bool advance, bool batch = false,
-                           bool gather = true, const RowMap* rm = nullptr) {
+// Prompt processing on the tensor cores (LNB_ACC_FAST, S >= 32): the same forward pass as
+// enqueue_forward with every projection as a tensor-core GEMM (gemm_tc.cuh) and the elementwise steps
+// as separate memory-bound kernels that write the next GEMM's X8 operand directly.  Batched steps (at most 8 rows)
+// never qualify.
+static bool forward_tc_ok(const lnb_session* s, int S) {
+  const lnb_model* m = s->m;
+  const lnb_model_args& a = m->a;
+  return s->mode == LNB_ACC_FAST && s->xn8 && S >= 32 && (m->q_l + 2 * m->kv_l) % TC_BN == 0 && a.dim % TC_BN == 0 &&
+         (2 * m->ffn_l) % TC_BN == 0 && a.dim % TC_KT == 0 && m->q_l % TC_KT == 0 && m->ffn_l % TC_KT == 0;
+}
+static int enqueue_forward_tc(lnb_session* s, const Rows& R);
+
+// Enqueue one LlamaTransformer.Forward (llamatransformer.go:145-180) for the rows R on the session stream: on the tensor
+// cores when forward_tc_ok, else as the kernel chain below.  Every forward but the decode engines' comes through here.
+static int enqueue_forward(lnb_session* s, const Rows& R) {
+  s->last_was_engine = false;   // this forward's residual stream is s->x
+  if (forward_tc_ok(s, R.S)) return enqueue_forward_tc(s, R);
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
   const int mode = s->mode;
-  const int32_t* pos_ptr = &s->st->pos;
-  // single-sequence calls work on the cache of the active sequence; a batched step or a ragged call addresses all of them
-  const size_t seq_stride = (size_t)s->seq_len * m->kv_l;
-  const size_t cache_off = (batch || rm) ? 0 : (size_t)s->active_seq * seq_stride;
-  const int mb_rows = rm ? 8 : 0;
-  if (batch && !s->sdpa_smem_decode && !s->ss.sc)
-    return fail(LNB_EINVAL, "batched decode beyond the shared-memory attention kernel needs head_dim <= 128 and n_rep <= 8");
+  const int S = R.S, mb_rows = R.mb_rows;
   int rc;
-  rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd,
-                     (const int32_t*)(rm ? rm->tokens : from_state_token ? nullptr : s->d_tokens), (const LnbDevState*)s->st, s->x, a.dim);
+  rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd, R.tokens, (const LnbDevState*)s->st, s->x,
+                     a.dim);
   if (rc) return rc;
   const int n_layers = active_layers(s);
-  const float scale = attn_scale_bf16(a.head_dim);
-  const size_t sdpa_smem = (size_t)s->seq_len * 12 + (size_t)a.head_dim * 4;
   const bool strict = (mode == LNB_ACC_STRICT);
   auto strict_scale = [&](const uint16_t* xin, int rows) -> int {
     if (!strict) return 0;
@@ -1954,28 +2029,11 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
       p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm; p.eps = a.norm_eps;
       p.out_bf16 = s->q; p.ldo = m->q_l;
       p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
-      p.cache_k = s->ck[l] + cache_off; p.cache_v = s->cv[l] + cache_off; p.cis = m->cis; p.pos_ptr = pos_ptr;
-      if (batch) { p.pos_arr = s->d_pos_arr; p.cache_seq_stride = (long long)seq_stride; }
-      if (rm) { p.pos_arr = rm->pos; p.row_seq = rm->seq; p.cache_seq_stride = (long long)seq_stride; }
+      p.cache_k = s->ck[l] + R.cache_off; p.cache_v = s->cv[l] + R.cache_off; p.cis = m->cis; p.pos_ptr = &s->st->pos;
+      p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = R.seq_stride;
       if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, S, mb_rows))) return rc;
     }
-    if (rm) {   // one attention path for every ragged row, whatever the session's other calls use
-      rc = launch_stream_attn(L, stream_params(s, l, 0, false, s->o, 0, rm), S, m->kv_l / a.head_dim, s->ss);
-    } else if ((S == 1 || batch) && s->sdpa_smem_decode) {
-      const int n_rep = a.n_heads / a.n_kv_heads;
-      rc = launch_kernel(L, sdpa_decode_kernel, dim3(m->kv_l / a.head_dim, batch ? S : 1), dim3(128 * n_rep), s->sdpa_decode_smem,
-                         (const uint16_t*)s->q, (const uint16_t*)(s->ck[l] + cache_off), (const uint16_t*)(s->cv[l] + cache_off), m->kv_l,
-                         n_rep, a.head_dim, s->o, pos_ptr, s->seq_len, mode == LNB_ACC_STRICT ? 1 : 0, scale,
-                         (const int32_t*)(batch ? s->d_pos_arr : nullptr), (long long)seq_stride, m->q_l, (const LnbDevState*)s->st);
-    } else if (batch || s->stream_attn) {
-      rc = launch_stream_attn(L, stream_params(s, l, cache_off, batch, s->o, 0), S, m->kv_l / a.head_dim, s->ss);
-    } else {
-      rc = launch_kernel(L, sdpa_kernel, dim3(m->q_l / a.head_dim, S), dim3(128), sdpa_smem, (const uint16_t*)s->q, m->q_l,
-                         (const uint16_t*)(s->ck[l] + cache_off), (const uint16_t*)(s->cv[l] + cache_off), m->kv_l,
-                         a.n_heads / a.n_kv_heads, a.head_dim, s->o, m->q_l, pos_ptr, 0, S, S > 1 ? 1 : 0,
-                         mode == LNB_ACC_STRICT ? 1 : 0, scale, 0);
-    }
-    if (rc) return rc;
+    if ((rc = launch_attention(L, s, l, R, s->o, 0))) return rc;
     if ((rc = proj_resid(W.wo, m->q_l, s->o, s->x, s->h1))) return rc;            // wo + residual (:522, :232)
     if ((rc = strict_scale(s->h1, S))) return rc;
     {  // ffn_norm -> w1|w3 -> SiLU * up                             (:237, :601-614)
@@ -1987,67 +2045,43 @@ static int enqueue_forward(lnb_session* s, int S, bool from_state_token, int log
     }
     if ((rc = proj_resid(W.w2, m->ffn_l, s->mbuf, s->h1, s->x))) return rc;        // w2 + residual (:619, :248)
   }
-  if (rm) {
-    if ((rc = ragged_head(L, s, *rm))) return rc;
-  } else {  // output_norm -> output -> f32 logits (+ greedy argmax of the last row)   (:166-175; inference.go:207-216)
-    const int rows = (logits_rows > 1) ? S : 1;  // rows of the head actually computed
-    const int row0 = S - rows;
-    if ((rc = strict_scale(s->x + (size_t)row0 * a.dim, rows))) return rc;
-    GemvParams p{};
-    p.rscale = strict ? s->rs : nullptr;
-    p.W = m->output; p.N = m->vocab_l; p.K = a.dim;
-    p.x = s->x + (size_t)row0 * a.dim; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
-    p.out_f32 = logits_rows > 0 ? s->logits : nullptr; p.ldo = m->vocab_l;
-    p.n_offset = m->tp_rank * m->vocab_l;
-    p.st = batch ? nullptr : s->st; p.argmax_row = batch ? -1 : rows - 1; p.m_off = 0;
-    p.publish = (m->tp_size == 1) ? 1 : 0;
-    p.advance = advance ? 1 : 0; p.tok_out = s->d_tok_out;
-    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, rows))) return rc;
-    if (batch) {
-      // every row is the last row of its own sequence: one greedy argmax per row on the (gathered) logits
-      if ((rc = gather_logits(s, 0, rows))) return rc;
-      const float* lg = (m->tp_size > 1) ? s->logits_full : s->logits;
-      if ((rc = launch_kernel(L, argmax_f32_kernel, dim3(rows), dim3(256), 0, lg, a.vocab_size, s->d_next_arr))) return rc;
-    } else if (m->tp_size > 1) {
-      if (s->p2p_ready) rc = launch_kernel(L, p2p_argmax_kernel, dim3(1), dim3(32), 0, s->p2p, s->st, advance ? 1 : 0, s->d_tok_out);
-      else rc = reduce_argmax_publish(L, s, advance);
-      if (rc) return rc;
-      if (logits_rows > 0 && gather && (rc = gather_logits(s, 0, rows))) return rc;
-    }
+  if (R.head == HEAD_PER_ROW) return per_row_head(L, s, R);
+  // output_norm -> output -> f32 logits (+ greedy argmax of the last row)   (:166-175; inference.go:207-216)
+  const int rows = R.head_rows;
+  const int row0 = S - rows;
+  if ((rc = strict_scale(s->x + (size_t)row0 * a.dim, rows))) return rc;
+  GemvParams p{};
+  p.rscale = strict ? s->rs : nullptr;
+  p.W = m->output; p.N = m->vocab_l; p.K = a.dim;
+  p.x = s->x + (size_t)row0 * a.dim; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
+  p.out_f32 = R.head != HEAD_NONE ? s->logits : nullptr; p.ldo = m->vocab_l;
+  p.n_offset = m->tp_rank * m->vocab_l;
+  p.st = s->st; p.argmax_row = rows - 1; p.m_off = 0;
+  p.publish = (m->tp_size == 1) ? 1 : 0;
+  p.advance = R.advance ? 1 : 0; p.tok_out = s->d_tok_out;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, rows))) return rc;
+  if (m->tp_size > 1) {
+    if (s->p2p_ready) rc = launch_kernel(L, p2p_argmax_kernel, dim3(1), dim3(32), 0, s->p2p, s->st, R.advance ? 1 : 0, s->d_tok_out);
+    else rc = reduce_argmax_publish(L, s, R.advance);
+    if (rc) return rc;
+    if (R.head != HEAD_NONE && R.gather && (rc = gather_logits(s, 0, rows))) return rc;
   }
-  s->last_rows = S;
-  s->last_was_engine = false;
   return 0;
 }
 
-// Prompt processing on the tensor cores (LNB_ACC_FAST, S >= 32): the same forward pass as
-// enqueue_forward with every projection as a tensor-core GEMM (gemm_tc.cuh) and the elementwise steps
-// as separate memory-bound kernels that write the next GEMM's X8 operand directly.
-static bool forward_tc_ok(const lnb_session* s, int S) {
-  const lnb_model* m = s->m;
-  const lnb_model_args& a = m->a;
-  return s->mode == LNB_ACC_FAST && s->xn8 && S >= 32 && (m->q_l + 2 * m->kv_l) % TC_BN == 0 && a.dim % TC_BN == 0 &&
-         (2 * m->ffn_l) % TC_BN == 0 && a.dim % TC_KT == 0 && m->q_l % TC_KT == 0 && m->ffn_l % TC_KT == 0;
-}
-// rm: a ragged call (see enqueue_forward): projections stay on the tensor cores, RoPE / KV append follow the row map, and
-// attention runs on the streamed kernels
-static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gather = true, const RowMap* rm = nullptr) {
+// the tensor-core form of enqueue_forward (which routes here): projections as GEMMs, RoPE / KV append in rope_kv_kernel
+static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
-  const int32_t* pos_ptr = &s->st->pos;
+  const int S = R.S;
   const int Mpad = (S + TC_BM - 1) / TC_BM * TC_BM;
   const int qkv_n = m->q_l + 2 * m->kv_l;
-  const size_t seq_stride = (size_t)s->seq_len * m->kv_l;
-  const size_t tc_cache_off = rm ? 0 : (size_t)s->active_seq * seq_stride;
   int rc;
-  if ((rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd, (const int32_t*)(rm ? rm->tokens : s->d_tokens),
-                          (const LnbDevState*)s->st, s->x, a.dim)))
+  if ((rc = launch_kernel(L, gather_rows_kernel, dim3(S), dim3(256), 0, (const uint16_t*)m->tok_embd, R.tokens, (const LnbDevState*)s->st,
+                          s->x, a.dim)))
     return rc;
   const int n_layers = active_layers(s);
-  const float scale = attn_scale_bf16(a.head_dim);
-  const size_t sdpa_smem = (size_t)s->seq_len * 12 + (size_t)a.head_dim * 4;
-  const double* exp_tab = sdpa_tc_enabled() ? exp_table_device() : nullptr;
   const int ew_grid = m->sm_count * 8;
   // wo / w2 + residual: out = res + X W^T; tensor-parallel ranks sum their partials over NCCL first
   auto proj_resid = [&](const uint16_t* X8, const uint16_t* W, int K, const uint16_t* res, uint16_t* out) -> int {
@@ -2073,28 +2107,10 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
       if ((rc = launch_gemm_tc<TC_EPI_BF16>(L, g))) return rc;
     }
     if ((rc = launch_kernel(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
-                            a.head_dim, s->ck[l] + tc_cache_off, s->cv[l] + tc_cache_off, (const float*)m->cis, pos_ptr, S,
-                            (const int32_t*)(rm ? rm->pos : nullptr), (const int32_t*)(rm ? rm->seq : nullptr), (long long)seq_stride)))
+                            a.head_dim, s->ck[l] + R.cache_off, s->cv[l] + R.cache_off, (const float*)m->cis, (const int32_t*)&s->st->pos, S,
+                            R.pos_arr, R.row_seq, (long long)s->seq_len * m->kv_l)))
       return rc;
-    if (rm) {
-      if ((rc = launch_stream_attn(L, stream_params(s, l, 0, false, s->o8, 1, rm), S, m->kv_l / a.head_dim, s->ss))) return rc;
-    } else if (a.head_dim == SP_HD && exp_tab) {
-      if ((rc = launch_kernel(L, sdpa_tc_kernel, dim3(m->q_l / a.head_dim, (S + 127) / 128), dim3(256), (size_t)ST_SMEM,
-                              (const uint16_t*)s->q, m->q_l, (const uint16_t*)(s->ck[l] + tc_cache_off),
-                              (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l, a.n_heads / a.n_kv_heads, s->o8, m->q_l, pos_ptr, S, scale,
-                              exp_tab)))
-        return rc;
-    } else if (a.head_dim == SP_HD) {
-      if ((rc = launch_kernel(L, sdpa_prefill_kernel, dim3(m->q_l / a.head_dim, (S + SP_QB - 1) / SP_QB), dim3(256), (size_t)SP_SMEM,
-                              (const uint16_t*)s->q, m->q_l, (const uint16_t*)(s->ck[l] + tc_cache_off),
-                              (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l, a.n_heads / a.n_kv_heads, s->o8, m->q_l, pos_ptr, S, scale)))
-        return rc;
-    } else if (s->stream_attn) {
-      if ((rc = launch_stream_attn(L, stream_params(s, l, tc_cache_off, false, s->o8, 1), S, m->kv_l / a.head_dim, s->ss))) return rc;
-    } else if ((rc = launch_kernel(L, sdpa_kernel, dim3(m->q_l / a.head_dim, S), dim3(128), sdpa_smem, (const uint16_t*)s->q, m->q_l,
-                                   (const uint16_t*)(s->ck[l] + tc_cache_off), (const uint16_t*)(s->cv[l] + tc_cache_off), m->kv_l,
-                                   a.n_heads / a.n_kv_heads, a.head_dim, s->o8, m->q_l, pos_ptr, 0, S, 1, 0, scale, 1)))
-      return rc;
+    if ((rc = launch_attention(L, s, l, R, s->o8, 1))) return rc;
     if ((rc = proj_resid(s->o8, W.wo, m->q_l, s->x, s->h1))) return rc;
     if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->h1, a.dim, (const uint16_t*)W.ffn_norm,
                             s->xn8, S, a.dim, a.norm_eps)))
@@ -2109,19 +2125,15 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
   }
   // LM head: all rows on the tensor cores when asked for (and the vocabulary shard tiles), then the
   // last row through the GEMV, which also owns the greedy argmax (identical to the decode path)
-  if (rm) {
-    if ((rc = ragged_head(L, s, *rm))) return rc;
-    s->last_rows = S;
-    return 0;
-  }
-  if (logits_rows > 1 && m->vocab_l % TC_BN == 0) {
+  if (R.head == HEAD_PER_ROW) return per_row_head(L, s, R);
+  if (R.head == HEAD_ALL && m->vocab_l % TC_BN == 0) {
     if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->x, a.dim, (const uint16_t*)m->norm, s->xn8, S,
                             a.dim, a.norm_eps)))
       return rc;
     GemmTcParams g{};
     g.X8 = s->xn8; g.W = m->output; g.M = S - 1; g.N = m->vocab_l; g.K = a.dim; g.out_f32 = s->logits; g.ldo = m->vocab_l;
     if (S > 1 && (rc = launch_gemm_tc<TC_EPI_F32TRUNC>(L, g))) return rc;
-  } else if (logits_rows > 1 && S > 1) {
+  } else if (R.head == HEAD_ALL && S > 1) {
     GemvParams p{};
     p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
     p.out_f32 = s->logits; p.ldo = m->vocab_l; p.st = nullptr; p.argmax_row = -1;
@@ -2131,16 +2143,15 @@ static int enqueue_forward_tc(lnb_session* s, int S, int logits_rows, bool gathe
     GemvParams p{};
     p.W = m->output; p.N = m->vocab_l; p.K = a.dim;
     p.x = s->x + (size_t)(S - 1) * a.dim; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
-    p.out_f32 = logits_rows > 0 ? s->logits + (logits_rows > 1 ? (size_t)(S - 1) * m->vocab_l : 0) : nullptr;
+    p.out_f32 = R.head != HEAD_NONE ? s->logits + (R.head == HEAD_ALL ? (size_t)(S - 1) * m->vocab_l : 0) : nullptr;
     p.ldo = m->vocab_l; p.n_offset = m->tp_rank * m->vocab_l;
     p.st = s->st; p.argmax_row = 0; p.publish = (m->tp_size == 1) ? 1 : 0; p.advance = 0; p.tok_out = s->d_tok_out;
     if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1))) return rc;
     if (m->tp_size > 1) {
       if ((rc = reduce_argmax_publish(L, s, false))) return rc;
-      if (logits_rows > 0 && gather && (rc = gather_logits(s, 0, logits_rows > 1 ? S : 1))) return rc;
+      if (R.head != HEAD_NONE && R.gather && (rc = gather_logits(s, 0, R.head_rows))) return rc;
     }
   }
-  s->last_rows = S;
   return 0;
 }
 
@@ -2167,6 +2178,30 @@ static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_
   return launch_sample_job(Launcher{s->stream, LAUNCH_PDL, &s->launches}, J);
 }
 
+// The end of lnb_forward(_device), lnb_forward_batch and lnb_forward_ragged.  Output row i is logits row row0 + i, of
+// sequence seq[i] at next position p_next[i]; rows of sampled sequences draw into samp_out[i].  host_logits (or NULL) gets
+// logits rows [0, logits_rows), s->h_out[0, n) the tokens at d_tok (or NULL), then s->h_out[n] the sampled token of row 0
+// when the sampler writes beside them (samp_out != d_tok).
+static int call_tail(lnb_session* s, int n, int row0, const int32_t* seq, const int32_t* p_next, int32_t* samp_out,
+                     float* host_logits, int logits_rows, const int32_t* d_tok) {
+  int32_t srow[8], sseq[8], spn[8], sidx[8];
+  int ns = 0;
+  for (int i = 0; i < n; i++)
+    if (s->samp_on[seq[i]]) { srow[ns] = row0 + i; sseq[ns] = seq[i]; spn[ns] = p_next[i]; sidx[ns] = i; ns++; }
+  int rc;
+  if (ns && (rc = launch_sample(s, ns, srow, sseq, spn, sidx, samp_out, false))) return rc;
+  lnb_model* m = s->m;
+  if (host_logits) {
+    const float* src = (m->tp_size > 1) ? s->logits_full : s->logits;
+    CU(cudaMemcpyAsync(host_logits, src, (size_t)logits_rows * m->a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
+  }
+  if (d_tok) CU(cudaMemcpyAsync(s->h_out, d_tok, (size_t)n * 4, cudaMemcpyDeviceToHost, s->stream));
+  if (d_tok && ns && samp_out != d_tok) CU(cudaMemcpyAsync(s->h_out + n, samp_out, 4, cudaMemcpyDeviceToHost, s->stream));
+  if ((rc = p2p_err_enqueue(s))) return rc;
+  if ((rc = sync_stream(s))) return rc;
+  return p2p_err_check(s);
+}
+
 // The forward of lnb_forward and lnb_forward_device; the caller holds s->mu.  keep_logits: the logits of the last row, or
 // of all S rows (all_rows), stay in s->logits.  host_logits: NULL, or where those rows are copied (tensor-parallel:
 // gathered from the ranks first).  next_token: NULL, or receives the next token of the last row (greedy unless the active
@@ -2186,7 +2221,8 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
   lnb_model* m = s->m;
   CU(cudaSetDevice(m->device));
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
-  const bool samp = s->samp_on[s->active_seq];   // the sampler reads the last row's logits
+  const int32_t seq = s->active_seq, p_next = start_pos + S;
+  const bool samp = s->samp_on[seq];   // the sampler reads the last row's logits
   const int lrows = keep_logits ? (all_rows ? S : 1) : (samp ? 1 : 0);
   int rc;
   if (lrows && (rc = ensure_logits(s, (size_t)(keep_logits && all_rows ? s->max_rows : 1)))) return rc;
@@ -2195,29 +2231,17 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
     if ((rc = enqueue_decode_engine(s, tokens[0], start_pos, 1, false, false, lrows ? s->logits : nullptr))) return rc;
     if (host_logits && (rc = gather_logits(s, 0, 1))) return rc;
   } else {
-    memcpy(s->h_pin, tokens, (size_t)S * 4);
-    CU(cudaMemcpyAsync(s->d_tokens, s->h_pin, (size_t)S * 4, cudaMemcpyHostToDevice, s->stream));
+    memcpy(s->h_tok, tokens, (size_t)S * 4);
+    CU(cudaMemcpyAsync(s->d_tokens, s->h_tok, (size_t)S * 4, cudaMemcpyHostToDevice, s->stream));
     if ((rc = set_state(s, start_pos, S, -1, false))) return rc;
-    const bool gather = host_logits != nullptr;
-    rc = forward_tc_ok(s, S) ? enqueue_forward_tc(s, S, lrows, gather) : enqueue_forward(s, S, false, lrows, false, false, gather);
-    if (rc) return rc;
+    if ((rc = enqueue_forward(s, rows_single(s, S, s->d_tokens, lrows, false, host_logits != nullptr)))) return rc;
   }
-  if (samp) {   // the sampled token goes to d_samp_tok; st->next_token keeps the greedy one (lnb_session_logits_argmax)
-    const int32_t row = lrows - 1, seq = s->active_seq, pn = start_pos + S;
-    if ((rc = launch_sample(s, 1, &row, &seq, &pn, nullptr, s->d_samp_tok, false))) return rc;
-  }
-  if (host_logits) {
-    const float* src = (m->tp_size > 1) ? s->logits_full : s->logits;
-    CU(cudaMemcpyAsync(host_logits, src, (size_t)lrows * m->a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
-  }
-  int32_t* tokpin = s->h_pin + s->max_rows;
-  if (next_token || greedy_token) CU(cudaMemcpyAsync(tokpin, &s->st->next_token, 4, cudaMemcpyDeviceToHost, s->stream));
-  if (samp && next_token) CU(cudaMemcpyAsync(tokpin + 1, s->d_samp_tok, 4, cudaMemcpyDeviceToHost, s->stream));
-  if ((rc = p2p_err_enqueue(s))) return rc;
-  if ((rc = sync_stream(s))) return rc;
-  if ((rc = p2p_err_check(s))) return rc;
-  if (next_token) *next_token = samp ? tokpin[1] : tokpin[0];
-  if (greedy_token) *greedy_token = tokpin[0];
+  // the sampled token goes to d_samp_tok; st->next_token keeps the greedy one (lnb_session_logits_argmax)
+  if ((rc = call_tail(s, 1, lrows - 1, &seq, &p_next, s->d_samp_tok, host_logits, lrows,
+                      (next_token || greedy_token) ? &s->st->next_token : nullptr)))
+    return rc;
+  if (next_token) *next_token = samp ? s->h_out[1] : s->h_out[0];
+  if (greedy_token) *greedy_token = s->h_out[0];
   return 0;
 }
 
@@ -2412,46 +2436,37 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
   int rc = ensure_logits(s, (size_t)s->max_rows);
   if (rc) return rc;
-  memcpy(s->h_pin, tokens, (size_t)n * 4);
-  int32_t* ppin = s->h_pin + s->max_rows;
-  memcpy(ppin, positions, (size_t)n * 4);
-  CU(cudaMemcpyAsync(s->d_tokens, s->h_pin, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
-  CU(cudaMemcpyAsync(s->d_pos_arr, ppin, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
-  int32_t srow[8], sseq[8], spn[8];
-  int ns = 0;
-  for (int i = 0; i < n; i++)
-    if (s->samp_on[i]) { srow[ns] = i; sseq[ns] = i; spn[ns] = positions[i] + 1; ns++; }
+  memcpy(s->h_tok, tokens, (size_t)n * 4);
+  memcpy(s->h_pos, positions, (size_t)n * 4);
+  CU(cudaMemcpyAsync(s->d_tokens, s->h_tok, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
+  CU(cudaMemcpyAsync(s->d_pos_arr, s->h_pos, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
+  int32_t seq[8], p_next[8];
+  bool samp = false;
+  for (int i = 0; i < n; i++) { seq[i] = i; p_next[i] = positions[i] + 1; samp |= s->samp_on[i]; }
   if (batch_engine_ok(s)) {
     // ONE launch of the batch engine: every weight matrix streamed once for all n sequences
-    if ((rc = batch_engine_build(s, (logits || ns) ? s->logits : nullptr))) return rc;
+    if ((rc = batch_engine_build(s, (logits || samp) ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, n))) return rc;
     if (logits && (rc = gather_logits(s, 0, n))) return rc;
   } else {
+    if (!s->sdpa_smem_decode && !s->ss.sc)
+      return fail(LNB_EINVAL, "batched decode beyond the shared-memory attention kernel needs head_dim <= 128 and n_rep <= 8");
     if ((rc = set_state(s, 0, n, -1, false))) return rc;
-    if ((rc = enqueue_forward(s, n, false, n > 1 ? n : 2, false, true))) return rc;
+    if ((rc = enqueue_forward(s, rows_batch(s, n)))) return rc;
   }
-  if (ns && (rc = launch_sample(s, ns, srow, sseq, spn, srow, s->d_next_arr, false))) return rc;
-  if (logits) {
-    const float* src = (m->tp_size > 1) ? s->logits_full : s->logits;
-    CU(cudaMemcpyAsync(logits, src, (size_t)n * m->a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
-  }
-  int32_t* npin = s->h_pin + s->max_rows + 16;
-  if (argmax_out) CU(cudaMemcpyAsync(npin, s->d_next_arr, (size_t)n * 4, cudaMemcpyDeviceToHost, s->stream));
-  if ((rc = p2p_err_enqueue(s))) return rc;
-  if ((rc = sync_stream(s))) return rc;
-  if ((rc = p2p_err_check(s))) return rc;
-  if (argmax_out) memcpy(argmax_out, npin, (size_t)n * 4);
+  if ((rc = call_tail(s, n, 0, seq, p_next, s->d_next_arr, logits, n, argmax_out ? s->d_next_arr : nullptr))) return rc;
+  if (argmax_out) memcpy(argmax_out, s->h_out, (size_t)n * 4);
   return 0;
 }
 
 // ---- ragged calls (continuous batching): segments of several sequences at their own positions in ONE forward ----------
-// Buffers of the first ragged call: the row map (device + pinned staging) and, when the session has none or a smaller one,
+// Buffers of the first ragged call: the row map on the device and, when the session has none or a smaller one,
 // stream-attention scratch for max_rows rows per launch group.  Nothing is replaced unless every allocation succeeded, so a
 // failure (LNB_ENOMEM) leaves the session as it was.
 static int ragged_alloc(lnb_session* s) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
-  const size_t words = (size_t)s->max_rows * 3 + 16;   // + 8 segment last rows + 8 greedy tokens (host side)
+  const size_t words = row_map_words(s->max_rows);
   SsScratch x{};
   size_t sc_b, z_b, op_b;
   ss_plan(x, s->seq_len, s->max_rows, m->q_l / a.head_dim, a.head_dim, &sc_b, &z_b, &op_b);
@@ -2459,23 +2474,19 @@ static int ragged_alloc(lnb_session* s) {
   if (s->d_rag && !need_ss) return 0;
   const size_t asked = (s->d_rag ? 0 : words * 4) + (need_ss ? sc_b + z_b + op_b : 0);
   int32_t* d_rag = nullptr;
-  int32_t* h_rag = nullptr;
   cudaError_t e = cudaSuccess;
-  if (!s->d_rag) {
-    e = cudaMalloc((void**)&d_rag, words * 4);
-    if (e == cudaSuccess) e = cudaMallocHost((void**)&h_rag, words * 4);
-  }
+  if (!s->d_rag) e = cudaMalloc((void**)&d_rag, words * 4);
   if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.sc, sc_b);
   if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.z, z_b);
   if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.op, op_b);
   if (e != cudaSuccess) {
     cudaGetLastError();
-    cudaFree(d_rag); cudaFreeHost(h_rag); cudaFree(x.sc); cudaFree(x.z); cudaFree(x.op);
+    cudaFree(d_rag); cudaFree(x.sc); cudaFree(x.z); cudaFree(x.op);
     cudaGetLastError();
     return fail(LNB_ENOMEM, "ragged-call buffers: %zu bytes of device memory asked for (stream-attention scratch for %d rows: %zu): %s", asked,
                 x.rows, need_ss ? sc_b + z_b + op_b : (size_t)0, cudaGetErrorString(e));
   }
-  if (!s->d_rag) { s->d_rag = d_rag; s->h_rag = h_rag; }
+  if (d_rag) s->d_rag = d_rag;
   if (need_ss) {
     CU(cudaStreamSynchronize(s->stream));   // batched steps may still read the old scratch
     cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
@@ -2516,7 +2527,7 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
   if ((rc = ensure_logits(s, (size_t)n_segs))) return rc;
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward
   // [tokens | row_seq | row_pos | last row of each segment]: one pinned staging copy
-  int32_t* h = s->h_rag;
+  int32_t* h = s->h_tok;
   memcpy(h, tokens, (size_t)rows * 4);
   for (int i = 0, r = 0; i < n_segs; i++) {
     for (int k = 0; k < len[i]; k++, r++) {
@@ -2526,24 +2537,11 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
     h[3 * rows + i] = r - 1;
   }
   CU(cudaMemcpyAsync(s->d_rag, h, (size_t)(3 * rows + n_segs) * 4, cudaMemcpyHostToDevice, s->stream));
-  const RowMap rm{s->d_rag, s->d_rag + rows, s->d_rag + 2 * rows, s->d_rag + 3 * rows, n_segs};
-  // FAST prompts of >= 32 rows: one pass over the weights on the tensor cores; everything else: the GEMV chain
-  rc = (s->mode == LNB_ACC_FAST && forward_tc_ok(s, rows)) ? enqueue_forward_tc(s, rows, 0, false, &rm)
-                                                          : enqueue_forward(s, rows, false, 0, false, false, false, &rm);
-  if (rc) return rc;
-  s->last_was_engine = false;
-  {   // segments of sampled sequences: the sampler over their rows of s->logits, into d_next_arr
-    int32_t srow[8], sseq[8], spn[8];
-    int ns = 0;
-    for (int i = 0; i < n_segs; i++)
-      if (s->samp_on[seq[i]]) { srow[ns] = i; sseq[ns] = seq[i]; spn[ns] = start_pos[i] + len[i]; ns++; }
-    if (ns && (rc = launch_sample(s, ns, srow, sseq, spn, srow, s->d_next_arr, false))) return rc;
-  }
-  if (logits) CU(cudaMemcpyAsync(logits, s->logits, (size_t)n_segs * a.vocab_size * 4, cudaMemcpyDeviceToHost, s->stream));
-  int32_t* npin = s->h_rag + (size_t)s->max_rows * 3 + 8;
-  if (argmax_out) CU(cudaMemcpyAsync(npin, s->d_next_arr, (size_t)n_segs * 4, cudaMemcpyDeviceToHost, s->stream));
-  if ((rc = sync_stream(s))) return rc;
-  if (argmax_out) memcpy(argmax_out, npin, (size_t)n_segs * 4);
+  if ((rc = enqueue_forward(s, rows_ragged(s, rows, n_segs)))) return rc;
+  int32_t p_next[8];
+  for (int i = 0; i < n_segs; i++) p_next[i] = start_pos[i] + len[i];
+  if ((rc = call_tail(s, n_segs, 0, seq, p_next, s->d_next_arr, logits, n_segs, argmax_out ? s->d_next_arr : nullptr))) return rc;
+  if (argmax_out) memcpy(argmax_out, s->h_out, (size_t)n_segs * 4);
   return 0;
 }
 
@@ -2569,18 +2567,18 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     CU(cudaEventRecord(s->ev0, s->stream));
     if ((rc = engine_launch(s, n_steps, true))) return rc;
     CU(cudaEventRecord(s->ev1, s->stream));
-    CU(cudaMemcpyAsync(s->h_pin + s->max_rows + 8, s->d_tok_out, (size_t)n_steps * 4, cudaMemcpyDeviceToHost, s->stream));
+    CU(cudaMemcpyAsync(s->h_out, s->d_tok_out, (size_t)n_steps * 4, cudaMemcpyDeviceToHost, s->stream));
     if ((rc = sync_stream(s))) return rc;
     float ms = 0.f;
     CU(cudaEventElapsedTime(&ms, s->ev0, s->ev1));
     if (ms_out) *ms_out = ms;
-    if (tokens_out) memcpy(tokens_out, s->h_pin + s->max_rows + 8, (size_t)n_steps * 4);
+    if (tokens_out) memcpy(tokens_out, s->h_out, (size_t)n_steps * 4);
     return use_graph ? 1 : 0;   // (no graph is needed: there is nothing left to replay)
   }
   if (samp && (rc = ensure_logits(s, 1))) return rc;
   if (s->graph_tried && (s->graph_sampled != samp || (samp && s->graph_logits != s->logits))) drop_graph(s);
   auto step = [&]() -> int {
-    const int r = enqueue_forward(s, 1, true, samp ? 1 : 0, true);
+    const int r = enqueue_forward(s, rows_single(s, 1, nullptr, samp ? 1 : 0, true, true));
     if (r || !samp) return r;
     const int32_t row = 0, seq = s->active_seq, pn = -1;
     return launch_sample(s, 1, &row, &seq, &pn, nullptr, nullptr, true);
@@ -2618,7 +2616,7 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     }
   }
   CU(cudaEventRecord(s->ev1, s->stream));
-  CU(cudaMemcpyAsync(s->h_pin + s->max_rows + 8, s->d_tok_out, (size_t)n_steps * 4, cudaMemcpyDeviceToHost, s->stream));
+  CU(cudaMemcpyAsync(s->h_out, s->d_tok_out, (size_t)n_steps * 4, cudaMemcpyDeviceToHost, s->stream));
   if ((rc = p2p_err_enqueue(s))) return rc;
   CU(cudaStreamSynchronize(s->stream));
   CU(cudaGetLastError());
@@ -2626,7 +2624,7 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
   float ms = 0.f;
   CU(cudaEventElapsedTime(&ms, s->ev0, s->ev1));
   if (ms_out) *ms_out = ms;
-  if (tokens_out) memcpy(tokens_out, s->h_pin + s->max_rows + 8, (size_t)n_steps * 4);
+  if (tokens_out) memcpy(tokens_out, s->h_out, (size_t)n_steps * 4);
   return graph ? 1 : 0;
 }
 

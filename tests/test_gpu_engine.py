@@ -30,11 +30,11 @@ def tiny(L):
     om.close()
 
 
-def _context(L, gm, seq, acc, engine: bool, **kw):
+def _context(L, gm, seq, acc, engine: bool, max_rows=8, **kw):
     old = os.environ.get("LNB_ENGINE")
     os.environ["LNB_ENGINE"] = "1" if engine else "0"      # read when the session first decodes
     try:
-        ctx = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(seq), max_rows=8, acc_mode=acc, **kw)
+        ctx = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(seq), max_rows=max_rows, acc_mode=acc, **kw)
         # force the probe now, while the variable is set
         gm.Transformer.forward_argmax(ctx, np.array([1], np.int32), 0)
     finally:
@@ -87,6 +87,28 @@ def test_engine_equals_kernel_chain_and_oracle(L, tiny, mode):
             assert [first] + list(a) == list(om.generate(prompt, seq, stop_ids=(10**9,)))
     finally:
         ce.close(); cc.close(); osess.close()
+
+
+def test_tensor_core_prompt_after_an_engine_step_reads_back_its_own_residual(L, tiny):
+    """The engine keeps its residual row as tagged words; a FAST prompt of >= 32 rows on the tensor cores that follows an
+    engine step must leave LNB_BUF_RESIDUAL holding the prompt's [S, dim] rows, equal to those of a session without the
+    engine."""
+    args, om, gm = tiny
+    acc, seq, S = L._capi.LNB_ACC_FAST, 48, 40
+    prompt = np.random.default_rng(11).integers(0, args["vocab_size"], size=S).astype(np.int32)
+    ce = _context(L, gm, seq, acc, True, max_rows=S)     # _context runs one S=1 step: on the engine here
+    cc = _context(L, gm, seq, acc, False, max_rows=S)
+    try:
+        assert ce.uses_engine() and not cc.uses_engine()
+        n0 = ce.launch_count()
+        te, le = gm.Transformer.forward_argmax(ce, prompt, 0, want_logits="last")
+        # the tensor-core path: set_state, gather_rows, 8 kernels per layer (sdpa_kernel at head_dim 32), the last row's GEMV
+        assert ce.launch_count() - n0 == 1 + 1 + 8 * args["n_layers"] + 1
+        tc, lc = gm.Transformer.forward_argmax(cc, prompt, 0, want_logits="last")
+        assert te == tc and np.array_equal(le, lc)
+        assert np.array_equal(ce.residual(S), cc.residual(S))
+    finally:
+        ce.close(); cc.close()
 
 
 def test_engine_follows_active_sequence_layer_limit_and_kept_logits(L, tiny):

@@ -594,10 +594,10 @@ def _ulps(got, exp):
 
 
 def _tc_launches(n_layers, S, all_rows):
-    """kernels enqueue_forward_tc launches for one forward on one GPU, plus the set_state_kernel of the call: gather_rows,
-    then per layer rmsnorm_x8, gemm_tc (wq|wk|wv), rope_kv, the attention kernel, gemm_tc (wo + residual), rmsnorm_x8,
-    gemm_tc (w1|w3 + SwiGLU), gemm_tc (w2 + residual); all-rows logits add rmsnorm_x8 + gemm_tc for rows < S - 1; the last
-    row's LM head GEMV"""
+    """kernels the tensor-core path (enqueue_forward_tc) launches for one forward on one GPU, plus the set_state_kernel of
+    the call: gather_rows, then per layer rmsnorm_x8, gemm_tc (wq|wk|wv), rope_kv, the attention kernel of launch_attention,
+    gemm_tc (wo + residual), rmsnorm_x8, gemm_tc (w1|w3 + SwiGLU), gemm_tc (w2 + residual); all-rows logits add
+    rmsnorm_x8 + gemm_tc for rows < S - 1; the last row's LM head GEMV"""
     return 1 + 1 + 8 * n_layers + (2 if all_rows and S > 1 else 0) + 1
 
 
@@ -609,9 +609,9 @@ def _kernel_env(monkeypatch, kernel):
 
 
 def test_tiny128_prefill_runs_the_tensor_core_path(L, tiny128, monkeypatch):
-    """the path the other tiny128 tests claim to cover is the one that runs: head_dim 128 selects the sdpa_tc_kernel branch
-    of enqueue_forward_tc, the launch count of one forward is that function's, and LNB_SDPA_TC=0 (sdpa_prefill_kernel) gives
-    different bits"""
+    """the path the other tiny128 tests claim to cover is the one that runs: on the tensor-core path (enqueue_forward_tc),
+    head_dim 128 selects the sdpa_tc_kernel branch of launch_attention, the launch count of one forward is that path's, and
+    LNB_SDPA_TC=0 (sdpa_prefill_kernel) gives different bits"""
     args, _, _, gm = tiny128
     monkeypatch.delenv("LNB_SDPA_TC", raising=False)
     assert args["head_dim"] == 128
