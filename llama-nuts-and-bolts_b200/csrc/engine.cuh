@@ -842,7 +842,9 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) decode_engine_kernel(const Eng
           uint16_t* sV = sK + (size_t)T_max * kstride;
           double* sE = reinterpret_cast<double*>(sV + (size_t)T_max * hd);
           float* sP = reinterpret_cast<float*>(sE + (size_t)T_max);
-          float* sQ = sP + (size_t)T_max;
+          // the query is stored as float4, so it starts on a 16-byte boundary: sE and sP take 12 * T_max bytes, which left sQ
+          // misaligned whenever T_max % 4 != 0 (eng_sdpa_smem's slack covers the padding)
+          float* sQ = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(sP + (size_t)T_max) + 15) & ~(uintptr_t)15);
           double* sZ = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(sQ + (size_t)hd) + 15) & ~(uintptr_t)15);
           // rows of earlier positions come from the cache (complete since the previous step's grid barrier); this step's
           // k / v row and the query head come from the tagged q | k | v vector the projection phase is writing right now

@@ -157,3 +157,85 @@ def test_8b_fast_tensor_core_prefill_all_rows(L, big):
     print(f"8B prefill S={S}: oracle {t_oracle:.1f} s, max-abs per row: max {per_row.max():.4f}, median {np.median(per_row):.4f}")
     assert nxt == int(np.argmax(got[-1]))
     assert per_row.max() <= PREFILL_136_MAX_ABS, (int(per_row.argmax()), float(per_row.max()))
+
+
+# ---- the engines at the 8B shapes, against the kernel chain (pinned to the oracle above) ---------------------------------
+ENGINE_SEQ = 145      # the longest SequenceLength the engines accept at head_dim 128 with 4 query heads per KV head
+
+
+def _engine_context(L, gm, acc, engine, max_rows=8, n_seq=1):
+    import os
+    old = os.environ.get("LNB_ENGINE")
+    os.environ["LNB_ENGINE"] = "1" if engine else "0"       # read at the session's first decode
+    try:
+        ctx = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(ENGINE_SEQ), max_rows=max_rows, acc_mode=acc,
+                                       n_seq=n_seq)
+        gm.Transformer.forward_argmax(ctx, np.array([1], np.int32), 0)
+    finally:
+        if old is None:
+            os.environ.pop("LNB_ENGINE", None)
+        else:
+            os.environ["LNB_ENGINE"] = old
+    return ctx
+
+
+@pytest.mark.parametrize("mode", ["strict", "fast"])
+def test_8b_batch_engine_equals_the_batched_chain(L, big, mode, monkeypatch):
+    """8 sequences with prompts of 8 .. 136 tokens, batched steps until the longest reaches position 144: every step's logits
+    and tokens, and the caches of layers 0 and 31, of the batch engine equal those of the batched kernel chain"""
+    monkeypatch.delenv("LNB_BATCH_TC", raising=False)
+    args, om, gm = big[:3]
+    acc = L._capi.LNB_ACC_STRICT if mode == "strict" else L._capi.LNB_ACC_FAST
+    rng = np.random.default_rng(8)
+    lens = (136, 8, 40, 100, 17, 64, 9, 121)
+    prompts = [rng.integers(0, args["vocab_size"], size=k).astype(np.int32) for k in lens]
+    ce = _engine_context(L, gm, acc, True, max_rows=136, n_seq=8)
+    cc = _engine_context(L, gm, acc, False, max_rows=136, n_seq=8)
+    try:
+        cur, pos = [], []
+        for i, p in enumerate(prompts):
+            got = []
+            for ctx in (ce, cc):
+                ctx.set_active_sequence(i)
+                got.append(gm.Transformer.forward_argmax(ctx, p, 0))
+            assert got[0][0] == got[1][0]
+            cur.append(got[0][0]); pos.append(len(p))
+        while max(pos) < ENGINE_SEQ:
+            l0 = ce.launch_count()
+            te, le = ce.forward_batch(cur, pos, want_logits=True)
+            assert ce.launch_count() - l0 == 1, "the batch engine did not run"
+            tc, lc = cc.forward_batch(cur, pos, want_logits=True)
+            assert np.array_equal(le, lc), f"positions {pos}"
+            assert list(te) == list(tc)
+            cur = [int(t) for t in te]; pos = [p + 1 for p in pos]
+        for i in range(8):
+            ce.set_active_sequence(i); cc.set_active_sequence(i)
+            for layer in (0, 31):
+                assert np.array_equal(ce.CacheK(layer).RawData[:pos[i]], cc.CacheK(layer).RawData[:pos[i]]), (i, layer)
+                assert np.array_equal(ce.CacheV(layer).RawData[:pos[i]], cc.CacheV(layer).RawData[:pos[i]]), (i, layer)
+    finally:
+        ce.close(); cc.close()
+
+
+def test_8b_fast_decode_engine_equals_the_fast_chain(L, big):
+    """LNB_ENGINE=1 in FAST: ten host-driven steps up to position 144 equal the FAST kernel chain's, logits and tokens"""
+    args, om, gm = big[:3]
+    acc = L._capi.LNB_ACC_FAST
+    prompt = np.random.default_rng(135).integers(0, args["vocab_size"], size=135).astype(np.int32)
+    ce = _engine_context(L, gm, acc, True, max_rows=135)
+    cc = _engine_context(L, gm, acc, False, max_rows=135)
+    try:
+        assert ce.uses_engine() and not cc.uses_engine()
+        te, _ = gm.Transformer.forward_argmax(ce, prompt, 0)
+        tc, _ = gm.Transformer.forward_argmax(cc, prompt, 0)
+        assert te == tc
+        for p in range(135, ENGINE_SEQ):
+            x = np.array([te], np.int32)
+            te, le = gm.Transformer.forward_argmax(ce, x, p, want_logits="last")
+            tc, lc = gm.Transformer.forward_argmax(cc, x, p, want_logits="last")
+            assert np.array_equal(le, lc), f"position {p}"
+            assert te == tc
+        for layer in (0, 31):
+            assert np.array_equal(ce.CacheK(layer).RawData[:ENGINE_SEQ], cc.CacheK(layer).RawData[:ENGINE_SEQ])
+    finally:
+        ce.close(); cc.close()

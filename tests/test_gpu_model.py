@@ -317,12 +317,21 @@ def check_batched_decode(L, model, mode):
     seq, nseq = 32, 5
     prompts = [rng.integers(0, args["vocab_size"], size=k).astype(np.int32) for k in (3, 8, 1, 6, 8)]
     ctx = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(seq), max_rows=8, acc_mode=acc, n_seq=nseq)
+    # FAST on the FMA pipe: every batched row must equal its sequence's own S=1 forward on the kernel chain (a single-GPU FAST
+    # session's S=1 default); the tensor-core form's order is the hardware's and keeps the tolerance
+    own = None
+    if mode == "fast":
+        own = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(seq), max_rows=8, acc_mode=acc, n_seq=nseq)
     osess = [om.new_session(seq) for _ in range(nseq)]
     try:
         cur, pos = [], []
         for i, p in enumerate(prompts):                      # prefill every sequence through the ordinary Forward
             ctx.set_active_sequence(i)
             nxt, lg = gm.Transformer.forward_argmax(ctx, p, 0, want_logits="last")
+            if own is not None:
+                own.set_active_sequence(i)
+                assert not own.uses_engine()
+                assert np.array_equal(gm.Transformer.forward_argmax(own, p, 0, want_logits="last")[1], lg)
             exp = osess[i].forward(p, 0, all_rows=False)
             if mode == "strict":
                 assert np.array_equal(lg, exp)
@@ -337,6 +346,11 @@ def check_batched_decode(L, model, mode):
                     assert nxt[i] == O.argmax_f32(exp[0])
                 else:
                     assert np.abs(lg[i] - exp[0]).max() <= 1e-2
+                if own is not None:
+                    own.set_active_sequence(i)
+                    t1, l1 = gm.Transformer.forward_argmax(own, np.array([cur[i]], np.int32), pos[i], want_logits="last")
+                    assert np.array_equal(lg[i], l1[0]), f"sequence {i} step {step}: batched row != its own S=1 forward"
+                    assert nxt[i] == t1
                 cur[i] = int(np.argmax(exp[0])); pos[i] += 1   # teacher-forced with the oracle's token
         if mode == "strict":
             for i in range(nseq):                            # caches of every sequence, all layers
@@ -351,6 +365,8 @@ def check_batched_decode(L, model, mode):
             ctx.set_active_sequence(nseq)
     finally:
         ctx.close()
+        if own is not None:
+            own.close()
         for o in osess:
             o.close()
 
