@@ -6,6 +6,8 @@
 // batch=N slots=K: the same N prompts through K live sequences with continuous batching (inference::GenerateTokensContinuous).
 // temp=T [top_k=K] [top_p=P] [seed=S]: seeded sampling instead of the greedy argmax (lnb_session_set_sampling); prompt b of a
 // batch samples with seed S + b.
+// spec=K: speculative decoding -- each call verifies the last token plus up to K prompt-lookup drafts in one pass over the
+// weights (lnb_forward_speculative); the generated ids are the same as without it.  Not with slots=.
 // prompt=TEXT (with <modelDir>/tokenizer.model): TEXT goes through the chat template and the BPE tokenizer, the
 // generated ids come back as text (cmd/main.go's flow without the console UI).
 // <modelDir> holds params.json + consolidated.00.pth (model.LoadModel, src/model/loader.go:18-70);
@@ -106,7 +108,9 @@ int main(int argc, char** argv) {
     int batch = 0, slots = 0;
     const char* prompt_text = nullptr;
     model::SamplingArgs sampling;   // temp= top_k= top_p= seed= (temp 0, the default: greedy)
+    model::SpeculativeArgs spec;    // spec=K: speculative decoding with up to K prompt-lookup drafts per call (0: plain steps)
     for (int i = 1; i < argc; i++) {
+      if (!strncmp(argv[i], "spec=", 5)) spec.MaxDraft = atoi(argv[i] + 5);
       if (!strncmp(argv[i], "batch=", 6)) batch = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "slots=", 6)) slots = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "prompt=", 7)) prompt_text = argv[i] + 7;
@@ -125,6 +129,8 @@ int main(int argc, char** argv) {
       vocab = tokenizer->GetVocabulary();
       prompt = tokenizer->Tokenize({{"user", prompt_text}});
     }
+    const model::SpeculativeArgs* speculative = spec.MaxDraft > 0 ? &spec : nullptr;
+    if (speculative && slots > 0) throw Error("spec= is not built for continuous batching (slots=)");
     if (batch > 0) {
       const int mod = transformer.args.vocab_size < 128256 ? 1000 : 128000;
       std::vector<std::vector<int32_t>> prompts(batch, prompt);
@@ -134,7 +140,7 @@ int main(int argc, char** argv) {
       auto b0 = std::chrono::steady_clock::now();
       auto collect = [&](int seq, inference::GenerationState, int32_t tok) { outs[seq].push_back(tok); };
       if (slots > 0) inference::GenerateTokensContinuous(transformer, vocab, seq_len, acc, prompts, slots, std::max(slots, 64), collect, &sampling);
-      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling);
+      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling, speculative);
       const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - b0).count();
       size_t total = 0;
       for (int b = 0; b < batch; b++) {
@@ -152,7 +158,7 @@ int main(int argc, char** argv) {
     inference::GenerateTokens(transformer, vocab, seq_len, acc, prompt, [&](inference::GenerationState, int32_t tok) {
       if (out.empty()) t_first = std::chrono::steady_clock::now();
       out.push_back(tok);
-    }, &sampling);
+    }, &sampling, speculative);
     auto t1 = std::chrono::steady_clock::now();
     if (tokenizer) printf("text: %s\n", tokenizer->TokenBatchToString(out).c_str());
     printf("tokens:");

@@ -289,6 +289,29 @@ struct SamplingArgs {
   SamplingArgs ForPrompt(int i) const { SamplingArgs a = *this; a.Seed += (uint64_t)i; return a; }
 };
 
+// EXTENSION: speculative decoding (lnb_forward_speculative) with prompt-lookup drafts of up to MaxDraft tokens
+struct SpeculativeArgs {
+  int MaxDraft = 0;
+  int NgramMax = 3;
+  int NgramMin = 1;
+};
+
+// Prompt-lookup drafter (the Python mirror's prompt_lookup_drafts), a pure function of the history h[0..L) whose last token
+// is about to be fed: for n = ngramMax down to ngramMin, the largest j with j + n < L and h[j..j+n) == h[L-n..L); the first n
+// that matches gives the drafts h[j+n .. min(j+n+maxDraft, L)).  No match gives no drafts.
+inline std::vector<int32_t> PromptLookupDrafts(const std::vector<int32_t>& h, int maxDraft, int ngramMax = 3, int ngramMin = 1) {
+  const int L = (int)h.size();
+  if (maxDraft <= 0) return {};
+  for (int n = ngramMax; n >= std::max(ngramMin, 1); n--) {
+    if (L < n + 1) continue;
+    for (int j = L - n - 1; j >= 0; j--) {
+      if (!std::equal(h.begin() + j, h.begin() + j + n, h.begin() + (L - n))) continue;
+      return std::vector<int32_t>(h.begin() + j + n, h.begin() + std::min(j + n + maxDraft, L));
+    }
+  }
+  return {};
+}
+
 class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
  public:
   int SequenceLength;
@@ -334,6 +357,23 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
       flat.insert(flat.end(), s.tokens.begin(), s.tokens.end());
     }
     check(lnb_forward_ragged(h_, (int)segs.size(), seq.data(), start.data(), len.data(), flat.data(), nullptr, next.data()));
+    return next;
+  }
+  // EXTENSION (speculative verification, lnb_forward_speculative): segment tokens = the sequence's last emitted token + drafts,
+  // row j at startPos + j.  -> next token of every row; accepted[i] = drafts of segment i the model agrees with (segment i
+  // emits the next tokens of its rows 0 .. accepted[i])
+  std::vector<int32_t> ForwardSpeculative(const std::vector<Segment>& segs, std::vector<int32_t>& accepted) {
+    std::vector<int32_t> seq, start, n_draft, flat;
+    for (const Segment& s : segs) {
+      seq.push_back(s.seq);
+      start.push_back(s.startPos);
+      n_draft.push_back((int32_t)s.tokens.size() - 1);
+      flat.insert(flat.end(), s.tokens.begin(), s.tokens.end());
+    }
+    std::vector<int32_t> next(flat.size(), -1);
+    accepted.assign(segs.size(), 0);
+    check(lnb_forward_speculative(h_, (int)segs.size(), seq.data(), start.data(), n_draft.data(), flat.data(), nullptr, next.data(),
+                                  accepted.data()));
     return next;
   }
   int MaxRows() const { return maxRows_; }
@@ -385,10 +425,56 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
 namespace inference {  // ---- src/inference ------------------------------------------------------------------
 enum GenerationState { GSInProgress = 0, GSFinishedByReachingEOS = 1, GSFinishedByReachingSeqLen = 2 };
 
+// The speculative loop of the Python mirror's _generate_speculative: hists[i] = the tokens of sequence i so far, its last one
+// emitted and fed next (at position size - 1); every live sequence gets a row per call, the rest of min(8, maxRows) rows go to
+// prompt-lookup drafts in sequence order, no row past position SequenceLength - 2; the accepted tokens are emitted one at a
+// time through the stop logic of generateTokensInternal (inference.go:218-248).  emit(sequence, state, token).
+inline void GenerateSpeculative(model::InferenceContext& infContext, const model::Vocabulary& vocab,
+                                std::vector<std::vector<int32_t>>& hists, std::vector<int> live, const model::SpeculativeArgs& spec,
+                                const std::function<void(int, GenerationState, int32_t)>& emit) {
+  const int seqLen = infContext.SequenceLength;
+  const int budget = std::min(8, infContext.MaxRows());
+  if ((int)live.size() > budget) throw Error("more live sequences than rows in a speculative call");
+  while (!live.empty()) {
+    int left = budget - (int)live.size();
+    std::vector<model::InferenceContext::Segment> segs;
+    for (int i : live) {
+      const int pos = (int)hists[i].size() - 1;
+      std::vector<int32_t> toks{hists[i].back()};
+      const std::vector<int32_t> d =
+          model::PromptLookupDrafts(hists[i], std::min({spec.MaxDraft, left, seqLen - 2 - pos}), spec.NgramMax, spec.NgramMin);
+      left -= (int)d.size();
+      toks.insert(toks.end(), d.begin(), d.end());
+      segs.push_back({i, pos, toks});
+    }
+    std::vector<int32_t> accepted;
+    const std::vector<int32_t> next = infContext.ForwardSpeculative(segs, accepted);
+    std::vector<int> still;
+    int r0 = 0;
+    for (size_t k = 0; k < segs.size(); k++) {
+      const int i = segs[k].seq;
+      bool finished = false;
+      for (int j = 0; j <= accepted[k] && !finished; j++) {
+        const int32_t tok = next[r0 + j];
+        const int curPos = segs[k].startPos + 1 + j;
+        hists[i].push_back(tok);
+        bool eos = false;
+        for (int32_t s : vocab.StopTokenIds) eos |= (s == tok);
+        const GenerationState st = eos ? GSFinishedByReachingEOS : (curPos + 1 == seqLen ? GSFinishedByReachingSeqLen : GSInProgress);
+        emit(i, st, tok);
+        finished = st != GSInProgress;
+      }
+      r0 += (int)segs[k].tokens.size();
+      if (!finished) still.push_back(i);
+    }
+    live = still;
+  }
+}
+
 // generateTokensInternal (inference.go:173-254); `emit` plays generatedTokensCh
 inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                            const std::vector<int32_t>& promptTokens, const std::function<void(GenerationState, int32_t)>& emit,
-                           const model::SamplingArgs* sampling = nullptr) {
+                           const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr) {
   // the prefill call carries the whole prompt: size the session's row buffers for it
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max<int>(8, (int)promptTokens.size()));
   const bool samples = sampling && sampling->Samples();
@@ -421,6 +507,11 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
     if (eos) { emit(GSFinishedByReachingEOS, nextTokenId); break; }                 // :233-240
     if (curPos + 1 == infContext.SequenceLength) { emit(GSFinishedByReachingSeqLen, nextTokenId); break; }
     emit(GSInProgress, nextTokenId);
+    if (speculative) {   // EXTENSION: the prompt is in the cache; from here on every call verifies drafts (same stream)
+      std::vector<std::vector<int32_t>> hists{std::vector<int32_t>(tokens.begin(), tokens.begin() + curPos + 1)};
+      GenerateSpeculative(infContext, vocab, hists, {0}, *speculative, [&](int, GenerationState st, int32_t tok) { emit(st, tok); });
+      break;
+    }
   }
 }
 
@@ -430,7 +521,7 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
 inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                                 const std::vector<std::vector<int32_t>>& prompts,
                                 const std::function<void(int, GenerationState, int32_t)>& emit,
-                                const model::SamplingArgs* sampling = nullptr) {
+                                const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr) {
   const int n = (int)prompts.size();
   if (n < 1) throw Error("empty prompt batch");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, n), n);
@@ -458,6 +549,17 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
   for (int i = 0; i < n; i++) {                           // prefill on sequence i's cache
     infContext.SetActiveSequence(i);
     record(i, infContext.ForwardArgmax(prompts[i], 0), (int)prompts[i].size());
+  }
+  if (speculative) {   // EXTENSION: one lnb_forward_speculative per call, a row per unfinished sequence, drafts in the rest
+    std::vector<std::vector<int32_t>> hists(n);
+    std::vector<int> live;
+    for (int i = 0; i < n; i++) {
+      hists[i] = prompts[i];
+      hists[i].push_back(cur[i]);
+      if (!done[i]) live.push_back(i);
+    }
+    GenerateSpeculative(infContext, vocab, hists, live, *speculative, emit);
+    return;
   }
   while (n_done < n) {
     // finished sequences are stepped again at their last position (a no-op for their state)

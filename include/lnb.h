@@ -258,6 +258,28 @@ int lnb_session_set_chunked_prefill(lnb_session* s, int on);
 int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq, const int32_t* start_pos, const int32_t* len,
                        const int32_t* tokens, float* logits, int32_t* argmax_out);
 
+/* EXTENSION: speculative verification.  Segment i = sequence seq[i], rows at positions start_pos[i] .. start_pos[i] + n_draft[i]:
+ * row 0 feeds the sequence's last emitted token, rows 1.. feed the drafts (tokens: segment after segment, 1 + n_draft[i] ids each).
+ * next_out[r] = the next token of row r (greedy, or sampled with p_next = its position + 1); n_accepted[i] = the largest a with
+ * next_out[row j] == draft j+1 for all j < a.  The emitted tokens of segment i are next_out[its rows 0 .. a].
+ * logits: NULL or host [rows, vocab].
+ *   valid: any session (single or batch); 1 <= n_segs <= n_seq; seq[] distinct, in [0, n_seq); n_draft[i] >= 0;
+ *   start_pos[i] >= 0, start_pos[i] + n_draft[i] < seq_len; total rows <= min(8, max_rows); token ids in range.  Anything
+ *   else, and tp_size > 1 (not built), is LNB_EINVAL with nothing enqueued.  next_out / n_accepted may be NULL.
+ *   Every row gets the arithmetic of its sequence's own S=1 Forward at its position: LNB_ACC_STRICT rows are bit-identical
+ *   to it (and to the reference); LNB_ACC_FAST rows too on the batch engine's default form and, beyond the engines' limit,
+ *   within the shared-memory decode kernel's fit (351 positions at head_dim 128).  Beyond that fit, and with
+ *   LNB_BATCH_TC=1, FAST rows have the bits lnb_forward_batch gives those rows.  So a speculative stream is the plain stream.
+ *   Routing: one row (one segment, no draft) is the ordinary S=1 step; >= 2 rows run ONE batch-engine launch when the session
+ *   can run the engines (LNB_BATCH_ENGINE=0 opts out), else the kernel chain.
+ *   Stale cache rows: the K/V rows of rejected drafts (positions start_pos + a + 1 and above) hold the drafts' keys and
+ *   values.  Nothing reads them before the next call at start_pos + a + 1 overwrites them.
+ *   Afterwards a lnb_forward_device handle is stale; the active sequence and a captured decode graph are unchanged (except
+ *   that the first sampled call of more rows than the session has sequences grows the sampler's scratch, LNB_ENOMEM with the
+ *   bytes on failure, and re-captures a sampled decode graph). */
+int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t* seq, const int32_t* start_pos, const int32_t* n_draft,
+                            const int32_t* tokens, float* logits, int32_t* next_out, int32_t* n_accepted);
+
 /* Device-resident greedy decode: runs n_steps consecutive S=1 forwards starting with
  * `first_token` at position start_pos, feeding each argmax back on the device (no host
  * sync inside), optionally as CUDA-graph replays.  tokens_out[n_steps]; ms_out = device

@@ -1129,8 +1129,9 @@ struct lnb_session {
   // sequence in device memory (a captured graph reads them there), the weights of up to n_seq rows, the sampled token of
   // a single-sequence forward (st->next_token keeps the greedy one)
   lnb_sampling* d_samp = nullptr;           // [n_seq]
-  unsigned long long* d_samp_w = nullptr;   // [n_seq][vocab]
-  unsigned long long* d_samp_cand = nullptr;   // [n_seq][SMP_MERGE] split-sampler candidates, then [n_seq] u32 counters
+  unsigned long long* d_samp_w = nullptr;   // [samp_rows][vocab]
+  unsigned long long* d_samp_cand = nullptr;   // [samp_rows][SMP_MERGE] split-sampler candidates, then [samp_rows] u32 counters
+  int samp_rows = 0;                        // rows one sampler launch may draw: n_seq, grown by speculative calls (samp_grow)
   int32_t* d_samp_tok = nullptr;
   bool samp_on[8] = {false, false, false, false, false, false, false, false};
   bool graph_sampled = false;               // the captured decode graph ends in the sampler ...
@@ -1702,14 +1703,18 @@ static int engine_fault(lnb_session* s, cudaError_t e) {
 }
 
 // ---- batch engine (engine_batch.cuh): one launch advances all sequences of a batched session by one token -------------------
-static bool batch_engine_ok(lnb_session* s) {
-  if (s->n_seq < 2 || !engine_capable(s)) return false;
+static bool batch_engine_usable(lnb_session* s) {
+  if (!engine_capable(s)) return false;
   const lnb_model_args& a = s->m->a;
   if ((size_t)a.dim * 4 > 16 * 1024) return false;                      // norm weights as f32 in 16 KB of shared memory
   const char* e = getenv("LNB_BATCH_ENGINE");
   if (e && !strcmp(e, "0")) return false;
   return true;
 }
+static bool batch_engine_ok(lnb_session* s) { return s->n_seq >= 2 && batch_engine_usable(s); }
+// speculative verification: a call of >= 2 rows runs the batch engine, single-sequence sessions included (engine_capable
+// already holds every position below the engine's limit, eng_sdpa_smem)
+static bool spec_engine_ok(lnb_session* s, int rows) { return rows >= 2 && batch_engine_usable(s); }
 static int batch_engine_build(lnb_session* s, const float* logits_out) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
@@ -1809,8 +1814,8 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
   s->bkey_layers = n_layers; s->bkey_logits = logits_out;
   return 0;
 }
-// tokens / positions of the n sequences are already in s->d_tokens / s->d_pos_arr
-static int batch_engine_launch(lnb_session* s, int n) {
+// n rows: token tokens[m] at position pos_arr[m] on the cache of sequence row_seq[m] (NULL: sequence m), already on the device
+static int batch_engine_launch(lnb_session* s, int n, const int32_t* tokens, const int32_t* pos_arr, const int32_t* row_seq) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   BatchParams P{};
@@ -1818,7 +1823,7 @@ static int batch_engine_launch(lnb_session* s, int n) {
   P.emb = m->tok_embd; P.dim = a.dim; P.head_dim = a.head_dim; P.n_rep = a.n_heads / a.n_kv_heads; P.seq_len = s->seq_len;
   P.cis = m->cis; P.silu_tab = m->silu_tab; P.eps = a.norm_eps; P.attn_scale = attn_scale_bf16(a.head_dim);
   P.strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
-  P.tokens = s->d_tokens; P.pos_arr = s->d_pos_arr; P.cache_seq_stride = (long long)s->seq_len * m->kv_l;
+  P.tokens = tokens; P.pos_arr = pos_arr; P.row_seq = row_seq; P.cache_seq_stride = (long long)s->seq_len * m->kv_l;
   P.rscale = s->rs; P.keys = s->d_bkeys; P.next_arr = s->d_next_arr; P.bar_ctr = s->d_bar;
   P.p2p = s->p2p; P.tp = m->tp_size;
   P.timeout_ns = p2p_timeout_ns();
@@ -1851,8 +1856,9 @@ static int enqueue_decode_engine(lnb_session* s, int32_t token, int start_pos, i
 }
 
 // The rows of one forward: where row r's token, position and KV cache come from, and what the LM head makes of them.
-// rows_single, rows_batch and rows_ragged are the only places that decide this; the forward builders read it from here.
-enum RowsKind { ROWS_SINGLE, ROWS_BATCH, ROWS_RAGGED };
+// rows_single, rows_batch, rows_ragged and rows_spec are the only places that decide this; the forward builders read it from
+// here.
+enum RowsKind { ROWS_SINGLE, ROWS_BATCH, ROWS_RAGGED, ROWS_SPEC };
 // what the LM head produces: the last row's greedy token with no logits kept, the last row's or every row's (NONE, LAST,
 // ALL); or, for output rows that each end their own sequence, the logits and a greedy token in d_next_arr per row (PER_ROW)
 enum RowsHead { HEAD_NONE, HEAD_LAST, HEAD_ALL, HEAD_PER_ROW };
@@ -1861,7 +1867,7 @@ struct Rows {
   int S;
   const int32_t* tokens;    // device token id of each row, or NULL: st->next_token (a device-driven decode step)
   const int32_t* pos_arr;   // device position of each row, or NULL: st->pos + r
-  const int32_t* row_seq;   // ragged: the sequence of each row
+  const int32_t* row_seq;   // ragged, speculative: the sequence of each row
   size_t cache_off;         // elements to the cache every row addresses (the active sequence's), or 0
   long long seq_stride;     // rows on several caches: elements between consecutive sequences' caches, else 0
   int mb_rows;              // launch_gemv's mb_rows: ragged 8, else 0
@@ -1900,6 +1906,16 @@ static Rows rows_ragged(const lnb_session* s, int rows, int n_segs) {
   R.head = HEAD_PER_ROW; R.head_rows = n_segs;
   return R;
 }
+// a speculative verification call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each; consecutive
+// rows of a segment are consecutive positions of one sequence, and EVERY row is an output row (its next token is compared
+// with the following draft), so the LM head runs over all of them
+static Rows rows_spec(const lnb_session* s, int rows) {
+  Rows R{};
+  R.kind = ROWS_SPEC; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
+  R.seq_stride = (long long)s->seq_len * s->m->kv_l;
+  R.head = HEAD_PER_ROW; R.head_rows = rows;
+  return R;
+}
 
 // Attention of layer l for the rows R (queries in s->q), written to out: plain rows, or the X8 operand of the tensor-core
 // Wo GEMM (out_x8).  Ragged rows always stream, so a ragged call has one attention path whatever the session's other calls
@@ -1912,7 +1928,9 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
   const int32_t* pos_ptr = &s->st->pos;
   const float scale = attn_scale_bf16(a.head_dim);
   const int strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
-  const bool batched = R.kind == ROWS_BATCH;
+  // rows on a row -> position map (a batched step, or a speculative call whose rows follow each other in one sequence's
+  // cache): the decode kernel within its fit, else the streamed kernels -- the attention a batched step of those rows runs
+  const bool batched = R.kind == ROWS_BATCH || R.kind == ROWS_SPEC;
   auto streamed = [&]() {
     StreamAttn P{};
     P.q = s->q; P.ldq = m->q_l;
@@ -1928,7 +1946,7 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
   if (!out_x8 && (S == 1 || batched) && s->sdpa_smem_decode)
     return launch_kernel(L, sdpa_decode_kernel, dim3(n_kv, S), dim3(128 * n_rep), s->sdpa_decode_smem, (const uint16_t*)s->q, ck, cv,
                          m->kv_l, n_rep, a.head_dim, out, pos_ptr, s->seq_len, strict, scale, R.pos_arr,
-                         (long long)s->seq_len * m->kv_l, m->q_l, (const LnbDevState*)s->st);
+                         (long long)s->seq_len * m->kv_l, m->q_l, (const LnbDevState*)s->st, R.row_seq);
   if (out_x8 && a.head_dim == SP_HD) {
     const double* exp_tab = sdpa_tc_enabled() ? exp_table_device() : nullptr;
     if (exp_tab)
@@ -2170,7 +2188,7 @@ static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_
   SampleJob J{};
   J.logits = s->logits; J.ld = s->m->vocab_l; J.V = s->m->a.vocab_size; J.n = n;
   J.params = s->d_samp; J.wbuf = s->d_samp_w; J.pos_ptr = &s->st->pos; J.out = out;
-  J.cand = s->d_samp_cand; J.cnt = reinterpret_cast<unsigned int*>(s->d_samp_cand + (size_t)s->n_seq * SMP_MERGE);
+  J.cand = s->d_samp_cand; J.cnt = reinterpret_cast<unsigned int*>(s->d_samp_cand + (size_t)s->samp_rows * SMP_MERGE);
   J.st = decode ? s->st : nullptr; J.tok_out = decode ? s->d_tok_out : nullptr;
   for (int i = 0; i < n; i++) {
     J.row[i] = row[i]; J.slot[i] = seq[i]; J.p_next[i] = p_next[i]; J.out_idx[i] = out_idx ? out_idx[i] : 0;
@@ -2409,6 +2427,7 @@ extern "C" int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampl
       return fail(LNB_ENOMEM, "sampler buffers: %zu bytes of device memory asked for: %s", b_par + b_w + 16 + b_cand, cudaGetErrorString(e));
     }
     s->d_samp = d_par; s->d_samp_w = d_w; s->d_samp_tok = d_tok; s->d_samp_cand = d_cand;
+    s->samp_rows = s->n_seq;
   }
   if (on) {   // stream-ordered, no host synchronisation; a captured decode graph reads the slot when it replays
     sample_set_params_kernel<<<1, 1, 0, s->stream>>>(s->d_samp + seq, *p);
@@ -2446,7 +2465,7 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
   if (batch_engine_ok(s)) {
     // ONE launch of the batch engine: every weight matrix streamed once for all n sequences
     if ((rc = batch_engine_build(s, (logits || samp) ? s->logits : nullptr))) return rc;
-    if ((rc = batch_engine_launch(s, n))) return rc;
+    if ((rc = batch_engine_launch(s, n, s->d_tokens, s->d_pos_arr, nullptr))) return rc;
     if (logits && (rc = gather_logits(s, 0, n))) return rc;
   } else {
     if (!s->sdpa_smem_decode && !s->ss.sc)
@@ -2542,6 +2561,121 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
   for (int i = 0; i < n_segs; i++) p_next[i] = start_pos[i] + len[i];
   if ((rc = call_tail(s, n_segs, 0, seq, p_next, s->d_next_arr, logits, n_segs, argmax_out ? s->d_next_arr : nullptr))) return rc;
   if (argmax_out) memcpy(argmax_out, s->h_out, (size_t)n_segs * 4);
+  return 0;
+}
+
+// ---- speculative verification: a sequence's last emitted token and k drafted tokens as k + 1 rows of ONE forward -------
+// Sampler scratch for one launch of `rows` rows (a speculative call may draw up to 8 rows of one sequence, more than the
+// session has sequences).  Nothing is replaced unless every allocation succeeded.  A captured decode graph that ends in the
+// sampler holds the old scratch: it is dropped and re-captured by the next lnb_decode_run.
+static int samp_grow(lnb_session* s, int rows) {
+  if (s->samp_rows >= rows) return 0;
+  const size_t b_w = (size_t)rows * s->m->a.vocab_size * 8, b_cand = (size_t)rows * (SMP_MERGE * 8 + 4);
+  unsigned long long *d_w = nullptr, *d_cand = nullptr;
+  cudaError_t e = cudaMalloc((void**)&d_w, b_w);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&d_cand, b_cand);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_cand, 0, b_cand, s->stream);   // the split sampler's counters start at 0
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(d_w); cudaFree(d_cand);
+    cudaGetLastError();
+    return fail(LNB_ENOMEM, "sampler scratch for %d rows: %zu bytes of device memory asked for: %s", rows, b_w + b_cand, cudaGetErrorString(e));
+  }
+  if (s->graph_sampled) drop_graph(s);
+  CU(cudaStreamSynchronize(s->stream));   // earlier sampler launches may still use the old scratch
+  cudaFree(s->d_samp_w); cudaFree(s->d_samp_cand);
+  s->d_samp_w = d_w; s->d_samp_cand = d_cand; s->samp_rows = rows;
+  return 0;
+}
+
+extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t* seq, const int32_t* start_pos, const int32_t* n_draft,
+                                       const int32_t* tokens, float* logits, int32_t* next_out, int32_t* n_accepted) {
+  if (!s || !seq || !start_pos || !n_draft || !tokens) return fail(LNB_EINVAL, "NULL argument");
+  lnb_model* m = s->m;
+  const lnb_model_args& a = m->a;
+  if (m->tp_size > 1) return fail(LNB_EINVAL, "lnb_forward_speculative is not built for tensor parallelism (tp_size %d)", m->tp_size);
+  if (n_segs < 1 || n_segs > s->n_seq) return fail(LNB_EINVAL, "n_segs %d must be in [1, %d] (the session's sequences)", n_segs, s->n_seq);
+  const int budget = std::min(8, s->max_rows);
+  bool used[8] = {false, false, false, false, false, false, false, false};
+  int64_t rows64 = 0;
+  for (int i = 0; i < n_segs; i++) {
+    if (seq[i] < 0 || seq[i] >= s->n_seq) return fail(LNB_EINVAL, "segment %d: sequence %d out of range (session has %d)", i, seq[i], s->n_seq);
+    if (used[seq[i]]) return fail(LNB_EINVAL, "segment %d: sequence %d has a segment already (one per sequence per call)", i, seq[i]);
+    used[seq[i]] = true;
+    if (n_draft[i] < 0) return fail(LNB_EINVAL, "segment %d: n_draft %d must be >= 0", i, n_draft[i]);
+    if (start_pos[i] < 0 || (int64_t)start_pos[i] + n_draft[i] >= s->seq_len)
+      return fail(LNB_EINVAL, "segment %d: positions [%d, %lld] exceed SequenceLength %d", i, start_pos[i],
+                  (long long)start_pos[i] + n_draft[i], s->seq_len);
+    rows64 += 1 + (int64_t)n_draft[i];
+  }
+  if (rows64 > budget)
+    return fail(LNB_EINVAL, "the segments carry %lld rows, more than min(8, max_rows) = %d", (long long)rows64, budget);
+  const int rows = (int)rows64;
+  for (int r = 0; r < rows; r++)
+    if (tokens[r] < 0 || tokens[r] >= a.vocab_size) return fail(LNB_EINVAL, "token id %d (row %d) out of range", tokens[r], r);
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(m->device));
+  int rc;
+  if (rows == 1) {
+    // no draft: the ordinary S=1 step of that sequence (the decode engine or the chain, same bits), so a call without drafts
+    // costs exactly a plain step
+    const int saved = s->active_seq;
+    s->active_seq = seq[0];
+    int32_t nxt = -1;
+    rc = forward_locked(s, tokens, 1, start_pos[0], logits != nullptr, false, logits, &nxt);
+    s->active_seq = saved;
+    if (rc) return rc;
+    if (next_out) next_out[0] = nxt;
+    if (n_accepted) n_accepted[0] = 0;
+    return 0;
+  }
+  const bool eng = spec_engine_ok(s, rows);
+  if (!eng && !s->sdpa_smem_decode && !s->ss.sc)
+    return fail(LNB_EINVAL, "speculative calls beyond the shared-memory attention kernel need head_dim <= 128 and n_rep <= 8");
+  int32_t row_seq[8], row_pos[8];
+  bool samp = false;
+  for (int i = 0, r = 0; i < n_segs; i++)
+    for (int k = 0; k <= n_draft[i]; k++, r++) {
+      row_seq[r] = seq[i];
+      row_pos[r] = start_pos[i] + k;
+      samp |= s->samp_on[seq[i]];
+    }
+  if (!s->d_rag) {   // the row map (shared with ragged calls)
+    const cudaError_t e = cudaMalloc((void**)&s->d_rag, row_map_words(s->max_rows) * 4);
+    if (e != cudaSuccess) {
+      s->d_rag = nullptr;
+      cudaGetLastError();
+      return fail(LNB_ENOMEM, "speculative row map: %zu bytes of device memory asked for: %s", row_map_words(s->max_rows) * 4,
+                  cudaGetErrorString(e));
+    }
+  }
+  if (samp && (rc = samp_grow(s, rows))) return rc;
+  if ((rc = ensure_logits(s, (size_t)rows))) return rc;
+  s->kept_rows = 0;   // a logits handle is valid until the session's next forward
+  // [tokens | row_seq | row_pos]: one pinned staging copy
+  int32_t* h = s->h_tok;
+  memcpy(h, tokens, (size_t)rows * 4);
+  memcpy(h + rows, row_seq, (size_t)rows * 4);
+  memcpy(h + 2 * rows, row_pos, (size_t)rows * 4);
+  CU(cudaMemcpyAsync(s->d_rag, h, (size_t)3 * rows * 4, cudaMemcpyHostToDevice, s->stream));
+  if (eng) {
+    // ONE launch of the batch engine: every weight matrix streamed once for all rows
+    if ((rc = batch_engine_build(s, (logits || samp) ? s->logits : nullptr))) return rc;
+    if ((rc = batch_engine_launch(s, rows, s->d_rag, s->d_rag + 2 * rows, s->d_rag + rows))) return rc;
+  } else {
+    if ((rc = set_state(s, 0, rows, -1, false))) return rc;
+    if ((rc = enqueue_forward(s, rows_spec(s, rows)))) return rc;
+  }
+  int32_t p_next[8];
+  for (int r = 0; r < rows; r++) p_next[r] = row_pos[r] + 1;
+  if ((rc = call_tail(s, rows, 0, row_seq, p_next, s->d_next_arr, logits, rows, s->d_next_arr))) return rc;
+  // acceptance: row j of a segment predicts the token at position start + j + 1, which draft j + 1 claims
+  for (int i = 0, r0 = 0; i < n_segs; r0 += 1 + n_draft[i], i++) {
+    int acc = 0;
+    while (acc < n_draft[i] && s->h_out[r0 + acc] == tokens[r0 + acc + 1]) acc++;
+    if (n_accepted) n_accepted[i] = acc;
+  }
+  if (next_out) memcpy(next_out, s->h_out, (size_t)rows * 4);
   return 0;
 }
 

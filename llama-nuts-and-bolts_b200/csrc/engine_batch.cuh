@@ -51,10 +51,16 @@ struct BatchPhase {
   uint16_t* xn;             // SCALE, tensor-core form: the normalised row t(t(x * r[m]) * norm_w[k]), chunk-major (else NULL)
   float* out_f32;           // EPI_LOGITS: [8][ldo] f32 (row-major) or NULL
   int ldo, n_offset;
-  uint16_t* cache_k;        // this layer's caches, sequence 0 (sequence m at + m * cache_seq_stride)
+  uint16_t* cache_k;        // this layer's caches, sequence 0 (row m's sequence at + that sequence * cache_seq_stride)
   uint16_t* cache_v;
   int q_dim, kv_dim;
 };
+
+// the sequence whose cache row m reads and appends to: row_seq[m] (speculative verification: consecutive positions of one
+// sequence), or m (a batched step)
+LNB_DEVINL size_t be_cache_base(const int32_t* row_seq, int m, long long cache_seq_stride) {
+  return (size_t)(row_seq ? row_seq[m] : m) * (size_t)cache_seq_stride;
+}
 
 struct BatchParams {
   const BatchPhase* phases;
@@ -68,6 +74,7 @@ struct BatchParams {
   int strict;
   const int32_t* tokens;    // [n] input token of every sequence
   const int32_t* pos_arr;   // [n] position it is fed at
+  const int32_t* row_seq;   // [n] sequence of every row (its KV cache), or NULL: row m is sequence m
   long long cache_seq_stride;
   float* rscale;            // [8] RMSNorm scales of the running norm
   unsigned long long* keys; // [8] greedy-argmax keys (cleared by the host before the launch)
@@ -192,8 +199,8 @@ LNB_DEVINL void bt_epilogue(const GemvParams& p, int epi, const float (&v)[8], i
   } else if (epi == EPI_QKV_ROPE) {
     if (valid) {
       const int pos = p.pos_arr[m];
-      uint16_t* ck = p.cache_k + (size_t)m * (size_t)p.cache_seq_stride;
-      uint16_t* cv = p.cache_v + (size_t)m * (size_t)p.cache_seq_stride;
+      uint16_t* ck = p.cache_k + be_cache_base(p.row_seq, m, p.cache_seq_stride);
+      uint16_t* cv = p.cache_v + be_cache_base(p.row_seq, m, p.cache_seq_stride);
       uint32_t o[4];
       if (n0 < p.q_dim + p.kv_dim) {
         const int nn0 = (n0 < p.q_dim) ? n0 : n0 - p.q_dim;
@@ -455,6 +462,7 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
             g.out_bf16 = E->out; g.out_f32 = E->out_f32; g.ldo = E->ldo; g.res = E->res; g.cm = 1;
             g.q_dim = E->q_dim; g.kv_dim = E->kv_dim; g.head_dim = P.head_dim;
             g.cache_k = E->cache_k; g.cache_v = E->cache_v; g.pos_arr = P.pos_arr; g.cache_seq_stride = P.cache_seq_stride;
+            g.row_seq = P.row_seq;
             g.cis = P.cis; g.silu_tab = P.silu_tab;
             g.n_offset = E->n_offset; g.st = nullptr; g.argmax_row = -1; g.amax_keys_row = P.keys;
             g.pos_ptr = P.pos_arr; g.m_off = 0;
@@ -585,6 +593,7 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
           g.out_bf16 = E->out; g.out_f32 = E->out_f32; g.ldo = E->ldo; g.res = E->res; g.cm = 1;
           g.q_dim = E->q_dim; g.kv_dim = E->kv_dim; g.head_dim = P.head_dim;
           g.cache_k = E->cache_k; g.cache_v = E->cache_v; g.pos_arr = P.pos_arr; g.cache_seq_stride = P.cache_seq_stride;
+          g.row_seq = P.row_seq;
           g.cis = P.cis; g.silu_tab = P.silu_tab;
           g.n_offset = E->n_offset; g.st = nullptr; g.argmax_row = -1; g.amax_keys_row = P.keys;
           g.pos_ptr = P.pos_arr; g.m_off = 0;
@@ -746,9 +755,9 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
       double* sZ = reinterpret_cast<double*>((reinterpret_cast<uintptr_t>(sQ + (size_t)hd) + 15) & ~(uintptr_t)15);
       for (int item = bid; item < n_qh * n; item += G) {
         const int H = item % n_qh, m = item / n_qh, h = H / n_rep;
-        const int T = P.pos_arr[m] + 1;
-        const uint16_t* ck = E->cache_k + (size_t)m * (size_t)P.cache_seq_stride;
-        const uint16_t* cv = E->cache_v + (size_t)m * (size_t)P.cache_seq_stride;
+        const int T = P.pos_arr[m] + 1;   // keys 0 .. pos: earlier rows of the same sequence appended theirs in the QKV phase
+        const uint16_t* ck = E->cache_k + be_cache_base(P.row_seq, m, P.cache_seq_stride);
+        const uint16_t* cv = E->cache_v + be_cache_base(P.row_seq, m, P.cache_seq_stride);
         for (int i = c; i < T * cpr; i += ENG_NCONS) {
           const int t = i / cpr, cc = i % cpr;
           *reinterpret_cast<uint4*>(sK + (size_t)t * kstride + cc * 8) = ldcg_u4(ck + (size_t)t * E->kv_dim + (size_t)h * hd + cc * 8);

@@ -195,7 +195,7 @@ __global__ void __launch_bounds__(1024) sdpa_decode_kernel(const uint16_t* __res
                                                            uint16_t* __restrict__ out, const int32_t* __restrict__ pos_ptr,
                                                            int T_max, int strict, float scale_bf16_as_f32,
                                                            const int32_t* __restrict__ pos_arr, long long cache_seq_stride, int ldq,
-                                                           const LnbDevState* __restrict__ st) {
+                                                           const LnbDevState* __restrict__ st, const int32_t* __restrict__ row_seq) {
   extern __shared__ __align__(16) uint8_t sm[];
   const int kstride = hd + 8;
   uint16_t* sK = reinterpret_cast<uint16_t*>(sm);                       // [T_max][hd + 8]
@@ -208,11 +208,13 @@ __global__ void __launch_bounds__(1024) sdpa_decode_kernel(const uint16_t* __res
   const int tid = threadIdx.x, nthr = blockDim.x;
   const int hh = tid / 128, tt = tid % 128;
   const int cpr = hd / 8;  // 16-byte chunks per row
-  // batched decode: blockIdx.y = independent sequence (own cache, own position, own q / output row)
+  // batched decode: blockIdx.y = row with its own position and q / output row, on the cache of sequence blockIdx.y, or of
+  // row_seq[blockIdx.y] (speculative verification: several rows of one sequence, the later ones seeing the earlier ones' keys)
   if (pos_arr) {
+    const size_t seq = row_seq ? (size_t)row_seq[blockIdx.y] : (size_t)blockIdx.y;
     pos_ptr = pos_arr + blockIdx.y;
-    cache_k += (size_t)blockIdx.y * (size_t)cache_seq_stride;
-    cache_v += (size_t)blockIdx.y * (size_t)cache_seq_stride;
+    cache_k += seq * (size_t)cache_seq_stride;
+    cache_v += seq * (size_t)cache_seq_stride;
     q += (size_t)blockIdx.y * ldq;
     out += (size_t)blockIdx.y * ldq;
   }

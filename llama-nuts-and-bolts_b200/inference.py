@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import collections
 import time
+from dataclasses import dataclass
 
 import numpy as np
 
@@ -16,11 +17,54 @@ GSInProgress, GSFinishedByReachingEOS, GSFinishedByReachingSeqLen = 0, 1, 2
 SamplingArgs = model_mod.SamplingArgs
 
 
+@dataclass
+class SpeculativeArgs:
+    """EXTENSION: speculative decoding (lnb_forward_speculative).  Each call feeds a sequence's last token plus up to MaxDraft
+    tokens drafted by prompt lookup (prompt_lookup_drafts, n-grams of NgramMax down to NgramMin tokens) and keeps the drafts
+    the model agrees with.  Every verified row has the bits of the plain step, so the generated stream is the plain one."""
+    MaxDraft: int
+    NgramMax: int = 3
+    NgramMin: int = 1
+
+
+# Rows of one speculative call (the batch engine serves at most 8 rows per launch).
+SPEC_MAX_ROWS = 8
+
+
+def prompt_lookup_drafts(history, max_draft: int, ngram_max: int = 3, ngram_min: int = 1) -> list[int]:
+    """Prompt-lookup drafter, a pure function of the token history h[0..L) (h[L-1] is the token about to be fed): for
+    n = ngram_max down to ngram_min, the largest j with j + n < L and h[j..j+n) == h[L-n..L); the first n that matches gives
+    the drafts h[j+n .. min(j+n+max_draft, L)).  No match (or max_draft <= 0) gives no drafts."""
+    h = np.asarray(history, np.int64).reshape(-1)
+    L = h.shape[0]
+    if max_draft <= 0:
+        return []
+    for n in range(ngram_max, max(ngram_min, 1) - 1, -1):
+        if L < n + 1:
+            continue
+        # windows h[j..j+n) for j = 0 .. L-n-1 (j + n < L keeps the suffix itself out and leaves at least one draft)
+        win = np.lib.stride_tricks.sliding_window_view(h[:L - 1], n)
+        hit = np.flatnonzero(np.all(win == h[L - n:], axis=1))
+        if hit.size:
+            j = int(hit[-1])
+            return [int(t) for t in h[j + n:min(j + n + max_draft, L)]]
+    return []
+
+
 def _sampling_for(sampling, i: int):
     """prompt i of a batch or continuous run samples with Seed + i: its stream is GenerateTokens(prompts[i]) with that seed"""
     if sampling is None or sampling.Temperature == 0:
         return None
     return SamplingArgs(sampling.Temperature, sampling.TopK, sampling.TopP, (sampling.Seed + i) & (2**64 - 1))
+
+
+def _check_speculative(speculative, use_reference_api: bool = False):
+    if speculative is None:
+        return
+    if use_reference_api:
+        raise ml.MlError("use_reference_api=True runs the reference's Forward -> Slice -> ml.Argmax calls; it cannot verify drafts")
+    if speculative.MaxDraft < 0 or not 1 <= speculative.NgramMin <= speculative.NgramMax:
+        raise ml.MlError(f"SpeculativeArgs {speculative}: MaxDraft must be >= 0 and 1 <= NgramMin <= NgramMax")
 
 # Row budget of one GenerateTokensContinuous step.  FAST ragged steps of >= 32 rows run on the tensor cores (one pass over
 # the weights); steps of 9..31 rows run the GEMV chain, which streams the weights once per 8 rows (up to 4 passes), and
@@ -105,7 +149,8 @@ class InferenceEngine:
                        IsResendOfWaiting=True, GenerationState=last_state if i + 1 == len(waiting) else GSInProgress)
 
     def GenerateTokens(self, promptTokens, use_reference_api: bool = False, step_times: list | None = None,
-                       prefill_chunk: int = 0, sampling: "SamplingArgs | None" = None):
+                       prefill_chunk: int = 0, sampling: "SamplingArgs | None" = None,
+                       speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None):
         """Generator over (state, token id) exactly like generatedTokensCh.
 
         use_reference_api=True goes through the reference-shaped calls of every iteration
@@ -117,10 +162,17 @@ class InferenceEngine:
         max_rows become possible, and the generated stream is the same.
 
         sampling (EXTENSION): SamplingArgs of a seeded sampler in place of the greedy argmax (None / Temperature 0: greedy).
-        The reference call sequence ends in ml.Argmax, so use_reference_api=True with a sampler is an error."""
+        The reference call sequence ends in ml.Argmax, so use_reference_api=True with a sampler is an error.
+
+        speculative (EXTENSION): SpeculativeArgs.  After the prompt, every call verifies the last token plus prompt-lookup
+        drafts in one pass over the weights (lnb_forward_speculative) and emits the accepted tokens one at a time through
+        the same stop logic, so the stream (tokens, length, final state) is the plain loop's, greedy or sampled.  step_times
+        then gets one entry per call, and spec_stats (optional) one (rows, accepted drafts) pair per call.  It also needs
+        the fused entry: use_reference_api=True with speculative is an error."""
         sampling = _sampling_for(sampling, 0)
         if sampling is not None and use_reference_api:
             raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax (inference.go:207-216); it cannot sample")
+        _check_speculative(speculative, use_reference_api)
         infContext = self.CreateInferenceContext()
         try:
             if sampling is not None:
@@ -167,8 +219,64 @@ class InferenceEngine:
                     yield GSFinishedByReachingSeqLen, nextTokenId
                     break
                 yield GSInProgress, nextTokenId
+                if speculative is not None:   # the prompt is in the cache: from here on, verify drafts
+                    hist = [[int(t) for t in tokens.RawData[:curPos + 1]]]
+                    for _, state, tok in self._generate_speculative(infContext, hist, [0], speculative, step_times, spec_stats):
+                        yield state, tok
+                    break
         finally:
             infContext.close()
+
+    def _generate_speculative(self, infContext, hists, live, speculative: "SpeculativeArgs", step_times: list | None = None,
+                              spec_stats: list | None = None):
+        """The speculative loop on a given context (anything with SequenceLength, max_rows and forward_speculative).
+        hists[i]: the tokens of sequence i so far, its last one emitted and not yet fed (it is fed at position
+        len(hists[i]) - 1); live: the sequences still generating, each gets a row in every call.  The rows left of the
+        budget min(8, max_rows) go to drafts in sequence order, clamped so that no row passes position SequenceLength - 2
+        (the last position the plain loop feeds).  Yields (sequence, state, token) per emitted token, a segment's accepted
+        tokens in order; hists grow with them."""
+        seqLen = infContext.SequenceLength
+        stop = self.model.Vocabulary.StopTokenIds
+        budget = min(SPEC_MAX_ROWS, infContext.max_rows)
+        live = list(live)
+        if len(live) > budget:
+            raise ml.MlError(f"{len(live)} sequences do not fit the row budget {budget} of a speculative call")
+        while live:
+            left = budget - len(live)
+            segs = []
+            for i in live:
+                h = hists[i]
+                pos = len(h) - 1
+                k = min(speculative.MaxDraft, left, seqLen - 2 - pos)
+                drafts = prompt_lookup_drafts(h, k, speculative.NgramMax, speculative.NgramMin)
+                left -= len(drafts)
+                segs.append((i, pos, [h[-1]] + drafts))
+            t0 = time.perf_counter()
+            nxt, acc, _ = infContext.forward_speculative(segs)
+            if step_times is not None:
+                step_times.append(time.perf_counter() - t0)
+            if spec_stats is not None:
+                spec_stats.append((sum(len(t) for _, _, t in segs), int(sum(int(a) for a in acc))))
+            still, r0 = [], 0
+            for (i, pos, toks), a in zip(segs, acc):
+                finished = False
+                for j in range(int(a) + 1):            # the next tokens of rows 0 .. a, one at a time (:218-248)
+                    tok, curPos = int(nxt[r0 + j]), pos + 1 + j
+                    hists[i].append(tok)
+                    if tok in stop:
+                        state = GSFinishedByReachingEOS
+                    elif curPos + 1 == seqLen:
+                        state = GSFinishedByReachingSeqLen
+                    else:
+                        state = GSInProgress
+                    yield i, state, tok
+                    if state != GSInProgress:
+                        finished = True
+                        break
+                r0 += len(toks)
+                if not finished:
+                    still.append(i)
+            live = still
 
     def GenerateTokensContinuous(self, prompts, slots: int = 8, step_tokens: int | None = None,
                                  step_times: list | None = None, sampling: "SamplingArgs | None" = None):
@@ -268,18 +376,23 @@ class InferenceEngine:
                     slot[k] = None
                 yield sl["i"], state, tok
 
-    def GenerateTokensBatch(self, prompts, step_times: list | None = None, sampling: "SamplingArgs | None" = None):
+    def GenerateTokensBatch(self, prompts, step_times: list | None = None, sampling: "SamplingArgs | None" = None,
+                            speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None):
         """The consumer `InferenceEngine.TokenizeBatch` (src/inference/tokenize.go:97-107) never got in the
         reference (SURVEY 8f-4): every prompt runs the loop of generateTokensInternal (:173-254) -- own
         InferenceContext / KV cache, own positions, own stop condition -- but all sequences advance together,
         one pass over the weights per step (lnb_forward_batch).  Yields (sequence index, state, token id);
         per sequence the stream is exactly what GenerateTokens(prompts[i]) yields.  sampling: sequence i samples with
-        Seed + i (the stream of GenerateTokens(prompts[i]) with that seed)."""
+        Seed + i (the stream of GenerateTokens(prompts[i]) with that seed).
+        speculative (EXTENSION): after the prompts, every call is one lnb_forward_speculative in which each unfinished
+        sequence gets its row and the rest of the 8-row budget goes to prompt-lookup drafts in sequence order; the streams
+        are the same.  spec_stats as in GenerateTokens."""
+        _check_speculative(speculative)
         n = len(prompts)
         if n < 1:
             raise ml.MlError("empty prompt batch")
         if n == 1:
-            for state, tok in self.GenerateTokens(prompts[0], sampling=sampling):
+            for state, tok in self.GenerateTokens(prompts[0], sampling=sampling, speculative=speculative, spec_stats=spec_stats):
                 yield 0, state, tok
             return
         infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
@@ -320,6 +433,11 @@ class InferenceEngine:
                 yield i, emit(i, int(nxt), len(p)), int(nxt)
             if step_times is not None:
                 step_times.append(time.perf_counter() - t0)
+            if speculative is not None:
+                hists = [[int(t) for t in p] + [cur[i]] for i, p in enumerate(prompts)]
+                live = [i for i in range(n) if not done[i]]
+                yield from self._generate_speculative(infContext, hists, live, speculative, step_times, spec_stats)
+                return
             while not all(done):
                 t0 = time.perf_counter()
                 # finished sequences are stepped again at their last position (same token, same cache row: a no-op

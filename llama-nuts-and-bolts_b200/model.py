@@ -231,6 +231,26 @@ class InferenceContext:
                                      ptr(nxt, _capi.i32p)))
         return nxt, logits
 
+    def forward_speculative(self, segments, want_logits: bool = False):
+        """EXTENSION (speculative verification, lnb_forward_speculative): ONE forward over segments (seq, start_pos, tokens)
+        whose tokens are the sequence's last emitted token followed by drafted tokens, row j at position start_pos + j.
+        Returns (next token of every row [rows], accepted drafts of every segment [n_segs], logits [rows, vocab] or None);
+        segment i emits the next tokens of its rows 0 .. accepted[i]."""
+        n = len(segments)
+        seq = np.array([s for s, _, _ in segments], np.int32)
+        start = np.array([p for _, p, _ in segments], np.int32)
+        toks = [np.asarray(t, np.int32).reshape(-1) for _, _, t in segments]
+        n_draft = np.array([len(t) - 1 for t in toks], np.int32)
+        flat = np.ascontiguousarray(np.concatenate(toks) if toks else np.zeros(0, np.int32), np.int32)
+        rows = flat.shape[0]
+        nxt = np.empty(rows, np.int32)
+        acc = np.empty(n, np.int32)
+        logits = np.empty((rows, self.transformer.args.VocabSize), np.float32) if want_logits else None
+        check(lib.lnb_forward_speculative(self.h, n, ptr(seq, _capi.i32p), ptr(start, _capi.i32p), ptr(n_draft, _capi.i32p),
+                                          ptr(flat, _capi.i32p), ptr(logits, _capi.f32p) if want_logits else None,
+                                          ptr(nxt, _capi.i32p), ptr(acc, _capi.i32p)))
+        return nxt, acc, logits
+
     def set_sampling(self, seq: int, args: "SamplingArgs | None"):
         """EXTENSION: sequence `seq` samples its next tokens with `args` (None or Temperature 0: greedy) from its next
         forward on; every token output of forward_argmax / forward_batch / forward_ragged / decode_run then carries the
