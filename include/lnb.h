@@ -183,6 +183,11 @@ int lnb_model_get_silu_table(lnb_model* m, uint16_t* out65536);
 /* checks all 291 tensors are present, builds tables, makes the model immutable */
 int lnb_model_finalize(lnb_model* m);
 int lnb_model_destroy(lnb_model* m); /* hook for model.Model.Free (src/model/model.go:56) */
+/* The packed copy the STRICT decode engine streams for w1|w3 of `layer` (layer -1: the LM head), built on first use
+ * (DESIGN §4): data = [N/8 panels][12 * K] bytes, units = [N/8][k-tiles] unit bytes (0xFF = raw), src = the panel-major
+ * bf16 it encodes [N/8][K/8][8][8]; any of them may be NULL.  info[5] = {kt, units, packed units, bytes the engine reads
+ * per pass, N}.  Returns 1, or 0 when the engine streams bf16 (lnb_last_error says why).  The model must be finalized. */
+int lnb_model_wpack_read(lnb_model* m, int layer, uint8_t* data, uint8_t* units, uint16_t* src, int64_t* info);
 
 /* model.NewInferenceContext (src/model/inferencecontext.go:17-46): KV cache of seq_len rows
  * per layer, zero-filled.  max_rows = largest S a forward call may carry (>=1).

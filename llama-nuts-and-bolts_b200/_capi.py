@@ -53,6 +53,7 @@ SIGNATURES = {
     "lnb_model_get_silu_table": (C.c_int, [vp, u16p]),
     "lnb_model_finalize": (C.c_int, [vp]),
     "lnb_model_destroy": (C.c_int, [vp]),
+    "lnb_model_wpack_read": (C.c_int, [vp, C.c_int, vp, vp, u16p, i64p]),
     "lnb_session_create": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
     "lnb_session_destroy": (C.c_int, [vp]),
     "lnb_forward": (C.c_int, [vp, i32p, C.c_int, C.c_int, f32p, C.c_int, i32p]),

@@ -139,6 +139,22 @@ struct lnb_model {
   void* staging = nullptr;
   size_t staging_bytes = 0;
   int sm_count = 132;
+  // the STRICT decode engine's packed copies of w1|w3 (per layer) and the LM head (wpack.cuh), built by the first STRICT
+  // engine session (ensure_wpack).  Sessions need a finalized model and a finalized model takes no more weights, so a
+  // packed copy can never fall behind the bf16 matrix it was built from.
+  struct WPack {
+    uint8_t* data = nullptr;
+    uint8_t* units = nullptr;
+    int kt = 0;
+    int64_t read_bytes = 0;        // bytes the engine reads per pass (packed units, raw units, unit table)
+    int64_t packed_units = 0, n_units = 0;
+  };
+  std::vector<WPack> wp_w13;
+  WPack wp_out;
+  void* wpack_mem = nullptr;
+  int wpack_state = 0;             // 0 = not built, 1 = built, -1 = the engine streams bf16 (wpack_why says why)
+  std::string wpack_why;
+  std::mutex wpack_mu;
 };
 
 static int parse_name(const lnb_model* m, const char* name, int* kind, int* layer) {
@@ -309,7 +325,7 @@ extern "C" int lnb_model_destroy(lnb_model* m) {
   for (auto& L : m->layers) {
     cudaFree(L.attn_norm); cudaFree(L.ffn_norm); cudaFree(L.wqkv); cudaFree(L.wo); cudaFree(L.w13); cudaFree(L.w2);
   }
-  cudaFree(m->cis); cudaFree(m->silu_tab); cudaFree(m->staging);
+  cudaFree(m->cis); cudaFree(m->silu_tab); cudaFree(m->staging); cudaFree(m->wpack_mem);
   delete m;
   return 0;
 }
@@ -1531,6 +1547,79 @@ static int eng_kt(int mode, int N, int K, int G) {
   while (kt > 64 && maxp * kt * 16 > EngCfg<1>::kStage) kt >>= 1;
   return std::min(kt, K);
 }
+// The packed copies the STRICT decode engine streams for w1|w3 and the LM head (wpack.cuh, DESIGN §4): built once per
+// model, on its device, from the panel-major bf16.  If the memory is not there the engine streams bf16 (same bits).
+static bool ensure_wpack(lnb_model* m) {
+  std::lock_guard<std::mutex> lk(m->wpack_mu);
+  if (m->wpack_state) return m->wpack_state > 0;
+  if (cudaSetDevice(m->device) != cudaSuccess) { cudaGetLastError(); return false; }
+  const lnb_model_args& a = m->a;
+  const int G = m->sm_count, L = a.n_layers;
+  auto no = [&](const std::string& why) { m->wpack_state = -1; m->wpack_why = why; return false; };
+  struct Mat { const uint16_t* W; int N; lnb_model::WPack* wp; };
+  std::vector<Mat> mats;
+  m->wp_w13.assign(L, lnb_model::WPack{});
+  for (int l = 0; l < L; l++) mats.push_back({m->layers[l].w13, 2 * m->ffn_l, &m->wp_w13[l]});
+  mats.push_back({m->output, m->vocab_l, &m->wp_out});
+  const int K = a.dim;
+  size_t total = 0;
+  std::vector<size_t> off_data, off_units;
+  for (Mat& x : mats) {
+    const int kt = eng_kt(LNB_ACC_STRICT, x.N, K, G);
+    if (K % 32 || kt % 32) return no("packed weights need K and the k-tile to be multiples of 32");
+    x.wp->kt = kt;
+    x.wp->n_units = (int64_t)(x.N / 8) * ((K + kt - 1) / kt);
+    off_data.push_back(total);
+    total += (size_t)x.N / 8 * K * 12;
+    off_units.push_back(total);
+    total = (total + x.wp->n_units + 255) & ~(size_t)255;
+  }
+  unsigned long long* ctr = nullptr;
+  if (cudaMalloc(&m->wpack_mem, total) != cudaSuccess || cudaMalloc((void**)&ctr, mats.size() * 16) != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(m->wpack_mem);
+    m->wpack_mem = nullptr;
+    char why[160];
+    snprintf(why, sizeof(why), "cudaMalloc of the %.2f GB packed weight copy failed: the engine streams bf16", total / 1e9);
+    return no(why);
+  }
+  cudaMemset(ctr, 0, mats.size() * 16);
+  for (size_t i = 0; i < mats.size(); i++) {
+    lnb_model::WPack& wp = *mats[i].wp;
+    wp.data = static_cast<uint8_t*>(m->wpack_mem) + off_data[i];
+    wp.units = static_cast<uint8_t*>(m->wpack_mem) + off_units[i];
+    wpack_encode_kernel<<<G * 8, 256>>>(mats[i].W, mats[i].N / 8, K, wp.kt, wp.data, wp.units, ctr + 2 * i);
+  }
+  std::vector<unsigned long long> h(mats.size() * 2);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpy(h.data(), ctr, h.size() * 8, cudaMemcpyDeviceToHost);
+  cudaFree(ctr);
+  if (e != cudaSuccess) {
+    cudaFree(m->wpack_mem);
+    m->wpack_mem = nullptr;
+    return no(std::string("packing the weights failed: ") + cudaGetErrorString(e));
+  }
+  for (size_t i = 0; i < mats.size(); i++) {
+    mats[i].wp->read_bytes = (int64_t)h[2 * i];
+    mats[i].wp->packed_units = (int64_t)h[2 * i + 1];
+  }
+  m->wpack_state = 1;
+  return true;
+}
+extern "C" int lnb_model_wpack_read(lnb_model* m, int layer, uint8_t* data, uint8_t* units, uint16_t* src, int64_t* info) {
+  if (!m) return fail(LNB_EINVAL, "model is NULL");
+  if (!m->finalized) return fail(LNB_ESTATE, "model is not finalized");
+  if (layer < -1 || layer >= m->a.n_layers) return fail(LNB_EINVAL, "layer %d out of range", layer);
+  CU(cudaSetDevice(m->device));
+  if (!ensure_wpack(m)) { g_err = m->wpack_why; return 0; }
+  const lnb_model::WPack& wp = layer < 0 ? m->wp_out : m->wp_w13[layer];
+  const int64_t N = layer < 0 ? m->vocab_l : 2 * (int64_t)m->ffn_l, K = m->a.dim;
+  if (data) CU(cudaMemcpy(data, wp.data, (size_t)(N / 8) * K * 12, cudaMemcpyDeviceToHost));
+  if (units) CU(cudaMemcpy(units, wp.units, (size_t)wp.n_units, cudaMemcpyDeviceToHost));
+  if (src) CU(cudaMemcpy(src, layer < 0 ? m->output : m->layers[layer].w13, (size_t)N * K * 2, cudaMemcpyDeviceToHost));
+  if (info) { info[0] = wp.kt; info[1] = wp.n_units; info[2] = wp.packed_units; info[3] = wp.read_bytes; info[4] = N; }
+  return 1;
+}
 // kind -1: the full step; 0..4: independent copies of one projection of every layer (kernel-alone timing, plain buffers)
 static int engine_build(lnb_session* s, int kind, const float* logits_out) {
   lnb_model* m = s->m;
@@ -1559,6 +1648,11 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
     if (full && writer >= 0) { e.res_t = vec; e.res_delta = (int)ph.size() - writer; }
   };
   const bool tp = m->tp_size > 1;
+  // STRICT streams the packed copies of w1|w3 and the LM head (the FAST engine's KS = 8 chains read bf16 only)
+  const bool wpack = mode == LNB_ACC_STRICT && ensure_wpack(m);
+  auto packed = [&](EnginePhase& e, const lnb_model::WPack& wp) {
+    if (wpack && wp.kt == e.kt) { e.Wp = wp.data; e.Wu = wp.units; }
+  };
   for (int l = 0; l < n_layers; l++) {
     LayerW& W = m->layers[l];
     if (full || kind == 0) {  // attn_norm -> wq|wk|wv -> RoPE -> KV append
@@ -1595,6 +1689,7 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
     }
     if (full || kind == 2) {  // ffn_norm -> w1|w3 -> SiLU * up
       EnginePhase e = gemv(PRO_RMSNORM, EPI_SWIGLU, W.w13, 2 * m->ffn_l, a.dim, s->h1, W.ffn_norm, s->mbuf, m->ffn_l, nullptr);
+      packed(e, m->wp_w13[l]);
       input(e, s->h1_t, w_h1);
       if (full) { e.out_t = s->m_t; w_m = (int)ph.size(); }
       ph.push_back(e);
@@ -1617,6 +1712,7 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
     const int reps = kind == 4 ? 4 : 1;
     for (int i = 0; i < reps; i++) {
       EnginePhase e = gemv(PRO_RMSNORM, EPI_LOGITS, m->output, m->vocab_l, a.dim, s->x, m->norm, nullptr, m->vocab_l, nullptr);
+      packed(e, m->wp_out);
       e.out_f32 = const_cast<float*>(logits_out); e.n_offset = m->tp_rank * m->vocab_l;
       if (full && n_layers > 0) input(e, s->x_t, w_x);
       if (full) e.flags |= EF_GRID_SYNC;
@@ -2796,6 +2892,17 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
       case 2: bytes = (int64_t)2 * m->ffn_l * a.dim * 2; break;
       case 3: bytes = (int64_t)a.dim * m->ffn_l * 2; break;
       default: bytes = (int64_t)m->vocab_l * a.dim * 2; break;
+    }
+    // packed phases read what their units hold: the mean over the phases of the sweep
+    std::vector<EnginePhase> hp(s->n_phases);
+    CU(cudaMemcpy(hp.data(), s->d_phases, hp.size() * sizeof(EnginePhase), cudaMemcpyDeviceToHost));
+    if (!hp.empty() && hp[0].Wp) {
+      int64_t sum = 0;
+      for (int i = 0; i < s->n_phases; i++) {
+        const lnb_model::WPack& wp = (kind == 4) ? m->wp_out : m->wp_w13[i];
+        sum += hp[i].Wp ? wp.read_bytes : bytes;
+      }
+      bytes = sum / s->n_phases;
     }
     if (ms_per_launch) *ms_per_launch = ms / (float)n;
     if (bytes_per_launch) *bytes_per_launch = bytes;

@@ -36,6 +36,7 @@
 #include "gemv.cuh"
 #include "kernels.cuh"
 #include "seqsum.cuh"
+#include "wpack.cuh"
 
 namespace lnb {
 
@@ -50,6 +51,8 @@ struct EnginePhase {
   int type, pro, epi, flags;
   int N, K, kt, ldx;
   const uint16_t* W;
+  const uint8_t* Wp;        // STRICT: the packed copy of W (wpack.cuh) and its unit bytes [N/8][k-tiles], NULL: stream W
+  const uint8_t* Wu;
   const uint16_t* x;        // GEMV: activations [K] / REDUCE: residual [dim]
   const uint16_t* norm_w;
   const uint16_t* res;
@@ -368,6 +371,69 @@ LNB_DEVINL float eng_chain_tile(const uint8_t* __restrict__ tile, const float* _
 #undef ENG_FMA
   return acc;
 }
+// The same chain over a packed unit (wpack.cuh): NG groups of 384 bytes, each decoded to the bf16 words eng_chain_tile
+// reads and fed to the same FMAs in the same order.  The decode does not depend on the accumulator, so it is software-
+// pipelined: the pair words of group g + 1 are decoded between the dependent FMAs of group g (decoded just before its own
+// FMAs, a chunk cost its decode latency on top of its FMA chain: ~14 cycles per weight instead of the issue rate), and the
+// packed words of group g + 2 are loaded meanwhile.  NG = 0: a run-time number of groups (unit lengths other than 64..512).
+LNB_DEVINL uint32_t eng_wp_pair(const uint4 (&w)[3], int q, int p, uint32_t bb) {
+  const uint4& s = (q < 2) ? w[0] : w[1];                    // sign|mantissa bytes: chunks 0, 1 then 2, 3
+  const uint32_t sm = (q & 1) ? ((p < 2) ? s.z : s.w) : ((p < 2) ? s.x : s.y);
+  const uint32_t cw = (q == 0) ? w[2].x : (q == 1) ? w[2].y : (q == 2) ? w[2].z : w[2].w;
+  switch (p) {
+    case 0: return wp_pair<0>(sm, cw, bb);
+    case 1: return wp_pair<1>(sm, cw, bb);
+    case 2: return wp_pair<2>(sm, cw, bb);
+    default: return wp_pair<3>(sm, cw, bb);
+  }
+}
+template <int NG>
+LNB_DEVINL float eng_chain_tile_wp(const uint8_t* __restrict__ unit, const float* __restrict__ xt, float acc, uint32_t bb, int ng = NG) {
+  auto ld = [&](int g, uint4 (&w)[3]) {
+    w[0] = *reinterpret_cast<const uint4*>(unit + g * WP_GROUP_BYTES);
+    w[1] = *reinterpret_cast<const uint4*>(unit + g * WP_GROUP_BYTES + 128);
+    w[2] = *reinterpret_cast<const uint4*>(unit + g * WP_GROUP_BYTES + 256);
+  };
+  auto fma_pair = [&](const float* x, uint32_t w) {
+    acc = __fmaf_rn(x[0], bf_lo(w), acc);
+    acc = __fmaf_rn(x[1], bf_hi(w), acc);
+  };
+  if (NG == 0) {
+    for (int g = 0; g < ng; g++) {
+      uint4 w[3];
+      ld(g, w);
+#pragma unroll
+      for (int q = 0; q < 4; q++)
+#pragma unroll
+        for (int p = 0; p < 4; p++) fma_pair(xt + g * 32 + q * 8 + p * 2, eng_wp_pair(w, q, p, bb));
+    }
+    return acc;
+  }
+  uint4 pw[2][3];                 // packed words: group g + 1 in pw[(g + 1) & 1], group g + 2 loading into pw[g & 1]
+  uint32_t cur[16], nxt[16];      // pair words of groups g and g + 1
+  ld(0, pw[0]);
+  if (NG > 1) ld(1, pw[1]);
+#pragma unroll
+  for (int i = 0; i < 16; i++) cur[i] = eng_wp_pair(pw[0], i >> 2, i & 3, bb);
+#pragma unroll
+  for (int g = 0; g < NG; g++) {
+    if (g + 2 < NG) ld(g + 2, pw[g & 1]);
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const float4 x0 = *reinterpret_cast<const float4*>(xt + g * 32 + q * 8);
+      const float4 x1 = *reinterpret_cast<const float4*>(xt + g * 32 + q * 8 + 4);
+      const float xs[8] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w};
+#pragma unroll
+      for (int p = 0; p < 4; p++) {
+        if (g + 1 < NG) nxt[q * 4 + p] = eng_wp_pair(pw[(g + 1) & 1], q, p, bb);
+        fma_pair(xs + p * 2, cur[q * 4 + p]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 16; i++) cur[i] = nxt[i];
+  }
+  return acc;
+}
 
 // four consecutive words of a tagged vector, polled until all of them carry `tag_hi`
 // (relaxed at gpu scope, not volatile: volatile loads are kept in order by the hardware, one L2 round trip each -- a
@@ -426,6 +492,8 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) decode_engine_kernel(const Eng
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem);              // [NST]
   uint64_t* empty_bar = full_bar + NST;                                // [NST]
+  uint8_t* s_unit = smem + 64;                                         // [NST][PT] unit bytes of a packed phase's stages
+  static_assert(64 + NST * PT <= 256, "unit bytes must fit below s_scalar");
   float* s_scalar = reinterpret_cast<float*>(smem + 256);              // rms scale etc.
   EngCtl* ctl = reinterpret_cast<EngCtl*>(smem + 320);
   GemvParams* gp = reinterpret_cast<GemvParams*>(smem + 512);          // the running phase as the epilogues see it
@@ -463,24 +531,37 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) decode_engine_kernel(const Eng
         int p0, p1;
         eng_split(E->N / 8, bid, G, &p0, &p1);
         const uint8_t* wbase = reinterpret_cast<const uint8_t*>(E->W);
+        const uint8_t* pbase = (KS == 1) ? E->Wp : nullptr;   // packed phase: each panel's unit byte picks its source
         for (int rt = p0; rt < p1; rt += PT) {
           const int np = min(PT, p1 - rt);
           const uint8_t* src_row = wbase + (size_t)(rt + tid) * (size_t)K * 16u;
+          const uint8_t* psrc_row = pbase ? pbase + (size_t)(rt + tid) * (size_t)K * 12u : nullptr;
           const int kt = eng_tile_kt(KS, np, K, E->kt, STAGE);
           const int n_tiles = (K + kt - 1) / kt;
+          const uint8_t* urow = pbase ? E->Wu + (size_t)(rt + tid) * (size_t)n_tiles : nullptr;
+          uint32_t u_next = (pbase && tid < np) ? (uint32_t)__ldg(urow) : (uint32_t)WP_RAW;
           for (int t = 0; t < n_tiles; t++, seq++) {
             const int s = seq % NST;
             const uint32_t par = (seq / NST) & 1u;
             const int k0 = t * kt;
-            const uint32_t bytes_per_panel = (uint32_t)min(kt, K - k0) * 16u;
+            const uint32_t len = (uint32_t)min(kt, K - k0);
+            // the unit byte of the next k-tile is loaded one stage ahead: its latency hides behind this stage's wait and issue
+            const uint32_t u = u_next;
+            if (pbase && tid < np && t + 1 < n_tiles) u_next = (uint32_t)__ldg(urow + t + 1);
+            const bool packed = u != (uint32_t)WP_RAW;
+            const uint32_t my_bytes = tid < np ? len * (packed ? 12u : 16u) : 0u;
+            const uint32_t stage_bytes = pbase ? __reduce_add_sync(0xffffffffu, my_bytes) : len * 16u * (uint32_t)np;
             // every issuing lane observes the stage's release itself (an acquire by lane 0 plus __syncwarp orders the
             // other lanes' copies too, but compute-sanitizer's racecheck does not follow that edge for async-proxy writes)
             eng_mbar_wait(&empty_bar[s], par ^ 1u, P.err_host, P.timeout_ns, false, seq);
-            if (tid == 0) mbar_expect_tx(&full_bar[s], bytes_per_panel * (uint32_t)np);
+            if (pbase && tid < np) s_unit[s * PT + tid] = (uint8_t)u;   // published by lane 0's arrive below
+            __syncwarp();
+            if (tid == 0) mbar_expect_tx(&full_bar[s], stage_bytes);
             __syncwarp();
             if (tid < np)
-              bulk_g2s(s_ring + (size_t)s * STAGE + (size_t)tid * ((size_t)kt * 16), src_row + (size_t)k0 * 16u, bytes_per_panel, &full_bar[s], pol);
-            issued += (unsigned long long)bytes_per_panel * (unsigned long long)np;
+              bulk_g2s(s_ring + (size_t)s * STAGE + (size_t)tid * ((size_t)kt * 16),
+                       packed ? psrc_row + (size_t)k0 * 12u : src_row + (size_t)k0 * 16u, my_bytes, &full_bar[s], pol);
+            issued += (unsigned long long)stage_bytes;
             if (tid == 0) ctl->ld_bytes = issued;
           }
         }
@@ -505,13 +586,16 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) decode_engine_kernel(const Eng
         const int n_tiles = (K + kt - 1) / kt;
         int p0, p1;
         eng_split(E->N / 8, bid, G, &p0, &p1);
-        const uint8_t* wbase = reinterpret_cast<const uint8_t*>(E->W);
+        // (a packed phase: the packed copy, whatever the units' bytes say -- a hint, not a copy)
+        const bool pk = KS == 1 && E->Wp;
+        const uint8_t* wbase = pk ? E->Wp : reinterpret_cast<const uint8_t*>(E->W);
+        const uint32_t epc = pk ? 12u : 16u;   // bytes per column of a panel
         for (int rt = p0; rt < p1; rt += PT) {
           const int np = min(PT, p1 - rt);
           const int kt = eng_tile_kt(KS, np, K, E->kt, STAGE);
           const int n_tiles = (K + kt - 1) / kt;
           for (int t = 0; t < n_tiles; t++) {
-            const uint32_t bpp = (uint32_t)min(kt, K - t * kt) * 16u;
+            const uint32_t bpp = (uint32_t)min(kt, K - t * kt) * epc;
             const unsigned long long tile_bytes = (unsigned long long)bpp * (unsigned long long)np;
             unsigned long long ld = ctl->ld_bytes;
             uint32_t spins = 0;
@@ -521,7 +605,7 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) decode_engine_kernel(const Eng
               if (++spins > (1u << 26)) return;
             }
             if (pf >= ld + lead && lane < np)
-              l2_prefetch_bulk(wbase + ((size_t)(rt + lane) * (size_t)K + (size_t)t * kt) * 16u, bpp);
+              l2_prefetch_bulk(wbase + ((size_t)(rt + lane) * (size_t)K + (size_t)t * kt) * epc, bpp);
             pf += tile_bytes;
           }
         }
@@ -696,7 +780,16 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) decode_engine_kernel(const Eng
                 //  are never stored: `valid` is false for them)
                 const uint8_t* tile0 = s_ring + (size_t)s * STAGE + (on0 ? (size_t)pp0 * ((size_t)kt * 16) : (size_t)0) + rr * 16;
                 const float* xt = s_x + k0;
-                if (KS == 1) {
+                // packed phase: this panel's unit byte, published with the stage (a lane with a raw panel runs the bf16 chain)
+                const uint32_t ub = (KS == 1 && E->Wp && on0) ? (uint32_t)s_unit[s * PT + pp0] : (uint32_t)WP_RAW;
+                if (KS == 1 && ub != (uint32_t)WP_RAW) {
+                  const uint32_t bb = (ub - 15u) << 7;
+                  if (nchunks == 64) acc0 = eng_chain_tile_wp<16>(tile0, xt, acc0, bb);
+                  else if (nchunks == 32) acc0 = eng_chain_tile_wp<8>(tile0, xt, acc0, bb);
+                  else if (nchunks == 16) acc0 = eng_chain_tile_wp<4>(tile0, xt, acc0, bb);
+                  else if (nchunks == 8) acc0 = eng_chain_tile_wp<2>(tile0, xt, acc0, bb);
+                  else acc0 = eng_chain_tile_wp<0>(tile0, xt, acc0, bb, nchunks / 4);
+                } else if (KS == 1) {
                   if (on0) {
                     if (nchunks == 64) acc0 = eng_chain_tile<16>(tile0, xt, acc0);
                     else if (nchunks == 32) acc0 = eng_chain_tile<8>(tile0, xt, acc0);
