@@ -1,19 +1,24 @@
 // lnb_generate -- the cmd/main.go of this repository for the synthetic checkpoint: loads (random-inits)
 // Llama-3.1-8B on device 0 through the C++ host mirror, runs the reference generate loop on the fixed
 // 8-token prompt and prints the generated token ids and the decode rate.
-// Build: make -C host      Run: host/lnb_generate [seq_len=136] [strict|fast] [tiny | <modelDir>] [batch=N]
+// Build: make -C host      Run: host/lnb_generate [seq_len=136] [strict|fast] [tiny | <modelDir>] [batch=N] [logprobs=N]
 // batch=N: N prompts (SURVEY 8d: prompt b = ids[1:] + 977 b) generated together, one pass over the weights per step.
 // batch=N slots=K: the same N prompts through K live sequences with continuous batching (inference::GenerateTokensContinuous).
 // temp=T [top_k=K] [top_p=P] [seed=S]: seeded sampling instead of the greedy argmax (lnb_session_set_sampling); prompt b of a
 // batch samples with seed S + b.
 // spec=K: speculative decoding -- each call verifies the last token plus up to K prompt-lookup drafts in one pass over the
 // weights (lnb_forward_speculative); the generated ids are the same as without it.  Not with slots=.
+// logprobs=N (0..20): after the generated ids, one line per generated token with its logprob, its rank and the top N
+// alternatives (lnb_session_set_logprobs; the raw model distribution, also for sampled tokens).
+// score=TEXT (with <modelDir>/tokenizer.model): TEXT is tokenized without the chat template and scored in chunks of 64 tokens
+// (lnb_score): each token's logprob given the tokens before it, their sum and the perplexity exp(-mean).
 // prompt=TEXT (with <modelDir>/tokenizer.model): TEXT goes through the chat template and the BPE tokenizer, the
 // generated ids come back as text (cmd/main.go's flow without the console UI).
 // <modelDir> holds params.json + consolidated.00.pth (model.LoadModel, src/model/loader.go:18-70);
 // `lnb_generate --write-synthetic <modelDir> [tiny]` writes such a directory for the synthetic weights (host-only).
 // `lnb_generate --tokenize <tokenizer.model> <text>` prints the chat-template token ids of <text> (host-only).
 #include <chrono>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -21,6 +26,36 @@
 #include "lnb_host.hpp"
 
 using namespace lnb_host;
+
+static void print_logprob(const char* tag, const lnb_logprob& r) {
+  printf("%s %d %d %.17g |", tag, r.token, r.rank, r.logprob);
+  for (int j = 0; j < r.n_top; j++) printf(" %d:%.17g", r.top_token[j], r.top_logprob[j]);
+  printf("\n");
+}
+
+// score=TEXT: chunks of kScoreRows scored rows, each call overlapping the previous one by a token
+static const int kScoreRows = 64;
+static void score_text(model::LlamaTransformer& transformer, const model::Tokenizer& tok, int seq_len, int acc, const char* text) {
+  const std::vector<int32_t> ids = tok.TokenizeString(text);
+  const int n = (int)ids.size();
+  if (n < 2) throw Error("score= needs a text of at least two tokens");
+  if (n - 1 > seq_len) throw Error("score= text of " + std::to_string(n) + " tokens exceeds SequenceLength " + std::to_string(seq_len) + " + 1");
+  model::InferenceContext ctx(transformer, seq_len, acc, kScoreRows);
+  ctx.AllowChunkedPrefill(true);
+  ctx.SetLogprobs(0, 0);
+  std::vector<lnb_logprob> recs;
+  for (int start = 0; start + 1 < n; start += kScoreRows) {
+    const int end = std::min(n, start + kScoreRows + 1);
+    const std::vector<lnb_logprob> r = ctx.Score(std::vector<int32_t>(ids.begin() + start, ids.begin() + end), start);
+    recs.insert(recs.end(), r.begin(), r.end());
+  }
+  double sum = 0.0;
+  for (size_t i = 0; i < recs.size(); i++) {
+    printf("score %zu %d %.17g\n", i + 1, recs[i].token, recs[i].logprob);
+    sum += recs[i].logprob;
+  }
+  printf("sum %.17g\nperplexity %.17g\n", sum, std::exp(-sum / (double)recs.size()));
+}
 
 static int write_synthetic_dir(const char* dir, bool tiny) {
   model::ModelArgs args = model::ModelArgs::Llama31_8B();
@@ -107,6 +142,8 @@ int main(int argc, char** argv) {
     if (tiny || transformer.args.vocab_size < 128256) vocab.StopTokenIds = {1000000000};
     int batch = 0, slots = 0;
     const char* prompt_text = nullptr;
+    const char* score_text_arg = nullptr;
+    int logprobs = -1;              // logprobs=N: top N alternatives per generated token
     model::SamplingArgs sampling;   // temp= top_k= top_p= seed= (temp 0, the default: greedy)
     model::SpeculativeArgs spec;    // spec=K: speculative decoding with up to K prompt-lookup drafts per call (0: plain steps)
     for (int i = 1; i < argc; i++) {
@@ -114,12 +151,19 @@ int main(int argc, char** argv) {
       if (!strncmp(argv[i], "batch=", 6)) batch = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "slots=", 6)) slots = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "prompt=", 7)) prompt_text = argv[i] + 7;
+      if (!strncmp(argv[i], "score=", 6)) score_text_arg = argv[i] + 6;
+      if (!strncmp(argv[i], "logprobs=", 9)) logprobs = atoi(argv[i] + 9);
       if (!strncmp(argv[i], "temp=", 5)) sampling.Temperature = (float)atof(argv[i] + 5);
       if (!strncmp(argv[i], "top_k=", 6)) sampling.TopK = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "top_p=", 6)) sampling.TopP = (float)atof(argv[i] + 6);
       if (!strncmp(argv[i], "seed=", 5)) sampling.Seed = strtoull(argv[i] + 5, nullptr, 10);
     }
     std::unique_ptr<model::Tokenizer> tokenizer;
+    if (score_text_arg) {
+      if (!from_dir) throw Error("score= needs a model directory with tokenizer.model");
+      score_text(transformer, model::Tokenizer(std::string(argv[3]) + "/tokenizer.model"), seq_len, acc, score_text_arg);
+      return 0;
+    }
     if (prompt_text) {
       if (!from_dir) throw Error("prompt= needs a model directory with tokenizer.model");
       tokenizer = std::make_unique<model::Tokenizer>(std::string(argv[3]) + "/tokenizer.model");
@@ -137,28 +181,35 @@ int main(int argc, char** argv) {
       for (int b = 0; b < batch; b++)
         for (size_t j = 1; j < prompt.size(); j++) prompts[b][j] = (prompt[j] + 977 * b) % mod;
       std::vector<std::vector<int32_t>> outs(batch);
+      std::vector<std::vector<lnb_logprob>> lps;
       auto b0 = std::chrono::steady_clock::now();
       auto collect = [&](int seq, inference::GenerationState, int32_t tok) { outs[seq].push_back(tok); };
-      if (slots > 0) inference::GenerateTokensContinuous(transformer, vocab, seq_len, acc, prompts, slots, std::max(slots, 64), collect, &sampling);
-      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling, speculative);
+      if (slots > 0)
+        inference::GenerateTokensContinuous(transformer, vocab, seq_len, acc, prompts, slots, std::max(slots, 64), collect, &sampling, logprobs,
+                                            &lps);
+      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling, speculative, logprobs, &lps);
       const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - b0).count();
       size_t total = 0;
       for (int b = 0; b < batch; b++) {
         printf("tokens[%d]:", b);
         for (int32_t t : outs[b]) printf(" %d", t);
         printf("\n");
+        const std::string tag = "logprob[" + std::to_string(b) + "]:";
+        if (logprobs >= 0)
+          for (const lnb_logprob& r : lps[(size_t)b]) print_logprob(tag.c_str(), r);
         total += outs[b].size();
       }
       printf("generated %zu tokens for %d prompts in %.1f ms = %.1f tokens/s aggregate (prefill included)\n", total, batch, sec * 1e3, total / sec);
       return 0;
     }
     std::vector<int32_t> out;
+    std::vector<lnb_logprob> lp;
     auto t0 = std::chrono::steady_clock::now();
     std::chrono::steady_clock::time_point t_first;
     inference::GenerateTokens(transformer, vocab, seq_len, acc, prompt, [&](inference::GenerationState, int32_t tok) {
       if (out.empty()) t_first = std::chrono::steady_clock::now();
       out.push_back(tok);
-    }, &sampling, speculative);
+    }, &sampling, speculative, logprobs, &lp);
     auto t1 = std::chrono::steady_clock::now();
     if (tokenizer) printf("text: %s\n", tokenizer->TokenBatchToString(out).c_str());
     printf("tokens:");
@@ -167,6 +218,7 @@ int main(int argc, char** argv) {
     printf("\ngenerated %zu tokens (%s); prefill+first token %.1f ms; decode %.2f tokens/s through the reference-shaped host loop\n",
            out.size(), acc == LNB_ACC_STRICT ? "strict" : "fast", std::chrono::duration<double>(t_first - t0).count() * 1e3,
            out.size() > 1 ? (out.size() - 1) / dec_s : 0.0);
+    for (const lnb_logprob& r : lp) print_logprob("logprob:", r);
   } catch (const std::exception& e) {
     fprintf(stderr, "error: %s\n", e.what());
     return 1;

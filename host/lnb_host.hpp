@@ -333,6 +333,21 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
     const lnb_sampling p{a->Temperature, a->TopK, a->TopP, a->Seed};
     check(lnb_session_set_sampling(h_, seq, &p));
   }
+  // EXTENSION: token log-probabilities (lnb_session_set_logprobs).  topN 0..20 turns them on for sequence seq, -1 off; every
+  // token the context then emits for seq writes the record of the position it occupies (the raw model distribution).
+  void SetLogprobs(int seq, int topN) { check(lnb_session_set_logprobs(h_, seq, topN)); }
+  // records [pos0, pos0 + n) of sequence seq (token -1: never written)
+  std::vector<lnb_logprob> ReadLogprobs(int seq, int pos0, int n) {
+    std::vector<lnb_logprob> out((size_t)n);
+    check(lnb_session_logprobs_read(h_, seq, pos0, n, out.data()));
+    return out;
+  }
+  // lnb_score: the log-probability of tokens[1..] given what precedes them, one forward of the active sequence over
+  // tokens[0 .. n-1) at startPos -> the records of positions startPos + 1 .. startPos + n - 1
+  std::vector<lnb_logprob> Score(const std::vector<int32_t>& tokens, int startPos, int seq = 0) {
+    check(lnb_score(h_, tokens.data(), (int)tokens.size(), startPos));
+    return ReadLogprobs(seq, startPos + 1, (int)tokens.size() - 1);
+  }
   // Forward + last-row ml.Argmax in one call (inference.go:202-216), 4-byte read-back
   int32_t ForwardArgmax(const std::vector<int32_t>& tokens, int startPos) {
     int32_t next = -1;
@@ -431,7 +446,8 @@ enum GenerationState { GSInProgress = 0, GSFinishedByReachingEOS = 1, GSFinished
 // time through the stop logic of generateTokensInternal (inference.go:218-248).  emit(sequence, state, token).
 inline void GenerateSpeculative(model::InferenceContext& infContext, const model::Vocabulary& vocab,
                                 std::vector<std::vector<int32_t>>& hists, std::vector<int> live, const model::SpeculativeArgs& spec,
-                                const std::function<void(int, GenerationState, int32_t)>& emit) {
+                                const std::function<void(int, GenerationState, int32_t)>& emit,
+                                std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr) {
   const int seqLen = infContext.SequenceLength;
   const int budget = std::min(8, infContext.MaxRows());
   if ((int)live.size() > budget) throw Error("more live sequences than rows in a speculative call");
@@ -454,10 +470,13 @@ inline void GenerateSpeculative(model::InferenceContext& infContext, const model
     for (size_t k = 0; k < segs.size(); k++) {
       const int i = segs[k].seq;
       bool finished = false;
+      std::vector<lnb_logprob> recs;   // the records of the accepted positions
+      if (logprobsOut) recs = infContext.ReadLogprobs(i, segs[k].startPos + 1, accepted[k] + 1);
       for (int j = 0; j <= accepted[k] && !finished; j++) {
         const int32_t tok = next[r0 + j];
         const int curPos = segs[k].startPos + 1 + j;
         hists[i].push_back(tok);
+        if (logprobsOut) (*logprobsOut)[(size_t)i].push_back(recs[(size_t)j]);
         bool eos = false;
         for (int32_t s : vocab.StopTokenIds) eos |= (s == tok);
         const GenerationState st = eos ? GSFinishedByReachingEOS : (curPos + 1 == seqLen ? GSFinishedByReachingSeqLen : GSInProgress);
@@ -471,14 +490,18 @@ inline void GenerateSpeculative(model::InferenceContext& infContext, const model
   }
 }
 
-// generateTokensInternal (inference.go:173-254); `emit` plays generatedTokensCh
+// generateTokensInternal (inference.go:173-254); `emit` plays generatedTokensCh.  EXTENSION: logprobs 0..20 turns on token
+// log-probabilities; logprobsOut (or nullptr) then gets one record per emitted token, in order.
 inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                            const std::vector<int32_t>& promptTokens, const std::function<void(GenerationState, int32_t)>& emit,
-                           const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr) {
+                           const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr,
+                           int logprobs = -1, std::vector<lnb_logprob>* logprobsOut = nullptr) {
   // the prefill call carries the whole prompt: size the session's row buffers for it
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max<int>(8, (int)promptTokens.size()));
   const bool samples = sampling && sampling->Samples();
   if (samples) infContext.SetSampling(0, sampling);   // the sampled token instead of Slice + ml.Argmax
+  if (logprobs >= 0) infContext.SetLogprobs(0, logprobs);
+  if (logprobs < 0) logprobsOut = nullptr;
   const int promptLength = (int)promptTokens.size();
   if (promptLength >= infContext.SequenceLength)
     throw Error("context SequenceLength " + std::to_string(infContext.SequenceLength) + " must be higher than prompt tokens length " +
@@ -501,6 +524,7 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
     }
     if (tokens[curPos] != vocab.PadId) nextTokenId = tokens[curPos];               // :218-226
     tokens[curPos] = nextTokenId;
+    if (logprobsOut) logprobsOut->push_back(infContext.ReadLogprobs(0, curPos, 1)[0]);
     bool eos = false;
     for (int32_t s : vocab.StopTokenIds) eos |= (s == nextTokenId);
     prevPos = curPos;
@@ -509,7 +533,10 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
     emit(GSInProgress, nextTokenId);
     if (speculative) {   // EXTENSION: the prompt is in the cache; from here on every call verifies drafts (same stream)
       std::vector<std::vector<int32_t>> hists{std::vector<int32_t>(tokens.begin(), tokens.begin() + curPos + 1)};
-      GenerateSpeculative(infContext, vocab, hists, {0}, *speculative, [&](int, GenerationState st, int32_t tok) { emit(st, tok); });
+      std::vector<std::vector<lnb_logprob>> lp(1);
+      GenerateSpeculative(infContext, vocab, hists, {0}, *speculative, [&](int, GenerationState st, int32_t tok) { emit(st, tok); },
+                          logprobsOut ? &lp : nullptr);
+      if (logprobsOut) logprobsOut->insert(logprobsOut->end(), lp[0].begin(), lp[0].end());
       break;
     }
   }
@@ -517,14 +544,20 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
 
 // The consumer InferenceEngine.TokenizeBatch (src/inference/tokenize.go:97-107) never got in the reference
 // (SURVEY 8f-4): every prompt runs the loop above -- own KV cache, positions and stop condition -- but all
-// sequences advance together, one pass over the weights per step.  emit(sequence, state, token).
+// sequences advance together, one pass over the weights per step.  emit(sequence, state, token).  logprobs / logprobsOut as in
+// GenerateTokens, one list per prompt.
 inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                                 const std::vector<std::vector<int32_t>>& prompts,
                                 const std::function<void(int, GenerationState, int32_t)>& emit,
-                                const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr) {
+                                const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr,
+                                int logprobs = -1, std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr) {
   const int n = (int)prompts.size();
   if (n < 1) throw Error("empty prompt batch");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, n), n);
+  if (logprobs >= 0)
+    for (int i = 0; i < n; i++) infContext.SetLogprobs(i, logprobs);
+  if (logprobs < 0) logprobsOut = nullptr;
+  if (logprobsOut) logprobsOut->assign((size_t)n, {});
   if (sampling && sampling->Samples())
     for (int i = 0; i < n; i++) {
       const model::SamplingArgs a = sampling->ForPrompt(i);
@@ -540,6 +573,7 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
   auto record = [&](int i, int32_t tok, int curPos) {   // :218-248
     cur[i] = tok;
     pos[i] = curPos;
+    if (logprobsOut) (*logprobsOut)[(size_t)i].push_back(infContext.ReadLogprobs(i, curPos, 1)[0]);
     bool eos = false;
     for (int32_t s : vocab.StopTokenIds) eos |= (s == tok);
     GenerationState st = eos ? GSFinishedByReachingEOS : (curPos + 1 == seqLen ? GSFinishedByReachingSeqLen : GSInProgress);
@@ -558,7 +592,7 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
       hists[i].push_back(cur[i]);
       if (!done[i]) live.push_back(i);
     }
-    GenerateSpeculative(infContext, vocab, hists, live, *speculative, emit);
+    GenerateSpeculative(infContext, vocab, hists, live, *speculative, emit, logprobsOut);
     return;
   }
   while (n_done < n) {
@@ -573,11 +607,13 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
 // scheduler of the Python mirror's GenerateTokensContinuous.  Every step is ONE forward: each decoding sequence gets its
 // row, the rest of the stepTokens-row budget goes to prompt chunks first in first out, a prompt whose last chunk is in the
 // step emits its first token, a finished slot takes the next waiting prompt at position 0; steps without prompt rows run
-// lnb_forward_batch.  emit(prompt index, state, token); per prompt the stream is GenerateTokens' own.
+// lnb_forward_batch.  emit(prompt index, state, token); per prompt the stream is GenerateTokens' own.  logprobs / logprobsOut
+// as in GenerateTokens, one list per prompt.
 inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength,
                                      int accMode, const std::vector<std::vector<int32_t>>& prompts, int slots, int stepTokens,
                                      const std::function<void(int, GenerationState, int32_t)>& emit,
-                                     const model::SamplingArgs* sampling = nullptr) {
+                                     const model::SamplingArgs* sampling = nullptr, int logprobs = -1,
+                                     std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr) {
   if (slots < 1 || slots > 8) throw Error("slots must be in [1, 8]");
   if (stepTokens < slots) throw Error("stepTokens must be at least slots (every decoding sequence gets a row)");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, stepTokens), slots);
@@ -586,6 +622,10 @@ inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const
     if (p.empty() || (int)p.size() >= seqLen)
       throw Error("context SequenceLength " + std::to_string(seqLen) + " must be higher than prompt tokens length " + std::to_string(p.size()) +
                   " (and prompts must not be empty)");
+  if (logprobs >= 0)
+    for (int k = 0; k < slots; k++) infContext.SetLogprobs(k, logprobs);
+  if (logprobs < 0) logprobsOut = nullptr;
+  if (logprobsOut) logprobsOut->assign(prompts.size(), {});
   struct Slot { int i = -1, fed = 0, order = 0; int32_t cur = -1; int pos = 0; bool decoding = false; };
   std::vector<Slot> slot((size_t)slots);
   size_t next_prompt = 0;
@@ -644,6 +684,7 @@ inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const
       for (int32_t st : vocab.StopTokenIds) eos |= (st == tok);
       const GenerationState state = eos ? GSFinishedByReachingEOS : (curPos + 1 == seqLen ? GSFinishedByReachingSeqLen : GSInProgress);
       const int i = s.i;
+      if (logprobsOut) (*logprobsOut)[(size_t)i].push_back(infContext.ReadLogprobs(seg_slot[j], curPos, 1)[0]);
       if (state != GSInProgress) { s.i = -1; live--; }
       emit(i, state, tok);
     }

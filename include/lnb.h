@@ -317,6 +317,43 @@ typedef struct {
  * stream or invalidate a captured decode graph; switching the active sequence between greedy and sampled re-captures it. */
 int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampling* p);
 
+/* EXTENSION: token log-probabilities, computed on the device (csrc/logprob.cuh) and finished on the host (DESIGN.md §9d).
+ * For one row of logits l and a token t: the rank order is the sampler's (l descending, index ascending), m the rank-0
+ * logit, sum = the sum over the vocabulary of floor(2^40 exp(f32(l_i - m))) (0 below -28: the sampler's weights at
+ * temperature 1, integers, so any reduction order gives the same bits), rank(t) = 1 + the tokens ranked before t, and
+ * logprob(t) = (f64(l_t) - f64(m)) - log(f64(sum) 2^-40), within 1.2e-6 of the exact log-softmax at 128256 tokens.  The
+ * logprob is always the raw model distribution (temperature 1, no top-k or top-p cut), also for sampled tokens.  A row
+ * whose rank-0 logit is +inf or NaN gives NaN logprobs (rank 1 for its rank-0 token); a -inf logit gives -inf. */
+#define LNB_LOGPROBS_TOP_MAX 20
+typedef struct {
+  int32_t token;     /* the scored token; -1: the position was never written */
+  int32_t rank;      /* 1 = the greedy token */
+  double logprob;
+  int32_t n_top;     /* entries of top_token / top_logprob in use */
+  int32_t top_token[LNB_LOGPROBS_TOP_MAX];   /* the n_top first tokens in rank order */
+  double top_logprob[LNB_LOGPROBS_TOP_MAX];
+} lnb_logprob;
+/* top_n in [0, 20] turns logprobs on for sequence `seq` from its next forward on, -1 turns them off (the default).  Every
+ * token a forward emits for that sequence (lnb_forward / lnb_forward_device argmax_last, lnb_forward_batch /
+ * lnb_forward_ragged argmax_out, lnb_forward_speculative next_out, lnb_decode_run tokens_out; greedy or sampled) then writes
+ * the record of the position it will occupy: record p of a sequence describes the token at position p given the tokens
+ * before it, whatever the batching, chunking or scheduling.  Records of speculative rows beyond the accepted drafts, and of
+ * ragged segments that end a non-final prompt chunk, describe tokens the caller discards: only positions whose token was
+ * emitted or scored are meaningful (the stale-row rule of lnb_forward_speculative).  The first call that turns logprobs on
+ * allocates records for every sequence and position, about 192 bytes each (LNB_ENOMEM with the bytes; the session stays as
+ * it was).  LNB_EINVAL with nothing changed: seq outside [0, n_seq), top_n outside [-1, 20], tp_size > 1 (not built).
+ * Turning logprobs on or off for the active sequence re-captures a decode graph; changing top_n does not. */
+int lnb_session_set_logprobs(lnb_session* s, int seq, int top_n);
+/* records [pos0, pos0 + n) of sequence `seq`, finished on the host, to out[n].  LNB_EINVAL: seq out of range, n < 1, or a
+ * range outside [1, seq_len]. */
+int lnb_session_logprobs_read(lnb_session* s, int seq, int pos0, int n, lnb_logprob* out);
+/* Scoring: ONE forward of the active sequence over tokens[0 .. n-1) at positions start_pos .., with the LM head over all
+ * those rows, then the records of positions start_pos + 1 .. start_pos + n - 1, whose tokens are tokens[1 .. n).  Chunked
+ * scoring overlaps by one token: the next call starts at start_pos + n - 1 with tokens[n - 1].  2 <= n <= max_rows + 1,
+ * start_pos + n <= seq_len + 1; start_pos > 0 needs lnb_session_set_chunked_prefill as lnb_forward does.  LNB_ESTATE when the
+ * active sequence has logprobs off.  Afterwards a lnb_forward_device handle is stale. */
+int lnb_score(lnb_session* s, const int32_t* tokens, int n, int start_pos);
+
 /* Fused collective for tensor-parallel decode: instead of ncclAllReduce after Wo / w2, every rank's GEMV
  * epilogue stores its fp32 partials straight into all peers' memory over NVLink and a small kernel
  * reduces the N slots in rank order (bit-identical on every rank).  Setup: every rank exports the 64-byte
@@ -393,6 +430,9 @@ int lnb_op_argmax_f32(const float* x, int rows, int cols, int32_t* out);
 /* EXTENSION: the sampler of lnb_session_set_sampling alone on host rows (1..8 rows): logits[rows, vocab], parameters
  * p[rows], pos_next[rows] (the p_next of each draw) -> out[rows]; temperature 0 gives the greedy ml.Argmax (:513-548) */
 int lnb_op_sample_f32(const float* logits, int rows, int vocab, const lnb_sampling* p, const int32_t* pos_next, int32_t* out);
+/* EXTENSION: the logprob kernels of lnb_session_set_logprobs alone on host rows: logits[rows, vocab], targets[rows],
+ * top_n in [0, 20] -> out[rows] */
+int lnb_op_logprobs_f32(const float* logits, int rows, int vocab, const int32_t* targets, int top_n, lnb_logprob* out);
 /* ml.Fwd_Get_Rows (operations_impl.go:142-173) */
 int lnb_op_get_rows_bf16(const uint16_t* emb, const int32_t* tokens, uint16_t* out, int S, int vocab, int dim);
 

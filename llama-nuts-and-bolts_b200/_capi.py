@@ -29,6 +29,14 @@ class SamplingC(C.Structure):   # lnb_sampling
     _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("seed", C.c_uint64)]
 
 
+LNB_LOGPROBS_TOP_MAX = 20
+
+
+class LogprobC(C.Structure):   # lnb_logprob
+    _fields_ = [("token", C.c_int32), ("rank", C.c_int32), ("logprob", C.c_double), ("n_top", C.c_int32),
+                ("top_token", C.c_int32 * LNB_LOGPROBS_TOP_MAX), ("top_logprob", C.c_double * LNB_LOGPROBS_TOP_MAX)]
+
+
 u16p = C.POINTER(C.c_uint16)
 f32p = C.POINTER(C.c_float)
 i32p = C.POINTER(C.c_int32)
@@ -73,6 +81,9 @@ SIGNATURES = {
     "lnb_forward_ragged": (C.c_int, [vp, C.c_int, i32p, i32p, i32p, i32p, f32p, i32p]),
     "lnb_forward_speculative": (C.c_int, [vp, C.c_int, i32p, i32p, i32p, i32p, f32p, i32p, i32p]),
     "lnb_session_set_sampling": (C.c_int, [vp, C.c_int, C.POINTER(SamplingC)]),
+    "lnb_session_set_logprobs": (C.c_int, [vp, C.c_int, C.c_int]),
+    "lnb_session_logprobs_read": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp]),
+    "lnb_score": (C.c_int, [vp, i32p, C.c_int, C.c_int]),
     "lnb_session_read": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64]),
     "lnb_session_set_layer_limit": (C.c_int, [vp, C.c_int]),
     "lnb_session_launch_count": (C.c_int64, [vp]),
@@ -113,6 +124,7 @@ SIGNATURES = {
     "lnb_op_softmax_f32": (C.c_int, [f32p, f32p, C.c_int, C.c_int]),
     "lnb_op_argmax_f32": (C.c_int, [f32p, C.c_int, C.c_int, i32p]),
     "lnb_op_sample_f32": (C.c_int, [f32p, C.c_int, C.c_int, C.POINTER(SamplingC), i32p, i32p]),
+    "lnb_op_logprobs_f32": (C.c_int, [f32p, C.c_int, C.c_int, i32p, C.c_int, vp]),
     "lnb_op_get_rows_bf16": (C.c_int, [u16p, i32p, u16p, C.c_int, C.c_int, C.c_int]),
 }
 

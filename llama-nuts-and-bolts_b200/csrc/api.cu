@@ -25,6 +25,7 @@
 #include "engine.cuh"
 #include "engine_batch.cuh"
 #include "sample.cuh"
+#include "logprob.cuh"
 #include "pth.hpp"
 #include "tokenizer.hpp"
 
@@ -1152,6 +1153,18 @@ struct lnb_session {
   bool samp_on[8] = {false, false, false, false, false, false, false, false};
   bool graph_sampled = false;               // the captured decode graph ends in the sampler ...
   const float* graph_logits = nullptr;      // ... which reads this logits buffer
+  // token log-probabilities (logprob.cuh, lnb_session_set_logprobs), allocated by the first enable: the records of every
+  // sequence and position, the top_n of each sequence in device memory (a captured graph reads it there), the row table
+  // and scratch of one job of up to lp_rows rows, and the targets of lnb_score
+  LpRecord* d_lp_rec = nullptr;             // [n_seq][seq_len + 1], keyed by the position of the scored token
+  int32_t* d_lp_top = nullptr;              // [n_seq]
+  int32_t* d_lp_tgt = nullptr;              // [max_rows]
+  LpRow* d_lp_rows = nullptr;               // [lp_rows]
+  LpRow* h_lp_rows = nullptr;               // pinned staging of d_lp_rows
+  unsigned long long* d_lp_cand = nullptr;  // [lp_rows][slices][LP_TOP], then [lp_rows][slices] + [lp_rows] u32 counters
+  int lp_rows = 0;
+  int lp_top[8] = {-1, -1, -1, -1, -1, -1, -1, -1};   // -1: logprobs off
+  bool graph_lp = false;                    // the captured decode graph ends in the logprob job
 };
 
 static int set_state(lnb_session* s, int pos, int n_rows, int next_token, bool reset_step) {
@@ -1293,6 +1306,8 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
   cudaFree(s->d_rag);
   cudaFree(s->d_samp); cudaFree(s->d_samp_w); cudaFree(s->d_samp_tok); cudaFree(s->d_samp_cand);
+  cudaFree(s->d_lp_rec); cudaFree(s->d_lp_top); cudaFree(s->d_lp_tgt); cudaFree(s->d_lp_rows); cudaFree(s->d_lp_cand);
+  if (s->h_lp_rows) cudaFreeHost(s->h_lp_rows);
   for (auto p : s->ck) cudaFree(p);
   for (auto p : s->cv) cudaFree(p);
   if (s->h_tok) cudaFreeHost(s->h_tok);
@@ -2292,18 +2307,66 @@ static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_
   return launch_sample_job(Launcher{s->stream, LAUNCH_PDL, &s->launches}, J);
 }
 
-// The end of lnb_forward(_device), lnb_forward_batch and lnb_forward_ragged.  Output row i is logits row row0 + i, of
-// sequence seq[i] at next position p_next[i]; rows of sampled sequences draw into samp_out[i].  host_logits (or NULL) gets
-// logits rows [0, logits_rows), s->h_out[0, n) the tokens at d_tok (or NULL), then s->h_out[n] the sampled token of row 0
-// when the sampler writes beside them (samp_out != d_tok).
+// ---- token log-probabilities (logprob.cuh, DESIGN.md §9d) -------------------------------------------------------------
+static int launch_logprob_job(const Launcher& L, const LogprobJob& J, int n) {
+  const dim3 grid((J.V + LP_SLICE - 1) / LP_SLICE, n);
+  int rc = launch_kernel(L, logprob_rank_kernel, grid, dim3(LP_THREADS), 0, J);
+  if (rc) return rc;
+  return launch_kernel(L, logprob_mass_kernel, grid, dim3(LP_THREADS), 0, J);
+}
+// the job over rows d_lp_rows[0, n) (their table uploaded by lp_upload) of s->logits
+static int launch_logprob(lnb_session* s, int n) {
+  const int V = s->m->a.vocab_size, G = (V + LP_SLICE - 1) / LP_SLICE;
+  LogprobJob J{};
+  J.rows = s->d_lp_rows; J.top_n = s->d_lp_top; J.V = V;
+  J.cand = s->d_lp_cand;
+  J.above = reinterpret_cast<unsigned int*>(s->d_lp_cand + (size_t)s->lp_rows * G * LP_TOP);
+  J.done = J.above + (size_t)s->lp_rows * G;
+  return launch_logprob_job(Launcher{s->stream, LAUNCH_PDL, &s->launches}, J, n);
+}
+// row i of the next job: logits row `row` of s->logits, target *target, the record of sequence seq at position pos (+ *pos_ptr)
+static void lp_row(lnb_session* s, int i, int row, const int32_t* target, int seq, int pos, const int32_t* pos_ptr) {
+  LpRow& r = s->h_lp_rows[i];
+  r.logits = s->logits + (size_t)row * s->m->vocab_l;
+  r.target = target;
+  r.rec = s->d_lp_rec + (size_t)seq * (s->seq_len + 1) + pos;
+  r.rec_pos = pos_ptr;
+  r.seq = seq;
+  r.pad = 0;
+}
+// a written record -> its lnb_logprob (out zeroed by the caller)
+static void lp_finish(const LpRecord& r, lnb_logprob* out) {
+  const float m = lnb_logprob_key_logit(r.key[0]);
+  out->token = r.target;
+  out->rank = r.rank;
+  out->logprob = lnb_logprob_finish(r.target_logit, m, r.sum);
+  out->n_top = r.n_top;
+  for (int j = 0; j < r.n_top; j++) {
+    out->top_token[j] = lnb_logprob_key_index(r.key[j]);
+    out->top_logprob[j] = lnb_logprob_finish(lnb_logprob_key_logit(r.key[j]), m, r.sum);
+  }
+}
+static int lp_upload(lnb_session* s, int n) {
+  CU(cudaMemcpyAsync(s->d_lp_rows, s->h_lp_rows, (size_t)n * sizeof(LpRow), cudaMemcpyHostToDevice, s->stream));
+  return 0;
+}
+
+// The end of lnb_forward(_device), lnb_forward_batch, lnb_forward_ragged and lnb_forward_speculative.  Output row i is
+// logits row row0 + i, of sequence seq[i] at next position p_next[i]; rows of sampled sequences draw into samp_out[i], the
+// greedy token of row i is at greedy[i].  Rows of sequences with logprobs on then write the record of p_next[i] for the
+// token they emit.  host_logits (or NULL) gets logits rows [0, logits_rows), s->h_out[0, n) the tokens at d_tok (or NULL),
+// then s->h_out[n] the sampled token of row 0 when the sampler writes beside them (samp_out != d_tok).
 static int call_tail(lnb_session* s, int n, int row0, const int32_t* seq, const int32_t* p_next, int32_t* samp_out,
-                     float* host_logits, int logits_rows, const int32_t* d_tok) {
+                     const int32_t* greedy, float* host_logits, int logits_rows, const int32_t* d_tok) {
   int32_t srow[8], sseq[8], spn[8], sidx[8];
-  int ns = 0;
+  int ns = 0, nl = 0;
   for (int i = 0; i < n; i++)
     if (s->samp_on[seq[i]]) { srow[ns] = row0 + i; sseq[ns] = seq[i]; spn[ns] = p_next[i]; sidx[ns] = i; ns++; }
   int rc;
   if (ns && (rc = launch_sample(s, ns, srow, sseq, spn, sidx, samp_out, false))) return rc;
+  for (int i = 0; i < n; i++)
+    if (s->lp_top[seq[i]] >= 0) lp_row(s, nl++, row0 + i, s->samp_on[seq[i]] ? samp_out + i : greedy + i, seq[i], p_next[i], nullptr);
+  if (nl && ((rc = lp_upload(s, nl)) || (rc = launch_logprob(s, nl)))) return rc;
   lnb_model* m = s->m;
   if (host_logits) {
     const float* src = (m->tp_size > 1) ? s->logits_full : s->logits;
@@ -2319,9 +2382,10 @@ static int call_tail(lnb_session* s, int n, int row0, const int32_t* seq, const 
 // The forward of lnb_forward and lnb_forward_device; the caller holds s->mu.  keep_logits: the logits of the last row, or
 // of all S rows (all_rows), stay in s->logits.  host_logits: NULL, or where those rows are copied (tensor-parallel:
 // gathered from the ranks first).  next_token: NULL, or receives the next token of the last row (greedy unless the active
-// sequence samples); greedy_token: NULL, or receives the greedy token of the last row.
+// sequence samples); greedy_token: NULL, or receives the greedy token of the last row.  score (lnb_score, with all_rows):
+// no token is emitted; row i writes the logprob record of position start_pos + 1 + i for the target d_lp_tgt[i].
 static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int start_pos, bool keep_logits, bool all_rows,
-                          float* host_logits, int32_t* next_token, int32_t* greedy_token = nullptr) {
+                          float* host_logits, int32_t* next_token, int32_t* greedy_token = nullptr, bool score = false) {
   if (!tokens) return fail(LNB_EINVAL, "NULL argument");
   if (S <= 0) return fail(LNB_EINVAL, "empty token array");  // llamatransformer.go:146-148
   if (S > s->max_rows) return fail(LNB_EINVAL, "S %d exceeds the session's max_rows %d", S, s->max_rows);
@@ -2336,8 +2400,8 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
   CU(cudaSetDevice(m->device));
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
   const int32_t seq = s->active_seq, p_next = start_pos + S;
-  const bool samp = s->samp_on[seq];   // the sampler reads the last row's logits
-  const int lrows = keep_logits ? (all_rows ? S : 1) : (samp ? 1 : 0);
+  const bool samp = s->samp_on[seq];   // the sampler and the logprob job read the last row's logits
+  const int lrows = keep_logits ? (all_rows ? S : 1) : ((samp || s->lp_top[seq] >= 0) ? 1 : 0);
   int rc;
   if (lrows && (rc = ensure_logits(s, (size_t)(keep_logits && all_rows ? s->max_rows : 1)))) return rc;
   if (S == 1 && engine_ok(s)) {
@@ -2350,8 +2414,13 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
     if ((rc = set_state(s, start_pos, S, -1, false))) return rc;
     if ((rc = enqueue_forward(s, rows_single(s, S, s->d_tokens, lrows, false, host_logits != nullptr)))) return rc;
   }
+  if (score) {
+    for (int i = 0; i < S; i++) lp_row(s, i, i, s->d_lp_tgt + i, seq, start_pos + 1 + i, nullptr);
+    if ((rc = lp_upload(s, S)) || (rc = launch_logprob(s, S))) return rc;
+    return call_tail(s, 0, 0, &seq, &p_next, nullptr, nullptr, nullptr, 0, nullptr);
+  }
   // the sampled token goes to d_samp_tok; st->next_token keeps the greedy one (lnb_session_logits_argmax)
-  if ((rc = call_tail(s, 1, lrows - 1, &seq, &p_next, s->d_samp_tok, host_logits, lrows,
+  if ((rc = call_tail(s, 1, lrows - 1, &seq, &p_next, s->d_samp_tok, &s->st->next_token, host_logits, lrows,
                       (next_token || greedy_token) ? &s->st->next_token : nullptr)))
     return rc;
   if (next_token) *next_token = samp ? s->h_out[1] : s->h_out[0];
@@ -2533,6 +2602,92 @@ extern "C" int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampl
   return 0;
 }
 
+// ---- token log-probabilities: records, switches and scoring (logprob.cuh, DESIGN.md §9d) ------------------------------
+extern "C" int lnb_session_set_logprobs(lnb_session* s, int seq, int top_n) {
+  if (!s) return fail(LNB_EINVAL, "session is NULL");
+  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  if (top_n < -1 || top_n > LNB_LOGPROBS_TOP_MAX) return fail(LNB_EINVAL, "top_n %d must be in [-1, %d] (-1: off)", top_n, LNB_LOGPROBS_TOP_MAX);
+  if (s->m->tp_size > 1)
+    return fail(LNB_EINVAL, "logprobs are not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", s->m->tp_size);
+  const int V = s->m->a.vocab_size;
+  if (V > LP_MAX_VOCAB) return fail(LNB_EINVAL, "logprobs serve vocabularies of up to %d tokens (this model has %d)", LP_MAX_VOCAB, V);
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(s->m->device));
+  if (top_n >= 0 && !s->d_lp_rec) {   // records of every sequence and position, the job's table and scratch; all or nothing
+    const int rows = std::max(s->max_rows, 8), G = (V + LP_SLICE - 1) / LP_SLICE;
+    const size_t b_rec = (size_t)s->n_seq * (s->seq_len + 1) * sizeof(LpRecord), b_top = (size_t)s->n_seq * 4,
+                 b_tgt = (size_t)s->max_rows * 4, b_rows = (size_t)rows * sizeof(LpRow),
+                 b_cand = (size_t)rows * G * (LP_TOP * 8 + 4) + (size_t)rows * 4;
+    LpRecord* d_rec = nullptr;
+    int32_t *d_top = nullptr, *d_tgt = nullptr;
+    LpRow *d_rows = nullptr, *h_rows = nullptr;
+    unsigned long long* d_cand = nullptr;
+    cudaError_t e = cudaMalloc((void**)&d_rec, b_rec);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_top, b_top);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_tgt, b_tgt);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_rows, b_rows);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_cand, b_cand);
+    if (e == cudaSuccess) e = cudaMallocHost((void**)&h_rows, b_rows);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_rec, 0xff, b_rec, s->stream);   // target -1: never written
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_top, 0xff, b_top, s->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_cand, 0, b_cand, s->stream);     // the merge counters start at 0
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      cudaStreamSynchronize(s->stream);
+      cudaFree(d_rec); cudaFree(d_top); cudaFree(d_tgt); cudaFree(d_rows); cudaFree(d_cand);
+      if (h_rows) cudaFreeHost(h_rows);
+      cudaGetLastError();
+      return fail(LNB_ENOMEM, "logprob records and scratch: %zu bytes of device memory asked for (records %zu): %s",
+                  b_rec + b_top + b_tgt + b_rows + b_cand, b_rec, cudaGetErrorString(e));
+    }
+    s->d_lp_rec = d_rec; s->d_lp_top = d_top; s->d_lp_tgt = d_tgt; s->d_lp_rows = d_rows; s->d_lp_cand = d_cand; s->h_lp_rows = h_rows;
+    s->lp_rows = rows;
+  }
+  if (s->d_lp_top) {   // stream-ordered; a captured decode graph reads the slot when it replays
+    if (top_n >= 0 || s->lp_top[seq] >= 0) {
+      logprob_set_top_n_kernel<<<1, 1, 0, s->stream>>>(s->d_lp_top + seq, top_n);
+      CU(cudaGetLastError());
+    }
+  }
+  s->lp_top[seq] = top_n;
+  return 0;
+}
+
+extern "C" int lnb_session_logprobs_read(lnb_session* s, int seq, int pos0, int n, lnb_logprob* out) {
+  if (!s || !out) return fail(LNB_EINVAL, "NULL argument");
+  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  if (n < 1 || pos0 < 1 || (int64_t)pos0 + n - 1 > s->seq_len)
+    return fail(LNB_EINVAL, "positions [%d, %lld) outside [1, %d]", pos0, (long long)pos0 + n, s->seq_len);
+  std::lock_guard<std::mutex> lk(s->mu);
+  memset(out, 0, (size_t)n * sizeof(lnb_logprob));
+  for (int i = 0; i < n; i++) out[i].token = -1;
+  if (!s->d_lp_rec) return 0;   // logprobs were never on: nothing was written
+  CU(cudaSetDevice(s->m->device));
+  std::vector<LpRecord> rec((size_t)n);
+  CU(cudaMemcpyAsync(rec.data(), s->d_lp_rec + (size_t)seq * (s->seq_len + 1) + pos0, (size_t)n * sizeof(LpRecord),
+                     cudaMemcpyDeviceToHost, s->stream));
+  CU(cudaStreamSynchronize(s->stream));
+  for (int i = 0; i < n; i++)
+    if (rec[i].target >= 0) lp_finish(rec[i], out + i);
+  return 0;
+}
+
+extern "C" int lnb_score(lnb_session* s, const int32_t* tokens, int n, int start_pos) {
+  if (!s || !tokens) return fail(LNB_EINVAL, "NULL argument");
+  if (n < 2 || n - 1 > s->max_rows) return fail(LNB_EINVAL, "n %d must be in [2, max_rows + 1 = %d]", n, s->max_rows + 1);
+  if (tokens[n - 1] < 0 || tokens[n - 1] >= s->m->a.vocab_size) return fail(LNB_EINVAL, "token id %d out of range", tokens[n - 1]);
+  std::lock_guard<std::mutex> lk(s->mu);
+  if (s->lp_top[s->active_seq] < 0)
+    return fail(LNB_ESTATE, "sequence %d has logprobs off (lnb_session_set_logprobs)", s->active_seq);
+  CU(cudaSetDevice(s->m->device));
+  // the targets, stream-ordered before the job: staged in the pinned h_tok words [max_rows, 2 max_rows), beside the forward's
+  // token ids [0, n - 1); no earlier call still reads them (every call synchronises its stream before it returns)
+  int32_t* h_tgt = s->h_tok + s->max_rows;
+  memcpy(h_tgt, tokens + 1, (size_t)(n - 1) * 4);
+  CU(cudaMemcpyAsync(s->d_lp_tgt, h_tgt, (size_t)(n - 1) * 4, cudaMemcpyHostToDevice, s->stream));
+  return forward_locked(s, tokens, n - 1, start_pos, true, true, nullptr, nullptr, nullptr, true);
+}
+
 // One decode step for n independent sequences (rows 0..n-1 = sequences 0..n-1): tokens[i] is fed at
 // positions[i] of sequence i.  The weights are streamed ONCE for all rows (the reference would run n
 // separate Forward calls on n InferenceContexts, SURVEY F10; every row sees exactly the arithmetic of its
@@ -2556,8 +2711,8 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
   CU(cudaMemcpyAsync(s->d_tokens, s->h_tok, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
   CU(cudaMemcpyAsync(s->d_pos_arr, s->h_pos, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
   int32_t seq[8], p_next[8];
-  bool samp = false;
-  for (int i = 0; i < n; i++) { seq[i] = i; p_next[i] = positions[i] + 1; samp |= s->samp_on[i]; }
+  bool samp = false;   // a row samples or has logprobs on: the engine stores the logits
+  for (int i = 0; i < n; i++) { seq[i] = i; p_next[i] = positions[i] + 1; samp |= s->samp_on[i] || s->lp_top[i] >= 0; }
   if (batch_engine_ok(s)) {
     // ONE launch of the batch engine: every weight matrix streamed once for all n sequences
     if ((rc = batch_engine_build(s, (logits || samp) ? s->logits : nullptr))) return rc;
@@ -2569,7 +2724,7 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
     if ((rc = set_state(s, 0, n, -1, false))) return rc;
     if ((rc = enqueue_forward(s, rows_batch(s, n)))) return rc;
   }
-  if ((rc = call_tail(s, n, 0, seq, p_next, s->d_next_arr, logits, n, argmax_out ? s->d_next_arr : nullptr))) return rc;
+  if ((rc = call_tail(s, n, 0, seq, p_next, s->d_next_arr, s->d_next_arr, logits, n, argmax_out ? s->d_next_arr : nullptr))) return rc;
   if (argmax_out) memcpy(argmax_out, s->h_out, (size_t)n * 4);
   return 0;
 }
@@ -2655,7 +2810,7 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
   if ((rc = enqueue_forward(s, rows_ragged(s, rows, n_segs)))) return rc;
   int32_t p_next[8];
   for (int i = 0; i < n_segs; i++) p_next[i] = start_pos[i] + len[i];
-  if ((rc = call_tail(s, n_segs, 0, seq, p_next, s->d_next_arr, logits, n_segs, argmax_out ? s->d_next_arr : nullptr))) return rc;
+  if ((rc = call_tail(s, n_segs, 0, seq, p_next, s->d_next_arr, s->d_next_arr, logits, n_segs, argmax_out ? s->d_next_arr : nullptr))) return rc;
   if (argmax_out) memcpy(argmax_out, s->h_out, (size_t)n_segs * 4);
   return 0;
 }
@@ -2729,12 +2884,13 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
   if (!eng && !s->sdpa_smem_decode && !s->ss.sc)
     return fail(LNB_EINVAL, "speculative calls beyond the shared-memory attention kernel need head_dim <= 128 and n_rep <= 8");
   int32_t row_seq[8], row_pos[8];
-  bool samp = false;
+  bool samp = false, lp = false;
   for (int i = 0, r = 0; i < n_segs; i++)
     for (int k = 0; k <= n_draft[i]; k++, r++) {
       row_seq[r] = seq[i];
       row_pos[r] = start_pos[i] + k;
       samp |= s->samp_on[seq[i]];
+      lp |= s->lp_top[seq[i]] >= 0;
     }
   if (!s->d_rag) {   // the row map (shared with ragged calls)
     const cudaError_t e = cudaMalloc((void**)&s->d_rag, row_map_words(s->max_rows) * 4);
@@ -2756,7 +2912,7 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
   CU(cudaMemcpyAsync(s->d_rag, h, (size_t)3 * rows * 4, cudaMemcpyHostToDevice, s->stream));
   if (eng) {
     // ONE launch of the batch engine: every weight matrix streamed once for all rows
-    if ((rc = batch_engine_build(s, (logits || samp) ? s->logits : nullptr))) return rc;
+    if ((rc = batch_engine_build(s, (logits || samp || lp) ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, rows, s->d_rag, s->d_rag + 2 * rows, s->d_rag + rows))) return rc;
   } else {
     if ((rc = set_state(s, 0, rows, -1, false))) return rc;
@@ -2764,7 +2920,7 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
   }
   int32_t p_next[8];
   for (int r = 0; r < rows; r++) p_next[r] = row_pos[r] + 1;
-  if ((rc = call_tail(s, rows, 0, row_seq, p_next, s->d_next_arr, logits, rows, s->d_next_arr))) return rc;
+  if ((rc = call_tail(s, rows, 0, row_seq, p_next, s->d_next_arr, s->d_next_arr, logits, rows, s->d_next_arr))) return rc;
   // acceptance: row j of a segment predicts the token at position start + j + 1, which draft j + 1 claims
   for (int i = 0, r0 = 0; i < n_segs; r0 += 1 + n_draft[i], i++) {
     int acc = 0;
@@ -2786,10 +2942,14 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward
   int rc;
   // a sampled sequence decodes on the kernel chain (the persistent engine feeds back the greedy token inside the kernel):
-  // each step keeps its logits row and ends in the sampler, whose token is the next step's input
-  const bool samp = s->samp_on[s->active_seq];
+  // each step keeps its logits row and ends in the sampler, whose token is the next step's input.  A sequence with
+  // logprobs on decodes on the chain too, each step then ending in the logprob job keyed on st->pos (= p_next).
+  const int seq = s->active_seq;
+  const bool samp = s->samp_on[seq], lp = s->lp_top[seq] >= 0, keep = samp || lp;
   if (samp && engine_ok(s)) g_err = "the active sequence samples: lnb_decode_run runs the kernel chain (the decode engine has no sampler)";
-  if (!samp && engine_ok(s)) {
+  else if (lp && engine_ok(s))
+    g_err = "the active sequence has logprobs on: lnb_decode_run runs the kernel chain (the decode engine keeps no logits row)";
+  if (!keep && engine_ok(s)) {
     // the whole run is ONE launch of the persistent engine: n_steps forwards, the greedy token fed back on the device
     if ((rc = engine_build(s, -1, nullptr))) return rc;
     if ((rc = set_state(s, start_pos, 1, first_token, true))) return rc;
@@ -2805,17 +2965,23 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     if (tokens_out) memcpy(tokens_out, s->h_out, (size_t)n_steps * 4);
     return use_graph ? 1 : 0;   // (no graph is needed: there is nothing left to replay)
   }
-  if (samp && (rc = ensure_logits(s, 1))) return rc;
-  if (s->graph_tried && (s->graph_sampled != samp || (samp && s->graph_logits != s->logits))) drop_graph(s);
+  if (keep && (rc = ensure_logits(s, 1))) return rc;
+  if (s->graph_tried && (s->graph_sampled != samp || s->graph_lp != lp || (keep && s->graph_logits != s->logits))) drop_graph(s);
+  if (lp) {   // the job's one row, read by every step (and by the graph's replays): the token st->next_token, record st->pos
+    lp_row(s, 0, 0, &s->st->next_token, seq, 0, &s->st->pos);
+    if ((rc = lp_upload(s, 1))) return rc;
+  }
   auto step = [&]() -> int {
-    const int r = enqueue_forward(s, rows_single(s, 1, nullptr, samp ? 1 : 0, true, true));
-    if (r || !samp) return r;
-    const int32_t row = 0, seq = s->active_seq, pn = -1;
-    return launch_sample(s, 1, &row, &seq, &pn, nullptr, nullptr, true);
+    int r = enqueue_forward(s, rows_single(s, 1, nullptr, keep ? 1 : 0, true, true));
+    if (r) return r;
+    const int32_t row = 0, pn = -1;
+    if (samp && (r = launch_sample(s, 1, &row, &seq, &pn, nullptr, nullptr, true))) return r;
+    return lp ? launch_logprob(s, 1) : 0;
   };
   if (use_graph && !s->graph && !s->graph_tried) {
     s->graph_tried = true;
     s->graph_sampled = samp;
+    s->graph_lp = lp;
     s->graph_logits = s->logits;
     cudaGraph_t g = nullptr;
     const int64_t saved = s->launches;
@@ -3415,6 +3581,41 @@ extern "C" int lnb_op_sample_f32(const float* logits, int rows, int vocab, const
   if ((rc = launch_sample_job(Launcher{nullptr, LAUNCH_PLAIN, nullptr}, J))) return rc;
   if ((rc = op_finish())) return rc;
   D2H(out, dout, (size_t)rows * 4);
+  return 0;
+}
+
+// the logprob kernels alone on host rows: logits[rows, vocab], targets[rows], one top_n -> out[rows]
+extern "C" int lnb_op_logprobs_f32(const float* logits, int rows, int vocab, const int32_t* targets, int top_n, lnb_logprob* out) {
+  OpScope scope_;
+  if (!logits || !targets || !out) return fail(LNB_EINVAL, "NULL argument");
+  if (rows < 1 || vocab < 1 || vocab > LP_MAX_VOCAB) return fail(LNB_EINVAL, "rows %d must be >= 1 and vocab %d in [1, %d]", rows, vocab, LP_MAX_VOCAB);
+  if (top_n < 0 || top_n > LNB_LOGPROBS_TOP_MAX) return fail(LNB_EINVAL, "top_n %d must be in [0, %d]", top_n, LNB_LOGPROBS_TOP_MAX);
+  for (int r = 0; r < rows; r++)
+    if (targets[r] < 0 || targets[r] >= vocab) return fail(LNB_EINVAL, "targets[%d] = %d out of range", r, targets[r]);
+  const int G = (vocab + LP_SLICE - 1) / LP_SLICE;
+  const size_t b = (size_t)rows * vocab * 4, b_cand = (size_t)rows * G * (LP_TOP * 8 + 4) + (size_t)rows * 4;
+  OPBUF(dx, b); OPBUF(dt, (size_t)rows * 4); OPBUF(dtop, 4); OPBUF(drows, (size_t)rows * sizeof(LpRow));
+  OPBUF(drec, (size_t)rows * sizeof(LpRecord)); OPBUF(dc, b_cand);
+  H2D(dx, logits, b);
+  H2D(dt, targets, (size_t)rows * 4);
+  H2D(dtop, &top_n, 4);
+  CU(cudaMemset(dc.p, 0, b_cand));
+  std::vector<LpRow> hr((size_t)rows);
+  for (int r = 0; r < rows; r++)
+    hr[r] = LpRow{dx.as<float>() + (size_t)r * vocab, dt.as<int32_t>() + r, drec.as<LpRecord>() + r, nullptr, 0, 0};
+  H2D(drows, hr.data(), (size_t)rows * sizeof(LpRow));
+  LogprobJob J{};
+  J.rows = drows.as<LpRow>(); J.top_n = dtop.as<int32_t>(); J.V = vocab;
+  J.cand = dc.as<unsigned long long>();
+  J.above = reinterpret_cast<unsigned int*>(J.cand + (size_t)rows * G * LP_TOP);
+  J.done = J.above + (size_t)rows * G;
+  int rc;
+  if ((rc = launch_logprob_job(Launcher{nullptr, LAUNCH_PLAIN, nullptr}, J, rows))) return rc;
+  if ((rc = op_finish())) return rc;
+  std::vector<LpRecord> rec((size_t)rows);
+  D2H(rec.data(), drec, (size_t)rows * sizeof(LpRecord));
+  memset(out, 0, (size_t)rows * sizeof(lnb_logprob));
+  for (int i = 0; i < rows; i++) lp_finish(rec[i], out + i);
   return 0;
 }
 

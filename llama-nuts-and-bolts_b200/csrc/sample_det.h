@@ -81,6 +81,34 @@ LNB_SD_FN uint32_t lnb_sample_ord(float l) {
 #endif
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
+/* ---- token log-probabilities (DESIGN.md §9d) ----
+ * key = ord(l) << 32 | (2^32 - 1 - i): rank order is key descending, and a key gives its logit and index back, so a record
+ * of keys is enough to finish it on the host. */
+LNB_SD_FN uint64_t lnb_logprob_key(float l, int32_t i) {
+  return ((uint64_t)lnb_sample_ord(l) << 32) | (0xffffffffu - (uint32_t)i);
+}
+LNB_SD_FN int32_t lnb_logprob_key_index(uint64_t k) { return (int32_t)(0xffffffffu - (uint32_t)(k & 0xffffffffu)); }
+LNB_SD_FN float lnb_logprob_key_logit(uint64_t k) {
+  const uint32_t o = (uint32_t)(k >> 32);
+  const uint32_t u = (o & 0x80000000u) ? (o & 0x7fffffffu) : ~o;
+#if defined(__CUDA_ARCH__)
+  return __uint_as_float(u);
+#else
+  union { uint32_t u; float f; } c;
+  c.u = u;
+  return c.f;
+#endif
+}
+/* The host finish of a logprob: (f64(l) - f64(m)) - log(f64(sum) * 2^-40), every step one rounded f64 operation and the log
+ * the host libm's.  sum is the row's whole-vocabulary mass at T = 1 (sum of lnb_sample_weight(l_i, m, 1)), m its rank-0
+ * logit.  The device never evaluates a log: the record it writes holds integers and keys only. */
+#if defined(__CUDACC__)
+__host__
+#endif
+static inline double lnb_logprob_finish(float l, float m, uint64_t sum) {
+  return ((double)l - (double)m) - log(ldexp((double)sum, -40));
+}
+
 /* top-p target mass: Q = clamp(ceil(f64(P) * f64(W_C)), 1, W_C) (f64(W_C) rounds to nearest) */
 LNB_SD_FN uint64_t lnb_sample_top_p_mass(float P, uint64_t WC) {
 #if defined(__CUDA_ARCH__)

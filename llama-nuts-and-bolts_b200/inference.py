@@ -58,6 +58,23 @@ def _sampling_for(sampling, i: int):
     return SamplingArgs(sampling.Temperature, sampling.TopK, sampling.TopP, (sampling.Seed + i) & (2**64 - 1))
 
 
+def _logprob_lists(infContext, seqs, logprobs: int | None, logprobs_out: list | None, n_lists: int | None = None):
+    """Turns logprobs on for the context's sequences `seqs` (logprobs: top_n, None: off) and returns the lists the records
+    of emitted tokens go to: logprobs_out itself wrapped per sequence (n_lists None: logprobs_out is [the one list]), or
+    n_lists new lists appended to logprobs_out.  None when there is nothing to collect."""
+    if logprobs is None:
+        return None
+    for q in seqs:
+        infContext.set_logprobs(q, logprobs)
+    if n_lists is None:
+        return None if logprobs_out[0] is None else logprobs_out
+    if logprobs_out is None:
+        return None
+    lists = [[] for _ in range(n_lists)]
+    logprobs_out.extend(lists)
+    return lists
+
+
 def _check_speculative(speculative, use_reference_api: bool = False):
     if speculative is None:
         return
@@ -150,7 +167,8 @@ class InferenceEngine:
 
     def GenerateTokens(self, promptTokens, use_reference_api: bool = False, step_times: list | None = None,
                        prefill_chunk: int = 0, sampling: "SamplingArgs | None" = None,
-                       speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None):
+                       speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None,
+                       logprobs: int | None = None, logprobs_out: list | None = None):
         """Generator over (state, token id) exactly like generatedTokensCh.
 
         use_reference_api=True goes through the reference-shaped calls of every iteration
@@ -168,7 +186,10 @@ class InferenceEngine:
         drafts in one pass over the weights (lnb_forward_speculative) and emits the accepted tokens one at a time through
         the same stop logic, so the stream (tokens, length, final state) is the plain loop's, greedy or sampled.  step_times
         then gets one entry per call, and spec_stats (optional) one (rows, accepted drafts) pair per call.  It also needs
-        the fused entry: use_reference_api=True with speculative is an error."""
+        the fused entry: use_reference_api=True with speculative is an error.
+
+        logprobs (EXTENSION): 0..20 turns on token log-probabilities (lnb_session_set_logprobs); logprobs_out then gets one
+        model.TokenLogprob per emitted token, in order, with the top `logprobs` alternatives.  The stream is unchanged."""
         sampling = _sampling_for(sampling, 0)
         if sampling is not None and use_reference_api:
             raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax (inference.go:207-216); it cannot sample")
@@ -177,6 +198,7 @@ class InferenceEngine:
         try:
             if sampling is not None:
                 infContext.set_sampling(0, sampling)
+            lp_out = _logprob_lists(infContext, [0], logprobs, [logprobs_out])
             promptLength = len(promptTokens)
             if prefill_chunk > 0:
                 infContext.allow_chunked_prefill(True)
@@ -210,6 +232,8 @@ class InferenceEngine:
                 tokens.RawData[curPos] = nextTokenId
                 if step_times is not None:
                     step_times.append(time.perf_counter() - t0)
+                if lp_out is not None:   # after the step's time: step_times measures the same with logprobs on or off
+                    lp_out[0].append(infContext.read_logprobs(0, curPos, 1)[0])
                 eos = nextTokenId in self.model.Vocabulary.StopTokenIds
                 prevPos = curPos
                 if eos:
@@ -221,20 +245,22 @@ class InferenceEngine:
                 yield GSInProgress, nextTokenId
                 if speculative is not None:   # the prompt is in the cache: from here on, verify drafts
                     hist = [[int(t) for t in tokens.RawData[:curPos + 1]]]
-                    for _, state, tok in self._generate_speculative(infContext, hist, [0], speculative, step_times, spec_stats):
+                    for _, state, tok in self._generate_speculative(infContext, hist, [0], speculative, step_times, spec_stats,
+                                                                    lp_out):
                         yield state, tok
                     break
         finally:
             infContext.close()
 
     def _generate_speculative(self, infContext, hists, live, speculative: "SpeculativeArgs", step_times: list | None = None,
-                              spec_stats: list | None = None):
+                              spec_stats: list | None = None, lp_out: list | None = None):
         """The speculative loop on a given context (anything with SequenceLength, max_rows and forward_speculative).
         hists[i]: the tokens of sequence i so far, its last one emitted and not yet fed (it is fed at position
         len(hists[i]) - 1); live: the sequences still generating, each gets a row in every call.  The rows left of the
         budget min(8, max_rows) go to drafts in sequence order, clamped so that no row passes position SequenceLength - 2
         (the last position the plain loop feeds).  Yields (sequence, state, token) per emitted token, a segment's accepted
-        tokens in order; hists grow with them."""
+        tokens in order; hists grow with them.  lp_out (or None): per sequence, the list that gets the logprob record of each
+        emitted token (the records of the accepted positions)."""
         seqLen = infContext.SequenceLength
         stop = self.model.Vocabulary.StopTokenIds
         budget = min(SPEC_MAX_ROWS, infContext.max_rows)
@@ -260,9 +286,12 @@ class InferenceEngine:
             still, r0 = [], 0
             for (i, pos, toks), a in zip(segs, acc):
                 finished = False
+                recs = infContext.read_logprobs(i, pos + 1, int(a) + 1) if lp_out is not None else None
                 for j in range(int(a) + 1):            # the next tokens of rows 0 .. a, one at a time (:218-248)
                     tok, curPos = int(nxt[r0 + j]), pos + 1 + j
                     hists[i].append(tok)
+                    if recs is not None:
+                        lp_out[i].append(recs[j])
                     if tok in stop:
                         state = GSFinishedByReachingEOS
                     elif curPos + 1 == seqLen:
@@ -279,7 +308,8 @@ class InferenceEngine:
             live = still
 
     def GenerateTokensContinuous(self, prompts, slots: int = 8, step_tokens: int | None = None,
-                                 step_times: list | None = None, sampling: "SamplingArgs | None" = None):
+                                 step_times: list | None = None, sampling: "SamplingArgs | None" = None,
+                                 logprobs: int | None = None, logprobs_out: list | None = None):
         """Continuous batching (EXTENSION, lnb_forward_ragged): any number of prompts through at most `slots` live
         sequences.  Every step is ONE forward whose rows may belong to different sequences: each decoding sequence gets
         its one row, the rest of the step's row budget (min(step_tokens, max_rows)) goes to prompt chunks, first in first
@@ -287,7 +317,8 @@ class InferenceEngine:
         is refilled at position 0 by the next waiting prompt.  Steps without prompt rows run lnb_forward_batch (the
         batch engine: one launch per step).  Yields (prompt index, state, token id); per prompt the stream is exactly
         what GenerateTokens(prompts[i]) yields (the bookkeeping of generateTokensInternal, inference.go:173-254).
-        sampling: prompt i samples with Seed + i (the stream of GenerateTokens(prompts[i]) with that seed)."""
+        sampling: prompt i samples with Seed + i (the stream of GenerateTokens(prompts[i]) with that seed).
+        logprobs / logprobs_out as in GenerateTokens: logprobs_out gets one list per prompt."""
         if step_tokens is None:
             step_tokens = DEFAULT_STEP_TOKENS
         if not 1 <= slots <= 8:
@@ -301,14 +332,14 @@ class InferenceEngine:
             self.context_hook(infContext)
         try:
             yield from self._generate_continuous(infContext, prompts, slots, min(step_tokens, infContext.max_rows), step_times,
-                                                 sampling)
+                                                 sampling, logprobs, logprobs_out)
         finally:
             infContext.close()
 
     def _generate_continuous(self, infContext, prompts, slots: int, budget: int, step_times: list | None = None,
-                             sampling: "SamplingArgs | None" = None):
+                             sampling: "SamplingArgs | None" = None, logprobs: int | None = None, logprobs_out: list | None = None):
         """the scheduler of GenerateTokensContinuous on a given context (anything with SequenceLength, forward_ragged and
-        forward_batch, and set_sampling when `sampling` samples)"""
+        forward_batch, set_sampling when `sampling` samples, set_logprobs and read_logprobs when `logprobs` is set)"""
         seqLen = infContext.SequenceLength
         stop = self.model.Vocabulary.StopTokenIds
         for p in prompts:
@@ -316,6 +347,7 @@ class InferenceEngine:
                 raise ml.MlError(f"context SequenceLength {seqLen} must be higher than prompt tokens length {len(p)}")
             if len(p) < 1:
                 raise ml.MlError("empty prompt")
+        lp_out = _logprob_lists(infContext, range(slots), logprobs, logprobs_out, len(prompts))
         waiting = collections.deque(range(len(prompts)))
         # per slot: prompt index, prompt tokens already in the cache, token fed next and its position (cur None: prefilling),
         # admission number (first in, first out among the prefilling slots)
@@ -374,10 +406,13 @@ class InferenceEngine:
                     state = GSInProgress
                 if state != GSInProgress:
                     slot[k] = None
+                if lp_out is not None:
+                    lp_out[sl["i"]].append(infContext.read_logprobs(k, curPos, 1)[0])
                 yield sl["i"], state, tok
 
     def GenerateTokensBatch(self, prompts, step_times: list | None = None, sampling: "SamplingArgs | None" = None,
-                            speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None):
+                            speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None,
+                            logprobs: int | None = None, logprobs_out: list | None = None):
         """The consumer `InferenceEngine.TokenizeBatch` (src/inference/tokenize.go:97-107) never got in the
         reference (SURVEY 8f-4): every prompt runs the loop of generateTokensInternal (:173-254) -- own
         InferenceContext / KV cache, own positions, own stop condition -- but all sequences advance together,
@@ -386,13 +421,19 @@ class InferenceEngine:
         Seed + i (the stream of GenerateTokens(prompts[i]) with that seed).
         speculative (EXTENSION): after the prompts, every call is one lnb_forward_speculative in which each unfinished
         sequence gets its row and the rest of the 8-row budget goes to prompt-lookup drafts in sequence order; the streams
-        are the same.  spec_stats as in GenerateTokens."""
+        are the same.  spec_stats as in GenerateTokens; logprobs / logprobs_out as in GenerateTokens, logprobs_out gets one
+        list per prompt."""
         _check_speculative(speculative)
         n = len(prompts)
         if n < 1:
             raise ml.MlError("empty prompt batch")
         if n == 1:
-            for state, tok in self.GenerateTokens(prompts[0], sampling=sampling, speculative=speculative, spec_stats=spec_stats):
+            lp0 = None
+            if logprobs is not None and logprobs_out is not None:
+                lp0 = []
+                logprobs_out.append(lp0)
+            for state, tok in self.GenerateTokens(prompts[0], sampling=sampling, speculative=speculative, spec_stats=spec_stats,
+                                                  logprobs=logprobs, logprobs_out=lp0):
                 yield 0, state, tok
             return
         infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
@@ -411,6 +452,7 @@ class InferenceEngine:
                 sp = _sampling_for(sampling, i)
                 if sp is not None:
                     infContext.set_sampling(i, sp)
+            lp_out = _logprob_lists(infContext, range(n), logprobs, logprobs_out, n)
             cur = [0] * n                                  # token fed next / position it is fed at
             pos = [0] * n
             done = [False] * n
@@ -418,6 +460,8 @@ class InferenceEngine:
             def emit(i, tok, curPos):
                 """bookkeeping of one generated token at curPos (:218-248); returns the state to yield"""
                 cur[i], pos[i] = tok, curPos
+                if lp_out is not None:
+                    lp_out[i].append(infContext.read_logprobs(i, curPos, 1)[0])
                 if tok in stop:
                     done[i] = True
                     return GSFinishedByReachingEOS
@@ -436,7 +480,7 @@ class InferenceEngine:
             if speculative is not None:
                 hists = [[int(t) for t in p] + [cur[i]] for i, p in enumerate(prompts)]
                 live = [i for i in range(n) if not done[i]]
-                yield from self._generate_speculative(infContext, hists, live, speculative, step_times, spec_stats)
+                yield from self._generate_speculative(infContext, hists, live, speculative, step_times, spec_stats, lp_out)
                 return
             while not all(done):
                 t0 = time.perf_counter()

@@ -131,6 +131,15 @@ class LlamaTransformer:
                               1 if want_logits == "all" else 0, C.byref(nxt)))
         return nxt.value, logits
 
+    def score(self, infContext: "InferenceContext", tokens, startPos: int = 0) -> list:
+        """EXTENSION (lnb_score): the log-probability of tokens[1:] given what precedes them, one forward over tokens[:-1] at
+        startPos.  Returns a TokenLogprob per token of tokens[1:] (positions startPos + 1 ..).  Chunks overlap by one token:
+        the next call starts at startPos + len(tokens) - 1 with tokens[-1].  The active sequence must have logprobs on."""
+        tokens = np.ascontiguousarray(tokens, np.int32)
+        n = tokens.shape[0]
+        check(lib.lnb_score(infContext.h, ptr(tokens, _capi.i32p), n, startPos))
+        return infContext.read_logprobs(infContext.active_seq, startPos + 1, n - 1)
+
     def close(self):
         if self.h:
             lib.lnb_model_destroy(self.h)
@@ -156,6 +165,21 @@ class SamplingArgs:
         return _capi.SamplingC(float(self.Temperature), int(self.TopK), float(self.TopP), int(self.Seed) & (2**64 - 1))
 
 
+@dataclass
+class TokenLogprob:
+    """EXTENSION: one record of lnb_session_logprobs_read.  Logprob is the raw model distribution's (temperature 1, no
+    top-k / top-p); Rank 1 is the greedy token; Top holds (token, logprob) of the top_n first tokens in rank order."""
+    Token: int
+    Logprob: float
+    Rank: int
+    Top: list
+
+
+def _token_logprobs(recs) -> list:
+    return [TokenLogprob(int(r.token), float(r.logprob), int(r.rank),
+                         [(int(r.top_token[j]), float(r.top_logprob[j])) for j in range(r.n_top)]) for r in recs]
+
+
 class InferenceContext:
     """model.InferenceContext (inferencecontext.go:8-46): the KV cache (here: in HBM)."""
 
@@ -174,6 +198,7 @@ class InferenceContext:
         else:
             check(lib.lnb_session_create(transformer.h, self.SequenceLength, max_rows, acc_mode, C.byref(h)))
         self.h = h
+        self.active_seq = 0
         self.generation = 0        # forward calls made through lnb_forward_device (validity of ml.DeviceLogits handles)
         self.pre_close_hook = None  # tensor-parallel sessions: barrier before the peer-mapped region is freed
 
@@ -202,6 +227,7 @@ class InferenceContext:
 
     def set_active_sequence(self, seq: int):
         check(lib.lnb_session_set_active_sequence(self.h, seq))
+        self.active_seq = seq
 
     def forward_batch(self, tokens, positions, want_logits: bool = False):
         """one decode step for len(tokens) independent sequences: (greedy tokens [n], logits [n, vocab] or None)"""
@@ -260,6 +286,17 @@ class InferenceContext:
         else:
             c = args.c()
             check(lib.lnb_session_set_sampling(self.h, seq, C.byref(c)))
+
+    def set_logprobs(self, seq: int, top_n: int | None):
+        """EXTENSION: from its next forward on, every token sequence `seq` emits writes its logprob record (the raw model
+        distribution, its rank and the top_n first tokens, 0..20) at the position it occupies; None turns them off"""
+        check(lib.lnb_session_set_logprobs(self.h, seq, -1 if top_n is None else int(top_n)))
+
+    def read_logprobs(self, seq: int, pos0: int, n: int) -> list:
+        """the records of positions pos0 .. pos0 + n - 1 of sequence `seq` (TokenLogprob; Token -1: never written)"""
+        recs = (_capi.LogprobC * n)()
+        check(lib.lnb_session_logprobs_read(self.h, seq, pos0, n, recs))
+        return _token_logprobs(recs)
 
     def allow_chunked_prefill(self, on: bool = True):
         """EXTENSION (not in the reference): accept S > 1 at startPos > 0 with the [S,T] causal mask"""

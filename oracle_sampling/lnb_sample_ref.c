@@ -9,6 +9,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include "../include/lnb.h"
 #include "../llama-nuts-and-bolts_b200/csrc/sample_det.h"
 #include "../oracle/lnb_oracle.h"
 
@@ -92,6 +93,33 @@ int32_t orc_sample_row(const float* l, int V, float T, int32_t K, float P, uint6
   free(W);
   free(order);
   return tok;
+}
+
+/* one row: the log-probability record of token `target` (DESIGN.md §9d) -- a full sort for the ranks, a sequential sum of
+ * the weights at temperature 1, then the shared host finish */
+void orc_logprob_row(const float* l, int V, int32_t target, int top_n, lnb_logprob* out) {
+  memset(out, 0, sizeof(*out));
+  int32_t* order = (int32_t*)malloc((size_t)V * 4);
+  for (int i = 0; i < V; i++) order[i] = i;
+  g_rank_l = l;
+  qsort(order, (size_t)V, 4, rank_cmp);
+  const float m = l[order[0]];
+  uint64_t sum = 0;
+  for (int i = 0; i < V; i++) sum += lnb_sample_weight(l[i], m, 1.0f);
+  int rank = 1;
+  while (order[rank - 1] != target) rank++;
+  out->token = target;
+  out->rank = rank;
+  out->logprob = lnb_logprob_finish(l[target], m, sum);
+  out->n_top = top_n < V ? top_n : V;
+  for (int r = 0; r < out->n_top; r++) {
+    out->top_token[r] = order[r];
+    out->top_logprob[r] = lnb_logprob_finish(l[order[r]], m, sum);
+  }
+  free(order);
+}
+void orc_logprob_rows(const float* l, int rows, int V, const int32_t* targets, int top_n, lnb_logprob* out) {
+  for (int r = 0; r < rows; r++) orc_logprob_row(l + (size_t)r * V, V, targets[r], top_n, out + r);
 }
 
 /* rows x V logits -> rows tokens, parameters per row */

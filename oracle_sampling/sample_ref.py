@@ -27,7 +27,7 @@ _lib = None
 def build(force: bool = False) -> str:
     _oracle.build()
     src = [os.path.join(_HERE, f) for f in ("lnb_sample_ref.c", "Makefile")] + \
-          [os.path.join(_ROOT, "llama-nuts-and-bolts_b200", "csrc", "sample_det.h")]
+          [os.path.join(_ROOT, "llama-nuts-and-bolts_b200", "csrc", "sample_det.h"), os.path.join(_ROOT, "include", "lnb.h")]
     stale = (not os.path.exists(_SO)) or any(os.path.getmtime(s) > os.path.getmtime(_SO) for s in src)
     if force or stale:
         subprocess.check_call(["make", "-C", _HERE, "-s"])
@@ -48,6 +48,8 @@ def lib():
         L.orc_sample_row.argtypes = [_f32p, C.c_int, C.c_float, C.c_int32, C.c_float, C.c_uint64, C.c_int64]
         L.orc_sample_rows.restype = None
         L.orc_sample_rows.argtypes = [_f32p, C.c_int, C.c_int, _f32p, _i32p, _f32p, _u64p, _i64p, _i32p]
+        L.orc_logprob_rows.restype = None
+        L.orc_logprob_rows.argtypes = [_f32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_void_p]
         L.orc_generate_sampled.restype = C.c_int
         L.orc_generate_sampled.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
                                            C.c_float, C.c_uint64, _i32p]
@@ -76,6 +78,23 @@ def sample_weight(l: float, m: float, T: float) -> int:
 def sample_row(logits, T: float, K: int, P: float, seed: int, p_next: int) -> int:
     row = np.ascontiguousarray(logits, np.float32).reshape(-1)
     return int(lib().orc_sample_row(row.ctypes.data_as(_f32p), row.size, T, K, P, seed & (2**64 - 1), p_next))
+
+
+# lnb_logprob (include/lnb.h) as a numpy record
+LOGPROB_DTYPE = np.dtype([("token", "<i4"), ("rank", "<i4"), ("logprob", "<f8"), ("n_top", "<i4"), ("top_token", "<i4", (20,)),
+                          ("top_logprob", "<f8", (20,))], align=True)
+assert LOGPROB_DTYPE.itemsize == 264
+
+
+def logprob_rows(logits, targets, top_n: int) -> np.ndarray:
+    """orc_logprob_row of every row of logits [rows, V] with its target: LOGPROB_DTYPE [rows]"""
+    l = np.ascontiguousarray(logits, np.float32)
+    l = l.reshape(-1, l.shape[-1])
+    t = np.ascontiguousarray(targets, np.int32).reshape(-1)
+    assert t.shape[0] == l.shape[0]
+    out = np.zeros(l.shape[0], LOGPROB_DTYPE)
+    lib().orc_logprob_rows(l.ctypes.data_as(_f32p), l.shape[0], l.shape[1], t.ctypes.data_as(_i32p), top_n, out.ctypes.data)
+    return out
 
 
 def generate_sampled(om, prompt, seq_len: int, T: float, K: int, P: float, seed: int, stop_ids=(128008, 128009)) -> np.ndarray:
