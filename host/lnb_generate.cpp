@@ -8,6 +8,8 @@
 // batch samples with seed S + b.
 // spec=K: speculative decoding -- each call verifies the last token plus up to K prompt-lookup drafts in one pass over the
 // weights (lnb_forward_speculative); the generated ids are the same as without it.  Not with slots=.
+// rep=R freq=F pres=P [last_n=N]: repetition, frequency and presence penalties over the generated tokens (the last N positions;
+// 0, the default: all) before the sampler or the greedy pick (lnb_session_set_penalties).
 // logprobs=N (0..20): after the generated ids, one line per generated token with its logprob, its rank and the top N
 // alternatives (lnb_session_set_logprobs; the raw model distribution, also for sampled tokens).
 // score=TEXT (with <modelDir>/tokenizer.model): TEXT is tokenized without the chat template and scored in chunks of 64 tokens
@@ -146,7 +148,12 @@ int main(int argc, char** argv) {
     int logprobs = -1;              // logprobs=N: top N alternatives per generated token
     model::SamplingArgs sampling;   // temp= top_k= top_p= seed= (temp 0, the default: greedy)
     model::SpeculativeArgs spec;    // spec=K: speculative decoding with up to K prompt-lookup drafts per call (0: plain steps)
+    model::PenaltyArgs pen;         // rep= freq= pres= last_n= (the defaults: off)
     for (int i = 1; i < argc; i++) {
+      if (!strncmp(argv[i], "rep=", 4)) pen.RepetitionPenalty = (float)atof(argv[i] + 4);
+      if (!strncmp(argv[i], "freq=", 5)) pen.FrequencyPenalty = (float)atof(argv[i] + 5);
+      if (!strncmp(argv[i], "pres=", 5)) pen.PresencePenalty = (float)atof(argv[i] + 5);
+      if (!strncmp(argv[i], "last_n=", 7)) pen.Window = atoi(argv[i] + 7);
       if (!strncmp(argv[i], "spec=", 5)) spec.MaxDraft = atoi(argv[i] + 5);
       if (!strncmp(argv[i], "batch=", 6)) batch = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "slots=", 6)) slots = atoi(argv[i] + 6);
@@ -174,6 +181,7 @@ int main(int argc, char** argv) {
       prompt = tokenizer->Tokenize({{"user", prompt_text}});
     }
     const model::SpeculativeArgs* speculative = spec.MaxDraft > 0 ? &spec : nullptr;
+    const model::PenaltyArgs* penalties = pen.Neutral() ? nullptr : &pen;
     if (speculative && slots > 0) throw Error("spec= is not built for continuous batching (slots=)");
     if (batch > 0) {
       const int mod = transformer.args.vocab_size < 128256 ? 1000 : 128000;
@@ -186,8 +194,8 @@ int main(int argc, char** argv) {
       auto collect = [&](int seq, inference::GenerationState, int32_t tok) { outs[seq].push_back(tok); };
       if (slots > 0)
         inference::GenerateTokensContinuous(transformer, vocab, seq_len, acc, prompts, slots, std::max(slots, 64), collect, &sampling, logprobs,
-                                            &lps);
-      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling, speculative, logprobs, &lps);
+                                            &lps, penalties);
+      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling, speculative, logprobs, &lps, penalties);
       const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - b0).count();
       size_t total = 0;
       for (int b = 0; b < batch; b++) {
@@ -209,7 +217,7 @@ int main(int argc, char** argv) {
     inference::GenerateTokens(transformer, vocab, seq_len, acc, prompt, [&](inference::GenerationState, int32_t tok) {
       if (out.empty()) t_first = std::chrono::steady_clock::now();
       out.push_back(tok);
-    }, &sampling, speculative, logprobs, &lp);
+    }, &sampling, speculative, logprobs, &lp, penalties);
     auto t1 = std::chrono::steady_clock::now();
     if (tokenizer) printf("text: %s\n", tokenizer->TokenBatchToString(out).c_str());
     printf("tokens:");

@@ -289,6 +289,31 @@ struct SamplingArgs {
   SamplingArgs ForPrompt(int i) const { SamplingArgs a = *this; a.Seed += (uint64_t)i; return a; }
 };
 
+// EXTENSION: repetition, frequency and presence penalties and a logit bias over the sequence's token history
+// (lnb_session_set_penalties, DESIGN.md §9e).  The defaults are neutral (off).  CountPrompt false counts generated tokens only:
+// first_pos is the prompt's length.  A -inf bias bans its token.
+struct PenaltyArgs {
+  float RepetitionPenalty = 1.0f;
+  float FrequencyPenalty = 0.0f;
+  float PresencePenalty = 0.0f;
+  int32_t Window = 0;          // the last Window positions; 0: all
+  bool CountPrompt = false;
+  std::vector<std::pair<int32_t, float>> LogitBias;
+  bool Neutral() const { return RepetitionPenalty == 1.0f && FrequencyPenalty == 0.0f && PresencePenalty == 0.0f && LogitBias.empty(); }
+  lnb_penalties C(int promptLength) const {
+    if (LogitBias.size() > LNB_LOGIT_BIAS_MAX) throw Error("LogitBias has more than " + std::to_string(LNB_LOGIT_BIAS_MAX) + " entries");
+    lnb_penalties p{};
+    p.repetition_penalty = RepetitionPenalty;
+    p.frequency_penalty = FrequencyPenalty;
+    p.presence_penalty = PresencePenalty;
+    p.window = Window;
+    p.first_pos = CountPrompt ? 0 : promptLength;
+    p.n_bias = (int32_t)LogitBias.size();
+    for (size_t j = 0; j < LogitBias.size(); j++) { p.bias_token[j] = LogitBias[j].first; p.bias[j] = LogitBias[j].second; }
+    return p;
+  }
+};
+
 // EXTENSION: speculative decoding (lnb_forward_speculative) with prompt-lookup drafts of up to MaxDraft tokens
 struct SpeculativeArgs {
   int MaxDraft = 0;
@@ -332,6 +357,13 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
     if (!a || !a->Samples()) { check(lnb_session_set_sampling(h_, seq, nullptr)); return; }
     const lnb_sampling p{a->Temperature, a->TopK, a->TopP, a->Seed};
     check(lnb_session_set_sampling(h_, seq, &p));
+  }
+  // EXTENSION: sequence seq is penalized with *a (nullptr or neutral: off) for a prompt of promptLength tokens; turning
+  // penalties on clears its token history
+  void SetPenalties(int seq, const PenaltyArgs* a, int promptLength) {
+    if (!a) { check(lnb_session_set_penalties(h_, seq, nullptr)); return; }
+    const lnb_penalties p = a->C(promptLength);
+    check(lnb_session_set_penalties(h_, seq, &p));
   }
   // EXTENSION: token log-probabilities (lnb_session_set_logprobs).  topN 0..20 turns them on for sequence seq, -1 off; every
   // token the context then emits for seq writes the record of the position it occupies (the raw model distribution).
@@ -491,15 +523,19 @@ inline void GenerateSpeculative(model::InferenceContext& infContext, const model
 }
 
 // generateTokensInternal (inference.go:173-254); `emit` plays generatedTokensCh.  EXTENSION: logprobs 0..20 turns on token
-// log-probabilities; logprobsOut (or nullptr) then gets one record per emitted token, in order.
+// log-probabilities; logprobsOut (or nullptr) then gets one record per emitted token, in order.  penalties (or nullptr):
+// every emitted token is drawn from the penalized logits (the records stay the raw distribution's).
 inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                            const std::vector<int32_t>& promptTokens, const std::function<void(GenerationState, int32_t)>& emit,
                            const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr,
-                           int logprobs = -1, std::vector<lnb_logprob>* logprobsOut = nullptr) {
+                           int logprobs = -1, std::vector<lnb_logprob>* logprobsOut = nullptr,
+                           const model::PenaltyArgs* penalties = nullptr) {
   // the prefill call carries the whole prompt: size the session's row buffers for it
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max<int>(8, (int)promptTokens.size()));
-  const bool samples = sampling && sampling->Samples();
-  if (samples) infContext.SetSampling(0, sampling);   // the sampled token instead of Slice + ml.Argmax
+  if (penalties && penalties->Neutral()) penalties = nullptr;
+  const bool samples = (sampling && sampling->Samples()) || penalties;
+  if (sampling && sampling->Samples()) infContext.SetSampling(0, sampling);   // the sampled token instead of Slice + ml.Argmax
+  if (penalties) infContext.SetPenalties(0, penalties, (int)promptTokens.size());
   if (logprobs >= 0) infContext.SetLogprobs(0, logprobs);
   if (logprobs < 0) logprobsOut = nullptr;
   const int promptLength = (int)promptTokens.size();
@@ -545,15 +581,18 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
 // The consumer InferenceEngine.TokenizeBatch (src/inference/tokenize.go:97-107) never got in the reference
 // (SURVEY 8f-4): every prompt runs the loop above -- own KV cache, positions and stop condition -- but all
 // sequences advance together, one pass over the weights per step.  emit(sequence, state, token).  logprobs / logprobsOut as in
-// GenerateTokens, one list per prompt.
+// GenerateTokens, one list per prompt; penalties as in GenerateTokens, for every sequence.
 inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                                 const std::vector<std::vector<int32_t>>& prompts,
                                 const std::function<void(int, GenerationState, int32_t)>& emit,
                                 const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr,
-                                int logprobs = -1, std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr) {
+                                int logprobs = -1, std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr,
+                                const model::PenaltyArgs* penalties = nullptr) {
   const int n = (int)prompts.size();
   if (n < 1) throw Error("empty prompt batch");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, n), n);
+  if (penalties)
+    for (int i = 0; i < n; i++) infContext.SetPenalties(i, penalties, (int)prompts[i].size());
   if (logprobs >= 0)
     for (int i = 0; i < n; i++) infContext.SetLogprobs(i, logprobs);
   if (logprobs < 0) logprobsOut = nullptr;
@@ -608,12 +647,13 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
 // row, the rest of the stepTokens-row budget goes to prompt chunks first in first out, a prompt whose last chunk is in the
 // step emits its first token, a finished slot takes the next waiting prompt at position 0; steps without prompt rows run
 // lnb_forward_batch.  emit(prompt index, state, token); per prompt the stream is GenerateTokens' own.  logprobs / logprobsOut
-// as in GenerateTokens, one list per prompt.
+// as in GenerateTokens, one list per prompt; penalties as in GenerateTokens, set at each admission (first_pos follows the prompt).
 inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength,
                                      int accMode, const std::vector<std::vector<int32_t>>& prompts, int slots, int stepTokens,
                                      const std::function<void(int, GenerationState, int32_t)>& emit,
                                      const model::SamplingArgs* sampling = nullptr, int logprobs = -1,
-                                     std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr) {
+                                     std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr,
+                                     const model::PenaltyArgs* penalties = nullptr) {
   if (slots < 1 || slots > 8) throw Error("slots must be in [1, 8]");
   if (stepTokens < slots) throw Error("stepTokens must be at least slots (every decoding sequence gets a row)");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, stepTokens), slots);
@@ -638,6 +678,7 @@ inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const
           const model::SamplingArgs a = sampling->ForPrompt(s.i);
           infContext.SetSampling((int)(&s - slot.data()), &a);
         }
+        if (penalties) infContext.SetPenalties((int)(&s - slot.data()), penalties, (int)prompts[(size_t)s.i].size());
       }
     std::vector<int> decoding, prefilling;
     for (int k = 0; k < slots; k++)

@@ -317,6 +317,36 @@ typedef struct {
  * stream or invalidate a captured decode graph; switching the active sequence between greedy and sampled re-captures it. */
 int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampling* p);
 
+/* EXTENSION: repetition, frequency and presence penalties and a per-token logit bias, computed on the device
+ * (csrc/penalty.cuh) over each sequence's token history, before the sampler (DESIGN.md §9e).  For the row that emits the
+ * token at position p_next: c_t = how often token t was fed at positions [max(first_pos, p_next - window (0: no limit)),
+ * p_next) of the sequence; where c_t >= 1, a = rp != 1 ? (l > 0 ? f32(l / rp) : f32(l * rp)) : l and
+ * b = f32(a - f32(f32(f32(c_t) * fp) + pp)); then l' = f32(b + bias_t) for a biased token (-inf bias: l' = -inf, the token
+ * is never emitted).  Every step is one rounded IEEE operation; a NaN a step produces is 0x7FFFFFFF (the device's NaN).
+ * The sampler of lnb_session_set_sampling (greedy: rank 0) then runs unchanged on l', so a stream depends only on the
+ * model, the prompt and the parameters, however it was batched, chunked or drafted.  Logprobs and the logits read-backs
+ * keep reporting the raw distribution. */
+#define LNB_LOGIT_BIAS_MAX 64
+typedef struct {
+  float repetition_penalty;   /* finite, > 0; 1: off */
+  float frequency_penalty;    /* finite (may be negative); 0: off */
+  float presence_penalty;     /* finite (may be negative); 0: off */
+  int32_t window;             /* >= 0: count the last `window` positions; 0: every position */
+  int32_t first_pos;          /* >= 0: positions below it are never counted (e.g. the prompt) */
+  int32_t n_bias;             /* 0 .. LNB_LOGIT_BIAS_MAX */
+  int32_t bias_token[LNB_LOGIT_BIAS_MAX];   /* distinct, in [0, vocab) */
+  float bias[LNB_LOGIT_BIAS_MAX];           /* finite, or -inf (the token is never emitted) */
+} lnb_penalties;
+/* Sequence `seq` is penalized with *p from its next forward on; NULL or neutral parameters (rp 1, fp and pp 0, no bias)
+ * turn penalties off (the default: the session launches exactly what it does without them).  Turning them on clears the
+ * sequence's token history (stream-ordered); from then on every forward records the token of each of its rows at its
+ * position, and every token the sequence emits is drawn from l'.  The first enable allocates the history of every sequence
+ * and position (4 bytes each), the job's scratch and the sampler's slots (LNB_ENOMEM with the bytes; the session stays as
+ * it was).  LNB_EINVAL with nothing changed: seq outside [0, n_seq), a parameter outside the ranges above, a bias token
+ * repeated or outside [0, vocab), a +inf or NaN bias, tp_size > 1 (not built).  Turning penalties on or off for the active
+ * sequence re-captures a decode graph; changing their values does not. */
+int lnb_session_set_penalties(lnb_session* s, int seq, const lnb_penalties* p);
+
 /* EXTENSION: token log-probabilities, computed on the device (csrc/logprob.cuh) and finished on the host (DESIGN.md §9d).
  * For one row of logits l and a token t: the rank order is the sampler's (l descending, index ascending), m the rank-0
  * logit, sum = the sum over the vocabulary of floor(2^40 exp(f32(l_i - m))) (0 below -28: the sampler's weights at
@@ -433,6 +463,11 @@ int lnb_op_sample_f32(const float* logits, int rows, int vocab, const lnb_sampli
 /* EXTENSION: the logprob kernels of lnb_session_set_logprobs alone on host rows: logits[rows, vocab], targets[rows],
  * top_n in [0, 20] -> out[rows] */
 int lnb_op_logprobs_f32(const float* logits, int rows, int vocab, const int32_t* targets, int top_n, lnb_logprob* out);
+/* EXTENSION: the penalty kernels of lnb_session_set_penalties alone on host rows (1..8 rows): logits[rows, vocab],
+ * parameters p[rows] (any valid parameters; a neutral row is copied), row r's token history hist[r][hist_len] (-1: not
+ * counted), the position pos_next[r] in [0, hist_len] its token would occupy -> l' to out[rows, vocab] */
+int lnb_op_penalize_f32(const float* logits, int rows, int vocab, const lnb_penalties* p, const int32_t* hist, int hist_len,
+                        const int32_t* pos_next, float* out);
 /* ml.Fwd_Get_Rows (operations_impl.go:142-173) */
 int lnb_op_get_rows_bf16(const uint16_t* emb, const int32_t* tokens, uint16_t* out, int S, int vocab, int dim);
 

@@ -32,6 +32,15 @@ class SamplingC(C.Structure):   # lnb_sampling
 LNB_LOGPROBS_TOP_MAX = 20
 
 
+LNB_LOGIT_BIAS_MAX = 64
+
+
+class PenaltiesC(C.Structure):   # lnb_penalties
+    _fields_ = [("repetition_penalty", C.c_float), ("frequency_penalty", C.c_float), ("presence_penalty", C.c_float),
+                ("window", C.c_int32), ("first_pos", C.c_int32), ("n_bias", C.c_int32),
+                ("bias_token", C.c_int32 * LNB_LOGIT_BIAS_MAX), ("bias", C.c_float * LNB_LOGIT_BIAS_MAX)]
+
+
 class LogprobC(C.Structure):   # lnb_logprob
     _fields_ = [("token", C.c_int32), ("rank", C.c_int32), ("logprob", C.c_double), ("n_top", C.c_int32),
                 ("top_token", C.c_int32 * LNB_LOGPROBS_TOP_MAX), ("top_logprob", C.c_double * LNB_LOGPROBS_TOP_MAX)]
@@ -82,6 +91,7 @@ SIGNATURES = {
     "lnb_forward_speculative": (C.c_int, [vp, C.c_int, i32p, i32p, i32p, i32p, f32p, i32p, i32p]),
     "lnb_session_set_sampling": (C.c_int, [vp, C.c_int, C.POINTER(SamplingC)]),
     "lnb_session_set_logprobs": (C.c_int, [vp, C.c_int, C.c_int]),
+    "lnb_session_set_penalties": (C.c_int, [vp, C.c_int, C.POINTER(PenaltiesC)]),
     "lnb_session_logprobs_read": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp]),
     "lnb_score": (C.c_int, [vp, i32p, C.c_int, C.c_int]),
     "lnb_session_read": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64]),
@@ -125,6 +135,7 @@ SIGNATURES = {
     "lnb_op_argmax_f32": (C.c_int, [f32p, C.c_int, C.c_int, i32p]),
     "lnb_op_sample_f32": (C.c_int, [f32p, C.c_int, C.c_int, C.POINTER(SamplingC), i32p, i32p]),
     "lnb_op_logprobs_f32": (C.c_int, [f32p, C.c_int, C.c_int, i32p, C.c_int, vp]),
+    "lnb_op_penalize_f32": (C.c_int, [f32p, C.c_int, C.c_int, C.POINTER(PenaltiesC), i32p, C.c_int, i32p, f32p]),
     "lnb_op_get_rows_bf16": (C.c_int, [u16p, i32p, u16p, C.c_int, C.c_int, C.c_int]),
 }
 

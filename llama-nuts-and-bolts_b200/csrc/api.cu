@@ -26,6 +26,7 @@
 #include "engine_batch.cuh"
 #include "sample.cuh"
 #include "logprob.cuh"
+#include "penalty.cuh"
 #include "pth.hpp"
 #include "tokenizer.hpp"
 
@@ -1165,7 +1166,19 @@ struct lnb_session {
   int lp_rows = 0;
   int lp_top[8] = {-1, -1, -1, -1, -1, -1, -1, -1};   // -1: logprobs off
   bool graph_lp = false;                    // the captured decode graph ends in the logprob job
+  // penalties (penalty.cuh, lnb_session_set_penalties), allocated by the first enable: the token history of every sequence
+  // and position, the parameters of each sequence in device memory (a captured graph reads them there), and one job's
+  // counts and processed rows
+  int32_t* d_hist = nullptr;                // [n_seq][seq_len] the token fed at each position, -1: none
+  lnb_penalties* d_pen = nullptr;           // [n_seq]
+  unsigned int* d_pen_cnt = nullptr;        // [PEN_MAX_ROWS][vocab] (zero between jobs)
+  float* d_pen_out = nullptr;               // [PEN_MAX_ROWS][vocab] l', read by the sampler
+  bool pen_on[8] = {false, false, false, false, false, false, false, false};
+  bool graph_pen = false, graph_greedy = false;   // the captured decode graph runs the penalty job / the greedy slot
 };
+
+// a sequence whose tokens the sampler draws (sampled, or penalized: greedy is then the sampler's rank 0 of l')
+static bool processed(const lnb_session* s, int seq) { return s->samp_on[seq] || s->pen_on[seq]; }
 
 static int set_state(lnb_session* s, int pos, int n_rows, int next_token, bool reset_step) {
   return launch_kernel(Launcher{s->stream, LAUNCH_PLAIN, &s->launches}, set_state_kernel, dim3(1), dim3(1), 0, s->st, pos, n_rows,
@@ -1308,6 +1321,7 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->d_samp); cudaFree(s->d_samp_w); cudaFree(s->d_samp_tok); cudaFree(s->d_samp_cand);
   cudaFree(s->d_lp_rec); cudaFree(s->d_lp_top); cudaFree(s->d_lp_tgt); cudaFree(s->d_lp_rows); cudaFree(s->d_lp_cand);
   if (s->h_lp_rows) cudaFreeHost(s->h_lp_rows);
+  cudaFree(s->d_hist); cudaFree(s->d_pen); cudaFree(s->d_pen_cnt); cudaFree(s->d_pen_out);
   for (auto p : s->ck) cudaFree(p);
   for (auto p : s->cv) cudaFree(p);
   if (s->h_tok) cudaFreeHost(s->h_tok);
@@ -1987,6 +2001,7 @@ struct Rows {
   int head_rows;            // rows the LM head computes
   bool advance;             // the LM head advances st->pos and appends the token to d_tok_out (device-driven decode)
   bool gather;              // tensor-parallel: the kept logits are all-gathered for the host
+  bool record;              // a row's sequence is penalized: the forward records every row's token in d_hist
 };
 // rows 0..S-1 of the active sequence at st->pos + r.  tokens: device ids, or NULL for st->next_token.  logits_rows: logits
 // kept, 0 = none, 1 = the last row, S = all rows.
@@ -1997,6 +2012,7 @@ static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int 
   R.head = logits_rows == 0 ? HEAD_NONE : logits_rows == 1 ? HEAD_LAST : HEAD_ALL;
   R.head_rows = logits_rows > 1 ? S : 1;
   R.advance = advance; R.gather = gather;
+  R.record = s->pen_on[s->active_seq];
   return R;
 }
 // a batched step: row r is sequence r, token d_tokens[r] at position d_pos_arr[r]
@@ -2005,26 +2021,29 @@ static Rows rows_batch(const lnb_session* s, int n) {
   R.kind = ROWS_BATCH; R.S = n; R.tokens = s->d_tokens; R.pos_arr = s->d_pos_arr;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.head = HEAD_PER_ROW; R.head_rows = n;
+  for (int i = 0; i < n; i++) R.record |= s->pen_on[i];
   return R;
 }
 // a ragged call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each, then the last row of each segment
-static Rows rows_ragged(const lnb_session* s, int rows, int n_segs) {
+static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, bool record) {
   Rows R{};
   R.kind = ROWS_RAGGED; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.mb_rows = 8;
   R.seg_last = s->d_rag + 3 * rows;
   R.head = HEAD_PER_ROW; R.head_rows = n_segs;
+  R.record = record;
   return R;
 }
 // a speculative verification call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each; consecutive
 // rows of a segment are consecutive positions of one sequence, and EVERY row is an output row (its next token is compared
 // with the following draft), so the LM head runs over all of them
-static Rows rows_spec(const lnb_session* s, int rows) {
+static Rows rows_spec(const lnb_session* s, int rows, bool record) {
   Rows R{};
   R.kind = ROWS_SPEC; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.head = HEAD_PER_ROW; R.head_rows = rows;
+  R.record = record;
   return R;
 }
 
@@ -2107,10 +2126,20 @@ static bool forward_tc_ok(const lnb_session* s, int S) {
 }
 static int enqueue_forward_tc(lnb_session* s, const Rows& R);
 
+// The history write of a forward over the rows R (R.record: a row's sequence is penalized), before anything advances
+// st->pos.  token / pos0 (>= 0): the one row's token and position when they ride in a launch argument (the decode engine).
+static int launch_record(lnb_session* s, const Rows& R, int32_t token = -1, int pos0 = -1) {
+  if (!R.record) return 0;
+  return launch_kernel(Launcher{s->stream, LAUNCH_PDL, &s->launches}, penalty_record_kernel, dim3((R.S + 255) / 256), dim3(256), 0,
+                       s->d_hist, s->seq_len, (const LnbDevState*)s->st, R.tokens, R.pos_arr, R.row_seq,
+                       R.kind == ROWS_SINGLE ? s->active_seq : -1, token, pos0, R.S);
+}
+
 // Enqueue one LlamaTransformer.Forward (llamatransformer.go:145-180) for the rows R on the session stream: on the tensor
 // cores when forward_tc_ok, else as the kernel chain below.  Every forward but the decode engines' comes through here.
 static int enqueue_forward(lnb_session* s, const Rows& R) {
   s->last_was_engine = false;   // this forward's residual stream is s->x
+  if (const int rc = launch_record(s, R)) return rc;
   if (forward_tc_ok(s, R.S)) return enqueue_forward_tc(s, R);
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
@@ -2291,20 +2320,46 @@ static int launch_sample_job(const Launcher& L, const SampleJob& J) {
   if (rc) return rc;
   return launch_kernel(L, sample_kernel, dim3(J.n), dim3(SMP_THREADS), 0, J);
 }
+// ---- penalties (penalty.cuh, DESIGN.md §9e) ---------------------------------------------------------------------------
+static int launch_penalty_job(const Launcher& L, const PenaltyJob& J) {
+  int rc = launch_kernel(L, penalty_count_kernel, dim3(PEN_COUNT_CTAS, J.n), dim3(PEN_THREADS), 0, J);
+  if (rc) return rc;
+  return launch_kernel(L, penalty_apply_kernel, dim3((J.V + PEN_SLICE - 1) / PEN_SLICE, J.n), dim3(PEN_THREADS), 0, J);
+}
+
 // One sampler launch over n rows of s->logits: row[i] of sequence seq[i] draws with p_next[i] (-1: st->pos, for a decode
 // run whose step has advanced) into out[out_idx[i]]; decode: the token also feeds the next step (st->next_token) and
-// lands in d_tok_out.  Only calls with a sampled row launch it.
+// lands in d_tok_out.  Only calls with a processed row launch it.  When a row is penalized, the penalty job first writes
+// every row to d_pen_out (rows of other sequences unchanged) and the sampler reads them there; a penalized sequence that
+// does not sample draws from the greedy slot d_samp[n_seq] (temperature 0: rank 0 of l').
 static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_t* seq, const int32_t* p_next, const int32_t* out_idx,
                          int32_t* out, bool decode) {
+  const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
+  const int V = s->m->a.vocab_size;
   SampleJob J{};
-  J.logits = s->logits; J.ld = s->m->vocab_l; J.V = s->m->a.vocab_size; J.n = n;
+  J.logits = s->logits; J.ld = s->m->vocab_l; J.V = V; J.n = n;
   J.params = s->d_samp; J.wbuf = s->d_samp_w; J.pos_ptr = &s->st->pos; J.out = out;
   J.cand = s->d_samp_cand; J.cnt = reinterpret_cast<unsigned int*>(s->d_samp_cand + (size_t)s->samp_rows * SMP_MERGE);
   J.st = decode ? s->st : nullptr; J.tok_out = decode ? s->d_tok_out : nullptr;
+  bool pen = false;
   for (int i = 0; i < n; i++) {
-    J.row[i] = row[i]; J.slot[i] = seq[i]; J.p_next[i] = p_next[i]; J.out_idx[i] = out_idx ? out_idx[i] : 0;
+    J.row[i] = row[i]; J.slot[i] = s->samp_on[seq[i]] ? seq[i] : s->n_seq; J.p_next[i] = p_next[i]; J.out_idx[i] = out_idx ? out_idx[i] : 0;
+    pen |= s->pen_on[seq[i]];
   }
-  return launch_sample_job(Launcher{s->stream, LAUNCH_PDL, &s->launches}, J);
+  if (pen) {
+    PenaltyJob P{};
+    P.logits = s->logits; P.ld = s->m->vocab_l; P.V = V; P.n = n;
+    P.params = s->d_pen; P.hist = s->d_hist; P.hist_len = s->seq_len;
+    P.cnt = s->d_pen_cnt; P.out = s->d_pen_out; P.pos_ptr = &s->st->pos;
+    for (int i = 0; i < n; i++) {
+      P.row[i] = row[i]; P.slot[i] = seq[i]; P.seq[i] = seq[i]; P.p_next[i] = p_next[i]; P.on[i] = s->pen_on[seq[i]] ? 1 : 0;
+      J.row[i] = i;
+    }
+    int rc = launch_penalty_job(L, P);
+    if (rc) return rc;
+    J.logits = s->d_pen_out; J.ld = V;
+  }
+  return launch_sample_job(L, J);
 }
 
 // ---- token log-probabilities (logprob.cuh, DESIGN.md §9d) -------------------------------------------------------------
@@ -2352,7 +2407,7 @@ static int lp_upload(lnb_session* s, int n) {
 }
 
 // The end of lnb_forward(_device), lnb_forward_batch, lnb_forward_ragged and lnb_forward_speculative.  Output row i is
-// logits row row0 + i, of sequence seq[i] at next position p_next[i]; rows of sampled sequences draw into samp_out[i], the
+// logits row row0 + i, of sequence seq[i] at next position p_next[i]; rows of processed sequences draw into samp_out[i], the
 // greedy token of row i is at greedy[i].  Rows of sequences with logprobs on then write the record of p_next[i] for the
 // token they emit.  host_logits (or NULL) gets logits rows [0, logits_rows), s->h_out[0, n) the tokens at d_tok (or NULL),
 // then s->h_out[n] the sampled token of row 0 when the sampler writes beside them (samp_out != d_tok).
@@ -2361,11 +2416,11 @@ static int call_tail(lnb_session* s, int n, int row0, const int32_t* seq, const 
   int32_t srow[8], sseq[8], spn[8], sidx[8];
   int ns = 0, nl = 0;
   for (int i = 0; i < n; i++)
-    if (s->samp_on[seq[i]]) { srow[ns] = row0 + i; sseq[ns] = seq[i]; spn[ns] = p_next[i]; sidx[ns] = i; ns++; }
+    if (processed(s, seq[i])) { srow[ns] = row0 + i; sseq[ns] = seq[i]; spn[ns] = p_next[i]; sidx[ns] = i; ns++; }
   int rc;
   if (ns && (rc = launch_sample(s, ns, srow, sseq, spn, sidx, samp_out, false))) return rc;
   for (int i = 0; i < n; i++)
-    if (s->lp_top[seq[i]] >= 0) lp_row(s, nl++, row0 + i, s->samp_on[seq[i]] ? samp_out + i : greedy + i, seq[i], p_next[i], nullptr);
+    if (s->lp_top[seq[i]] >= 0) lp_row(s, nl++, row0 + i, processed(s, seq[i]) ? samp_out + i : greedy + i, seq[i], p_next[i], nullptr);
   if (nl && ((rc = lp_upload(s, nl)) || (rc = launch_logprob(s, nl)))) return rc;
   lnb_model* m = s->m;
   if (host_logits) {
@@ -2400,12 +2455,13 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
   CU(cudaSetDevice(m->device));
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
   const int32_t seq = s->active_seq, p_next = start_pos + S;
-  const bool samp = s->samp_on[seq];   // the sampler and the logprob job read the last row's logits
+  const bool samp = processed(s, seq);   // the sampler and the logprob job read the last row's logits
   const int lrows = keep_logits ? (all_rows ? S : 1) : ((samp || s->lp_top[seq] >= 0) ? 1 : 0);
   int rc;
   if (lrows && (rc = ensure_logits(s, (size_t)(keep_logits && all_rows ? s->max_rows : 1)))) return rc;
   if (S == 1 && engine_ok(s)) {
     // decode step: ONE persistent kernel; the token id rides in the launch of set_state_kernel (4 bytes of kernel arguments)
+    if ((rc = launch_record(s, rows_single(s, 1, nullptr, 0, false, false), tokens[0], start_pos))) return rc;
     if ((rc = enqueue_decode_engine(s, tokens[0], start_pos, 1, false, false, lrows ? s->logits : nullptr))) return rc;
     if (host_logits && (rc = gather_logits(s, 0, 1))) return rc;
   } else {
@@ -2564,6 +2620,33 @@ static int sampling_check(const lnb_sampling* p) {
   if (!(p->top_p > 0.0f && p->top_p <= 1.0f)) return fail(LNB_EINVAL, "top_p %g must be in (0, 1]", (double)p->top_p);
   return 0;
 }
+// The sampler's buffers, allocated by the first sampler set or penalty enable: n_seq parameter slots plus the greedy slot
+// d_samp[n_seq] (zeroed: temperature 0) of penalized sequences that do not sample, weights of n_seq rows, one token; all or
+// nothing
+static int samp_alloc(lnb_session* s) {
+  if (s->d_samp) return 0;
+  const size_t b_par = (size_t)(s->n_seq + 1) * sizeof(lnb_sampling), b_w = (size_t)s->n_seq * s->m->a.vocab_size * 8;
+  const size_t b_cand = (size_t)s->n_seq * (SMP_MERGE * 8 + 4);
+  lnb_sampling* d_par = nullptr;
+  unsigned long long *d_w = nullptr, *d_cand = nullptr;
+  int32_t* d_tok = nullptr;
+  cudaError_t e = cudaMalloc((void**)&d_par, b_par);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&d_w, b_w);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&d_tok, 16);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&d_cand, b_cand);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_par, 0, b_par, s->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_cand, 0, b_cand, s->stream);   // the split sampler's counters start at 0
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    cudaStreamSynchronize(s->stream);
+    cudaFree(d_par); cudaFree(d_w); cudaFree(d_tok); cudaFree(d_cand);
+    cudaGetLastError();
+    return fail(LNB_ENOMEM, "sampler buffers: %zu bytes of device memory asked for: %s", b_par + b_w + 16 + b_cand, cudaGetErrorString(e));
+  }
+  s->d_samp = d_par; s->d_samp_w = d_w; s->d_samp_tok = d_tok; s->d_samp_cand = d_cand;
+  s->samp_rows = s->n_seq;
+  return 0;
+}
 extern "C" int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampling* p) {
   if (!s) return fail(LNB_EINVAL, "session is NULL");
   if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
@@ -2574,31 +2657,81 @@ extern "C" int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampl
   const bool on = p && p->temperature > 0.0f;
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(s->m->device));
-  if (on && !s->d_samp) {   // parameter slots, weights of n_seq rows, one token; all or nothing
-    const size_t b_par = (size_t)s->n_seq * sizeof(lnb_sampling), b_w = (size_t)s->n_seq * s->m->a.vocab_size * 8;
-    const size_t b_cand = (size_t)s->n_seq * (SMP_MERGE * 8 + 4);
-    lnb_sampling* d_par = nullptr;
-    unsigned long long *d_w = nullptr, *d_cand = nullptr;
-    int32_t* d_tok = nullptr;
-    cudaError_t e = cudaMalloc((void**)&d_par, b_par);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_w, b_w);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_tok, 16);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_cand, b_cand);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_cand, 0, b_cand, s->stream);   // the split sampler's counters start at 0
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      cudaFree(d_par); cudaFree(d_w); cudaFree(d_tok); cudaFree(d_cand);
-      cudaGetLastError();
-      return fail(LNB_ENOMEM, "sampler buffers: %zu bytes of device memory asked for: %s", b_par + b_w + 16 + b_cand, cudaGetErrorString(e));
-    }
-    s->d_samp = d_par; s->d_samp_w = d_w; s->d_samp_tok = d_tok; s->d_samp_cand = d_cand;
-    s->samp_rows = s->n_seq;
-  }
+  if (on && (rc = samp_alloc(s))) return rc;
   if (on) {   // stream-ordered, no host synchronisation; a captured decode graph reads the slot when it replays
     sample_set_params_kernel<<<1, 1, 0, s->stream>>>(s->d_samp + seq, *p);
     CU(cudaGetLastError());
   }
   s->samp_on[seq] = on;
+  return 0;
+}
+
+// ---- penalties: parameters of one sequence and its token history (penalty.cuh, DESIGN.md §9e) --------------------------
+static int penalties_check(const lnb_penalties* p, int V) {
+  if (!std::isfinite(p->repetition_penalty) || !(p->repetition_penalty > 0.0f))
+    return fail(LNB_EINVAL, "repetition_penalty %g must be finite and > 0", (double)p->repetition_penalty);
+  if (!std::isfinite(p->frequency_penalty)) return fail(LNB_EINVAL, "frequency_penalty %g must be finite", (double)p->frequency_penalty);
+  if (!std::isfinite(p->presence_penalty)) return fail(LNB_EINVAL, "presence_penalty %g must be finite", (double)p->presence_penalty);
+  if (p->window < 0) return fail(LNB_EINVAL, "window %d must be >= 0 (0: every position)", p->window);
+  if (p->first_pos < 0) return fail(LNB_EINVAL, "first_pos %d must be >= 0", p->first_pos);
+  if (p->n_bias < 0 || p->n_bias > LNB_LOGIT_BIAS_MAX) return fail(LNB_EINVAL, "n_bias %d must be in [0, %d]", p->n_bias, LNB_LOGIT_BIAS_MAX);
+  for (int j = 0; j < p->n_bias; j++) {
+    const int t = p->bias_token[j];
+    if (t < 0 || t >= V) return fail(LNB_EINVAL, "bias_token[%d] = %d outside [0, %d)", j, t, V);
+    for (int k = 0; k < j; k++)
+      if (p->bias_token[k] == t) return fail(LNB_EINVAL, "bias_token[%d] = %d repeats bias_token[%d]", j, t, k);
+    const float b = p->bias[j];
+    if (!(std::isfinite(b) || b == -INFINITY)) return fail(LNB_EINVAL, "bias[%d] = %g must be finite or -inf", j, (double)b);
+  }
+  return 0;
+}
+extern "C" int lnb_session_set_penalties(lnb_session* s, int seq, const lnb_penalties* p) {
+  if (!s) return fail(LNB_EINVAL, "session is NULL");
+  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  if (s->m->tp_size > 1)
+    return fail(LNB_EINVAL, "penalties are not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", s->m->tp_size);
+  const int V = s->m->a.vocab_size;
+  int rc;
+  if (p && (rc = penalties_check(p, V))) return rc;
+  const bool on = p && !lnb_pen_neutral(p);
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(s->m->device));
+  if (on && !s->d_hist) {   // history of every sequence and position, parameter slots, the job's scratch; all or nothing
+    const size_t b_hist = (size_t)s->n_seq * s->seq_len * 4, b_par = (size_t)s->n_seq * sizeof(lnb_penalties),
+                 b_cnt = (size_t)PEN_MAX_ROWS * V * 4, b_out = (size_t)PEN_MAX_ROWS * V * 4;
+    int32_t* d_hist = nullptr;
+    lnb_penalties* d_par = nullptr;
+    unsigned int* d_cnt = nullptr;
+    float* d_out = nullptr;
+    cudaError_t e = cudaMalloc((void**)&d_hist, b_hist);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_par, b_par);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_cnt, b_cnt);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_out, b_out);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_hist, 0xff, b_hist, s->stream);   // -1: no token recorded
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt, 0, b_cnt, s->stream);        // the counts start at 0
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      cudaStreamSynchronize(s->stream);
+      cudaFree(d_hist); cudaFree(d_par); cudaFree(d_cnt); cudaFree(d_out);
+      cudaGetLastError();
+      return fail(LNB_ENOMEM, "penalty history and scratch: %zu bytes of device memory asked for (history %zu): %s",
+                  b_hist + b_par + b_cnt + b_out, b_hist, cudaGetErrorString(e));
+    }
+    if ((rc = samp_alloc(s))) {   // the sampler draws every penalized token
+      cudaStreamSynchronize(s->stream);
+      cudaFree(d_hist); cudaFree(d_par); cudaFree(d_cnt); cudaFree(d_out);
+      return rc;
+    }
+    s->d_hist = d_hist; s->d_pen = d_par; s->d_pen_cnt = d_cnt; s->d_pen_out = d_out;
+  } else if (on && (rc = samp_alloc(s))) {
+    return rc;
+  }
+  if (on) {   // stream-ordered, no host synchronisation; a captured decode graph reads the slot when it replays
+    if (!s->pen_on[seq]) CU(cudaMemsetAsync(s->d_hist + (size_t)seq * s->seq_len, 0xff, (size_t)s->seq_len * 4, s->stream));
+    penalty_set_params_kernel<<<1, 1, 0, s->stream>>>(s->d_pen + seq, *p);
+    CU(cudaGetLastError());
+  }
+  s->pen_on[seq] = on;
   return 0;
 }
 
@@ -2711,10 +2844,11 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
   CU(cudaMemcpyAsync(s->d_tokens, s->h_tok, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
   CU(cudaMemcpyAsync(s->d_pos_arr, s->h_pos, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
   int32_t seq[8], p_next[8];
-  bool samp = false;   // a row samples or has logprobs on: the engine stores the logits
-  for (int i = 0; i < n; i++) { seq[i] = i; p_next[i] = positions[i] + 1; samp |= s->samp_on[i] || s->lp_top[i] >= 0; }
+  bool samp = false;   // a row is processed or has logprobs on: the engine stores the logits
+  for (int i = 0; i < n; i++) { seq[i] = i; p_next[i] = positions[i] + 1; samp |= processed(s, i) || s->lp_top[i] >= 0; }
   if (batch_engine_ok(s)) {
     // ONE launch of the batch engine: every weight matrix streamed once for all n sequences
+    if ((rc = launch_record(s, rows_batch(s, n)))) return rc;
     if ((rc = batch_engine_build(s, (logits || samp) ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, n, s->d_tokens, s->d_pos_arr, nullptr))) return rc;
     if (logits && (rc = gather_logits(s, 0, n))) return rc;
@@ -2807,7 +2941,9 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
     h[3 * rows + i] = r - 1;
   }
   CU(cudaMemcpyAsync(s->d_rag, h, (size_t)(3 * rows + n_segs) * 4, cudaMemcpyHostToDevice, s->stream));
-  if ((rc = enqueue_forward(s, rows_ragged(s, rows, n_segs)))) return rc;
+  bool pen = false;
+  for (int i = 0; i < n_segs; i++) pen |= s->pen_on[seq[i]];
+  if ((rc = enqueue_forward(s, rows_ragged(s, rows, n_segs, pen)))) return rc;
   int32_t p_next[8];
   for (int i = 0; i < n_segs; i++) p_next[i] = start_pos[i] + len[i];
   if ((rc = call_tail(s, n_segs, 0, seq, p_next, s->d_next_arr, s->d_next_arr, logits, n_segs, argmax_out ? s->d_next_arr : nullptr))) return rc;
@@ -2884,12 +3020,13 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
   if (!eng && !s->sdpa_smem_decode && !s->ss.sc)
     return fail(LNB_EINVAL, "speculative calls beyond the shared-memory attention kernel need head_dim <= 128 and n_rep <= 8");
   int32_t row_seq[8], row_pos[8];
-  bool samp = false, lp = false;
+  bool samp = false, lp = false, pen = false;
   for (int i = 0, r = 0; i < n_segs; i++)
     for (int k = 0; k <= n_draft[i]; k++, r++) {
       row_seq[r] = seq[i];
       row_pos[r] = start_pos[i] + k;
-      samp |= s->samp_on[seq[i]];
+      samp |= processed(s, seq[i]);
+      pen |= s->pen_on[seq[i]];
       lp |= s->lp_top[seq[i]] >= 0;
     }
   if (!s->d_rag) {   // the row map (shared with ragged calls)
@@ -2912,11 +3049,12 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
   CU(cudaMemcpyAsync(s->d_rag, h, (size_t)3 * rows * 4, cudaMemcpyHostToDevice, s->stream));
   if (eng) {
     // ONE launch of the batch engine: every weight matrix streamed once for all rows
+    if ((rc = launch_record(s, rows_spec(s, rows, pen)))) return rc;
     if ((rc = batch_engine_build(s, (logits || samp || lp) ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, rows, s->d_rag, s->d_rag + 2 * rows, s->d_rag + rows))) return rc;
   } else {
     if ((rc = set_state(s, 0, rows, -1, false))) return rc;
-    if ((rc = enqueue_forward(s, rows_spec(s, rows)))) return rc;
+    if ((rc = enqueue_forward(s, rows_spec(s, rows, pen)))) return rc;
   }
   int32_t p_next[8];
   for (int r = 0; r < rows; r++) p_next[r] = row_pos[r] + 1;
@@ -2943,10 +3081,14 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
   int rc;
   // a sampled sequence decodes on the kernel chain (the persistent engine feeds back the greedy token inside the kernel):
   // each step keeps its logits row and ends in the sampler, whose token is the next step's input.  A sequence with
-  // logprobs on decodes on the chain too, each step then ending in the logprob job keyed on st->pos (= p_next).
+  // logprobs on decodes on the chain too, each step then ending in the logprob job keyed on st->pos (= p_next).  A
+  // penalized sequence records its token, runs the penalty job and draws from the sampler (greedy: its rank 0) each step.
   const int seq = s->active_seq;
-  const bool samp = s->samp_on[seq], lp = s->lp_top[seq] >= 0, keep = samp || lp;
-  if (samp && engine_ok(s)) g_err = "the active sequence samples: lnb_decode_run runs the kernel chain (the decode engine has no sampler)";
+  const bool pen = s->pen_on[seq], samp = processed(s, seq), greedy_slot = samp && !s->samp_on[seq];
+  const bool lp = s->lp_top[seq] >= 0, keep = samp || lp;
+  if (s->samp_on[seq] && engine_ok(s)) g_err = "the active sequence samples: lnb_decode_run runs the kernel chain (the decode engine has no sampler)";
+  else if (pen && engine_ok(s))
+    g_err = "the active sequence is penalized: lnb_decode_run runs the kernel chain (the decode engine keeps no token history)";
   else if (lp && engine_ok(s))
     g_err = "the active sequence has logprobs on: lnb_decode_run runs the kernel chain (the decode engine keeps no logits row)";
   if (!keep && engine_ok(s)) {
@@ -2966,7 +3108,9 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     return use_graph ? 1 : 0;   // (no graph is needed: there is nothing left to replay)
   }
   if (keep && (rc = ensure_logits(s, 1))) return rc;
-  if (s->graph_tried && (s->graph_sampled != samp || s->graph_lp != lp || (keep && s->graph_logits != s->logits))) drop_graph(s);
+  if (s->graph_tried && (s->graph_sampled != samp || s->graph_lp != lp || s->graph_pen != pen || s->graph_greedy != greedy_slot ||
+                         (keep && s->graph_logits != s->logits)))
+    drop_graph(s);
   if (lp) {   // the job's one row, read by every step (and by the graph's replays): the token st->next_token, record st->pos
     lp_row(s, 0, 0, &s->st->next_token, seq, 0, &s->st->pos);
     if ((rc = lp_upload(s, 1))) return rc;
@@ -2982,6 +3126,8 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     s->graph_tried = true;
     s->graph_sampled = samp;
     s->graph_lp = lp;
+    s->graph_pen = pen;
+    s->graph_greedy = greedy_slot;
     s->graph_logits = s->logits;
     cudaGraph_t g = nullptr;
     const int64_t saved = s->launches;
@@ -3616,6 +3762,35 @@ extern "C" int lnb_op_logprobs_f32(const float* logits, int rows, int vocab, con
   D2H(rec.data(), drec, (size_t)rows * sizeof(LpRecord));
   memset(out, 0, (size_t)rows * sizeof(lnb_logprob));
   for (int i = 0; i < rows; i++) lp_finish(rec[i], out + i);
+  return 0;
+}
+
+// the penalty kernels alone on host rows: logits[rows, vocab], p[rows], histories hist[rows][hist_len], pos_next[rows] -> out
+extern "C" int lnb_op_penalize_f32(const float* logits, int rows, int vocab, const lnb_penalties* p, const int32_t* hist, int hist_len,
+                                   const int32_t* pos_next, float* out) {
+  OpScope scope_;
+  if (!logits || !p || !hist || !pos_next || !out) return fail(LNB_EINVAL, "NULL argument");
+  if (rows < 1 || rows > PEN_MAX_ROWS || vocab < 1 || hist_len < 1)
+    return fail(LNB_EINVAL, "rows %d must be in [1, %d], vocab %d and hist_len %d >= 1", rows, PEN_MAX_ROWS, vocab, hist_len);
+  int rc;
+  for (int r = 0; r < rows; r++) {
+    if ((rc = penalties_check(p + r, vocab))) return rc;
+    if (pos_next[r] < 0 || pos_next[r] > hist_len) return fail(LNB_EINVAL, "pos_next[%d] = %d outside [0, %d]", r, pos_next[r], hist_len);
+  }
+  const size_t b = (size_t)rows * vocab * 4, bh = (size_t)rows * hist_len * 4;
+  OPBUF(dx, b); OPBUF(dp, (size_t)rows * sizeof(lnb_penalties)); OPBUF(dh, bh); OPBUF(dc, b); OPBUF(dout, b);
+  H2D(dx, logits, b);
+  H2D(dp, p, (size_t)rows * sizeof(lnb_penalties));
+  H2D(dh, hist, bh);
+  CU(cudaMemset(dc.p, 0, b));
+  PenaltyJob J{};
+  J.logits = dx.as<float>(); J.ld = vocab; J.V = vocab; J.n = rows;
+  J.params = dp.as<lnb_penalties>(); J.hist = dh.as<int32_t>(); J.hist_len = hist_len;
+  J.cnt = dc.as<unsigned int>(); J.out = dout.as<float>(); J.pos_ptr = nullptr;
+  for (int r = 0; r < rows; r++) { J.row[r] = r; J.slot[r] = r; J.seq[r] = r; J.p_next[r] = pos_next[r]; J.on[r] = lnb_pen_neutral(p + r) ? 0 : 1; }
+  if ((rc = launch_penalty_job(Launcher{nullptr, LAUNCH_PLAIN, nullptr}, J))) return rc;
+  if ((rc = op_finish())) return rc;
+  D2H(out, dout, b);
   return 0;
 }
 

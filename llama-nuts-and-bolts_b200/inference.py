@@ -15,6 +15,7 @@ from . import ml, model as model_mod
 
 GSInProgress, GSFinishedByReachingEOS, GSFinishedByReachingSeqLen = 0, 1, 2
 SamplingArgs = model_mod.SamplingArgs
+PenaltyArgs = model_mod.PenaltyArgs
 
 
 @dataclass
@@ -73,6 +74,12 @@ def _logprob_lists(infContext, seqs, logprobs: int | None, logprobs_out: list | 
     lists = [[] for _ in range(n_lists)]
     logprobs_out.extend(lists)
     return lists
+
+
+def _set_penalties(infContext, seq: int, penalties: "PenaltyArgs | None", prompt_len: int):
+    """sequence `seq` of the context is penalized with `penalties` for a prompt of prompt_len tokens (None: left off)"""
+    if penalties is not None:
+        infContext.set_penalties(seq, penalties, prompt_len)
 
 
 def _check_speculative(speculative, use_reference_api: bool = False):
@@ -168,7 +175,8 @@ class InferenceEngine:
     def GenerateTokens(self, promptTokens, use_reference_api: bool = False, step_times: list | None = None,
                        prefill_chunk: int = 0, sampling: "SamplingArgs | None" = None,
                        speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None,
-                       logprobs: int | None = None, logprobs_out: list | None = None):
+                       logprobs: int | None = None, logprobs_out: list | None = None,
+                       penalties: "PenaltyArgs | None" = None):
         """Generator over (state, token id) exactly like generatedTokensCh.
 
         use_reference_api=True goes through the reference-shaped calls of every iteration
@@ -189,10 +197,16 @@ class InferenceEngine:
         the fused entry: use_reference_api=True with speculative is an error.
 
         logprobs (EXTENSION): 0..20 turns on token log-probabilities (lnb_session_set_logprobs); logprobs_out then gets one
-        model.TokenLogprob per emitted token, in order, with the top `logprobs` alternatives.  The stream is unchanged."""
+        model.TokenLogprob per emitted token, in order, with the top `logprobs` alternatives.  The stream is unchanged.
+
+        penalties (EXTENSION): PenaltyArgs, applied on the device to every emitted token's logits before the sampler (or
+        the greedy pick); CountPrompt False starts the counted history at the prompt's length.  The records of logprobs
+        stay those of the raw distribution.  use_reference_api=True with penalties is an error."""
         sampling = _sampling_for(sampling, 0)
         if sampling is not None and use_reference_api:
             raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax (inference.go:207-216); it cannot sample")
+        if penalties is not None and use_reference_api:
+            raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax of the raw logits; it cannot apply penalties")
         _check_speculative(speculative, use_reference_api)
         infContext = self.CreateInferenceContext()
         try:
@@ -200,6 +214,7 @@ class InferenceEngine:
                 infContext.set_sampling(0, sampling)
             lp_out = _logprob_lists(infContext, [0], logprobs, [logprobs_out])
             promptLength = len(promptTokens)
+            _set_penalties(infContext, 0, penalties, promptLength)
             if prefill_chunk > 0:
                 infContext.allow_chunked_prefill(True)
                 if prefill_chunk > infContext.max_rows:
@@ -309,7 +324,8 @@ class InferenceEngine:
 
     def GenerateTokensContinuous(self, prompts, slots: int = 8, step_tokens: int | None = None,
                                  step_times: list | None = None, sampling: "SamplingArgs | None" = None,
-                                 logprobs: int | None = None, logprobs_out: list | None = None):
+                                 logprobs: int | None = None, logprobs_out: list | None = None,
+                                 penalties: "PenaltyArgs | None" = None):
         """Continuous batching (EXTENSION, lnb_forward_ragged): any number of prompts through at most `slots` live
         sequences.  Every step is ONE forward whose rows may belong to different sequences: each decoding sequence gets
         its one row, the rest of the step's row budget (min(step_tokens, max_rows)) goes to prompt chunks, first in first
@@ -318,7 +334,8 @@ class InferenceEngine:
         batch engine: one launch per step).  Yields (prompt index, state, token id); per prompt the stream is exactly
         what GenerateTokens(prompts[i]) yields (the bookkeeping of generateTokensInternal, inference.go:173-254).
         sampling: prompt i samples with Seed + i (the stream of GenerateTokens(prompts[i]) with that seed).
-        logprobs / logprobs_out as in GenerateTokens: logprobs_out gets one list per prompt."""
+        logprobs / logprobs_out as in GenerateTokens: logprobs_out gets one list per prompt.  penalties as in GenerateTokens,
+        for every prompt (set again at each admission: its first_pos follows the admitted prompt)."""
         if step_tokens is None:
             step_tokens = DEFAULT_STEP_TOKENS
         if not 1 <= slots <= 8:
@@ -332,14 +349,16 @@ class InferenceEngine:
             self.context_hook(infContext)
         try:
             yield from self._generate_continuous(infContext, prompts, slots, min(step_tokens, infContext.max_rows), step_times,
-                                                 sampling, logprobs, logprobs_out)
+                                                 sampling, logprobs, logprobs_out, penalties)
         finally:
             infContext.close()
 
     def _generate_continuous(self, infContext, prompts, slots: int, budget: int, step_times: list | None = None,
-                             sampling: "SamplingArgs | None" = None, logprobs: int | None = None, logprobs_out: list | None = None):
+                             sampling: "SamplingArgs | None" = None, logprobs: int | None = None, logprobs_out: list | None = None,
+                             penalties: "PenaltyArgs | None" = None):
         """the scheduler of GenerateTokensContinuous on a given context (anything with SequenceLength, forward_ragged and
-        forward_batch, set_sampling when `sampling` samples, set_logprobs and read_logprobs when `logprobs` is set)"""
+        forward_batch, set_sampling when `sampling` samples, set_logprobs and read_logprobs when `logprobs` is set,
+        set_penalties when `penalties` is set)"""
         seqLen = infContext.SequenceLength
         stop = self.model.Vocabulary.StopTokenIds
         for p in prompts:
@@ -361,6 +380,7 @@ class InferenceEngine:
                     sp = _sampling_for(sampling, slot[k]["i"])
                     if sp is not None:   # before the prompt's first segment (the slot's previous prompt had another seed)
                         infContext.set_sampling(k, sp)
+                    _set_penalties(infContext, k, penalties, len(prompts[slot[k]["i"]]))
             decoding = [k for k in range(slots) if slot[k] is not None and slot[k]["cur"] is not None]
             prefilling = sorted((k for k in range(slots) if slot[k] is not None and slot[k]["cur"] is None),
                                 key=lambda k: slot[k]["order"])
@@ -412,7 +432,8 @@ class InferenceEngine:
 
     def GenerateTokensBatch(self, prompts, step_times: list | None = None, sampling: "SamplingArgs | None" = None,
                             speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None,
-                            logprobs: int | None = None, logprobs_out: list | None = None):
+                            logprobs: int | None = None, logprobs_out: list | None = None,
+                            penalties: "PenaltyArgs | None" = None):
         """The consumer `InferenceEngine.TokenizeBatch` (src/inference/tokenize.go:97-107) never got in the
         reference (SURVEY 8f-4): every prompt runs the loop of generateTokensInternal (:173-254) -- own
         InferenceContext / KV cache, own positions, own stop condition -- but all sequences advance together,
@@ -422,7 +443,7 @@ class InferenceEngine:
         speculative (EXTENSION): after the prompts, every call is one lnb_forward_speculative in which each unfinished
         sequence gets its row and the rest of the 8-row budget goes to prompt-lookup drafts in sequence order; the streams
         are the same.  spec_stats as in GenerateTokens; logprobs / logprobs_out as in GenerateTokens, logprobs_out gets one
-        list per prompt."""
+        list per prompt; penalties as in GenerateTokens, for every sequence."""
         _check_speculative(speculative)
         n = len(prompts)
         if n < 1:
@@ -433,7 +454,7 @@ class InferenceEngine:
                 lp0 = []
                 logprobs_out.append(lp0)
             for state, tok in self.GenerateTokens(prompts[0], sampling=sampling, speculative=speculative, spec_stats=spec_stats,
-                                                  logprobs=logprobs, logprobs_out=lp0):
+                                                  logprobs=logprobs, logprobs_out=lp0, penalties=penalties):
                 yield 0, state, tok
             return
         infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
@@ -452,6 +473,7 @@ class InferenceEngine:
                 sp = _sampling_for(sampling, i)
                 if sp is not None:
                     infContext.set_sampling(i, sp)
+                _set_penalties(infContext, i, penalties, len(prompts[i]))
             lp_out = _logprob_lists(infContext, range(n), logprobs, logprobs_out, n)
             cur = [0] * n                                  # token fed next / position it is fed at
             pos = [0] * n

@@ -166,6 +166,41 @@ class SamplingArgs:
 
 
 @dataclass
+class PenaltyArgs:
+    """EXTENSION: repetition, frequency and presence penalties and a logit bias over the sequence's token history,
+    lnb_session_set_penalties (DESIGN.md §9e).  For the token at position p, a token fed c >= 1 times among the last Window
+    positions (0: all) has its logit l divided (l > 0) or multiplied (l <= 0) by RepetitionPenalty, then lowered by
+    c * FrequencyPenalty + PresencePenalty; LogitBias {token: bias} adds bias (-inf: the token is never emitted).  The
+    sampler (greedy at Temperature 0) then draws from those logits.  CountPrompt False counts generated tokens only (the
+    OpenAI semantics): the prompt's positions are never counted.  The defaults are neutral (penalties off)."""
+    RepetitionPenalty: float = 1.0
+    FrequencyPenalty: float = 0.0
+    PresencePenalty: float = 0.0
+    Window: int = 0
+    CountPrompt: bool = False
+    LogitBias: dict = field(default_factory=dict)
+
+    def first_pos(self, prompt_len: int) -> int:
+        return 0 if self.CountPrompt else int(prompt_len)
+
+    def c(self, prompt_len: int = 0) -> "_capi.PenaltiesC":
+        """the lnb_penalties of a sequence whose prompt has prompt_len tokens"""
+        if len(self.LogitBias) > _capi.LNB_LOGIT_BIAS_MAX:
+            raise ml.MlError(f"LogitBias has {len(self.LogitBias)} entries, at most {_capi.LNB_LOGIT_BIAS_MAX}")
+        p = _capi.PenaltiesC()
+        p.repetition_penalty = float(self.RepetitionPenalty)
+        p.frequency_penalty = float(self.FrequencyPenalty)
+        p.presence_penalty = float(self.PresencePenalty)
+        p.window = int(self.Window)
+        p.first_pos = self.first_pos(prompt_len)
+        p.n_bias = len(self.LogitBias)
+        for j, (t, b) in enumerate(self.LogitBias.items()):
+            p.bias_token[j] = int(t)
+            p.bias[j] = float(b)
+        return p
+
+
+@dataclass
 class TokenLogprob:
     """EXTENSION: one record of lnb_session_logprobs_read.  Logprob is the raw model distribution's (temperature 1, no
     top-k / top-p); Rank 1 is the greedy token; Top holds (token, logprob) of the top_n first tokens in rank order."""
@@ -286,6 +321,15 @@ class InferenceContext:
         else:
             c = args.c()
             check(lib.lnb_session_set_sampling(self.h, seq, C.byref(c)))
+
+    def set_penalties(self, seq: int, args: "PenaltyArgs | None", prompt_len: int = 0):
+        """EXTENSION: sequence `seq` is penalized with `args` (None or neutral values: off) from its next forward on.
+        Turning them on clears the sequence's token history; prompt_len gives first_pos when args.CountPrompt is False."""
+        if args is None:
+            check(lib.lnb_session_set_penalties(self.h, seq, None))
+        else:
+            c = args.c(prompt_len)
+            check(lib.lnb_session_set_penalties(self.h, seq, C.byref(c)))
 
     def set_logprobs(self, seq: int, top_n: int | None):
         """EXTENSION: from its next forward on, every token sequence `seq` emits writes its logprob record (the raw model

@@ -11,6 +11,7 @@
 
 #include "../include/lnb.h"
 #include "../llama-nuts-and-bolts_b200/csrc/sample_det.h"
+#include "../llama-nuts-and-bolts_b200/csrc/penalty_det.h"
 #include "../oracle/lnb_oracle.h"
 
 double orc_exp_det(double z) { return lnb_exp_det(z); }
@@ -122,6 +123,29 @@ void orc_logprob_rows(const float* l, int rows, int V, const int32_t* targets, i
   for (int r = 0; r < rows; r++) orc_logprob_row(l + (size_t)r * V, V, targets[r], top_n, out + r);
 }
 
+/* one row: l' of the penalties and bias (DESIGN.md §9e) for the token at position p_next, given the tokens hist[0, p_next)
+ * fed before it (-1: not counted) -- counts by a plain walk over the window, then the steps of csrc/penalty_det.h */
+void orc_penalize_row(const float* l, int V, const lnb_penalties* p, const int32_t* hist, int32_t p_next, float* out) {
+  if (lnb_pen_neutral(p)) {   /* off: the row itself */
+    memcpy(out, l, (size_t)V * sizeof(float));
+    return;
+  }
+  uint32_t* c = (uint32_t*)calloc((size_t)V, 4);
+  int32_t lo = lnb_pen_lo(p, p_next);
+  if (lo < 0) lo = 0;
+  for (int32_t i = lo; i < p_next; i++)
+    if (hist[i] >= 0 && hist[i] < V) c[hist[i]]++;
+  for (int i = 0; i < V; i++) out[i] = lnb_pen_apply(l[i], c[i], p->repetition_penalty, p->frequency_penalty, p->presence_penalty);
+  for (int j = 0; j < p->n_bias; j++) out[p->bias_token[j]] = lnb_pen_bias(out[p->bias_token[j]], p->bias[j]);
+  free(c);
+}
+/* rows x V logits, row r with parameters p[r], history hist[r][hist_len] and p_next[r] -> out[rows][V] */
+void orc_penalize_rows(const float* l, int rows, int V, const lnb_penalties* p, const int32_t* hist, int hist_len, const int32_t* p_next,
+                       float* out) {
+  for (int r = 0; r < rows; r++)
+    orc_penalize_row(l + (size_t)r * V, V, p + r, hist + (size_t)r * hist_len, p_next[r], out + (size_t)r * V);
+}
+
 /* rows x V logits -> rows tokens, parameters per row */
 void orc_sample_rows(const float* l, int rows, int V, const float* T, const int32_t* K, const float* P, const uint64_t* seed,
                      const int64_t* p_next, int32_t* out) {
@@ -152,6 +176,36 @@ int orc_generate_sampled(const orc_model* m, int vocab, const int32_t* prompt, i
     if (cur + 1 == seq_len) break;
   }
   free(tokens); free(logits);
+  orc_session_free(s);
+  return n_out;
+}
+
+/* orc_generate_sampled with the penalties in front of the sampler (greedy at T = 0): the token for position cur is drawn
+ * from orc_penalize_row of the logits with the tokens fed at [0, cur) (pen NULL: orc_generate_sampled) */
+int orc_generate_processed(const orc_model* m, int vocab, const int32_t* prompt, int n_prompt, int seq_len, const int32_t* stop_ids,
+                           int n_stop, float T, int32_t K, float P, uint64_t seed, const lnb_penalties* pen, int32_t* out) {
+  if (n_prompt >= seq_len) return -1;
+  orc_session* s = orc_session_new(m, seq_len);
+  int32_t* tokens = (int32_t*)malloc((size_t)seq_len * 4);
+  for (int i = 0; i < seq_len; i++) tokens[i] = -1;
+  for (int i = 0; i < n_prompt; i++) tokens[i] = prompt[i];
+  float* logits = (float*)malloc((size_t)vocab * sizeof(float));
+  float* proc = (float*)malloc((size_t)vocab * sizeof(float));
+  int prev = 0, n_out = 0;
+  for (int cur = n_prompt; cur < seq_len; cur++) {
+    if (orc_forward(m, s, tokens + prev, cur - prev, prev, logits, 0, NULL) != 0) { n_out = -1; break; }
+    if (pen) orc_penalize_row(logits, vocab, pen, tokens, cur, proc);
+    int32_t next = orc_sample_row(pen ? proc : logits, vocab, T, K, P, seed, cur);
+    if (tokens[cur] != -1) next = tokens[cur];
+    tokens[cur] = next;
+    out[n_out++] = next;
+    prev = cur;
+    int eos = 0;
+    for (int i = 0; i < n_stop; i++) eos |= (stop_ids[i] == next);
+    if (eos) break;
+    if (cur + 1 == seq_len) break;
+  }
+  free(tokens); free(logits); free(proc);
   orc_session_free(s);
   return n_out;
 }

@@ -1,4 +1,4 @@
-"""ctypes binding of the sampler's sequential C statement (TEST INFRASTRUCTURE, NOT PRODUCT CODE; DESIGN.md §9b).
+"""ctypes binding of the sampler's sequential C statement (TEST INFRASTRUCTURE, NOT PRODUCT CODE; DESIGN.md §9b, §9e).
 
 Only tests/ and tools/ may import this module.  See lnb_sample_ref.c.
 """
@@ -23,11 +23,30 @@ _f32p, _i32p, _i64p, _u64p, _f64p = (C.POINTER(C.c_float), C.POINTER(C.c_int32),
                                      C.POINTER(C.c_double))
 _lib = None
 
+LOGIT_BIAS_MAX = 64
+
+
+class Penalties(C.Structure):   # lnb_penalties (include/lnb.h)
+    _fields_ = [("repetition_penalty", C.c_float), ("frequency_penalty", C.c_float), ("presence_penalty", C.c_float),
+                ("window", C.c_int32), ("first_pos", C.c_int32), ("n_bias", C.c_int32),
+                ("bias_token", C.c_int32 * LOGIT_BIAS_MAX), ("bias", C.c_float * LOGIT_BIAS_MAX)]
+
+
+def penalties(rp: float = 1.0, fp: float = 0.0, pp: float = 0.0, window: int = 0, first_pos: int = 0, bias=None) -> Penalties:
+    """an lnb_penalties; bias: {token: bias}"""
+    p = Penalties(float(rp), float(fp), float(pp), int(window), int(first_pos), 0)
+    for j, (t, b) in enumerate((bias or {}).items()):
+        p.bias_token[j] = int(t)
+        p.bias[j] = float(b)
+        p.n_bias = j + 1
+    return p
+
 
 def build(force: bool = False) -> str:
     _oracle.build()
     src = [os.path.join(_HERE, f) for f in ("lnb_sample_ref.c", "Makefile")] + \
-          [os.path.join(_ROOT, "llama-nuts-and-bolts_b200", "csrc", "sample_det.h"), os.path.join(_ROOT, "include", "lnb.h")]
+          [os.path.join(_ROOT, "llama-nuts-and-bolts_b200", "csrc", f) for f in ("sample_det.h", "penalty_det.h")] + \
+          [os.path.join(_ROOT, "include", "lnb.h")]
     stale = (not os.path.exists(_SO)) or any(os.path.getmtime(s) > os.path.getmtime(_SO) for s in src)
     if force or stale:
         subprocess.check_call(["make", "-C", _HERE, "-s"])
@@ -50,6 +69,11 @@ def lib():
         L.orc_sample_rows.argtypes = [_f32p, C.c_int, C.c_int, _f32p, _i32p, _f32p, _u64p, _i64p, _i32p]
         L.orc_logprob_rows.restype = None
         L.orc_logprob_rows.argtypes = [_f32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_void_p]
+        L.orc_penalize_rows.restype = None
+        L.orc_penalize_rows.argtypes = [_f32p, C.c_int, C.c_int, C.POINTER(Penalties), _i32p, C.c_int, _i32p, _f32p]
+        L.orc_generate_processed.restype = C.c_int
+        L.orc_generate_processed.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
+                                             C.c_float, C.c_uint64, C.POINTER(Penalties), _i32p]
         L.orc_generate_sampled.restype = C.c_int
         L.orc_generate_sampled.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
                                            C.c_float, C.c_uint64, _i32p]
@@ -106,4 +130,35 @@ def generate_sampled(om, prompt, seq_len: int, T: float, K: int, P: float, seed:
                                    stop.ctypes.data_as(_i32p), len(stop), T, K, P, seed & (2**64 - 1), out.ctypes.data_as(_i32p))
     if n < 0:
         raise RuntimeError("orc_generate_sampled failed")
+    return out[:n].copy()
+
+
+def penalize_rows(logits, params, hist, p_next) -> np.ndarray:
+    """orc_penalize_row of every row of logits [rows, V] with params[r] (Penalties), history hist[r] (a row of a
+    [rows, hist_len] int array, -1: not counted) and p_next[r]: l' [rows, V] f32"""
+    l = np.ascontiguousarray(logits, np.float32)
+    l = l.reshape(-1, l.shape[-1])
+    rows = l.shape[0]
+    h = np.ascontiguousarray(hist, np.int32).reshape(rows, -1)
+    pn = np.ascontiguousarray(p_next, np.int32).reshape(-1)
+    assert pn.shape[0] == rows and len(params) == rows
+    assert all(0 <= int(x) <= h.shape[1] for x in pn)
+    par = (Penalties * rows)(*params)
+    out = np.empty_like(l)
+    lib().orc_penalize_rows(l.ctypes.data_as(_f32p), rows, l.shape[1], par, h.ctypes.data_as(_i32p), h.shape[1],
+                            pn.ctypes.data_as(_i32p), out.ctypes.data_as(_f32p))
+    return out
+
+
+def generate_processed(om, prompt, seq_len: int, T: float, K: int, P: float, seed: int, pen: "Penalties | None",
+                       stop_ids=(128008, 128009)) -> np.ndarray:
+    """orc_generate with the penalties, then the sampler (greedy at T = 0), in place of the argmax (om: oracle.OracleModel)"""
+    prompt = np.ascontiguousarray(prompt, np.int32)
+    stop = np.ascontiguousarray(stop_ids, np.int32)
+    out = np.empty(seq_len, np.int32)
+    n = lib().orc_generate_processed(om.h, om.args.vocab, prompt.ctypes.data_as(_i32p), len(prompt), seq_len,
+                                     stop.ctypes.data_as(_i32p), len(stop), T, K, P, seed & (2**64 - 1),
+                                     C.byref(pen) if pen is not None else None, out.ctypes.data_as(_i32p))
+    if n < 0:
+        raise RuntimeError("orc_generate_processed failed")
     return out[:n].copy()
