@@ -10,6 +10,9 @@
 // weights (lnb_forward_speculative); the generated ids are the same as without it.  Not with slots=.
 // rep=R freq=F pres=P [last_n=N]: repetition, frequency and presence penalties over the generated tokens (the last N positions;
 // 0, the default: all) before the sampler or the greedy pick (lnb_session_set_penalties).
+// beams=B [len_pen=A] [early_stop=1]: beam search with B in [1, 8] beams (inference::GenerateBeams): one line per hypothesis,
+// best first, with its state (1 EOS, 2 SequenceLength), raw score s and normalised score h = s / len^A, then its tokens (or
+// text with a tokenizer).  Not with batch=, temp=, spec= or the penalties.
 // logprobs=N (0..20): after the generated ids, one line per generated token with its logprob, its rank and the top N
 // alternatives (lnb_session_set_logprobs; the raw model distribution, also for sampled tokens).
 // score=TEXT (with <modelDir>/tokenizer.model): TEXT is tokenized without the chat template and scored in chunks of 64 tokens
@@ -149,11 +152,16 @@ int main(int argc, char** argv) {
     model::SamplingArgs sampling;   // temp= top_k= top_p= seed= (temp 0, the default: greedy)
     model::SpeculativeArgs spec;    // spec=K: speculative decoding with up to K prompt-lookup drafts per call (0: plain steps)
     model::PenaltyArgs pen;         // rep= freq= pres= last_n= (the defaults: off)
+    inference::BeamSearchArgs beam_args;   // beams= len_pen= early_stop= (NumBeams 0: no beam search)
+    beam_args.NumBeams = 0;
     for (int i = 1; i < argc; i++) {
       if (!strncmp(argv[i], "rep=", 4)) pen.RepetitionPenalty = (float)atof(argv[i] + 4);
       if (!strncmp(argv[i], "freq=", 5)) pen.FrequencyPenalty = (float)atof(argv[i] + 5);
       if (!strncmp(argv[i], "pres=", 5)) pen.PresencePenalty = (float)atof(argv[i] + 5);
       if (!strncmp(argv[i], "last_n=", 7)) pen.Window = atoi(argv[i] + 7);
+      if (!strncmp(argv[i], "beams=", 6)) beam_args.NumBeams = atoi(argv[i] + 6);
+      if (!strncmp(argv[i], "len_pen=", 8)) beam_args.LengthPenalty = atof(argv[i] + 8);
+      if (!strncmp(argv[i], "early_stop=", 11)) beam_args.EarlyStopping = atoi(argv[i] + 11) != 0;
       if (!strncmp(argv[i], "spec=", 5)) spec.MaxDraft = atoi(argv[i] + 5);
       if (!strncmp(argv[i], "batch=", 6)) batch = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "slots=", 6)) slots = atoi(argv[i] + 6);
@@ -183,6 +191,21 @@ int main(int argc, char** argv) {
     const model::SpeculativeArgs* speculative = spec.MaxDraft > 0 ? &spec : nullptr;
     const model::PenaltyArgs* penalties = pen.Neutral() ? nullptr : &pen;
     if (speculative && slots > 0) throw Error("spec= is not built for continuous batching (slots=)");
+    if (beam_args.NumBeams != 0) {
+      if (batch > 0) throw Error("beams= is not built with batch=");
+      beam_args.NumReturn = std::max(1, beam_args.NumBeams);
+      const std::vector<inference::BeamHypothesis> hyps =
+          inference::GenerateBeams(transformer, vocab, seq_len, acc, prompt, beam_args, &sampling, penalties, speculative);
+      for (size_t i = 0; i < hyps.size(); i++) {
+        const inference::BeamHypothesis& h = hyps[i];
+        printf("beam[%zu]: state %d s %.17g h %.17g |", i, (int)h.State, h.Score, h.NormalizedScore);
+        if (tokenizer) printf(" text: %s", tokenizer->TokenBatchToString(h.Tokens).c_str());
+        else
+          for (int32_t t : h.Tokens) printf(" %d", t);
+        printf("\n");
+      }
+      return 0;
+    }
     if (batch > 0) {
       const int mod = transformer.args.vocab_size < 128256 ? 1000 : 128000;
       std::vector<std::vector<int32_t>> prompts(batch, prompt);

@@ -11,6 +11,7 @@
 #include <functional>
 #include <stdexcept>
 #include <algorithm>
+#include <cmath>
 #include <memory>
 #include <string>
 #include <vector>
@@ -423,6 +424,12 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
                                   accepted.data()));
     return next;
   }
+  // EXTENSION (lnb_session_copy_sequences): positions [pos0, pos1) of sequence dst[i] get what sequence src[i] held there
+  // before the call (K and V of every layer, the penalty history, the logprob records); the sources are read as a snapshot
+  void CopySequences(const std::vector<int32_t>& src, const std::vector<int32_t>& dst, int pos0, int pos1) {
+    if (src.size() != dst.size()) throw Error(std::to_string(src.size()) + " sources for " + std::to_string(dst.size()) + " destinations");
+    check(lnb_session_copy_sequences(h_, (int)src.size(), src.data(), dst.data(), pos0, pos1));
+  }
   int MaxRows() const { return maxRows_; }
   InferenceContext(const InferenceContext&) = delete;
   // LlamaTransformer.Forward (llamatransformer.go:145-180): tokens [S] -> f32 logits [S, vocab]
@@ -730,6 +737,147 @@ inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const
       emit(i, state, tok);
     }
   }
+}
+// EXTENSION: beam search (DESIGN.md §9f), the rules of the Python mirror's GenerateBeams.  NumBeams B in [1, 8]; a hypothesis
+// of raw score s (the f64 sum of its tokens' logprobs) and n generated tokens ranks by h = s / pow(n, LengthPenalty).
+struct BeamSearchArgs {
+  int NumBeams = 1;
+  double LengthPenalty = 1.0;
+  bool EarlyStopping = false;
+  int NumReturn = 1;
+};
+struct BeamHypothesis {
+  std::vector<int32_t> Tokens;
+  double Score = 0.0, NormalizedScore = 0.0;
+  std::vector<double> Logprobs;
+  GenerationState State = GSInProgress;
+};
+
+namespace beam_detail {
+// -1: a before b, 1: after, 0: tie -- score descending, -inf after every finite score, NaN last
+inline int ScoreOrder(double a, double b) {
+  const bool na = std::isnan(a), nb = std::isnan(b);
+  if (na || nb) return (int)na - (int)nb;
+  return a > b ? -1 : a < b ? 1 : 0;
+}
+struct Cand { double score, lp; int beam, rank; int32_t token; };
+// the pool: the best B by h, ties won by the earlier insertion
+struct Pool {
+  int B;
+  std::vector<std::pair<BeamHypothesis, int64_t>> items;
+  int64_t n_ins = 0;
+  static bool Worse(const std::pair<BeamHypothesis, int64_t>& a, const std::pair<BeamHypothesis, int64_t>& b) {
+    const int c = ScoreOrder(a.first.NormalizedScore, b.first.NormalizedScore);
+    return c ? c > 0 : a.second > b.second;
+  }
+  size_t WorstIndex() const {
+    size_t w = 0;
+    for (size_t j = 1; j < items.size(); j++)
+      if (Worse(items[j], items[w])) w = j;
+    return w;
+  }
+  void Add(BeamHypothesis h) {
+    const int64_t ins = n_ins++;
+    if ((int)items.size() < B) { items.emplace_back(std::move(h), ins); return; }
+    const size_t w = WorstIndex();
+    if (ScoreOrder(h.NormalizedScore, items[w].first.NormalizedScore) < 0) items[w] = {std::move(h), ins};
+  }
+  std::vector<BeamHypothesis> Result() const {
+    auto v = items;
+    std::sort(v.begin(), v.end(), [](const auto& a, const auto& b) { return Worse(b, a); });
+    std::vector<BeamHypothesis> out;
+    for (auto& e : v) out.push_back(e.first);
+    return out;
+  }
+};
+}  // namespace beam_detail
+
+// The prompt is prefilled on sequence 0 and forked to the other beams (CopySequences); every step is one ForwardBatch of the B
+// beams, whose logprob records (top 2B) give the candidates, then one CopySequences moves each surviving beam's parent rows.
+// Returns the NumReturn best hypotheses, best first.  Beam search ranks the raw distribution deterministically: sampling,
+// penalties or speculation are an error.
+inline std::vector<BeamHypothesis> GenerateBeams(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength,
+                                                 int accMode, const std::vector<int32_t>& promptTokens, const BeamSearchArgs& beams,
+                                                 const model::SamplingArgs* sampling = nullptr, const model::PenaltyArgs* penalties = nullptr,
+                                                 const model::SpeculativeArgs* speculative = nullptr) {
+  using beam_detail::Cand;
+  if ((sampling && sampling->Samples()) || penalties || speculative)
+    throw Error("beam search ranks the raw distribution deterministically: it takes no sampling, penalties or speculative decoding");
+  const int B = beams.NumBeams;
+  if (B < 1 || B > 8) throw Error("NumBeams " + std::to_string(B) + " must be in [1, 8]");
+  if (!std::isfinite(beams.LengthPenalty)) throw Error("LengthPenalty must be finite");
+  if (beams.NumReturn < 1 || beams.NumReturn > B) throw Error("NumReturn must be in [1, NumBeams]");
+  const int L = (int)promptTokens.size();
+  model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, L), B);
+  const int seqLen = infContext.SequenceLength;
+  if (L < 1 || L >= seqLen)
+    throw Error("context SequenceLength " + std::to_string(seqLen) + " must be higher than prompt tokens length " + std::to_string(L));
+  for (int b = 0; b < B; b++) infContext.SetLogprobs(b, 2 * B);
+  const double alpha = beams.LengthPenalty;
+  auto norm = [&](double s, size_t n) { return s / std::pow((double)n, alpha); };
+  auto is_stop = [&](int32_t t) { return std::find(vocab.StopTokenIds.begin(), vocab.StopTokenIds.end(), t) != vocab.StopTokenIds.end(); };
+  beam_detail::Pool pool{B, {}, 0};
+  struct Live { std::vector<int32_t> g; double s; std::vector<double> lps; };
+  std::vector<Live> live{{{}, 0.0, {}}};
+  for (int k = 0; k < seqLen - L; k++) {
+    if (k == 0) {
+      infContext.ForwardArgmax(promptTokens, 0);
+    } else {
+      std::vector<int32_t> toks, pos((size_t)live.size(), L + k - 1);
+      for (const Live& b : live) toks.push_back(b.g.back());
+      infContext.ForwardBatch(toks, pos);
+    }
+    std::vector<Cand> cands;
+    for (size_t b = 0; b < live.size(); b++) {
+      const lnb_logprob r = infContext.ReadLogprobs((int)b, L + k, 1)[0];
+      for (int j = 0; j < r.n_top; j++) cands.push_back({live[b].s + r.top_logprob[j], r.top_logprob[j], (int)b, j, r.top_token[j]});
+    }
+    std::sort(cands.begin(), cands.end(), [](const Cand& a, const Cand& b) {
+      const int c = beam_detail::ScoreOrder(a.score, b.score);
+      if (c) return c < 0;
+      return a.beam != b.beam ? a.beam < b.beam : a.rank < b.rank;
+    });
+    std::vector<Cand> next;
+    for (size_t i = 0; i < cands.size() && (int)next.size() < B; i++) {
+      const Cand& c = cands[i];
+      if (!is_stop(c.token)) { next.push_back(c); continue; }
+      if ((int)i >= B) continue;
+      BeamHypothesis h{live[(size_t)c.beam].g, c.score, 0.0, live[(size_t)c.beam].lps, GSFinishedByReachingEOS};
+      h.Tokens.push_back(c.token);
+      h.Logprobs.push_back(c.lp);
+      h.NormalizedScore = norm(c.score, h.Tokens.size());
+      pool.Add(std::move(h));
+    }
+    if ((int)next.size() < B) break;   // fewer than B new beams: the search ends with the pool it has
+    std::vector<Live> nl;
+    std::vector<int32_t> parent;
+    for (const Cand& c : next) {
+      Live b = live[(size_t)c.beam];
+      b.g.push_back(c.token);
+      b.lps.push_back(c.lp);
+      b.s = c.score;
+      nl.push_back(std::move(b));
+      parent.push_back(c.beam);
+    }
+    live = std::move(nl);
+    if (L + k == seqLen - 1) {   // the new tokens sit at the last position: every live beam finishes, in beam order
+      for (const Live& b : live) pool.Add(BeamHypothesis{b.g, b.s, norm(b.s, b.g.size()), b.lps, GSFinishedByReachingSeqLen});
+      break;
+    }
+    if ((int)pool.items.size() == B) {
+      double best = norm(live[0].s, live[0].g.size());
+      for (const Live& b : live)
+        if (beam_detail::ScoreOrder(norm(b.s, b.g.size()), best) < 0) best = norm(b.s, b.g.size());
+      if (beams.EarlyStopping || beam_detail::ScoreOrder(best, pool.items[pool.WorstIndex()].first.NormalizedScore) >= 0) break;
+    }
+    std::vector<int32_t> src, dst;
+    for (int i = 0; i < B; i++)
+      if (parent[(size_t)i] != i) { src.push_back(parent[(size_t)i]); dst.push_back(i); }
+    if (!src.empty()) infContext.CopySequences(src, dst, k == 0 ? 0 : L, L + k);   // the prompt after the prefill, later the generated rows
+  }
+  std::vector<BeamHypothesis> out = pool.Result();
+  if ((int)out.size() > beams.NumReturn) out.resize((size_t)beams.NumReturn);
+  return out;
 }
 }  // namespace inference
 }  // namespace lnb_host

@@ -384,6 +384,18 @@ int lnb_session_logprobs_read(lnb_session* s, int seq, int pos0, int n, lnb_logp
  * active sequence has logprobs off.  Afterwards a lnb_forward_device handle is stale. */
 int lnb_score(lnb_session* s, const int32_t* tokens, int n, int start_pos);
 
+/* EXTENSION: fork and permute sequences on the device (csrc/seqcopy.cuh, DESIGN.md §9f), e.g. for beam search.  For every
+ * i < n, positions [pos0, pos1) of sequence dst[i] get what sequence src[i] held there BEFORE the call: K and V of every
+ * layer, the penalty history (if allocated) and the logprob records (if allocated; record p is the token at position p).
+ * The sources are read as a snapshot, so swaps, cycles and one source copied to many destinations are legal in one call;
+ * a pair with src == dst is a no-op.  ONE stream-ordered launch (counted by lnb_session_launch_count), no host
+ * synchronisation.  The active sequence, a lnb_forward_device logits handle and a captured decode graph stay valid.
+ * Sampler and penalty parameters belong to the slot and are not copied: to fork a penalized sequence, enable penalties on
+ * the destination first (enabling clears its history).  LNB_EINVAL with nothing enqueued: n outside [1, n_seq], dst[]
+ * repeated or outside [0, n_seq), src[] outside [0, n_seq), not 0 <= pos0 < pos1 <= seq_len, more than 128 layers,
+ * tp_size > 1 (not built). */
+int lnb_session_copy_sequences(lnb_session* s, int n, const int32_t* src, const int32_t* dst, int pos0, int pos1);
+
 /* Fused collective for tensor-parallel decode: instead of ncclAllReduce after Wo / w2, every rank's GEMV
  * epilogue stores its fp32 partials straight into all peers' memory over NVLink and a small kernel
  * reduces the N slots in rank order (bit-identical on every rank).  Setup: every rank exports the 64-byte

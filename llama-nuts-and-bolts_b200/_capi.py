@@ -94,6 +94,7 @@ SIGNATURES = {
     "lnb_session_set_penalties": (C.c_int, [vp, C.c_int, C.POINTER(PenaltiesC)]),
     "lnb_session_logprobs_read": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp]),
     "lnb_score": (C.c_int, [vp, i32p, C.c_int, C.c_int]),
+    "lnb_session_copy_sequences": (C.c_int, [vp, C.c_int, i32p, i32p, C.c_int, C.c_int]),
     "lnb_session_read": (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int64]),
     "lnb_session_set_layer_limit": (C.c_int, [vp, C.c_int]),
     "lnb_session_launch_count": (C.c_int64, [vp]),

@@ -27,6 +27,7 @@
 #include "sample.cuh"
 #include "logprob.cuh"
 #include "penalty.cuh"
+#include "seqcopy.cuh"
 #include "pth.hpp"
 #include "tokenizer.hpp"
 
@@ -2819,6 +2820,57 @@ extern "C" int lnb_score(lnb_session* s, const int32_t* tokens, int n, int start
   memcpy(h_tgt, tokens + 1, (size_t)(n - 1) * 4);
   CU(cudaMemcpyAsync(s->d_lp_tgt, h_tgt, (size_t)(n - 1) * 4, cudaMemcpyHostToDevice, s->stream));
   return forward_locked(s, tokens, n - 1, start_pos, true, true, nullptr, nullptr, nullptr, true);
+}
+
+// ---- fork / permute sequences (seqcopy.cuh, DESIGN.md §9f) -------------------------------------------------------------
+// ONE stream-ordered launch: positions [pos0, pos1) of sequence dst[i] get what sequence src[i] held there before the call,
+// in K and V of every layer, the penalty history and the logprob records (the last two when allocated).  Sampler and
+// penalty parameters stay with their slot; the active sequence, a logits handle and a captured decode graph are untouched.
+extern "C" int lnb_session_copy_sequences(lnb_session* s, int n, const int32_t* src, const int32_t* dst, int pos0, int pos1) {
+  if (!s || !src || !dst) return fail(LNB_EINVAL, "NULL argument");
+  lnb_model* m = s->m;
+  if (m->tp_size > 1) return fail(LNB_EINVAL, "copying sequences is not built for tensor parallelism (tp_size %d)", m->tp_size);
+  if (n < 1 || n > s->n_seq) return fail(LNB_EINVAL, "n %d must be in [1, n_seq = %d]", n, s->n_seq);
+  for (int i = 0; i < n; i++) {
+    if (src[i] < 0 || src[i] >= s->n_seq) return fail(LNB_EINVAL, "src[%d] = %d outside [0, %d)", i, src[i], s->n_seq);
+    if (dst[i] < 0 || dst[i] >= s->n_seq) return fail(LNB_EINVAL, "dst[%d] = %d outside [0, %d)", i, dst[i], s->n_seq);
+    for (int j = 0; j < i; j++)
+      if (dst[j] == dst[i]) return fail(LNB_EINVAL, "dst[%d] = %d repeats dst[%d]", i, dst[i], j);
+  }
+  if (pos0 < 0 || pos0 >= pos1 || pos1 > s->seq_len)
+    return fail(LNB_EINVAL, "positions [%d, %d) must satisfy 0 <= pos0 < pos1 <= seq_len = %d", pos0, pos1, s->seq_len);
+  const int L = m->a.n_layers;
+  if (L > SC_MAX_LAYERS) return fail(LNB_EINVAL, "copying sequences serves up to %d layers (this model has %d)", SC_MAX_LAYERS, L);
+  static_assert(sizeof(LpRecord) % 16 == 0, "records move as 16-byte vectors");
+  // cache rows move as 16-byte vectors too: kv_l * 2 bytes must be a multiple of 16 (model creation makes kv_l a multiple of 32)
+  if ((m->kv_l * 2) % 16) return fail(LNB_EINVAL, "cache rows of %d bytes are not a multiple of 16", m->kv_l * 2);
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(m->device));
+  const long long row16 = (long long)m->kv_l * 2 / 16, rec16 = (long long)sizeof(LpRecord) / 16, np = pos1 - pos0;
+  SeqCopyJob J{};
+  J.n = n;
+  for (int i = 0; i < n; i++) { J.src[i] = src[i]; J.dst[i] = dst[i]; }
+  J.n_kv = 2 * L;
+  J.kv_stride = (long long)s->seq_len * row16; J.kv_len = np * row16;
+  J.kv_tiles = (J.kv_len + SC_TILE - 1) / SC_TILE;
+  for (int l = 0; l < L; l++) {
+    J.kv[l] = reinterpret_cast<uint4*>(s->ck[l]) + pos0 * row16;
+    J.kv[L + l] = reinterpret_cast<uint4*>(s->cv[l]) + pos0 * row16;
+  }
+  if (s->d_lp_rec) {
+    J.rec = reinterpret_cast<uint4*>(s->d_lp_rec + pos0);
+    J.rec_stride = (long long)(s->seq_len + 1) * rec16; J.rec_len = np * rec16;
+    J.rec_tiles = (J.rec_len + SC_TILE - 1) / SC_TILE;
+  }
+  long long hist_tiles = 0;
+  if (s->d_hist) {
+    J.hist = s->d_hist + pos0;
+    J.hist_stride = s->seq_len; J.hist_len = np;
+    hist_tiles = (J.hist_len + SC_TILE - 1) / SC_TILE;
+  }
+  const long long grid = (long long)J.n_kv * J.kv_tiles + J.rec_tiles + hist_tiles;
+  if (grid > 0x7fffffffLL) return fail(LNB_EINVAL, "%lld tiles exceed one grid", grid);
+  return launch_kernel(Launcher{s->stream, LAUNCH_PDL, &s->launches}, seqcopy_kernel, dim3((unsigned)grid), dim3(SC_THREADS), 0, J);
 }
 
 // One decode step for n independent sequences (rows 0..n-1 = sequences 0..n-1): tokens[i] is fed at

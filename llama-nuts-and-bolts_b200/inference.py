@@ -6,6 +6,7 @@ the Go original; each iteration is one call through the C-ABI.
 from __future__ import annotations
 
 import collections
+import math
 import time
 from dataclasses import dataclass
 
@@ -26,6 +27,85 @@ class SpeculativeArgs:
     MaxDraft: int
     NgramMax: int = 3
     NgramMin: int = 1
+
+
+@dataclass
+class BeamSearchArgs:
+    """EXTENSION: beam search (DESIGN.md §9f).  NumBeams B in [1, 8] hypotheses advance together, one lnb_forward_batch
+    per step; a hypothesis of raw score s (the f64 sum of its tokens' logprobs) and n generated tokens ranks by
+    h = s / n ** LengthPenalty.  EarlyStopping ends the search as soon as B hypotheses have finished; otherwise it ends when
+    no live beam can beat the worst finished one.  GenerateBeams returns the NumReturn (1 .. B) best."""
+    NumBeams: int
+    LengthPenalty: float = 1.0
+    EarlyStopping: bool = False
+    NumReturn: int = 1
+
+
+@dataclass
+class BeamHypothesis:
+    """one result of GenerateBeams: the generated tokens, their raw score s, h = s / len(Tokens) ** LengthPenalty, each
+    token's logprob, and the state that ended it (GSFinishedByReachingEOS or GSFinishedByReachingSeqLen)"""
+    Tokens: list
+    Score: float
+    NormalizedScore: float
+    Logprobs: list
+    State: int
+
+
+def beam_order(x: float) -> tuple:
+    """sort key of a score, best first: descending, -inf after every finite score, NaN last"""
+    return (1, 0.0) if math.isnan(x) else (0, -x)
+
+
+def beam_normalized(s: float, n: int, alpha: float) -> float:
+    """h = s / n ** alpha (libm pow)"""
+    return s / math.pow(float(n), alpha)
+
+
+def beam_select(cands, B: int, stop) -> tuple[list, list]:
+    """The selection of one beam step.  cands: (score, beam, rank, token).  Sorted by score (beam_order), then beam, then
+    rank; walking the list with index i, a stop token goes to `finished` when i < B (skipped otherwise), any other token
+    becomes the next new beam until B exist.  Returns (new beams, finished), each a list of candidates in walk order."""
+    order = sorted(cands, key=lambda c: (beam_order(c[0]), c[1], c[2]))
+    new, finished = [], []
+    for i, c in enumerate(order):
+        if len(new) == B:
+            break
+        if c[3] in stop:
+            if i < B:
+                finished.append(c)
+        else:
+            new.append(c)
+    return new, finished
+
+
+class BeamPool:
+    """the finished hypotheses: the best B by h, ties won by the earlier insertion"""
+
+    def __init__(self, B: int):
+        self.B, self.items, self.n_ins = B, [], 0
+
+    def _worst(self) -> int:
+        return max(range(len(self.items)), key=lambda j: (beam_order(self.items[j][0].NormalizedScore), self.items[j][1]))
+
+    def add(self, hyp: BeamHypothesis):
+        entry = (hyp, self.n_ins)
+        self.n_ins += 1
+        if len(self.items) < self.B:
+            self.items.append(entry)
+            return
+        w = self._worst()
+        if beam_order(hyp.NormalizedScore) < beam_order(self.items[w][0].NormalizedScore):
+            self.items[w] = entry
+
+    def full(self) -> bool:
+        return len(self.items) == self.B
+
+    def worst_h(self) -> float:
+        return self.items[self._worst()][0].NormalizedScore
+
+    def result(self) -> list:
+        return [h for h, _ in sorted(self.items, key=lambda e: (beam_order(e[0].NormalizedScore), e[1]))]
 
 
 # Rows of one speculative call (the batch engine serves at most 8 rows per launch).
@@ -266,6 +346,85 @@ class InferenceEngine:
                     break
         finally:
             infContext.close()
+
+    def GenerateBeams(self, promptTokens, beams: BeamSearchArgs, step_times: list | None = None,
+                      sampling: "SamplingArgs | None" = None, penalties: "PenaltyArgs | None" = None,
+                      speculative: "SpeculativeArgs | None" = None) -> list:
+        """EXTENSION: beam search (DESIGN.md §9f) over a session of NumBeams sequences.  The prompt is prefilled once on
+        sequence 0 and forked to the other beams (lnb_session_copy_sequences); each step is one lnb_forward_batch, whose
+        logprob records give every beam's top 2B candidates, and one copy moves each surviving beam's parent rows.  Returns
+        the NumReturn best BeamHypothesis, best first.  Beam search is deterministic on the raw distribution: it takes no
+        sampling, penalties or speculation.  step_times gets the time of the prefill and of every step."""
+        if _sampling_for(sampling, 0) is not None or penalties is not None or speculative is not None:
+            raise ml.MlError("beam search ranks the raw distribution deterministically: it takes no sampling, penalties or "
+                             "speculative decoding")
+        B = int(beams.NumBeams)
+        if not 1 <= B <= 8:
+            raise ml.MlError(f"NumBeams {B} must be in [1, 8]")
+        if not math.isfinite(beams.LengthPenalty):
+            raise ml.MlError(f"LengthPenalty {beams.LengthPenalty} must be finite")
+        if not 1 <= beams.NumReturn <= B:
+            raise ml.MlError(f"NumReturn {beams.NumReturn} must be in [1, NumBeams = {B}]")
+        prompt = [int(t) for t in promptTokens]
+        infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
+                                                max_rows=max(self.max_rows, B), acc_mode=self.acc_mode, n_seq=B)
+        if self.context_hook is not None:
+            self.context_hook(infContext)
+        try:
+            if len(prompt) >= infContext.SequenceLength:  # :176-179
+                raise ml.MlError(f"context SequenceLength {infContext.SequenceLength} must be higher than prompt "
+                                 f"tokens length {len(prompt)}")
+            if len(prompt) < 1 or len(prompt) > infContext.max_rows:
+                raise ml.MlError(f"prompt length {len(prompt)} must be in [1, {infContext.max_rows}]")
+            return self._generate_beams(infContext, prompt, beams, step_times)[:beams.NumReturn]
+        finally:
+            infContext.close()
+
+    def _generate_beams(self, infContext, prompt, beams: BeamSearchArgs, step_times: list | None = None) -> list:
+        """the search of GenerateBeams on a given context (anything with SequenceLength, set_logprobs, read_logprobs,
+        forward_batch and copy_sequences, whose sequence 0 the Transformer's forward_argmax prefills); returns the whole
+        pool, best first"""
+        B, alpha = int(beams.NumBeams), float(beams.LengthPenalty)
+        seqLen, L = infContext.SequenceLength, len(prompt)
+        stop = self.model.Vocabulary.StopTokenIds
+        for b in range(B):
+            infContext.set_logprobs(b, 2 * B)
+        pool = BeamPool(B)
+        # live beams: (tokens, raw score, logprobs)
+        live = [([], 0.0, [])]
+        for k in range(seqLen - L):
+            t0 = time.perf_counter()
+            if k == 0:
+                self.model.Transformer.forward_argmax(infContext, np.asarray(prompt, np.int32), 0)
+            else:
+                infContext.forward_batch([g[-1] for g, _, _ in live], [L + k - 1] * len(live))
+            if step_times is not None:
+                step_times.append(time.perf_counter() - t0)
+            cands = []
+            for b, (_, sb, _) in enumerate(live):
+                rec = infContext.read_logprobs(b, L + k, 1)[0]
+                for j, (tok, lp) in enumerate(rec.Top):
+                    cands.append((sb + lp, b, j, tok, lp))
+            new, finished = beam_select(cands, B, stop)
+            for sc, b, _, tok, lp in finished:
+                g, _, lps = live[b]
+                pool.add(BeamHypothesis(g + [tok], sc, beam_normalized(sc, len(g) + 1, alpha), lps + [lp], GSFinishedByReachingEOS))
+            if len(new) < B:      # the search ends with the pool it has
+                break
+            parents = [c[1] for c in new]
+            live = [(live[b][0] + [tok], sc, live[b][2] + [lp]) for sc, b, _, tok, lp in new]
+            if L + k == seqLen - 1:   # the new tokens sit at the last position: every live beam finishes
+                for g, sb, lps in live:
+                    pool.add(BeamHypothesis(g, sb, beam_normalized(sb, len(g), alpha), lps, GSFinishedByReachingSeqLen))
+                break
+            if pool.full():
+                best = min(beam_order(beam_normalized(sb, len(g), alpha)) for g, sb, _ in live)
+                if beams.EarlyStopping or best >= beam_order(pool.worst_h()):
+                    break
+            moved = [i for i in range(B) if parents[i] != i]
+            if moved:   # each new beam takes its parent's rows: the prompt after the prefill, the generated rows later
+                infContext.copy_sequences([parents[i] for i in moved], moved, 0 if k == 0 else L, L + k)
+        return pool.result()
 
     def _generate_speculative(self, infContext, hists, live, speculative: "SpeculativeArgs", step_times: list | None = None,
                               spec_stats: list | None = None, lp_out: list | None = None):

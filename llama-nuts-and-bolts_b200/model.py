@@ -342,6 +342,17 @@ class InferenceContext:
         check(lib.lnb_session_logprobs_read(self.h, seq, pos0, n, recs))
         return _token_logprobs(recs)
 
+    def copy_sequences(self, src, dst, pos0: int, pos1: int):
+        """EXTENSION (lnb_session_copy_sequences): positions [pos0, pos1) of sequence dst[i] get what sequence src[i] held
+        there before the call -- K and V of every layer, the penalty history and the logprob records.  The sources are read
+        as a snapshot (swaps, cycles and forks are legal in one call); one launch, stream-ordered."""
+        src = np.ascontiguousarray(src, np.int32).reshape(-1)
+        dst = np.ascontiguousarray(dst, np.int32).reshape(-1)
+        if src.shape != dst.shape:
+            raise ml.MlError(f"{src.shape[0]} sources for {dst.shape[0]} destinations")
+        check(lib.lnb_session_copy_sequences(self.h, int(src.shape[0]), ptr(src, _capi.i32p), ptr(dst, _capi.i32p), int(pos0),
+                                             int(pos1)))
+
     def allow_chunked_prefill(self, on: bool = True):
         """EXTENSION (not in the reference): accept S > 1 at startPos > 0 with the [S,T] causal mask"""
         check(lib.lnb_session_set_chunked_prefill(self.h, int(on)))

@@ -209,3 +209,284 @@ int orc_generate_processed(const orc_model* m, int vocab, const int32_t* prompt,
   orc_session_free(s);
   return n_out;
 }
+
+/* ---- beam search (DESIGN.md §9f), written from the contract: the selection, the pool and the end rules in plain C ------ */
+#include <math.h>
+
+typedef struct {
+  double score;
+  int32_t beam, rank, token;
+  double lp;
+} orc_beam_cand;
+
+/* score descending, -inf after every finite score, NaN last; then beam ascending; then rank ascending */
+static int beam_score_cmp(double a, double b) {
+  const int na = isnan(a), nb = isnan(b);
+  if (na || nb) return na - nb;
+  return a > b ? -1 : a < b ? 1 : 0;
+}
+static int beam_cand_cmp(const void* pa, const void* pb) {
+  const orc_beam_cand *a = (const orc_beam_cand*)pa, *b = (const orc_beam_cand*)pb;
+  const int c = beam_score_cmp(a->score, b->score);
+  if (c) return c;
+  if (a->beam != b->beam) return a->beam < b->beam ? -1 : 1;
+  return a->rank < b->rank ? -1 : a->rank > b->rank ? 1 : 0;
+}
+static int beam_is_stop(int32_t t, const int32_t* stop, int n_stop) {
+  for (int i = 0; i < n_stop; i++)
+    if (stop[i] == t) return 1;
+  return 0;
+}
+/* sorts c[n] in place; new_idx[*n_new] / fin_idx[*n_fin]: positions in the sorted list of the new beams and the finished */
+static void beam_select(orc_beam_cand* c, int n, int B, const int32_t* stop, int n_stop, int32_t* new_idx, int* n_new,
+                        int32_t* fin_idx, int* n_fin) {
+  qsort(c, (size_t)n, sizeof(orc_beam_cand), beam_cand_cmp);
+  *n_new = *n_fin = 0;
+  for (int i = 0; i < n && *n_new < B; i++) {
+    if (beam_is_stop(c[i].token, stop, n_stop)) {
+      if (i < B) fin_idx[(*n_fin)++] = i;
+    } else {
+      new_idx[(*n_new)++] = i;
+    }
+  }
+}
+/* the selection alone on a candidate table (for the tests): the sorted table back in score/beam/rank/token, and the indices */
+void orc_beam_select(double* score, int32_t* beam, int32_t* rank, int32_t* token, int n, int B, const int32_t* stop, int n_stop,
+                     int32_t* new_idx, int32_t* n_new, int32_t* fin_idx, int32_t* n_fin) {
+  orc_beam_cand* c = (orc_beam_cand*)malloc((size_t)(n > 0 ? n : 1) * sizeof(orc_beam_cand));
+  for (int i = 0; i < n; i++) { c[i].score = score[i]; c[i].beam = beam[i]; c[i].rank = rank[i]; c[i].token = token[i]; c[i].lp = 0; }
+  int nn, nf;
+  beam_select(c, n, B, stop, n_stop, new_idx, &nn, fin_idx, &nf);
+  for (int i = 0; i < n; i++) { score[i] = c[i].score; beam[i] = c[i].beam; rank[i] = c[i].rank; token[i] = c[i].token; }
+  *n_new = nn;
+  *n_fin = nf;
+  free(c);
+}
+
+typedef struct {
+  int32_t* tok;   /* [seq_len] */
+  double* lp;     /* [seq_len] */
+  int len;
+  double s, h;
+  int state;      /* 1: EOS, 2: SeqLen */
+  int64_t ins;
+} orc_beam_hyp;
+
+/* a worse than b in the pool: lower h (NaN lowest), on equal h the later insertion */
+static int beam_hyp_worse(const orc_beam_hyp* a, const orc_beam_hyp* b) {
+  const int c = beam_score_cmp(a->h, b->h);
+  if (c) return c > 0;
+  return a->ins > b->ins;
+}
+typedef struct {
+  int B, n, seq_len;
+  int64_t n_ins;
+  orc_beam_hyp* e;
+} orc_beam_pool;
+static int beam_pool_worst(const orc_beam_pool* p) {
+  int w = 0;
+  for (int j = 1; j < p->n; j++)
+    if (beam_hyp_worse(&p->e[j], &p->e[w])) w = j;
+  return w;
+}
+static void beam_pool_add(orc_beam_pool* p, const int32_t* tok, const double* lp, int len, double s, double h, int state) {
+  orc_beam_hyp* slot;
+  const int64_t ins = p->n_ins++;
+  if (p->n < p->B) {
+    slot = &p->e[p->n++];
+  } else {
+    const int w = beam_pool_worst(p);
+    if (beam_score_cmp(h, p->e[w].h) >= 0) return;   /* not strictly better: the earlier insertion keeps its place */
+    slot = &p->e[w];
+  }
+  memcpy(slot->tok, tok, (size_t)len * 4);
+  memcpy(slot->lp, lp, (size_t)len * 8);
+  slot->len = len; slot->s = s; slot->h = h; slot->state = state; slot->ins = ins;
+}
+/* the pool rule alone (for the tests): hypotheses with normalised scores h[n] inserted in order into a pool of B; kept[]
+ * gets the indices the pool ends with, best first (ties: insertion order); returns how many, -1 for B outside [1, 8] */
+int orc_beam_pool_run(const double* h, int n, int B, int32_t* kept) {
+  if (B < 1 || B > 8) return -1;
+  orc_beam_pool p = {B, 0, 1, 0, (orc_beam_hyp*)calloc((size_t)B, sizeof(orc_beam_hyp))};
+  int32_t dummy_t = 0;
+  double dummy_l = 0;
+  for (int j = 0; j < B; j++) { p.e[j].tok = (int32_t*)malloc(4); p.e[j].lp = (double*)malloc(8); }
+  for (int i = 0; i < n; i++) beam_pool_add(&p, &dummy_t, &dummy_l, 0, 0.0, h[i], 1);
+  int m = 0;
+  for (int used[8] = {0}; m < p.n; m++) {   /* selection sort: best first */
+    int b = -1;
+    for (int j = 0; j < p.n; j++)
+      if (!used[j] && (b < 0 || beam_hyp_worse(&p.e[b], &p.e[j]))) b = j;
+    used[b] = 1;
+    kept[m] = (int32_t)p.e[b].ins;
+  }
+  for (int j = 0; j < B; j++) { free(p.e[j].tok); free(p.e[j].lp); }
+  free(p.e);
+  return m;
+}
+
+/* what the search reads and moves: the model side (an oracle model below, a table in the tests) */
+typedef struct {
+  void* ctx;
+  /* step k: the rows after the prompt (k == 0, beam 0 only, n == 1) or after beam b was fed last[b] at position L + k - 1;
+   * writes beam b's top tokens and logprobs to top_tok[b * 20 ..], top_lp[b * 20 ..], their count to n_top[b] */
+  int (*step)(void* ctx, int k, int n, const int32_t* last, int32_t* top_tok, double* top_lp, int32_t* n_top);
+  /* beams dst[i] take rows [pos0, pos1) of beam src[i], read as a snapshot */
+  int (*reorder)(void* ctx, int n, const int32_t* src, const int32_t* dst, int pos0, int pos1);
+} orc_beam_io;
+
+/* The search of DESIGN.md §9f.  Results (best first) to out_tok[h * seq_len ..], out_lp[h * seq_len ..], out_len[h],
+ * out_s[h], out_h[h], out_state[h] (1 EOS, 2 SeqLen); moves[] (or NULL) counts the copies whose parent differs from the
+ * beam; returns the number of hypotheses, -1 on an error of io */
+int orc_beam_search_io(const orc_beam_io* io, int n_prompt, int seq_len, const int32_t* stop, int n_stop, int B, double alpha,
+                       int early, int32_t* out_tok, double* out_lp, int32_t* out_len, double* out_s, double* out_h, int32_t* out_state) {
+  if (B < 1 || B > 8 || n_prompt < 1 || n_prompt >= seq_len) return -1;
+  const int L = n_prompt, TOPW = 20;
+  orc_beam_pool pool = {B, 0, seq_len, 0, (orc_beam_hyp*)calloc((size_t)B, sizeof(orc_beam_hyp))};
+  for (int j = 0; j < B; j++) { pool.e[j].tok = (int32_t*)malloc((size_t)seq_len * 4); pool.e[j].lp = (double*)malloc((size_t)seq_len * 8); }
+  /* live beams, and the next step's beams */
+  int32_t *tok = (int32_t*)malloc((size_t)B * seq_len * 4), *tok2 = (int32_t*)malloc((size_t)B * seq_len * 4);
+  double *lp = (double*)malloc((size_t)B * seq_len * 8), *lp2 = (double*)malloc((size_t)B * seq_len * 8);
+  double s[8], s2[8];
+  int n_live = 1, len = 0, rc = 0;
+  s[0] = 0.0;
+  int32_t top_tok[8 * 20], n_top[8], last[8], parent[8], new_idx[8 * 20], fin_idx[8 * 20];
+  double top_lp[8 * 20];
+  orc_beam_cand* c = (orc_beam_cand*)malloc((size_t)8 * TOPW * sizeof(orc_beam_cand));
+  for (int k = 0; k < seq_len - L; k++) {
+    for (int b = 0; b < n_live; b++) last[b] = len ? tok[b * seq_len + len - 1] : -1;
+    if (io->step(io->ctx, k, n_live, last, top_tok, top_lp, n_top)) { rc = -1; break; }
+    int nc = 0;
+    for (int b = 0; b < n_live; b++)
+      for (int j = 0; j < n_top[b]; j++) {
+        c[nc].score = s[b] + top_lp[b * TOPW + j];
+        c[nc].beam = b; c[nc].rank = j; c[nc].token = top_tok[b * TOPW + j]; c[nc].lp = top_lp[b * TOPW + j];
+        nc++;
+      }
+    int nn, nf;
+    beam_select(c, nc, B, stop, n_stop, new_idx, &nn, fin_idx, &nf);
+    for (int f = 0; f < nf; f++) {   /* finished: the parent's tokens and this one */
+      const orc_beam_cand* x = &c[fin_idx[f]];
+      int32_t* t = tok + (size_t)x->beam * seq_len;
+      double* l = lp + (size_t)x->beam * seq_len;
+      const int32_t keep_t = t[len];
+      const double keep_l = l[len];
+      t[len] = x->token; l[len] = x->lp;
+      beam_pool_add(&pool, t, l, len + 1, x->score, x->score / pow((double)(len + 1), alpha), 1);
+      t[len] = keep_t; l[len] = keep_l;
+    }
+    if (nn < B) break;   /* fewer than B new beams: the search ends with the pool it has */
+    for (int i = 0; i < B; i++) {
+      const orc_beam_cand* x = &c[new_idx[i]];
+      parent[i] = x->beam;
+      memcpy(tok2 + (size_t)i * seq_len, tok + (size_t)x->beam * seq_len, (size_t)len * 4);
+      memcpy(lp2 + (size_t)i * seq_len, lp + (size_t)x->beam * seq_len, (size_t)len * 8);
+      tok2[(size_t)i * seq_len + len] = x->token;
+      lp2[(size_t)i * seq_len + len] = x->lp;
+      s2[i] = x->score;
+    }
+    { int32_t* t = tok; tok = tok2; tok2 = t; double* l = lp; lp = lp2; lp2 = l; }
+    memcpy(s, s2, sizeof(s));
+    n_live = B;
+    len++;
+    if (L + k == seq_len - 1) {   /* the new tokens sit at the last position: every live beam finishes, in beam order */
+      for (int b = 0; b < B; b++)
+        beam_pool_add(&pool, tok + (size_t)b * seq_len, lp + (size_t)b * seq_len, len, s[b], s[b] / pow((double)len, alpha), 2);
+      break;
+    }
+    if (pool.n == B) {
+      double hb = s[0] / pow((double)len, alpha);   /* the best live h */
+      for (int b = 1; b < B; b++) {
+        const double h = s[b] / pow((double)len, alpha);
+        if (beam_score_cmp(h, hb) < 0) hb = h;
+      }
+      if (early || beam_score_cmp(hb, pool.e[beam_pool_worst(&pool)].h) >= 0) break;
+    }
+    int32_t src[8], dst[8];
+    int nm = 0;
+    for (int i = 0; i < B; i++)
+      if (parent[i] != i) { src[nm] = parent[i]; dst[nm] = i; nm++; }
+    if (nm && io->reorder(io->ctx, nm, src, dst, k == 0 ? 0 : L, L + k)) { rc = -1; break; }
+  }
+  int n_out = 0;
+  if (rc == 0) {
+    int used[8] = {0};
+    for (; n_out < pool.n; n_out++) {   /* best first, ties in insertion order */
+      int b = -1;
+      for (int j = 0; j < pool.n; j++)
+        if (!used[j] && (b < 0 || beam_hyp_worse(&pool.e[b], &pool.e[j]))) b = j;
+      used[b] = 1;
+      const orc_beam_hyp* x = &pool.e[b];
+      memcpy(out_tok + (size_t)n_out * seq_len, x->tok, (size_t)x->len * 4);
+      memcpy(out_lp + (size_t)n_out * seq_len, x->lp, (size_t)x->len * 8);
+      out_len[n_out] = x->len; out_s[n_out] = x->s; out_h[n_out] = x->h; out_state[n_out] = x->state;
+    }
+  }
+  for (int j = 0; j < B; j++) { free(pool.e[j].tok); free(pool.e[j].lp); }
+  free(pool.e); free(tok); free(tok2); free(lp); free(lp2); free(c);
+  return rc ? -1 : n_out;
+}
+
+/* the oracle model side: B sessions, orc_forward per beam at S = 1, orc_logprob_row(top_n = min(2B, V)) of each row;
+ * reorder by memcpy of the caches through a snapshot of every source */
+typedef struct {
+  const orc_model* m;
+  int vocab, B, seq_len, n_layers, kv_row;   /* kv_row: elements per position of one cache */
+  const int32_t* prompt;
+  int n_prompt;
+  orc_session* s[8];
+  float* logits;
+  uint16_t* snap;
+  int64_t* n_moves;
+} orc_beam_oracle;
+
+static int beam_oracle_step(void* ctx, int k, int n, const int32_t* last, int32_t* top_tok, double* top_lp, int32_t* n_top) {
+  orc_beam_oracle* o = (orc_beam_oracle*)ctx;
+  const int top_n = 2 * o->B < o->vocab ? 2 * o->B : o->vocab;
+  lnb_logprob rec;
+  for (int b = 0; b < n; b++) {
+    const int rc = k == 0 ? orc_forward(o->m, o->s[0], o->prompt, o->n_prompt, 0, o->logits, 0, NULL)
+                          : orc_forward(o->m, o->s[b], last + b, 1, o->n_prompt + k - 1, o->logits, 0, NULL);
+    if (rc != 0) return -1;
+    orc_logprob_row(o->logits, o->vocab, 0, top_n, &rec);
+    n_top[b] = rec.n_top;
+    for (int j = 0; j < rec.n_top; j++) { top_tok[b * 20 + j] = rec.top_token[j]; top_lp[b * 20 + j] = rec.top_logprob[j]; }
+  }
+  return 0;
+}
+static int beam_oracle_reorder(void* ctx, int n, const int32_t* src, const int32_t* dst, int pos0, int pos1) {
+  orc_beam_oracle* o = (orc_beam_oracle*)ctx;
+  const size_t off = (size_t)pos0 * o->kv_row, cnt = (size_t)(pos1 - pos0) * o->kv_row;
+  for (int l = 0; l < o->n_layers; l++)
+    for (int kv = 0; kv < 2; kv++) {
+      for (int i = 0; i < n; i++) {   /* snapshot of every source first ... */
+        const uint16_t* c = kv ? orc_session_cache_v(o->s[src[i]], l) : orc_session_cache_k(o->s[src[i]], l);
+        memcpy(o->snap + (size_t)i * cnt, c + off, cnt * 2);
+      }
+      for (int i = 0; i < n; i++) {   /* ... then the destinations */
+        uint16_t* c = kv ? orc_session_cache_v(o->s[dst[i]], l) : orc_session_cache_k(o->s[dst[i]], l);
+        memcpy(c + off, o->snap + (size_t)i * cnt, cnt * 2);
+      }
+    }
+  if (o->n_moves) (*o->n_moves)++;
+  return 0;
+}
+
+/* beam search on the oracle model (n_layers and kv_row = n_kv_heads * head_dim describe its caches); n_moves (or NULL)
+ * counts the reorders */
+int orc_beam_search(const orc_model* m, int vocab, int n_layers, int kv_row, const int32_t* prompt, int n_prompt, int seq_len,
+                    const int32_t* stop, int n_stop, int B, double alpha, int early, int32_t* out_tok, double* out_lp,
+                    int32_t* out_len, double* out_s, double* out_h, int32_t* out_state, int64_t* n_moves) {
+  if (B < 1 || B > 8) return -1;
+  orc_beam_oracle o = {m, vocab, B, seq_len, n_layers, kv_row, prompt, n_prompt, {0}, NULL, NULL, n_moves};
+  for (int b = 0; b < B; b++) o.s[b] = orc_session_new(m, seq_len);
+  o.logits = (float*)malloc((size_t)vocab * n_prompt * sizeof(float));
+  o.snap = (uint16_t*)malloc((size_t)B * seq_len * kv_row * 2);
+  if (n_moves) *n_moves = 0;
+  const orc_beam_io io = {&o, beam_oracle_step, beam_oracle_reorder};
+  const int n = orc_beam_search_io(&io, n_prompt, seq_len, stop, n_stop, B, alpha, early, out_tok, out_lp, out_len, out_s, out_h,
+                                   out_state);
+  for (int b = 0; b < B; b++) orc_session_free(o.s[b]);
+  free(o.logits); free(o.snap);
+  return n;
+}

@@ -162,3 +162,108 @@ def generate_processed(om, prompt, seq_len: int, T: float, K: int, P: float, see
     if n < 0:
         raise RuntimeError("orc_generate_processed failed")
     return out[:n].copy()
+
+
+# ---- beam search (DESIGN.md §9f) -----------------------------------------------------------------------------------------
+_STEP_CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.c_int, _i32p, _i32p, _f64p, _i32p)
+_REORDER_CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, _i32p, _i32p, C.c_int, C.c_int)
+
+
+class _BeamIO(C.Structure):   # orc_beam_io
+    _fields_ = [("ctx", C.c_void_p), ("step", _STEP_CB), ("reorder", _REORDER_CB)]
+
+
+def _beam_lib():
+    L = lib()
+    if not getattr(L, "_beam_bound", False):
+        L.orc_beam_select.restype = None
+        L.orc_beam_select.argtypes = [_f64p, _i32p, _i32p, _i32p, C.c_int, C.c_int, _i32p, C.c_int, _i32p, _i32p, _i32p, _i32p]
+        L.orc_beam_pool_run.restype = C.c_int
+        L.orc_beam_pool_run.argtypes = [_f64p, C.c_int, C.c_int, _i32p]
+        out = [_i32p, _f64p, _i32p, _f64p, _f64p, _i32p]
+        L.orc_beam_search_io.restype = C.c_int
+        L.orc_beam_search_io.argtypes = [C.POINTER(_BeamIO), C.c_int, C.c_int, _i32p, C.c_int, C.c_int, C.c_double, C.c_int] + out
+        L.orc_beam_search.restype = C.c_int
+        L.orc_beam_search.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_int,
+                                      C.c_double, C.c_int] + out + [_i64p]
+        L._beam_bound = True
+    return L
+
+
+def beam_select(cands, B: int, stop):
+    """orc_beam_select: cands (score, beam, rank, token) -> (new beams, finished) as lists of candidate tuples in walk order"""
+    n = len(cands)
+    sc = np.array([c[0] for c in cands], np.float64)
+    bm = np.array([c[1] for c in cands], np.int32)
+    rk = np.array([c[2] for c in cands], np.int32)
+    tk = np.array([c[3] for c in cands], np.int32)
+    st = np.ascontiguousarray(list(stop) or [-1], np.int32)
+    ni, fi = np.zeros(max(n, 1), np.int32), np.zeros(max(n, 1), np.int32)
+    nn, nf = C.c_int32(0), C.c_int32(0)
+    _beam_lib().orc_beam_select(sc.ctypes.data_as(_f64p), bm.ctypes.data_as(_i32p), rk.ctypes.data_as(_i32p), tk.ctypes.data_as(_i32p),
+                                n, B, st.ctypes.data_as(_i32p), len(list(stop)), ni.ctypes.data_as(_i32p), C.byref(nn),
+                                fi.ctypes.data_as(_i32p), C.byref(nf))
+    row = lambda i: (float(sc[i]), int(bm[i]), int(rk[i]), int(tk[i]))   # noqa: E731
+    return [row(i) for i in ni[:nn.value]], [row(i) for i in fi[:nf.value]]
+
+
+def beam_pool_run(h, B: int) -> list:
+    """orc_beam_pool_run: the insertion indices a pool of B keeps after inserting h[0..n) in order, best first"""
+    hh = np.ascontiguousarray(h, np.float64)
+    kept = np.zeros(B, np.int32)
+    m = _beam_lib().orc_beam_pool_run(hh.ctypes.data_as(_f64p), hh.shape[0], B, kept.ctypes.data_as(_i32p))
+    if m < 0:
+        raise ValueError(f"pool size {B} outside [1, 8]")
+    return [int(x) for x in kept[:m]]
+
+
+def _beam_out(n, tok, lp, ln, s, h, state):
+    return [dict(tokens=[int(t) for t in tok[i, :ln[i]]], logprobs=[float(x) for x in lp[i, :ln[i]]], s=float(s[i]), h=float(h[i]),
+                 state=int(state[i])) for i in range(n)]
+
+
+def beam_search_io(step, reorder, n_prompt: int, seq_len: int, stop, B: int, alpha: float, early: bool) -> list:
+    """orc_beam_search_io with Python callbacks: step(k, last[n]) -> per live beam a list of (token, logprob) in rank order;
+    reorder(src, dst, pos0, pos1).  Returns the hypotheses (dicts: tokens, logprobs, s, h, state), best first."""
+    def _step(ctx, k, n, last, top_tok, top_lp, n_top):
+        rows = step(k, [int(last[b]) for b in range(n)])
+        for b, r in enumerate(rows):
+            n_top[b] = len(r)
+            for j, (t, x) in enumerate(r):
+                top_tok[b * 20 + j] = int(t)
+                top_lp[b * 20 + j] = float(x)
+        return 0
+
+    def _reorder(ctx, n, src, dst, pos0, pos1):
+        reorder([int(src[i]) for i in range(n)], [int(dst[i]) for i in range(n)], int(pos0), int(pos1))
+        return 0
+
+    io = _BeamIO(None, _STEP_CB(_step), _REORDER_CB(_reorder))
+    st = np.ascontiguousarray(list(stop) or [-1], np.int32)
+    tok, lp = np.zeros((B, seq_len), np.int32), np.zeros((B, seq_len), np.float64)
+    ln, state = np.zeros(B, np.int32), np.zeros(B, np.int32)
+    s, h = np.zeros(B, np.float64), np.zeros(B, np.float64)
+    n = _beam_lib().orc_beam_search_io(C.byref(io), n_prompt, seq_len, st.ctypes.data_as(_i32p), len(list(stop)), B, alpha, int(early),
+                                       tok.ctypes.data_as(_i32p), lp.ctypes.data_as(_f64p), ln.ctypes.data_as(_i32p),
+                                       s.ctypes.data_as(_f64p), h.ctypes.data_as(_f64p), state.ctypes.data_as(_i32p))
+    if n < 0:
+        raise RuntimeError("orc_beam_search_io failed")
+    return _beam_out(n, tok, lp, ln, s, h, state)
+
+
+def beam_search(om, prompt, seq_len: int, B: int, alpha: float = 1.0, early: bool = False, stop_ids=(128008, 128009)):
+    """orc_beam_search on the oracle model (om: oracle.OracleModel): (hypotheses best first, number of reorders)"""
+    a = om.args
+    prompt = np.ascontiguousarray(prompt, np.int32)
+    st = np.ascontiguousarray(list(stop_ids) or [-1], np.int32)
+    tok, lp = np.zeros((B, seq_len), np.int32), np.zeros((B, seq_len), np.float64)
+    ln, state = np.zeros(B, np.int32), np.zeros(B, np.int32)
+    s, h = np.zeros(B, np.float64), np.zeros(B, np.float64)
+    moves = C.c_int64(0)
+    n = _beam_lib().orc_beam_search(om.h, a.vocab, a.n_layers, a.n_kv_heads * a.head_dim, prompt.ctypes.data_as(_i32p), len(prompt),
+                                    seq_len, st.ctypes.data_as(_i32p), len(list(stop_ids)), B, alpha, int(early),
+                                    tok.ctypes.data_as(_i32p), lp.ctypes.data_as(_f64p), ln.ctypes.data_as(_i32p),
+                                    s.ctypes.data_as(_f64p), h.ctypes.data_as(_f64p), state.ctypes.data_as(_i32p), C.byref(moves))
+    if n < 0:
+        raise RuntimeError("orc_beam_search failed")
+    return _beam_out(n, tok, lp, ln, s, h, state), int(moves.value)
