@@ -167,6 +167,47 @@ static void linear_bf16_ksplit(const uint16_t* x, const uint16_t* w, uint16_t* o
   free(part);
 }
 
+/* LNB_ACC_FAST order of gemv.cuh: stream j of `ks` owns the 8-element chunks g with g % ks == j and adds them sequentially
+ * in f32; the streams are combined as ((p0 + p1) + p2) + ...  ks == 1 is the reference's k = 0,1,2,... order. */
+static void linear_ks(const uint16_t* x, const uint16_t* w, float* accout, int S, int K, int N, int ks) {
+  const int nch = K / 8;
+  float* xf = (float*)malloc((size_t)S * K * sizeof(float));
+  for (size_t i = 0; i < (size_t)S * K; i++) xf[i] = bf(x[i]);
+#pragma omp parallel for collapse(2) schedule(static)
+  for (int s = 0; s < S; s++)
+    for (int n = 0; n < N; n++) {
+      const float* xr = xf + (size_t)s * K;
+      const uint16_t* wr = w + (size_t)n * K;
+      float part[ORC_MAX_KS] = {0.0f};
+      for (int g = 0; g < nch; g++) {
+        float a = part[g % ks];
+        for (int e = 0; e < 8; e++) a += xr[8 * g + e] * bf(wr[8 * g + e]); /* exact product, one rounding per add */
+        part[g % ks] = a;
+      }
+      float tot = part[0];
+      for (int j = 1; j < ks; j++) tot = tot + part[j];
+      accout[(size_t)s * N + n] = tot;
+    }
+  free(xf);
+}
+
+static void linear_order_bf16(const uint16_t* x, const uint16_t* w, uint16_t* out, int S, int K, int N, int ks) {
+  if (ks <= 1) {
+    orc_linear_bf16(x, w, out, S, K, N);
+    return;
+  }
+  float* acc = (float*)malloc((size_t)S * N * sizeof(float));
+  linear_ks(x, w, acc, S, K, N, ks);
+  for (size_t i = 0; i < (size_t)S * N; i++) out[i] = tr(acc[i]);
+  free(acc);
+}
+
+int orc_linear_order_bf16(const uint16_t* x, const uint16_t* w, uint16_t* out, int S, int K, int N, int ks) {
+  if (ks < 1 || ks > ORC_MAX_KS || (ks > 1 && K % 8)) return -1;
+  linear_order_bf16(x, w, out, S, K, N, ks);
+  return 0;
+}
+
 /* operations_lineartransform.go:72-103 (F32 flavour: same loop on float32 data) */
 void orc_linear_f32(const float* x, const float* w, float* out, int S, int K, int N) {
   for (int s = 0; s < S; s++)
@@ -278,9 +319,36 @@ static float rms_scale(const uint16_t* xr, int D, float eps) {
   return (float)(1.0 / sqrt((double)me));     /* RSqrt :300 */
 }
 
+/* LNB_ACC_FAST order of the sum of squares (gemv.cuh prologue, rmsnorm_kernel): element i goes to partial i % parts, each
+ * partial adds its elements in index order, a 5-level xor butterfly (16, 8, 4, 2, 1) runs inside each group of 32
+ * partials (one warp), then the groups are added in order.  parts == 1 is the reference's sequential sum. */
+static float rms_scale_parts(const uint16_t* xr, int D, float eps, int parts) {
+  if (parts <= 1) return rms_scale(xr, D, eps);
+  float part[ORC_MAX_RMS_PARTS], nxt[ORC_MAX_RMS_PARTS];
+  for (int i = 0; i < parts; i++) part[i] = 0.0f;
+  for (int j = 0; j < D; j++) {
+    double v = (double)bf(xr[j]);
+    part[j % parts] += (float)(v * v);
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    for (int i = 0; i < parts; i++) nxt[i] = part[i] + part[i ^ o];
+    memcpy(part, nxt, (size_t)parts * sizeof(float));
+  }
+  float sum = 0.0f;
+  for (int g = 0; g < parts; g += 32) sum += part[g];
+  float mean = sum / (float)D;
+  float me = mean + eps;
+  return (float)(1.0 / sqrt((double)me));
+}
+
 /* the scale alone (llamatransformer.go:641-656), for white-box checks of the GPU scale kernels */
 void orc_rms_scale(const uint16_t* x, float* r, int S, int D, float eps) {
   for (int s = 0; s < S; s++) r[s] = rms_scale(x + (size_t)s * D, D, eps);
+}
+int orc_rms_scale_order(const uint16_t* x, float* r, int S, int D, float eps, int parts) {
+  if (parts < 1 || parts > ORC_MAX_RMS_PARTS || (parts > 1 && parts % 32)) return -1;
+  for (int s = 0; s < S; s++) r[s] = rms_scale_parts(x + (size_t)s * D, D, eps, parts);
+  return 0;
 }
 
 void orc_rmsnorm_stage1(const uint16_t* x, uint16_t* out, int S, int D, float eps) {
@@ -291,15 +359,18 @@ void orc_rmsnorm_stage1(const uint16_t* x, uint16_t* out, int S, int D, float ep
   }
 }
 
-void orc_rmsnorm(const uint16_t* x, const uint16_t* w, uint16_t* out, int S, int D, float eps) {
+static void rmsnorm_parts(const uint16_t* x, const uint16_t* w, uint16_t* out, int S, int D, float eps, int parts) {
   for (int s = 0; s < S; s++) {
     const uint16_t* xr = x + (size_t)s * D;
-    float r = rms_scale(xr, D, eps);
+    float r = rms_scale_parts(xr, D, eps, parts);
     for (int j = 0; j < D; j++) {
       uint16_t n1 = tr(bf(xr[j]) * r);
       out[(size_t)s * D + j] = tr(bf(n1) * bf(w[j])); /* llamatransformer.go:638 */
     }
   }
+}
+void orc_rmsnorm(const uint16_t* x, const uint16_t* w, uint16_t* out, int S, int D, float eps) {
+  rmsnorm_parts(x, w, out, S, D, eps, 1);
 }
 
 /* ------------------------------------------------------------------- RoPE */
@@ -374,8 +445,36 @@ void orc_rope_apply(const uint16_t* x, const float* cis, uint16_t* out, int S, i
 /* q_pos0 = absolute position of query row 0.  The reference only ever builds the [S,S] mask for startPos 0 (T == S,
  * q_pos0 = 0: `t > s`, llamatransformer.go:128-136); q_pos0 > 0 is the chunked-prefill EXTENSION (beyond the reference):
  * the [S,T] mask a correct broadcast would need, row s sees the keys t <= q_pos0 + s. */
+/* ORC_ATTN_TREE: the softmax denominator of sdpa_kernel / sdpa_decode_kernel and of one chunk of ss_scores_kernel.  128 f64
+ * partials (key t -> partial t % 128, in t order), a 5-level xor butterfly inside each group of 32, then
+ * ((w0 + w1) + w2) + w3 over the 4 groups. */
+static double z_tree(const double* e, int n) {
+  double part[128], nxt[128];
+  for (int i = 0; i < 128; i++) part[i] = 0.0;
+  for (int t = 0; t < n; t++) part[t % 128] += e[t];
+  for (int o = 16; o > 0; o >>= 1) {
+    for (int i = 0; i < 128; i++) nxt[i] = part[i] + part[i ^ o];
+    memcpy(part, nxt, sizeof(part));
+  }
+  return ((part[0] + part[32]) + part[64]) + part[96];
+}
+
+/* Z = sum of e[0..n) in the order `attn`; ORC_ATTN_STREAM: the tree of each chunk of ORC_STREAM_CHUNK keys, the chunk
+ * sums added to 0.0 in chunk order (ss_scores_kernel, ss_out_kernel) */
+static double z_order(const double* e, int n, int attn) {
+  double z = 0.0;
+  if (attn == ORC_ATTN_TREE) return z_tree(e, n);
+  if (attn == ORC_ATTN_STREAM) {
+    for (int t0 = 0; t0 < n; t0 += ORC_STREAM_CHUNK) z += z_tree(e + t0, n - t0 < ORC_STREAM_CHUNK ? n - t0 : ORC_STREAM_CHUNK);
+    return z;
+  }
+  for (int t = 0; t < n; t++) z += e[t];
+  return z;
+}
+double orc_attention_z(const double* e, int n, int attn) { return z_order(e, n, attn); }
+
 static void attention_impl(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out, int S, int T,
-                           int n_heads, int n_kv, int hd, int causal_mask, int q_pos0) {
+                           int n_heads, int n_kv, int hd, int causal_mask, int q_pos0, int attn) {
   int n_rep = n_heads / n_kv;
   /* dtype.BFloat16fromFloat32(float32(math.Sqrt(float64(HeadDim)))) llamatransformer.go:464 */
   float scale = bf(tr((float)sqrt((double)hd)));
@@ -399,16 +498,22 @@ static void attention_impl(const uint16_t* q, const uint16_t* cacheK, const uint
         }
         sc[t] = v;
       }
-      double z = 0.0;
-      for (int t = 0; t < T; t++) {
-        e[t] = exp((double)bf(sc[t])); /* ToFloat32 -> Softmax (f64, no max-subtraction) :484-490 */
-        z += e[t];
-      }
+      for (int t = 0; t < T; t++) e[t] = exp((double)bf(sc[t])); /* ToFloat32 -> Softmax (f64, no max-subtraction) :484-490 */
+      /* the FAST orders only visit the keys the row sees (masked keys add exact zeros to either sum) */
+      const int Tv = (attn != ORC_ATTN_REF && causal_mask) ? (T < q_pos0 + s + 1 ? T : q_pos0 + s + 1) : T;
+      double z = z_order(e, Tv, attn);
       for (int t = 0; t < T; t++) sc[t] = tr((float)(e[t] / z)); /* -> f32 -> ToBFloat16 :493 */
       uint16_t* orow = out + (size_t)s * n_heads * hd + (size_t)H * hd; /* Transpose(0,1)+Reshape :508-514 */
+      const int chunk = attn == ORC_ATTN_STREAM ? ORC_STREAM_CHUNK : Tv;
       for (int d = 0; d < hd; d++) {
+        /* one f32 chain per chunk of keys, the chunk results added to 0 in chunk order (one chunk outside STREAM) */
         float acc = 0.0f;
-        for (int t = 0; t < T; t++) acc += bf(sc[t]) * bf(cacheV[((size_t)t * n_kv + h) * hd + d]); /* :504 */
+        for (int t0 = 0; t0 < Tv; t0 += chunk) {
+          float part = 0.0f;
+          const int t1 = Tv - t0 < chunk ? Tv : t0 + chunk;
+          for (int t = t0; t < t1; t++) part += bf(sc[t]) * bf(cacheV[((size_t)t * n_kv + h) * hd + d]); /* :504 */
+          acc = attn == ORC_ATTN_STREAM ? acc + part : part;
+        }
         orow[d] = tr(acc);
       }
       free(sc);
@@ -418,12 +523,19 @@ static void attention_impl(const uint16_t* q, const uint16_t* cacheK, const uint
 
 void orc_attention(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out, int S, int T,
                    int n_heads, int n_kv, int hd, int causal_mask) {
-  attention_impl(q, cacheK, cacheV, out, S, T, n_heads, n_kv, hd, causal_mask, 0);
+  attention_impl(q, cacheK, cacheV, out, S, T, n_heads, n_kv, hd, causal_mask, 0, ORC_ATTN_REF);
 }
 
 void orc_attention_pos(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out, int S, int T,
                        int n_heads, int n_kv, int hd, int causal_mask, int q_pos0) {
-  attention_impl(q, cacheK, cacheV, out, S, T, n_heads, n_kv, hd, causal_mask, q_pos0);
+  attention_impl(q, cacheK, cacheV, out, S, T, n_heads, n_kv, hd, causal_mask, q_pos0, ORC_ATTN_REF);
+}
+
+int orc_attention_order(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out, int S, int T,
+                        int n_heads, int n_kv, int hd, int causal_mask, int q_pos0, int attn) {
+  if (attn < ORC_ATTN_REF || attn > ORC_ATTN_STREAM) return -1;
+  attention_impl(q, cacheK, cacheV, out, S, T, n_heads, n_kv, hd, causal_mask, q_pos0, attn);
+  return 0;
 }
 
 /* ------------------------------------------------------------ whole model */
@@ -504,9 +616,18 @@ uint16_t* orc_session_cache_k(orc_session* s, int layer) { return s->ck[layer]; 
 uint16_t* orc_session_cache_v(orc_session* s, int layer) { return s->cv[layer]; }
 
 static int g_allow_chunk = 0; /* set only inside orc_forward_chunk (extension) */
+static const orc_order g_ref_order = {1, 1, ORC_ATTN_REF};
+static int order_ok(const orc_order* o) {
+  return o->ks >= 1 && o->ks <= ORC_MAX_KS && o->rms_parts >= 1 && o->rms_parts <= ORC_MAX_RMS_PARTS &&
+         (o->rms_parts == 1 || o->rms_parts % 32 == 0) && o->attn >= ORC_ATTN_REF && o->attn <= ORC_ATTN_STREAM;
+}
+/* ord: the summation order of every linear, RMSNorm scale and attention (g_ref_order: the reference's) */
 static int forward_impl(const orc_model* m, orc_session* ss, const int32_t* tokens, int S, int start_pos,
-                        float* logits, int all_rows, uint16_t* trace, int tp) {
+                        float* logits, int all_rows, uint16_t* trace, int tp, const orc_order* ord) {
   const orc_args* a = &m->a;
+  if (!order_ok(ord) || (tp > 1 && ord->ks > 1)) return -1;
+  if (ord->ks > 1 && (a->dim % 8 || a->ffn_dim % 8 || (a->n_heads * a->head_dim) % 8)) return -1;
+  const int ks = ord->ks, np = ord->rms_parts;
   if (S <= 0) return -1; /* "empty token array" llamatransformer.go:146-148 */
   if (start_pos + S > ss->seq_len) return -1;
   if (S > 1 && start_pos != 0 && !g_allow_chunk) return -1; /* mask [S,S] only broadcasts when T==S (SURVEY F11) */
@@ -533,34 +654,34 @@ static int forward_impl(const orc_model* m, orc_session* ss, const int32_t* toke
   orc_get_rows_bf16(m->tok_embd, tokens, x, S, D); /* prepare :118 */
   if (trace) memcpy(trace, x, SD * 2);
   for (int l = 0; l < a->n_layers; l++) {
-    orc_rmsnorm(x, m->attn_norm[l], xn, S, D, a->norm_eps);          /* :222 */
-    orc_linear_bf16(xn, m->wq[l], q, S, D, qd);                      /* :306 */
-    orc_linear_bf16(xn, m->wk[l], k, S, D, kvd);                     /* :325 */
-    orc_linear_bf16(xn, m->wv[l], v, S, D, kvd);                     /* :344 */
+    rmsnorm_parts(x, m->attn_norm[l], xn, S, D, a->norm_eps, np); /* :222 */
+    linear_order_bf16(xn, m->wq[l], q, S, D, qd, ks);               /* :306 */
+    linear_order_bf16(xn, m->wk[l], k, S, D, kvd, ks);              /* :325 */
+    linear_order_bf16(xn, m->wv[l], v, S, D, kvd, ks);              /* :344 */
     orc_rope_apply(q, m->cis, q2, S, nh, hd, start_pos);             /* :392 */
     orc_rope_apply(k, m->cis, k2, S, nkv, hd, start_pos);
     memcpy(ss->ck[l] + (size_t)start_pos * kvd, k2, (size_t)S * kvd * 2); /* SetSlice :402 */
     memcpy(ss->cv[l] + (size_t)start_pos * kvd, v, (size_t)S * kvd * 2);  /* :403 */
-    attention_impl(q2, ss->ck[l], ss->cv[l], o, S, T, nh, nkv, hd, S > 1, start_pos); /* :409-514 (start_pos > 0: extension) */
+    attention_impl(q2, ss->ck[l], ss->cv[l], o, S, T, nh, nkv, hd, S > 1, start_pos, ord->attn); /* :409-514 (start_pos > 0: extension) */
     if (tp > 1) linear_bf16_ksplit(o, m->wo[l], att, S, qd, D, tp);
-    else orc_linear_bf16(o, m->wo[l], att, S, qd, D);                /* :522 */
+    else linear_order_bf16(o, m->wo[l], att, S, qd, D, ks);         /* :522 */
     orc_add_bf16(x, att, h1, (int64_t)SD);                           /* :232 */
-    orc_rmsnorm(h1, m->ffn_norm[l], xn, S, D, a->norm_eps);          /* :237 */
-    orc_linear_bf16(xn, m->w1[l], g, S, D, F);                       /* :601 */
+    rmsnorm_parts(h1, m->ffn_norm[l], xn, S, D, a->norm_eps, np);  /* :237 */
+    linear_order_bf16(xn, m->w1[l], g, S, D, F, ks);                /* :601 */
     orc_silu_bf16(g, g, (int64_t)S * F);                             /* :605 */
-    orc_linear_bf16(xn, m->w3[l], u, S, D, F);                       /* :610 */
+    linear_order_bf16(xn, m->w3[l], u, S, D, F, ks);                /* :610 */
     orc_mul_bf16(g, u, g, (int64_t)S * F);                           /* :614 */
     if (tp > 1) linear_bf16_ksplit(g, m->w2[l], ff, S, F, D, tp);
-    else orc_linear_bf16(g, m->w2[l], ff, S, F, D);                  /* :619 */
+    else linear_order_bf16(g, m->w2[l], ff, S, F, D, ks);           /* :619 */
     orc_add_bf16(h1, ff, x, (int64_t)SD);                            /* :248 */
     if (trace) memcpy(trace + (size_t)(l + 1) * SD, x, SD * 2);
   }
-  orc_rmsnorm(x, m->norm, xn, S, D, a->norm_eps); /* :166 */
+  rmsnorm_parts(x, m->norm, xn, S, D, a->norm_eps, np); /* :166 */
   if (logits) {
     int rows = all_rows ? S : 1;
     const uint16_t* src = all_rows ? xn : xn + (size_t)(S - 1) * D;
     uint16_t* lg = (uint16_t*)malloc((size_t)rows * V * 2);
-    orc_linear_bf16(src, m->output, lg, rows, D, V);                 /* :170 */
+    linear_order_bf16(src, m->output, lg, rows, D, V, ks);          /* :170 */
     for (size_t i = 0; i < (size_t)rows * V; i++) logits[i] = bf(lg[i]); /* ToFloat32 :175 */
     free(lg);
   }
@@ -571,7 +692,11 @@ static int forward_impl(const orc_model* m, orc_session* ss, const int32_t* toke
 
 int orc_forward(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos, float* logits,
                 int all_rows, uint16_t* trace) {
-  return forward_impl(m, s, tokens, S, start_pos, logits, all_rows, trace, 1);
+  return forward_impl(m, s, tokens, S, start_pos, logits, all_rows, trace, 1, &g_ref_order);
+}
+int orc_forward_order(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos, float* logits,
+                      int all_rows, uint16_t* trace, const orc_order* order) {
+  return forward_impl(m, s, tokens, S, start_pos, logits, all_rows, trace, 1, order ? order : &g_ref_order);
 }
 /* EXTENSION, beyond the reference: a prompt chunk of S > 1 tokens at start_pos > 0 (chunked prefill).  The reference
  * cannot do this (its [S,S] mask does not broadcast against [S,T] scores; the only caller prefills at 0).  Everything
@@ -579,14 +704,18 @@ int orc_forward(const orc_model* m, orc_session* s, const int32_t* tokens, int S
  * results to prefilling it at once. */
 int orc_forward_chunk(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos, float* logits,
                       int all_rows) {
+  return orc_forward_chunk_order(m, s, tokens, S, start_pos, logits, all_rows, NULL);
+}
+int orc_forward_chunk_order(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos, float* logits,
+                            int all_rows, const orc_order* order) {
   g_allow_chunk = 1;
-  int rc = forward_impl(m, s, tokens, S, start_pos, logits, all_rows, NULL, 1);
+  int rc = forward_impl(m, s, tokens, S, start_pos, logits, all_rows, NULL, 1, order ? order : &g_ref_order);
   g_allow_chunk = 0;
   return rc;
 }
 int orc_forward_tp(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos, float* logits,
                    int all_rows, int tp) {
-  return forward_impl(m, s, tokens, S, start_pos, logits, all_rows, NULL, tp);
+  return forward_impl(m, s, tokens, S, start_pos, logits, all_rows, NULL, tp, &g_ref_order);
 }
 
 static double now_s(void) {

@@ -85,6 +85,33 @@ void orc_attention(const uint16_t* q, const uint16_t* cacheK, const uint16_t* ca
 void orc_attention_pos(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out,
                        int S, int T, int n_heads, int n_kv, int hd, int causal_mask, int q_pos0);
 
+/* ---- summation orders (EXTENSION, beyond the reference): the LNB_ACC_FAST statement ----
+ * The FAST routes on the FMA pipe keep every truncation point of the reference and reorder only these sums, in a fixed
+ * order read from the kernels (DESIGN.md section 3):
+ *   ks         linear: k-streams of 8-element chunks, chunk g -> stream g % ks, streams added in stream order (gemv.cuh)
+ *   rms_parts  RMSNorm sum of squares: element i -> partial i % rms_parts, xor butterfly inside each group of 32, groups in
+ *              order (gemv.cuh prologue, rmsnorm_kernel)
+ *   attn       REF: the reference's sequential Z and output chains.  TREE: Z of sdpa_kernel / sdpa_decode_kernel (128 strided
+ *              f64 partials, butterfly, ((w0 + w1) + w2) + w3).  STREAM: sdpa_stream.cuh -- keys in chunks of
+ *              ORC_STREAM_CHUNK, Z the TREE of each chunk added in chunk order, each output one f32 chain per chunk, the
+ *              chunk results added in chunk order.
+ * {1, 1, ORC_ATTN_REF} is the reference order: orc_forward's bits. */
+enum { ORC_ATTN_REF = 0, ORC_ATTN_TREE = 1, ORC_ATTN_STREAM = 2 };
+#define ORC_MAX_KS 64
+#define ORC_MAX_RMS_PARTS 1024
+#define ORC_STREAM_CHUNK 1024
+typedef struct {
+  int ks, rms_parts, attn;
+} orc_order;
+/* the pieces at op level; each returns 0, or -1 for an order it does not describe (K % 8 != 0 with ks > 1, parts not 1 or
+ * a multiple of 32) */
+int    orc_linear_order_bf16(const uint16_t* x, const uint16_t* w, uint16_t* out, int S, int K, int N, int ks);
+int    orc_rms_scale_order(const uint16_t* x, float* r, int S, int D, float eps, int parts);
+int    orc_attention_order(const uint16_t* q, const uint16_t* cacheK, const uint16_t* cacheV, uint16_t* out, int S, int T,
+                           int n_heads, int n_kv, int hd, int causal_mask, int q_pos0, int attn);
+/* the softmax denominator alone: sum of e[0..n) in the order attn */
+double orc_attention_z(const double* e, int n, int attn);
+
 /* ---- whole model ---- */
 typedef struct {
   int dim, n_layers, n_heads, n_kv_heads, head_dim, ffn_dim, vocab, max_seq_len;
@@ -118,6 +145,11 @@ int         orc_forward(const orc_model* m, orc_session* s, const int32_t* token
 /* extension (beyond the reference): S > 1 tokens at start_pos > 0 with the [S,T] causal mask -- chunked prefill */
 int         orc_forward_chunk(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos,
                               float* logits, int all_rows);
+/* orc_forward / orc_forward_chunk with every linear, RMSNorm scale and attention summed in `order` (NULL: the reference's) */
+int         orc_forward_order(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos,
+                              float* logits, int all_rows, uint16_t* trace, const orc_order* order);
+int         orc_forward_chunk_order(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos,
+                                    float* logits, int all_rows, const orc_order* order);
 int         orc_forward_tp(const orc_model* m, orc_session* s, const int32_t* tokens, int S, int start_pos,
                            float* logits, int all_rows, int tp);
 /* generateTokensInternal: src/inference/inference.go:173-254.  Returns number of

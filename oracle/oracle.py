@@ -67,6 +67,22 @@ class OrcArgs(C.Structure):
     ]
 
 
+class OrcOrder(C.Structure):
+    _fields_ = [("ks", C.c_int), ("rms_parts", C.c_int), ("attn", C.c_int)]
+
+
+# summation orders (lnb_oracle.h): (ks, rms_parts, attn).  ATTN_REF is the reference's order; FAST / FAST_STREAM state the
+# order of LNB_ACC_FAST on the FMA pipe with the shared-memory attention kernels / the streamed attention kernels
+ATTN_REF, ATTN_TREE, ATTN_STREAM = 0, 1, 2
+ORDER_REF = (1, 1, ATTN_REF)
+ORDER_FAST = (8, 256, ATTN_TREE)
+ORDER_FAST_STREAM = (8, 256, ATTN_STREAM)
+
+
+def _order(order):
+    return C.byref(OrcOrder(*order)) if order is not None else None
+
+
 _u16p = C.POINTER(C.c_uint16)
 _f32p = C.POINTER(C.c_float)
 _i32p = C.POINTER(C.c_int32)
@@ -118,6 +134,19 @@ def _declare(L):
     L.orc_forward_chunk.argtypes = [C.c_void_p, C.c_void_p, _i32p, C.c_int, C.c_int, _f32p, C.c_int]
     L.orc_forward_tp.restype = C.c_int
     L.orc_forward_tp.argtypes = [C.c_void_p, C.c_void_p, _i32p, C.c_int, C.c_int, _f32p, C.c_int, C.c_int]
+    L.orc_forward_order.restype = C.c_int
+    L.orc_forward_order.argtypes = [C.c_void_p, C.c_void_p, _i32p, C.c_int, C.c_int, _f32p, C.c_int, _u16p, C.POINTER(OrcOrder)]
+    L.orc_forward_chunk_order.restype = C.c_int
+    L.orc_forward_chunk_order.argtypes = [C.c_void_p, C.c_void_p, _i32p, C.c_int, C.c_int, _f32p, C.c_int, C.POINTER(OrcOrder)]
+    L.orc_linear_order_bf16.restype = C.c_int
+    L.orc_linear_order_bf16.argtypes = [_u16p, _u16p, _u16p, C.c_int, C.c_int, C.c_int, C.c_int]
+    L.orc_rms_scale_order.restype = C.c_int
+    L.orc_rms_scale_order.argtypes = [_u16p, _f32p, C.c_int, C.c_int, C.c_float, C.c_int]
+    L.orc_attention_order.restype = C.c_int
+    L.orc_attention_order.argtypes = [_u16p, _u16p, _u16p, _u16p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int]
+    L.orc_attention_z.restype = C.c_double
+    L.orc_attention_z.argtypes = [_f64p, C.c_int, C.c_int]
     L.orc_generate.restype = C.c_int
     L.orc_generate.argtypes = [C.c_void_p, _i32p, C.c_int, C.c_int, _i32p, C.c_int, _i32p, _f64p]
     L.orc_synth_fill.argtypes = [C.c_uint64, C.c_char_p, C.c_float, C.c_float, C.c_int64, _u16p]
@@ -287,6 +316,44 @@ def attention(q, cache_k, cache_v, T, causal_mask, q_pos0=0):
     return out
 
 
+def linear_order_bf16(x, w, ks):
+    """linear with k-streams of 8-element chunks (ks = 1: orc_linear_bf16's order)"""
+    S, K = x.shape
+    N = w.shape[0]
+    out = np.empty((S, N), np.uint16)
+    if lib().orc_linear_order_bf16(_p(x, _u16p), _p(w, _u16p), _p(out, _u16p), S, K, N, int(ks)) != 0:
+        raise ValueError(f"no linear order ks={ks} at K={K}")
+    return out
+
+
+def rms_scale_order(x, eps=1e-5, parts=1):
+    """rms_scale with the sum of squares in `parts` interleaved partials, butterfly and groups of 32 in order"""
+    x = np.ascontiguousarray(x, np.uint16)
+    S, D = x.shape
+    r = np.empty(S, np.float32)
+    if lib().orc_rms_scale_order(_p(x, _u16p), _p(r, _f32p), S, D, eps, int(parts)) != 0:
+        raise ValueError(f"no RMS order with {parts} partials")
+    return r
+
+
+def attention_order(q, cache_k, cache_v, T, causal_mask, q_pos0=0, attn=ATTN_REF):
+    """attention with the softmax denominator and the output chains in the order attn (ATTN_REF: attention's bits)"""
+    S, nh, hd = q.shape
+    nkv = cache_k.shape[1]
+    out = np.empty((S, nh * hd), np.uint16)
+    rc = lib().orc_attention_order(_p(q, _u16p), _p(cache_k, _u16p), _p(cache_v, _u16p), _p(out, _u16p), S, T, nh, nkv, hd,
+                                   int(causal_mask), int(q_pos0), int(attn))
+    if rc != 0:
+        raise ValueError(f"no attention order {attn}")
+    return out
+
+
+def attention_z(e, attn):
+    """the softmax denominator alone: the f64 sum of e in the order attn"""
+    e = np.ascontiguousarray(e, np.float64)
+    return float(lib().orc_attention_z(_p(e, _f64p), e.size, int(attn)))
+
+
 def synth_fill(seed: int, name: str, scale: float, offset: float, n: int, out: np.ndarray | None = None):
     if out is None:
         out = np.empty(n, np.uint16)
@@ -337,23 +404,34 @@ class OracleSession:
             lib().orc_session_free(self.h)
             self.h = None
 
-    def forward_chunk(self, tokens, start_pos, all_rows=True):
-        """EXTENSION (beyond the reference): a prompt chunk of S > 1 tokens at start_pos > 0 with the [S,T] causal mask"""
+    def forward_chunk(self, tokens, start_pos, all_rows=True, order=None):
+        """EXTENSION (beyond the reference): a prompt chunk of S > 1 tokens at start_pos > 0 with the [S,T] causal mask.
+        order (ks, rms_parts, attn): sum in that order (None: the reference's)"""
         tokens = np.ascontiguousarray(tokens, np.int32)
         S = len(tokens)
         logits = np.empty((S if all_rows else 1, self.model.args.vocab), np.float32)
-        rc = lib().orc_forward_chunk(self.model.h, self.h, _p(tokens, _i32p), S, start_pos, _p(logits, _f32p), int(all_rows))
+        if order is not None:
+            rc = lib().orc_forward_chunk_order(self.model.h, self.h, _p(tokens, _i32p), S, start_pos, _p(logits, _f32p),
+                                               int(all_rows), _order(order))
+        else:
+            rc = lib().orc_forward_chunk(self.model.h, self.h, _p(tokens, _i32p), S, start_pos, _p(logits, _f32p), int(all_rows))
         if rc != 0:
             raise RuntimeError("orc_forward_chunk failed (bad tokens / positions)")
         return logits
 
-    def forward(self, tokens, start_pos, all_rows=True, trace=False, tp=1):
+    def forward(self, tokens, start_pos, all_rows=True, trace=False, tp=1, order=None):
+        """order (ks, rms_parts, attn), e.g. ORDER_FAST: every sum in that order (None: the reference's)"""
         tokens = np.ascontiguousarray(tokens, np.int32)
         S = len(tokens)
         V, D, L = self.model.args.vocab, self.model.args.dim, self.model.args.n_layers
         logits = np.empty((S if all_rows else 1, V), np.float32)
         tr = np.empty((L + 1, S, D), np.uint16) if trace else None
-        if tp > 1:
+        if order is not None:
+            if tp > 1:
+                raise ValueError("a summation order and a tensor-parallel split do not combine")
+            rc = lib().orc_forward_order(self.model.h, self.h, _p(tokens, _i32p), S, start_pos, _p(logits, _f32p), int(all_rows),
+                                         _p(tr, _u16p) if trace else None, _order(order))
+        elif tp > 1:
             rc = lib().orc_forward_tp(self.model.h, self.h, _p(tokens, _i32p), S, start_pos, _p(logits, _f32p),
                                       int(all_rows), tp)
         else:

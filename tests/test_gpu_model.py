@@ -1,6 +1,7 @@
 """GPU parity of the model-level C-ABI (LlamaTransformer.Forward / generate loop) against the CPU
 oracle on a structurally identical miniature of Llama-3.1 (all fusion paths, GQA, RoPE, KV cache).
-STRICT mode must reproduce the oracle bit for bit; FAST within north_star's tolerance."""
+STRICT mode must reproduce the oracle bit for bit; FAST the oracle run in FAST's summation order (tests/test_gpu_fast_order.py),
+and within north_star's tolerance of the reference order."""
 import numpy as np
 import pytest
 
@@ -99,23 +100,27 @@ def test_forward_per_layer_trace_strict(L, tiny):
         ctx.close()
 
 
-def test_forward_fast_within_tolerance(L, tiny):
+def test_forward_fast_equals_the_fast_order_statement(L, tiny):
+    """FAST through the reference-shaped Forward: every prompt row and every decode step is the oracle run in FAST's
+    summation order (O.ORDER_FAST) bit for bit -- and so within north_star's tolerance of the reference order"""
     args, _, om, gm = tiny
     rng = np.random.default_rng(11)
     seq = 24
     toks = rng.integers(0, args["vocab_size"], size=seq).astype(np.int32)
     ctx = L.model.InferenceContext(gm.Transformer, L.model.InferenceArgs(seq), acc_mode=L._capi.LNB_ACC_FAST)
-    osess = om.new_session(seq)
+    osess, oref = om.new_session(seq), om.new_session(seq)
     try:
-        exp = osess.forward(toks[:8], 0)
+        exp = osess.forward(toks[:8], 0, order=O.ORDER_FAST)
         got = gm.Transformer.Forward(ctx, L.ml.Tensor(toks[:8], L.ml.DT_INT32), 0).RawData
-        assert np.abs(got - exp).max() <= 1e-2                      # north_star tolerance
+        assert np.array_equal(got, exp)
+        assert np.abs(got - oref.forward(toks[:8], 0)).max() <= 1e-2                      # north_star tolerance
         for pos in range(8, 16):
-            exp = osess.forward(toks[pos:pos + 1], pos)
+            exp = osess.forward(toks[pos:pos + 1], pos, order=O.ORDER_FAST)
             got = gm.Transformer.Forward(ctx, L.ml.Tensor(toks[pos:pos + 1], L.ml.DT_INT32), pos).RawData
-            assert np.abs(got - exp).max() <= 1e-2
+            assert np.array_equal(got, exp), f"position {pos}"
+            assert np.abs(got - oref.forward(toks[pos:pos + 1], pos)).max() <= 1e-2
     finally:
-        ctx.close(); osess.close()
+        ctx.close(); osess.close(); oref.close()
 
 
 def test_forward_errors_like_reference(L, tiny):
