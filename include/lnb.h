@@ -70,6 +70,10 @@ typedef struct lnb_session lnb_session; /* model.InferenceContext: KV cache + ac
  * device `device`.  tp_size==1: nccl_unique_id may be NULL.  tp_size>1: one process per
  * rank; nccl_unique_id is the 128-byte id from lnb_nccl_unique_id() of rank 0, sent by
  * the host (torch.distributed / Go) to every rank.
+ * Shapes (LNB_EINVAL otherwise, before any device call): n_heads a multiple of n_kv_heads; head_dim a
+ * multiple of 8 (every attention kernel reads a head's K/V row as 16-byte vectors); dim and each rank's
+ * n_heads * head_dim and n_kv_heads * head_dim multiples of 32, its ffn_dim and vocab_size shares
+ * multiples of 16.
  * Replaces: model.NewLlamaTransformer (src/model/llamatransformer.go:64-113). */
 int lnb_model_create(const lnb_model_args* args, int device, int tp_rank, int tp_size,
                      const void* nccl_unique_id, lnb_model** out);

@@ -269,7 +269,8 @@ extern "C" int lnb_model_create(const lnb_model_args* args, int device, int tp_r
       a.vocab_size <= 0 || a.max_seq_len <= 0)
     return fail(LNB_EINVAL, "non-positive model dimension");
   if (a.n_heads % a.n_kv_heads) return fail(LNB_EINVAL, "n_heads %d not a multiple of n_kv_heads %d", a.n_heads, a.n_kv_heads);
-  if (a.head_dim % 2) return fail(LNB_EINVAL, "head_dim must be even");
+  // every attention kernel reads a head's K/V row as 16-byte vectors (8 bf16) from cache + t * kv_dim + h * head_dim
+  if (a.head_dim % 8) return fail(LNB_EINVAL, "head_dim %d must be a multiple of 8 (the attention kernels read K/V rows 8 elements at a time)", a.head_dim);
   if (tp_size < 1 || tp_rank < 0 || tp_rank >= tp_size) return fail(LNB_EINVAL, "bad tp rank %d / size %d", tp_rank, tp_size);
   if (a.n_kv_heads % tp_size || a.ffn_dim % tp_size || a.vocab_size % tp_size)
     return fail(LNB_EINVAL, "tp_size %d must divide n_kv_heads, ffn_dim and vocab_size", tp_size);
