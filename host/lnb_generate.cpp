@@ -10,6 +10,9 @@
 // weights (lnb_forward_speculative); the generated ids are the same as without it.  Not with slots=.
 // rep=R freq=F pres=P [last_n=N]: repetition, frequency and presence penalties over the generated tokens (the last N positions;
 // 0, the default: all) before the sampler or the greedy pick (lnb_session_set_penalties).
+// regex=PATTERN (with <modelDir>/tokenizer.model): every generated token keeps the text a prefix of a string of
+// re.fullmatch(PATTERN, s, re.ASCII); a stop token of the tokenizer only follows a complete match (model::Grammar,
+// lnb_session_set_grammar).  Also with batch= (every prompt) and slots=; not with beams=.
 // beams=B [len_pen=A] [early_stop=1]: beam search with B in [1, 8] beams (inference::GenerateBeams): one line per hypothesis,
 // best first, with its state (1 EOS, 2 SequenceLength), raw score s and normalised score h = s / len^A, then its tokens (or
 // text with a tokenizer).  Not with batch=, temp=, spec= or the penalties.
@@ -148,6 +151,7 @@ int main(int argc, char** argv) {
     int batch = 0, slots = 0;
     const char* prompt_text = nullptr;
     const char* score_text_arg = nullptr;
+    const char* regex = nullptr;
     int logprobs = -1;              // logprobs=N: top N alternatives per generated token
     model::SamplingArgs sampling;   // temp= top_k= top_p= seed= (temp 0, the default: greedy)
     model::SpeculativeArgs spec;    // spec=K: speculative decoding with up to K prompt-lookup drafts per call (0: plain steps)
@@ -167,6 +171,7 @@ int main(int argc, char** argv) {
       if (!strncmp(argv[i], "slots=", 6)) slots = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "prompt=", 7)) prompt_text = argv[i] + 7;
       if (!strncmp(argv[i], "score=", 6)) score_text_arg = argv[i] + 6;
+      if (!strncmp(argv[i], "regex=", 6)) regex = argv[i] + 6;
       if (!strncmp(argv[i], "logprobs=", 9)) logprobs = atoi(argv[i] + 9);
       if (!strncmp(argv[i], "temp=", 5)) sampling.Temperature = (float)atof(argv[i] + 5);
       if (!strncmp(argv[i], "top_k=", 6)) sampling.TopK = atoi(argv[i] + 6);
@@ -179,15 +184,18 @@ int main(int argc, char** argv) {
       score_text(transformer, model::Tokenizer(std::string(argv[3]) + "/tokenizer.model"), seq_len, acc, score_text_arg);
       return 0;
     }
-    if (prompt_text) {
-      if (!from_dir) throw Error("prompt= needs a model directory with tokenizer.model");
+    if (prompt_text || regex) {
+      if (!from_dir) throw Error(std::string(prompt_text ? "prompt=" : "regex=") + " needs a model directory with tokenizer.model");
       tokenizer = std::make_unique<model::Tokenizer>(std::string(argv[3]) + "/tokenizer.model");
       if (tokenizer->Size() != transformer.args.vocab_size)   // checkModelArgs (loader.go:98-120)
         throw Error("VocabSize=" + std::to_string(transformer.args.vocab_size) + " and vocabulary model length=" +
                     std::to_string(tokenizer->Size()) + " aren't equal");
       vocab = tokenizer->GetVocabulary();
-      prompt = tokenizer->Tokenize({{"user", prompt_text}});
+      if (prompt_text) prompt = tokenizer->Tokenize({{"user", prompt_text}});
     }
+    std::unique_ptr<model::Grammar> grammar_owned;
+    if (regex) grammar_owned = std::make_unique<model::Grammar>(transformer, regex, *tokenizer);
+    const model::Grammar* grammar = grammar_owned.get();
     const model::SpeculativeArgs* speculative = spec.MaxDraft > 0 ? &spec : nullptr;
     const model::PenaltyArgs* penalties = pen.Neutral() ? nullptr : &pen;
     if (speculative && slots > 0) throw Error("spec= is not built for continuous batching (slots=)");
@@ -195,7 +203,7 @@ int main(int argc, char** argv) {
       if (batch > 0) throw Error("beams= is not built with batch=");
       beam_args.NumReturn = std::max(1, beam_args.NumBeams);
       const std::vector<inference::BeamHypothesis> hyps =
-          inference::GenerateBeams(transformer, vocab, seq_len, acc, prompt, beam_args, &sampling, penalties, speculative);
+          inference::GenerateBeams(transformer, vocab, seq_len, acc, prompt, beam_args, &sampling, penalties, speculative, grammar);
       for (size_t i = 0; i < hyps.size(); i++) {
         const inference::BeamHypothesis& h = hyps[i];
         printf("beam[%zu]: state %d s %.17g h %.17g |", i, (int)h.State, h.Score, h.NormalizedScore);
@@ -217,8 +225,10 @@ int main(int argc, char** argv) {
       auto collect = [&](int seq, inference::GenerationState, int32_t tok) { outs[seq].push_back(tok); };
       if (slots > 0)
         inference::GenerateTokensContinuous(transformer, vocab, seq_len, acc, prompts, slots, std::max(slots, 64), collect, &sampling, logprobs,
-                                            &lps, penalties);
-      else inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling, speculative, logprobs, &lps, penalties);
+                                            &lps, penalties, grammar);
+      else
+        inference::GenerateTokensBatch(transformer, vocab, seq_len, acc, prompts, collect, &sampling, speculative, logprobs, &lps, penalties,
+                                       grammar);
       const double sec = std::chrono::duration<double>(std::chrono::steady_clock::now() - b0).count();
       size_t total = 0;
       for (int b = 0; b < batch; b++) {
@@ -240,7 +250,7 @@ int main(int argc, char** argv) {
     inference::GenerateTokens(transformer, vocab, seq_len, acc, prompt, [&](inference::GenerationState, int32_t tok) {
       if (out.empty()) t_first = std::chrono::steady_clock::now();
       out.push_back(tok);
-    }, &sampling, speculative, logprobs, &lp, penalties);
+    }, &sampling, speculative, logprobs, &lp, penalties, grammar);
     auto t1 = std::chrono::steady_clock::now();
     if (tokenizer) printf("text: %s\n", tokenizer->TokenBatchToString(out).c_str());
     printf("tokens:");

@@ -338,6 +338,34 @@ inline std::vector<int32_t> PromptLookupDrafts(const std::vector<int32_t>& h, in
   return {};
 }
 
+// EXTENSION: regex-constrained generation (lnb_grammar_create, DESIGN.md §9g).  The tokens a sequence emits after the
+// grammar's first position spell a prefix of a string of re.fullmatch(regex, s, re.ASCII); a stop token (Z: the
+// tokenizer's stop ids) only follows a complete match.  Token bytes come from the tokenizer, special tokens are empty.  The
+// masks of every state are built on the model's device, once.
+class Grammar {
+ public:
+  Grammar(LlamaTransformer& t, const std::string& regex, const Tokenizer& tok) {
+    const int V = t.args.vocab_size, nMerge = tok.Size() - 256;
+    std::vector<uint8_t> bytes;
+    std::vector<int64_t> off(1, 0);
+    for (int i = 0; i < V; i++) {
+      if (i < nMerge) {
+        const std::string b = tok.IdToToken(i);
+        bytes.insert(bytes.end(), b.begin(), b.end());
+      }
+      off.push_back((int64_t)bytes.size());
+    }
+    const std::vector<int32_t> stop = tok.GetVocabulary().StopTokenIds;
+    check(lnb_grammar_create(t.handle(), regex.data(), (int64_t)regex.size(), bytes.data(), off.data(), stop.data(), (int)stop.size(), &h_));
+  }
+  ~Grammar() { lnb_grammar_destroy(h_); }
+  Grammar(const Grammar&) = delete;
+  const lnb_grammar* handle() const { return h_; }
+
+ private:
+  lnb_grammar* h_ = nullptr;
+};
+
 class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
  public:
   int SequenceLength;
@@ -366,6 +394,9 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
     const lnb_penalties p = a->C(promptLength);
     check(lnb_session_set_penalties(h_, seq, &p));
   }
+  // EXTENSION: sequence seq is constrained by *g (nullptr: off) from its next forward on, its grammar starting at position
+  // firstPos (typically the prompt's length)
+  void SetGrammar(int seq, const Grammar* g, int firstPos) { check(lnb_session_set_grammar(h_, seq, g ? g->handle() : nullptr, firstPos)); }
   // EXTENSION: token log-probabilities (lnb_session_set_logprobs).  topN 0..20 turns them on for sequence seq, -1 off; every
   // token the context then emits for seq writes the record of the position it occupies (the raw model distribution).
   void SetLogprobs(int seq, int topN) { check(lnb_session_set_logprobs(h_, seq, topN)); }
@@ -531,18 +562,20 @@ inline void GenerateSpeculative(model::InferenceContext& infContext, const model
 
 // generateTokensInternal (inference.go:173-254); `emit` plays generatedTokensCh.  EXTENSION: logprobs 0..20 turns on token
 // log-probabilities; logprobsOut (or nullptr) then gets one record per emitted token, in order.  penalties (or nullptr):
-// every emitted token is drawn from the penalized logits (the records stay the raw distribution's).
+// every emitted token is drawn from the penalized logits (the records stay the raw distribution's).  grammar (or nullptr):
+// every emitted token is one the grammar allows after the tokens emitted before it.
 inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                            const std::vector<int32_t>& promptTokens, const std::function<void(GenerationState, int32_t)>& emit,
                            const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr,
                            int logprobs = -1, std::vector<lnb_logprob>* logprobsOut = nullptr,
-                           const model::PenaltyArgs* penalties = nullptr) {
+                           const model::PenaltyArgs* penalties = nullptr, const model::Grammar* grammar = nullptr) {
   // the prefill call carries the whole prompt: size the session's row buffers for it
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max<int>(8, (int)promptTokens.size()));
   if (penalties && penalties->Neutral()) penalties = nullptr;
-  const bool samples = (sampling && sampling->Samples()) || penalties;
+  const bool samples = (sampling && sampling->Samples()) || penalties || grammar;
   if (sampling && sampling->Samples()) infContext.SetSampling(0, sampling);   // the sampled token instead of Slice + ml.Argmax
   if (penalties) infContext.SetPenalties(0, penalties, (int)promptTokens.size());
+  if (grammar) infContext.SetGrammar(0, grammar, (int)promptTokens.size());
   if (logprobs >= 0) infContext.SetLogprobs(0, logprobs);
   if (logprobs < 0) logprobsOut = nullptr;
   const int promptLength = (int)promptTokens.size();
@@ -588,18 +621,20 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
 // The consumer InferenceEngine.TokenizeBatch (src/inference/tokenize.go:97-107) never got in the reference
 // (SURVEY 8f-4): every prompt runs the loop above -- own KV cache, positions and stop condition -- but all
 // sequences advance together, one pass over the weights per step.  emit(sequence, state, token).  logprobs / logprobsOut as in
-// GenerateTokens, one list per prompt; penalties as in GenerateTokens, for every sequence.
+// GenerateTokens, one list per prompt; penalties and grammar as in GenerateTokens, for every sequence.
 inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength, int accMode,
                                 const std::vector<std::vector<int32_t>>& prompts,
                                 const std::function<void(int, GenerationState, int32_t)>& emit,
                                 const model::SamplingArgs* sampling = nullptr, const model::SpeculativeArgs* speculative = nullptr,
                                 int logprobs = -1, std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr,
-                                const model::PenaltyArgs* penalties = nullptr) {
+                                const model::PenaltyArgs* penalties = nullptr, const model::Grammar* grammar = nullptr) {
   const int n = (int)prompts.size();
   if (n < 1) throw Error("empty prompt batch");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, n), n);
   if (penalties)
     for (int i = 0; i < n; i++) infContext.SetPenalties(i, penalties, (int)prompts[i].size());
+  if (grammar)
+    for (int i = 0; i < n; i++) infContext.SetGrammar(i, grammar, (int)prompts[i].size());
   if (logprobs >= 0)
     for (int i = 0; i < n; i++) infContext.SetLogprobs(i, logprobs);
   if (logprobs < 0) logprobsOut = nullptr;
@@ -654,13 +689,14 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
 // row, the rest of the stepTokens-row budget goes to prompt chunks first in first out, a prompt whose last chunk is in the
 // step emits its first token, a finished slot takes the next waiting prompt at position 0; steps without prompt rows run
 // lnb_forward_batch.  emit(prompt index, state, token); per prompt the stream is GenerateTokens' own.  logprobs / logprobsOut
-// as in GenerateTokens, one list per prompt; penalties as in GenerateTokens, set at each admission (first_pos follows the prompt).
+// as in GenerateTokens, one list per prompt; penalties and grammar as in GenerateTokens, set at each admission (first_pos
+// follows the prompt).
 inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength,
                                      int accMode, const std::vector<std::vector<int32_t>>& prompts, int slots, int stepTokens,
                                      const std::function<void(int, GenerationState, int32_t)>& emit,
                                      const model::SamplingArgs* sampling = nullptr, int logprobs = -1,
                                      std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr,
-                                     const model::PenaltyArgs* penalties = nullptr) {
+                                     const model::PenaltyArgs* penalties = nullptr, const model::Grammar* grammar = nullptr) {
   if (slots < 1 || slots > 8) throw Error("slots must be in [1, 8]");
   if (stepTokens < slots) throw Error("stepTokens must be at least slots (every decoding sequence gets a row)");
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, stepTokens), slots);
@@ -686,6 +722,7 @@ inline void GenerateTokensContinuous(model::LlamaTransformer& transformer, const
           infContext.SetSampling((int)(&s - slot.data()), &a);
         }
         if (penalties) infContext.SetPenalties((int)(&s - slot.data()), penalties, (int)prompts[(size_t)s.i].size());
+        if (grammar) infContext.SetGrammar((int)(&s - slot.data()), grammar, (int)prompts[(size_t)s.i].size());
       }
     std::vector<int> decoding, prefilling;
     for (int k = 0; k < slots; k++)
@@ -795,14 +832,16 @@ struct Pool {
 // The prompt is prefilled on sequence 0 and forked to the other beams (CopySequences); every step is one ForwardBatch of the B
 // beams, whose logprob records (top 2B) give the candidates, then one CopySequences moves each surviving beam's parent rows.
 // Returns the NumReturn best hypotheses, best first.  Beam search ranks the raw distribution deterministically: sampling,
-// penalties or speculation are an error.
+// penalties, a grammar or speculation are an error.
 inline std::vector<BeamHypothesis> GenerateBeams(model::LlamaTransformer& transformer, const model::Vocabulary& vocab, int sequenceLength,
                                                  int accMode, const std::vector<int32_t>& promptTokens, const BeamSearchArgs& beams,
                                                  const model::SamplingArgs* sampling = nullptr, const model::PenaltyArgs* penalties = nullptr,
-                                                 const model::SpeculativeArgs* speculative = nullptr) {
+                                                 const model::SpeculativeArgs* speculative = nullptr,
+                                                 const model::Grammar* grammar = nullptr) {
   using beam_detail::Cand;
-  if ((sampling && sampling->Samples()) || penalties || speculative)
-    throw Error("beam search ranks the raw distribution deterministically: it takes no sampling, penalties or speculative decoding");
+  if ((sampling && sampling->Samples()) || penalties || speculative || grammar)
+    throw Error("beam search ranks the raw distribution deterministically: it takes no sampling, penalties, grammar or "
+                "speculative decoding");
   const int B = beams.NumBeams;
   if (B < 1 || B > 8) throw Error("NumBeams " + std::to_string(B) + " must be in [1, 8]");
   if (!std::isfinite(beams.LengthPenalty)) throw Error("LengthPenalty must be finite");

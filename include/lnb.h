@@ -351,6 +351,60 @@ typedef struct {
  * sequence re-captures a decode graph; changing their values does not. */
 int lnb_session_set_penalties(lnb_session* s, int seq, const lnb_penalties* p);
 
+/* EXTENSION: regex-constrained generation, computed on the device (csrc/grammar.cuh, DESIGN.md §9g).
+ * A grammar G is a byte-level DFA with states 0..Q-1, start q0 = 0, accepting set F and transition δ: Q x 256 -> Q ∪ {⊥},
+ * trimmed (every state reaches F; a transition into a state that cannot is ⊥), with the bytes b(t) of every token
+ * t < vocab_size (possibly empty) and a non-empty stop set Z.  δ*(q, b) walks the bytes; ⊥ absorbs.
+ *  - A text token t is allowed in q when t ∉ Z, |b(t)| >= 1 and δ*(q, b(t)) != ⊥; a stop token is allowed when q ∈ F.
+ *    mask(q) is the set of allowed tokens; if it is empty (q = ⊥, or no token continues and q ∉ F), mask(q) = Z.
+ *  - The state history of a sequence whose grammar starts at first_pos: g[first_pos] = q0, and for the token t fed at
+ *    position p >= first_pos, g[p+1] = δ*(g[p], b(t)) if t is an allowed text token in g[p], else ⊥.  A stop token or an
+ *    out-of-grammar token fed by the caller therefore ends in ⊥, where only Z is allowed.
+ *  - The row that emits position p_next >= first_pos uses l'_t = t ∈ mask(g[p_next]) ? l_t : -inf, after the penalties of
+ *    lnb_session_set_penalties and before the sampler of lnb_session_set_sampling (greedy: its rank 0).  Rows with
+ *    p_next < first_pos are not masked.  No rounding is involved.  Logprobs and the logits read-backs keep reporting the
+ *    raw distribution.
+ *  - The mask never un-bans anything: if every allowed token's l' is -inf (e.g. a -inf bias on all of them), the sampler's
+ *    rank order still picks a token, and the history then moves to ⊥.
+ * The history is keyed by position, so a stream does not depend on batching, chunking, ragged scheduling or speculation;
+ * rejected drafts leave stale g entries that the next call rewrites before any row reads them. */
+typedef struct lnb_grammar lnb_grammar;
+#define LNB_GRAMMAR_MAX_STATES 4096
+/* Compiles a UTF-8 regular expression (host only).  The language is re.fullmatch(pattern, s, re.ASCII) over the UTF-8
+ * encodings of s.  Syntax: literals; escaped metacharacters (any escaped ASCII punctuation or space); \n \t \r \f \v \xHH
+ * \uHHHH; \d \D \w \W \s \S (ASCII classes, as re.ASCII); . (any code point but \n); [...] with ranges, ^ negation and the
+ * shorthands; (...) and (?:...); |; * + ? {m} {m,} {m,n} (m, n <= 100000) and their lazy forms.  . and negated classes
+ * cover U+0000..U+10FFFF minus the surrogates.  trans[cap][256] (-1: ⊥), accept[cap], *n_states = Q; state 0 is the start
+ * and every state reaches an accepting one (the DFA is minimal and trimmed).  LNB_EINVAL (the message gives the byte
+ * offset for syntax): any other syntax (anchors, backreferences, lookaround, \b, inline flags, a '{' that is not a
+ * repeat, groups nested deeper than 1000), invalid UTF-8, a pattern that matches no string, more than LNB_GRAMMAR_MAX_STATES or cap states after
+ * minimisation (*n_states still says how many), or an intermediate automaton past its size bound. */
+int lnb_regex_dfa(const char* pattern, int64_t len, int32_t* trans, uint8_t* accept, int cap, int* n_states);
+/* Compiles `regex` (lnb_regex_dfa), uploads the DFA and the token bytes (token t: tok_bytes[tok_off[t] .. tok_off[t+1]),
+ * tok_off[0] = 0, non-decreasing, t < vocab_size) to the model's device and builds every state's mask there, once.
+ * stop_ids[n_stop]: Z, n_stop >= 1, ids in [0, vocab_size).  LNB_EINVAL: a bad argument or pattern; LNB_ENOMEM with the
+ * bytes. */
+int lnb_grammar_create(lnb_model* m, const char* regex, int64_t len, const uint8_t* tok_bytes, const int64_t* tok_off,
+                       const int32_t* stop_ids, int n_stop, lnb_grammar** out);
+/* info[4]: Q, the number of states whose mask is Z (no token continues them and they do not accept), the device bytes the
+ * grammar holds, the mask build's device time in nanoseconds */
+int lnb_grammar_info(const lnb_grammar* g, int64_t* info);
+/* mask(state) to out[⌈vocab_size/32⌉] (bit t & 31 of word t >> 5: token t allowed); state -1 is ⊥ (the mask Z) */
+int lnb_grammar_read_mask(const lnb_grammar* g, int state, uint32_t* out);
+/* LNB_ESTATE while a session's sequence still uses the grammar */
+int lnb_grammar_destroy(lnb_grammar* g);
+/* Sequence `seq` is constrained by g from its next forward on, its grammar starting at position first_pos; NULL turns the
+ * constraint off (the default: the session launches exactly what it does without grammars).  Enabling writes
+ * g[first_pos] = q0 and g[p] = ⊥ for every p > first_pos (stream-ordered); from then on every forward advances the
+ * sequence's state history over its rows at positions >= first_pos.  Tokens fed at positions >= first_pos BEFORE the call
+ * are not walked: feed them again (e.g. the prompt, or a chunk from first_pos on) before emitting from a later position,
+ * else that row sees ⊥ and only Z is allowed.  The first enable allocates the history of every sequence and position (4 bytes each), the slot
+ * table, the processed rows and the sampler's slots (LNB_ENOMEM with the bytes; the session stays as it was).  LNB_EINVAL
+ * with nothing changed: seq outside [0, n_seq), first_pos outside [0, seq_len], a grammar of another model, tp_size > 1
+ * (not built).  Turning the constraint on or off for the active sequence re-captures a decode graph; switching grammars
+ * or first_pos does not.  lnb_session_copy_sequences does not copy the state history. */
+int lnb_session_set_grammar(lnb_session* s, int seq, const lnb_grammar* g, int first_pos);
+
 /* EXTENSION: token log-probabilities, computed on the device (csrc/logprob.cuh) and finished on the host (DESIGN.md §9d).
  * For one row of logits l and a token t: the rank order is the sampler's (l descending, index ascending), m the rank-0
  * logit, sum = the sum over the vocabulary of floor(2^40 exp(f32(l_i - m))) (0 below -28: the sampler's weights at

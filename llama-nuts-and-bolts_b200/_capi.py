@@ -33,6 +33,7 @@ LNB_LOGPROBS_TOP_MAX = 20
 
 
 LNB_LOGIT_BIAS_MAX = 64
+LNB_GRAMMAR_MAX_STATES = 4096
 
 
 class PenaltiesC(C.Structure):   # lnb_penalties
@@ -92,6 +93,12 @@ SIGNATURES = {
     "lnb_session_set_sampling": (C.c_int, [vp, C.c_int, C.POINTER(SamplingC)]),
     "lnb_session_set_logprobs": (C.c_int, [vp, C.c_int, C.c_int]),
     "lnb_session_set_penalties": (C.c_int, [vp, C.c_int, C.POINTER(PenaltiesC)]),
+    "lnb_regex_dfa": (C.c_int, [C.c_char_p, C.c_int64, i32p, C.POINTER(C.c_uint8), C.c_int, C.POINTER(C.c_int)]),
+    "lnb_grammar_create": (C.c_int, [vp, C.c_char_p, C.c_int64, C.POINTER(C.c_uint8), i64p, i32p, C.c_int, C.POINTER(vp)]),
+    "lnb_grammar_info": (C.c_int, [vp, i64p]),
+    "lnb_grammar_read_mask": (C.c_int, [vp, C.c_int, C.POINTER(C.c_uint32)]),
+    "lnb_grammar_destroy": (C.c_int, [vp]),
+    "lnb_session_set_grammar": (C.c_int, [vp, C.c_int, vp, C.c_int]),
     "lnb_session_logprobs_read": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp]),
     "lnb_score": (C.c_int, [vp, i32p, C.c_int, C.c_int]),
     "lnb_session_copy_sequences": (C.c_int, [vp, C.c_int, i32p, i32p, C.c_int, C.c_int]),

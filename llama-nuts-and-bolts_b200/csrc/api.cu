@@ -27,9 +27,11 @@
 #include "sample.cuh"
 #include "logprob.cuh"
 #include "penalty.cuh"
+#include "grammar.cuh"
 #include "seqcopy.cuh"
 #include "pth.hpp"
 #include "tokenizer.hpp"
+#include "regex.hpp"
 
 namespace lnb {
 void build_rope_table(int dim, int end, double theta, bool use_scaled, std::vector<float>& out);
@@ -1067,6 +1069,26 @@ __global__ void publish_kernel(LnbDevState* st, int advance, int32_t* tok_out) {
 // words of a ragged call's row map [tokens | row_seq | row_pos | last row of each segment]: `rows` words each, <= 8 segments
 static size_t row_map_words(int max_rows) { return (size_t)max_rows * 3 + 8; }
 
+// a compiled grammar (grammar.cuh, lnb_grammar_create): its device tables, and the sequences of sessions that use it
+struct lnb_grammar {
+  lnb_model* m = nullptr;   // (compared, never dereferenced after creation: the model may be gone when the grammar is destroyed)
+  int device = 0;
+  GrammarDev d{};
+  int32_t* d_trans = nullptr;
+  uint32_t* d_masks = nullptr;
+  uint8_t* d_bytes = nullptr;
+  int64_t* d_off = nullptr;
+  int n_stuck = 0;
+  int64_t bytes = 0, build_ns = 0;
+  std::atomic<int> users{0};
+};
+// users of every grammar change under this lock, so lnb_grammar_destroy cannot free a grammar a session is taking up
+static std::mutex g_grammar_mu;
+static void grammar_release(const lnb_grammar* g) {
+  std::lock_guard<std::mutex> lk(g_grammar_mu);
+  const_cast<lnb_grammar*>(g)->users--;
+}
+
 struct lnb_session {
   lnb_model* m = nullptr;
   int seq_len = 0, max_rows = 1, mode = LNB_ACC_FAST;
@@ -1174,13 +1196,19 @@ struct lnb_session {
   int32_t* d_hist = nullptr;                // [n_seq][seq_len] the token fed at each position, -1: none
   lnb_penalties* d_pen = nullptr;           // [n_seq]
   unsigned int* d_pen_cnt = nullptr;        // [PEN_MAX_ROWS][vocab] (zero between jobs)
-  float* d_pen_out = nullptr;               // [PEN_MAX_ROWS][vocab] l', read by the sampler
+  float* d_pen_out = nullptr;               // [PEN_MAX_ROWS][vocab] l' (penalty and grammar jobs), read by the sampler
   bool pen_on[8] = {false, false, false, false, false, false, false, false};
   bool graph_pen = false, graph_greedy = false;   // the captured decode graph runs the penalty job / the greedy slot
+  // grammars (grammar.cuh, lnb_session_set_grammar), allocated by the first enable: the grammar state before every
+  // position of every sequence, and each sequence's grammar in device memory (a captured graph reads it there)
+  int32_t* d_gst = nullptr;                 // [n_seq][seq_len + 1], -1: ⊥
+  GrammarSlot* d_gslot = nullptr;           // [n_seq]
+  lnb_grammar* gram[8] = {};                // NULL: the sequence is not constrained
+  bool graph_gram = false;                  // the captured decode graph runs the grammar job
 };
 
-// a sequence whose tokens the sampler draws (sampled, or penalized: greedy is then the sampler's rank 0 of l')
-static bool processed(const lnb_session* s, int seq) { return s->samp_on[seq] || s->pen_on[seq]; }
+// a sequence whose tokens the sampler draws (sampled, penalized or constrained: greedy is then the sampler's rank 0 of l')
+static bool processed(const lnb_session* s, int seq) { return s->samp_on[seq] || s->pen_on[seq] || s->gram[seq]; }
 
 static int set_state(lnb_session* s, int pos, int n_rows, int next_token, bool reset_step) {
   return launch_kernel(Launcher{s->stream, LAUNCH_PLAIN, &s->launches}, set_state_kernel, dim3(1), dim3(1), 0, s->st, pos, n_rows,
@@ -1324,6 +1352,9 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->d_lp_rec); cudaFree(s->d_lp_top); cudaFree(s->d_lp_tgt); cudaFree(s->d_lp_rows); cudaFree(s->d_lp_cand);
   if (s->h_lp_rows) cudaFreeHost(s->h_lp_rows);
   cudaFree(s->d_hist); cudaFree(s->d_pen); cudaFree(s->d_pen_cnt); cudaFree(s->d_pen_out);
+  cudaFree(s->d_gst); cudaFree(s->d_gslot);
+  for (int q = 0; q < 8; q++)
+    if (s->gram[q]) grammar_release(s->gram[q]);
   for (auto p : s->ck) cudaFree(p);
   for (auto p : s->cv) cudaFree(p);
   if (s->h_tok) cudaFreeHost(s->h_tok);
@@ -2004,6 +2035,7 @@ struct Rows {
   bool advance;             // the LM head advances st->pos and appends the token to d_tok_out (device-driven decode)
   bool gather;              // tensor-parallel: the kept logits are all-gathered for the host
   bool record;              // a row's sequence is penalized: the forward records every row's token in d_hist
+  bool grammar;             // a row's sequence is constrained: the forward advances its grammar state in d_gst
 };
 // rows 0..S-1 of the active sequence at st->pos + r.  tokens: device ids, or NULL for st->next_token.  logits_rows: logits
 // kept, 0 = none, 1 = the last row, S = all rows.
@@ -2015,6 +2047,7 @@ static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int 
   R.head_rows = logits_rows > 1 ? S : 1;
   R.advance = advance; R.gather = gather;
   R.record = s->pen_on[s->active_seq];
+  R.grammar = s->gram[s->active_seq] != nullptr;
   return R;
 }
 // a batched step: row r is sequence r, token d_tokens[r] at position d_pos_arr[r]
@@ -2023,29 +2056,29 @@ static Rows rows_batch(const lnb_session* s, int n) {
   R.kind = ROWS_BATCH; R.S = n; R.tokens = s->d_tokens; R.pos_arr = s->d_pos_arr;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.head = HEAD_PER_ROW; R.head_rows = n;
-  for (int i = 0; i < n; i++) R.record |= s->pen_on[i];
+  for (int i = 0; i < n; i++) { R.record |= s->pen_on[i]; R.grammar |= s->gram[i] != nullptr; }
   return R;
 }
 // a ragged call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each, then the last row of each segment
-static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, bool record) {
+static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, bool record, bool grammar) {
   Rows R{};
   R.kind = ROWS_RAGGED; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.mb_rows = 8;
   R.seg_last = s->d_rag + 3 * rows;
   R.head = HEAD_PER_ROW; R.head_rows = n_segs;
-  R.record = record;
+  R.record = record; R.grammar = grammar;
   return R;
 }
 // a speculative verification call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each; consecutive
 // rows of a segment are consecutive positions of one sequence, and EVERY row is an output row (its next token is compared
 // with the following draft), so the LM head runs over all of them
-static Rows rows_spec(const lnb_session* s, int rows, bool record) {
+static Rows rows_spec(const lnb_session* s, int rows, bool record, bool grammar) {
   Rows R{};
   R.kind = ROWS_SPEC; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.head = HEAD_PER_ROW; R.head_rows = rows;
-  R.record = record;
+  R.record = record; R.grammar = grammar;
   return R;
 }
 
@@ -2128,13 +2161,21 @@ static bool forward_tc_ok(const lnb_session* s, int S) {
 }
 static int enqueue_forward_tc(lnb_session* s, const Rows& R);
 
-// The history write of a forward over the rows R (R.record: a row's sequence is penalized), before anything advances
-// st->pos.  token / pos0 (>= 0): the one row's token and position when they ride in a launch argument (the decode engine).
+// The history writes of a forward over the rows R (R.record: a row's sequence is penalized; R.grammar: constrained), before
+// anything advances st->pos.  token / pos0 (>= 0): the one row's token and position when they ride in a launch argument
+// (the decode engine).
 static int launch_record(lnb_session* s, const Rows& R, int32_t token = -1, int pos0 = -1) {
-  if (!R.record) return 0;
-  return launch_kernel(Launcher{s->stream, LAUNCH_PDL, &s->launches}, penalty_record_kernel, dim3((R.S + 255) / 256), dim3(256), 0,
-                       s->d_hist, s->seq_len, (const LnbDevState*)s->st, R.tokens, R.pos_arr, R.row_seq,
-                       R.kind == ROWS_SINGLE ? s->active_seq : -1, token, pos0, R.S);
+  const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
+  const int seq = R.kind == ROWS_SINGLE ? s->active_seq : -1;
+  if (R.record) {
+    const int rc = launch_kernel(L, penalty_record_kernel, dim3((R.S + 255) / 256), dim3(256), 0, s->d_hist, s->seq_len,
+                                 (const LnbDevState*)s->st, R.tokens, R.pos_arr, R.row_seq, seq, token, pos0, R.S);
+    if (rc) return rc;
+  }
+  if (!R.grammar) return 0;
+  return launch_kernel(L, grammar_record_kernel, dim3((R.S + 255) / 256), dim3(256), 0, s->d_gst, s->seq_len + 1,
+                       (const GrammarSlot*)s->d_gslot, (const LnbDevState*)s->st, R.tokens, R.pos_arr, R.row_seq, seq, token,
+                       pos0, R.S);
 }
 
 // Enqueue one LlamaTransformer.Forward (llamatransformer.go:145-180) for the rows R on the session stream: on the tensor
@@ -2332,8 +2373,10 @@ static int launch_penalty_job(const Launcher& L, const PenaltyJob& J) {
 // One sampler launch over n rows of s->logits: row[i] of sequence seq[i] draws with p_next[i] (-1: st->pos, for a decode
 // run whose step has advanced) into out[out_idx[i]]; decode: the token also feeds the next step (st->next_token) and
 // lands in d_tok_out.  Only calls with a processed row launch it.  When a row is penalized, the penalty job first writes
-// every row to d_pen_out (rows of other sequences unchanged) and the sampler reads them there; a penalized sequence that
-// does not sample draws from the greedy slot d_samp[n_seq] (temperature 0: rank 0 of l').
+// every row to d_pen_out (rows of other sequences unchanged); when a row is constrained, the grammar job then masks it there
+// (in place after the penalty job, else writing every row from the logits), and the sampler reads them there.  A
+// penalized or constrained sequence that does not sample draws from the greedy slot d_samp[n_seq] (temperature 0: rank 0
+// of l').
 static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_t* seq, const int32_t* p_next, const int32_t* out_idx,
                          int32_t* out, bool decode) {
   const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
@@ -2343,10 +2386,11 @@ static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_
   J.params = s->d_samp; J.wbuf = s->d_samp_w; J.pos_ptr = &s->st->pos; J.out = out;
   J.cand = s->d_samp_cand; J.cnt = reinterpret_cast<unsigned int*>(s->d_samp_cand + (size_t)s->samp_rows * SMP_MERGE);
   J.st = decode ? s->st : nullptr; J.tok_out = decode ? s->d_tok_out : nullptr;
-  bool pen = false;
+  bool pen = false, gram = false;
   for (int i = 0; i < n; i++) {
     J.row[i] = row[i]; J.slot[i] = s->samp_on[seq[i]] ? seq[i] : s->n_seq; J.p_next[i] = p_next[i]; J.out_idx[i] = out_idx ? out_idx[i] : 0;
     pen |= s->pen_on[seq[i]];
+    gram |= s->gram[seq[i]] != nullptr;
   }
   if (pen) {
     PenaltyJob P{};
@@ -2358,6 +2402,18 @@ static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_
       J.row[i] = i;
     }
     int rc = launch_penalty_job(L, P);
+    if (rc) return rc;
+    J.logits = s->d_pen_out; J.ld = V;
+  }
+  if (gram) {
+    GrammarJob G{};
+    G.in = pen ? s->d_pen_out : s->logits; G.ld = pen ? V : s->m->vocab_l; G.out = s->d_pen_out; G.V = V; G.n = n;
+    G.slots = s->d_gslot; G.gst = s->d_gst; G.gst_len = s->seq_len + 1; G.pos_ptr = &s->st->pos;
+    for (int i = 0; i < n; i++) {
+      G.row[i] = pen ? i : row[i]; G.seq[i] = seq[i]; G.p_next[i] = p_next[i]; G.on[i] = s->gram[seq[i]] ? 1 : 0;
+      J.row[i] = i;
+    }
+    int rc = launch_kernel(L, grammar_apply_kernel, dim3((V + GRM_SLICE - 1) / GRM_SLICE, n), dim3(GRM_THREADS), 0, G);
     if (rc) return rc;
     J.logits = s->d_pen_out; J.ld = V;
   }
@@ -2704,24 +2760,26 @@ extern "C" int lnb_session_set_penalties(lnb_session* s, int seq, const lnb_pena
     int32_t* d_hist = nullptr;
     lnb_penalties* d_par = nullptr;
     unsigned int* d_cnt = nullptr;
-    float* d_out = nullptr;
+    float* d_out = s->d_pen_out;   // (the processed rows: allocated here or by the first grammar enable)
     cudaError_t e = cudaMalloc((void**)&d_hist, b_hist);
     if (e == cudaSuccess) e = cudaMalloc((void**)&d_par, b_par);
     if (e == cudaSuccess) e = cudaMalloc((void**)&d_cnt, b_cnt);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_out, b_out);
+    if (e == cudaSuccess && !d_out) e = cudaMalloc((void**)&d_out, b_out);
     if (e == cudaSuccess) e = cudaMemsetAsync(d_hist, 0xff, b_hist, s->stream);   // -1: no token recorded
     if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt, 0, b_cnt, s->stream);        // the counts start at 0
     if (e != cudaSuccess) {
       cudaGetLastError();
       cudaStreamSynchronize(s->stream);
-      cudaFree(d_hist); cudaFree(d_par); cudaFree(d_cnt); cudaFree(d_out);
+      cudaFree(d_hist); cudaFree(d_par); cudaFree(d_cnt);
+      if (d_out != s->d_pen_out) cudaFree(d_out);
       cudaGetLastError();
       return fail(LNB_ENOMEM, "penalty history and scratch: %zu bytes of device memory asked for (history %zu): %s",
                   b_hist + b_par + b_cnt + b_out, b_hist, cudaGetErrorString(e));
     }
     if ((rc = samp_alloc(s))) {   // the sampler draws every penalized token
       cudaStreamSynchronize(s->stream);
-      cudaFree(d_hist); cudaFree(d_par); cudaFree(d_cnt); cudaFree(d_out);
+      cudaFree(d_hist); cudaFree(d_par); cudaFree(d_cnt);
+      if (d_out != s->d_pen_out) cudaFree(d_out);
       return rc;
     }
     s->d_hist = d_hist; s->d_pen = d_par; s->d_pen_cnt = d_cnt; s->d_pen_out = d_out;
@@ -2734,6 +2792,199 @@ extern "C" int lnb_session_set_penalties(lnb_session* s, int seq, const lnb_pena
     CU(cudaGetLastError());
   }
   s->pen_on[seq] = on;
+  return 0;
+}
+
+// ---- grammars (regex.cpp, grammar.cuh, DESIGN.md §9g) ------------------------------------------------------------------
+extern "C" int lnb_regex_dfa(const char* pattern, int64_t len, int32_t* trans, uint8_t* accept, int cap, int* n_states) {
+  if (!pattern || !trans || !accept || !n_states || len < 0 || cap < 1) return fail(LNB_EINVAL, "bad argument");
+  std::vector<int32_t> t;
+  std::vector<uint8_t> a;
+  std::string err;
+  int Q = 0;
+  const bool ok = regex_dfa(pattern, len, LNB_GRAMMAR_MAX_STATES, t, a, err, &Q);
+  *n_states = Q;
+  if (!ok) return fail(LNB_EINVAL, "%s", err.c_str());
+  if (Q > cap) return fail(LNB_EINVAL, "regex: the minimal DFA has %d states, more than cap %d", Q, cap);
+  memcpy(trans, t.data(), t.size() * 4);
+  memcpy(accept, a.data(), a.size());
+  return 0;
+}
+
+static void grammar_free(lnb_grammar* g) {
+  cudaFree(g->d_trans); cudaFree(g->d_masks); cudaFree(g->d_bytes); cudaFree(g->d_off);
+  delete g;
+}
+
+extern "C" int lnb_grammar_create(lnb_model* m, const char* regex, int64_t len, const uint8_t* tok_bytes, const int64_t* tok_off,
+                                  const int32_t* stop_ids, int n_stop, lnb_grammar** out) {
+  if (!m || !regex || !tok_off || !stop_ids || !out || len < 0) return fail(LNB_EINVAL, "NULL argument");
+  const int V = m->a.vocab_size, W = (V + 31) / 32;
+  if (n_stop < 1) return fail(LNB_EINVAL, "n_stop %d: a grammar needs at least one stop token", n_stop);
+  if (tok_off[0] != 0) return fail(LNB_EINVAL, "tok_off[0] = %lld must be 0", (long long)tok_off[0]);
+  for (int t = 0; t < V; t++)
+    if (tok_off[t + 1] < tok_off[t]) return fail(LNB_EINVAL, "tok_off[%d] < tok_off[%d]", t + 1, t);
+  const int64_t nb = tok_off[V];
+  if (nb > 0 && !tok_bytes) return fail(LNB_EINVAL, "tok_bytes is NULL");
+  std::vector<uint32_t> Z(W, 0u);
+  for (int i = 0; i < n_stop; i++) {
+    if (stop_ids[i] < 0 || stop_ids[i] >= V) return fail(LNB_EINVAL, "stop_ids[%d] = %d outside [0, %d)", i, stop_ids[i], V);
+    Z[stop_ids[i] >> 5] |= 1u << (stop_ids[i] & 31);
+  }
+  std::vector<int32_t> trans;
+  std::vector<uint8_t> accept;
+  std::string err;
+  if (!regex_dfa(regex, len, LNB_GRAMMAR_MAX_STATES, trans, accept, err)) return fail(LNB_EINVAL, "%s", err.c_str());
+  const int Q = (int)accept.size();
+  CU(cudaSetDevice(m->device));
+  lnb_grammar* g = new lnb_grammar();
+  g->m = m;
+  g->device = m->device;
+  const size_t b_trans = trans.size() * 4, b_masks = (size_t)(Q + 1) * W * 4, b_bytes = (size_t)std::max<int64_t>(nb, 1),
+               b_off = (size_t)(V + 1) * 8;
+  g->bytes = (int64_t)(b_trans + b_masks + b_bytes + b_off);
+  uint8_t* d_accept = nullptr;
+  unsigned int* d_stuck = nullptr;
+  cudaStream_t st = nullptr;
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  cudaError_t e = cudaMalloc((void**)&g->d_trans, b_trans);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&g->d_masks, b_masks);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&g->d_bytes, b_bytes);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&g->d_off, b_off);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&d_accept, Q + 4);
+  if (e == cudaSuccess) e = cudaMalloc((void**)&d_stuck, 4);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    cudaFree(d_accept); cudaFree(d_stuck);
+    grammar_free(g);
+    return fail(LNB_ENOMEM, "grammar tables: %lld bytes of device memory asked for (masks %zu): %s", (long long)(g->bytes + Q + 4),
+                b_masks, cudaGetErrorString(e));
+  }
+  int rc = 0;
+  auto run = [&]() -> int {
+    CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    CU(cudaEventCreate(&e0));
+    CU(cudaEventCreate(&e1));
+    CU(cudaMemcpyAsync(g->d_trans, trans.data(), b_trans, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(g->d_masks + (size_t)Q * W, Z.data(), (size_t)W * 4, cudaMemcpyHostToDevice, st));
+    if (nb > 0) CU(cudaMemcpyAsync(g->d_bytes, tok_bytes, (size_t)nb, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(g->d_off, tok_off, b_off, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_accept, accept.data(), Q, cudaMemcpyHostToDevice, st));
+    CU(cudaMemsetAsync(d_stuck, 0, 4, st));
+    g->d = GrammarDev{g->d_trans, g->d_masks, g->d_bytes, g->d_off, Q, W, V};
+    CU(cudaEventRecord(e0, st));
+    int r = launch_kernel(Launcher{st, LAUNCH_PDL, nullptr}, grammar_mask_kernel,
+                          dim3((Q + GRM_BUILD_STATES - 1) / GRM_BUILD_STATES), dim3(GRM_BUILD_THREADS), 0, g->d,
+                          (const uint8_t*)d_accept, g->d_masks, d_stuck);
+    if (r) return r;
+    CU(cudaEventRecord(e1, st));
+    unsigned int stuck = 0;
+    CU(cudaMemcpyAsync(&stuck, d_stuck, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, e0, e1));
+    g->n_stuck = (int)stuck;
+    g->build_ns = (int64_t)llround((double)ms * 1e6);
+    return 0;
+  };
+  rc = run();
+  if (st) cudaStreamSynchronize(st);
+  if (e0) cudaEventDestroy(e0);
+  if (e1) cudaEventDestroy(e1);
+  if (st) cudaStreamDestroy(st);
+  cudaFree(d_accept); cudaFree(d_stuck);
+  if (rc) { grammar_free(g); return rc; }
+  *out = g;
+  return 0;
+}
+
+extern "C" int lnb_grammar_info(const lnb_grammar* g, int64_t* info) {
+  if (!g || !info) return fail(LNB_EINVAL, "NULL argument");
+  info[0] = g->d.Q; info[1] = g->n_stuck; info[2] = g->bytes; info[3] = g->build_ns;
+  return 0;
+}
+
+extern "C" int lnb_grammar_read_mask(const lnb_grammar* g, int state, uint32_t* out) {
+  if (!g || !out) return fail(LNB_EINVAL, "NULL argument");
+  if (state < -1 || state >= g->d.Q) return fail(LNB_EINVAL, "state %d outside [-1, %d)", state, g->d.Q);
+  CU(cudaSetDevice(g->device));
+  const int row = state < 0 ? g->d.Q : state;
+  CU(cudaMemcpy(out, g->d_masks + (size_t)row * g->d.W, (size_t)g->d.W * 4, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+extern "C" int lnb_grammar_destroy(lnb_grammar* g) {
+  if (!g) return 0;
+  {
+    std::lock_guard<std::mutex> lk(g_grammar_mu);
+    if (g->users > 0) return fail(LNB_ESTATE, "the grammar is still used by %d session sequence(s)", g->users.load());
+  }
+  cudaSetDevice(g->device);
+  grammar_free(g);
+  return 0;
+}
+
+extern "C" int lnb_session_set_grammar(lnb_session* s, int seq, const lnb_grammar* g, int first_pos) {
+  if (!s) return fail(LNB_EINVAL, "session is NULL");
+  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  if (s->m->tp_size > 1)
+    return fail(LNB_EINVAL, "grammars are not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", s->m->tp_size);
+  if (g && g->m != s->m) return fail(LNB_EINVAL, "the grammar was created for another model");
+  if (g && (first_pos < 0 || first_pos > s->seq_len)) return fail(LNB_EINVAL, "first_pos %d outside [0, %d]", first_pos, s->seq_len);
+  const int V = s->m->a.vocab_size;
+  int rc;
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(s->m->device));
+  if (g && !s->d_gst) {   // state history of every sequence and position, slots, processed rows; all or nothing
+    const size_t b_gst = (size_t)s->n_seq * (s->seq_len + 1) * 4, b_slot = (size_t)s->n_seq * sizeof(GrammarSlot),
+                 b_out = s->d_pen_out ? 0 : (size_t)PEN_MAX_ROWS * V * 4;
+    int32_t* d_gst = nullptr;
+    GrammarSlot* d_slot = nullptr;
+    float* d_out = s->d_pen_out;
+    cudaError_t e = cudaMalloc((void**)&d_gst, b_gst);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&d_slot, b_slot);
+    if (e == cudaSuccess && !d_out) e = cudaMalloc((void**)&d_out, b_out);
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_gst, 0xff, b_gst, s->stream);    // -1: ⊥
+    if (e == cudaSuccess) e = cudaMemsetAsync(d_slot, 0, b_slot, s->stream);     // no grammar
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      cudaStreamSynchronize(s->stream);
+      cudaFree(d_gst); cudaFree(d_slot);
+      if (d_out != s->d_pen_out) cudaFree(d_out);
+      cudaGetLastError();
+      return fail(LNB_ENOMEM, "grammar state history and slots: %zu bytes of device memory asked for (history %zu): %s",
+                  b_gst + b_slot + b_out, b_gst, cudaGetErrorString(e));
+    }
+    if ((rc = samp_alloc(s))) {   // the sampler draws every constrained token
+      cudaStreamSynchronize(s->stream);
+      cudaFree(d_gst); cudaFree(d_slot);
+      if (d_out != s->d_pen_out) cudaFree(d_out);
+      return rc;
+    }
+    s->d_gst = d_gst; s->d_gslot = d_slot; s->d_pen_out = d_out;
+  } else if (g && (rc = samp_alloc(s))) {
+    return rc;
+  }
+  if (s->d_gslot) {   // stream-ordered, no host synchronisation; a captured decode graph reads the slot when it replays
+    GrammarSlot v{};
+    int32_t* first = nullptr;
+    if (g) {
+      v.g = g->d; v.first_pos = first_pos;
+      // g[first_pos] = q0 and every later state ⊥: states recorded before this call (another grammar's, or walks of tokens
+      // fed before it) are never read.  Tokens already fed at positions >= first_pos are not walked: the caller feeds them
+      // again (lnb.h)
+      first = s->d_gst + (size_t)seq * (s->seq_len + 1) + first_pos;
+      if (first_pos < s->seq_len) CU(cudaMemsetAsync(first + 1, 0xff, (size_t)(s->seq_len - first_pos) * 4, s->stream));
+    }
+    grammar_set_slot_kernel<<<1, 1, 0, s->stream>>>(s->d_gslot + seq, v, first);
+    CU(cudaGetLastError());
+  }
+  {
+    std::lock_guard<std::mutex> lk(g_grammar_mu);
+    if (g) const_cast<lnb_grammar*>(g)->users++;
+    if (s->gram[seq]) const_cast<lnb_grammar*>(s->gram[seq])->users--;
+  }
+  s->gram[seq] = const_cast<lnb_grammar*>(g);
   return 0;
 }
 
@@ -2994,9 +3245,9 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
     h[3 * rows + i] = r - 1;
   }
   CU(cudaMemcpyAsync(s->d_rag, h, (size_t)(3 * rows + n_segs) * 4, cudaMemcpyHostToDevice, s->stream));
-  bool pen = false;
-  for (int i = 0; i < n_segs; i++) pen |= s->pen_on[seq[i]];
-  if ((rc = enqueue_forward(s, rows_ragged(s, rows, n_segs, pen)))) return rc;
+  bool pen = false, gram = false;
+  for (int i = 0; i < n_segs; i++) { pen |= s->pen_on[seq[i]]; gram |= s->gram[seq[i]] != nullptr; }
+  if ((rc = enqueue_forward(s, rows_ragged(s, rows, n_segs, pen, gram)))) return rc;
   int32_t p_next[8];
   for (int i = 0; i < n_segs; i++) p_next[i] = start_pos[i] + len[i];
   if ((rc = call_tail(s, n_segs, 0, seq, p_next, s->d_next_arr, s->d_next_arr, logits, n_segs, argmax_out ? s->d_next_arr : nullptr))) return rc;
@@ -3073,13 +3324,14 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
   if (!eng && !s->sdpa_smem_decode && !s->ss.sc)
     return fail(LNB_EINVAL, "speculative calls beyond the shared-memory attention kernel need head_dim <= 128 and n_rep <= 8");
   int32_t row_seq[8], row_pos[8];
-  bool samp = false, lp = false, pen = false;
+  bool samp = false, lp = false, pen = false, gram = false;
   for (int i = 0, r = 0; i < n_segs; i++)
     for (int k = 0; k <= n_draft[i]; k++, r++) {
       row_seq[r] = seq[i];
       row_pos[r] = start_pos[i] + k;
       samp |= processed(s, seq[i]);
       pen |= s->pen_on[seq[i]];
+      gram |= s->gram[seq[i]] != nullptr;
       lp |= s->lp_top[seq[i]] >= 0;
     }
   if (!s->d_rag) {   // the row map (shared with ragged calls)
@@ -3102,12 +3354,12 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
   CU(cudaMemcpyAsync(s->d_rag, h, (size_t)3 * rows * 4, cudaMemcpyHostToDevice, s->stream));
   if (eng) {
     // ONE launch of the batch engine: every weight matrix streamed once for all rows
-    if ((rc = launch_record(s, rows_spec(s, rows, pen)))) return rc;
+    if ((rc = launch_record(s, rows_spec(s, rows, pen, gram)))) return rc;
     if ((rc = batch_engine_build(s, (logits || samp || lp) ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, rows, s->d_rag, s->d_rag + 2 * rows, s->d_rag + rows))) return rc;
   } else {
     if ((rc = set_state(s, 0, rows, -1, false))) return rc;
-    if ((rc = enqueue_forward(s, rows_spec(s, rows, pen)))) return rc;
+    if ((rc = enqueue_forward(s, rows_spec(s, rows, pen, gram)))) return rc;
   }
   int32_t p_next[8];
   for (int r = 0; r < rows; r++) p_next[r] = row_pos[r] + 1;
@@ -3135,13 +3387,16 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
   // a sampled sequence decodes on the kernel chain (the persistent engine feeds back the greedy token inside the kernel):
   // each step keeps its logits row and ends in the sampler, whose token is the next step's input.  A sequence with
   // logprobs on decodes on the chain too, each step then ending in the logprob job keyed on st->pos (= p_next).  A
-  // penalized sequence records its token, runs the penalty job and draws from the sampler (greedy: its rank 0) each step.
+  // penalized sequence records its token, runs the penalty job and draws from the sampler (greedy: its rank 0) each step; a
+  // constrained one advances its grammar state and masks the row the same way.
   const int seq = s->active_seq;
-  const bool pen = s->pen_on[seq], samp = processed(s, seq), greedy_slot = samp && !s->samp_on[seq];
+  const bool pen = s->pen_on[seq], gram = s->gram[seq] != nullptr, samp = processed(s, seq), greedy_slot = samp && !s->samp_on[seq];
   const bool lp = s->lp_top[seq] >= 0, keep = samp || lp;
   if (s->samp_on[seq] && engine_ok(s)) g_err = "the active sequence samples: lnb_decode_run runs the kernel chain (the decode engine has no sampler)";
   else if (pen && engine_ok(s))
     g_err = "the active sequence is penalized: lnb_decode_run runs the kernel chain (the decode engine keeps no token history)";
+  else if (gram && engine_ok(s))
+    g_err = "the active sequence is constrained by a grammar: lnb_decode_run runs the kernel chain (the decode engine keeps no grammar state)";
   else if (lp && engine_ok(s))
     g_err = "the active sequence has logprobs on: lnb_decode_run runs the kernel chain (the decode engine keeps no logits row)";
   if (!keep && engine_ok(s)) {
@@ -3161,7 +3416,8 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     return use_graph ? 1 : 0;   // (no graph is needed: there is nothing left to replay)
   }
   if (keep && (rc = ensure_logits(s, 1))) return rc;
-  if (s->graph_tried && (s->graph_sampled != samp || s->graph_lp != lp || s->graph_pen != pen || s->graph_greedy != greedy_slot ||
+  if (s->graph_tried && (s->graph_sampled != samp || s->graph_lp != lp || s->graph_pen != pen || s->graph_gram != gram ||
+                         s->graph_greedy != greedy_slot ||
                          (keep && s->graph_logits != s->logits)))
     drop_graph(s);
   if (lp) {   // the job's one row, read by every step (and by the graph's replays): the token st->next_token, record st->pos
@@ -3180,6 +3436,7 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     s->graph_sampled = samp;
     s->graph_lp = lp;
     s->graph_pen = pen;
+    s->graph_gram = gram;
     s->graph_greedy = greedy_slot;
     s->graph_logits = s->logits;
     cudaGraph_t g = nullptr;

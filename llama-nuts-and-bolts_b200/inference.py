@@ -156,6 +156,13 @@ def _logprob_lists(infContext, seqs, logprobs: int | None, logprobs_out: list | 
     return lists
 
 
+def _set_grammar(infContext, seq: int, grammar, i: int, prompt_len: int):
+    """sequence `seq` of the context is constrained by `grammar` (one model.Grammar, or one per prompt: the i-th; None:
+    left off; a None entry of the list turns it off) from the end of its prompt of prompt_len tokens on"""
+    if grammar is not None:
+        infContext.set_grammar(seq, grammar[i] if isinstance(grammar, (list, tuple)) else grammar, prompt_len)
+
+
 def _set_penalties(infContext, seq: int, penalties: "PenaltyArgs | None", prompt_len: int):
     """sequence `seq` of the context is penalized with `penalties` for a prompt of prompt_len tokens (None: left off)"""
     if penalties is not None:
@@ -256,7 +263,7 @@ class InferenceEngine:
                        prefill_chunk: int = 0, sampling: "SamplingArgs | None" = None,
                        speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None,
                        logprobs: int | None = None, logprobs_out: list | None = None,
-                       penalties: "PenaltyArgs | None" = None):
+                       penalties: "PenaltyArgs | None" = None, grammar: "model_mod.Grammar | None" = None):
         """Generator over (state, token id) exactly like generatedTokensCh.
 
         use_reference_api=True goes through the reference-shaped calls of every iteration
@@ -281,12 +288,19 @@ class InferenceEngine:
 
         penalties (EXTENSION): PenaltyArgs, applied on the device to every emitted token's logits before the sampler (or
         the greedy pick); CountPrompt False starts the counted history at the prompt's length.  The records of logprobs
-        stay those of the raw distribution.  use_reference_api=True with penalties is an error."""
+        stay those of the raw distribution.  use_reference_api=True with penalties is an error.
+
+        grammar (EXTENSION): a model.Grammar; every emitted token is masked on the device to those the grammar allows
+        after the tokens emitted so far (DESIGN.md §9g), after the penalties and before the sampler.  The generated bytes
+        are then always a prefix of a string of the grammar's language, and a stop token ends them only after a complete
+        match.  use_reference_api=True with a grammar is an error."""
         sampling = _sampling_for(sampling, 0)
         if sampling is not None and use_reference_api:
             raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax (inference.go:207-216); it cannot sample")
         if penalties is not None and use_reference_api:
             raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax of the raw logits; it cannot apply penalties")
+        if grammar is not None and use_reference_api:
+            raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax of the raw logits; it cannot apply a grammar")
         _check_speculative(speculative, use_reference_api)
         infContext = self.CreateInferenceContext()
         try:
@@ -295,6 +309,7 @@ class InferenceEngine:
             lp_out = _logprob_lists(infContext, [0], logprobs, [logprobs_out])
             promptLength = len(promptTokens)
             _set_penalties(infContext, 0, penalties, promptLength)
+            _set_grammar(infContext, 0, grammar, 0, promptLength)
             if prefill_chunk > 0:
                 infContext.allow_chunked_prefill(True)
                 if prefill_chunk > infContext.max_rows:
@@ -349,15 +364,15 @@ class InferenceEngine:
 
     def GenerateBeams(self, promptTokens, beams: BeamSearchArgs, step_times: list | None = None,
                       sampling: "SamplingArgs | None" = None, penalties: "PenaltyArgs | None" = None,
-                      speculative: "SpeculativeArgs | None" = None) -> list:
+                      speculative: "SpeculativeArgs | None" = None, grammar: "model_mod.Grammar | None" = None) -> list:
         """EXTENSION: beam search (DESIGN.md §9f) over a session of NumBeams sequences.  The prompt is prefilled once on
         sequence 0 and forked to the other beams (lnb_session_copy_sequences); each step is one lnb_forward_batch, whose
         logprob records give every beam's top 2B candidates, and one copy moves each surviving beam's parent rows.  Returns
         the NumReturn best BeamHypothesis, best first.  Beam search is deterministic on the raw distribution: it takes no
-        sampling, penalties or speculation.  step_times gets the time of the prefill and of every step."""
-        if _sampling_for(sampling, 0) is not None or penalties is not None or speculative is not None:
-            raise ml.MlError("beam search ranks the raw distribution deterministically: it takes no sampling, penalties or "
-                             "speculative decoding")
+        sampling, penalties, grammar or speculation.  step_times gets the time of the prefill and of every step."""
+        if _sampling_for(sampling, 0) is not None or penalties is not None or speculative is not None or grammar is not None:
+            raise ml.MlError("beam search ranks the raw distribution deterministically: it takes no sampling, penalties, "
+                             "grammar or speculative decoding")
         B = int(beams.NumBeams)
         if not 1 <= B <= 8:
             raise ml.MlError(f"NumBeams {B} must be in [1, 8]")
@@ -484,7 +499,7 @@ class InferenceEngine:
     def GenerateTokensContinuous(self, prompts, slots: int = 8, step_tokens: int | None = None,
                                  step_times: list | None = None, sampling: "SamplingArgs | None" = None,
                                  logprobs: int | None = None, logprobs_out: list | None = None,
-                                 penalties: "PenaltyArgs | None" = None):
+                                 penalties: "PenaltyArgs | None" = None, grammar=None):
         """Continuous batching (EXTENSION, lnb_forward_ragged): any number of prompts through at most `slots` live
         sequences.  Every step is ONE forward whose rows may belong to different sequences: each decoding sequence gets
         its one row, the rest of the step's row budget (min(step_tokens, max_rows)) goes to prompt chunks, first in first
@@ -494,7 +509,8 @@ class InferenceEngine:
         what GenerateTokens(prompts[i]) yields (the bookkeeping of generateTokensInternal, inference.go:173-254).
         sampling: prompt i samples with Seed + i (the stream of GenerateTokens(prompts[i]) with that seed).
         logprobs / logprobs_out as in GenerateTokens: logprobs_out gets one list per prompt.  penalties as in GenerateTokens,
-        for every prompt (set again at each admission: its first_pos follows the admitted prompt)."""
+        for every prompt (set again at each admission: its first_pos follows the admitted prompt).  grammar: one
+        model.Grammar for every prompt or one per prompt (None entries: unconstrained), set at each admission."""
         if step_tokens is None:
             step_tokens = DEFAULT_STEP_TOKENS
         if not 1 <= slots <= 8:
@@ -508,13 +524,13 @@ class InferenceEngine:
             self.context_hook(infContext)
         try:
             yield from self._generate_continuous(infContext, prompts, slots, min(step_tokens, infContext.max_rows), step_times,
-                                                 sampling, logprobs, logprobs_out, penalties)
+                                                 sampling, logprobs, logprobs_out, penalties, grammar)
         finally:
             infContext.close()
 
     def _generate_continuous(self, infContext, prompts, slots: int, budget: int, step_times: list | None = None,
                              sampling: "SamplingArgs | None" = None, logprobs: int | None = None, logprobs_out: list | None = None,
-                             penalties: "PenaltyArgs | None" = None):
+                             penalties: "PenaltyArgs | None" = None, grammar=None):
         """the scheduler of GenerateTokensContinuous on a given context (anything with SequenceLength, forward_ragged and
         forward_batch, set_sampling when `sampling` samples, set_logprobs and read_logprobs when `logprobs` is set,
         set_penalties when `penalties` is set)"""
@@ -540,6 +556,7 @@ class InferenceEngine:
                     if sp is not None:   # before the prompt's first segment (the slot's previous prompt had another seed)
                         infContext.set_sampling(k, sp)
                     _set_penalties(infContext, k, penalties, len(prompts[slot[k]["i"]]))
+                    _set_grammar(infContext, k, grammar, slot[k]["i"], len(prompts[slot[k]["i"]]))
             decoding = [k for k in range(slots) if slot[k] is not None and slot[k]["cur"] is not None]
             prefilling = sorted((k for k in range(slots) if slot[k] is not None and slot[k]["cur"] is None),
                                 key=lambda k: slot[k]["order"])
@@ -592,7 +609,7 @@ class InferenceEngine:
     def GenerateTokensBatch(self, prompts, step_times: list | None = None, sampling: "SamplingArgs | None" = None,
                             speculative: "SpeculativeArgs | None" = None, spec_stats: list | None = None,
                             logprobs: int | None = None, logprobs_out: list | None = None,
-                            penalties: "PenaltyArgs | None" = None):
+                            penalties: "PenaltyArgs | None" = None, grammar=None):
         """The consumer `InferenceEngine.TokenizeBatch` (src/inference/tokenize.go:97-107) never got in the
         reference (SURVEY 8f-4): every prompt runs the loop of generateTokensInternal (:173-254) -- own
         InferenceContext / KV cache, own positions, own stop condition -- but all sequences advance together,
@@ -602,7 +619,8 @@ class InferenceEngine:
         speculative (EXTENSION): after the prompts, every call is one lnb_forward_speculative in which each unfinished
         sequence gets its row and the rest of the 8-row budget goes to prompt-lookup drafts in sequence order; the streams
         are the same.  spec_stats as in GenerateTokens; logprobs / logprobs_out as in GenerateTokens, logprobs_out gets one
-        list per prompt; penalties as in GenerateTokens, for every sequence."""
+        list per prompt; penalties as in GenerateTokens, for every sequence; grammar: one model.Grammar for every
+        sequence or one per prompt (None entries: unconstrained)."""
         _check_speculative(speculative)
         n = len(prompts)
         if n < 1:
@@ -613,7 +631,8 @@ class InferenceEngine:
                 lp0 = []
                 logprobs_out.append(lp0)
             for state, tok in self.GenerateTokens(prompts[0], sampling=sampling, speculative=speculative, spec_stats=spec_stats,
-                                                  logprobs=logprobs, logprobs_out=lp0, penalties=penalties):
+                                                  logprobs=logprobs, logprobs_out=lp0, penalties=penalties,
+                                                  grammar=grammar[0] if isinstance(grammar, (list, tuple)) else grammar):
                 yield 0, state, tok
             return
         infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
@@ -633,6 +652,7 @@ class InferenceEngine:
                 if sp is not None:
                     infContext.set_sampling(i, sp)
                 _set_penalties(infContext, i, penalties, len(prompts[i]))
+                _set_grammar(infContext, i, grammar, i, len(prompts[i]))
             lp_out = _logprob_lists(infContext, range(n), logprobs, logprobs_out, n)
             cur = [0] * n                                  # token fed next / position it is fed at
             pos = [0] * n

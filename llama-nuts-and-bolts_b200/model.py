@@ -210,6 +210,80 @@ class TokenLogprob:
     Top: list
 
 
+def regex_dfa(pattern: str | bytes):
+    """EXTENSION: lnb_regex_dfa -> (trans int32 [Q, 256], -1: no string of the language continues; accept uint8 [Q]).
+    The language is re.fullmatch(pattern, s, re.ASCII) over the UTF-8 encodings of s; state 0 is the start, and the DFA
+    is minimal and trimmed.  Unsupported syntax raises _capi.LnbError (LNB_EINVAL, the message gives the byte offset)."""
+    b = pattern.encode("utf-8") if isinstance(pattern, str) else bytes(pattern)
+    cap = _capi.LNB_GRAMMAR_MAX_STATES
+    trans = np.empty((cap, 256), np.int32)
+    accept = np.empty(cap, np.uint8)
+    q = C.c_int(0)
+    check(lib.lnb_regex_dfa(b, len(b), ptr(trans, _capi.i32p), accept.ctypes.data_as(C.POINTER(C.c_uint8)), cap, C.byref(q)))
+    return trans[:q.value].copy(), accept[:q.value].copy()
+
+
+def token_bytes_table(token_bytes) -> tuple:
+    """[bytes of token t] -> (uint8 concatenation, int64 offsets [V + 1]) as lnb_grammar_create takes them"""
+    off = np.zeros(len(token_bytes) + 1, np.int64)
+    off[1:] = np.cumsum([len(b) for b in token_bytes])
+    data = np.frombuffer(b"".join(token_bytes), np.uint8).copy() if off[-1] else np.zeros(1, np.uint8)
+    return data, off
+
+
+def vocabulary_token_bytes(vocabulary, n: int) -> list:
+    """the bytes of tokens 0 .. n-1 of a loaded vocabulary.Vocabulary: special tokens (the 256 after the mergeable ones)
+    and ids past the vocabulary are empty, so a grammar never emits them as text"""
+    n_merge = len(vocabulary) - 256
+    return [vocabulary.IdToToken(t) if t < n_merge else b"" for t in range(n)]
+
+
+class Grammar:
+    """EXTENSION: regex-constrained generation, lnb_grammar_create (DESIGN.md §9g).  Tokens a sequence emits after its
+    grammar's first position spell a prefix of a string of re.fullmatch(regex, s, re.ASCII), and a stop token can only
+    follow a complete match; once a stop token (or a token the caller feeds outside the grammar) is fed, only stop tokens
+    may follow.  The token bytes come from `vocabulary` (a loaded vocabulary.Vocabulary; Z = its StopTokenIds) or from
+    token_bytes / stop_ids directly.  The masks of every DFA state are built on the model's device, once."""
+
+    def __init__(self, model, regex: str | bytes, vocabulary=None, token_bytes=None, stop_ids=None):
+        transformer = getattr(model, "Transformer", model)
+        V = transformer.args.VocabSize
+        if vocabulary is not None:
+            token_bytes = vocabulary_token_bytes(vocabulary, V)
+            stop_ids = vocabulary.StopTokenIds
+        if token_bytes is None or stop_ids is None or len(token_bytes) != V:
+            raise ml.MlError(f"a grammar needs the bytes of all {V} tokens and the stop ids")
+        self.transformer = transformer
+        self.regex = regex
+        b = regex.encode("utf-8") if isinstance(regex, str) else bytes(regex)
+        data, off = token_bytes_table(token_bytes)
+        stop = np.ascontiguousarray(stop_ids, np.int32)
+        h = C.c_void_p()
+        check(lib.lnb_grammar_create(transformer.h, b, len(b), data.ctypes.data_as(C.POINTER(C.c_uint8)), ptr(off, _capi.i64p),
+                                     ptr(stop, _capi.i32p), int(stop.shape[0]), C.byref(h)))
+        self.h = h
+        info = self.info()
+        self.NumStates, self.W = info["states"], (V + 31) // 32
+
+    def info(self) -> dict:
+        """states Q, stuck (states whose mask is the stop set), device bytes, the mask build's device time in ns"""
+        out = np.zeros(4, np.int64)
+        check(lib.lnb_grammar_info(self.h, ptr(out, _capi.i64p)))
+        return dict(states=int(out[0]), stuck=int(out[1]), bytes=int(out[2]), build_ns=int(out[3]))
+
+    def read_mask(self, state: int) -> np.ndarray:
+        """mask(state) as uint32 words (bit t & 31 of word t >> 5); state -1: ⊥ (the stop set)"""
+        out = np.zeros(self.W, np.uint32)
+        check(lib.lnb_grammar_read_mask(self.h, state, out.ctypes.data_as(C.POINTER(C.c_uint32))))
+        return out
+
+    def close(self):
+        """LnbError (LNB_ESTATE) while a session's sequence still uses the grammar"""
+        if self.h:
+            check(lib.lnb_grammar_destroy(self.h))
+            self.h = None
+
+
 def _token_logprobs(recs) -> list:
     return [TokenLogprob(int(r.token), float(r.logprob), int(r.rank),
                          [(int(r.top_token[j]), float(r.top_logprob[j])) for j in range(r.n_top)]) for r in recs]
@@ -330,6 +404,11 @@ class InferenceContext:
         else:
             c = args.c(prompt_len)
             check(lib.lnb_session_set_penalties(self.h, seq, C.byref(c)))
+
+    def set_grammar(self, seq: int, grammar: "Grammar | None", first_pos: int = 0):
+        """EXTENSION: sequence `seq` is constrained by `grammar` (None: off) from its next forward on; the grammar's start
+        state is the state before position first_pos (typically the prompt's length)"""
+        check(lib.lnb_session_set_grammar(self.h, seq, None if grammar is None else grammar.h, int(first_pos)))
 
     def set_logprobs(self, seq: int, top_n: int | None):
         """EXTENSION: from its next forward on, every token sequence `seq` emits writes its logprob record (the raw model

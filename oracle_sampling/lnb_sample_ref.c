@@ -490,3 +490,122 @@ int orc_beam_search(const orc_model* m, int vocab, int n_layers, int kv_row, con
   free(o.logits); free(o.snap);
   return n;
 }
+
+/* ---- grammars (DESIGN.md §9g), written from the contract of include/lnb.h: brute-force masks and the state history ---- */
+/* a grammar's tables: trans[Q][256] (-1: ⊥), accept[Q], token t's bytes bytes[off[t] .. off[t+1]), the stop set */
+typedef struct {
+  const int32_t* trans;
+  const uint8_t* accept;
+  int Q;
+  const uint8_t* bytes;
+  const int64_t* off;
+  int V;
+  const int32_t* stop;
+  int n_stop;
+} orc_grammar;
+
+static int grm_is_stop(const orc_grammar* g, int32_t t) {
+  for (int i = 0; i < g->n_stop; i++)
+    if (g->stop[i] == t) return 1;
+  return 0;
+}
+/* δ*(q, b(t)) */
+static int grm_walk(const orc_grammar* g, int q, int32_t t) {
+  for (int64_t i = g->off[t]; i < g->off[t + 1] && q >= 0; i++) q = g->trans[(size_t)q * 256 + g->bytes[i]];
+  return q;
+}
+static int grm_text_allowed(const orc_grammar* g, int q, int32_t t) {
+  return q >= 0 && !grm_is_stop(g, t) && g->off[t + 1] > g->off[t] && grm_walk(g, q, t) >= 0;
+}
+/* the state after feeding t in q: δ*(q, b(t)) if t is an allowed text token in q, else ⊥ */
+static int grm_next(const orc_grammar* g, int q, int32_t t) {
+  return (t >= 0 && t < g->V && grm_text_allowed(g, q, t)) ? grm_walk(g, q, t) : -1;
+}
+/* mask(q) as a 0/1 byte per token (q = -1: ⊥) */
+static void grm_mask(const orc_grammar* g, int q, uint8_t* m) {
+  int any = 0;
+  for (int t = 0; t < g->V; t++) {
+    m[t] = q >= 0 && (grm_is_stop(g, t) ? g->accept[q] != 0 : grm_text_allowed(g, q, t));
+    any |= m[t];
+  }
+  if (!any)
+    for (int t = 0; t < g->V; t++) m[t] = (uint8_t)grm_is_stop(g, t);
+}
+
+/* every state's mask, rows 0..Q-1, then ⊥'s as row Q, as u32 words [Q + 1][ceil(V / 32)] (bit t & 31 of word t >> 5);
+ * returns the number of states whose mask is Z */
+int orc_grammar_masks(const int32_t* trans, const uint8_t* accept, int Q, const uint8_t* bytes, const int64_t* off, int V,
+                      const int32_t* stop, int n_stop, uint32_t* out) {
+  const orc_grammar g = {trans, accept, Q, bytes, off, V, stop, n_stop};
+  const int W = (V + 31) / 32;
+  int stuck = 0;
+#pragma omp parallel for reduction(+ : stuck) schedule(dynamic, 1)
+  for (int q = -1; q < Q; q++) {
+    uint8_t* m = (uint8_t*)malloc((size_t)V);
+    grm_mask(&g, q, m);
+    uint32_t* row = out + (size_t)(q < 0 ? Q : q) * W;
+    memset(row, 0, (size_t)W * 4);
+    int text = 0;
+    for (int t = 0; t < V; t++) {
+      if (m[t]) row[t >> 5] |= 1u << (t & 31);
+      text |= m[t] && !grm_is_stop(&g, t);
+    }
+    if (q >= 0 && !text && !accept[q]) stuck++;
+    free(m);
+  }
+  return stuck;
+}
+
+/* the state history of tokens[0 .. n) fed at positions 0 .. n-1 with the grammar starting at first_pos: hist[p] for
+ * p in [0, n], -1 (⊥) below first_pos */
+void orc_grammar_history(const int32_t* trans, const uint8_t* accept, int Q, const uint8_t* bytes, const int64_t* off, int V,
+                         const int32_t* stop, int n_stop, const int32_t* tokens, int n, int first_pos, int32_t* hist) {
+  const orc_grammar g = {trans, accept, Q, bytes, off, V, stop, n_stop};
+  for (int p = 0; p <= n; p++) hist[p] = -1;
+  if (first_pos > n) return;
+  hist[first_pos] = 0;
+  for (int p = first_pos; p < n; p++) hist[p + 1] = grm_next(&g, hist[p], tokens[p]);
+}
+
+/* orc_generate_processed with the grammar: the row that emits position p >= first_pos keeps the logits of mask(g[p]) only,
+ * between the penalties and the sampler */
+int orc_generate_constrained(const orc_model* m, int vocab, const int32_t* prompt, int n_prompt, int seq_len, const int32_t* stop_ids,
+                             int n_stop, float T, int32_t K, float P, uint64_t seed, const lnb_penalties* pen,
+                             const int32_t* trans, const uint8_t* accept, int Q, const uint8_t* bytes, const int64_t* off,
+                             const int32_t* grammar_stop, int n_grammar_stop, int first_pos, int32_t* out) {
+  if (n_prompt >= seq_len) return -1;
+  const orc_grammar g = {trans, accept, Q, bytes, off, vocab, grammar_stop, n_grammar_stop};
+  orc_session* s = orc_session_new(m, seq_len);
+  int32_t* tokens = (int32_t*)malloc((size_t)seq_len * 4);
+  int32_t* hist = (int32_t*)malloc((size_t)(seq_len + 1) * 4);
+  for (int i = 0; i < seq_len; i++) tokens[i] = -1;
+  for (int i = 0; i < n_prompt; i++) tokens[i] = prompt[i];
+  for (int p = 0; p <= seq_len; p++) hist[p] = -1;
+  if (first_pos <= seq_len) hist[first_pos] = 0;
+  float* logits = (float*)malloc((size_t)vocab * sizeof(float));
+  float* proc = (float*)malloc((size_t)vocab * sizeof(float));
+  uint8_t* mask = (uint8_t*)malloc((size_t)vocab);
+  int prev = 0, n_out = 0, walked = first_pos;   /* hist[first_pos .. walked] are known */
+  for (int cur = n_prompt; cur < seq_len; cur++) {
+    if (orc_forward(m, s, tokens + prev, cur - prev, prev, logits, 0, NULL) != 0) { n_out = -1; break; }
+    if (pen) orc_penalize_row(logits, vocab, pen, tokens, cur, proc);
+    else memcpy(proc, logits, (size_t)vocab * sizeof(float));
+    if (cur >= first_pos) {
+      for (; walked < cur; walked++) hist[walked + 1] = grm_next(&g, hist[walked], tokens[walked]);
+      grm_mask(&g, hist[cur], mask);
+      for (int t = 0; t < vocab; t++)
+        if (!mask[t]) proc[t] = -INFINITY;
+    }
+    const int32_t next = orc_sample_row(proc, vocab, T, K, P, seed, cur);
+    tokens[cur] = next;
+    out[n_out++] = next;
+    prev = cur;
+    int eos = 0;
+    for (int i = 0; i < n_stop; i++) eos |= (stop_ids[i] == next);
+    if (eos) break;
+    if (cur + 1 == seq_len) break;
+  }
+  free(tokens); free(hist); free(logits); free(proc); free(mask);
+  orc_session_free(s);
+  return n_out;
+}

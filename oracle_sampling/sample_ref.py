@@ -1,4 +1,4 @@
-"""ctypes binding of the sampler's sequential C statement (TEST INFRASTRUCTURE, NOT PRODUCT CODE; DESIGN.md §9b, §9e).
+"""ctypes binding of the sampler's sequential C statement (TEST INFRASTRUCTURE, NOT PRODUCT CODE; DESIGN.md §9b, §9e, §9g).
 
 Only tests/ and tools/ may import this module.  See lnb_sample_ref.c.
 """
@@ -74,6 +74,15 @@ def lib():
         L.orc_generate_processed.restype = C.c_int
         L.orc_generate_processed.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
                                              C.c_float, C.c_uint64, C.POINTER(Penalties), _i32p]
+        _u8p = C.POINTER(C.c_uint8)
+        L.orc_grammar_masks.restype = C.c_int
+        L.orc_grammar_masks.argtypes = [_i32p, _u8p, C.c_int, _u8p, _i64p, C.c_int, _i32p, C.c_int, C.POINTER(C.c_uint32)]
+        L.orc_grammar_history.restype = None
+        L.orc_grammar_history.argtypes = [_i32p, _u8p, C.c_int, _u8p, _i64p, C.c_int, _i32p, C.c_int, _i32p, C.c_int, C.c_int, _i32p]
+        L.orc_generate_constrained.restype = C.c_int
+        L.orc_generate_constrained.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
+                                               C.c_float, C.c_uint64, C.POINTER(Penalties), _i32p, _u8p, C.c_int, _u8p, _i64p,
+                                               _i32p, C.c_int, C.c_int, _i32p]
         L.orc_generate_sampled.restype = C.c_int
         L.orc_generate_sampled.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
                                            C.c_float, C.c_uint64, _i32p]
@@ -161,6 +170,58 @@ def generate_processed(om, prompt, seq_len: int, T: float, K: int, P: float, see
                                      C.byref(pen) if pen is not None else None, out.ctypes.data_as(_i32p))
     if n < 0:
         raise RuntimeError("orc_generate_processed failed")
+    return out[:n].copy()
+
+
+# ---- grammars (DESIGN.md §9g) -----------------------------------------------------------------------------------------------
+class GrammarTables:
+    """a grammar as the C statement takes it: trans int32 [Q, 256] (-1: ⊥), accept [Q], the bytes of each of the V tokens,
+    the stop set"""
+
+    def __init__(self, trans, accept, token_bytes, stop_ids):
+        self.trans = np.ascontiguousarray(trans, np.int32)
+        self.accept = np.ascontiguousarray(accept, np.uint8)
+        self.Q = int(self.accept.shape[0])
+        self.V = len(token_bytes)
+        self.off = np.zeros(self.V + 1, np.int64)
+        self.off[1:] = np.cumsum([len(b) for b in token_bytes])
+        self.bytes = np.frombuffer(b"".join(token_bytes) + b"\0", np.uint8).copy()
+        self.stop = np.ascontiguousarray(stop_ids, np.int32)
+
+    def args(self):
+        u8 = C.POINTER(C.c_uint8)
+        return (self.trans.ctypes.data_as(_i32p), self.accept.ctypes.data_as(u8), self.Q, self.bytes.ctypes.data_as(u8),
+                self.off.ctypes.data_as(_i64p), self.V, self.stop.ctypes.data_as(_i32p), int(self.stop.shape[0]))
+
+
+def grammar_masks(g: GrammarTables) -> tuple:
+    """orc_grammar_masks: (uint32 [Q + 1, ceil(V / 32)], row Q = ⊥; the number of states whose mask is Z)"""
+    out = np.zeros((g.Q + 1, (g.V + 31) // 32), np.uint32)
+    stuck = lib().orc_grammar_masks(*g.args(), out.ctypes.data_as(C.POINTER(C.c_uint32)))
+    return out, int(stuck)
+
+
+def grammar_history(g: GrammarTables, tokens, first_pos: int) -> np.ndarray:
+    """orc_grammar_history: the state before each position 0 .. n of tokens fed at 0 .. n-1 (-1: ⊥)"""
+    t = np.ascontiguousarray(tokens, np.int32)
+    out = np.empty(t.shape[0] + 1, np.int32)
+    lib().orc_grammar_history(*g.args(), t.ctypes.data_as(_i32p), int(t.shape[0]), int(first_pos), out.ctypes.data_as(_i32p))
+    return out
+
+
+def generate_constrained(om, prompt, seq_len: int, T: float, K: int, P: float, seed: int, pen: "Penalties | None",
+                         g: GrammarTables, first_pos: int, stop_ids=(128008, 128009)) -> np.ndarray:
+    """orc_generate_processed with the grammar's mask between the penalties and the sampler (om: oracle.OracleModel)"""
+    prompt = np.ascontiguousarray(prompt, np.int32)
+    stop = np.ascontiguousarray(stop_ids, np.int32)
+    out = np.empty(seq_len, np.int32)
+    a = g.args()
+    n = lib().orc_generate_constrained(om.h, om.args.vocab, prompt.ctypes.data_as(_i32p), len(prompt), seq_len,
+                                       stop.ctypes.data_as(_i32p), len(stop), T, K, P, seed & (2**64 - 1),
+                                       C.byref(pen) if pen is not None else None, a[0], a[1], a[2], a[3], a[4], a[6], a[7],
+                                       int(first_pos), out.ctypes.data_as(_i32p))
+    if n < 0:
+        raise RuntimeError("orc_generate_constrained failed")
     return out[:n].copy()
 
 
