@@ -35,8 +35,10 @@ func lnbErr(rc C.int) error {
 type deviceModel struct{ h *C.lnb_model }
 type deviceSession struct{ h *C.lnb_session }
 
-// called at the end of NewLlamaTransformer, after every getTensor succeeded
-func newDeviceModel(args *ModelArgs, tensors map[string]*ml.Tensor, device, tpRank, tpSize int, ncclID []byte) (*deviceModel, error) {
+// called at the end of NewLlamaTransformer, after every getTensor succeeded.  weightFormat: C.LNB_WEIGHTS_BF16, or
+// C.LNB_WEIGHTS_MXFP8 to quantize the linear weights at finalize (tpSize 1 only)
+func newDeviceModel(args *ModelArgs, tensors map[string]*ml.Tensor, device, tpRank, tpSize int, ncclID []byte,
+	weightFormat int) (*deviceModel, error) {
 	ca := C.lnb_model_args{
 		dim: C.int32_t(args.Dim), n_layers: C.int32_t(args.N_Layers), n_heads: C.int32_t(args.N_Heads),
 		n_kv_heads: C.int32_t(args.N_KVHeads), head_dim: C.int32_t(args.HeadDim), ffn_dim: C.int32_t(args.FFNDim),
@@ -55,6 +57,10 @@ func newDeviceModel(args *ModelArgs, tensors map[string]*ml.Tensor, device, tpRa
 	if err := lnbErr(C.lnb_model_create(&ca, C.int(device), C.int(tpRank), C.int(tpSize), id, &dm.h)); err != nil {
 		return nil, err
 	}
+	if err := lnbErr(C.lnb_model_set_weight_format(dm.h, C.int(weightFormat))); err != nil {
+		C.lnb_model_destroy(dm.h)
+		return nil, err
+	}
 	for name, t := range tensors { // RawData aliases the checkpoint mmap (src/torch/types.go:51-56); the library copies it
 		cname := C.CString(name)
 		shape := make([]C.int64_t, len(t.Size))
@@ -70,6 +76,24 @@ func newDeviceModel(args *ModelArgs, tensors map[string]*ml.Tensor, device, tpRa
 	// the tables may also be uploaded from the Go-computed PrecomputedFreqsCis / TABLE_SILU:
 	// lnb_model_set_rope_table / lnb_model_set_silu_table; by default the library builds identical ones
 	return dm, lnbErr(C.lnb_model_finalize(dm.h))
+}
+
+// the E4M3 codes [rows*cols] and E8M0 scales [rows*ceil(cols/32)] of a linear tensor of an MXFP8 model (tests, tools)
+func (dm *deviceModel) mxfp8Read(name string, rows, cols int) ([]byte, []byte, error) {
+	codes := make([]byte, rows*cols)
+	scales := make([]byte, rows*((cols+31)/32))
+	cname := C.CString(name)
+	defer C.free(unsafe.Pointer(cname))
+	rc := C.lnb_model_mxfp8_read(dm.h, cname, (*C.uint8_t)(unsafe.Pointer(&codes[0])), (*C.uint8_t)(unsafe.Pointer(&scales[0])))
+	return codes, scales, lnbErr(rc)
+}
+
+// the format of the linear weights, the weight bytes held in HBM and the weight bytes one S = 1 step reads
+func (dm *deviceModel) weightInfo() (format int, deviceBytes, stepBytes int64, err error) {
+	var f C.int
+	var d, s C.int64_t
+	err = lnbErr(C.lnb_model_weight_info(dm.h, &f, &d, &s))
+	return int(f), int64(d), int64(s), err
 }
 
 func newDeviceSession(dm *deviceModel, inferenceArgs common.InferenceArgs, maxRows int, accMode int) (*deviceSession, error) {

@@ -22,6 +22,8 @@
 // (lnb_score): each token's logprob given the tokens before it, their sum and the perplexity exp(-mean).
 // prompt=TEXT (with <modelDir>/tokenizer.model): TEXT goes through the chat template and the BPE tokenizer, the
 // generated ids come back as text (cmd/main.go's flow without the console UI).
+// weights=mxfp8: the linear weights are quantized to MXFP8 at load (DESIGN §9h): half the weight bytes per step, and the
+// same ids as the bf16 model whose weights are the dequantized values.
 // <modelDir> holds params.json + consolidated.00.pth (model.LoadModel, src/model/loader.go:18-70);
 // `lnb_generate --write-synthetic <modelDir> [tiny]` writes such a directory for the synthetic weights (host-only).
 // `lnb_generate --tokenize <tokenizer.model> <text>` prints the chat-template token ids of <text> (host-only).
@@ -126,7 +128,7 @@ int main(int argc, char** argv) {
   const int seq_len = argc > 1 ? atoi(argv[1]) : 136;
   const int acc = (argc > 2 && !strcmp(argv[2], "fast")) ? LNB_ACC_FAST : LNB_ACC_STRICT;
   const bool tiny = argc > 3 && !strcmp(argv[3], "tiny");
-  const bool has_dir = argc > 3 && !tiny && strncmp(argv[3], "batch=", 6) != 0;
+  const bool has_dir = argc > 3 && !tiny && strncmp(argv[3], "batch=", 6) != 0 && strncmp(argv[3], "weights=", 8) != 0;
   try {
     model::ModelArgs args = model::ModelArgs::Llama31_8B();
     std::vector<int32_t> prompt{128000, 9906, 11, 856, 836, 374, 220, 16};
@@ -136,12 +138,18 @@ int main(int argc, char** argv) {
       prompt = {1, 50, 999, 7, 300, 12, 64, 2};
     }
     const bool from_dir = has_dir;
+    int weight_format = LNB_WEIGHTS_BF16;
+    for (int i = 3; i < argc; i++) {
+      if (!strcmp(argv[i], "weights=mxfp8")) weight_format = LNB_WEIGHTS_MXFP8;
+      else if (!strncmp(argv[i], "weights=", 8) && strcmp(argv[i], "weights=bf16")) throw lnb_host::Error(std::string("unknown ") + argv[i]);
+    }
     std::unique_ptr<model::LlamaTransformer> loaded;
     if (from_dir) {
-      loaded = model::LoadModel(argv[3], 0, 2048);
+      loaded = model::LoadModel(argv[3], 0, 2048, weight_format);
       if (loaded->args.vocab_size < 128256) prompt = {1, 50, 999, 7, 300, 12, 64, 2};
     } else {
       loaded = std::make_unique<model::LlamaTransformer>(args, 0);
+      loaded->SetWeightFormat(weight_format);
       loaded->InitSynthetic(tiny ? 7 : 0x4C4E42);
       loaded->Finalize();
     }

@@ -212,7 +212,24 @@ class LlamaTransformer {  // llamatransformer.go:16-113
     check(lnb_model_load_pth(h_, path.c_str(), &n));
     return n;
   }
+  // LNB_WEIGHTS_BF16 or LNB_WEIGHTS_MXFP8 (DESIGN §9h: Finalize quantizes the linear weights); before Finalize
+  void SetWeightFormat(int fmt) { check(lnb_model_set_weight_format(h_, fmt)); }
   void Finalize() { check(lnb_model_finalize(h_)); }
+  // MXFP8 model: the codes [rows][cols] and scales [rows][ceil(cols / 32)] of a linear checkpoint tensor
+  void MxFp8Read(const std::string& name, std::vector<uint8_t>& codes, std::vector<uint8_t>& scales, int64_t rows, int64_t cols) {
+    codes.resize((size_t)(rows * cols));
+    scales.resize((size_t)(rows * ((cols + 31) / 32)));
+    check(lnb_model_mxfp8_read(h_, name.c_str(), codes.data(), scales.data()));
+  }
+  struct WeightInfo {
+    int Format = LNB_WEIGHTS_BF16;
+    int64_t DeviceBytes = 0, StepBytes = 0;   // weight bytes in HBM; weight bytes one S = 1 step reads
+  };
+  WeightInfo GetWeightInfo() {
+    WeightInfo w;
+    check(lnb_model_weight_info(h_, &w.Format, &w.DeviceBytes, &w.StepBytes));
+    return w;
+  }
   lnb_model* handle() { return h_; }
 
  private:
@@ -271,8 +288,10 @@ inline ModelArgs LoadModelArgs(const std::string& modelDir, int maxSeqLen = 2048
 }
 
 // model.LoadModel (loader.go:18-70): <modelDir>/params.json + consolidated.00.pth -> a finalized transformer
-inline std::unique_ptr<LlamaTransformer> LoadModel(const std::string& modelDir, int device = 0, int maxSeqLen = 2048) {
+inline std::unique_ptr<LlamaTransformer> LoadModel(const std::string& modelDir, int device = 0, int maxSeqLen = 2048,
+                                                   int weightFormat = LNB_WEIGHTS_BF16) {
   auto t = std::make_unique<LlamaTransformer>(LoadModelArgs(modelDir, maxSeqLen), device);
+  t->SetWeightFormat(weightFormat);
   t->LoadPth(modelDir + "/consolidated.00.pth");
   t->Finalize();
   return t;

@@ -193,6 +193,27 @@ int lnb_model_destroy(lnb_model* m); /* hook for model.Model.Free (src/model/mod
  * per pass, N}.  Returns 1, or 0 when the engine streams bf16 (lnb_last_error says why).  The model must be finalized. */
 int lnb_model_wpack_read(lnb_model* m, int layer, uint8_t* data, uint8_t* units, uint16_t* src, int64_t* info);
 
+/* MXFP8 linear weights (DESIGN §9h).  With LNB_WEIGHTS_MXFP8, lnb_model_finalize quantizes wq, wk, wv, wo, w1, w2, w3 of
+ * every layer and output on the device and frees their bf16 copies (both are held during finalize); the embedding and the
+ * norms stay bf16.  Blocks of 32 columns of a row (the last one 16 wide when cols % 32 == 16) share one E8M0 scale X + 127
+ * with X = floor(log2(max |w|)) - 8 clamped to [-117, 119] (-117 for a zero block); each weight is the E4M3 code of
+ * w * 2^-X, round to nearest even, saturated to 448.  Every dequantized weight d = e4m3(code) * 2^X is a bf16 value, and
+ * every call on an MXFP8 model returns the bits the same call returns on the bf16 model with weights d.  A non-finite
+ * weight makes finalize return LNB_EINVAL naming the tensor, row and column.
+ * set_weight_format: before finalize (LNB_ESTATE after); LNB_EINVAL for an unknown format or tp_size > 1.
+ * The decode and batch engines and the STRICT packed stream read bf16 panels: MXFP8 sessions run the kernel chain, and
+ * lnb_session_decode_engine / lnb_model_wpack_read return 0 saying so.  FAST sessions with max_rows >= 32 hold a bf16
+ * scratch the size of the largest layer matrix for the tensor-core prompt path. */
+enum { LNB_WEIGHTS_BF16 = 0, LNB_WEIGHTS_MXFP8 = 1 };
+int lnb_model_set_weight_format(lnb_model* m, int fmt);
+/* the codes [rows][cols] and scales [rows][ceil(cols / 32)] of a linear checkpoint tensor, in the checkpoint's row order
+ * (either may be NULL); the model must be a finalized MXFP8 model */
+int lnb_model_mxfp8_read(lnb_model* m, const char* name, uint8_t* codes, uint8_t* scales);
+/* fmt = the format of the linear weights (bf16 until finalized); device_bytes = the weight bytes held in HBM (embedding,
+ * norms, linear weights with their scales); step_bytes = the weight bytes one single-GPU S = 1 step reads (every linear
+ * weight and norm once, one embedding row).  Any pointer may be NULL. */
+int lnb_model_weight_info(lnb_model* m, int* fmt, int64_t* device_bytes, int64_t* step_bytes);
+
 /* model.NewInferenceContext (src/model/inferencecontext.go:17-46): KV cache of seq_len rows
  * per layer, zero-filled.  max_rows = largest S a forward call may carry (>=1).
  * acc_mode = LNB_ACC_STRICT / LNB_ACC_FAST.

@@ -124,7 +124,10 @@ extern "C" int lnb_nccl_unique_id(void* out128) {
 // ------------------------------------------------------------------------------------------
 // model
 struct LayerW {
+  // the four projection matrices: bf16 panels, or after an MXFP8 finalize their E4M3 codes (mxfp8.cuh), whose scales are
+  // then in sqkv / so / s13 / s2 (NULL for bf16)
   uint16_t *attn_norm = nullptr, *wqkv = nullptr, *wo = nullptr, *ffn_norm = nullptr, *w13 = nullptr, *w2 = nullptr;
+  uint8_t *sqkv = nullptr, *so = nullptr, *s13 = nullptr, *s2 = nullptr;
   unsigned have = 0;  // bit per checkpoint tensor (9)
 };
 enum { T_ATTN_NORM = 0, T_WQ, T_WK, T_WV, T_WO, T_FFN_NORM, T_W1, T_W2, T_W3, T_EMBD, T_NORM, T_OUTPUT };
@@ -134,6 +137,8 @@ struct lnb_model {
   int device = 0, tp_rank = 0, tp_size = 1;
   int q_dim = 0, kv_dim = 0, q_l = 0, kv_l = 0, ffn_l = 0, vocab_l = 0;
   uint16_t *tok_embd = nullptr, *norm = nullptr, *output = nullptr;
+  uint8_t* output_s = nullptr;     // MXFP8 scales of the LM head (output then holds its codes)
+  int wfmt = LNB_WEIGHTS_BF16;     // lnb_model_set_weight_format; the linear weights are in this format once finalized
   bool have_embd = false, have_norm = false, have_output = false, finalized = false;
   std::vector<LayerW> layers;
   float* cis = nullptr;
@@ -327,9 +332,10 @@ extern "C" int lnb_model_destroy(lnb_model* m) {
   cudaSetDevice(m->device);
   cudaDeviceSynchronize();
   if (m->comm) g_nccl.CommDestroy(m->comm);
-  cudaFree(m->tok_embd); cudaFree(m->norm); cudaFree(m->output);
+  cudaFree(m->tok_embd); cudaFree(m->norm); cudaFree(m->output); cudaFree(m->output_s);
   for (auto& L : m->layers) {
     cudaFree(L.attn_norm); cudaFree(L.ffn_norm); cudaFree(L.wqkv); cudaFree(L.wo); cudaFree(L.w13); cudaFree(L.w2);
+    cudaFree(L.sqkv); cudaFree(L.so); cudaFree(L.s13); cudaFree(L.s2);
   }
   cudaFree(m->cis); cudaFree(m->silu_tab); cudaFree(m->staging); cudaFree(m->wpack_mem);
   delete m;
@@ -784,6 +790,147 @@ extern "C" int lnb_model_get_silu_table(lnb_model* m, uint16_t* out) {
   return 0;
 }
 
+// ---- MXFP8 linear weights (mxfp8.cuh, DESIGN.md §9h) ---------------------------------------------------------------
+extern "C" int lnb_model_set_weight_format(lnb_model* m, int fmt) {
+  if (!m) return fail(LNB_EINVAL, "model is NULL");
+  if (m->finalized) return fail(LNB_ESTATE, "model is finalized: the weight format is chosen before lnb_model_finalize");
+  if (fmt != LNB_WEIGHTS_BF16 && fmt != LNB_WEIGHTS_MXFP8) return fail(LNB_EINVAL, "unknown weight format %d", fmt);
+  if (fmt == LNB_WEIGHTS_MXFP8 && m->tp_size > 1) return fail(LNB_EINVAL, "MXFP8 weights need tp_size 1 (have %d)", m->tp_size);
+  m->wfmt = fmt;
+  return 0;
+}
+// one linear matrix of the device layout: its bf16 panels / codes, its scales, its shape
+struct LinMat {
+  uint16_t** w;
+  uint8_t** s;
+  int N, K;
+  int layer;   // -1: the LM head
+  int kind;    // T_WQ (the stacked wq|wk|wv), T_WO, T_W1 (the interleaved w1|w3), T_W2, T_OUTPUT
+};
+static std::vector<LinMat> linear_mats(lnb_model* m) {
+  std::vector<LinMat> v;
+  const int d = m->a.dim;
+  for (int l = 0; l < m->a.n_layers; l++) {
+    LayerW& L = m->layers[l];
+    v.push_back({&L.wqkv, &L.sqkv, m->q_l + 2 * m->kv_l, d, l, T_WQ});
+    v.push_back({&L.wo, &L.so, d, m->q_l, l, T_WO});
+    v.push_back({&L.w13, &L.s13, 2 * m->ffn_l, d, l, T_W1});
+    v.push_back({&L.w2, &L.s2, d, m->ffn_l, l, T_W2});
+  }
+  v.push_back({&m->output, &m->output_s, m->vocab_l, d, -1, T_OUTPUT});
+  return v;
+}
+static size_t mx_scale_bytes(int N, int K) { return (size_t)(N / 8) * mx_nbp(K) * 8; }
+static size_t mat_bytes(int fmt, int N, int K) {
+  return fmt == LNB_WEIGHTS_MXFP8 ? (size_t)N * K + mx_scale_bytes(N, K) : (size_t)N * K * 2;
+}
+// the checkpoint tensor and row of device row d of a matrix (inverse of placement + panel_dest_row)
+static void checkpoint_row(const lnb_model* m, const LinMat& x, int64_t d, const char** name, int64_t* row) {
+  static const char* kn[] = {"attention.wq.weight", "attention.wk.weight", "attention.wv.weight", "attention.wo.weight",
+                             "feed_forward.w1.weight", "feed_forward.w3.weight", "feed_forward.w2.weight", "output.weight"};
+  *row = d;
+  switch (x.kind) {
+    case T_WQ:
+      if (d < m->q_l) *name = kn[0];
+      else if (d < m->q_l + m->kv_l) { *name = kn[1]; *row = d - m->q_l; }
+      else { *name = kn[2]; *row = d - m->q_l - m->kv_l; }
+      break;
+    case T_WO: *name = kn[3]; break;
+    case T_W1: *name = (d & 4) ? kn[5] : kn[4]; *row = (d >> 3) * 4 + (d & 3); break;
+    case T_W2: *name = kn[6]; break;
+    default: *name = kn[7]; break;
+  }
+}
+// Quantize every linear matrix on the device, then free the bf16 copies.  Both copies are held until every matrix has
+// passed, so a refused weight leaves the bf16 model as it was.
+static int quantize_model(lnb_model* m) {
+  std::vector<LinMat> mats = linear_mats(m);
+  std::vector<uint8_t*> codes(mats.size(), nullptr), scales(mats.size(), nullptr);
+  unsigned long long* flags = nullptr;
+  auto drop = [&]() {
+    for (size_t i = 0; i < mats.size(); i++) { cudaFree(codes[i]); cudaFree(scales[i]); }
+    cudaFree(flags);
+  };
+  size_t total = 0;
+  for (const LinMat& x : mats) total += mat_bytes(LNB_WEIGHTS_MXFP8, x.N, x.K);
+  cudaError_t e = cudaMalloc((void**)&flags, mats.size() * 8);
+  if (e == cudaSuccess) e = cudaMemset(flags, 0xff, mats.size() * 8);
+  for (size_t i = 0; i < mats.size() && e == cudaSuccess; i++) {
+    e = cudaMalloc((void**)&codes[i], (size_t)mats[i].N * mats[i].K);
+    if (e == cudaSuccess) e = cudaMalloc((void**)&scales[i], mx_scale_bytes(mats[i].N, mats[i].K));
+    if (e == cudaSuccess) e = cudaMemset(scales[i], 0, mx_scale_bytes(mats[i].N, mats[i].K));
+    if (e == cudaSuccess) {
+      mxfp8_quantize_kernel<<<m->sm_count * 8, 256>>>(*mats[i].w, mats[i].N, mats[i].K, codes[i], scales[i], flags + i);
+      e = cudaGetLastError();
+    }
+  }
+  std::vector<unsigned long long> h(mats.size());
+  if (e == cudaSuccess) e = cudaMemcpy(h.data(), flags, h.size() * 8, cudaMemcpyDeviceToHost);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    drop();
+    return fail(e == cudaErrorMemoryAllocation ? LNB_ENOMEM : LNB_ECUDA, "MXFP8 quantization (%.2f GB beside the bf16 weights): %s",
+                total / 1e9, cudaGetErrorString(e));
+  }
+  for (size_t i = 0; i < mats.size(); i++) {
+    if (h[i] == ~0ull) continue;
+    const char* name;
+    int64_t row;
+    checkpoint_row(m, mats[i], (int64_t)(h[i] / (unsigned long long)mats[i].K), &name, &row);
+    const long long col = (long long)(h[i] % (unsigned long long)mats[i].K);
+    drop();
+    if (mats[i].layer < 0) return fail(LNB_EINVAL, "MXFP8: tensor \"%s\" has a non-finite weight at row %lld, column %lld", name, (long long)row, col);
+    return fail(LNB_EINVAL, "MXFP8: tensor \"layers.%d.%s\" has a non-finite weight at row %lld, column %lld", mats[i].layer, name,
+                (long long)row, col);
+  }
+  for (size_t i = 0; i < mats.size(); i++) {
+    cudaFree(*mats[i].w);
+    *mats[i].w = reinterpret_cast<uint16_t*>(codes[i]);
+    *mats[i].s = scales[i];
+  }
+  cudaFree(flags);
+  return 0;
+}
+extern "C" int lnb_model_mxfp8_read(lnb_model* m, const char* name, uint8_t* codes, uint8_t* scales) {
+  if (!m || !name) return fail(LNB_EINVAL, "NULL argument");
+  if (!m->finalized) return fail(LNB_ESTATE, "model is not finalized");
+  if (m->wfmt != LNB_WEIGHTS_MXFP8) return fail(LNB_ESTATE, "the model's weights are bf16");
+  int kind, layer;
+  if (parse_name(m, name, &kind, &layer)) return fail(LNB_EINVAL, "unknown tensor name \"%s\"", name);
+  if (kind == T_EMBD || kind == T_NORM || kind == T_ATTN_NORM || kind == T_FFN_NORM)
+    return fail(LNB_EINVAL, "tensor \"%s\" is not a linear weight: it stays bf16", name);
+  CU(cudaSetDevice(m->device));
+  const Placement p = placement(m, kind, layer);
+  const LinMat* x = nullptr;
+  std::vector<LinMat> mats = linear_mats(m);
+  for (const LinMat& c : mats)
+    if (c.layer == layer && *c.w == p.dst) x = &c;
+  const int K = x->K, nbp = mx_nbp(K), nb = (K + 31) / 32;
+  std::vector<uint8_t> hc((size_t)x->N * K), hs(mx_scale_bytes(x->N, K));
+  CU(cudaMemcpy(hc.data(), *x->w, hc.size(), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(hs.data(), *x->s, hs.size(), cudaMemcpyDeviceToHost));
+  for (int64_t r = 0; r < p.rows; r++) {
+    const int64_t d = p.dpanel_stride == 2 ? (r >> 2) * 8 + (p.dpanel0 ? 4 : 0) + (r & 3) : (int64_t)p.dpanel0 * 8 + r;
+    const int64_t dp = d / 8, rr = d % 8;
+    if (codes)
+      for (int k = 0; k < K; k++) codes[r * K + k] = hc[((dp * (K / 8) + k / 8) * 8 + rr) * 8 + k % 8];
+    if (scales)
+      for (int b = 0; b < nb; b++) scales[r * nb + b] = hs[(dp * nbp + b) * 8 + rr];
+  }
+  return 0;
+}
+extern "C" int lnb_model_weight_info(lnb_model* m, int* fmt, int64_t* device_bytes, int64_t* step_bytes) {
+  if (!m) return fail(LNB_EINVAL, "model is NULL");
+  const int f = m->finalized ? m->wfmt : LNB_WEIGHTS_BF16;
+  int64_t lin = 0;
+  for (const LinMat& x : linear_mats(m)) lin += (int64_t)mat_bytes(f, x.N, x.K);
+  const int64_t norms = (int64_t)(2 * m->a.n_layers + 1) * m->a.dim * 2;
+  if (fmt) *fmt = f;
+  if (device_bytes) *device_bytes = lin + norms + (int64_t)m->a.vocab_size * m->a.dim * 2;
+  if (step_bytes) *step_bytes = lin + norms + (int64_t)m->a.dim * 2;   // every matrix and norm once, one embedding row
+  return 0;
+}
+
 extern "C" int lnb_model_finalize(lnb_model* m) {
   if (!m) return fail(LNB_EINVAL, "model is NULL");
   if (m->finalized) return 0;
@@ -808,6 +955,8 @@ extern "C" int lnb_model_finalize(lnb_model* m) {
   }
   if (m->staging) { cudaFree(m->staging); m->staging = nullptr; m->staging_bytes = 0; }
   CU(cudaDeviceSynchronize());
+  if (m->wfmt == LNB_WEIGHTS_MXFP8)
+    if (int rc = quantize_model(m)) return rc;
   m->finalized = true;
   return 0;
 }
@@ -819,15 +968,17 @@ extern "C" int lnb_model_finalize(lnb_model* m) {
 // itself: ONE CTA per SM (>113 KB of shared memory each) holding 1, 2 or 4 chain warps (warps 1..4
 // sit on SMSPs 1,2,3,0; the producer warp 0 sleeps on its mbarrier), picked from N so that the grid
 // stays close to one wave.  Two chain warps on one scheduler run at half speed each.
-using CfgS1 = GemvCfg<32, 1, 1, 512, 3>;    // N <= 32*kWaveSMs rows
-using CfgS1M = GemvCfg<64, 1, 1, 512, 3>;   // N <= 64*kWaveSMs
-using CfgS1W = GemvCfg<128, 1, 1, 256, 3>;  // larger N (w1|w3, LM head): several waves, HBM-bound
-using CfgS2 = GemvCfg<32, 1, 2, 256, 4>;
-using CfgS8 = GemvCfg<32, 1, 8, 256, 4>;
-using CfgF1 = GemvCfg<32, 8, 1, 256, 4>;
-using CfgF1L = GemvCfg<32, 8, 1, 512, 3>;  // at most one CTA per SM (wo, w2): larger bulk copies
-using CfgF2 = GemvCfg<32, 8, 2, 256, 4>;
-using CfgF8 = GemvCfg<32, 8, 8, 256, 4>;
+// F = the weight format: MXFP8 configs take twice the k-tile, so a stage carries as many bytes as its bf16 twin.
+template <int F> using CfgS1_ = GemvCfg<32, 1, 1, 512 << F, 3, F>;    // N <= 32*kWaveSMs rows
+template <int F> using CfgS1M_ = GemvCfg<64, 1, 1, 512 << F, 3, F>;   // N <= 64*kWaveSMs
+template <int F> using CfgS1W_ = GemvCfg<128, 1, 1, 256 << F, 3, F>;  // larger N (w1|w3, LM head): several waves, HBM-bound
+template <int F> using CfgS2_ = GemvCfg<32, 1, 2, 256 << F, 4, F>;
+template <int F> using CfgS8_ = GemvCfg<32, 1, 8, 256 << F, 4, F>;
+template <int F> using CfgF1_ = GemvCfg<32, 8, 1, 256 << F, 4, F>;
+template <int F> using CfgF1L_ = GemvCfg<32, 8, 1, 512 << F, 3, F>;  // at most one CTA per SM (wo, w2): larger bulk copies
+template <int F> using CfgF2_ = GemvCfg<32, 8, 2, 256 << F, 4, F>;
+template <int F> using CfgF8_ = GemvCfg<32, 8, 8, 256 << F, 4, F>;
+using CfgF1 = CfgF1_<WF_BF16>;
 
 static const size_t kMaxSmem = 227 * 1024;
 static const int kWaveSMs = 132;   // H100 SXM: one wave of one-CTA-per-SM GEMV blocks
@@ -926,19 +1077,20 @@ static int launch_stream_attn(const Launcher& L, StreamAttn P, int rows, int n_k
 }
 
 template <class Cfg, int PRO, int EPI>
-static int launch_gemv_cfg(const Launcher& L, const GemvParams& p) {
+static int launch_gemv_cfg(const Launcher& L, const GemvParams& p, const uint8_t* Ws) {
   if (int rc = smem_opt_in<gemv_kernel<Cfg, PRO, EPI>>((int)kMaxSmem)) return rc;
   return launch_kernel(L, gemv_kernel<Cfg, PRO, EPI>, dim3((p.N / 8 + Cfg::kP - 1) / Cfg::kP), dim3(Cfg::kThreads),
-                       Cfg::smem_bytes(p.K), p);
+                       Cfg::smem_bytes(p.K), p, Ws);
 }
 
 // picks the row-block size: largest MB in {8,2,1} that is useful for M and whose smem fits.  mb_rows > 0 chooses it for
 // that many rows instead of M_total (ragged calls pass 8: the block size, and with it a row's FAST summation order, then
 // depends on K alone, not on how many rows share the call)
-template <int PRO, int EPI>
-static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total, int mb_rows = 0) {
-  if (p.N % 16 || p.K % 8) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 16 and K %d of 8", p.N, p.K);  // 16: panel pairs
-  if ((EPI == EPI_QKV_ROPE || EPI == EPI_SWIGLU) && p.N % 32) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 32", p.N);
+// (the weight format F comes from Ws: launch_gemv below)
+template <int PRO, int EPI, int F>
+static int launch_gemv_fmt(const Launcher& L, int mode, GemvParams p, int M_total, int mb_rows, const uint8_t* Ws) {
+  using CfgS1 = CfgS1_<F>; using CfgS1M = CfgS1M_<F>; using CfgS1W = CfgS1W_<F>; using CfgS2 = CfgS2_<F>; using CfgS8 = CfgS8_<F>;
+  using CfgF1 = CfgF1_<F>; using CfgF1L = CfgF1L_<F>; using CfgF2 = CfgF2_<F>; using CfgF8 = CfgF8_<F>;
   const bool strict = (mode == LNB_ACC_STRICT);
   p.strict_norm = strict ? 1 : 0;
   const int mb_for = mb_rows > 0 ? mb_rows : M_total;
@@ -970,20 +1122,28 @@ static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total, i
     }
     int rc;
     if (strict) {
-      if (mb == 1 && p.N > 64 * kWaveSMs && p.N % 128 == 0 && CfgS1W::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgS1W, PRO, EPI>(L, p);
-      else if (mb == 1 && p.N > 32 * kWaveSMs && p.N % 64 == 0 && CfgS1M::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgS1M, PRO, EPI>(L, p);
-      else if (mb == 1) rc = launch_gemv_cfg<CfgS1, PRO, EPI>(L, p);
-      else if (mb == 8) rc = launch_gemv_cfg<CfgS8, PRO, EPI>(L, p);
-      else rc = launch_gemv_cfg<CfgS2, PRO, EPI>(L, p);
+      if (mb == 1 && p.N > 64 * kWaveSMs && p.N % 128 == 0 && CfgS1W::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgS1W, PRO, EPI>(L, p, Ws);
+      else if (mb == 1 && p.N > 32 * kWaveSMs && p.N % 64 == 0 && CfgS1M::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgS1M, PRO, EPI>(L, p, Ws);
+      else if (mb == 1) rc = launch_gemv_cfg<CfgS1, PRO, EPI>(L, p, Ws);
+      else if (mb == 8) rc = launch_gemv_cfg<CfgS8, PRO, EPI>(L, p, Ws);
+      else rc = launch_gemv_cfg<CfgS2, PRO, EPI>(L, p, Ws);
     } else {
-      if (mb == 8) rc = launch_gemv_cfg<CfgF8, PRO, EPI>(L, p);
-      else if (mb == 2) rc = launch_gemv_cfg<CfgF2, PRO, EPI>(L, p);
-      else if (p.N <= 32 * kWaveSMs && CfgF1L::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgF1L, PRO, EPI>(L, p);
-      else rc = launch_gemv_cfg<CfgF1, PRO, EPI>(L, p);
+      if (mb == 8) rc = launch_gemv_cfg<CfgF8, PRO, EPI>(L, p, Ws);
+      else if (mb == 2) rc = launch_gemv_cfg<CfgF2, PRO, EPI>(L, p, Ws);
+      else if (p.N <= 32 * kWaveSMs && CfgF1L::smem_bytes(p.K) <= kMaxSmem) rc = launch_gemv_cfg<CfgF1L, PRO, EPI>(L, p, Ws);
+      else rc = launch_gemv_cfg<CfgF1, PRO, EPI>(L, p, Ws);
     }
     if (rc) return rc;
   }
   return 0;
+}
+// Ws: the scales of an MXFP8 matrix (p.W then points at its codes); NULL: p.W is bf16
+template <int PRO, int EPI>
+static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total, int mb_rows = 0, const uint8_t* Ws = nullptr) {
+  if (p.N % 16 || p.K % 8) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 16 and K %d of 8", p.N, p.K);  // 16: panel pairs
+  if ((EPI == EPI_QKV_ROPE || EPI == EPI_SWIGLU) && p.N % 32) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 32", p.N);
+  if (Ws) return launch_gemv_fmt<PRO, EPI, WF_MXFP8>(L, mode, p, M_total, mb_rows, Ws);
+  return launch_gemv_fmt<PRO, EPI, WF_BF16>(L, mode, p, M_total, mb_rows, nullptr);
 }
 
 // LNB_ACC_STRICT RMSNorm scale r[row] (the reference's sequential fp32 sum of squares, bit-exact).  Three
@@ -1099,6 +1259,9 @@ struct lnb_session {
   // tensor-core prefill path (LNB_ACC_FAST, S >= 32): X8-layout activations + raw GEMM outputs
   uint16_t *xn8 = nullptr, *o8 = nullptr, *m8 = nullptr, *qkv_raw = nullptr, *gu = nullptr;
   int mpad = 0;
+  // MXFP8 models: the bf16 panels of the matrix the next GEMM reads (mxfp8_dequant_kernel), as large as the largest one
+  uint16_t* wdq = nullptr;
+  size_t wdq_elems = 0;
   // peer-memory all-reduce (tp_size > 1, optional): own region + the peers' mapped regions
   uint8_t* p2p_region = nullptr;
   size_t p2p_bytes = 0;
@@ -1297,6 +1460,10 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
     al((void**)&s->m8, (size_t)s->mpad * m->ffn_l * 2);
     al((void**)&s->qkv_raw, (size_t)max_rows * (m->q_l + 2 * m->kv_l) * 2);
     al((void**)&s->gu, (size_t)max_rows * 2 * m->ffn_l * 2);
+    if (m->wfmt == LNB_WEIGHTS_MXFP8) {
+      for (const LinMat& x : linear_mats(m)) s->wdq_elems = std::max(s->wdq_elems, x.layer < 0 ? (size_t)TC_BN * x.K : (size_t)x.N * x.K);
+      al((void**)&s->wdq, s->wdq_elems * 2);
+    }
   }
   al((void**)&s->d_tokens, (size_t)max_rows * 4);
   al((void**)&s->st, sizeof(LnbDevState));
@@ -1338,7 +1505,7 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   if (s->stream) cudaStreamSynchronize(s->stream);
   if (s->graph) cudaGraphExecDestroy(s->graph);
   cudaFree(s->x); cudaFree(s->h1); cudaFree(s->q); cudaFree(s->o); cudaFree(s->mbuf); cudaFree(s->part); cudaFree(s->rs);
-  cudaFree(s->xn8); cudaFree(s->o8); cudaFree(s->m8); cudaFree(s->qkv_raw); cudaFree(s->gu);
+  cudaFree(s->xn8); cudaFree(s->o8); cudaFree(s->m8); cudaFree(s->qkv_raw); cudaFree(s->gu); cudaFree(s->wdq);
   for (int r = 0; r < 8; r++)
     if (s->p2p_peer[r]) cudaIpcCloseMemHandle(s->p2p_peer[r]);
   cudaFree(s->p2p_region);
@@ -1531,6 +1698,7 @@ static bool engine_probe(lnb_session* s) {
   // FAST sessions; LNB_ENGINE=1 / 0 forces it on / off.
   const char* e = getenv("LNB_ENGINE");
   if (e && !strcmp(e, "0")) return no("LNB_ENGINE=0");
+  if (m->wfmt == LNB_WEIGHTS_MXFP8) return no("MXFP8 weights: the decode and batch engines stream bf16 panels");
   // single-sequence steps of single-GPU FAST sessions stay on the kernel chain by default (the batch engine does not care)
   s->eng_single_default = (e && !strcmp(e, "1")) || !(s->mode == LNB_ACC_FAST && m->tp_size == 1);
   const int kmax = std::max(a.dim, std::max(m->q_l, m->ffn_l));
@@ -1618,6 +1786,7 @@ static bool ensure_wpack(lnb_model* m) {
   const lnb_model_args& a = m->a;
   const int G = m->sm_count, L = a.n_layers;
   auto no = [&](const std::string& why) { m->wpack_state = -1; m->wpack_why = why; return false; };
+  if (m->wfmt == LNB_WEIGHTS_MXFP8) return no("MXFP8 weights: the packed copies are built from bf16 panels");
   struct Mat { const uint16_t* W; int N; lnb_model::WPack* wp; };
   std::vector<Mat> mats;
   m->wp_w13.assign(L, lnb_model::WPack{});
@@ -2143,7 +2312,7 @@ static int per_row_head(const Launcher& L, lnb_session* s, const Rows& R) {
   p.rscale = strict ? s->rs : nullptr;
   p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
   p.out_f32 = s->logits; p.ldo = m->vocab_l; p.n_offset = m->tp_rank * m->vocab_l; p.st = nullptr; p.argmax_row = -1;
-  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, n, R.mb_rows))) return rc;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, n, R.mb_rows, m->output_s))) return rc;
   if ((rc = gather_logits(s, 0, n))) return rc;
   const float* lg = (m->tp_size > 1) ? s->logits_full : s->logits;
   return launch_kernel(L, argmax_f32_kernel, dim3(n), dim3(256), 0, lg, a.vocab_size, s->d_next_arr);
@@ -2200,12 +2369,12 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
     return launch_rms_scale(L, xin, a.dim, s->rs, rows, a.dim, a.norm_eps);
   };
   // wo / w2 + residual: out = res + x W^T; tensor-parallel ranks sum their partials first (peer all-reduce or NCCL)
-  auto proj_resid = [&](const uint16_t* W, int K, const uint16_t* x, const uint16_t* res, uint16_t* out) -> int {
+  auto proj_resid = [&](const uint16_t* W, const uint8_t* Ws, int K, const uint16_t* x, const uint16_t* res, uint16_t* out) -> int {
     GemvParams p{};
     p.W = W; p.N = a.dim; p.K = K; p.x = x; p.ldx = K; p.ldo = a.dim;
     if (m->tp_size == 1) {
       p.out_bf16 = out; p.res = res;
-      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S, mb_rows);
+      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S, mb_rows, Ws);
     }
     int rc2;
     if (s->p2p_ready) {
@@ -2232,19 +2401,19 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
       p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
       p.cache_k = s->ck[l] + R.cache_off; p.cache_v = s->cv[l] + R.cache_off; p.cis = m->cis; p.pos_ptr = &s->st->pos;
       p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = R.seq_stride;
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, S, mb_rows))) return rc;
+      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, S, mb_rows, W.sqkv))) return rc;
     }
     if ((rc = launch_attention(L, s, l, R, s->o, 0))) return rc;
-    if ((rc = proj_resid(W.wo, m->q_l, s->o, s->x, s->h1))) return rc;            // wo + residual (:522, :232)
+    if ((rc = proj_resid(W.wo, W.so, m->q_l, s->o, s->x, s->h1))) return rc;            // wo + residual (:522, :232)
     if ((rc = strict_scale(s->h1, S))) return rc;
     {  // ffn_norm -> w1|w3 -> SiLU * up                             (:237, :601-614)
       GemvParams p{};
       p.rscale = strict ? s->rs : nullptr;
       p.W = W.w13; p.N = 2 * m->ffn_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm; p.eps = a.norm_eps;
       p.out_bf16 = s->mbuf; p.ldo = m->ffn_l; p.silu_tab = m->silu_tab;
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, S, mb_rows))) return rc;
+      if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, S, mb_rows, W.s13))) return rc;
     }
-    if ((rc = proj_resid(W.w2, m->ffn_l, s->mbuf, s->h1, s->x))) return rc;        // w2 + residual (:619, :248)
+    if ((rc = proj_resid(W.w2, W.s2, m->ffn_l, s->mbuf, s->h1, s->x))) return rc;        // w2 + residual (:619, :248)
   }
   if (R.head == HEAD_PER_ROW) return per_row_head(L, s, R);
   // output_norm -> output -> f32 logits (+ greedy argmax of the last row)   (:166-175; inference.go:207-216)
@@ -2260,7 +2429,7 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
   p.st = s->st; p.argmax_row = rows - 1; p.m_off = 0;
   p.publish = (m->tp_size == 1) ? 1 : 0;
   p.advance = R.advance ? 1 : 0; p.tok_out = s->d_tok_out;
-  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, rows))) return rc;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, rows, 0, m->output_s))) return rc;
   if (m->tp_size > 1) {
     if (s->p2p_ready) rc = launch_kernel(L, p2p_argmax_kernel, dim3(1), dim3(32), 0, s->p2p, s->st, R.advance ? 1 : 0, s->d_tok_out);
     else rc = reduce_argmax_publish(L, s, R.advance);
@@ -2284,10 +2453,17 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
     return rc;
   const int n_layers = active_layers(s);
   const int ew_grid = m->sm_count * 8;
+  // the bf16 panels a GEMM reads: the matrix itself, or (MXFP8) rows [0, N) dequantized into the session's scratch
+  auto tc_w = [&](GemmTcParams& g, const uint16_t* W, const uint8_t* Ws, int N, int K) -> int {
+    g.W = Ws ? s->wdq : W;
+    if (!Ws) return 0;
+    return launch_kernel(L, mxfp8_dequant_kernel, dim3(ew_grid), dim3(256), 0, reinterpret_cast<const uint8_t*>(W), Ws, N, K, s->wdq);
+  };
   // wo / w2 + residual: out = res + X W^T; tensor-parallel ranks sum their partials over NCCL first
-  auto proj_resid = [&](const uint16_t* X8, const uint16_t* W, int K, const uint16_t* res, uint16_t* out) -> int {
+  auto proj_resid = [&](const uint16_t* X8, const uint16_t* W, const uint8_t* Ws, int K, const uint16_t* res, uint16_t* out) -> int {
     GemmTcParams g{};
-    g.X8 = X8; g.W = W; g.M = S; g.N = a.dim; g.K = K; g.ldo = a.dim;
+    g.X8 = X8; g.M = S; g.N = a.dim; g.K = K; g.ldo = a.dim;
+    if (int rc2 = tc_w(g, W, Ws, a.dim, K)) return rc2;
     if (m->tp_size == 1) {
       g.out_bf16 = out; g.res = res;
       return launch_gemm_tc<TC_EPI_RESID>(L, g);
@@ -2304,7 +2480,8 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
       return rc;
     {
       GemmTcParams g{};
-      g.X8 = s->xn8; g.W = W.wqkv; g.M = S; g.N = qkv_n; g.K = a.dim; g.out_bf16 = s->qkv_raw; g.ldo = qkv_n;
+      g.X8 = s->xn8; g.M = S; g.N = qkv_n; g.K = a.dim; g.out_bf16 = s->qkv_raw; g.ldo = qkv_n;
+      if ((rc = tc_w(g, W.wqkv, W.sqkv, qkv_n, a.dim))) return rc;
       if ((rc = launch_gemm_tc<TC_EPI_BF16>(L, g))) return rc;
     }
     if ((rc = launch_kernel(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
@@ -2312,17 +2489,18 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
                             R.pos_arr, R.row_seq, (long long)s->seq_len * m->kv_l)))
       return rc;
     if ((rc = launch_attention(L, s, l, R, s->o8, 1))) return rc;
-    if ((rc = proj_resid(s->o8, W.wo, m->q_l, s->x, s->h1))) return rc;
+    if ((rc = proj_resid(s->o8, W.wo, W.so, m->q_l, s->x, s->h1))) return rc;
     if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->h1, a.dim, (const uint16_t*)W.ffn_norm,
                             s->xn8, S, a.dim, a.norm_eps)))
       return rc;
     {
       GemmTcParams g{};
       // SwiGLU in the epilogue: the hidden activations go straight into the X8 operand of the w2 GEMM
-      g.X8 = s->xn8; g.W = W.w13; g.M = S; g.N = 2 * m->ffn_l; g.K = a.dim; g.out_bf16 = s->m8; g.ldo = m->ffn_l; g.silu_tab = m->silu_tab;
+      g.X8 = s->xn8; g.M = S; g.N = 2 * m->ffn_l; g.K = a.dim; g.out_bf16 = s->m8; g.ldo = m->ffn_l; g.silu_tab = m->silu_tab;
+      if ((rc = tc_w(g, W.w13, W.s13, 2 * m->ffn_l, a.dim))) return rc;
       if ((rc = launch_gemm_tc<TC_EPI_SWIGLU>(L, g))) return rc;
     }
-    if ((rc = proj_resid(s->m8, W.w2, m->ffn_l, s->h1, s->x))) return rc;
+    if ((rc = proj_resid(s->m8, W.w2, W.s2, m->ffn_l, s->h1, s->x))) return rc;
   }
   // LM head: all rows on the tensor cores when asked for (and the vocabulary shard tiles), then the
   // last row through the GEMV, which also owns the greedy argmax (identical to the decode path)
@@ -2333,12 +2511,20 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
       return rc;
     GemmTcParams g{};
     g.X8 = s->xn8; g.W = m->output; g.M = S - 1; g.N = m->vocab_l; g.K = a.dim; g.out_f32 = s->logits; g.ldo = m->vocab_l;
-    if (S > 1 && (rc = launch_gemm_tc<TC_EPI_F32TRUNC>(L, g))) return rc;
+    // MXFP8: the LM head in row slices that fit the scratch (whole 128-row tiles), each dequantized before its GEMM
+    const int slice = m->output_s ? (int)std::min<size_t>(m->vocab_l, s->wdq_elems / a.dim / TC_BN * TC_BN) : m->vocab_l;
+    for (int n0 = 0; S > 1 && n0 < m->vocab_l; n0 += slice) {
+      g.N = std::min(slice, m->vocab_l - n0);
+      g.out_f32 = s->logits + n0;
+      const uint16_t* codes = reinterpret_cast<const uint16_t*>(reinterpret_cast<const uint8_t*>(m->output) + (size_t)n0 * a.dim);
+      if (m->output_s && (rc = tc_w(g, codes, m->output_s + (size_t)(n0 / 8) * mx_nbp(a.dim) * 8, g.N, a.dim))) return rc;
+      if ((rc = launch_gemm_tc<TC_EPI_F32TRUNC>(L, g))) return rc;
+    }
   } else if (R.head == HEAD_ALL && S > 1) {
     GemvParams p{};
     p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
     p.out_f32 = s->logits; p.ldo = m->vocab_l; p.st = nullptr; p.argmax_row = -1;
-    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, S - 1))) return rc;
+    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, S - 1, 0, m->output_s))) return rc;
   }
   {
     GemvParams p{};
@@ -2347,7 +2533,7 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
     p.out_f32 = R.head != HEAD_NONE ? s->logits + (R.head == HEAD_ALL ? (size_t)(S - 1) * m->vocab_l : 0) : nullptr;
     p.ldo = m->vocab_l; p.n_offset = m->tp_rank * m->vocab_l;
     p.st = s->st; p.argmax_row = 0; p.publish = (m->tp_size == 1) ? 1 : 0; p.advance = 0; p.tok_out = s->d_tok_out;
-    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1))) return rc;
+    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1, 0, m->output_s))) return rc;
     if (m->tp_size > 1) {
       if ((rc = reduce_argmax_publish(L, s, false))) return rc;
       if (R.head != HEAD_NONE && R.gather && (rc = gather_logits(s, 0, R.head_rows))) return rc;
@@ -3544,33 +3730,34 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
       GemvParams p{};
       p.eps = a.norm_eps;
       p.rscale = (s->mode == LNB_ACC_STRICT) ? s->rs : nullptr;
+      const uint8_t* ws = kind == 0 ? W.sqkv : kind == 1 ? W.so : kind == 2 ? W.s13 : kind == 3 ? W.s2 : m->output_s;
       switch (kind) {
         case 0:
           p.W = W.wqkv; p.N = m->q_l + 2 * m->kv_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm;
           p.out_bf16 = s->q; p.ldo = m->q_l; p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
           p.cache_k = s->ck[l]; p.cache_v = s->cv[l]; p.cis = m->cis; p.pos_ptr = &s->st->pos;
-          rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, s->mode, p, 1);
+          rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, s->mode, p, 1, 0, ws);
           break;
         case 1:
           p.W = W.wo; p.N = a.dim; p.K = m->q_l; p.x = s->o; p.ldx = m->q_l; p.ldo = a.dim; p.out_bf16 = s->h1; p.res = s->x;
-          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1);
+          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1, 0, ws);
           break;
         case 2:
           p.W = W.w13; p.N = 2 * m->ffn_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm;
           p.out_bf16 = s->mbuf; p.ldo = m->ffn_l; p.silu_tab = m->silu_tab;
-          rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, s->mode, p, 1);
+          rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, s->mode, p, 1, 0, ws);
           break;
         case 3:
           p.W = W.w2; p.N = a.dim; p.K = m->ffn_l; p.x = s->mbuf; p.ldx = m->ffn_l; p.ldo = a.dim; p.out_bf16 = s->h1; p.res = s->x;
-          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1);
+          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1, 0, ws);
           break;
         case 4:
           p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.ldo = m->vocab_l;
           p.st = nullptr; p.argmax_row = -1;
-          rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1);
+          rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1, 0, ws);
           break;
       }
-      bytes = (int64_t)p.N * p.K * 2;
+      bytes = (int64_t)mat_bytes(ws ? LNB_WEIGHTS_MXFP8 : LNB_WEIGHTS_BF16, p.N, p.K);
       n_launch++;
     }
     return rc;

@@ -23,8 +23,13 @@
 // accumulates them sequentially (fp32 FMA; bf16*bf16 products are exact in fp32, so FMA ==
 // mul-then-add).  KS == 1 (LNB_ACC_STRICT) is exactly the reference's k = 0,1,2,... order.
 // KS > 1 (LNB_ACC_FAST): out = ((p0 + p1) + p2) + ... + p_{KS-1}, combined in stream order.
+//
+// MXFP8 weights (FMT == WF_MXFP8, mxfp8.cuh): the same producer streams each panel's E4M3 codes (64 B per chunk) and its
+// E8M0 scales; a stage carries twice the k-range of the bf16 config it mirrors, so as many bytes are in flight.  Consumers
+// decode every weight to the exact fp32 value of the bf16 number it stands for and run the same FMAs in the same order.
 #pragma once
 #include "common.cuh"
+#include "mxfp8.cuh"
 
 namespace lnb {
 
@@ -40,7 +45,7 @@ enum {
 };
 
 struct GemvParams {
-  const uint16_t* W;       // panel-major weights
+  const uint16_t* W;       // panel-major weights (MXFP8: the codes; their scales are the kernel's second argument)
   int N, K;                // N = rows of W (multiple of 8), K multiple of 8
   int M;                   // activation rows in this launch (<= MB)
   // prologue
@@ -86,17 +91,22 @@ struct GemvParams {
   uint32_t res_tag_hi;     // tag << 16 of the phase that produced the residual
 };
 
-template <int TN, int KS, int MB, int KT, int NST>
+template <int TN, int KS, int MB, int KT, int NST, int FMT = WF_BF16>
 struct GemvCfg {
-  static constexpr int kTN = TN, kKS = KS, kMB = MB, kKT = KT, kNST = NST;
+  static constexpr int kTN = TN, kKS = KS, kMB = MB, kKT = KT, kNST = NST, kFmt = FMT;
   static constexpr int kP = TN / 8;                    // 8-row panels per CTA
   static constexpr int kNCons = TN * KS;               // consumer threads
   static constexpr int kThreads = kNCons + 32;         // + producer warp
-  static constexpr int kStageBytes = TN * KT * 2;
+  // MXFP8: a panel's codes take KT * 8 bytes plus 64 bytes of padding, so the two panels a half-warp reads sit in opposite
+  // halves of the banks (conflict-free 8-byte loads); the panels' scales (KT / 4 bytes each) follow
+  static constexpr int kPanelBytes = FMT == WF_MXFP8 ? KT * 8 + 64 : KT * 16;
+  static constexpr int kScaleOff = kP * kPanelBytes;
+  static constexpr int kStageBytes = FMT == WF_MXFP8 ? kScaleOff + kP * (KT / 4) : TN * KT * 2;
   static constexpr int kChunksPerTile = KT / 8;
   static_assert(TN % 32 == 0 && TN <= 128, "TN");
   static_assert(kNCons % 32 == 0, "consumer warps");
   static_assert(kChunksPerTile % KS == 0, "k-tile must hold a whole number of chunk rounds");
+  static_assert(FMT == WF_BF16 || KT % 64 == 0, "MXFP8 k-tiles hold whole, 16-byte-aligned scale ranges");
   static size_t smem_bytes(int K) {
     size_t b = 1024;                                   // barriers + scalars (first 1 KB)
     b += (size_t)NST * kStageBytes;
@@ -239,7 +249,7 @@ LNB_DEVINL void logits_publish(const GemvParams& p) {
 
 // ------------------------------------------------------------------------------------------
 template <class Cfg, int PRO, int EPI>
-__global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p) {
+__global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p, const uint8_t* Ws) {   // Ws: MXFP8 scales
   constexpr int TN = Cfg::kTN, KS = Cfg::kKS, MB = Cfg::kMB, KT = Cfg::kKT, NST = Cfg::kNST;
   constexpr int P = Cfg::kP, NCONS = Cfg::kNCons, STAGE = Cfg::kStageBytes;
   constexpr int CPT = Cfg::kChunksPerTile;
@@ -282,11 +292,25 @@ __global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p)
         mbar_wait(&empty_bar[s], ph ^ 1u);
         const int k0 = t * KT;
         const int kt = min(KT, K - k0);
-        const uint32_t bytes_per_panel = (uint32_t)kt * 16u;  // kt/8 chunks * 128 B
-        mbar_expect_tx(&full_bar[s], bytes_per_panel * (uint32_t)my_panels);
-        for (int pp = 0; pp < my_panels; pp++) {
-          const uint8_t* src = wbase + ((size_t)(panel0 + pp) * (size_t)K + (size_t)k0) * 16u;
-          bulk_g2s(s_stage + (size_t)s * STAGE + (size_t)pp * (KT * 16), src, bytes_per_panel, &full_bar[s], pol);
+        if constexpr (Cfg::kFmt == WF_MXFP8) {
+          const uint32_t code_bytes = (uint32_t)kt * 8u;                          // kt/8 chunks * 64 B
+          const uint32_t scale_bytes = (uint32_t)(((kt + 31) / 32 + 1) & ~1) * 8u;  // whole 16-byte pairs of blocks
+          const int nbp = mx_nbp(K);
+          mbar_expect_tx(&full_bar[s], (code_bytes + scale_bytes) * (uint32_t)my_panels);
+          for (int pp = 0; pp < my_panels; pp++) {
+            const size_t panel = (size_t)(panel0 + pp);
+            bulk_g2s(s_stage + (size_t)s * STAGE + (size_t)pp * Cfg::kPanelBytes, wbase + (panel * (size_t)K + (size_t)k0) * 8u,
+                     code_bytes, &full_bar[s], pol);
+            bulk_g2s(s_stage + (size_t)s * STAGE + Cfg::kScaleOff + (size_t)pp * (KT / 4), Ws + (panel * nbp + k0 / 32) * 8u,
+                     scale_bytes, &full_bar[s], pol);
+          }
+        } else {
+          const uint32_t bytes_per_panel = (uint32_t)kt * 16u;  // kt/8 chunks * 128 B
+          mbar_expect_tx(&full_bar[s], bytes_per_panel * (uint32_t)my_panels);
+          for (int pp = 0; pp < my_panels; pp++) {
+            const uint8_t* src = wbase + ((size_t)(panel0 + pp) * (size_t)K + (size_t)k0) * 16u;
+            bulk_g2s(s_stage + (size_t)s * STAGE + (size_t)pp * (KT * 16), src, bytes_per_panel, &full_bar[s], pol);
+          }
         }
       }
     }
@@ -382,6 +406,32 @@ __global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p)
     mbar_wait(&full_bar[s], ph);
     const int k0 = t * KT;
     const int nchunks = min(KT, K - k0) / 8;
+    if constexpr (Cfg::kFmt == WF_MXFP8) {
+      const uint8_t* ctile = s_stage + (size_t)s * STAGE + (size_t)pp * Cfg::kPanelBytes + rr * 8;
+      const uint8_t* stile = s_stage + (size_t)s * STAGE + Cfg::kScaleOff + (size_t)pp * (KT / 4) + rr;
+      constexpr int UNROLL = MB > 2 ? 1 : 4;   // eight rows' accumulators and operands fill the registers already
+#pragma unroll UNROLL
+      for (int ch = j; ch < nchunks; ch += KS) {
+        float w[8];
+        mx_decode8(*reinterpret_cast<const uint2*>(ctile + ch * 64), mx_scale(stile[(ch >> 2) * 8]), w);
+        const float* xk = s_x + k0 + ch * 8;
+#pragma unroll
+        for (int m = 0; m < MB; m++) {
+          const float4 xa = *reinterpret_cast<const float4*>(xk + (size_t)m * K);
+          const float4 xb = *reinterpret_cast<const float4*>(xk + (size_t)m * K + 4);
+          float a = acc[m];
+          a = __fmaf_rn(xa.x, w[0], a);
+          a = __fmaf_rn(xa.y, w[1], a);
+          a = __fmaf_rn(xa.z, w[2], a);
+          a = __fmaf_rn(xa.w, w[3], a);
+          a = __fmaf_rn(xb.x, w[4], a);
+          a = __fmaf_rn(xb.y, w[5], a);
+          a = __fmaf_rn(xb.z, w[6], a);
+          a = __fmaf_rn(xb.w, w[7], a);
+          acc[m] = a;
+        }
+      }
+    } else {
     const uint8_t* tile = s_stage + (size_t)s * STAGE + (size_t)pp * (KT * 16) + rr * 16;
     if (MB == 1 && NI % 4 == 0 && nchunks == CPT) {
       // Full tile, one activation row: groups of 4 chunks with register double buffering, so the
@@ -444,6 +494,7 @@ __global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p)
           acc[m] = a;
         }
       }
+    }
     }
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty_bar[s]);

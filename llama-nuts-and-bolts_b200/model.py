@@ -58,18 +58,32 @@ class Vocabulary:  # src/model/vocabulary.go (ids only; the tokenizer is out of 
     StopTokenIds: tuple = synth.STOP_IDS
 
 
+WEIGHT_FORMATS = {"bf16": _capi.LNB_WEIGHTS_BF16, "mxfp8": _capi.LNB_WEIGHTS_MXFP8}
+
+
 class LlamaTransformer:
     """model.LlamaTransformer: owns the device-side weights of one tensor-parallel rank."""
 
-    def __init__(self, args: ModelArgs, device: int = 0, tp_rank: int = 0, tp_size: int = 1, nccl_id: bytes | None = None):
+    def __init__(self, args: ModelArgs, device: int = 0, tp_rank: int = 0, tp_size: int = 1, nccl_id: bytes | None = None,
+                 weight_format: str = "bf16"):
+        """weight_format: "bf16", or "mxfp8": finalize quantizes the linear weights (DESIGN.md §9h)"""
         self.args = args
         self.device, self.tp_rank, self.tp_size = device, tp_rank, tp_size
         self._cargs = _capi.ModelArgsC(**args.to_c_dict())
+        fmt = WEIGHT_FORMATS.get(weight_format)
+        if fmt is None:
+            raise ValueError(f"unknown weight_format {weight_format!r} (known: {', '.join(WEIGHT_FORMATS)})")
         h = C.c_void_p()
         idbuf = C.create_string_buffer(nccl_id, 128) if nccl_id is not None else None
         check(lib.lnb_model_create(C.byref(self._cargs), device, tp_rank, tp_size, idbuf, C.byref(h)))
         self.h = h
         self.finalized = False
+        try:
+            check(lib.lnb_model_set_weight_format(h, fmt))
+        except Exception:
+            self.close()
+            raise
+        self.weight_format = weight_format
 
     # --- weights -----------------------------------------------------------------------------
     def upload_tensor(self, name: str, data: np.ndarray):
@@ -91,6 +105,23 @@ class LlamaTransformer:
     def finalize(self):
         check(lib.lnb_model_finalize(self.h))
         self.finalized = True
+
+    def mxfp8_read(self, name: str) -> tuple[np.ndarray, np.ndarray]:
+        """the E4M3 codes [rows, cols] and E8M0 scales [rows, ceil(cols / 32)] of a linear checkpoint tensor of a finalized
+        MXFP8 model, in the checkpoint's row order"""
+        shape = synth.tensor_shapes(self.args.to_c_dict()).get(name, (0,))
+        rows, cols = shape if len(shape) == 2 else (shape[0], 1)   # the library names what is wrong with other names
+        codes = np.empty((rows, cols), np.uint8)
+        scales = np.empty((rows, (cols + 31) // 32), np.uint8)
+        check(lib.lnb_model_mxfp8_read(self.h, name.encode(), codes.ctypes.data, scales.ctypes.data))
+        return codes, scales
+
+    def weight_info(self) -> dict:
+        """{"format": "bf16" | "mxfp8", "device_bytes": weight bytes in HBM, "step_bytes": weight bytes one S = 1 step reads}"""
+        fmt, dev, step = C.c_int(0), C.c_int64(0), C.c_int64(0)
+        check(lib.lnb_model_weight_info(self.h, C.byref(fmt), C.byref(dev), C.byref(step)))
+        names = {v: k for k, v in WEIGHT_FORMATS.items()}
+        return {"format": names[fmt.value], "device_bytes": dev.value, "step_bytes": step.value}
 
     def rope_table(self, rows: int | None = None) -> np.ndarray:
         rows = rows or self.args.MaxSequenceLength * 2
@@ -497,32 +528,33 @@ class InferenceContext:
 class Model:
     """model.Model (src/model/model.go:43-107): args + vocabulary + transformer."""
 
-    def __init__(self, args: ModelArgs, device: int = 0, tp_rank: int = 0, tp_size: int = 1, nccl_id=None):
+    def __init__(self, args: ModelArgs, device: int = 0, tp_rank: int = 0, tp_size: int = 1, nccl_id=None,
+                 weight_format: str = "bf16"):
         self.ModelArgs = args
         self.Vocabulary = Vocabulary()
-        self.Transformer = LlamaTransformer(args, device, tp_rank, tp_size, nccl_id)
+        self.Transformer = LlamaTransformer(args, device, tp_rank, tp_size, nccl_id, weight_format)
 
     def Free(self):
         self.Transformer.close()
 
 
 def LoadSyntheticModel(args_dict: dict | None = None, seed: int = synth.SEED, device: int = 0, tp_rank: int = 0,
-                       tp_size: int = 1, nccl_id=None) -> Model:
+                       tp_size: int = 1, nccl_id=None, weight_format: str = "bf16") -> Model:
     """Stand-in for model.LoadModel (src/model/loader.go:18-70) when no checkpoint exists:
     random-init weights of the given architecture, generated directly in HBM."""
     args = ModelArgs.from_c_dict(args_dict or synth.LLAMA31_8B)
-    m = Model(args, device, tp_rank, tp_size, nccl_id)
+    m = Model(args, device, tp_rank, tp_size, nccl_id, weight_format)
     m.Transformer.init_synthetic(seed)
     m.Transformer.finalize()
     return m
 
 
 def LoadModelFromTensors(args_dict: dict, tensors: dict[str, np.ndarray], device: int = 0, tp_rank: int = 0,
-                         tp_size: int = 1, nccl_id=None) -> Model:
+                         tp_size: int = 1, nccl_id=None, weight_format: str = "bf16") -> Model:
     """The reference's flow (loader.go:22-70): tensors come from host memory (the checkpoint mmap)
     and are bound by name + shape."""
     args = ModelArgs.from_c_dict(args_dict)
-    m = Model(args, device, tp_rank, tp_size, nccl_id)
+    m = Model(args, device, tp_rank, tp_size, nccl_id, weight_format)
     for name, arr in tensors.items():
         m.Transformer.upload_tensor(name, arr)
     m.Transformer.finalize()
@@ -537,7 +569,8 @@ def load_model_args(modelDir: str, max_seq_len: int = 2048) -> dict:
     return {f: getattr(c, f) for f, _ in _capi.ModelArgsC._fields_}
 
 
-def LoadModel(modelDir: str, device: int = 0, tp_rank: int = 0, tp_size: int = 1, nccl_id=None, max_seq_len: int = 2048) -> Model:
+def LoadModel(modelDir: str, device: int = 0, tp_rank: int = 0, tp_size: int = 1, nccl_id=None, max_seq_len: int = 2048,
+              weight_format: str = "bf16") -> Model:
     """model.LoadModel (src/model/loader.go:18-70): <modelDir>/consolidated.00.pth + params.json.
     tokenizer.model is optional here: when present it becomes model.Vocabulary and supplies / checks VocabSize like
     the reference (loader.go:84-120); when absent VocabSize falls back to the rows of tok_embeddings.weight."""
@@ -561,7 +594,7 @@ def LoadModel(modelDir: str, device: int = 0, tp_rank: int = 0, tp_size: int = 1
         if t is None:
             raise _capi.LnbError(-1, 'tensor "tok_embeddings.weight" not found')
         d["vocab_size"] = t.Size[0]
-    m = Model(ModelArgs.from_c_dict(d), device, tp_rank, tp_size, nccl_id)
+    m = Model(ModelArgs.from_c_dict(d), device, tp_rank, tp_size, nccl_id, weight_format)
     if vocab is not None:
         m.Vocabulary = vocab
     try:

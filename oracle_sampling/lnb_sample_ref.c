@@ -5,6 +5,7 @@
  * sampler kernel (csrc/sample.cuh) against.  The floating-point steps come from csrc/sample_det.h, the header the kernel
  * compiles too.  orc_generate_sampled drives the CPU oracle's forward (oracle/lnb_oracle.h) like orc_generate, with the
  * sampler in place of the argmax. */
+#include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
@@ -608,4 +609,66 @@ int orc_generate_constrained(const orc_model* m, int vocab, const int32_t* promp
   free(tokens); free(hist); free(logits); free(proc); free(mask);
   orc_session_free(s);
   return n_out;
+}
+
+/* ---- MXFP8 weights (DESIGN.md §9h; the device form is csrc/mxfp8.cuh) ------------------------------------------------
+ * w: a row-major bf16 matrix [rows][cols]; codes [rows][cols], scales [rows][ceil(cols / 32)].  Each run of 32 columns of a
+ * row (the last one shorter) is a block: X = floor(log2(amax)) - 8 clamped to [-117, 119] (-117 for a zero block), scale
+ * byte X + 127; code = E4M3 of w * 2^-X, round to nearest even, magnitudes of 448 and above saturated to 448 (0x7E).  The
+ * scaled value is formed exactly in double.  Returns -1, or row * cols + col of the first non-finite weight (nothing is
+ * written then). */
+static uint8_t e4m3_rne_sat(double v) {
+  const uint8_t sign = signbit(v) ? 0x80 : 0;
+  const double a = fabs(v);
+  if (a >= 448.0) return sign | 0x7E;
+  if (a < 0x1p-6) return sign | (uint8_t)rint(a * 0x1p9);   /* subnormal quantum 2^-9; 8 quanta carry into 2^-6 = 0x08 */
+  int e;
+  frexp(a, &e);                                              /* a = f * 2^e, f in [0.5, 1): binade 2^(e-1) */
+  const double r = rint(ldexp(a, 3 - (e - 1)));              /* 8..16 eighths of the binade */
+  return sign | (uint8_t)((((e - 1) + 7) << 3) + (int)r - 8); /* r == 16 carries into the next binade */
+}
+int64_t orc_mxfp8_quantize(const uint16_t* w, int rows, int cols, uint8_t* codes, uint8_t* scales) {
+  for (int64_t i = 0; i < (int64_t)rows * cols; i++)
+    if ((w[i] & 0x7f80) == 0x7f80) return i;
+  const int nb = (cols + 31) / 32;
+  for (int r = 0; r < rows; r++)
+    for (int b = 0; b < nb; b++) {
+      const int c0 = b * 32, c1 = c0 + 32 < cols ? c0 + 32 : cols;
+      uint16_t amax = 0;
+      for (int c = c0; c < c1; c++) {
+        const uint16_t mag = w[(int64_t)r * cols + c] & 0x7fff;
+        if (mag > amax) amax = mag;
+      }
+      const int E = amax >> 7;
+      int X = E == 0 ? -117 : E - 127 - 8;
+      if (X < -117) X = -117;
+      if (X > 119) X = 119;
+      scales[(int64_t)r * nb + b] = (uint8_t)(X + 127);
+      for (int c = c0; c < c1; c++) {
+        const uint32_t bits = (uint32_t)w[(int64_t)r * cols + c] << 16;
+        float f;
+        memcpy(&f, &bits, 4);
+        codes[(int64_t)r * cols + c] = e4m3_rne_sat(ldexp((double)f, -X));
+      }
+    }
+  return -1;
+}
+/* e4m3(code) * 2^X as bf16 bits (exact: the value is zero or a normal number of at most 4 significant bits, so the f32
+ * product of the code's value and 2^X, X in [-117, 119], is exact too) */
+void orc_mxfp8_dequantize(const uint8_t* codes, const uint8_t* scales, int rows, int cols, uint16_t* out) {
+  float val[256];
+  for (int q = 0; q < 256; q++) {
+    const int e = (q >> 3) & 15, mnt = q & 7;
+    const double v = (q & 0x7f) == 0x7f ? NAN : e == 0 ? ldexp((double)mnt, -9) : ldexp(8.0 + mnt, e - 7 - 3);
+    val[q] = (float)((q & 0x80) ? -v : v);
+  }
+  const int nb = (cols + 31) / 32;
+  for (int r = 0; r < rows; r++)
+    for (int c = 0; c < cols; c++) {
+      const int X = (int)scales[(int64_t)r * nb + c / 32] - 127;
+      const float f = val[codes[(int64_t)r * cols + c]] * ldexpf(1.0f, X);
+      uint32_t bits;
+      memcpy(&bits, &f, 4);
+      out[(int64_t)r * cols + c] = (uint16_t)(bits >> 16);
+    }
 }

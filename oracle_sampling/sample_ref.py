@@ -83,6 +83,11 @@ def lib():
         L.orc_generate_constrained.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
                                                C.c_float, C.c_uint64, C.POINTER(Penalties), _i32p, _u8p, C.c_int, _u8p, _i64p,
                                                _i32p, C.c_int, C.c_int, _i32p]
+        _u16p = C.POINTER(C.c_uint16)
+        L.orc_mxfp8_quantize.restype = C.c_int64
+        L.orc_mxfp8_quantize.argtypes = [_u16p, C.c_int, C.c_int, _u8p, _u8p]
+        L.orc_mxfp8_dequantize.restype = None
+        L.orc_mxfp8_dequantize.argtypes = [_u8p, _u8p, C.c_int, C.c_int, _u16p]
         L.orc_generate_sampled.restype = C.c_int
         L.orc_generate_sampled.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
                                            C.c_float, C.c_uint64, _i32p]
@@ -328,3 +333,31 @@ def beam_search(om, prompt, seq_len: int, B: int, alpha: float = 1.0, early: boo
     if n < 0:
         raise RuntimeError("orc_beam_search failed")
     return _beam_out(n, tok, lp, ln, s, h, state), int(moves.value)
+
+
+def mxfp8_quantize(w) -> tuple[np.ndarray, np.ndarray]:
+    """orc_mxfp8_quantize of a bf16 matrix (uint16 bits [rows, cols]): (codes [rows, cols] u8, scales [rows, ceil(cols/32)]
+    u8).  A non-finite weight raises ValueError naming its row and column."""
+    w = np.ascontiguousarray(w, np.uint16)
+    rows, cols = w.shape
+    codes = np.empty((rows, cols), np.uint8)
+    scales = np.empty((rows, (cols + 31) // 32), np.uint8)
+    u8 = C.POINTER(C.c_uint8)
+    bad = lib().orc_mxfp8_quantize(w.ctypes.data_as(C.POINTER(C.c_uint16)), rows, cols, codes.ctypes.data_as(u8),
+                                   scales.ctypes.data_as(u8))
+    if bad >= 0:
+        raise ValueError(f"non-finite weight at row {bad // cols}, column {bad % cols}")
+    return codes, scales
+
+
+def mxfp8_dequantize(codes, scales) -> np.ndarray:
+    """orc_mxfp8_dequantize: the bf16 bits [rows, cols] of e4m3(code) * 2^X"""
+    codes = np.ascontiguousarray(codes, np.uint8)
+    scales = np.ascontiguousarray(scales, np.uint8)
+    rows, cols = codes.shape
+    assert scales.shape == (rows, (cols + 31) // 32)
+    out = np.empty((rows, cols), np.uint16)
+    u8 = C.POINTER(C.c_uint8)
+    lib().orc_mxfp8_dequantize(codes.ctypes.data_as(u8), scales.ctypes.data_as(u8), rows, cols,
+                               out.ctypes.data_as(C.POINTER(C.c_uint16)))
+    return out
