@@ -1249,6 +1249,55 @@ static void grammar_release(const lnb_grammar* g) {
   const_cast<lnb_grammar*>(g)->users--;
 }
 
+// A group of buffers allocated all or nothing: add() queues a device buffer and the byte it is filled with (-1: none),
+// add_host() a pinned host buffer.  commit() allocates every piece; only when all succeeded does it enqueue the fills on
+// `stream` and write the destinations.  On failure nothing is written: the CUDA error state is cleared, every piece is freed
+// and LNB_ENOMEM names what was being allocated, the bytes asked for (with the largest piece, when `big` names it) and why.
+struct AllocBatch {
+  struct Piece { void** dst; size_t bytes; int fill; bool host; void* p; };
+  std::vector<Piece> pieces;
+  size_t asked = 0;
+  template <class T> void add(T** dst, size_t bytes, int fill = -1) { pieces.push_back({(void**)dst, bytes, fill, false, nullptr}); asked += bytes; }
+  template <class T> void add_host(T** dst, size_t bytes) { pieces.push_back({(void**)dst, bytes, -1, true, nullptr}); asked += bytes; }
+  int commit(cudaStream_t stream, const char* what, const char* big = nullptr, size_t big_bytes = 0) {
+    cudaError_t e = cudaSuccess;
+    for (Piece& q : pieces)
+      if (e == cudaSuccess) e = q.host ? cudaMallocHost(&q.p, q.bytes) : cudaMalloc(&q.p, q.bytes);
+    bool filled = false;
+    for (Piece& q : pieces)
+      if (e == cudaSuccess && q.fill >= 0) { e = cudaMemsetAsync(q.p, q.fill, q.bytes, stream); filled = true; }
+    if (e == cudaSuccess) {
+      for (Piece& q : pieces) *q.dst = q.p;
+      return 0;
+    }
+    cudaGetLastError();
+    if (filled) cudaStreamSynchronize(stream);   // the fills enqueued so far may still write the pieces
+    for (Piece& q : pieces)
+      if (q.p) q.host ? cudaFreeHost(q.p) : cudaFree(q.p);
+    cudaGetLastError();
+    if (big) return fail(LNB_ENOMEM, "%s: %zu bytes of device memory asked for (%s %zu bytes): %s", what, asked, big, big_bytes, cudaGetErrorString(e));
+    return fail(LNB_ENOMEM, "%s: %zu bytes of device memory asked for: %s", what, asked, cudaGetErrorString(e));
+  }
+};
+
+// the generation controls of one sequence of a session
+struct SeqCtl {
+  bool samp = false;               // draws with its sampler parameters (lnb_session_set_sampling)
+  bool pen = false;                // penalized (lnb_session_set_penalties)
+  lnb_grammar* gram = nullptr;     // NULL: not constrained (lnb_session_set_grammar)
+  int lp_top = -1;                 // top_n of its logprobs, -1: off (lnb_session_set_logprobs)
+  // the sampler draws its tokens (sampled, penalized or constrained: greedy is then the sampler's rank 0 of l')
+  bool processed() const { return samp || pen || gram; }
+};
+// what the sequences of a call ask of it: any row processed, penalized, constrained, scoring (logprobs on), or drawing from
+// the greedy slot (processed without sampling)
+struct CtlSum {
+  bool processed = false, pen = false, gram = false, lp = false, greedy = false;
+  bool operator==(const CtlSum& o) const {
+    return processed == o.processed && pen == o.pen && gram == o.gram && lp == o.lp && greedy == o.greedy;
+  }
+};
+
 struct lnb_session {
   lnb_model* m = nullptr;
   int seq_len = 0, max_rows = 1, mode = LNB_ACC_FAST;
@@ -1338,9 +1387,10 @@ struct lnb_session {
   unsigned long long* d_samp_cand = nullptr;   // [samp_rows][SMP_MERGE] split-sampler candidates, then [samp_rows] u32 counters
   int samp_rows = 0;                        // rows one sampler launch may draw: n_seq, grown by speculative calls (samp_grow)
   int32_t* d_samp_tok = nullptr;
-  bool samp_on[8] = {false, false, false, false, false, false, false, false};
-  bool graph_sampled = false;               // the captured decode graph ends in the sampler ...
-  const float* graph_logits = nullptr;      // ... which reads this logits buffer
+  SeqCtl ctl[8];                            // the controls of each sequence
+  // what the captured decode graph runs after the forward (sampler, penalty, grammar and logprob jobs, the greedy slot) and
+  // the logits buffer those jobs read (NULL: none); a step that would run otherwise drops the graph
+  struct { CtlSum use; const float* logits = nullptr; } graph_key;
   // token log-probabilities (logprob.cuh, lnb_session_set_logprobs), allocated by the first enable: the records of every
   // sequence and position, the top_n of each sequence in device memory (a captured graph reads it there), the row table
   // and scratch of one job of up to lp_rows rows, and the targets of lnb_score
@@ -1351,8 +1401,6 @@ struct lnb_session {
   LpRow* h_lp_rows = nullptr;               // pinned staging of d_lp_rows
   unsigned long long* d_lp_cand = nullptr;  // [lp_rows][slices][LP_TOP], then [lp_rows][slices] + [lp_rows] u32 counters
   int lp_rows = 0;
-  int lp_top[8] = {-1, -1, -1, -1, -1, -1, -1, -1};   // -1: logprobs off
-  bool graph_lp = false;                    // the captured decode graph ends in the logprob job
   // penalties (penalty.cuh, lnb_session_set_penalties), allocated by the first enable: the token history of every sequence
   // and position, the parameters of each sequence in device memory (a captured graph reads them there), and one job's
   // counts and processed rows
@@ -1360,18 +1408,33 @@ struct lnb_session {
   lnb_penalties* d_pen = nullptr;           // [n_seq]
   unsigned int* d_pen_cnt = nullptr;        // [PEN_MAX_ROWS][vocab] (zero between jobs)
   float* d_pen_out = nullptr;               // [PEN_MAX_ROWS][vocab] l' (penalty and grammar jobs), read by the sampler
-  bool pen_on[8] = {false, false, false, false, false, false, false, false};
-  bool graph_pen = false, graph_greedy = false;   // the captured decode graph runs the penalty job / the greedy slot
   // grammars (grammar.cuh, lnb_session_set_grammar), allocated by the first enable: the grammar state before every
   // position of every sequence, and each sequence's grammar in device memory (a captured graph reads it there)
   int32_t* d_gst = nullptr;                 // [n_seq][seq_len + 1], -1: ⊥
   GrammarSlot* d_gslot = nullptr;           // [n_seq]
-  lnb_grammar* gram[8] = {};                // NULL: the sequence is not constrained
-  bool graph_gram = false;                  // the captured decode graph runs the grammar job
 };
 
-// a sequence whose tokens the sampler draws (sampled, penalized or constrained: greedy is then the sampler's rank 0 of l')
-static bool processed(const lnb_session* s, int seq) { return s->samp_on[seq] || s->pen_on[seq] || s->gram[seq]; }
+// the controls of sequences seq[0, n) (NULL: sequences 0..n-1), summarised
+static CtlSum ctl_sum(const lnb_session* s, int n, const int32_t* seq) {
+  CtlSum u;
+  for (int i = 0; i < n; i++) {
+    const SeqCtl& c = s->ctl[seq ? seq[i] : i];
+    u.processed |= c.processed();
+    u.pen |= c.pen;
+    u.gram |= c.gram != nullptr;
+    u.lp |= c.lp_top >= 0;
+    u.greedy |= c.processed() && !c.samp;
+  }
+  return u;
+}
+// the checks every per-sequence control call starts with; what (or NULL): the feature, refused under tensor parallelism
+static int seq_ctl_check(const lnb_session* s, int seq, const char* what) {
+  if (!s) return fail(LNB_EINVAL, "session is NULL");
+  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  if (what && s->m->tp_size > 1)
+    return fail(LNB_EINVAL, "%s: not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", what, s->m->tp_size);
+  return 0;
+}
 
 static int set_state(lnb_session* s, int pos, int n_rows, int next_token, bool reset_step) {
   return launch_kernel(Launcher{s->stream, LAUNCH_PLAIN, &s->launches}, set_state_kernel, dim3(1), dim3(1), 0, s->st, pos, n_rows,
@@ -1429,71 +1492,66 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
     }
   }
   s->stream_attn = stream_attn;
+  s->samp_rows = n_seq;
+  s->lp_rows = std::max(max_rows, 8);
   cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
-  // every allocation is counted, so a failure can say how much the session asked for
-  size_t asked = 0, failed_bytes = 0;
-  auto al = [&](void** p, size_t bytes) {
-    asked += bytes;
-    if (e != cudaSuccess) return;
-    e = cudaMalloc(p, bytes);
-    if (e != cudaSuccess) { failed_bytes = bytes; *p = nullptr; }
-  };
+  AllocBatch A;
   if (stream_attn || (!s->sdpa_smem_decode && ss_shape_ok(a.head_dim, a.n_heads / a.n_kv_heads))) {
     // streamed rows: every row of a long session, or the n_seq rows of a batched step
     size_t sc_b, z_b, op_b;
     ss_plan(s->ss, seq_len, stream_attn ? max_rows : n_seq, m->q_l / a.head_dim, a.head_dim, &sc_b, &z_b, &op_b);
-    al((void**)&s->ss.sc, sc_b);
-    al((void**)&s->ss.z, z_b);
-    al((void**)&s->ss.op, op_b);
+    A.add(&s->ss.sc, sc_b);
+    A.add(&s->ss.z, z_b);
+    A.add(&s->ss.op, op_b);
   }
-  al((void**)&s->x, (size_t)max_rows * a.dim * 2);
-  al((void**)&s->h1, (size_t)max_rows * a.dim * 2);
-  al((void**)&s->q, (size_t)max_rows * m->q_l * 2);
-  al((void**)&s->o, (size_t)max_rows * m->q_l * 2);
-  al((void**)&s->mbuf, (size_t)max_rows * m->ffn_l * 2);
-  al((void**)&s->part, (size_t)max_rows * a.dim * 4);
-  al((void**)&s->rs, (size_t)max_rows * 4);
+  A.add(&s->x, (size_t)max_rows * a.dim * 2);
+  A.add(&s->h1, (size_t)max_rows * a.dim * 2);
+  A.add(&s->q, (size_t)max_rows * m->q_l * 2);
+  A.add(&s->o, (size_t)max_rows * m->q_l * 2);
+  A.add(&s->mbuf, (size_t)max_rows * m->ffn_l * 2);
+  A.add(&s->part, (size_t)max_rows * a.dim * 4);
+  A.add(&s->rs, (size_t)max_rows * 4);
   if (max_rows >= 32 && acc_mode == LNB_ACC_FAST) {
     s->mpad = (max_rows + TC_BM - 1) / TC_BM * TC_BM;
-    al((void**)&s->xn8, (size_t)s->mpad * a.dim * 2);
-    al((void**)&s->o8, (size_t)s->mpad * m->q_l * 2);
-    al((void**)&s->m8, (size_t)s->mpad * m->ffn_l * 2);
-    al((void**)&s->qkv_raw, (size_t)max_rows * (m->q_l + 2 * m->kv_l) * 2);
-    al((void**)&s->gu, (size_t)max_rows * 2 * m->ffn_l * 2);
+    A.add(&s->xn8, (size_t)s->mpad * a.dim * 2);
+    A.add(&s->o8, (size_t)s->mpad * m->q_l * 2);
+    A.add(&s->m8, (size_t)s->mpad * m->ffn_l * 2);
+    A.add(&s->qkv_raw, (size_t)max_rows * (m->q_l + 2 * m->kv_l) * 2);
+    A.add(&s->gu, (size_t)max_rows * 2 * m->ffn_l * 2);
     if (m->wfmt == LNB_WEIGHTS_MXFP8) {
       for (const LinMat& x : linear_mats(m)) s->wdq_elems = std::max(s->wdq_elems, x.layer < 0 ? (size_t)TC_BN * x.K : (size_t)x.N * x.K);
-      al((void**)&s->wdq, s->wdq_elems * 2);
+      A.add(&s->wdq, s->wdq_elems * 2);
     }
   }
-  al((void**)&s->d_tokens, (size_t)max_rows * 4);
-  al((void**)&s->st, sizeof(LnbDevState));
-  al((void**)&s->d_tok_out, (size_t)seq_len * 4);
+  A.add(&s->d_tokens, (size_t)max_rows * 4);
+  A.add(&s->st, sizeof(LnbDevState), 0);
+  A.add(&s->d_tok_out, (size_t)seq_len * 4);
   s->ck.assign(a.n_layers, nullptr);
   s->cv.assign(a.n_layers, nullptr);
   const size_t cbytes = (size_t)n_seq * seq_len * m->kv_l * 2;
-  al((void**)&s->d_pos_arr, 8 * 4);
-  al((void**)&s->d_next_arr, 8 * 4);
+  A.add(&s->d_pos_arr, 8 * 4);
+  A.add(&s->d_next_arr, 8 * 4);
   for (int l = 0; l < a.n_layers; l++) {
-    al((void**)&s->ck[l], cbytes);
-    al((void**)&s->cv[l], cbytes);
-    if (e == cudaSuccess) e = cudaMemsetAsync(s->ck[l], 0, cbytes, s->stream);  // ml.Zeros, inferencecontext.go:31-43
-    if (e == cudaSuccess) e = cudaMemsetAsync(s->cv[l], 0, cbytes, s->stream);
+    A.add(&s->ck[l], cbytes, 0);  // ml.Zeros, inferencecontext.go:31-43
+    A.add(&s->cv[l], cbytes, 0);
   }
-  if (e == cudaSuccess) e = cudaMemsetAsync(s->st, 0, sizeof(LnbDevState), s->stream);
   const size_t in_words = row_map_words(max_rows);
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_tok, (in_words + 8 + seq_len + 8) * 4);
-  if (e == cudaSuccess) { s->h_pos = s->h_tok + in_words; s->h_out = s->h_tok + in_words + 8; }
-  if (e == cudaSuccess) e = cudaMallocHost((void**)&s->h_err, 64);
-  if (e == cudaSuccess) *s->h_err = 0;
-  if (e == cudaSuccess) e = cudaEventCreate(&s->ev0);
-  if (e == cudaSuccess) e = cudaEventCreate(&s->ev1);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
-  if (e != cudaSuccess) {
+  A.add_host(&s->h_tok, (in_words + 8 + seq_len + 8) * 4);
+  A.add_host(&s->h_err, 64);
+  int rc = e == cudaSuccess ? A.commit(s->stream, "session allocation", "KV cache", (size_t)2 * a.n_layers * cbytes) : 0;
+  if (rc == 0 && e == cudaSuccess) {
+    s->h_pos = s->h_tok + in_words;
+    s->h_out = s->h_tok + in_words + 8;
+    *s->h_err = 0;
+    e = cudaEventCreate(&s->ev0);
+    if (e == cudaSuccess) e = cudaEventCreate(&s->ev1);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
+  }
+  if (rc || e != cudaSuccess) {
     cudaGetLastError();
     lnb_session_destroy(s);
     cudaGetLastError();
-    return fail(LNB_ENOMEM, "session allocation failed: %zu bytes of device memory asked for (KV cache %zu bytes), %zu-byte allocation: %s",
-                asked, (size_t)2 * a.n_layers * cbytes, failed_bytes, cudaGetErrorString(e));
+    return rc ? rc : fail(LNB_ECUDA, "session setup failed: %s", cudaGetErrorString(e));
   }
   *out = s;
   return 0;
@@ -1521,7 +1579,7 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->d_hist); cudaFree(s->d_pen); cudaFree(s->d_pen_cnt); cudaFree(s->d_pen_out);
   cudaFree(s->d_gst); cudaFree(s->d_gslot);
   for (int q = 0; q < 8; q++)
-    if (s->gram[q]) grammar_release(s->gram[q]);
+    if (s->ctl[q].gram) grammar_release(s->ctl[q].gram);
   for (auto p : s->ck) cudaFree(p);
   for (auto p : s->cv) cudaFree(p);
   if (s->h_tok) cudaFreeHost(s->h_tok);
@@ -1721,16 +1779,15 @@ static bool engine_probe(lnb_session* s) {
     if (ce == cudaSuccess) ce = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, decode_engine_kernel<8>, ENG_THREADS, ENG_SMEM);
   }
   if (ce != cudaSuccess || occ < 1) { cudaGetLastError(); return no("the engine kernel does not fit an SM"); }
-  if (cudaMalloc((void**)&s->d_bar, 256) != cudaSuccess) { cudaGetLastError(); return no("cudaMalloc"); }
-  {
-    cudaError_t e2 = cudaMalloc((void**)&s->x_t, (size_t)a.dim * 4);
-    if (e2 == cudaSuccess) e2 = cudaMalloc((void**)&s->h1_t, (size_t)a.dim * 4);
-    if (e2 == cudaSuccess) e2 = cudaMalloc((void**)&s->qkv_t, (size_t)(m->q_l + 2 * m->kv_l) * 4);
-    if (e2 == cudaSuccess) e2 = cudaMalloc((void**)&s->o_t, (size_t)m->q_l * 4);
-    if (e2 == cudaSuccess) e2 = cudaMalloc((void**)&s->m_t, (size_t)m->ffn_l * 4);
-    if (e2 != cudaSuccess) { cudaGetLastError(); return no("cudaMalloc"); }
-    s->eng_tag = 0;   // forces the zero-fill of the tagged vectors before the first launch
-  }
+  AllocBatch A;
+  A.add(&s->d_bar, 256);
+  A.add(&s->x_t, (size_t)a.dim * 4);
+  A.add(&s->h1_t, (size_t)a.dim * 4);
+  A.add(&s->qkv_t, (size_t)(m->q_l + 2 * m->kv_l) * 4);
+  A.add(&s->o_t, (size_t)m->q_l * 4);
+  A.add(&s->m_t, (size_t)m->ffn_l * 4);
+  if (A.commit(s->stream, "decode engine buffers")) return no("cudaMalloc");
+  s->eng_tag = 0;   // forces the zero-fill of the tagged vectors before the first launch
   {
     const char* pe = getenv("LNB_ENGINE_PROF");
     if (pe && strcmp(pe, "0")) {
@@ -2048,17 +2105,15 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
   const int n_layers = active_layers(s);
   if (s->d_bphases && s->bkey_layers == n_layers && s->bkey_logits == logits_out) return 0;
   if (!s->bx) {
-    cudaError_t e = cudaMalloc((void**)&s->bx, (size_t)a.dim * 16);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&s->bh1, (size_t)a.dim * 16);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&s->bq, (size_t)m->q_l * 16);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&s->bo, (size_t)m->q_l * 16);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&s->bm, (size_t)m->ffn_l * 16);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&s->d_bkeys, 64);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&s->bxn, (size_t)a.dim * 16);
-    if (e != cudaSuccess) return fail(LNB_ENOMEM, "batch engine buffers: %s", cudaGetErrorString(e));
-    CU(cudaMemset(s->bx, 0, (size_t)a.dim * 16)); CU(cudaMemset(s->bh1, 0, (size_t)a.dim * 16));
-    CU(cudaMemset(s->bq, 0, (size_t)m->q_l * 16)); CU(cudaMemset(s->bo, 0, (size_t)m->q_l * 16));
-    CU(cudaMemset(s->bm, 0, (size_t)m->ffn_l * 16)); CU(cudaMemset(s->bxn, 0, (size_t)a.dim * 16));
+    AllocBatch A;
+    A.add(&s->bx, (size_t)a.dim * 16, 0);
+    A.add(&s->bh1, (size_t)a.dim * 16, 0);
+    A.add(&s->bq, (size_t)m->q_l * 16, 0);
+    A.add(&s->bo, (size_t)m->q_l * 16, 0);
+    A.add(&s->bm, (size_t)m->ffn_l * 16, 0);
+    A.add(&s->d_bkeys, 64);
+    A.add(&s->bxn, (size_t)a.dim * 16, 0);
+    if (const int rc = A.commit(s->stream, "batch engine buffers")) return rc;
     // FAST: the FMA-pipe kernel by default -- on an H100 (3.35 TB/s) it keeps up with the weight stream at 8 rows and beat
     // the tensor-core form, 880 vs 602 tokens/s (bench.py --config batch8 --acc fast, H100 SXM 700 W); LNB_BATCH_TC=1 selects
     // the tensor-core form (every K a multiple of 16)
@@ -2215,8 +2270,8 @@ static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int 
   R.head = logits_rows == 0 ? HEAD_NONE : logits_rows == 1 ? HEAD_LAST : HEAD_ALL;
   R.head_rows = logits_rows > 1 ? S : 1;
   R.advance = advance; R.gather = gather;
-  R.record = s->pen_on[s->active_seq];
-  R.grammar = s->gram[s->active_seq] != nullptr;
+  const CtlSum u = ctl_sum(s, 1, &s->active_seq);
+  R.record = u.pen; R.grammar = u.gram;
   return R;
 }
 // a batched step: row r is sequence r, token d_tokens[r] at position d_pos_arr[r]
@@ -2225,29 +2280,30 @@ static Rows rows_batch(const lnb_session* s, int n) {
   R.kind = ROWS_BATCH; R.S = n; R.tokens = s->d_tokens; R.pos_arr = s->d_pos_arr;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.head = HEAD_PER_ROW; R.head_rows = n;
-  for (int i = 0; i < n; i++) { R.record |= s->pen_on[i]; R.grammar |= s->gram[i] != nullptr; }
+  const CtlSum u = ctl_sum(s, n, nullptr);
+  R.record = u.pen; R.grammar = u.gram;
   return R;
 }
 // a ragged call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each, then the last row of each segment
-static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, bool record, bool grammar) {
+static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, const CtlSum& u) {
   Rows R{};
   R.kind = ROWS_RAGGED; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.mb_rows = 8;
   R.seg_last = s->d_rag + 3 * rows;
   R.head = HEAD_PER_ROW; R.head_rows = n_segs;
-  R.record = record; R.grammar = grammar;
+  R.record = u.pen; R.grammar = u.gram;
   return R;
 }
 // a speculative verification call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each; consecutive
 // rows of a segment are consecutive positions of one sequence, and EVERY row is an output row (its next token is compared
 // with the following draft), so the LM head runs over all of them
-static Rows rows_spec(const lnb_session* s, int rows, bool record, bool grammar) {
+static Rows rows_spec(const lnb_session* s, int rows, const CtlSum& u) {
   Rows R{};
   R.kind = ROWS_SPEC; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
   R.seq_stride = (long long)s->seq_len * s->m->kv_l;
   R.head = HEAD_PER_ROW; R.head_rows = rows;
-  R.record = record; R.grammar = grammar;
+  R.record = u.pen; R.grammar = u.gram;
   return R;
 }
 
@@ -2572,11 +2628,10 @@ static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_
   J.params = s->d_samp; J.wbuf = s->d_samp_w; J.pos_ptr = &s->st->pos; J.out = out;
   J.cand = s->d_samp_cand; J.cnt = reinterpret_cast<unsigned int*>(s->d_samp_cand + (size_t)s->samp_rows * SMP_MERGE);
   J.st = decode ? s->st : nullptr; J.tok_out = decode ? s->d_tok_out : nullptr;
-  bool pen = false, gram = false;
+  const CtlSum u = ctl_sum(s, n, seq);
+  const bool pen = u.pen, gram = u.gram;
   for (int i = 0; i < n; i++) {
-    J.row[i] = row[i]; J.slot[i] = s->samp_on[seq[i]] ? seq[i] : s->n_seq; J.p_next[i] = p_next[i]; J.out_idx[i] = out_idx ? out_idx[i] : 0;
-    pen |= s->pen_on[seq[i]];
-    gram |= s->gram[seq[i]] != nullptr;
+    J.row[i] = row[i]; J.slot[i] = s->ctl[seq[i]].samp ? seq[i] : s->n_seq; J.p_next[i] = p_next[i]; J.out_idx[i] = out_idx ? out_idx[i] : 0;
   }
   if (pen) {
     PenaltyJob P{};
@@ -2584,7 +2639,7 @@ static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_
     P.params = s->d_pen; P.hist = s->d_hist; P.hist_len = s->seq_len;
     P.cnt = s->d_pen_cnt; P.out = s->d_pen_out; P.pos_ptr = &s->st->pos;
     for (int i = 0; i < n; i++) {
-      P.row[i] = row[i]; P.slot[i] = seq[i]; P.seq[i] = seq[i]; P.p_next[i] = p_next[i]; P.on[i] = s->pen_on[seq[i]] ? 1 : 0;
+      P.row[i] = row[i]; P.slot[i] = seq[i]; P.seq[i] = seq[i]; P.p_next[i] = p_next[i]; P.on[i] = s->ctl[seq[i]].pen ? 1 : 0;
       J.row[i] = i;
     }
     int rc = launch_penalty_job(L, P);
@@ -2596,7 +2651,7 @@ static int launch_sample(lnb_session* s, int n, const int32_t* row, const int32_
     G.in = pen ? s->d_pen_out : s->logits; G.ld = pen ? V : s->m->vocab_l; G.out = s->d_pen_out; G.V = V; G.n = n;
     G.slots = s->d_gslot; G.gst = s->d_gst; G.gst_len = s->seq_len + 1; G.pos_ptr = &s->st->pos;
     for (int i = 0; i < n; i++) {
-      G.row[i] = pen ? i : row[i]; G.seq[i] = seq[i]; G.p_next[i] = p_next[i]; G.on[i] = s->gram[seq[i]] ? 1 : 0;
+      G.row[i] = pen ? i : row[i]; G.seq[i] = seq[i]; G.p_next[i] = p_next[i]; G.on[i] = s->ctl[seq[i]].gram ? 1 : 0;
       J.row[i] = i;
     }
     int rc = launch_kernel(L, grammar_apply_kernel, dim3((V + GRM_SLICE - 1) / GRM_SLICE, n), dim3(GRM_THREADS), 0, G);
@@ -2660,11 +2715,12 @@ static int call_tail(lnb_session* s, int n, int row0, const int32_t* seq, const 
   int32_t srow[8], sseq[8], spn[8], sidx[8];
   int ns = 0, nl = 0;
   for (int i = 0; i < n; i++)
-    if (processed(s, seq[i])) { srow[ns] = row0 + i; sseq[ns] = seq[i]; spn[ns] = p_next[i]; sidx[ns] = i; ns++; }
+    if (s->ctl[seq[i]].processed()) { srow[ns] = row0 + i; sseq[ns] = seq[i]; spn[ns] = p_next[i]; sidx[ns] = i; ns++; }
   int rc;
   if (ns && (rc = launch_sample(s, ns, srow, sseq, spn, sidx, samp_out, false))) return rc;
   for (int i = 0; i < n; i++)
-    if (s->lp_top[seq[i]] >= 0) lp_row(s, nl++, row0 + i, processed(s, seq[i]) ? samp_out + i : greedy + i, seq[i], p_next[i], nullptr);
+    if (s->ctl[seq[i]].lp_top >= 0)
+      lp_row(s, nl++, row0 + i, s->ctl[seq[i]].processed() ? samp_out + i : greedy + i, seq[i], p_next[i], nullptr);
   if (nl && ((rc = lp_upload(s, nl)) || (rc = launch_logprob(s, nl)))) return rc;
   lnb_model* m = s->m;
   if (host_logits) {
@@ -2699,8 +2755,9 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
   CU(cudaSetDevice(m->device));
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
   const int32_t seq = s->active_seq, p_next = start_pos + S;
-  const bool samp = processed(s, seq);   // the sampler and the logprob job read the last row's logits
-  const int lrows = keep_logits ? (all_rows ? S : 1) : ((samp || s->lp_top[seq] >= 0) ? 1 : 0);
+  const CtlSum u = ctl_sum(s, 1, &seq);   // the sampler and the logprob job read the last row's logits
+  const bool samp = u.processed;
+  const int lrows = keep_logits ? (all_rows ? S : 1) : ((samp || u.lp) ? 1 : 0);
   int rc;
   if (lrows && (rc = ensure_logits(s, (size_t)(keep_logits && all_rows ? s->max_rows : 1)))) return rc;
   if (S == 1 && engine_ok(s)) {
@@ -2864,49 +2921,31 @@ static int sampling_check(const lnb_sampling* p) {
   if (!(p->top_p > 0.0f && p->top_p <= 1.0f)) return fail(LNB_EINVAL, "top_p %g must be in (0, 1]", (double)p->top_p);
   return 0;
 }
-// The sampler's buffers, allocated by the first sampler set or penalty enable: n_seq parameter slots plus the greedy slot
-// d_samp[n_seq] (zeroed: temperature 0) of penalized sequences that do not sample, weights of n_seq rows, one token; all or
-// nothing
-static int samp_alloc(lnb_session* s) {
-  if (s->d_samp) return 0;
-  const size_t b_par = (size_t)(s->n_seq + 1) * sizeof(lnb_sampling), b_w = (size_t)s->n_seq * s->m->a.vocab_size * 8;
-  const size_t b_cand = (size_t)s->n_seq * (SMP_MERGE * 8 + 4);
-  lnb_sampling* d_par = nullptr;
-  unsigned long long *d_w = nullptr, *d_cand = nullptr;
-  int32_t* d_tok = nullptr;
-  cudaError_t e = cudaMalloc((void**)&d_par, b_par);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&d_w, b_w);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&d_tok, 16);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&d_cand, b_cand);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_par, 0, b_par, s->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_cand, 0, b_cand, s->stream);   // the split sampler's counters start at 0
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    cudaStreamSynchronize(s->stream);
-    cudaFree(d_par); cudaFree(d_w); cudaFree(d_tok); cudaFree(d_cand);
-    cudaGetLastError();
-    return fail(LNB_ENOMEM, "sampler buffers: %zu bytes of device memory asked for: %s", b_par + b_w + 16 + b_cand, cudaGetErrorString(e));
-  }
-  s->d_samp = d_par; s->d_samp_w = d_w; s->d_samp_tok = d_tok; s->d_samp_cand = d_cand;
-  s->samp_rows = s->n_seq;
-  return 0;
+// The sampler's buffers, added to A by the first sampler set, penalty or grammar enable: n_seq parameter slots plus the
+// greedy slot d_samp[n_seq] (zeroed: temperature 0) of processed sequences that do not sample, weights of samp_rows rows,
+// one token
+static void samp_add(lnb_session* s, AllocBatch& A) {
+  if (s->d_samp) return;
+  A.add(&s->d_samp, (size_t)(s->n_seq + 1) * sizeof(lnb_sampling), 0);
+  A.add(&s->d_samp_w, (size_t)s->samp_rows * s->m->a.vocab_size * 8);
+  A.add(&s->d_samp_tok, 16);
+  A.add(&s->d_samp_cand, (size_t)s->samp_rows * (SMP_MERGE * 8 + 4), 0);   // the split sampler's counters start at 0
 }
 extern "C" int lnb_session_set_sampling(lnb_session* s, int seq, const lnb_sampling* p) {
-  if (!s) return fail(LNB_EINVAL, "session is NULL");
-  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
-  if (s->m->tp_size > 1)
-    return fail(LNB_EINVAL, "sampling is not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", s->m->tp_size);
-  int rc;
+  int rc = seq_ctl_check(s, seq, "sampling");
+  if (rc) return rc;
   if (p && (rc = sampling_check(p))) return rc;
   const bool on = p && p->temperature > 0.0f;
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(s->m->device));
-  if (on && (rc = samp_alloc(s))) return rc;
   if (on) {   // stream-ordered, no host synchronisation; a captured decode graph reads the slot when it replays
+    AllocBatch A;
+    samp_add(s, A);
+    if ((rc = A.commit(s->stream, "sampler buffers"))) return rc;
     sample_set_params_kernel<<<1, 1, 0, s->stream>>>(s->d_samp + seq, *p);
     CU(cudaGetLastError());
   }
-  s->samp_on[seq] = on;
+  s->ctl[seq].samp = on;
   return 0;
 }
 
@@ -2930,54 +2969,31 @@ static int penalties_check(const lnb_penalties* p, int V) {
   return 0;
 }
 extern "C" int lnb_session_set_penalties(lnb_session* s, int seq, const lnb_penalties* p) {
-  if (!s) return fail(LNB_EINVAL, "session is NULL");
-  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
-  if (s->m->tp_size > 1)
-    return fail(LNB_EINVAL, "penalties are not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", s->m->tp_size);
+  int rc = seq_ctl_check(s, seq, "penalties");
+  if (rc) return rc;
   const int V = s->m->a.vocab_size;
-  int rc;
   if (p && (rc = penalties_check(p, V))) return rc;
   const bool on = p && !lnb_pen_neutral(p);
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(s->m->device));
-  if (on && !s->d_hist) {   // history of every sequence and position, parameter slots, the job's scratch; all or nothing
-    const size_t b_hist = (size_t)s->n_seq * s->seq_len * 4, b_par = (size_t)s->n_seq * sizeof(lnb_penalties),
-                 b_cnt = (size_t)PEN_MAX_ROWS * V * 4, b_out = (size_t)PEN_MAX_ROWS * V * 4;
-    int32_t* d_hist = nullptr;
-    lnb_penalties* d_par = nullptr;
-    unsigned int* d_cnt = nullptr;
-    float* d_out = s->d_pen_out;   // (the processed rows: allocated here or by the first grammar enable)
-    cudaError_t e = cudaMalloc((void**)&d_hist, b_hist);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_par, b_par);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_cnt, b_cnt);
-    if (e == cudaSuccess && !d_out) e = cudaMalloc((void**)&d_out, b_out);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_hist, 0xff, b_hist, s->stream);   // -1: no token recorded
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_cnt, 0, b_cnt, s->stream);        // the counts start at 0
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      cudaStreamSynchronize(s->stream);
-      cudaFree(d_hist); cudaFree(d_par); cudaFree(d_cnt);
-      if (d_out != s->d_pen_out) cudaFree(d_out);
-      cudaGetLastError();
-      return fail(LNB_ENOMEM, "penalty history and scratch: %zu bytes of device memory asked for (history %zu): %s",
-                  b_hist + b_par + b_cnt + b_out, b_hist, cudaGetErrorString(e));
-    }
-    if ((rc = samp_alloc(s))) {   // the sampler draws every penalized token
-      cudaStreamSynchronize(s->stream);
-      cudaFree(d_hist); cudaFree(d_par); cudaFree(d_cnt);
-      if (d_out != s->d_pen_out) cudaFree(d_out);
-      return rc;
-    }
-    s->d_hist = d_hist; s->d_pen = d_par; s->d_pen_cnt = d_cnt; s->d_pen_out = d_out;
-  } else if (on && (rc = samp_alloc(s))) {
-    return rc;
-  }
   if (on) {   // stream-ordered, no host synchronisation; a captured decode graph reads the slot when it replays
-    if (!s->pen_on[seq]) CU(cudaMemsetAsync(s->d_hist + (size_t)seq * s->seq_len, 0xff, (size_t)s->seq_len * 4, s->stream));
+    // history of every sequence and position, parameter slots, the job's scratch, and the sampler, which draws every
+    // penalized token
+    AllocBatch A;
+    const size_t b_hist = (size_t)s->n_seq * s->seq_len * 4;
+    if (!s->d_hist) {
+      A.add(&s->d_hist, b_hist, 0xff);                            // -1: no token recorded
+      A.add(&s->d_pen, (size_t)s->n_seq * sizeof(lnb_penalties));
+      A.add(&s->d_pen_cnt, (size_t)PEN_MAX_ROWS * V * 4, 0);       // the counts start at 0
+    }
+    if (!s->d_pen_out) A.add(&s->d_pen_out, (size_t)PEN_MAX_ROWS * V * 4);   // (shared with the grammar job)
+    samp_add(s, A);
+    if ((rc = A.commit(s->stream, "penalty history and scratch", "history", b_hist))) return rc;
+    if (!s->ctl[seq].pen) CU(cudaMemsetAsync(s->d_hist + (size_t)seq * s->seq_len, 0xff, (size_t)s->seq_len * 4, s->stream));
     penalty_set_params_kernel<<<1, 1, 0, s->stream>>>(s->d_pen + seq, *p);
     CU(cudaGetLastError());
   }
-  s->pen_on[seq] = on;
+  s->ctl[seq].pen = on;
   return 0;
 }
 
@@ -3033,20 +3049,18 @@ extern "C" int lnb_grammar_create(lnb_model* m, const char* regex, int64_t len, 
   unsigned int* d_stuck = nullptr;
   cudaStream_t st = nullptr;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
-  cudaError_t e = cudaMalloc((void**)&g->d_trans, b_trans);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&g->d_masks, b_masks);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&g->d_bytes, b_bytes);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&g->d_off, b_off);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&d_accept, Q + 4);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&d_stuck, 4);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    cudaFree(d_accept); cudaFree(d_stuck);
+  AllocBatch A;
+  A.add(&g->d_trans, b_trans);
+  A.add(&g->d_masks, b_masks);
+  A.add(&g->d_bytes, b_bytes);
+  A.add(&g->d_off, b_off);
+  A.add(&d_accept, Q + 4);
+  A.add(&d_stuck, 4);
+  int rc = A.commit(nullptr, "grammar tables", "masks", b_masks);
+  if (rc) {
     grammar_free(g);
-    return fail(LNB_ENOMEM, "grammar tables: %lld bytes of device memory asked for (masks %zu): %s", (long long)(g->bytes + Q + 4),
-                b_masks, cudaGetErrorString(e));
+    return rc;
   }
-  int rc = 0;
   auto run = [&]() -> int {
     CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
     CU(cudaEventCreate(&e0));
@@ -3111,45 +3125,23 @@ extern "C" int lnb_grammar_destroy(lnb_grammar* g) {
 }
 
 extern "C" int lnb_session_set_grammar(lnb_session* s, int seq, const lnb_grammar* g, int first_pos) {
-  if (!s) return fail(LNB_EINVAL, "session is NULL");
-  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
-  if (s->m->tp_size > 1)
-    return fail(LNB_EINVAL, "grammars are not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", s->m->tp_size);
+  int rc = seq_ctl_check(s, seq, "grammars");
+  if (rc) return rc;
   if (g && g->m != s->m) return fail(LNB_EINVAL, "the grammar was created for another model");
   if (g && (first_pos < 0 || first_pos > s->seq_len)) return fail(LNB_EINVAL, "first_pos %d outside [0, %d]", first_pos, s->seq_len);
-  const int V = s->m->a.vocab_size;
-  int rc;
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(s->m->device));
-  if (g && !s->d_gst) {   // state history of every sequence and position, slots, processed rows; all or nothing
-    const size_t b_gst = (size_t)s->n_seq * (s->seq_len + 1) * 4, b_slot = (size_t)s->n_seq * sizeof(GrammarSlot),
-                 b_out = s->d_pen_out ? 0 : (size_t)PEN_MAX_ROWS * V * 4;
-    int32_t* d_gst = nullptr;
-    GrammarSlot* d_slot = nullptr;
-    float* d_out = s->d_pen_out;
-    cudaError_t e = cudaMalloc((void**)&d_gst, b_gst);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_slot, b_slot);
-    if (e == cudaSuccess && !d_out) e = cudaMalloc((void**)&d_out, b_out);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_gst, 0xff, b_gst, s->stream);    // -1: ⊥
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_slot, 0, b_slot, s->stream);     // no grammar
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      cudaStreamSynchronize(s->stream);
-      cudaFree(d_gst); cudaFree(d_slot);
-      if (d_out != s->d_pen_out) cudaFree(d_out);
-      cudaGetLastError();
-      return fail(LNB_ENOMEM, "grammar state history and slots: %zu bytes of device memory asked for (history %zu): %s",
-                  b_gst + b_slot + b_out, b_gst, cudaGetErrorString(e));
+  if (g) {   // state history of every sequence and position, slots, processed rows, and the sampler, which draws every
+             // constrained token
+    AllocBatch A;
+    const size_t b_gst = (size_t)s->n_seq * (s->seq_len + 1) * 4;
+    if (!s->d_gst) {
+      A.add(&s->d_gst, b_gst, 0xff);                                 // -1: ⊥
+      A.add(&s->d_gslot, (size_t)s->n_seq * sizeof(GrammarSlot), 0);  // no grammar
     }
-    if ((rc = samp_alloc(s))) {   // the sampler draws every constrained token
-      cudaStreamSynchronize(s->stream);
-      cudaFree(d_gst); cudaFree(d_slot);
-      if (d_out != s->d_pen_out) cudaFree(d_out);
-      return rc;
-    }
-    s->d_gst = d_gst; s->d_gslot = d_slot; s->d_pen_out = d_out;
-  } else if (g && (rc = samp_alloc(s))) {
-    return rc;
+    if (!s->d_pen_out) A.add(&s->d_pen_out, (size_t)PEN_MAX_ROWS * s->m->a.vocab_size * 4);   // (shared with the penalty job)
+    samp_add(s, A);
+    if ((rc = A.commit(s->stream, "grammar state history and slots", "history", b_gst))) return rc;
   }
   if (s->d_gslot) {   // stream-ordered, no host synchronisation; a captured decode graph reads the slot when it replays
     GrammarSlot v{};
@@ -3168,66 +3160,46 @@ extern "C" int lnb_session_set_grammar(lnb_session* s, int seq, const lnb_gramma
   {
     std::lock_guard<std::mutex> lk(g_grammar_mu);
     if (g) const_cast<lnb_grammar*>(g)->users++;
-    if (s->gram[seq]) const_cast<lnb_grammar*>(s->gram[seq])->users--;
+    if (s->ctl[seq].gram) s->ctl[seq].gram->users--;
   }
-  s->gram[seq] = const_cast<lnb_grammar*>(g);
+  s->ctl[seq].gram = const_cast<lnb_grammar*>(g);
   return 0;
 }
 
 // ---- token log-probabilities: records, switches and scoring (logprob.cuh, DESIGN.md §9d) ------------------------------
 extern "C" int lnb_session_set_logprobs(lnb_session* s, int seq, int top_n) {
-  if (!s) return fail(LNB_EINVAL, "session is NULL");
-  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  int rc = seq_ctl_check(s, seq, "logprobs");
+  if (rc) return rc;
   if (top_n < -1 || top_n > LNB_LOGPROBS_TOP_MAX) return fail(LNB_EINVAL, "top_n %d must be in [-1, %d] (-1: off)", top_n, LNB_LOGPROBS_TOP_MAX);
-  if (s->m->tp_size > 1)
-    return fail(LNB_EINVAL, "logprobs are not built for tensor parallelism (tp_size %d: the logits are sharded over the vocabulary)", s->m->tp_size);
   const int V = s->m->a.vocab_size;
   if (V > LP_MAX_VOCAB) return fail(LNB_EINVAL, "logprobs serve vocabularies of up to %d tokens (this model has %d)", LP_MAX_VOCAB, V);
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(s->m->device));
-  if (top_n >= 0 && !s->d_lp_rec) {   // records of every sequence and position, the job's table and scratch; all or nothing
-    const int rows = std::max(s->max_rows, 8), G = (V + LP_SLICE - 1) / LP_SLICE;
-    const size_t b_rec = (size_t)s->n_seq * (s->seq_len + 1) * sizeof(LpRecord), b_top = (size_t)s->n_seq * 4,
-                 b_tgt = (size_t)s->max_rows * 4, b_rows = (size_t)rows * sizeof(LpRow),
-                 b_cand = (size_t)rows * G * (LP_TOP * 8 + 4) + (size_t)rows * 4;
-    LpRecord* d_rec = nullptr;
-    int32_t *d_top = nullptr, *d_tgt = nullptr;
-    LpRow *d_rows = nullptr, *h_rows = nullptr;
-    unsigned long long* d_cand = nullptr;
-    cudaError_t e = cudaMalloc((void**)&d_rec, b_rec);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_top, b_top);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_tgt, b_tgt);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_rows, b_rows);
-    if (e == cudaSuccess) e = cudaMalloc((void**)&d_cand, b_cand);
-    if (e == cudaSuccess) e = cudaMallocHost((void**)&h_rows, b_rows);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_rec, 0xff, b_rec, s->stream);   // target -1: never written
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_top, 0xff, b_top, s->stream);
-    if (e == cudaSuccess) e = cudaMemsetAsync(d_cand, 0, b_cand, s->stream);     // the merge counters start at 0
-    if (e != cudaSuccess) {
-      cudaGetLastError();
-      cudaStreamSynchronize(s->stream);
-      cudaFree(d_rec); cudaFree(d_top); cudaFree(d_tgt); cudaFree(d_rows); cudaFree(d_cand);
-      if (h_rows) cudaFreeHost(h_rows);
-      cudaGetLastError();
-      return fail(LNB_ENOMEM, "logprob records and scratch: %zu bytes of device memory asked for (records %zu): %s",
-                  b_rec + b_top + b_tgt + b_rows + b_cand, b_rec, cudaGetErrorString(e));
-    }
-    s->d_lp_rec = d_rec; s->d_lp_top = d_top; s->d_lp_tgt = d_tgt; s->d_lp_rows = d_rows; s->d_lp_cand = d_cand; s->h_lp_rows = h_rows;
-    s->lp_rows = rows;
+  if (top_n >= 0 && !s->d_lp_rec) {   // records of every sequence and position, the job's table and scratch
+    const int rows = s->lp_rows, G = (V + LP_SLICE - 1) / LP_SLICE;
+    const size_t b_rec = (size_t)s->n_seq * (s->seq_len + 1) * sizeof(LpRecord);
+    AllocBatch A;
+    A.add(&s->d_lp_rec, b_rec, 0xff);   // target -1: never written
+    A.add(&s->d_lp_top, (size_t)s->n_seq * 4, 0xff);
+    A.add(&s->d_lp_tgt, (size_t)s->max_rows * 4);
+    A.add(&s->d_lp_rows, (size_t)rows * sizeof(LpRow));
+    A.add(&s->d_lp_cand, (size_t)rows * G * (LP_TOP * 8 + 4) + (size_t)rows * 4, 0);   // the merge counters start at 0
+    A.add_host(&s->h_lp_rows, (size_t)rows * sizeof(LpRow));
+    if ((rc = A.commit(s->stream, "logprob records and scratch", "records", b_rec))) return rc;
   }
   if (s->d_lp_top) {   // stream-ordered; a captured decode graph reads the slot when it replays
-    if (top_n >= 0 || s->lp_top[seq] >= 0) {
+    if (top_n >= 0 || s->ctl[seq].lp_top >= 0) {
       logprob_set_top_n_kernel<<<1, 1, 0, s->stream>>>(s->d_lp_top + seq, top_n);
       CU(cudaGetLastError());
     }
   }
-  s->lp_top[seq] = top_n;
+  s->ctl[seq].lp_top = top_n;
   return 0;
 }
 
 extern "C" int lnb_session_logprobs_read(lnb_session* s, int seq, int pos0, int n, lnb_logprob* out) {
-  if (!s || !out) return fail(LNB_EINVAL, "NULL argument");
-  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  if (!out) return fail(LNB_EINVAL, "NULL argument");
+  if (const int rc = seq_ctl_check(s, seq, nullptr)) return rc;
   if (n < 1 || pos0 < 1 || (int64_t)pos0 + n - 1 > s->seq_len)
     return fail(LNB_EINVAL, "positions [%d, %lld) outside [1, %d]", pos0, (long long)pos0 + n, s->seq_len);
   std::lock_guard<std::mutex> lk(s->mu);
@@ -3249,7 +3221,7 @@ extern "C" int lnb_score(lnb_session* s, const int32_t* tokens, int n, int start
   if (n < 2 || n - 1 > s->max_rows) return fail(LNB_EINVAL, "n %d must be in [2, max_rows + 1 = %d]", n, s->max_rows + 1);
   if (tokens[n - 1] < 0 || tokens[n - 1] >= s->m->a.vocab_size) return fail(LNB_EINVAL, "token id %d out of range", tokens[n - 1]);
   std::lock_guard<std::mutex> lk(s->mu);
-  if (s->lp_top[s->active_seq] < 0)
+  if (s->ctl[s->active_seq].lp_top < 0)
     return fail(LNB_ESTATE, "sequence %d has logprobs off (lnb_session_set_logprobs)", s->active_seq);
   CU(cudaSetDevice(s->m->device));
   // the targets, stream-ordered before the job: staged in the pinned h_tok words [max_rows, 2 max_rows), beside the forward's
@@ -3334,12 +3306,12 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
   CU(cudaMemcpyAsync(s->d_tokens, s->h_tok, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
   CU(cudaMemcpyAsync(s->d_pos_arr, s->h_pos, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
   int32_t seq[8], p_next[8];
-  bool samp = false;   // a row is processed or has logprobs on: the engine stores the logits
-  for (int i = 0; i < n; i++) { seq[i] = i; p_next[i] = positions[i] + 1; samp |= processed(s, i) || s->lp_top[i] >= 0; }
+  for (int i = 0; i < n; i++) { seq[i] = i; p_next[i] = positions[i] + 1; }
+  const CtlSum u = ctl_sum(s, n, nullptr);   // a row is processed or has logprobs on: the engine stores the logits
   if (batch_engine_ok(s)) {
     // ONE launch of the batch engine: every weight matrix streamed once for all n sequences
     if ((rc = launch_record(s, rows_batch(s, n)))) return rc;
-    if ((rc = batch_engine_build(s, (logits || samp) ? s->logits : nullptr))) return rc;
+    if ((rc = batch_engine_build(s, (logits || u.processed || u.lp) ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, n, s->d_tokens, s->d_pos_arr, nullptr))) return rc;
     if (logits && (rc = gather_logits(s, 0, n))) return rc;
   } else {
@@ -3354,38 +3326,77 @@ extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const in
 }
 
 // ---- ragged calls (continuous batching): segments of several sequences at their own positions in ONE forward ----------
-// Buffers of the first ragged call: the row map on the device and, when the session has none or a smaller one,
-// stream-attention scratch for max_rows rows per launch group.  Nothing is replaced unless every allocation succeeded, so a
-// failure (LNB_ENOMEM) leaves the session as it was.
-static int ragged_alloc(lnb_session* s) {
-  lnb_model* m = s->m;
-  const lnb_model_args& a = m->a;
-  const size_t words = row_map_words(s->max_rows);
+// The row map of ragged and speculative calls, allocated by the first one, and for ragged calls (streamed) stream-attention
+// scratch for max_rows rows per launch group when the session has none or a smaller one.  Nothing is replaced unless every
+// allocation succeeded, so a failure (LNB_ENOMEM) leaves the session as it was.
+static int ensure_row_map(lnb_session* s, bool streamed) {
+  const lnb_model* m = s->m;
+  AllocBatch A;
+  if (!s->d_rag) A.add(&s->d_rag, row_map_words(s->max_rows) * 4);
   SsScratch x{};
   size_t sc_b, z_b, op_b;
-  ss_plan(x, s->seq_len, s->max_rows, m->q_l / a.head_dim, a.head_dim, &sc_b, &z_b, &op_b);
-  const bool need_ss = !s->ss.sc || s->ss.rows < x.rows;
-  if (s->d_rag && !need_ss) return 0;
-  const size_t asked = (s->d_rag ? 0 : words * 4) + (need_ss ? sc_b + z_b + op_b : 0);
-  int32_t* d_rag = nullptr;
-  cudaError_t e = cudaSuccess;
-  if (!s->d_rag) e = cudaMalloc((void**)&d_rag, words * 4);
-  if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.sc, sc_b);
-  if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.z, z_b);
-  if (e == cudaSuccess && need_ss) e = cudaMalloc((void**)&x.op, op_b);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    cudaFree(d_rag); cudaFree(x.sc); cudaFree(x.z); cudaFree(x.op);
-    cudaGetLastError();
-    return fail(LNB_ENOMEM, "ragged-call buffers: %zu bytes of device memory asked for (stream-attention scratch for %d rows: %zu): %s", asked,
-                x.rows, need_ss ? sc_b + z_b + op_b : (size_t)0, cudaGetErrorString(e));
+  ss_plan(x, s->seq_len, s->max_rows, m->q_l / m->a.head_dim, m->a.head_dim, &sc_b, &z_b, &op_b);
+  const bool need_ss = streamed && (!s->ss.sc || s->ss.rows < x.rows);
+  if (need_ss) {
+    A.add(&x.sc, sc_b);
+    A.add(&x.z, z_b);
+    A.add(&x.op, op_b);
   }
-  if (d_rag) s->d_rag = d_rag;
+  if (const int rc = A.commit(s->stream, "row map", need_ss ? "stream-attention scratch" : nullptr, sc_b + z_b + op_b)) return rc;
   if (need_ss) {
     CU(cudaStreamSynchronize(s->stream));   // batched steps may still read the old scratch
     cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
     s->ss = x;
   }
+  return 0;
+}
+
+// The segments of a ragged or speculative call: segment i feeds rows(i) = cnt[i] + extra tokens of sequence seq[i] at
+// positions start_pos[i] + k (ragged: cnt = len, extra 0; speculative: cnt = n_draft, extra 1).
+struct Segments {
+  int n;
+  const int32_t *seq, *start_pos, *cnt;
+  int extra;
+  int64_t rows(int i) const { return (int64_t)cnt[i] + extra; }
+};
+// Each segment names its own sequence of the session, has at least one row and stays inside SequenceLength; the rows total
+// at most `budget` and carry token ids in range.  *rows: the row count.
+static int segments_check(const lnb_session* s, const Segments& g, const int32_t* tokens, int budget, int* rows) {
+  if (g.n < 1 || g.n > s->n_seq) return fail(LNB_EINVAL, "n_segs %d must be in [1, %d] (the session's sequences)", g.n, s->n_seq);
+  bool used[8] = {false, false, false, false, false, false, false, false};
+  int64_t total = 0;
+  for (int i = 0; i < g.n; i++) {
+    const int q = g.seq[i];
+    if (q < 0 || q >= s->n_seq) return fail(LNB_EINVAL, "segment %d: sequence %d out of range (session has %d)", i, q, s->n_seq);
+    if (used[q]) return fail(LNB_EINVAL, "segment %d: sequence %d has a segment already (one per sequence per call)", i, q);
+    used[q] = true;
+    if (g.rows(i) < 1) return fail(LNB_EINVAL, "segment %d: %lld rows, must be >= 1", i, (long long)g.rows(i));
+    if (g.start_pos[i] < 0 || g.start_pos[i] + g.rows(i) > s->seq_len)
+      return fail(LNB_EINVAL, "segment %d: positions [%d, %lld) exceed SequenceLength %d", i, g.start_pos[i],
+                  (long long)(g.start_pos[i] + g.rows(i)), s->seq_len);
+    total += g.rows(i);
+  }
+  if (total > budget)
+    return fail(LNB_EINVAL, "the segments carry %lld rows, more than the call's budget of %d (max_rows %d)", (long long)total, budget,
+                s->max_rows);
+  *rows = (int)total;
+  for (int r = 0; r < *rows; r++)
+    if (tokens[r] < 0 || tokens[r] >= s->m->a.vocab_size) return fail(LNB_EINVAL, "token id %d (row %d) out of range", tokens[r], r);
+  return 0;
+}
+// the row map in d_rag, [tokens | row_seq | row_pos | last row of each segment]: one pinned staging copy (the host words stay
+// in s->h_tok for the rest of the call)
+static int stage_row_map(lnb_session* s, const Segments& g, const int32_t* tokens, int rows) {
+  int32_t* h = s->h_tok;
+  memcpy(h, tokens, (size_t)rows * 4);
+  for (int i = 0, r = 0; i < g.n; i++) {
+    for (int k = 0; k < g.rows(i); k++, r++) {
+      h[rows + r] = g.seq[i];
+      h[2 * rows + r] = g.start_pos[i] + k;
+    }
+    h[3 * rows + i] = r - 1;
+  }
+  CU(cudaMemcpyAsync(s->d_rag, h, (size_t)(3 * rows + g.n) * 4, cudaMemcpyHostToDevice, s->stream));
   return 0;
 }
 
@@ -3397,43 +3408,16 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
   if (m->tp_size > 1) return fail(LNB_EINVAL, "lnb_forward_ragged is not built for tensor parallelism (tp_size %d)", m->tp_size);
   if (!ss_shape_ok(a.head_dim, a.n_heads / a.n_kv_heads))
     return fail(LNB_EINVAL, "ragged calls run the streamed attention kernels, which serve head_dim <= 128 and n_rep <= 8");
-  if (n_segs < 1 || n_segs > s->n_seq) return fail(LNB_EINVAL, "n_segs %d must be in [1, %d] (the session's sequences)", n_segs, s->n_seq);
-  bool used[8] = {false, false, false, false, false, false, false, false};
-  int64_t rows64 = 0;
-  for (int i = 0; i < n_segs; i++) {
-    if (seq[i] < 0 || seq[i] >= s->n_seq) return fail(LNB_EINVAL, "segment %d: sequence %d out of range (session has %d)", i, seq[i], s->n_seq);
-    if (used[seq[i]]) return fail(LNB_EINVAL, "segment %d: sequence %d has a segment already (one per sequence per call)", i, seq[i]);
-    used[seq[i]] = true;
-    if (len[i] < 1) return fail(LNB_EINVAL, "segment %d: len %d must be >= 1", i, len[i]);
-    if (start_pos[i] < 0 || (int64_t)start_pos[i] + len[i] > s->seq_len)
-      return fail(LNB_EINVAL, "segment %d: positions [%d, %lld) exceed SequenceLength %d", i, start_pos[i], (long long)start_pos[i] + len[i],
-                  s->seq_len);
-    rows64 += len[i];
-  }
-  if (rows64 > s->max_rows) return fail(LNB_EINVAL, "the segments carry %lld rows, more than the session's max_rows %d", (long long)rows64, s->max_rows);
-  const int rows = (int)rows64;
-  for (int r = 0; r < rows; r++)
-    if (tokens[r] < 0 || tokens[r] >= a.vocab_size) return fail(LNB_EINVAL, "token id %d (row %d) out of range", tokens[r], r);
+  const Segments g{n_segs, seq, start_pos, len, 0};
+  int rows, rc;
+  if ((rc = segments_check(s, g, tokens, s->max_rows, &rows))) return rc;
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(m->device));
-  int rc;
-  if ((rc = ragged_alloc(s))) return rc;
+  if ((rc = ensure_row_map(s, true))) return rc;
   if ((rc = ensure_logits(s, (size_t)n_segs))) return rc;
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward
-  // [tokens | row_seq | row_pos | last row of each segment]: one pinned staging copy
-  int32_t* h = s->h_tok;
-  memcpy(h, tokens, (size_t)rows * 4);
-  for (int i = 0, r = 0; i < n_segs; i++) {
-    for (int k = 0; k < len[i]; k++, r++) {
-      h[rows + r] = seq[i];
-      h[2 * rows + r] = start_pos[i] + k;
-    }
-    h[3 * rows + i] = r - 1;
-  }
-  CU(cudaMemcpyAsync(s->d_rag, h, (size_t)(3 * rows + n_segs) * 4, cudaMemcpyHostToDevice, s->stream));
-  bool pen = false, gram = false;
-  for (int i = 0; i < n_segs; i++) { pen |= s->pen_on[seq[i]]; gram |= s->gram[seq[i]] != nullptr; }
-  if ((rc = enqueue_forward(s, rows_ragged(s, rows, n_segs, pen, gram)))) return rc;
+  if ((rc = stage_row_map(s, g, tokens, rows))) return rc;
+  if ((rc = enqueue_forward(s, rows_ragged(s, rows, n_segs, ctl_sum(s, n_segs, seq))))) return rc;
   int32_t p_next[8];
   for (int i = 0; i < n_segs; i++) p_next[i] = start_pos[i] + len[i];
   if ((rc = call_tail(s, n_segs, 0, seq, p_next, s->d_next_arr, s->d_next_arr, logits, n_segs, argmax_out ? s->d_next_arr : nullptr))) return rc;
@@ -3447,18 +3431,12 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
 // sampler holds the old scratch: it is dropped and re-captured by the next lnb_decode_run.
 static int samp_grow(lnb_session* s, int rows) {
   if (s->samp_rows >= rows) return 0;
-  const size_t b_w = (size_t)rows * s->m->a.vocab_size * 8, b_cand = (size_t)rows * (SMP_MERGE * 8 + 4);
   unsigned long long *d_w = nullptr, *d_cand = nullptr;
-  cudaError_t e = cudaMalloc((void**)&d_w, b_w);
-  if (e == cudaSuccess) e = cudaMalloc((void**)&d_cand, b_cand);
-  if (e == cudaSuccess) e = cudaMemsetAsync(d_cand, 0, b_cand, s->stream);   // the split sampler's counters start at 0
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    cudaFree(d_w); cudaFree(d_cand);
-    cudaGetLastError();
-    return fail(LNB_ENOMEM, "sampler scratch for %d rows: %zu bytes of device memory asked for: %s", rows, b_w + b_cand, cudaGetErrorString(e));
-  }
-  if (s->graph_sampled) drop_graph(s);
+  AllocBatch A;
+  A.add(&d_w, (size_t)rows * s->m->a.vocab_size * 8);
+  A.add(&d_cand, (size_t)rows * (SMP_MERGE * 8 + 4), 0);   // the split sampler's counters start at 0
+  if (const int rc = A.commit(s->stream, "speculative sampler scratch")) return rc;
+  if (s->graph_key.use.processed) drop_graph(s);
   CU(cudaStreamSynchronize(s->stream));   // earlier sampler launches may still use the old scratch
   cudaFree(s->d_samp_w); cudaFree(s->d_samp_cand);
   s->d_samp_w = d_w; s->d_samp_cand = d_cand; s->samp_rows = rows;
@@ -3469,30 +3447,12 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
                                        const int32_t* tokens, float* logits, int32_t* next_out, int32_t* n_accepted) {
   if (!s || !seq || !start_pos || !n_draft || !tokens) return fail(LNB_EINVAL, "NULL argument");
   lnb_model* m = s->m;
-  const lnb_model_args& a = m->a;
   if (m->tp_size > 1) return fail(LNB_EINVAL, "lnb_forward_speculative is not built for tensor parallelism (tp_size %d)", m->tp_size);
-  if (n_segs < 1 || n_segs > s->n_seq) return fail(LNB_EINVAL, "n_segs %d must be in [1, %d] (the session's sequences)", n_segs, s->n_seq);
-  const int budget = std::min(8, s->max_rows);
-  bool used[8] = {false, false, false, false, false, false, false, false};
-  int64_t rows64 = 0;
-  for (int i = 0; i < n_segs; i++) {
-    if (seq[i] < 0 || seq[i] >= s->n_seq) return fail(LNB_EINVAL, "segment %d: sequence %d out of range (session has %d)", i, seq[i], s->n_seq);
-    if (used[seq[i]]) return fail(LNB_EINVAL, "segment %d: sequence %d has a segment already (one per sequence per call)", i, seq[i]);
-    used[seq[i]] = true;
-    if (n_draft[i] < 0) return fail(LNB_EINVAL, "segment %d: n_draft %d must be >= 0", i, n_draft[i]);
-    if (start_pos[i] < 0 || (int64_t)start_pos[i] + n_draft[i] >= s->seq_len)
-      return fail(LNB_EINVAL, "segment %d: positions [%d, %lld] exceed SequenceLength %d", i, start_pos[i],
-                  (long long)start_pos[i] + n_draft[i], s->seq_len);
-    rows64 += 1 + (int64_t)n_draft[i];
-  }
-  if (rows64 > budget)
-    return fail(LNB_EINVAL, "the segments carry %lld rows, more than min(8, max_rows) = %d", (long long)rows64, budget);
-  const int rows = (int)rows64;
-  for (int r = 0; r < rows; r++)
-    if (tokens[r] < 0 || tokens[r] >= a.vocab_size) return fail(LNB_EINVAL, "token id %d (row %d) out of range", tokens[r], r);
+  const Segments g{n_segs, seq, start_pos, n_draft, 1};
+  int rows, rc;
+  if ((rc = segments_check(s, g, tokens, std::min(8, s->max_rows), &rows))) return rc;
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(m->device));
-  int rc;
   if (rows == 1) {
     // no draft: the ordinary S=1 step of that sequence (the decode engine or the chain, same bits), so a call without drafts
     // costs exactly a plain step
@@ -3509,43 +3469,21 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
   const bool eng = spec_engine_ok(s, rows);
   if (!eng && !s->sdpa_smem_decode && !s->ss.sc)
     return fail(LNB_EINVAL, "speculative calls beyond the shared-memory attention kernel need head_dim <= 128 and n_rep <= 8");
-  int32_t row_seq[8], row_pos[8];
-  bool samp = false, lp = false, pen = false, gram = false;
-  for (int i = 0, r = 0; i < n_segs; i++)
-    for (int k = 0; k <= n_draft[i]; k++, r++) {
-      row_seq[r] = seq[i];
-      row_pos[r] = start_pos[i] + k;
-      samp |= processed(s, seq[i]);
-      pen |= s->pen_on[seq[i]];
-      gram |= s->gram[seq[i]] != nullptr;
-      lp |= s->lp_top[seq[i]] >= 0;
-    }
-  if (!s->d_rag) {   // the row map (shared with ragged calls)
-    const cudaError_t e = cudaMalloc((void**)&s->d_rag, row_map_words(s->max_rows) * 4);
-    if (e != cudaSuccess) {
-      s->d_rag = nullptr;
-      cudaGetLastError();
-      return fail(LNB_ENOMEM, "speculative row map: %zu bytes of device memory asked for: %s", row_map_words(s->max_rows) * 4,
-                  cudaGetErrorString(e));
-    }
-  }
-  if (samp && (rc = samp_grow(s, rows))) return rc;
+  const CtlSum u = ctl_sum(s, n_segs, seq);
+  if ((rc = ensure_row_map(s, false))) return rc;
+  if (u.processed && (rc = samp_grow(s, rows))) return rc;
   if ((rc = ensure_logits(s, (size_t)rows))) return rc;
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward
-  // [tokens | row_seq | row_pos]: one pinned staging copy
-  int32_t* h = s->h_tok;
-  memcpy(h, tokens, (size_t)rows * 4);
-  memcpy(h + rows, row_seq, (size_t)rows * 4);
-  memcpy(h + 2 * rows, row_pos, (size_t)rows * 4);
-  CU(cudaMemcpyAsync(s->d_rag, h, (size_t)3 * rows * 4, cudaMemcpyHostToDevice, s->stream));
+  if ((rc = stage_row_map(s, g, tokens, rows))) return rc;
+  const int32_t *row_seq = s->h_tok + rows, *row_pos = s->h_tok + 2 * rows;
   if (eng) {
     // ONE launch of the batch engine: every weight matrix streamed once for all rows
-    if ((rc = launch_record(s, rows_spec(s, rows, pen, gram)))) return rc;
-    if ((rc = batch_engine_build(s, (logits || samp || lp) ? s->logits : nullptr))) return rc;
+    if ((rc = launch_record(s, rows_spec(s, rows, u)))) return rc;
+    if ((rc = batch_engine_build(s, (logits || u.processed || u.lp) ? s->logits : nullptr))) return rc;
     if ((rc = batch_engine_launch(s, rows, s->d_rag, s->d_rag + 2 * rows, s->d_rag + rows))) return rc;
   } else {
     if ((rc = set_state(s, 0, rows, -1, false))) return rc;
-    if ((rc = enqueue_forward(s, rows_spec(s, rows, pen, gram)))) return rc;
+    if ((rc = enqueue_forward(s, rows_spec(s, rows, u)))) return rc;
   }
   int32_t p_next[8];
   for (int r = 0; r < rows; r++) p_next[r] = row_pos[r] + 1;
@@ -3576,15 +3514,15 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
   // penalized sequence records its token, runs the penalty job and draws from the sampler (greedy: its rank 0) each step; a
   // constrained one advances its grammar state and masks the row the same way.
   const int seq = s->active_seq;
-  const bool pen = s->pen_on[seq], gram = s->gram[seq] != nullptr, samp = processed(s, seq), greedy_slot = samp && !s->samp_on[seq];
-  const bool lp = s->lp_top[seq] >= 0, keep = samp || lp;
-  if (s->samp_on[seq] && engine_ok(s)) g_err = "the active sequence samples: lnb_decode_run runs the kernel chain (the decode engine has no sampler)";
-  else if (pen && engine_ok(s))
-    g_err = "the active sequence is penalized: lnb_decode_run runs the kernel chain (the decode engine keeps no token history)";
-  else if (gram && engine_ok(s))
-    g_err = "the active sequence is constrained by a grammar: lnb_decode_run runs the kernel chain (the decode engine keeps no grammar state)";
-  else if (lp && engine_ok(s))
-    g_err = "the active sequence has logprobs on: lnb_decode_run runs the kernel chain (the decode engine keeps no logits row)";
+  const SeqCtl& c = s->ctl[seq];
+  const CtlSum u = ctl_sum(s, 1, &seq);
+  const bool samp = u.processed, lp = u.lp, keep = samp || lp;
+  if (keep && engine_ok(s))
+    g_err = std::string("the active sequence ") +
+            (c.samp  ? "samples: lnb_decode_run runs the kernel chain (the decode engine has no sampler)"
+             : c.pen ? "is penalized: lnb_decode_run runs the kernel chain (the decode engine keeps no token history)"
+             : c.gram ? "is constrained by a grammar: lnb_decode_run runs the kernel chain (the decode engine keeps no grammar state)"
+                      : "has logprobs on: lnb_decode_run runs the kernel chain (the decode engine keeps no logits row)");
   if (!keep && engine_ok(s)) {
     // the whole run is ONE launch of the persistent engine: n_steps forwards, the greedy token fed back on the device
     if ((rc = engine_build(s, -1, nullptr))) return rc;
@@ -3602,10 +3540,8 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     return use_graph ? 1 : 0;   // (no graph is needed: there is nothing left to replay)
   }
   if (keep && (rc = ensure_logits(s, 1))) return rc;
-  if (s->graph_tried && (s->graph_sampled != samp || s->graph_lp != lp || s->graph_pen != pen || s->graph_gram != gram ||
-                         s->graph_greedy != greedy_slot ||
-                         (keep && s->graph_logits != s->logits)))
-    drop_graph(s);
+  const float* key_logits = keep ? s->logits : nullptr;
+  if (s->graph_tried && !(s->graph_key.use == u && s->graph_key.logits == key_logits)) drop_graph(s);
   if (lp) {   // the job's one row, read by every step (and by the graph's replays): the token st->next_token, record st->pos
     lp_row(s, 0, 0, &s->st->next_token, seq, 0, &s->st->pos);
     if ((rc = lp_upload(s, 1))) return rc;
@@ -3619,12 +3555,8 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
   };
   if (use_graph && !s->graph && !s->graph_tried) {
     s->graph_tried = true;
-    s->graph_sampled = samp;
-    s->graph_lp = lp;
-    s->graph_pen = pen;
-    s->graph_gram = gram;
-    s->graph_greedy = greedy_slot;
-    s->graph_logits = s->logits;
+    s->graph_key.use = u;
+    s->graph_key.logits = key_logits;
     cudaGraph_t g = nullptr;
     const int64_t saved = s->launches;
     cudaError_t e = cudaStreamBeginCapture(s->stream, cudaStreamCaptureModeThreadLocal);
