@@ -489,10 +489,24 @@ int lnb_session_p2p_import(lnb_session* s, const void* handles /* tp_size x 64 b
 int lnb_session_p2p_disable(lnb_session* s);
 
 /* debugging / parity probes */
-enum { LNB_BUF_RESIDUAL = 0, LNB_BUF_CACHE_K = 1, LNB_BUF_CACHE_V = 2, LNB_BUF_LOGITS = 3 };
+enum { LNB_BUF_RESIDUAL = 0, LNB_BUF_CACHE_K = 1, LNB_BUF_CACHE_V = 2, LNB_BUF_LOGITS = 3,
+       LNB_BUF_Q = 4, LNB_BUF_ATTN = 5, LNB_BUF_POST_ATTN = 6, LNB_BUF_NORMED = 7, LNB_BUF_FFN = 8 };
 /* copies a device buffer of the session to host: RESIDUAL [S,dim] bf16 (after the last
  * forward; with lnb_session_set_layer_limit, after that many layers), CACHE_K/V of `layer`
- * [seq_len, n_kv_local, head_dim] bf16, LOGITS [rows, vocab_local] f32. */
+ * [seq_len, n_kv_local, head_dim] bf16, LOGITS [rows, vocab_local] f32.
+ * Stage probes: the buffers of the last layer the last forward ran (with lnb_session_set_layer_limit(n), layer n-1), as
+ * row-major bf16 [rows, width] whatever the route's internal layout (X8 tiles on the tensor-core prompt path, chunk-major
+ * rows in the batch engine):
+ *   Q          [S, q_local]    the rotated queries
+ *   ATTN       [S, q_local]    the attention output (the Wo GEMM's input)
+ *   POST_ATTN  [S, dim]        h = x + Wo(attention); refused after a ragged call, whose LM head reuses the buffer
+ *   NORMED     [S, dim]        the normalised rows the last normalising GEMM read: the w1|w3 input, or, after a tensor-core
+ *                              prompt that kept all rows' logits or a tensor-core batch-engine step, the output norm of the
+ *                              final residual rows.  Refused on the kernel chain and the batch engine's FMA form, which
+ *                              normalise inside the GEMV prologue
+ *   FFN        [S, ffn_local]  SiLU(gate) * up, the w2 input
+ * RESIDUAL and the probes read at most the rows the last forward wrote (a batched step: one row per sequence, in call
+ * order).  After a decode-engine step only RESIDUAL is readable: the engine keeps its stage vectors as tagged words. */
 int lnb_session_read(lnb_session* s, int which, int layer, void* host, int64_t nbytes);
 int lnb_session_set_layer_limit(lnb_session* s, int n_layers_to_run); /* <=0: all */
 /* Which decode path does the session use?  1 = the persistent decode engine (csrc/engine.cuh: one kernel launch runs n

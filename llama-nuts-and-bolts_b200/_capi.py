@@ -9,6 +9,7 @@ LIB_PATH = os.path.join(_HERE, "liblnb.so")
 
 LNB_ACC_STRICT, LNB_ACC_FAST = 0, 1
 LNB_BUF_RESIDUAL, LNB_BUF_CACHE_K, LNB_BUF_CACHE_V, LNB_BUF_LOGITS = 0, 1, 2, 3
+LNB_BUF_Q, LNB_BUF_ATTN, LNB_BUF_POST_ATTN, LNB_BUF_NORMED, LNB_BUF_FFN = 4, 5, 6, 7, 8
 LNB_WEIGHTS_BF16, LNB_WEIGHTS_MXFP8 = 0, 1
 
 

@@ -1298,6 +1298,10 @@ struct CtlSum {
   }
 };
 
+// the route the session's last forward took: where lnb_session_read finds its residual stream and stage buffers, and in which
+// layout
+enum FwdRoute { FWD_NONE, FWD_CHAIN, FWD_TC, FWD_BATCH_ENGINE, FWD_DECODE_ENGINE };
+
 struct lnb_session {
   lnb_model* m = nullptr;
   int seq_len = 0, max_rows = 1, mode = LNB_ACC_FAST;
@@ -1367,7 +1371,9 @@ struct lnb_session {
   int bkey_layers = -1;
   const float* bkey_logits = nullptr;
   uint32_t eng_tag = 1;          // next free tag (tags of one launch: [eng_tag, eng_tag + n_steps * n_phases))
-  bool last_was_engine = false;  // the residual stream of the last forward lives in x_t
+  // the last forward: its route (FwdRoute), the rows it wrote, and whether its LM head reused h1 for the segments' last rows
+  int last_route = FWD_NONE, last_rows = 0;
+  bool last_h1_head = false;
   unsigned long long* d_prof = nullptr;   // LNB_ENGINE_PROF=1: per-CTA cycle counters of the engine's consumer thread 0
   int eng_state = 0;             // 0 = not probed, 1 = usable, -1 = this session uses the kernel chain
   bool eng_single_default = true; // single-sequence S=1 steps use the engine (false: single-GPU FAST, where the kernel chain is faster)
@@ -2070,7 +2076,7 @@ static int engine_launch(lnb_session* s, int n_steps, bool advance) {
     if (rc) return rc;
     done += n;
   }
-  s->last_was_engine = true;
+  s->last_route = FWD_DECODE_ENGINE; s->last_rows = 1; s->last_h1_head = false;
   return 0;
 }
 // after a failed stream sync: did the engine trap, and why?
@@ -2218,7 +2224,7 @@ static int batch_engine_launch(lnb_session* s, int n, const int32_t* tokens, con
   const int rc = launch_kernel(Launcher{s->stream, LAUNCH_COOP, &s->launches}, kern, dim3(m->sm_count), dim3(ENG_THREADS),
                                s->batch_tc ? BT_SMEM : ENG_SMEM, P);
   if (rc) return rc;
-  s->last_was_engine = false;
+  s->last_route = FWD_BATCH_ENGINE; s->last_rows = n; s->last_h1_head = false;
   return 0;
 }
 
@@ -2406,7 +2412,9 @@ static int launch_record(lnb_session* s, const Rows& R, int32_t token = -1, int 
 // Enqueue one LlamaTransformer.Forward (llamatransformer.go:145-180) for the rows R on the session stream: on the tensor
 // cores when forward_tc_ok, else as the kernel chain below.  Every forward but the decode engines' comes through here.
 static int enqueue_forward(lnb_session* s, const Rows& R) {
-  s->last_was_engine = false;   // this forward's residual stream is s->x
+  s->last_route = forward_tc_ok(s, R.S) ? FWD_TC : FWD_CHAIN;
+  s->last_rows = R.S;
+  s->last_h1_head = R.seg_last != nullptr;   // per_row_head compacts the segments' last rows into h1
   if (const int rc = launch_record(s, R)) return rc;
   if (forward_tc_ok(s, R.S)) return enqueue_forward_tc(s, R);
   lnb_model* m = s->m;
@@ -3575,6 +3583,7 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
     s->launches = saved;
   }
   const bool graph = use_graph && s->graph;
+  if (graph) { s->last_route = FWD_CHAIN; s->last_rows = 1; s->last_h1_head = false; }   // what a replay runs
   if ((rc = set_state(s, start_pos, 1, first_token, true))) return rc;
   CU(cudaEventRecord(s->ev0, s->stream));
   for (int i = 0; i < n_steps; i++) {
@@ -3748,24 +3757,86 @@ extern "C" int lnb_session_engine_profile(lnb_session* s, double* out16) {   // 
   return 0;
 }
 
+// layouts of the activation buffers a forward leaves behind: plain rows, the X8 tiles of the tensor-core GEMM operands
+// (x8_index), or the batch engine's chunk-major rows (cm_idx)
+enum { LAY_ROWS, LAY_X8, LAY_CM };
+// rows [0, nbytes / (2 width)) of a [*, width] bf16 activation buffer as row-major rows on the host
+static int read_rows(lnb_session* s, const uint16_t* src, int layout, int width, void* host, int64_t nbytes) {
+  const int rows = (int)(nbytes / ((int64_t)width * 2));
+  if (layout == LAY_ROWS) {
+    CU(cudaStreamSynchronize(s->stream));
+    CU(cudaMemcpy(host, src, (size_t)nbytes, cudaMemcpyDeviceToHost));
+    return 0;
+  }
+  if (nbytes % ((int64_t)width * 2)) return fail(LNB_EINVAL, "a tiled stage buffer is read in whole rows of %d values", width);
+  // the tiles that hold the rows: whole 128-row tiles (X8), or the 8 row slots of every chunk (chunk-major)
+  const size_t n = layout == LAY_X8 ? (size_t)(rows + TC_BM - 1) / TC_BM * TC_BM * width : (size_t)width * 8;
+  std::vector<uint16_t> t(n);
+  CU(cudaStreamSynchronize(s->stream));
+  CU(cudaMemcpy(t.data(), src, n * 2, cudaMemcpyDeviceToHost));
+  uint16_t* o = (uint16_t*)host;
+  for (int r = 0; r < rows; r++)
+    for (int c = 0; c < width; c++) o[(size_t)r * width + c] = t[layout == LAY_X8 ? x8_index(r, c, width) : cm_idx(r, c)];
+  return 0;
+}
+
 extern "C" int lnb_session_read(lnb_session* s, int which, int layer, void* host, int64_t nbytes) {
   if (!s || !host) return fail(LNB_EINVAL, "NULL argument");
   lnb_model* m = s->m;
   CU(cudaSetDevice(m->device));
   const void* src = nullptr;
   int64_t avail = 0;
+  const int route = s->last_route;
+  const bool tc = route == FWD_TC, be = route == FWD_BATCH_ENGINE;
+  if (which == LNB_BUF_RESIDUAL || (which >= LNB_BUF_Q && which <= LNB_BUF_FFN)) {
+    // a row-addressed buffer of the last forward: [rows, width] bf16, rows <= the rows that forward wrote
+    if (route == FWD_NONE) return fail(LNB_EINVAL, "buffer %d: the session has run no forward yet", which);
+    if (route == FWD_DECODE_ENGINE) {
+      if (which != LNB_BUF_RESIDUAL)
+        return fail(LNB_EINVAL, "buffer %d: the decode engine keeps its stage vectors as tagged words between phases; only the "
+                    "residual stream is readable after its steps", which);
+      // the engine keeps the residual stream as tagged words: strip the tags
+      if (nbytes > (int64_t)m->a.dim * 2) return fail(LNB_EINVAL, "the decode engine keeps one row");
+      std::vector<uint32_t> t((size_t)m->a.dim);
+      CU(cudaStreamSynchronize(s->stream));
+      CU(cudaMemcpy(t.data(), s->x_t, t.size() * 4, cudaMemcpyDeviceToHost));
+      uint16_t* o = (uint16_t*)host;
+      for (int64_t i = 0; i < nbytes / 2; i++) o[i] = (uint16_t)(t[(size_t)i] & 0xffffu);
+      return 0;
+    }
+    const uint16_t* buf = nullptr;
+    int width = 0, layout = be ? LAY_CM : LAY_ROWS;
+    switch (which) {
+      case LNB_BUF_RESIDUAL: buf = be ? s->bx : s->x; width = m->a.dim; break;
+      case LNB_BUF_Q: buf = be ? s->bq : s->q; width = m->q_l; break;
+      case LNB_BUF_ATTN:
+        buf = be ? s->bo : tc ? s->o8 : s->o; width = m->q_l;
+        if (tc) layout = LAY_X8;
+        break;
+      case LNB_BUF_POST_ATTN:
+        if (s->last_h1_head)
+          return fail(LNB_EINVAL, "buffer %d: the LM head of the last (ragged) call compacted its segments' last rows into it", which);
+        buf = be ? s->bh1 : s->h1; width = m->a.dim;
+        break;
+      case LNB_BUF_NORMED:
+        if (route == FWD_CHAIN)
+          return fail(LNB_EINVAL, "buffer %d: the kernel chain normalises inside the w1|w3 GEMV's prologue and keeps no rows", which);
+        if (be && !s->batch_tc)
+          return fail(LNB_EINVAL, "buffer %d: the batch engine's FMA form normalises inside its GEMV prologue and keeps no rows", which);
+        buf = be ? s->bxn : s->xn8; width = m->a.dim;
+        if (tc) layout = LAY_X8;
+        break;
+      case LNB_BUF_FFN:
+        buf = be ? s->bm : tc ? s->m8 : s->mbuf; width = m->ffn_l;
+        if (tc) layout = LAY_X8;
+        break;
+    }
+    if (nbytes < 0 || nbytes > (int64_t)s->last_rows * width * 2)
+      return fail(LNB_EINVAL, "buffer %d holds the %d rows of %d values the last forward wrote, %lld bytes requested", which, s->last_rows,
+                  width, (long long)nbytes);
+    return read_rows(s, buf, layout, width, host, nbytes);
+  }
   switch (which) {
-    case LNB_BUF_RESIDUAL:
-      if (s->last_was_engine) {   // the engine keeps the residual stream as tagged words: strip the tags
-        if (nbytes > (int64_t)m->a.dim * 2) return fail(LNB_EINVAL, "the decode engine keeps one row");
-        std::vector<uint32_t> t((size_t)m->a.dim);
-        CU(cudaStreamSynchronize(s->stream));
-        CU(cudaMemcpy(t.data(), s->x_t, t.size() * 4, cudaMemcpyDeviceToHost));
-        uint16_t* o = (uint16_t*)host;
-        for (int64_t i = 0; i < nbytes / 2; i++) o[i] = (uint16_t)(t[(size_t)i] & 0xffffu);
-        return 0;
-      }
-      src = s->x; avail = (int64_t)s->max_rows * m->a.dim * 2; break;
     case LNB_BUF_CACHE_K:
     case LNB_BUF_CACHE_V:
       if (layer < 0 || layer >= m->a.n_layers) return fail(LNB_EINVAL, "bad layer %d", layer);

@@ -7,6 +7,7 @@
 #include <stdint.h>
 
 #define LNB_DEVINL __device__ __forceinline__
+#define LNB_HDINL __host__ __device__ __forceinline__   // layout helpers the host also uses (lnb_session_read de-tiles with them)
 
 LNB_DEVINL float bf2f(uint16_t b) { return __uint_as_float(((uint32_t)b) << 16); }
 LNB_DEVINL uint16_t f2bf(float f) { return (uint16_t)(__float_as_uint(f) >> 16); }  // truncation

@@ -48,7 +48,7 @@ static_assert(TC_SMEM <= 227 * 1024, "shared memory per CTA");
 
 // ---- layout helpers for the tensor-core path (X8 = tile-major activations, see the header comment)
 // X8 address of element (row, col) of a [*, K] activation matrix
-LNB_DEVINL size_t x8_index(int row, int col, int K) {
+LNB_HDINL size_t x8_index(int row, int col, int K) {
   const size_t tile = (size_t)(row >> 7) * (K >> 7) + (col >> 7);                 // [M/128][K/128]
   const int g = (row >> 3) & 15, ch = (col >> 3) & 15;                            // [16 groups][16 chunks]
   return (((tile * 16 + g) * 16 + ch) * 8 + (row & 7)) * 8 + (col & 7);

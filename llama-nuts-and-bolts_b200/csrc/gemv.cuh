@@ -118,7 +118,7 @@ struct GemvCfg {
 
 // chunk-major activation layout of the batch engine: 8 sequences' values of one 8-element k-chunk are 128 contiguous bytes, so
 // the k-range of a k-tile is ONE contiguous block for all rows (engine_batch.cuh)
-LNB_DEVINL size_t cm_idx(int m, int n) { return ((((size_t)(n >> 3)) * 8 + (size_t)m) << 3) + (size_t)(n & 7); }
+LNB_HDINL size_t cm_idx(int m, int n) { return ((((size_t)(n >> 3)) * 8 + (size_t)m) << 3) + (size_t)(n & 7); }
 
 // one word of a tagged activation vector, as soon as its producer has stored it (bounded: a word that never comes is a
 // bug or a dead SM -> trap, never a hang)

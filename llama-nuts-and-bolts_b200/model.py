@@ -365,6 +365,20 @@ class InferenceContext:
         check(lib.lnb_session_read(self.h, _capi.LNB_BUF_RESIDUAL, 0, out.ctypes.data_as(C.c_void_p), out.nbytes))
         return out
 
+    _STAGES = {"q": (_capi.LNB_BUF_Q, "q"), "attn": (_capi.LNB_BUF_ATTN, "q"), "post_attn": (_capi.LNB_BUF_POST_ATTN, "dim"),
+               "normed": (_capi.LNB_BUF_NORMED, "dim"), "ffn": (_capi.LNB_BUF_FFN, "ffn")}
+
+    def stage(self, name: str, rows: int) -> np.ndarray:
+        """the first `rows` rows of a stage buffer of the last forward's last layer (lnb_session_read): "q" (rotated
+        queries), "attn" (attention output), "post_attn" (x + Wo), "normed" (the rows the last normalising GEMM read) or
+        "ffn" (SiLU(gate) * up), as [rows, width] bf16 bits"""
+        which, w = self._STAGES[name]
+        a, tp = self.transformer.args, self.transformer.tp_size
+        width = {"q": a.N_Heads * a.HeadDim // tp, "dim": a.Dim, "ffn": a.FFNDim // tp}[w]
+        out = np.empty((rows, width), np.uint16)
+        check(lib.lnb_session_read(self.h, which, 0, out.ctypes.data_as(C.c_void_p), out.nbytes))
+        return out
+
     def set_active_sequence(self, seq: int):
         check(lib.lnb_session_set_active_sequence(self.h, seq))
         self.active_seq = seq
