@@ -1226,7 +1226,7 @@ __global__ void publish_kernel(LnbDevState* st, int advance, int32_t* tok_out) {
   }
 }
 
-// words of a ragged call's row map [tokens | row_seq | row_pos | last row of each segment]: `rows` words each, <= 8 segments
+// words of a call's row map [tokens | row_seq | row_pos | last row of each segment]: `rows` words each, <= 8 segments
 static size_t row_map_words(int max_rows) { return (size_t)max_rows * 3 + 8; }
 
 // a compiled grammar (grammar.cuh, lnb_grammar_create): its device tables, and the sequences of sessions that use it
@@ -1325,13 +1325,11 @@ struct lnb_session {
   size_t logits_rows = 0;
   float* logits_full = nullptr;  // tp>1: gathered [rows, vocab]
   std::vector<uint16_t*> ck, cv;
-  int32_t* d_tokens = nullptr;
   LnbDevState* st = nullptr;
   int32_t* d_tok_out = nullptr;
-  // pinned staging, one allocation (at h_tok) carved into three views: token ids on their way to d_tokens, or a ragged
-  // call's row map on its way to d_rag [row_map_words]; the positions of a batched step on their way to d_pos_arr [8]; the
-  // tokens a call hands back [seq_len + 8]
-  int32_t *h_tok = nullptr, *h_pos = nullptr, *h_out = nullptr;
+  // pinned staging, one allocation (at h_tok) carved into two views: a call's token ids or row map on their way to d_rag
+  // [row_map_words]; the tokens a call hands back [seq_len + 8]
+  int32_t *h_tok = nullptr, *h_out = nullptr;
   uint32_t* h_err = nullptr;     // pinned mirror of st->ar_error (peer all-reduce timeout flag)
   // logits of the last forward stay in HBM (lnb_forward_device); the host reads rows / argmaxes on demand
   int kept_rows = 0;             // rows of s->logits that belong to the last forward (0: none)
@@ -1345,7 +1343,6 @@ struct lnb_session {
   // batched decode (BASELINE config 5): n_seq independent sequences share the weights; caches are
   // [n_seq][seq_len][kv]; single-sequence calls address the cache of `active_seq`
   int n_seq = 1, active_seq = 0;
-  int32_t* d_pos_arr = nullptr;   // [n_seq] positions of the current batched step
   int32_t* d_next_arr = nullptr;  // [n_seq] greedy tokens of the current batched step
   bool sdpa_smem_decode = false;  // the whole K/V history of one KV head fits in shared memory
   size_t sdpa_decode_smem = 0;
@@ -1353,7 +1350,7 @@ struct lnb_session {
   // (stream_attn); batched steps run it when sdpa_decode_kernel cannot.  Scratch for ss.rows rows per launch group.
   bool stream_attn = false;
   SsScratch ss{};
-  int32_t* d_rag = nullptr;       // the row map of a ragged call, allocated by the first one (ONE host-to-device copy per call)
+  int32_t* d_rag = nullptr;       // a call's row map [row_map_words], or its token ids alone (ONE host-to-device copy per call)
   int64_t launches = 0;
   // persistent decode engine (engine.cuh): the phase list of one S=1 step in device memory
   EnginePhase* d_phases = nullptr;
@@ -1420,11 +1417,11 @@ struct lnb_session {
   GrammarSlot* d_gslot = nullptr;           // [n_seq]
 };
 
-// the controls of sequences seq[0, n) (NULL: sequences 0..n-1), summarised
+// the controls of sequences seq[0, n), summarised
 static CtlSum ctl_sum(const lnb_session* s, int n, const int32_t* seq) {
   CtlSum u;
   for (int i = 0; i < n; i++) {
-    const SeqCtl& c = s->ctl[seq ? seq[i] : i];
+    const SeqCtl& c = s->ctl[seq[i]];
     u.processed |= c.processed();
     u.pen |= c.pen;
     u.gram |= c.gram != nullptr;
@@ -1529,25 +1526,23 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
       A.add(&s->wdq, s->wdq_elems * 2);
     }
   }
-  A.add(&s->d_tokens, (size_t)max_rows * 4);
+  const size_t in_words = row_map_words(max_rows);
+  A.add(&s->d_rag, in_words * 4);
   A.add(&s->st, sizeof(LnbDevState), 0);
   A.add(&s->d_tok_out, (size_t)seq_len * 4);
   s->ck.assign(a.n_layers, nullptr);
   s->cv.assign(a.n_layers, nullptr);
   const size_t cbytes = (size_t)n_seq * seq_len * m->kv_l * 2;
-  A.add(&s->d_pos_arr, 8 * 4);
   A.add(&s->d_next_arr, 8 * 4);
   for (int l = 0; l < a.n_layers; l++) {
     A.add(&s->ck[l], cbytes, 0);  // ml.Zeros, inferencecontext.go:31-43
     A.add(&s->cv[l], cbytes, 0);
   }
-  const size_t in_words = row_map_words(max_rows);
-  A.add_host(&s->h_tok, (in_words + 8 + seq_len + 8) * 4);
+  A.add_host(&s->h_tok, (in_words + seq_len + 8) * 4);
   A.add_host(&s->h_err, 64);
   int rc = e == cudaSuccess ? A.commit(s->stream, "session allocation", "KV cache", (size_t)2 * a.n_layers * cbytes) : 0;
   if (rc == 0 && e == cudaSuccess) {
-    s->h_pos = s->h_tok + in_words;
-    s->h_out = s->h_tok + in_words + 8;
+    s->h_out = s->h_tok + in_words;
     *s->h_err = 0;
     e = cudaEventCreate(&s->ev0);
     if (e == cudaSuccess) e = cudaEventCreate(&s->ev1);
@@ -1576,9 +1571,8 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->d_phases); cudaFree(s->d_bar); cudaFree(s->d_prof);
   cudaFree(s->x_t); cudaFree(s->h1_t); cudaFree(s->qkv_t); cudaFree(s->o_t); cudaFree(s->m_t);
   cudaFree(s->bx); cudaFree(s->bh1); cudaFree(s->bq); cudaFree(s->bo); cudaFree(s->bm); cudaFree(s->bxn); cudaFree(s->d_bphases); cudaFree(s->d_bkeys);
-  cudaFree(s->logits); cudaFree(s->logits_full); cudaFree(s->d_tokens); cudaFree(s->st); cudaFree(s->d_tok_out); cudaFree(s->d_pos_arr); cudaFree(s->d_next_arr);
+  cudaFree(s->logits); cudaFree(s->logits_full); cudaFree(s->d_rag); cudaFree(s->st); cudaFree(s->d_tok_out); cudaFree(s->d_next_arr);
   cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
-  cudaFree(s->d_rag);
   cudaFree(s->d_samp); cudaFree(s->d_samp_w); cudaFree(s->d_samp_tok); cudaFree(s->d_samp_cand);
   cudaFree(s->d_lp_rec); cudaFree(s->d_lp_top); cudaFree(s->d_lp_tgt); cudaFree(s->d_lp_rows); cudaFree(s->d_lp_cand);
   if (s->h_lp_rows) cudaFreeHost(s->h_lp_rows);
@@ -2101,10 +2095,6 @@ static bool batch_engine_usable(lnb_session* s) {
   if (e && !strcmp(e, "0")) return false;
   return true;
 }
-static bool batch_engine_ok(lnb_session* s) { return s->n_seq >= 2 && batch_engine_usable(s); }
-// speculative verification: a call of >= 2 rows runs the batch engine, single-sequence sessions included (engine_capable
-// already holds every position below the engine's limit, eng_sdpa_smem)
-static bool spec_engine_ok(lnb_session* s, int rows) { return rows >= 2 && batch_engine_usable(s); }
 static int batch_engine_build(lnb_session* s, const float* logits_out) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
@@ -2202,7 +2192,7 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
   s->bkey_layers = n_layers; s->bkey_logits = logits_out;
   return 0;
 }
-// n rows: token tokens[m] at position pos_arr[m] on the cache of sequence row_seq[m] (NULL: sequence m), already on the device
+// n rows: token tokens[m] at position pos_arr[m] on the cache of sequence row_seq[m], already on the device
 static int batch_engine_launch(lnb_session* s, int n, const int32_t* tokens, const int32_t* pos_arr, const int32_t* row_seq) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
@@ -2244,9 +2234,9 @@ static int enqueue_decode_engine(lnb_session* s, int32_t token, int start_pos, i
 }
 
 // The rows of one forward: where row r's token, position and KV cache come from, and what the LM head makes of them.
-// rows_single, rows_batch, rows_ragged and rows_spec are the only places that decide this; the forward builders read it from
-// here.
-enum RowsKind { ROWS_SINGLE, ROWS_BATCH, ROWS_RAGGED, ROWS_SPEC };
+// rows_single, rows_ragged and rows_spec are the only places that decide this; the forward builders read it from here.
+// Rows of several sequences always carry row_seq; without it every row is on the cache at cache_off.
+enum RowsKind { ROWS_SINGLE, ROWS_RAGGED, ROWS_SPEC };
 // what the LM head produces: the last row's greedy token with no logits kept, the last row's or every row's (NONE, LAST,
 // ALL); or, for output rows that each end their own sequence, the logits and a greedy token in d_next_arr per row (PER_ROW)
 enum RowsHead { HEAD_NONE, HEAD_LAST, HEAD_ALL, HEAD_PER_ROW };
@@ -2255,7 +2245,7 @@ struct Rows {
   int S;
   const int32_t* tokens;    // device token id of each row, or NULL: st->next_token (a device-driven decode step)
   const int32_t* pos_arr;   // device position of each row, or NULL: st->pos + r
-  const int32_t* row_seq;   // ragged, speculative: the sequence of each row
+  const int32_t* row_seq;   // ragged, speculative, batched: the sequence of each row
   size_t cache_off;         // elements to the cache every row addresses (the active sequence's), or 0
   long long seq_stride;     // rows on several caches: elements between consecutive sequences' caches, else 0
   int mb_rows;              // launch_gemv's mb_rows: ragged 8, else 0
@@ -2280,16 +2270,6 @@ static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int 
   R.record = u.pen; R.grammar = u.gram;
   return R;
 }
-// a batched step: row r is sequence r, token d_tokens[r] at position d_pos_arr[r]
-static Rows rows_batch(const lnb_session* s, int n) {
-  Rows R{};
-  R.kind = ROWS_BATCH; R.S = n; R.tokens = s->d_tokens; R.pos_arr = s->d_pos_arr;
-  R.seq_stride = (long long)s->seq_len * s->m->kv_l;
-  R.head = HEAD_PER_ROW; R.head_rows = n;
-  const CtlSum u = ctl_sum(s, n, nullptr);
-  R.record = u.pen; R.grammar = u.gram;
-  return R;
-}
 // a ragged call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each, then the last row of each segment
 static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, const CtlSum& u) {
   Rows R{};
@@ -2301,9 +2281,9 @@ static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, const CtlSum
   R.record = u.pen; R.grammar = u.gram;
   return R;
 }
-// a speculative verification call: the row map in d_rag, [tokens | row_seq | row_pos] of `rows` words each; consecutive
-// rows of a segment are consecutive positions of one sequence, and EVERY row is an output row (its next token is compared
-// with the following draft), so the LM head runs over all of them
+// a speculative verification call or a batched step (segments of one row): the row map in d_rag, [tokens | row_seq | row_pos]
+// of `rows` words each; consecutive rows of a segment are consecutive positions of one sequence, and EVERY row is an output
+// row (a verified row's next token is compared with the following draft), so the LM head runs over all of them
 static Rows rows_spec(const lnb_session* s, int rows, const CtlSum& u) {
   Rows R{};
   R.kind = ROWS_SPEC; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
@@ -2324,9 +2304,9 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
   const int32_t* pos_ptr = &s->st->pos;
   const float scale = attn_scale_bf16(a.head_dim);
   const int strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
-  // rows on a row -> position map (a batched step, or a speculative call whose rows follow each other in one sequence's
-  // cache): the decode kernel within its fit, else the streamed kernels -- the attention a batched step of those rows runs
-  const bool batched = R.kind == ROWS_BATCH || R.kind == ROWS_SPEC;
+  // ROWS_SPEC rows (a batched step, or a speculative call whose rows follow each other in one sequence's cache) run the
+  // decode kernel within its fit, else the streamed kernels
+  const bool spec = R.kind == ROWS_SPEC;
   auto streamed = [&]() {
     StreamAttn P{};
     P.q = s->q; P.ldq = m->q_l;
@@ -2339,7 +2319,7 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
     return launch_stream_attn(L, P, S, n_kv, s->ss);
   };
   if (R.kind == ROWS_RAGGED) return streamed();
-  if (!out_x8 && (S == 1 || batched) && s->sdpa_smem_decode)
+  if (!out_x8 && (S == 1 || spec) && s->sdpa_smem_decode)
     return launch_kernel(L, sdpa_decode_kernel, dim3(n_kv, S), dim3(128 * n_rep), s->sdpa_decode_smem, (const uint16_t*)s->q, ck, cv,
                          m->kv_l, n_rep, a.head_dim, out, pos_ptr, s->seq_len, strict, scale, R.pos_arr,
                          (long long)s->seq_len * m->kv_l, m->q_l, (const LnbDevState*)s->st, R.row_seq);
@@ -2351,7 +2331,7 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
     return launch_kernel(L, sdpa_prefill_kernel, dim3(n_q, (S + SP_QB - 1) / SP_QB), dim3(256), (size_t)SP_SMEM, (const uint16_t*)s->q,
                          m->q_l, ck, cv, m->kv_l, n_rep, out, m->q_l, pos_ptr, S, scale);
   }
-  if (batched || s->stream_attn) return streamed();
+  if (spec || s->stream_attn) return streamed();
   return launch_kernel(L, sdpa_kernel, dim3(n_q, S), dim3(128), (size_t)s->seq_len * 12 + (size_t)a.head_dim * 4, (const uint16_t*)s->q,
                        m->q_l, ck, cv, m->kv_l, n_rep, a.head_dim, out, m->q_l, pos_ptr, 0, S, S > 1 ? 1 : 0, strict, scale, out_x8);
 }
@@ -2397,7 +2377,7 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R);
 // (the decode engine).
 static int launch_record(lnb_session* s, const Rows& R, int32_t token = -1, int pos0 = -1) {
   const Launcher L{s->stream, LAUNCH_PDL, &s->launches};
-  const int seq = R.kind == ROWS_SINGLE ? s->active_seq : -1;
+  const int seq = s->active_seq;   // the sequence of rows without a row map
   if (R.record) {
     const int rc = launch_kernel(L, penalty_record_kernel, dim3((R.S + 255) / 256), dim3(256), 0, s->d_hist, s->seq_len,
                                  (const LnbDevState*)s->st, R.tokens, R.pos_arr, R.row_seq, seq, token, pos0, R.S);
@@ -2713,7 +2693,7 @@ static int lp_upload(lnb_session* s, int n) {
   return 0;
 }
 
-// The end of lnb_forward(_device), lnb_forward_batch, lnb_forward_ragged and lnb_forward_speculative.  Output row i is
+// The end of lnb_forward(_device), forward_segments and lnb_forward_ragged.  Output row i is
 // logits row row0 + i, of sequence seq[i] at next position p_next[i]; rows of processed sequences draw into samp_out[i], the
 // greedy token of row i is at greedy[i].  Rows of sequences with logprobs on then write the record of p_next[i] for the
 // token they emit.  host_logits (or NULL) gets logits rows [0, logits_rows), s->h_out[0, n) the tokens at d_tok (or NULL),
@@ -2775,9 +2755,9 @@ static int forward_locked(lnb_session* s, const int32_t* tokens, int S, int star
     if (host_logits && (rc = gather_logits(s, 0, 1))) return rc;
   } else {
     memcpy(s->h_tok, tokens, (size_t)S * 4);
-    CU(cudaMemcpyAsync(s->d_tokens, s->h_tok, (size_t)S * 4, cudaMemcpyHostToDevice, s->stream));
+    CU(cudaMemcpyAsync(s->d_rag, s->h_tok, (size_t)S * 4, cudaMemcpyHostToDevice, s->stream));
     if ((rc = set_state(s, start_pos, S, -1, false))) return rc;
-    if ((rc = enqueue_forward(s, rows_single(s, S, s->d_tokens, lrows, false, host_logits != nullptr)))) return rc;
+    if ((rc = enqueue_forward(s, rows_single(s, S, s->d_rag, lrows, false, host_logits != nullptr)))) return rc;
   }
   if (score) {
     for (int i = 0; i < S; i++) lp_row(s, i, i, s->d_lp_tgt + i, seq, start_pos + 1 + i, nullptr);
@@ -3291,76 +3271,29 @@ extern "C" int lnb_session_copy_sequences(lnb_session* s, int n, const int32_t* 
   return launch_kernel(Launcher{s->stream, LAUNCH_PDL, &s->launches}, seqcopy_kernel, dim3((unsigned)grid), dim3(SC_THREADS), 0, J);
 }
 
-// One decode step for n independent sequences (rows 0..n-1 = sequences 0..n-1): tokens[i] is fed at
-// positions[i] of sequence i.  The weights are streamed ONCE for all rows (the reference would run n
-// separate Forward calls on n InferenceContexts, SURVEY F10; every row sees exactly the arithmetic of its
-// own S=1 Forward).  logits: NULL or host [n, vocab] f32; argmax_out[n] = greedy token per sequence.
-extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const int32_t* positions, int n, float* logits,
-                                 int32_t* argmax_out) {
-  if (!s || !tokens || !positions) return fail(LNB_EINVAL, "NULL argument");
-  if (n < 1 || n > s->n_seq) return fail(LNB_EINVAL, "n %d exceeds the session's %d sequences", n, s->n_seq);
-  for (int i = 0; i < n; i++) {
-    if (tokens[i] < 0 || tokens[i] >= s->m->a.vocab_size) return fail(LNB_EINVAL, "token id %d out of range", tokens[i]);
-    if (positions[i] < 0 || positions[i] >= s->seq_len) return fail(LNB_EINVAL, "position %d exceeds SequenceLength %d", positions[i], s->seq_len);
-  }
-  std::lock_guard<std::mutex> lk(s->mu);
-  lnb_model* m = s->m;
-  CU(cudaSetDevice(m->device));
-  s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
-  int rc = ensure_logits(s, (size_t)s->max_rows);
-  if (rc) return rc;
-  memcpy(s->h_tok, tokens, (size_t)n * 4);
-  memcpy(s->h_pos, positions, (size_t)n * 4);
-  CU(cudaMemcpyAsync(s->d_tokens, s->h_tok, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
-  CU(cudaMemcpyAsync(s->d_pos_arr, s->h_pos, (size_t)n * 4, cudaMemcpyHostToDevice, s->stream));
-  int32_t seq[8], p_next[8];
-  for (int i = 0; i < n; i++) { seq[i] = i; p_next[i] = positions[i] + 1; }
-  const CtlSum u = ctl_sum(s, n, nullptr);   // a row is processed or has logprobs on: the engine stores the logits
-  if (batch_engine_ok(s)) {
-    // ONE launch of the batch engine: every weight matrix streamed once for all n sequences
-    if ((rc = launch_record(s, rows_batch(s, n)))) return rc;
-    if ((rc = batch_engine_build(s, (logits || u.processed || u.lp) ? s->logits : nullptr))) return rc;
-    if ((rc = batch_engine_launch(s, n, s->d_tokens, s->d_pos_arr, nullptr))) return rc;
-    if (logits && (rc = gather_logits(s, 0, n))) return rc;
-  } else {
-    if (!s->sdpa_smem_decode && !s->ss.sc)
-      return fail(LNB_EINVAL, "batched decode beyond the shared-memory attention kernel needs head_dim <= 128 and n_rep <= 8");
-    if ((rc = set_state(s, 0, n, -1, false))) return rc;
-    if ((rc = enqueue_forward(s, rows_batch(s, n)))) return rc;
-  }
-  if ((rc = call_tail(s, n, 0, seq, p_next, s->d_next_arr, s->d_next_arr, logits, n, argmax_out ? s->d_next_arr : nullptr))) return rc;
-  if (argmax_out) memcpy(argmax_out, s->h_out, (size_t)n * 4);
-  return 0;
-}
-
 // ---- ragged calls (continuous batching): segments of several sequences at their own positions in ONE forward ----------
-// The row map of ragged and speculative calls, allocated by the first one, and for ragged calls (streamed) stream-attention
-// scratch for max_rows rows per launch group when the session has none or a smaller one.  Nothing is replaced unless every
-// allocation succeeded, so a failure (LNB_ENOMEM) leaves the session as it was.
-static int ensure_row_map(lnb_session* s, bool streamed) {
+// Stream-attention scratch for max_rows rows per launch group (every ragged row streams its attention), allocated when the
+// session has none or a smaller one.  Nothing is replaced unless every allocation succeeded, so a failure (LNB_ENOMEM)
+// leaves the session as it was.
+static int ensure_ragged_scratch(lnb_session* s) {
   const lnb_model* m = s->m;
-  AllocBatch A;
-  if (!s->d_rag) A.add(&s->d_rag, row_map_words(s->max_rows) * 4);
   SsScratch x{};
   size_t sc_b, z_b, op_b;
   ss_plan(x, s->seq_len, s->max_rows, m->q_l / m->a.head_dim, m->a.head_dim, &sc_b, &z_b, &op_b);
-  const bool need_ss = streamed && (!s->ss.sc || s->ss.rows < x.rows);
-  if (need_ss) {
-    A.add(&x.sc, sc_b);
-    A.add(&x.z, z_b);
-    A.add(&x.op, op_b);
-  }
-  if (const int rc = A.commit(s->stream, "row map", need_ss ? "stream-attention scratch" : nullptr, sc_b + z_b + op_b)) return rc;
-  if (need_ss) {
-    CU(cudaStreamSynchronize(s->stream));   // batched steps may still read the old scratch
-    cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
-    s->ss = x;
-  }
+  if (s->ss.sc && s->ss.rows >= x.rows) return 0;
+  AllocBatch A;
+  A.add(&x.sc, sc_b);
+  A.add(&x.z, z_b);
+  A.add(&x.op, op_b);
+  if (const int rc = A.commit(s->stream, "stream-attention scratch")) return rc;
+  CU(cudaStreamSynchronize(s->stream));   // batched steps may still read the old scratch
+  cudaFree(s->ss.sc); cudaFree(s->ss.z); cudaFree(s->ss.op);
+  s->ss = x;
   return 0;
 }
 
-// The segments of a ragged or speculative call: segment i feeds rows(i) = cnt[i] + extra tokens of sequence seq[i] at
-// positions start_pos[i] + k (ragged: cnt = len, extra 0; speculative: cnt = n_draft, extra 1).
+// The segments of a ragged, speculative or batched call: segment i feeds rows(i) = cnt[i] + extra tokens of sequence seq[i]
+// at positions start_pos[i] + k (ragged: cnt = len, extra 0; speculative: cnt = n_draft, extra 1; batched: cnt = 0, extra 1).
 struct Segments {
   int n;
   const int32_t *seq, *start_pos, *cnt;
@@ -3421,7 +3354,7 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
   if ((rc = segments_check(s, g, tokens, s->max_rows, &rows))) return rc;
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(m->device));
-  if ((rc = ensure_row_map(s, true))) return rc;
+  if ((rc = ensure_ragged_scratch(s))) return rc;
   if ((rc = ensure_logits(s, (size_t)n_segs))) return rc;
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward
   if ((rc = stage_row_map(s, g, tokens, rows))) return rc;
@@ -3433,7 +3366,8 @@ extern "C" int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq
   return 0;
 }
 
-// ---- speculative verification: a sequence's last emitted token and k drafted tokens as k + 1 rows of ONE forward -------
+// ---- calls whose every row is an output row: speculative verification (a sequence's last emitted token and k drafted
+// tokens as k + 1 rows of ONE forward) and batched steps (one row of each of n sequences) -----------------------------------
 // Sampler scratch for one launch of `rows` rows (a speculative call may draw up to 8 rows of one sequence, more than the
 // session has sequences).  Nothing is replaced unless every allocation succeeded.  A captured decode graph that ends in the
 // sampler holds the old scratch: it is dropped and re-captured by the next lnb_decode_run.
@@ -3448,6 +3382,57 @@ static int samp_grow(lnb_session* s, int rows) {
   CU(cudaStreamSynchronize(s->stream));   // earlier sampler launches may still use the old scratch
   cudaFree(s->d_samp_w); cudaFree(s->d_samp_cand);
   s->d_samp_w = d_w; s->d_samp_cand = d_cand; s->samp_rows = rows;
+  return 0;
+}
+
+// The forward of a call whose every row is an output row, its segments checked (segments_check): speculative calls of >= 2
+// rows and batched steps.  The greedy (or drawn) token of row r lands in s->h_out[r] when want_tokens.
+static int forward_segments(lnb_session* s, const Segments& g, const int32_t* tokens, int rows, float* logits, bool want_tokens) {
+  // the batch engine for >= 2 rows (single-sequence sessions included: engine_capable already holds every position below
+  // the engine's limit, eng_sdpa_smem), and for one row on a session of several sequences
+  const bool eng = batch_engine_usable(s) && (rows >= 2 || s->n_seq >= 2);
+  if (!eng && !s->sdpa_smem_decode && !s->ss.sc)
+    return fail(LNB_EINVAL, "batched and speculative calls beyond the shared-memory attention kernel need head_dim <= 128 and n_rep <= 8");
+  const CtlSum u = ctl_sum(s, g.n, g.seq);   // a row is processed or has logprobs on: the engine stores the logits
+  int rc;
+  if (u.processed && (rc = samp_grow(s, rows))) return rc;
+  if ((rc = ensure_logits(s, (size_t)rows))) return rc;
+  s->kept_rows = 0;   // a logits handle is valid until the session's next forward
+  if ((rc = stage_row_map(s, g, tokens, rows))) return rc;
+  if (eng) {
+    // ONE launch of the batch engine: every weight matrix streamed once for all rows
+    if ((rc = launch_record(s, rows_spec(s, rows, u)))) return rc;
+    if ((rc = batch_engine_build(s, (logits || u.processed || u.lp) ? s->logits : nullptr))) return rc;
+    if ((rc = batch_engine_launch(s, rows, s->d_rag, s->d_rag + 2 * rows, s->d_rag + rows))) return rc;
+    if (logits && (rc = gather_logits(s, 0, rows))) return rc;
+  } else {
+    if ((rc = set_state(s, 0, rows, -1, false))) return rc;
+    if ((rc = enqueue_forward(s, rows_spec(s, rows, u)))) return rc;
+  }
+  const int32_t *row_seq = s->h_tok + rows, *row_pos = s->h_tok + 2 * rows;
+  int32_t p_next[8];
+  for (int r = 0; r < rows; r++) p_next[r] = row_pos[r] + 1;
+  return call_tail(s, rows, 0, row_seq, p_next, s->d_next_arr, s->d_next_arr, logits, rows, want_tokens ? s->d_next_arr : nullptr);
+}
+
+// One decode step for n independent sequences (rows 0..n-1 = sequences 0..n-1): tokens[i] is fed at
+// positions[i] of sequence i.  The weights are streamed ONCE for all rows (the reference would run n
+// separate Forward calls on n InferenceContexts, SURVEY F10; every row sees exactly the arithmetic of its
+// own S=1 Forward).  logits: NULL or host [n, vocab] f32; argmax_out[n] = greedy token per sequence.
+extern "C" int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const int32_t* positions, int n, float* logits,
+                                 int32_t* argmax_out) {
+  if (!s || !tokens || !positions) return fail(LNB_EINVAL, "NULL argument");
+  static const int32_t seq[8] = {0, 1, 2, 3, 4, 5, 6, 7}, no_draft[8] = {};
+  const Segments g{n, seq, positions, no_draft, 1};
+  int rows, rc;
+  if ((rc = segments_check(s, g, tokens, s->max_rows, &rows))) return rc;
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(s->m->device));
+  s->kept_rows = 0;   // a logits handle is valid until the session's next forward (this call may overwrite or move them)
+  // room for max_rows logits rows (as much as any call asks), so later calls keep the buffer the batch engine's phases point at
+  if ((rc = ensure_logits(s, (size_t)s->max_rows))) return rc;
+  if ((rc = forward_segments(s, g, tokens, rows, logits, argmax_out != nullptr))) return rc;
+  if (argmax_out) memcpy(argmax_out, s->h_out, (size_t)n * 4);
   return 0;
 }
 
@@ -3474,28 +3459,7 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
     if (n_accepted) n_accepted[0] = 0;
     return 0;
   }
-  const bool eng = spec_engine_ok(s, rows);
-  if (!eng && !s->sdpa_smem_decode && !s->ss.sc)
-    return fail(LNB_EINVAL, "speculative calls beyond the shared-memory attention kernel need head_dim <= 128 and n_rep <= 8");
-  const CtlSum u = ctl_sum(s, n_segs, seq);
-  if ((rc = ensure_row_map(s, false))) return rc;
-  if (u.processed && (rc = samp_grow(s, rows))) return rc;
-  if ((rc = ensure_logits(s, (size_t)rows))) return rc;
-  s->kept_rows = 0;   // a logits handle is valid until the session's next forward
-  if ((rc = stage_row_map(s, g, tokens, rows))) return rc;
-  const int32_t *row_seq = s->h_tok + rows, *row_pos = s->h_tok + 2 * rows;
-  if (eng) {
-    // ONE launch of the batch engine: every weight matrix streamed once for all rows
-    if ((rc = launch_record(s, rows_spec(s, rows, u)))) return rc;
-    if ((rc = batch_engine_build(s, (logits || u.processed || u.lp) ? s->logits : nullptr))) return rc;
-    if ((rc = batch_engine_launch(s, rows, s->d_rag, s->d_rag + 2 * rows, s->d_rag + rows))) return rc;
-  } else {
-    if ((rc = set_state(s, 0, rows, -1, false))) return rc;
-    if ((rc = enqueue_forward(s, rows_spec(s, rows, u)))) return rc;
-  }
-  int32_t p_next[8];
-  for (int r = 0; r < rows; r++) p_next[r] = row_pos[r] + 1;
-  if ((rc = call_tail(s, rows, 0, row_seq, p_next, s->d_next_arr, s->d_next_arr, logits, rows, s->d_next_arr))) return rc;
+  if ((rc = forward_segments(s, g, tokens, rows, logits, true))) return rc;
   // acceptance: row j of a segment predicts the token at position start + j + 1, which draft j + 1 claims
   for (int i = 0, r0 = 0; i < n_segs; r0 += 1 + n_draft[i], i++) {
     int acc = 0;

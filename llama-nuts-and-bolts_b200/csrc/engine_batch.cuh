@@ -56,10 +56,10 @@ struct BatchPhase {
   int q_dim, kv_dim;
 };
 
-// the sequence whose cache row m reads and appends to: row_seq[m] (speculative verification: consecutive positions of one
-// sequence), or m (a batched step)
+// the sequence whose cache row m reads and appends to: row_seq[m] (a batched step: one row per sequence; speculative
+// verification: consecutive positions of one sequence)
 LNB_DEVINL size_t be_cache_base(const int32_t* row_seq, int m, long long cache_seq_stride) {
-  return (size_t)(row_seq ? row_seq[m] : m) * (size_t)cache_seq_stride;
+  return (size_t)row_seq[m] * (size_t)cache_seq_stride;
 }
 
 struct BatchParams {
@@ -74,7 +74,7 @@ struct BatchParams {
   int strict;
   const int32_t* tokens;    // [n] input token of every sequence
   const int32_t* pos_arr;   // [n] position it is fed at
-  const int32_t* row_seq;   // [n] sequence of every row (its KV cache), or NULL: row m is sequence m
+  const int32_t* row_seq;   // [n] sequence of every row (its KV cache)
   long long cache_seq_stride;
   float* rscale;            // [8] RMSNorm scales of the running norm
   unsigned long long* keys; // [8] greedy-argmax keys (cleared by the host before the launch)

@@ -66,7 +66,7 @@ struct GemvParams {
   uint16_t* cache_v;
   const int32_t* pos_arr;  // batched decode (one row per independent sequence): position of row m; NULL -> *pos_ptr + m
   long long cache_seq_stride;  // elements between the caches of consecutive sequences (batched decode)
-  const int32_t* row_seq;  // ragged calls: sequence of row m (its cache at + row_seq[m] * cache_seq_stride); NULL: row m
+  const int32_t* row_seq;  // rows of several sequences: row m's sequence (cache at + row_seq[m] * cache_seq_stride); NULL: cache_k
   const float* cis;        // [rows][head_dim/2][2]
   // EPI_SWIGLU
   const uint16_t* silu_tab;
@@ -187,7 +187,7 @@ LNB_DEVINL void gemv_epilogue(const GemvParams& p, float v, int n, int em, bool 
     if (valid) {
       const int row = p.m_off + em;
       const int pos = p.pos_arr ? p.pos_arr[row] : *p.pos_ptr + row;
-      const size_t cb = p.pos_arr ? (size_t)(p.row_seq ? p.row_seq[row] : row) * (size_t)p.cache_seq_stride : 0;
+      const size_t cb = p.row_seq ? (size_t)p.row_seq[row] * (size_t)p.cache_seq_stride : 0;
       uint16_t* ck = p.cache_k + cb;
       uint16_t* cv = p.cache_v + cb;
       if (n < p.q_dim + p.kv_dim) {

@@ -102,7 +102,7 @@ __global__ void grammar_set_slot_kernel(GrammarSlot* slot, GrammarSlot v, int32_
 
 // The state history write of one forward (rows as penalty_record_kernel reads them): row r holds token tokens[r] (else
 // `token` if >= 0, else st->next_token) at position pos_arr[r] (else (pos0 >= 0 ? pos0 : st->pos) + r) of sequence
-// row_seq[r] (else `seq` if >= 0, else r).  Rows of one sequence are consecutive positions, in order.
+// row_seq[r] (else `seq`).  Rows of one sequence are consecutive positions, in order.
 __global__ void grammar_record_kernel(int32_t* gst, int gst_len, const GrammarSlot* __restrict__ slots, const LnbDevState* st,
                                       const int32_t* tokens, const int32_t* pos_arr, const int32_t* row_seq, int seq, int token,
                                       int pos0, int S) {
@@ -110,7 +110,7 @@ __global__ void grammar_record_kernel(int32_t* gst, int gst_len, const GrammarSl
   pdl_wait();
   const int r0 = blockIdx.x * blockDim.x + threadIdx.x;
   if (r0 >= S) return;
-  auto seq_of = [&](int r) { return row_seq ? row_seq[r] : (seq >= 0 ? seq : r); };
+  auto seq_of = [&](int r) { return row_seq ? row_seq[r] : seq; };
   const int q = seq_of(r0);
   if (r0 > 0 && seq_of(r0 - 1) == q) return;   // not the first row of its sequence's run
   const GrammarSlot& sl = slots[q];

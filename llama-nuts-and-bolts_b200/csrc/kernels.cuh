@@ -208,10 +208,10 @@ __global__ void __launch_bounds__(1024) sdpa_decode_kernel(const uint16_t* __res
   const int tid = threadIdx.x, nthr = blockDim.x;
   const int hh = tid / 128, tt = tid % 128;
   const int cpr = hd / 8;  // 16-byte chunks per row
-  // batched decode: blockIdx.y = row with its own position and q / output row, on the cache of sequence blockIdx.y, or of
-  // row_seq[blockIdx.y] (speculative verification: several rows of one sequence, the later ones seeing the earlier ones' keys)
+  // batched decode: blockIdx.y = row with its own position and q / output row, on the cache of sequence row_seq[blockIdx.y]
+  // (speculative verification: several rows of one sequence, the later ones seeing the earlier ones' keys)
   if (pos_arr) {
-    const size_t seq = row_seq ? (size_t)row_seq[blockIdx.y] : (size_t)blockIdx.y;
+    const size_t seq = (size_t)row_seq[blockIdx.y];
     pos_ptr = pos_arr + blockIdx.y;
     cache_k += seq * (size_t)cache_seq_stride;
     cache_v += seq * (size_t)cache_seq_stride;

@@ -44,7 +44,7 @@ __global__ void penalty_set_params_kernel(lnb_penalties* slot, lnb_penalties p) 
 }
 
 // The history write of one forward: row r's token (tokens[r], else `token` if >= 0, else st->next_token) at its position
-// (pos_arr[r], else (pos0 >= 0 ? pos0 : st->pos) + r) of its sequence (row_seq[r], else `seq` if >= 0, else r).
+// (pos_arr[r], else (pos0 >= 0 ? pos0 : st->pos) + r) of its sequence (row_seq[r], else `seq`).
 __global__ void penalty_record_kernel(int32_t* __restrict__ hist, int hist_len, const LnbDevState* st, const int32_t* tokens,
                                       const int32_t* pos_arr, const int32_t* row_seq, int seq, int token, int pos0, int S) {
   pdl_launch_dependents();
@@ -53,7 +53,7 @@ __global__ void penalty_record_kernel(int32_t* __restrict__ hist, int hist_len, 
   if (r >= S) return;
   const int32_t t = tokens ? tokens[r] : (token >= 0 ? token : st->next_token);
   const int32_t p = pos_arr ? pos_arr[r] : (pos0 >= 0 ? pos0 : st->pos) + r;
-  const int32_t q = row_seq ? row_seq[r] : (seq >= 0 ? seq : r);
+  const int32_t q = row_seq ? row_seq[r] : seq;
   if (p >= 0 && p < hist_len) hist[(size_t)q * hist_len + p] = t;
 }
 

@@ -3,8 +3,8 @@
 // fit, and lnb_op_attention_bf16 beyond sdpa_kernel's T limit.
 //
 // One description covers every caller: query row r (global index r of the call) has its own cache base
-// (cache + r * row_cache_stride: batched decode; cache + row_seq[r] * row_cache_stride: ragged calls, where rows of one
-// sequence follow each other) and its own position p_r (pos_arr[r], or base + pos_step * r: S = 1
+// (cache + row_seq[r] * row_cache_stride: batched, ragged and speculative calls, where rows of one sequence follow each
+// other; cache without a row map) and its own position p_r (pos_arr[r], or base + pos_step * r: S = 1
 // decode, a prompt or chunked prefill under the [S,T] mask, or pos_step = 0 for the op's unmasked form) and sees keys
 // 0..p_r.  The arithmetic is sdpa_kernel's (llamatransformer.go:459-514):
 //   sc_t = t( t(sum_seq_d q_d k_td) / t(sqrt(hd)) );  e_t = exp_f64(sc_t);  p_t = t(f32(e_t / Z));  o_d = t(sum_t p_t v_td)
@@ -38,8 +38,8 @@ struct StreamAttn {
   const uint16_t* cache_k;
   const uint16_t* cache_v;
   int kv_dim;
-  long long row_cache_stride;   // elements between the caches of consecutive rows (batched decode), else 0
-  const int32_t* row_seq;       // ragged calls: row r reads the cache of sequence row_seq[r] (+ row_seq[r] * row_cache_stride)
+  long long row_cache_stride;   // elements between the caches of consecutive sequences
+  const int32_t* row_seq;       // rows of several sequences: row r reads the cache of sequence row_seq[r]; NULL: cache_k
   int n_rep, hd, n_heads;       // n_heads: query heads of this rank
   const int32_t* pos_arr;       // per-row positions, or NULL:
   const int32_t* pos_ptr;       //   p_r = (pos_ptr ? *pos_ptr : pos_fixed) + pos_step * r
@@ -61,7 +61,7 @@ LNB_DEVINL int ss_keys(const StreamAttn& P, int r) {   // keys row r sees (call 
   return p + 1;
 }
 LNB_DEVINL size_t ss_cache_base(const StreamAttn& P, int r) {   // (call only after pdl_wait)
-  return (size_t)(P.row_seq ? __ldcg(P.row_seq + r) : r) * (size_t)P.row_cache_stride;
+  return P.row_seq ? (size_t)__ldcg(P.row_seq + r) * (size_t)P.row_cache_stride : 0;
 }
 LNB_DEVINL uint16_t* ss_score_row(const StreamAttn& P, int rl, int H) {
   return P.sc + ((size_t)rl * P.n_heads + H) * (size_t)P.t_stride;
