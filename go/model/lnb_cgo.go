@@ -36,7 +36,7 @@ type deviceModel struct{ h *C.lnb_model }
 type deviceSession struct{ h *C.lnb_session }
 
 // called at the end of NewLlamaTransformer, after every getTensor succeeded.  weightFormat: C.LNB_WEIGHTS_BF16, or
-// C.LNB_WEIGHTS_MXFP8 to quantize the linear weights at finalize (tpSize 1 only)
+// C.LNB_WEIGHTS_MXFP8 / C.LNB_WEIGHTS_MXFP4 to quantize the linear weights at finalize (tpSize 1 only)
 func newDeviceModel(args *ModelArgs, tensors map[string]*ml.Tensor, device, tpRank, tpSize int, ncclID []byte,
 	weightFormat int) (*deviceModel, error) {
 	ca := C.lnb_model_args{
@@ -85,6 +85,17 @@ func (dm *deviceModel) mxfp8Read(name string, rows, cols int) ([]byte, []byte, e
 	cname := C.CString(name)
 	defer C.free(unsafe.Pointer(cname))
 	rc := C.lnb_model_mxfp8_read(dm.h, cname, (*C.uint8_t)(unsafe.Pointer(&codes[0])), (*C.uint8_t)(unsafe.Pointer(&scales[0])))
+	return codes, scales, lnbErr(rc)
+}
+
+// the E2M1 codes [rows*cols/2] (the even column in a byte's low nibble) and E8M0 scales [rows*ceil(cols/32)] of a linear
+// tensor of an MXFP4 model (tests, tools)
+func (dm *deviceModel) mxfp4Read(name string, rows, cols int) ([]byte, []byte, error) {
+	codes := make([]byte, rows*(cols/2))
+	scales := make([]byte, rows*((cols+31)/32))
+	cname := C.CString(name)
+	defer C.free(unsafe.Pointer(cname))
+	rc := C.lnb_model_mxfp4_read(dm.h, cname, (*C.uint8_t)(unsafe.Pointer(&codes[0])), (*C.uint8_t)(unsafe.Pointer(&scales[0])))
 	return codes, scales, lnbErr(rc)
 }
 

@@ -23,7 +23,7 @@
 // prompt=TEXT (with <modelDir>/tokenizer.model): TEXT goes through the chat template and the BPE tokenizer, the
 // generated ids come back as text (cmd/main.go's flow without the console UI).
 // weights=mxfp8: the linear weights are quantized to MXFP8 at load (DESIGN §9h): half the weight bytes per step, and the
-// same ids as the bf16 model whose weights are the dequantized values.
+// same ids as the bf16 model whose weights are the dequantized values.  weights=mxfp4: the same with 4-bit codes (DESIGN §9i).
 // <modelDir> holds params.json + consolidated.00.pth (model.LoadModel, src/model/loader.go:18-70);
 // `lnb_generate --write-synthetic <modelDir> [tiny]` writes such a directory for the synthetic weights (host-only).
 // `lnb_generate --tokenize <tokenizer.model> <text>` prints the chat-template token ids of <text> (host-only).
@@ -141,6 +141,7 @@ int main(int argc, char** argv) {
     int weight_format = LNB_WEIGHTS_BF16;
     for (int i = 3; i < argc; i++) {
       if (!strcmp(argv[i], "weights=mxfp8")) weight_format = LNB_WEIGHTS_MXFP8;
+      else if (!strcmp(argv[i], "weights=mxfp4")) weight_format = LNB_WEIGHTS_MXFP4;
       else if (!strncmp(argv[i], "weights=", 8) && strcmp(argv[i], "weights=bf16")) throw lnb_host::Error(std::string("unknown ") + argv[i]);
     }
     std::unique_ptr<model::LlamaTransformer> loaded;

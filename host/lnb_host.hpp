@@ -212,7 +212,8 @@ class LlamaTransformer {  // llamatransformer.go:16-113
     check(lnb_model_load_pth(h_, path.c_str(), &n));
     return n;
   }
-  // LNB_WEIGHTS_BF16 or LNB_WEIGHTS_MXFP8 (DESIGN §9h: Finalize quantizes the linear weights); before Finalize
+  // LNB_WEIGHTS_BF16, LNB_WEIGHTS_MXFP8 or LNB_WEIGHTS_MXFP4 (DESIGN §9h, §9i: Finalize quantizes the linear weights);
+  // before Finalize
   void SetWeightFormat(int fmt) { check(lnb_model_set_weight_format(h_, fmt)); }
   void Finalize() { check(lnb_model_finalize(h_)); }
   // MXFP8 model: the codes [rows][cols] and scales [rows][ceil(cols / 32)] of a linear checkpoint tensor
@@ -220,6 +221,12 @@ class LlamaTransformer {  // llamatransformer.go:16-113
     codes.resize((size_t)(rows * cols));
     scales.resize((size_t)(rows * ((cols + 31) / 32)));
     check(lnb_model_mxfp8_read(h_, name.c_str(), codes.data(), scales.data()));
+  }
+  // MXFP4 model: the codes [rows][cols / 2] (the even column in a byte's low nibble) and scales [rows][ceil(cols / 32)]
+  void MxFp4Read(const std::string& name, std::vector<uint8_t>& codes, std::vector<uint8_t>& scales, int64_t rows, int64_t cols) {
+    codes.resize((size_t)(rows * (cols / 2)));
+    scales.resize((size_t)(rows * ((cols + 31) / 32)));
+    check(lnb_model_mxfp4_read(h_, name.c_str(), codes.data(), scales.data()));
   }
   struct WeightInfo {
     int Format = LNB_WEIGHTS_BF16;

@@ -203,12 +203,22 @@ int lnb_model_wpack_read(lnb_model* m, int layer, uint8_t* data, uint8_t* units,
  * set_weight_format: before finalize (LNB_ESTATE after); LNB_EINVAL for an unknown format or tp_size > 1.
  * The decode and batch engines and the STRICT packed stream read bf16 panels: MXFP8 sessions run the kernel chain, and
  * lnb_session_decode_engine / lnb_model_wpack_read return 0 saying so.  FAST sessions with max_rows >= 32 hold a bf16
- * scratch the size of the largest layer matrix for the tensor-core prompt path. */
-enum { LNB_WEIGHTS_BF16 = 0, LNB_WEIGHTS_MXFP8 = 1 };
+ * scratch the size of the largest layer matrix for the tensor-core prompt path.
+ * MXFP4 linear weights (DESIGN §9i), LNB_WEIGHTS_MXFP4: the same matrices, blocks, scale layout, routing and refusals, with
+ * one E2M1 code per weight ({0, 0.5, 1, 1.5, 2, 3, 4, 6} and a sign).  Let e, f be the unbiased exponent and 7-bit mantissa
+ * field of the bf16 max |w| of a block: X = e - 2 if f <= 64 else e - 1 (the smallest X with max |w| <= 6 * 2^X), clamped
+ * to [-125, 125]; a zero or subnormal maximum gets -125.  Each code is sign(w) and |w| * 2^-X rounded to the nearest grid
+ * value, ties to the even mantissa bit, saturated to 6.  Every d = e2m1(code) * 2^X is a bf16 value, and every call on an
+ * MXFP4 model returns the bits the same call returns on the bf16 model with weights d. */
+enum { LNB_WEIGHTS_BF16 = 0, LNB_WEIGHTS_MXFP8 = 1, LNB_WEIGHTS_MXFP4 = 2 };
 int lnb_model_set_weight_format(lnb_model* m, int fmt);
 /* the codes [rows][cols] and scales [rows][ceil(cols / 32)] of a linear checkpoint tensor, in the checkpoint's row order
  * (either may be NULL); the model must be a finalized MXFP8 model */
 int lnb_model_mxfp8_read(lnb_model* m, const char* name, uint8_t* codes, uint8_t* scales);
+/* the codes [rows][cols / 2] (two a byte, the even column in the low nibble, as torch.float4_e2m1fn_x2 packs) and scales
+ * [rows][ceil(cols / 32)] of a linear checkpoint tensor, in the checkpoint's row order (either may be NULL); the model must
+ * be a finalized MXFP4 model */
+int lnb_model_mxfp4_read(lnb_model* m, const char* name, uint8_t* codes, uint8_t* scales);
 /* fmt = the format of the linear weights (bf16 until finalized); device_bytes = the weight bytes held in HBM (embedding,
  * norms, linear weights with their scales); step_bytes = the weight bytes one single-GPU S = 1 step reads (every linear
  * weight and norm once, one embedding row).  Any pointer may be NULL. */

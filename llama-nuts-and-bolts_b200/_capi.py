@@ -10,7 +10,7 @@ LIB_PATH = os.path.join(_HERE, "liblnb.so")
 LNB_ACC_STRICT, LNB_ACC_FAST = 0, 1
 LNB_BUF_RESIDUAL, LNB_BUF_CACHE_K, LNB_BUF_CACHE_V, LNB_BUF_LOGITS = 0, 1, 2, 3
 LNB_BUF_Q, LNB_BUF_ATTN, LNB_BUF_POST_ATTN, LNB_BUF_NORMED, LNB_BUF_FFN = 4, 5, 6, 7, 8
-LNB_WEIGHTS_BF16, LNB_WEIGHTS_MXFP8 = 0, 1
+LNB_WEIGHTS_BF16, LNB_WEIGHTS_MXFP8, LNB_WEIGHTS_MXFP4 = 0, 1, 2
 
 
 class LnbError(RuntimeError):
@@ -76,6 +76,7 @@ SIGNATURES = {
     "lnb_model_wpack_read": (C.c_int, [vp, C.c_int, vp, vp, u16p, i64p]),
     "lnb_model_set_weight_format": (C.c_int, [vp, C.c_int]),
     "lnb_model_mxfp8_read": (C.c_int, [vp, C.c_char_p, vp, vp]),
+    "lnb_model_mxfp4_read": (C.c_int, [vp, C.c_char_p, vp, vp]),
     "lnb_model_weight_info": (C.c_int, [vp, C.POINTER(C.c_int), i64p, i64p]),
     "lnb_session_create": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
     "lnb_session_destroy": (C.c_int, [vp]),

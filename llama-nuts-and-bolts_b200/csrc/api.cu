@@ -790,12 +790,13 @@ extern "C" int lnb_model_get_silu_table(lnb_model* m, uint16_t* out) {
   return 0;
 }
 
-// ---- MXFP8 linear weights (mxfp8.cuh, DESIGN.md §9h) ---------------------------------------------------------------
+// ---- MXFP8 and MXFP4 linear weights (mxfp8.cuh, mxfp4.cuh, DESIGN.md §9h, §9i) -----------------------------------------
+static const char* wfmt_name(int fmt) { return fmt == LNB_WEIGHTS_MXFP4 ? "MXFP4" : "MXFP8"; }
 extern "C" int lnb_model_set_weight_format(lnb_model* m, int fmt) {
   if (!m) return fail(LNB_EINVAL, "model is NULL");
   if (m->finalized) return fail(LNB_ESTATE, "model is finalized: the weight format is chosen before lnb_model_finalize");
-  if (fmt != LNB_WEIGHTS_BF16 && fmt != LNB_WEIGHTS_MXFP8) return fail(LNB_EINVAL, "unknown weight format %d", fmt);
-  if (fmt == LNB_WEIGHTS_MXFP8 && m->tp_size > 1) return fail(LNB_EINVAL, "MXFP8 weights need tp_size 1 (have %d)", m->tp_size);
+  if (fmt != LNB_WEIGHTS_BF16 && fmt != LNB_WEIGHTS_MXFP8 && fmt != LNB_WEIGHTS_MXFP4) return fail(LNB_EINVAL, "unknown weight format %d", fmt);
+  if (fmt != LNB_WEIGHTS_BF16 && m->tp_size > 1) return fail(LNB_EINVAL, "%s weights need tp_size 1 (have %d)", wfmt_name(fmt), m->tp_size);
   m->wfmt = fmt;
   return 0;
 }
@@ -821,9 +822,11 @@ static std::vector<LinMat> linear_mats(lnb_model* m) {
   return v;
 }
 static size_t mx_scale_bytes(int N, int K) { return (size_t)(N / 8) * mx_nbp(K) * 8; }
-static size_t mat_bytes(int fmt, int N, int K) {
-  return fmt == LNB_WEIGHTS_MXFP8 ? (size_t)N * K + mx_scale_bytes(N, K) : (size_t)N * K * 2;
+// the bytes of the codes (bf16: of the panels) of N rows
+static size_t code_bytes(int fmt, int N, int K) {
+  return fmt == LNB_WEIGHTS_MXFP4 ? (size_t)N * K / 2 : fmt == LNB_WEIGHTS_MXFP8 ? (size_t)N * K : (size_t)N * K * 2;
 }
+static size_t mat_bytes(int fmt, int N, int K) { return code_bytes(fmt, N, K) + (fmt == LNB_WEIGHTS_BF16 ? 0 : mx_scale_bytes(N, K)); }
 // the checkpoint tensor and row of device row d of a matrix (inverse of placement + panel_dest_row)
 static void checkpoint_row(const lnb_model* m, const LinMat& x, int64_t d, const char** name, int64_t* row) {
   static const char* kn[] = {"attention.wq.weight", "attention.wk.weight", "attention.wv.weight", "attention.wo.weight",
@@ -841,9 +844,9 @@ static void checkpoint_row(const lnb_model* m, const LinMat& x, int64_t d, const
     default: *name = kn[7]; break;
   }
 }
-// Quantize every linear matrix on the device, then free the bf16 copies.  Both copies are held until every matrix has
-// passed, so a refused weight leaves the bf16 model as it was.
-static int quantize_model(lnb_model* m) {
+// Quantize every linear matrix on the device to format fmt (MXFP8 or MXFP4), then free the bf16 copies.  Both copies are
+// held until every matrix has passed, so a refused weight leaves the bf16 model as it was.
+static int quantize_model(lnb_model* m, int fmt) {
   std::vector<LinMat> mats = linear_mats(m);
   std::vector<uint8_t*> codes(mats.size(), nullptr), scales(mats.size(), nullptr);
   unsigned long long* flags = nullptr;
@@ -852,15 +855,16 @@ static int quantize_model(lnb_model* m) {
     cudaFree(flags);
   };
   size_t total = 0;
-  for (const LinMat& x : mats) total += mat_bytes(LNB_WEIGHTS_MXFP8, x.N, x.K);
+  for (const LinMat& x : mats) total += mat_bytes(fmt, x.N, x.K);
   cudaError_t e = cudaMalloc((void**)&flags, mats.size() * 8);
   if (e == cudaSuccess) e = cudaMemset(flags, 0xff, mats.size() * 8);
   for (size_t i = 0; i < mats.size() && e == cudaSuccess; i++) {
-    e = cudaMalloc((void**)&codes[i], (size_t)mats[i].N * mats[i].K);
+    e = cudaMalloc((void**)&codes[i], code_bytes(fmt, mats[i].N, mats[i].K));
     if (e == cudaSuccess) e = cudaMalloc((void**)&scales[i], mx_scale_bytes(mats[i].N, mats[i].K));
     if (e == cudaSuccess) e = cudaMemset(scales[i], 0, mx_scale_bytes(mats[i].N, mats[i].K));
     if (e == cudaSuccess) {
-      mxfp8_quantize_kernel<<<m->sm_count * 8, 256>>>(*mats[i].w, mats[i].N, mats[i].K, codes[i], scales[i], flags + i);
+      (fmt == LNB_WEIGHTS_MXFP4 ? mxfp4_quantize_kernel : mxfp8_quantize_kernel)<<<m->sm_count * 8, 256>>>(
+          *mats[i].w, mats[i].N, mats[i].K, codes[i], scales[i], flags + i);
       e = cudaGetLastError();
     }
   }
@@ -869,8 +873,8 @@ static int quantize_model(lnb_model* m) {
   if (e != cudaSuccess) {
     cudaGetLastError();
     drop();
-    return fail(e == cudaErrorMemoryAllocation ? LNB_ENOMEM : LNB_ECUDA, "MXFP8 quantization (%.2f GB beside the bf16 weights): %s",
-                total / 1e9, cudaGetErrorString(e));
+    return fail(e == cudaErrorMemoryAllocation ? LNB_ENOMEM : LNB_ECUDA, "%s quantization (%.2f GB beside the bf16 weights): %s",
+                wfmt_name(fmt), total / 1e9, cudaGetErrorString(e));
   }
   for (size_t i = 0; i < mats.size(); i++) {
     if (h[i] == ~0ull) continue;
@@ -879,9 +883,10 @@ static int quantize_model(lnb_model* m) {
     checkpoint_row(m, mats[i], (int64_t)(h[i] / (unsigned long long)mats[i].K), &name, &row);
     const long long col = (long long)(h[i] % (unsigned long long)mats[i].K);
     drop();
-    if (mats[i].layer < 0) return fail(LNB_EINVAL, "MXFP8: tensor \"%s\" has a non-finite weight at row %lld, column %lld", name, (long long)row, col);
-    return fail(LNB_EINVAL, "MXFP8: tensor \"layers.%d.%s\" has a non-finite weight at row %lld, column %lld", mats[i].layer, name,
-                (long long)row, col);
+    if (mats[i].layer < 0)
+      return fail(LNB_EINVAL, "%s: tensor \"%s\" has a non-finite weight at row %lld, column %lld", wfmt_name(fmt), name, (long long)row, col);
+    return fail(LNB_EINVAL, "%s: tensor \"layers.%d.%s\" has a non-finite weight at row %lld, column %lld", wfmt_name(fmt), mats[i].layer,
+                name, (long long)row, col);
   }
   for (size_t i = 0; i < mats.size(); i++) {
     cudaFree(*mats[i].w);
@@ -891,10 +896,13 @@ static int quantize_model(lnb_model* m) {
   cudaFree(flags);
   return 0;
 }
-extern "C" int lnb_model_mxfp8_read(lnb_model* m, const char* name, uint8_t* codes, uint8_t* scales) {
+// the codes and scales of a linear checkpoint tensor of a finalized model of format fmt, in the checkpoint's row order:
+// codes [rows][cols] (MXFP8) or [rows][cols / 2] (MXFP4, two codes a byte, the even column in the low nibble)
+static int mx_read(lnb_model* m, int fmt, const char* name, uint8_t* codes, uint8_t* scales) {
   if (!m || !name) return fail(LNB_EINVAL, "NULL argument");
   if (!m->finalized) return fail(LNB_ESTATE, "model is not finalized");
-  if (m->wfmt != LNB_WEIGHTS_MXFP8) return fail(LNB_ESTATE, "the model's weights are bf16");
+  if (m->wfmt != fmt) return fail(LNB_ESTATE, m->wfmt == LNB_WEIGHTS_BF16 ? "the model's weights are bf16" : "the model's weights are %s",
+                                  wfmt_name(m->wfmt));
   int kind, layer;
   if (parse_name(m, name, &kind, &layer)) return fail(LNB_EINVAL, "unknown tensor name \"%s\"", name);
   if (kind == T_EMBD || kind == T_NORM || kind == T_ATTN_NORM || kind == T_FFN_NORM)
@@ -906,18 +914,25 @@ extern "C" int lnb_model_mxfp8_read(lnb_model* m, const char* name, uint8_t* cod
   for (const LinMat& c : mats)
     if (c.layer == layer && *c.w == p.dst) x = &c;
   const int K = x->K, nbp = mx_nbp(K), nb = (K + 31) / 32;
-  std::vector<uint8_t> hc((size_t)x->N * K), hs(mx_scale_bytes(x->N, K));
+  const int rb = (int)code_bytes(fmt, 1, K), cpc = rb / (K / 8);   // code bytes of one row, of one chunk row (8 or 4)
+  std::vector<uint8_t> hc(code_bytes(fmt, x->N, K)), hs(mx_scale_bytes(x->N, K));
   CU(cudaMemcpy(hc.data(), *x->w, hc.size(), cudaMemcpyDeviceToHost));
   CU(cudaMemcpy(hs.data(), *x->s, hs.size(), cudaMemcpyDeviceToHost));
   for (int64_t r = 0; r < p.rows; r++) {
     const int64_t d = p.dpanel_stride == 2 ? (r >> 2) * 8 + (p.dpanel0 ? 4 : 0) + (r & 3) : (int64_t)p.dpanel0 * 8 + r;
     const int64_t dp = d / 8, rr = d % 8;
     if (codes)
-      for (int k = 0; k < K; k++) codes[r * K + k] = hc[((dp * (K / 8) + k / 8) * 8 + rr) * 8 + k % 8];
+      for (int k = 0; k < rb; k++) codes[r * rb + k] = hc[((dp * (K / 8) + k / cpc) * 8 + rr) * cpc + k % cpc];
     if (scales)
       for (int b = 0; b < nb; b++) scales[r * nb + b] = hs[(dp * nbp + b) * 8 + rr];
   }
   return 0;
+}
+extern "C" int lnb_model_mxfp8_read(lnb_model* m, const char* name, uint8_t* codes, uint8_t* scales) {
+  return mx_read(m, LNB_WEIGHTS_MXFP8, name, codes, scales);
+}
+extern "C" int lnb_model_mxfp4_read(lnb_model* m, const char* name, uint8_t* codes, uint8_t* scales) {
+  return mx_read(m, LNB_WEIGHTS_MXFP4, name, codes, scales);
 }
 extern "C" int lnb_model_weight_info(lnb_model* m, int* fmt, int64_t* device_bytes, int64_t* step_bytes) {
   if (!m) return fail(LNB_EINVAL, "model is NULL");
@@ -955,8 +970,8 @@ extern "C" int lnb_model_finalize(lnb_model* m) {
   }
   if (m->staging) { cudaFree(m->staging); m->staging = nullptr; m->staging_bytes = 0; }
   CU(cudaDeviceSynchronize());
-  if (m->wfmt == LNB_WEIGHTS_MXFP8)
-    if (int rc = quantize_model(m)) return rc;
+  if (m->wfmt != LNB_WEIGHTS_BF16)
+    if (int rc = quantize_model(m, m->wfmt)) return rc;
   m->finalized = true;
   return 0;
 }
@@ -968,16 +983,16 @@ extern "C" int lnb_model_finalize(lnb_model* m) {
 // itself: ONE CTA per SM (>113 KB of shared memory each) holding 1, 2 or 4 chain warps (warps 1..4
 // sit on SMSPs 1,2,3,0; the producer warp 0 sleeps on its mbarrier), picked from N so that the grid
 // stays close to one wave.  Two chain warps on one scheduler run at half speed each.
-// F = the weight format: MXFP8 configs take twice the k-tile, so a stage carries as many bytes as its bf16 twin.
-template <int F> using CfgS1_ = GemvCfg<32, 1, 1, 512 << F, 3, F>;    // N <= 32*kWaveSMs rows
-template <int F> using CfgS1M_ = GemvCfg<64, 1, 1, 512 << F, 3, F>;   // N <= 64*kWaveSMs
-template <int F> using CfgS1W_ = GemvCfg<128, 1, 1, 256 << F, 3, F>;  // larger N (w1|w3, LM head): several waves, HBM-bound
-template <int F> using CfgS2_ = GemvCfg<32, 1, 2, 256 << F, 4, F>;
-template <int F> using CfgS8_ = GemvCfg<32, 1, 8, 256 << F, 4, F>;
-template <int F> using CfgF1_ = GemvCfg<32, 8, 1, 256 << F, 4, F>;
-template <int F> using CfgF1L_ = GemvCfg<32, 8, 1, 512 << F, 3, F>;  // at most one CTA per SM (wo, w2): larger bulk copies
-template <int F> using CfgF2_ = GemvCfg<32, 8, 2, 256 << F, 4, F>;
-template <int F> using CfgF8_ = GemvCfg<32, 8, 8, 256 << F, 4, F>;
+// F = the weight format: the MX configs take the k-tile gemv_kt, so a stage carries about as many bytes as its bf16 twin.
+template <int F> using CfgS1_ = GemvCfg<32, 1, 1, gemv_kt(512, F), 3, F>;    // N <= 32*kWaveSMs rows
+template <int F> using CfgS1M_ = GemvCfg<64, 1, 1, gemv_kt(512, F), 3, F>;   // N <= 64*kWaveSMs
+template <int F> using CfgS1W_ = GemvCfg<128, 1, 1, gemv_kt(256, F), 3, F>;  // larger N (w1|w3, LM head): several waves, HBM-bound
+template <int F> using CfgS2_ = GemvCfg<32, 1, 2, gemv_kt(256, F), 4, F>;
+template <int F> using CfgS8_ = GemvCfg<32, 1, 8, gemv_kt(256, F), 4, F>;
+template <int F> using CfgF1_ = GemvCfg<32, 8, 1, gemv_kt(256, F), 4, F>;
+template <int F> using CfgF1L_ = GemvCfg<32, 8, 1, gemv_kt(512, F), 3, F>;  // at most one CTA per SM (wo, w2): larger bulk copies
+template <int F> using CfgF2_ = GemvCfg<32, 8, 2, gemv_kt(256, F), 4, F>;
+template <int F> using CfgF8_ = GemvCfg<32, 8, 8, gemv_kt(256, F), 4, F>;
 using CfgF1 = CfgF1_<WF_BF16>;
 
 static const size_t kMaxSmem = 227 * 1024;
@@ -1086,18 +1101,21 @@ static int launch_gemv_cfg(const Launcher& L, const GemvParams& p, const uint8_t
 // picks the row-block size: largest MB in {8,2,1} that is useful for M and whose smem fits.  mb_rows > 0 chooses it for
 // that many rows instead of M_total (ragged calls pass 8: the block size, and with it a row's FAST summation order, then
 // depends on K alone, not on how many rows share the call)
-// (the weight format F comes from Ws: launch_gemv below)
+// (the weight format F: launch_gemv below)
 template <int PRO, int EPI, int F>
 static int launch_gemv_fmt(const Launcher& L, int mode, GemvParams p, int M_total, int mb_rows, const uint8_t* Ws) {
   using CfgS1 = CfgS1_<F>; using CfgS1M = CfgS1M_<F>; using CfgS1W = CfgS1W_<F>; using CfgS2 = CfgS2_<F>; using CfgS8 = CfgS8_<F>;
   using CfgF1 = CfgF1_<F>; using CfgF1L = CfgF1L_<F>; using CfgF2 = CfgF2_<F>; using CfgF8 = CfgF8_<F>;
+  // MXFP4 takes the row block of its bf16 twin (its stages are no larger, so it fits wherever the twin fits): the FAST
+  // order of a row then is that of the bf16 matrix of its dequantized weights for every M and K
+  constexpr int FB = F == WF_MXFP4 ? WF_BF16 : F;
   const bool strict = (mode == LNB_ACC_STRICT);
   p.strict_norm = strict ? 1 : 0;
   const int mb_for = mb_rows > 0 ? mb_rows : M_total;
   int mb = 1;
-  if (mb_for >= 3 && (strict ? CfgS8::smem_bytes(p.K) : CfgF8::smem_bytes(p.K)) <= kMaxSmem) mb = 8;
-  else if (mb_for >= 2 && (strict ? CfgS2::smem_bytes(p.K) : CfgF2::smem_bytes(p.K)) <= kMaxSmem) mb = 2;
-  if ((strict ? CfgS1::smem_bytes(p.K) : CfgF1::smem_bytes(p.K)) > kMaxSmem)
+  if (mb_for >= 3 && (strict ? CfgS8_<FB>::smem_bytes(p.K) : CfgF8_<FB>::smem_bytes(p.K)) <= kMaxSmem) mb = 8;
+  else if (mb_for >= 2 && (strict ? CfgS2_<FB>::smem_bytes(p.K) : CfgF2_<FB>::smem_bytes(p.K)) <= kMaxSmem) mb = 2;
+  if ((strict ? CfgS1_<FB>::smem_bytes(p.K) : CfgF1_<FB>::smem_bytes(p.K)) > kMaxSmem)
     return fail(LNB_EINVAL, "gemv: K %d too large for shared memory", p.K);
   const uint16_t* x0 = p.x;
   uint16_t* ob0 = p.out_bf16;
@@ -1137,12 +1155,14 @@ static int launch_gemv_fmt(const Launcher& L, int mode, GemvParams p, int M_tota
   }
   return 0;
 }
-// Ws: the scales of an MXFP8 matrix (p.W then points at its codes); NULL: p.W is bf16
+// wfmt: the model's weight format (LNB_WEIGHTS_*); for MXFP8 and MXFP4, p.W points at the matrix's codes and Ws at its scales
 template <int PRO, int EPI>
-static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total, int mb_rows = 0, const uint8_t* Ws = nullptr) {
+static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total, int mb_rows = 0, const uint8_t* Ws = nullptr,
+                       int wfmt = LNB_WEIGHTS_BF16) {
   if (p.N % 16 || p.K % 8) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 16 and K %d of 8", p.N, p.K);  // 16: panel pairs
   if ((EPI == EPI_QKV_ROPE || EPI == EPI_SWIGLU) && p.N % 32) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 32", p.N);
-  if (Ws) return launch_gemv_fmt<PRO, EPI, WF_MXFP8>(L, mode, p, M_total, mb_rows, Ws);
+  if (wfmt == LNB_WEIGHTS_MXFP8) return launch_gemv_fmt<PRO, EPI, WF_MXFP8>(L, mode, p, M_total, mb_rows, Ws);
+  if (wfmt == LNB_WEIGHTS_MXFP4) return launch_gemv_fmt<PRO, EPI, WF_MXFP4>(L, mode, p, M_total, mb_rows, Ws);
   return launch_gemv_fmt<PRO, EPI, WF_BF16>(L, mode, p, M_total, mb_rows, nullptr);
 }
 
@@ -1312,7 +1332,7 @@ struct lnb_session {
   // tensor-core prefill path (LNB_ACC_FAST, S >= 32): X8-layout activations + raw GEMM outputs
   uint16_t *xn8 = nullptr, *o8 = nullptr, *m8 = nullptr, *qkv_raw = nullptr, *gu = nullptr;
   int mpad = 0;
-  // MXFP8 models: the bf16 panels of the matrix the next GEMM reads (mxfp8_dequant_kernel), as large as the largest one
+  // MXFP8 and MXFP4 models: the bf16 panels of the matrix the next GEMM reads (mx*_dequant_kernel), as large as the largest one
   uint16_t* wdq = nullptr;
   size_t wdq_elems = 0;
   // peer-memory all-reduce (tp_size > 1, optional): own region + the peers' mapped regions
@@ -1521,7 +1541,7 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
     A.add(&s->m8, (size_t)s->mpad * m->ffn_l * 2);
     A.add(&s->qkv_raw, (size_t)max_rows * (m->q_l + 2 * m->kv_l) * 2);
     A.add(&s->gu, (size_t)max_rows * 2 * m->ffn_l * 2);
-    if (m->wfmt == LNB_WEIGHTS_MXFP8) {
+    if (m->wfmt != LNB_WEIGHTS_BF16) {
       for (const LinMat& x : linear_mats(m)) s->wdq_elems = std::max(s->wdq_elems, x.layer < 0 ? (size_t)TC_BN * x.K : (size_t)x.N * x.K);
       A.add(&s->wdq, s->wdq_elems * 2);
     }
@@ -1757,6 +1777,7 @@ static bool engine_probe(lnb_session* s) {
   const char* e = getenv("LNB_ENGINE");
   if (e && !strcmp(e, "0")) return no("LNB_ENGINE=0");
   if (m->wfmt == LNB_WEIGHTS_MXFP8) return no("MXFP8 weights: the decode and batch engines stream bf16 panels");
+  if (m->wfmt == LNB_WEIGHTS_MXFP4) return no("MXFP4 weights: the decode and batch engines stream bf16 panels");
   // single-sequence steps of single-GPU FAST sessions stay on the kernel chain by default (the batch engine does not care)
   s->eng_single_default = (e && !strcmp(e, "1")) || !(s->mode == LNB_ACC_FAST && m->tp_size == 1);
   const int kmax = std::max(a.dim, std::max(m->q_l, m->ffn_l));
@@ -1844,6 +1865,7 @@ static bool ensure_wpack(lnb_model* m) {
   const int G = m->sm_count, L = a.n_layers;
   auto no = [&](const std::string& why) { m->wpack_state = -1; m->wpack_why = why; return false; };
   if (m->wfmt == LNB_WEIGHTS_MXFP8) return no("MXFP8 weights: the packed copies are built from bf16 panels");
+  if (m->wfmt == LNB_WEIGHTS_MXFP4) return no("MXFP4 weights: the packed copies are built from bf16 panels");
   struct Mat { const uint16_t* W; int N; lnb_model::WPack* wp; };
   std::vector<Mat> mats;
   m->wp_w13.assign(L, lnb_model::WPack{});
@@ -2354,7 +2376,7 @@ static int per_row_head(const Launcher& L, lnb_session* s, const Rows& R) {
   p.rscale = strict ? s->rs : nullptr;
   p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
   p.out_f32 = s->logits; p.ldo = m->vocab_l; p.n_offset = m->tp_rank * m->vocab_l; p.st = nullptr; p.argmax_row = -1;
-  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, n, R.mb_rows, m->output_s))) return rc;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, n, R.mb_rows, m->output_s, m->wfmt))) return rc;
   if ((rc = gather_logits(s, 0, n))) return rc;
   const float* lg = (m->tp_size > 1) ? s->logits_full : s->logits;
   return launch_kernel(L, argmax_f32_kernel, dim3(n), dim3(256), 0, lg, a.vocab_size, s->d_next_arr);
@@ -2418,7 +2440,7 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
     p.W = W; p.N = a.dim; p.K = K; p.x = x; p.ldx = K; p.ldo = a.dim;
     if (m->tp_size == 1) {
       p.out_bf16 = out; p.res = res;
-      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S, mb_rows, Ws);
+      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S, mb_rows, Ws, m->wfmt);
     }
     int rc2;
     if (s->p2p_ready) {
@@ -2445,7 +2467,7 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
       p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
       p.cache_k = s->ck[l] + R.cache_off; p.cache_v = s->cv[l] + R.cache_off; p.cis = m->cis; p.pos_ptr = &s->st->pos;
       p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = R.seq_stride;
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, S, mb_rows, W.sqkv))) return rc;
+      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, S, mb_rows, W.sqkv, m->wfmt))) return rc;
     }
     if ((rc = launch_attention(L, s, l, R, s->o, 0))) return rc;
     if ((rc = proj_resid(W.wo, W.so, m->q_l, s->o, s->x, s->h1))) return rc;            // wo + residual (:522, :232)
@@ -2455,7 +2477,7 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
       p.rscale = strict ? s->rs : nullptr;
       p.W = W.w13; p.N = 2 * m->ffn_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm; p.eps = a.norm_eps;
       p.out_bf16 = s->mbuf; p.ldo = m->ffn_l; p.silu_tab = m->silu_tab;
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, S, mb_rows, W.s13))) return rc;
+      if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, S, mb_rows, W.s13, m->wfmt))) return rc;
     }
     if ((rc = proj_resid(W.w2, W.s2, m->ffn_l, s->mbuf, s->h1, s->x))) return rc;        // w2 + residual (:619, :248)
   }
@@ -2473,7 +2495,7 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
   p.st = s->st; p.argmax_row = rows - 1; p.m_off = 0;
   p.publish = (m->tp_size == 1) ? 1 : 0;
   p.advance = R.advance ? 1 : 0; p.tok_out = s->d_tok_out;
-  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, rows, 0, m->output_s))) return rc;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, rows, 0, m->output_s, m->wfmt))) return rc;
   if (m->tp_size > 1) {
     if (s->p2p_ready) rc = launch_kernel(L, p2p_argmax_kernel, dim3(1), dim3(32), 0, s->p2p, s->st, R.advance ? 1 : 0, s->d_tok_out);
     else rc = reduce_argmax_publish(L, s, R.advance);
@@ -2497,11 +2519,12 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
     return rc;
   const int n_layers = active_layers(s);
   const int ew_grid = m->sm_count * 8;
-  // the bf16 panels a GEMM reads: the matrix itself, or (MXFP8) rows [0, N) dequantized into the session's scratch
+  // the bf16 panels a GEMM reads: the matrix itself, or (MXFP8, MXFP4) rows [0, N) dequantized into the session's scratch
   auto tc_w = [&](GemmTcParams& g, const uint16_t* W, const uint8_t* Ws, int N, int K) -> int {
     g.W = Ws ? s->wdq : W;
     if (!Ws) return 0;
-    return launch_kernel(L, mxfp8_dequant_kernel, dim3(ew_grid), dim3(256), 0, reinterpret_cast<const uint8_t*>(W), Ws, N, K, s->wdq);
+    return launch_kernel(L, m->wfmt == LNB_WEIGHTS_MXFP4 ? mxfp4_dequant_kernel : mxfp8_dequant_kernel, dim3(ew_grid), dim3(256), 0,
+                         reinterpret_cast<const uint8_t*>(W), Ws, N, K, s->wdq);
   };
   // wo / w2 + residual: out = res + X W^T; tensor-parallel ranks sum their partials over NCCL first
   auto proj_resid = [&](const uint16_t* X8, const uint16_t* W, const uint8_t* Ws, int K, const uint16_t* res, uint16_t* out) -> int {
@@ -2555,12 +2578,12 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
       return rc;
     GemmTcParams g{};
     g.X8 = s->xn8; g.W = m->output; g.M = S - 1; g.N = m->vocab_l; g.K = a.dim; g.out_f32 = s->logits; g.ldo = m->vocab_l;
-    // MXFP8: the LM head in row slices that fit the scratch (whole 128-row tiles), each dequantized before its GEMM
+    // MXFP8, MXFP4: the LM head in row slices that fit the scratch (whole 128-row tiles), each dequantized before its GEMM
     const int slice = m->output_s ? (int)std::min<size_t>(m->vocab_l, s->wdq_elems / a.dim / TC_BN * TC_BN) : m->vocab_l;
     for (int n0 = 0; S > 1 && n0 < m->vocab_l; n0 += slice) {
       g.N = std::min(slice, m->vocab_l - n0);
       g.out_f32 = s->logits + n0;
-      const uint16_t* codes = reinterpret_cast<const uint16_t*>(reinterpret_cast<const uint8_t*>(m->output) + (size_t)n0 * a.dim);
+      const uint16_t* codes = reinterpret_cast<const uint16_t*>(reinterpret_cast<const uint8_t*>(m->output) + code_bytes(m->wfmt, n0, a.dim));
       if (m->output_s && (rc = tc_w(g, codes, m->output_s + (size_t)(n0 / 8) * mx_nbp(a.dim) * 8, g.N, a.dim))) return rc;
       if ((rc = launch_gemm_tc<TC_EPI_F32TRUNC>(L, g))) return rc;
     }
@@ -2568,7 +2591,7 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
     GemvParams p{};
     p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
     p.out_f32 = s->logits; p.ldo = m->vocab_l; p.st = nullptr; p.argmax_row = -1;
-    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, S - 1, 0, m->output_s))) return rc;
+    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, S - 1, 0, m->output_s, m->wfmt))) return rc;
   }
   {
     GemvParams p{};
@@ -2577,7 +2600,7 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
     p.out_f32 = R.head != HEAD_NONE ? s->logits + (R.head == HEAD_ALL ? (size_t)(S - 1) * m->vocab_l : 0) : nullptr;
     p.ldo = m->vocab_l; p.n_offset = m->tp_rank * m->vocab_l;
     p.st = s->st; p.argmax_row = 0; p.publish = (m->tp_size == 1) ? 1 : 0; p.advance = 0; p.tok_out = s->d_tok_out;
-    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1, 0, m->output_s))) return rc;
+    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1, 0, m->output_s, m->wfmt))) return rc;
     if (m->tp_size > 1) {
       if ((rc = reduce_argmax_publish(L, s, false))) return rc;
       if (R.head != HEAD_NONE && R.gather && (rc = gather_logits(s, 0, R.head_rows))) return rc;
@@ -3641,28 +3664,28 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
           p.W = W.wqkv; p.N = m->q_l + 2 * m->kv_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm;
           p.out_bf16 = s->q; p.ldo = m->q_l; p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
           p.cache_k = s->ck[l]; p.cache_v = s->cv[l]; p.cis = m->cis; p.pos_ptr = &s->st->pos;
-          rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, s->mode, p, 1, 0, ws);
+          rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, s->mode, p, 1, 0, ws, m->wfmt);
           break;
         case 1:
           p.W = W.wo; p.N = a.dim; p.K = m->q_l; p.x = s->o; p.ldx = m->q_l; p.ldo = a.dim; p.out_bf16 = s->h1; p.res = s->x;
-          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1, 0, ws);
+          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1, 0, ws, m->wfmt);
           break;
         case 2:
           p.W = W.w13; p.N = 2 * m->ffn_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm;
           p.out_bf16 = s->mbuf; p.ldo = m->ffn_l; p.silu_tab = m->silu_tab;
-          rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, s->mode, p, 1, 0, ws);
+          rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, s->mode, p, 1, 0, ws, m->wfmt);
           break;
         case 3:
           p.W = W.w2; p.N = a.dim; p.K = m->ffn_l; p.x = s->mbuf; p.ldx = m->ffn_l; p.ldo = a.dim; p.out_bf16 = s->h1; p.res = s->x;
-          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1, 0, ws);
+          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1, 0, ws, m->wfmt);
           break;
         case 4:
           p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.ldo = m->vocab_l;
           p.st = nullptr; p.argmax_row = -1;
-          rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1, 0, ws);
+          rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1, 0, ws, m->wfmt);
           break;
       }
-      bytes = (int64_t)mat_bytes(ws ? LNB_WEIGHTS_MXFP8 : LNB_WEIGHTS_BF16, p.N, p.K);
+      bytes = (int64_t)mat_bytes(m->wfmt, p.N, p.K);
       n_launch++;
     }
     return rc;

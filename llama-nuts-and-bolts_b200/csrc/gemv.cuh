@@ -27,9 +27,12 @@
 // MXFP8 weights (FMT == WF_MXFP8, mxfp8.cuh): the same producer streams each panel's E4M3 codes (64 B per chunk) and its
 // E8M0 scales; a stage carries twice the k-range of the bf16 config it mirrors, so as many bytes are in flight.  Consumers
 // decode every weight to the exact fp32 value of the bf16 number it stands for and run the same FMAs in the same order.
+// MXFP4 weights (FMT == WF_MXFP4, mxfp4.cuh) likewise, with 32 B of codes per chunk and the largest k-tile whose stage is
+// no larger than its bf16 twin's (gemv_kt), so an MXFP4 matrix gets the row block of the bf16 matrix it stands for.
 #pragma once
 #include "common.cuh"
 #include "mxfp8.cuh"
+#include "mxfp4.cuh"
 
 namespace lnb {
 
@@ -91,6 +94,10 @@ struct GemvParams {
   uint32_t res_tag_hi;     // tag << 16 of the phase that produced the residual
 };
 
+// the k-tile of format F for a bf16 k-tile kt: MXFP8 twice kt; MXFP4 the largest multiple of 64 whose codes, pad and
+// scales (kt4 * 4 + 32 + kt4 / 4 bytes per panel) fit in the bf16 panel's kt * 16 bytes
+constexpr int gemv_kt(int kt, int F) { return F == WF_MXFP4 ? ((64 * kt - 128) / 17) & ~63 : kt << F; }
+
 template <int TN, int KS, int MB, int KT, int NST, int FMT = WF_BF16>
 struct GemvCfg {
   static constexpr int kTN = TN, kKS = KS, kMB = MB, kKT = KT, kNST = NST, kFmt = FMT;
@@ -99,14 +106,15 @@ struct GemvCfg {
   static constexpr int kThreads = kNCons + 32;         // + producer warp
   // MXFP8: a panel's codes take KT * 8 bytes plus 64 bytes of padding, so the two panels a half-warp reads sit in opposite
   // halves of the banks (conflict-free 8-byte loads); the panels' scales (KT / 4 bytes each) follow
-  static constexpr int kPanelBytes = FMT == WF_MXFP8 ? KT * 8 + 64 : KT * 16;
+  // MXFP4: KT * 4 bytes plus 32, so the four panels a warp reads (4 bytes a lane) start in four different 8-bank groups
+  static constexpr int kPanelBytes = FMT == WF_MXFP8 ? KT * 8 + 64 : FMT == WF_MXFP4 ? KT * 4 + 32 : KT * 16;
   static constexpr int kScaleOff = kP * kPanelBytes;
-  static constexpr int kStageBytes = FMT == WF_MXFP8 ? kScaleOff + kP * (KT / 4) : TN * KT * 2;
+  static constexpr int kStageBytes = FMT != WF_BF16 ? kScaleOff + kP * (KT / 4) : TN * KT * 2;
   static constexpr int kChunksPerTile = KT / 8;
   static_assert(TN % 32 == 0 && TN <= 128, "TN");
   static_assert(kNCons % 32 == 0, "consumer warps");
   static_assert(kChunksPerTile % KS == 0, "k-tile must hold a whole number of chunk rounds");
-  static_assert(FMT == WF_BF16 || KT % 64 == 0, "MXFP8 k-tiles hold whole, 16-byte-aligned scale ranges");
+  static_assert(FMT == WF_BF16 || KT % 64 == 0, "MX k-tiles hold whole, 16-byte-aligned scale ranges");
   static size_t smem_bytes(int K) {
     size_t b = 1024;                                   // barriers + scalars (first 1 KB)
     b += (size_t)NST * kStageBytes;
@@ -249,7 +257,7 @@ LNB_DEVINL void logits_publish(const GemvParams& p) {
 
 // ------------------------------------------------------------------------------------------
 template <class Cfg, int PRO, int EPI>
-__global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p, const uint8_t* Ws) {   // Ws: MXFP8 scales
+__global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p, const uint8_t* Ws) {   // Ws: MX scales
   constexpr int TN = Cfg::kTN, KS = Cfg::kKS, MB = Cfg::kMB, KT = Cfg::kKT, NST = Cfg::kNST;
   constexpr int P = Cfg::kP, NCONS = Cfg::kNCons, STAGE = Cfg::kStageBytes;
   constexpr int CPT = Cfg::kChunksPerTile;
@@ -292,14 +300,15 @@ __global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p,
         mbar_wait(&empty_bar[s], ph ^ 1u);
         const int k0 = t * KT;
         const int kt = min(KT, K - k0);
-        if constexpr (Cfg::kFmt == WF_MXFP8) {
-          const uint32_t code_bytes = (uint32_t)kt * 8u;                          // kt/8 chunks * 64 B
+        if constexpr (Cfg::kFmt != WF_BF16) {
+          constexpr uint32_t cb = Cfg::kFmt == WF_MXFP8 ? 8u : 4u;               // code bytes per column of a panel
+          const uint32_t code_bytes = (uint32_t)kt * cb;                          // kt/8 chunks * 64 B (MXFP4: 32 B)
           const uint32_t scale_bytes = (uint32_t)(((kt + 31) / 32 + 1) & ~1) * 8u;  // whole 16-byte pairs of blocks
           const int nbp = mx_nbp(K);
           mbar_expect_tx(&full_bar[s], (code_bytes + scale_bytes) * (uint32_t)my_panels);
           for (int pp = 0; pp < my_panels; pp++) {
             const size_t panel = (size_t)(panel0 + pp);
-            bulk_g2s(s_stage + (size_t)s * STAGE + (size_t)pp * Cfg::kPanelBytes, wbase + (panel * (size_t)K + (size_t)k0) * 8u,
+            bulk_g2s(s_stage + (size_t)s * STAGE + (size_t)pp * Cfg::kPanelBytes, wbase + (panel * (size_t)K + (size_t)k0) * cb,
                      code_bytes, &full_bar[s], pol);
             bulk_g2s(s_stage + (size_t)s * STAGE + Cfg::kScaleOff + (size_t)pp * (KT / 4), Ws + (panel * nbp + k0 / 32) * 8u,
                      scale_bytes, &full_bar[s], pol);
@@ -428,6 +437,31 @@ __global__ void __launch_bounds__(Cfg::kThreads) gemv_kernel(const GemvParams p,
           a = __fmaf_rn(xb.y, w[5], a);
           a = __fmaf_rn(xb.z, w[6], a);
           a = __fmaf_rn(xb.w, w[7], a);
+          acc[m] = a;
+        }
+      }
+    } else if constexpr (Cfg::kFmt == WF_MXFP4) {
+      const uint8_t* ctile = s_stage + (size_t)s * STAGE + (size_t)pp * Cfg::kPanelBytes + rr * 4;
+      const uint8_t* stile = s_stage + (size_t)s * STAGE + Cfg::kScaleOff + (size_t)pp * (KT / 4) + rr;
+      constexpr int UNROLL = MB > 2 ? 1 : 4;
+#pragma unroll UNROLL
+      for (int ch = j; ch < nchunks; ch += KS) {
+        uint32_t P[4];   // P[g] = {column g, column g + 4}
+        mx4_decode8(*reinterpret_cast<const uint32_t*>(ctile + ch * 32), mx4_scale2(stile[(ch >> 2) * 8]), P);
+        const float* xk = s_x + k0 + ch * 8;
+#pragma unroll
+        for (int m = 0; m < MB; m++) {
+          const float4 xa = *reinterpret_cast<const float4*>(xk + (size_t)m * K);
+          const float4 xb = *reinterpret_cast<const float4*>(xk + (size_t)m * K + 4);
+          float a = acc[m];
+          a = __fmaf_rn(xa.x, bf_lo(P[0]), a);
+          a = __fmaf_rn(xa.y, bf_lo(P[1]), a);
+          a = __fmaf_rn(xa.z, bf_lo(P[2]), a);
+          a = __fmaf_rn(xa.w, bf_lo(P[3]), a);
+          a = __fmaf_rn(xb.x, bf_hi(P[0]), a);
+          a = __fmaf_rn(xb.y, bf_hi(P[1]), a);
+          a = __fmaf_rn(xb.z, bf_hi(P[2]), a);
+          a = __fmaf_rn(xb.w, bf_hi(P[3]), a);
           acc[m] = a;
         }
       }

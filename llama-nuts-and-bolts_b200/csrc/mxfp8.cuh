@@ -19,7 +19,7 @@
 
 namespace lnb {
 
-enum { WF_BF16 = 0, WF_MXFP8 = 1 };
+enum { WF_BF16 = 0, WF_MXFP8 = 1, WF_MXFP4 = 2 };   // = LNB_WEIGHTS_*; WF_MXFP4: mxfp4.cuh
 
 // scale bytes per panel row of 8 rows: blocks of 32 columns, padded to an even count
 __host__ __device__ inline int mx_nbp(int K) { return ((K + 31) / 32 + 1) & ~1; }

@@ -58,7 +58,7 @@ class Vocabulary:  # src/model/vocabulary.go (ids only; the tokenizer is out of 
     StopTokenIds: tuple = synth.STOP_IDS
 
 
-WEIGHT_FORMATS = {"bf16": _capi.LNB_WEIGHTS_BF16, "mxfp8": _capi.LNB_WEIGHTS_MXFP8}
+WEIGHT_FORMATS = {"bf16": _capi.LNB_WEIGHTS_BF16, "mxfp8": _capi.LNB_WEIGHTS_MXFP8, "mxfp4": _capi.LNB_WEIGHTS_MXFP4}
 
 
 class LlamaTransformer:
@@ -66,7 +66,7 @@ class LlamaTransformer:
 
     def __init__(self, args: ModelArgs, device: int = 0, tp_rank: int = 0, tp_size: int = 1, nccl_id: bytes | None = None,
                  weight_format: str = "bf16"):
-        """weight_format: "bf16", or "mxfp8": finalize quantizes the linear weights (DESIGN.md §9h)"""
+        """weight_format: "bf16", or "mxfp8" / "mxfp4": finalize quantizes the linear weights (DESIGN.md §9h, §9i)"""
         self.args = args
         self.device, self.tp_rank, self.tp_size = device, tp_rank, tp_size
         self._cargs = _capi.ModelArgsC(**args.to_c_dict())
@@ -116,8 +116,18 @@ class LlamaTransformer:
         check(lib.lnb_model_mxfp8_read(self.h, name.encode(), codes.ctypes.data, scales.ctypes.data))
         return codes, scales
 
+    def mxfp4_read(self, name: str) -> tuple[np.ndarray, np.ndarray]:
+        """the E2M1 codes [rows, cols / 2] (two a byte, the even column in the low nibble) and E8M0 scales
+        [rows, ceil(cols / 32)] of a linear checkpoint tensor of a finalized MXFP4 model, in the checkpoint's row order"""
+        shape = synth.tensor_shapes(self.args.to_c_dict()).get(name, (0,))
+        rows, cols = shape if len(shape) == 2 else (shape[0], 2)   # the library names what is wrong with other names
+        codes = np.empty((rows, cols // 2), np.uint8)
+        scales = np.empty((rows, (cols + 31) // 32), np.uint8)
+        check(lib.lnb_model_mxfp4_read(self.h, name.encode(), codes.ctypes.data, scales.ctypes.data))
+        return codes, scales
+
     def weight_info(self) -> dict:
-        """{"format": "bf16" | "mxfp8", "device_bytes": weight bytes in HBM, "step_bytes": weight bytes one S = 1 step reads}"""
+        """{"format": "bf16" | "mxfp8" | "mxfp4", "device_bytes": weight bytes in HBM, "step_bytes": weight bytes one S = 1 step reads}"""
         fmt, dev, step = C.c_int(0), C.c_int64(0), C.c_int64(0)
         check(lib.lnb_model_weight_info(self.h, C.byref(fmt), C.byref(dev), C.byref(step)))
         names = {v: k for k, v in WEIGHT_FORMATS.items()}

@@ -672,3 +672,60 @@ void orc_mxfp8_dequantize(const uint8_t* codes, const uint8_t* scales, int rows,
       out[(int64_t)r * cols + c] = (uint16_t)(bits >> 16);
     }
 }
+
+/* MXFP4 linear weights (DESIGN.md §9i): the MXFP8 blocks, one E2M1 code per weight, packed two a byte with the even
+ * column in the low nibble: codes [rows][cols / 2], scales [rows][ceil(cols / 32)].  X = e - 2 if the 7-bit mantissa field
+ * f of the bf16 block maximum is <= 64, else e - 1 (e its unbiased exponent), clamped to [-125, 125]; -125 for a zero or
+ * subnormal maximum.  code = sign bit | |w| * 2^-X rounded to the nearest of {0, 0.5, 1, 1.5, 2, 3, 4, 6}, ties to the even
+ * mantissa bit (index), saturated at 6.  Returns the index of the first non-finite weight, or -1. */
+int64_t orc_mxfp4_quantize(const uint16_t* w, int rows, int cols, uint8_t* codes, uint8_t* scales) {
+  static const double grid[8] = {0.0, 0.5, 1.0, 1.5, 2.0, 3.0, 4.0, 6.0};
+  for (int64_t i = 0; i < (int64_t)rows * cols; i++)
+    if ((w[i] & 0x7f80) == 0x7f80) return i;
+  const int nb = (cols + 31) / 32;
+  memset(codes, 0, (size_t)rows * (cols / 2));
+  for (int r = 0; r < rows; r++)
+    for (int b = 0; b < nb; b++) {
+      const int c0 = b * 32, c1 = c0 + 32 < cols ? c0 + 32 : cols;
+      uint16_t amax = 0;
+      for (int c = c0; c < c1; c++) {
+        const uint16_t mag = w[(int64_t)r * cols + c] & 0x7fff;
+        if (mag > amax) amax = mag;
+      }
+      const int E = amax >> 7;
+      int X = E == 0 ? -125 : E - 127 - ((amax & 0x7f) <= 64 ? 2 : 1);
+      if (X < -125) X = -125;
+      if (X > 125) X = 125;
+      scales[(int64_t)r * nb + b] = (uint8_t)(X + 127);
+      for (int c = c0; c < c1; c++) {
+        const uint16_t h = w[(int64_t)r * cols + c];
+        const uint32_t bits = (uint32_t)(h & 0x7fff) << 16;
+        float f;
+        memcpy(&f, &bits, 4);
+        const double q = ldexp((double)f, -X);
+        int k = 0;   /* nearest grid point; on a tie the one with the even index */
+        for (int j = 1; j < 8; j++) {
+          const double d0 = q - grid[k], d1 = grid[j] - q;
+          if (d1 < d0 || (d1 == d0 && (j & 1) == 0)) k = j;
+        }
+        const uint8_t code = (uint8_t)(((h >> 12) & 8) | k);
+        codes[(int64_t)r * (cols / 2) + c / 2] |= (uint8_t)(code << (4 * (c & 1)));
+      }
+    }
+  return -1;
+}
+/* e2m1(code) * 2^X as bf16 bits (exact: zero or a normal number of at most 2 significant bits inside the bf16 range) */
+void orc_mxfp4_dequantize(const uint8_t* codes, const uint8_t* scales, int rows, int cols, uint16_t* out) {
+  static const double grid[8] = {0.0, 0.5, 1.0, 1.5, 2.0, 3.0, 4.0, 6.0};
+  const int nb = (cols + 31) / 32;
+  for (int r = 0; r < rows; r++)
+    for (int c = 0; c < cols; c++) {
+      const int code = (codes[(int64_t)r * (cols / 2) + c / 2] >> (4 * (c & 1))) & 15;
+      const int X = (int)scales[(int64_t)r * nb + c / 32] - 127;
+      const double v = ldexp(grid[code & 7], X);
+      const float f = (float)((code & 8) ? -v : v);
+      uint32_t bits;
+      memcpy(&bits, &f, 4);
+      out[(int64_t)r * cols + c] = (uint16_t)(bits >> 16);
+    }
+}

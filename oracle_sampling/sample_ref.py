@@ -88,6 +88,10 @@ def lib():
         L.orc_mxfp8_quantize.argtypes = [_u16p, C.c_int, C.c_int, _u8p, _u8p]
         L.orc_mxfp8_dequantize.restype = None
         L.orc_mxfp8_dequantize.argtypes = [_u8p, _u8p, C.c_int, C.c_int, _u16p]
+        L.orc_mxfp4_quantize.restype = C.c_int64
+        L.orc_mxfp4_quantize.argtypes = [_u16p, C.c_int, C.c_int, _u8p, _u8p]
+        L.orc_mxfp4_dequantize.restype = None
+        L.orc_mxfp4_dequantize.argtypes = [_u8p, _u8p, C.c_int, C.c_int, _u16p]
         L.orc_generate_sampled.restype = C.c_int
         L.orc_generate_sampled.argtypes = [C.c_void_p, C.c_int, _i32p, C.c_int, C.c_int, _i32p, C.c_int, C.c_float, C.c_int32,
                                            C.c_float, C.c_uint64, _i32p]
@@ -359,5 +363,35 @@ def mxfp8_dequantize(codes, scales) -> np.ndarray:
     out = np.empty((rows, cols), np.uint16)
     u8 = C.POINTER(C.c_uint8)
     lib().orc_mxfp8_dequantize(codes.ctypes.data_as(u8), scales.ctypes.data_as(u8), rows, cols,
+                               out.ctypes.data_as(C.POINTER(C.c_uint16)))
+    return out
+
+
+def mxfp4_quantize(w) -> tuple[np.ndarray, np.ndarray]:
+    """orc_mxfp4_quantize of a bf16 matrix (uint16 bits [rows, cols], cols even): (codes [rows, cols / 2] u8, two a byte
+    with the even column in the low nibble, scales [rows, ceil(cols/32)] u8).  A non-finite weight raises ValueError
+    naming its row and column."""
+    w = np.ascontiguousarray(w, np.uint16)
+    rows, cols = w.shape
+    assert cols % 2 == 0
+    codes = np.empty((rows, cols // 2), np.uint8)
+    scales = np.empty((rows, (cols + 31) // 32), np.uint8)
+    u8 = C.POINTER(C.c_uint8)
+    bad = lib().orc_mxfp4_quantize(w.ctypes.data_as(C.POINTER(C.c_uint16)), rows, cols, codes.ctypes.data_as(u8),
+                                   scales.ctypes.data_as(u8))
+    if bad >= 0:
+        raise ValueError(f"non-finite weight at row {bad // cols}, column {bad % cols}")
+    return codes, scales
+
+
+def mxfp4_dequantize(codes, scales) -> np.ndarray:
+    """orc_mxfp4_dequantize: the bf16 bits [rows, 2 * codes.shape[1]] of e2m1(code) * 2^X"""
+    codes = np.ascontiguousarray(codes, np.uint8)
+    scales = np.ascontiguousarray(scales, np.uint8)
+    rows, cols = codes.shape[0], 2 * codes.shape[1]
+    assert scales.shape == (rows, (cols + 31) // 32)
+    out = np.empty((rows, cols), np.uint16)
+    u8 = C.POINTER(C.c_uint8)
+    lib().orc_mxfp4_dequantize(codes.ctypes.data_as(u8), scales.ctypes.data_as(u8), rows, cols,
                                out.ctypes.data_as(C.POINTER(C.c_uint16)))
     return out

@@ -1,0 +1,469 @@
+"""MXFP4 linear weights on the GPU (DESIGN.md §9i): the checks of the MXFP8 suite for the 4-bit format.  The quantizer
+against the C statement (orc_mxfp4_quantize), bit for bit; then the identity the format promises: an MXFP4 model returns
+the bits of the bf16 model D(W) whose linear weights are the dequantized values (orc_mxfp4_dequantize) on every route --
+prompts on the FMA pipes and on the tensor cores, host-driven and device-resident decode, batched, ragged, speculative and
+chunked calls, streamed attention and the generate loops -- in STRICT and FAST; STRICT against the CPU oracle of D(W); and
+the routing: the engines and the packed stream refuse MXFP4 and say why."""
+import ctypes
+import os
+
+import numpy as np
+import pytest
+
+from oracle_sampling import sample_ref as SR
+from tests import engine_shapes as ES
+from tests import model_shapes as MS
+from tests.helpers import host_tensors, oracle_model
+from tests.test_gpu_mxfp8 import LAYER_LINEAR, _acc, _caches_equal, _ctx, _steps, _tc_extra, linear_names
+
+pytestmark = pytest.mark.gpu
+
+PROMPT = [1, 50, 999, 7, 300, 12, 64, 2]
+NO_STOP = (10**9,)
+SEED = 2718
+
+
+@pytest.fixture(scope="module")
+def L():
+    import lnb_b200
+    return lnb_b200
+
+
+def dequantized(args, tensors):
+    """D(W): the checkpoint with every linear weight replaced by its dequantized MXFP4 value (the C statement)"""
+    out = dict(tensors)
+    for name in linear_names(args):
+        codes, scales = SR.mxfp4_quantize(tensors[name])
+        out[name] = SR.mxfp4_dequantize(codes, scales)
+    return out
+
+
+class Pair:
+    """an MXFP4 model and the bf16 model of its D(W), from one synthetic checkpoint"""
+
+    def __init__(self, L, args):
+        self.args = args
+        self.tensors = host_tensors(args, SEED)
+        self.dw_tensors = dequantized(args, self.tensors)
+        self.mx = L.model.LoadModelFromTensors(args, self.tensors, weight_format="mxfp4")
+        self.dw = L.model.LoadModelFromTensors(args, self.dw_tensors)
+
+    def close(self):
+        self.mx.Free()
+        self.dw.Free()
+
+
+def _pair(L, args):
+    p = Pair(L, args)
+    yield p
+    p.close()
+
+
+@pytest.fixture(scope="module")
+def tiny(L):
+    yield from _pair(L, dict(L.synth.TINY))
+
+
+@pytest.fixture(scope="module")
+def tiny128(L):
+    yield from _pair(L, dict(L.synth.TINY128))
+
+
+@pytest.fixture(scope="module")
+def wide(L):
+    import torch
+    yield from _pair(L, ES.wide_args(torch.cuda.get_device_properties(0).multi_processor_count))   # w2: K % 32 == 16
+
+
+@pytest.fixture(scope="module")
+def tail16(L):
+    # ffn_dim % 32 == 16: w2's last block of every row is 16 wide; w1|w3 hold 33 blocks of 16 rows
+    yield from _pair(L, dict(MS.CATALOGUE["one_layer"], ffn_dim=528))
+
+
+# ---- quantizer ----------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("model", ["tiny", "tiny128", "wide", "tail16"])
+def test_quantizer_equals_the_c_statement(L, request, model):
+    p = request.getfixturevalue(model)
+    for name in linear_names(p.args):
+        codes, scales = p.mx.Transformer.mxfp4_read(name)
+        want_c, want_s = SR.mxfp4_quantize(p.tensors[name])
+        assert np.array_equal(scales, want_s), name
+        assert np.array_equal(codes, want_c), name
+
+
+@pytest.mark.parametrize("name,row,col,bits", [("layers.1.feed_forward.w3.weight", 5, 17, 0x7F80),
+                                               ("layers.0.attention.wk.weight", 40, 3, 0xFFC0),
+                                               ("output.weight", 1000, 255, 0xFF80)])
+def test_non_finite_weight_fails_finalize_with_its_index(L, name, row, col, bits):
+    args = dict(L.synth.TINY)
+    tensors = host_tensors(args, SEED)
+    tensors[name] = tensors[name].copy()
+    tensors[name][row, col] = bits
+    m = L.model.Model(L.model.ModelArgs.from_c_dict(args), weight_format="mxfp4")
+    try:
+        for k, v in tensors.items():
+            m.Transformer.upload_tensor(k, v)
+        with pytest.raises(L._capi.LnbError, match=f'"{name}" has a non-finite weight at row {row}, column {col}') as e:
+            m.Transformer.finalize()
+        assert e.value.code == -1
+    finally:
+        m.Free()
+
+
+# ---- identity: prompts ----------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("model", ["tiny", "tiny128", "wide", "tail16"])
+@pytest.mark.parametrize("mode", ["strict", "fast"])
+def test_prompt_logits_and_caches(L, request, model, mode):
+    p = request.getfixturevalue(model)
+    acc, seq = _acc(L, mode), 64
+    rng = np.random.default_rng(3)
+    for S in (1, 7, 40):
+        toks = rng.integers(0, p.args["vocab_size"], S).astype(np.int32)
+        # the bf16 session on the kernel chain too, so that launch counts compare (the engine's bits are the chain's)
+        a, b = _ctx(L, p.mx, seq, acc, max_rows=40), _ctx(L, p.dw, seq, acc, max_rows=40, engine=False)
+        try:
+            la, lb = a.launch_count(), b.launch_count()
+            ga = p.mx.Transformer.Forward(a, L.ml.Tensor(toks, L.ml.DT_INT32), 0).RawData
+            gb = p.dw.Transformer.Forward(b, L.ml.Tensor(toks, L.ml.DT_INT32), 0).RawData
+            assert np.array_equal(ga, gb), (S, np.abs(ga - gb).max())
+            _caches_equal(p.args, a, b, S)
+            extra = _tc_extra(p.args, S, mode == "strict", 40)
+            assert (a.launch_count() - la) - (b.launch_count() - lb) == extra, S
+            if model == "tiny128" and mode == "fast" and S == 40:
+                assert extra > 0, "the tensor-core route was not taken"
+        finally:
+            a.close(); b.close()
+
+
+def test_chunked_prefill(L, tiny128):
+    p = tiny128
+    for mode in ("strict", "fast"):
+        a, b = _ctx(L, p.mx, 64, _acc(L, mode), max_rows=40), _ctx(L, p.dw, 64, _acc(L, mode), max_rows=40)
+        try:
+            out = []
+            for ctx, m in ((a, p.mx), (b, p.dw)):
+                ctx.allow_chunked_prefill()
+                toks = np.arange(3, 3 + 45, dtype=np.int32)
+                lg = []
+                for s0, s1 in ((0, 5), (5, 38), (38, 45)):
+                    lg.append(m.Transformer.Forward(ctx, L.ml.Tensor(toks[s0:s1], L.ml.DT_INT32), s0).RawData)
+                out.append(np.concatenate(lg))
+            assert np.array_equal(out[0], out[1]), mode
+            _caches_equal(p.args, a, b, 45)
+        finally:
+            a.close(); b.close()
+
+
+# ---- identity: decode ---------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("model", ["tiny", "tiny128", "wide"])
+@pytest.mark.parametrize("mode", ["strict", "fast"])
+def test_decode_host_driven_and_device_resident(L, request, model, mode):
+    p = request.getfixturevalue(model)
+    acc, seq, n = _acc(L, mode), 48, 24
+    a, b = _ctx(L, p.mx, seq, acc), _ctx(L, p.dw, seq, acc)
+    try:
+        ta, la = _steps(p.mx, a, n)
+        tb, lb = _steps(p.dw, b, n)
+        assert ta == tb
+        assert np.array_equal(la, lb)
+        _caches_equal(p.args, a, b, len(PROMPT) + n)
+    finally:
+        a.close(); b.close()
+    for use_graph in (False, True):
+        got = []
+        for m in (p.mx, p.dw):
+            ctx = _ctx(L, m, seq, acc, engine=False if m is p.dw else None)
+            first, _ = m.Transformer.forward_argmax(ctx, np.array(PROMPT, np.int32), 0)
+            toks, _, _ = ctx.decode_run(first, len(PROMPT), n, use_graph=use_graph)
+            got.append([first] + list(toks))
+            ctx.close()
+        assert got[0] == got[1], use_graph
+
+
+@pytest.mark.parametrize("n_seq", [3, 8])
+@pytest.mark.parametrize("mode", ["strict", "fast"])
+def test_batched_steps(L, tiny128, n_seq, mode):
+    p = tiny128
+    acc, seq = _acc(L, mode), 40
+    prompts = [[1 + i, 50 + 3 * i, 999 - i, 7, 300 + i] for i in range(n_seq)]
+    res = []
+    ctxs = [_ctx(L, p.mx, seq, acc, n_seq=n_seq), _ctx(L, p.dw, seq, acc, n_seq=n_seq)]
+    try:
+        for ctx, m in zip(ctxs, (p.mx, p.dw)):
+            last = []
+            for s, pr in enumerate(prompts):
+                ctx.set_active_sequence(s)
+                last.append(m.Transformer.forward_argmax(ctx, np.array(pr, np.int32), 0)[0])
+            lg = []
+            for j in range(6):
+                nxt, l = ctx.forward_batch(last, [len(prompts[0]) + j] * n_seq, want_logits=True)
+                last = list(nxt)
+                lg.append(l)
+            res.append(np.array(lg))
+        assert np.array_equal(res[0], res[1])
+        _caches_equal(p.args, ctxs[0], ctxs[1], len(prompts[0]) + 6, seqs=range(n_seq))
+    finally:
+        for c in ctxs:
+            c.close()
+
+
+@pytest.mark.parametrize("mode", ["strict", "fast"])
+def test_ragged_and_speculative_calls(L, tiny128, mode):
+    p = tiny128
+    acc, seq = _acc(L, mode), 64
+    res = []
+    for m in (p.mx, p.dw):
+        ctx = _ctx(L, m, seq, acc, n_seq=3, max_rows=40)
+        try:
+            n1, l1 = ctx.forward_ragged([(0, 0, PROMPT), (1, 0, PROMPT[:3]), (2, 0, list(range(5, 30)))], want_logits=True)
+            n2, l2 = ctx.forward_ragged([(0, 8, [int(n1[0])]), (1, 3, PROMPT[3:]), (2, 25, [int(n1[2])])], want_logits=True)
+            nx, na, l3 = ctx.forward_speculative([(0, 9, [int(n2[0]), 5, 6, 7]), (2, 26, [int(n2[2]), 11, 12])], want_logits=True)
+            res.append((n1, l1, n2, l2, nx, na, l3))
+        finally:
+            ctx.close()
+    for x, y in zip(*res):
+        assert np.array_equal(np.asarray(x), np.asarray(y))
+
+
+@pytest.mark.parametrize("mode", ["strict", "fast"])
+def test_streamed_attention_past_the_decode_kernel(L, mode):
+    """batched steps of a session one key past sdpa_decode_kernel's fit run the streamed kernels"""
+    args = dict(L.synth.TINY, max_seq_len=4096)
+    seq = MS.sdpa_decode_fit(args) + 1
+    assert not MS.sdpa_smem_decode(args, seq)
+    p = Pair(L, args)
+    try:
+        res = []
+        for m in (p.mx, p.dw):
+            ctx = _ctx(L, m, seq, _acc(L, mode), n_seq=2)
+            last = []
+            for s in range(2):
+                ctx.set_active_sequence(s)
+                last.append(m.Transformer.forward_argmax(ctx, np.array(PROMPT[s:], np.int32), 0)[0])
+            lg = []
+            for j in range(4):
+                nxt, l = ctx.forward_batch(last, [len(PROMPT) - s + j for s in range(2)], want_logits=True)
+                last = list(nxt)
+                lg.append(l)
+            res.append(np.array(lg))
+            ctx.close()
+        assert np.array_equal(res[0], res[1])
+    finally:
+        p.close()
+
+
+# ---- identity: generate loops -------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("mode", ["strict", "fast"])
+def test_generate_loops(L, tiny, mode, tmp_path):
+    p = tiny
+    acc, seq = _acc(L, mode), 40
+    path = str(tmp_path / "tokenizer.model")
+    L._capi.check(L._capi.lib.lnb_vocab_write_synthetic(path.encode(), p.args["vocab_size"] - 256))
+    vocab = L.vocabulary.Load(path)
+    runs = []
+    for m in (p.mx, p.dw):
+        saved = m.Vocabulary
+        m.Vocabulary = vocab
+        try:
+            eng = L.inference.InferenceEngine(m, L.model.InferenceArgs(seq), acc_mode=acc)
+            out = {}
+            out["sampled"] = [t for _, t in eng.GenerateTokens(PROMPT, sampling=L.model.SamplingArgs(0.8, 40, 0.95, 77))]
+            out["penalized"] = [t for _, t in eng.GenerateTokens(PROMPT, penalties=L.model.PenaltyArgs(1.3, 0.4, 0.2))]
+            lp = []
+            out["logprobs"] = [t for _, t in eng.GenerateTokens(PROMPT, logprobs=5, logprobs_out=lp)]
+            out["logprob_records"] = [repr(r) for r in lp]
+            g = L.model.Grammar(m.Transformer, r"[a-z]+( [a-z]+)*\.", vocab)
+            out["grammar"] = [t for _, t in eng.GenerateTokens(PROMPT, grammar=g)]
+            g.close()
+            out["beams"] = [repr(h) for h in eng.GenerateBeams(PROMPT, L.inference.BeamSearchArgs(3, NumReturn=3))]
+            runs.append(out)
+        finally:
+            m.Vocabulary = saved
+    for k in runs[0]:
+        assert runs[0][k] == runs[1][k], k
+        assert len(runs[0][k]) > 0, k
+
+
+# ---- oracle ---------------------------------------------------------------------------------------------------------------
+def test_strict_equals_the_oracle_of_dw(L, tiny):
+    p = tiny
+    om = oracle_model(p.args, p.dw_tensors)
+    try:
+        want = list(om.generate(PROMPT, 40, stop_ids=NO_STOP))
+        eng = L.inference.InferenceEngine(p.mx, L.model.InferenceArgs(40), acc_mode=L._capi.LNB_ACC_STRICT)
+        saved = p.mx.Vocabulary
+
+        class V:
+            StopTokenIds = NO_STOP
+            PadId = saved.PadId
+        p.mx.Vocabulary = V
+        try:
+            assert [t for _, t in eng.GenerateTokens(PROMPT)] == want
+        finally:
+            p.mx.Vocabulary = saved
+        os_ = om.new_session(40)
+        ctx = _ctx(L, p.mx, 40, L._capi.LNB_ACC_STRICT)
+        try:
+            lo = os_.forward(np.array(PROMPT, np.int32), 0)
+            lg = p.mx.Transformer.Forward(ctx, L.ml.Tensor(np.array(PROMPT, np.int32), L.ml.DT_INT32), 0).RawData
+            assert np.array_equal(lo, lg)
+        finally:
+            ctx.close(); os_.close()
+    finally:
+        om.close()
+
+
+def test_cli_and_load_model_take_the_weight_format(L, tmp_path):
+    """host/lnb_generate <seq_len> strict <dir> weights=mxfp4 (the C++ mirror's LoadModel) prints the tokens of the Python
+    mirror's LoadModel(dir, weight_format="mxfp4"), which are those of the bf16 model of its D(W)"""
+    import subprocess
+    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+    exe = os.path.join(root, "host", "lnb_generate")
+    if not os.path.exists(exe):
+        subprocess.check_call(["make", "-C", os.path.join(root, "host"), "-s"])
+    d = str(tmp_path)
+    subprocess.run([exe, "--write-synthetic", d, "tiny"], check=True, capture_output=True, timeout=120)
+    mx = L.model.LoadModel(d, weight_format="mxfp4")
+    dw = None
+    try:
+        args = mx.Transformer.args.to_c_dict()
+        dw = L.model.Model(mx.Transformer.args)
+        lin = set(linear_names(args))
+        with L.torch_reader.TorchModelReader(os.path.join(d, "consolidated.00.pth")) as r:
+            for name, t in r.Load().items():
+                if name in L.synth.tensor_shapes(args):
+                    dw.Transformer.upload_tensor(name, SR.mxfp4_dequantize(*mx.Transformer.mxfp4_read(name)) if name in lin
+                                                 else np.asarray(t.RawData).view(np.uint16).reshape(t.Size))
+        dw.Transformer.finalize()
+        want = []
+        for m in (mx, dw):
+            m.Vocabulary = L.model.Vocabulary(StopTokenIds=NO_STOP)   # the CLI's stop set below the 8B vocabulary
+            eng = L.inference.InferenceEngine(m, L.model.InferenceArgs(32), acc_mode=L._capi.LNB_ACC_STRICT)
+            want.append([t for _, t in eng.GenerateTokens(PROMPT)])
+        assert want[0] == want[1] and want[0]
+        out = subprocess.run([exe, "32", "strict", d, "weights=mxfp4"], capture_output=True, text=True, timeout=120)
+        assert out.returncode == 0, out.stderr
+        line = next(ln for ln in out.stdout.splitlines() if ln.startswith("tokens:"))
+        assert [int(t) for t in line.split()[1:]] == want[0]
+        bad = subprocess.run([exe, "32", "strict", d, "weights=fp4"], capture_output=True, text=True, timeout=120)
+        assert bad.returncode != 0 and "weights=fp4" in bad.stderr
+    finally:
+        mx.Free()
+        if dw is not None:
+            dw.Free()
+
+
+# ---- routing ------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("mode", ["strict", "fast"])
+@pytest.mark.parametrize("env", [None, True])
+def test_engines_refuse_and_the_session_stays_usable(L, tiny128, mode, env):
+    p = tiny128
+    acc = _acc(L, mode)
+    a = _ctx(L, p.mx, 40, acc, engine=env)
+    b = _ctx(L, p.dw, 40, acc, engine=False)
+    try:
+        assert not a.uses_engine()
+        assert "MXFP4" in L._capi.lib.lnb_last_error().decode()
+        ta, la = _steps(p.mx, a, 4)
+        tb, lb = _steps(p.dw, b, 4)
+        assert ta == tb and np.array_equal(la, lb)
+    finally:
+        a.close(); b.close()
+    # batched and speculative calls take the kernel chain: one launch per call would be the batch engine
+    c = _ctx(L, p.mx, 40, acc, n_seq=2, engine=env)
+    try:
+        for s in range(2):
+            c.set_active_sequence(s)
+            p.mx.Transformer.forward_argmax(c, np.array(PROMPT, np.int32), 0)
+        l0 = c.launch_count()
+        c.forward_batch([3, 4], [8, 8])
+        assert c.launch_count() - l0 > 1
+    finally:
+        c.close()
+
+
+def test_packed_stream_refuses(L, tiny128):
+    info = (ctypes.c_int64 * 5)()
+    assert L._capi.lib.lnb_model_wpack_read(tiny128.mx.Transformer.h, -1, None, None, None, info) == 0
+    assert "MXFP4" in L._capi.lib.lnb_last_error().decode()
+
+
+def test_weight_format_errors_and_weight_info(L, tiny128):
+    p = tiny128
+    lib = L._capi.lib
+    assert lib.lnb_model_set_weight_format(p.mx.Transformer.h, L._capi.LNB_WEIGHTS_BF16) == -4      # LNB_ESTATE
+    m = L.model.Model(L.model.ModelArgs.from_c_dict(p.args))
+    try:
+        assert lib.lnb_model_set_weight_format(m.Transformer.h, 7) == -1                             # LNB_EINVAL
+        assert lib.lnb_model_set_weight_format(m.Transformer.h, L._capi.LNB_WEIGHTS_MXFP4) == 0
+    finally:
+        m.Free()
+    with pytest.raises(ValueError):
+        L.model.Model(L.model.ModelArgs.from_c_dict(p.args), weight_format="fp4")
+    a, b = p.mx.Transformer.weight_info(), p.dw.Transformer.weight_info()
+    assert a["format"] == "mxfp4" and b["format"] == "bf16"
+    w = MS.widths(p.args)
+    d, q, kv, f, v = p.args["dim"], w["q_l"], w["kv_l"], w["ffn_l"], w["vocab_l"]
+    mats = [(q + 2 * kv, d), (d, q), (2 * f, d), (d, f)] * p.args["n_layers"] + [(v, d)]
+    drop = sum(N * K * 2 - (N * K // 2 + N // 8 * ((-(-K // 32) + 1) & ~1) * 8) for N, K in mats)
+    assert b["device_bytes"] - a["device_bytes"] == drop
+    assert b["step_bytes"] - a["step_bytes"] == drop
+    # the tensor-parallel refusal is in lnb_model_set_weight_format (this suite has one GPU): read it there
+    src = open(os.path.join(os.path.dirname(os.path.dirname(__file__)), "llama-nuts-and-bolts_b200", "csrc", "api.cu")).read()
+    body = src[src.index('extern "C" int lnb_model_set_weight_format'):]
+    body = body[:body.index("\n}\n")]
+    assert "m->tp_size > 1" in body and "LNB_EINVAL" in body
+
+
+# ---- 8B ---------------------------------------------------------------------------------------------------------------------
+def test_8b_mxfp4_equals_its_dequantized_model(L):
+    """synthetic 8B: the LM head's and layer 0's codes against the C statement; then an MXFP4 model against the bf16 model of
+    its D(W), built tensor by tensor from the library's own codes (both fit in 80 GB): FAST 8-token prompt and 32 decode
+    steps, STRICT 8 + 10 with the first and last layer's caches"""
+    args = dict(L.synth.LLAMA31_8B)
+    mx = L.model.LoadSyntheticModel(args, weight_format="mxfp4")
+    dw = None
+    try:
+        for name in ["output.weight"] + [f"layers.0.{n}" for n in LAYER_LINEAR]:
+            w = L.synth.fill_host(args, name)
+            codes, scales = mx.Transformer.mxfp4_read(name)
+            wc, ws = SR.mxfp4_quantize(w)
+            assert np.array_equal(scales, ws) and np.array_equal(codes, wc), name
+            del w, wc, ws
+        dw = L.model.Model(L.model.ModelArgs.from_c_dict(args))
+        lin = set(linear_names(args))
+        for name in L.synth.tensor_shapes(args):
+            if name in lin:
+                codes, scales = mx.Transformer.mxfp4_read(name)
+                dw.Transformer.upload_tensor(name, SR.mxfp4_dequantize(codes, scales))
+            else:
+                dw.Transformer.upload_tensor(name, L.synth.fill_host(args, name))
+        dw.Transformer.finalize()
+        prompt = L.synth.PROMPT_8
+        for mode, n in (("fast", 32), ("strict", 10)):
+            a, b = _ctx(L, mx, 64, _acc(L, mode)), _ctx(L, dw, 64, _acc(L, mode), engine=False)
+            try:
+                ta, la = [], []
+                for m, ctx in ((mx, a), (dw, b)):
+                    t, lg0 = m.Transformer.forward_argmax(ctx, np.array(prompt, np.int32), 0, want_logits="last")
+                    toks, lgs = [t], [lg0[0]]
+                    for j in range(n):
+                        t, lg = m.Transformer.forward_argmax(ctx, np.array([toks[-1]], np.int32), len(prompt) + j, want_logits="last")
+                        toks.append(t)
+                        lgs.append(lg[0])
+                    ta.append(toks)
+                    la.append(np.array(lgs))
+                assert ta[0] == ta[1], mode
+                assert np.array_equal(la[0], la[1]), mode
+                if mode == "strict":
+                    for layer in (0, args["n_layers"] - 1):
+                        for rd in ("CacheK", "CacheV"):
+                            assert np.array_equal(getattr(a, rd)(layer).RawData[:len(prompt) + n],
+                                                  getattr(b, rd)(layer).RawData[:len(prompt) + n]), (layer, rd)
+            finally:
+                a.close(); b.close()
+    finally:
+        mx.Free()
+        if dw is not None:
+            dw.Free()

@@ -1,16 +1,20 @@
-"""MXFP8 against bf16 weights (DESIGN.md §9h) on the synthetic 8B model, both held on one GPU.
+"""MXFP8 (and MXFP4) against bf16 weights (DESIGN.md §9h, §9i) on the synthetic 8B model, all held on one GPU.
 
-The two models are built from the same synthetic weights, and every measurement alternates them, --rounds times each:
+The models of --formats (default bf16,mxfp8; the first is the reference) are built from the same synthetic weights, and
+every measurement alternates them, --rounds times each:
   decode      lnb_decode_run of 127 steps after the 8-token prompt, FAST and STRICT, device time (CUDA events); each
-              model on its default route (bf16 STRICT: the decode engine; MXFP8: the kernel chain)
+              model on its default route (bf16 STRICT: the decode engine; MXFP8, MXFP4: the kernel chain)
   batch8      FAST lnb_forward_batch over 8 sequences, 64 steps, host clock around the synchronised calls
   prefill     one FAST forward of S = 2048 tokens at position 0 (tensor-core route), host clock
   kernels     every projection alone (lnb_session_bench_kernel, FAST kernel chain): ms per launch and GB/s of the bytes the
               weight format streams
-  error       the MXFP8 model against the bf16 one over 128 teacher-forced tokens (the 8-token prompt and the bf16 model's
+  error       each model against the reference over 128 teacher-forced tokens (the 8-token prompt and the bf16 model's
               120 greedy tokens, one FAST forward): logits max-abs difference and argmax agreement.  Reported, not asserted.
-Prints the card name and power limit, read in the same run, then one JSON line per measurement.
-Usage: python tools/mxfp8_bench.py [--rounds 3] [--legs decode,batch8,prefill,kernels,error]
+              Synthetic weights say nothing about the quantization error of a trained checkpoint.
+Prints the card name and power limit, read in the same run, then one JSON line per measurement.  With two formats the
+ratio and overlap keys compare the second with the first; with more, ratio_median_<fmt> compares each with the first and
+overlap_<a>_<b> says whether two formats' samples overlap.
+Usage: python tools/mxfp8_bench.py [--rounds 3] [--formats bf16,mxfp8,mxfp4] [--legs decode,batch8,prefill,kernels,error]
 """
 import argparse
 import json
@@ -31,7 +35,10 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--legs", default="decode,batch8,prefill,kernels,error")
+    ap.add_argument("--formats", default="bf16,mxfp8")
     a = ap.parse_args()
+    fmts = a.formats.split(",")
+    ref = fmts[0]
     legs = set(a.legs.split(","))
     import numpy as np
     import torch
@@ -41,7 +48,7 @@ def main():
     print(json.dumps({"card": name, "power_limit": power}), flush=True)
     emit = lambda d: print(json.dumps(d), flush=True)   # noqa: E731
     models = {}
-    for fmt in ("bf16", "mxfp8"):
+    for fmt in fmts:
         t0 = time.perf_counter()
         models[fmt] = L.model.LoadSyntheticModel(dict(L.synth.LLAMA31_8B), weight_format=fmt)
         emit(dict(leg="load", weights=fmt, s=round(time.perf_counter() - t0, 1), **models[fmt].Transformer.weight_info()))
@@ -52,9 +59,9 @@ def main():
         return L.model.InferenceContext(models[fmt].Transformer, L.model.InferenceArgs(seq), acc_mode=acc, **kw)
 
     def alternate(measure):
-        vals = {"bf16": [], "mxfp8": []}
+        vals = {fmt: [] for fmt in fmts}
         for _ in range(a.rounds):
-            for fmt in ("bf16", "mxfp8"):
+            for fmt in fmts:
                 vals[fmt].append(measure(fmt))
         return vals
 
@@ -63,8 +70,16 @@ def main():
         for fmt, v in vals.items():
             out[fmt] = [round(x, 2) for x in v]
             out[fmt + "_median"] = round(statistics.median(v), 2)
-        out["ratio_median"] = round(out["mxfp8_median"] / out["bf16_median"], 3)
-        out["overlap"] = not (min(vals["mxfp8"]) > max(vals["bf16"]) or max(vals["mxfp8"]) < min(vals["bf16"]))
+        overlap = lambda x, y: not (min(vals[y]) > max(vals[x]) or max(vals[y]) < min(vals[x]))   # noqa: E731
+        if len(fmts) == 2:
+            out["ratio_median"] = round(out[fmts[1] + "_median"] / out[ref + "_median"], 3)
+            out["overlap"] = overlap(ref, fmts[1])
+        else:
+            for i, x in enumerate(fmts):
+                if i:
+                    out["ratio_median_" + x] = round(out[x + "_median"] / out[ref + "_median"], 3)
+                for y in fmts[i + 1:]:
+                    out[f"overlap_{x}_{y}"] = overlap(x, y)
         emit(out)
 
     if "decode" in legs:
@@ -143,8 +158,8 @@ def main():
 
     if "error" in legs:
         n = 128
-        c = ctx_of("bf16", n + 8, FAST)
-        first, _ = models["bf16"].Transformer.forward_argmax(c, prompt, 0)
+        c = ctx_of(ref, n + 8, FAST)
+        first, _ = models[ref].Transformer.forward_argmax(c, prompt, 0)
         gen, _, _ = c.decode_run(first, len(prompt), n - len(prompt) - 1, use_graph=False)
         c.close()
         seq = np.concatenate([prompt, [first], gen]).astype(np.int32)[:n]
@@ -153,10 +168,11 @@ def main():
             c = ctx_of(fmt, n + 1, FAST, max_rows=n)
             lg[fmt] = models[fmt].Transformer.forward_argmax(c, seq, 0, want_logits="all")[1]
             c.close()
-        d = np.abs(lg["bf16"] - lg["mxfp8"])
-        emit(dict(leg="error", tokens=n, logits_max_abs=float(d.max()), logits_mean_abs=float(d.mean()),
-                  argmax_agreement=float((lg["bf16"].argmax(1) == lg["mxfp8"].argmax(1)).mean()),
-                  bf16_logits_max_abs=float(np.abs(lg["bf16"]).max())))
+        for fmt in fmts[1:]:
+            d = np.abs(lg[ref] - lg[fmt])
+            emit(dict(leg="error", **({} if len(fmts) == 2 else {"weights": fmt}), tokens=n, logits_max_abs=float(d.max()),
+                      logits_mean_abs=float(d.mean()), argmax_agreement=float((lg[ref].argmax(1) == lg[fmt].argmax(1)).mean()),
+                      **{ref + "_logits_max_abs": float(np.abs(lg[ref]).max())}))
 
     for m in models.values():
         m.Free()
