@@ -13,6 +13,7 @@ import pytest
 from oracle_sampling import sample_ref as SR
 from tests import engine_shapes as ES
 from tests import model_shapes as MS
+from tests import mx_cases as MC
 from tests.helpers import host_tensors, oracle_model
 
 pytestmark = pytest.mark.gpu
@@ -46,9 +47,9 @@ def dequantized(args, tensors):
 class Pair:
     """an MXFP8 model and the bf16 model of its D(W), from one synthetic checkpoint"""
 
-    def __init__(self, L, args):
+    def __init__(self, L, args, tensors=None):
         self.args = args
-        self.tensors = host_tensors(args, SEED)
+        self.tensors = host_tensors(args, SEED) if tensors is None else tensors
         self.dw_tensors = dequantized(args, self.tensors)
         self.mx = L.model.LoadModelFromTensors(args, self.tensors, weight_format="mxfp8")
         self.dw = L.model.LoadModelFromTensors(args, self.dw_tensors)
@@ -84,6 +85,92 @@ def wide(L):
 def tail16(L):
     # ffn_dim % 32 == 16: w2's last block of every row is 16 wide; w1|w3 hold 33 blocks of 16 rows
     yield from _pair(L, dict(MS.CATALOGUE["one_layer"], ffn_dim=528))
+
+
+@pytest.fixture(scope="module")
+def tiny128_8k(L):
+    # prompts past one 128-row tile: the layer GEMMs span several M tiles, and the LM head runs in 2048-row slices
+    yield from _pair(L, dict(L.synth.TINY128, vocab_size=8192))
+
+
+def case_args(L, model):
+    """the shapes whose every linear matrix is built from tests/mx_cases.py"""
+    import torch
+    if model == "wide":
+        return ES.wide_args(torch.cuda.get_device_properties(0).multi_processor_count)
+    if model == "tail16":
+        return dict(MS.CATALOGUE["one_layer"], ffn_dim=528)
+    return dict(L.synth.TINY if model == "tiny" else L.synth.TINY128)
+
+
+def check_case_matrices(L, fmt, args):
+    """a model whose every linear matrix is built from the format's edge and tie blocks: the device quantizer's codes and
+    scales against the C statement.  No forward runs: these weights make no meaningful activations."""
+    tensors = host_tensors(args, SEED)
+    names = linear_names(args)
+    for i, name in enumerate(names):
+        tensors[name] = MC.matrix(fmt, *tensors[name].shape, shift=7 * i)
+    m = L.model.LoadModelFromTensors(args, tensors, weight_format=fmt)
+    try:
+        for name in names:
+            codes, scales = getattr(m.Transformer, f"{fmt}_read")(name)
+            want_c, want_s = (SR.mxfp8_quantize if fmt == "mxfp8" else SR.mxfp4_quantize)(tensors[name])
+            assert np.array_equal(scales, want_s), (name, np.argwhere(scales != want_s)[:4])
+            assert np.array_equal(codes, want_c), (name, np.argwhere(codes != want_c)[:4])
+    finally:
+        m.Free()
+
+
+def check_extreme_head(L, p):
+    """the MX and D(W) models of mx_cases.extreme_head, bit for bit: host-driven decode steps (the 1-row LM-head configs),
+    a ragged call of 8 segments and batched steps of 2 and 8 rows, and a 40-row prompt whose FAST LM head runs as
+    dequantized tensor-core slices; STRICT prompt logits also against the oracle of D(W)"""
+    om = oracle_model(p.args, p.dw_tensors)
+    try:
+        toks = np.random.default_rng(5).integers(0, p.args["vocab_size"], 40).astype(np.int32)
+        for mode in ("strict", "fast"):
+            acc = _acc(L, mode)
+            a, b = _ctx(L, p.mx, 64, acc), _ctx(L, p.dw, 64, acc, engine=False)
+            try:
+                ta, la = _steps(p.mx, a, 6)
+                tb, lb = _steps(p.dw, b, 6)
+                assert ta == tb and np.array_equal(la, lb), mode
+                assert np.isfinite(la).all() and (np.abs(la[:, 0::MC.HEAD_CLASSES]) > 2.0 ** 90).mean() > 0.9, mode
+            finally:
+                a.close(); b.close()
+            res = []
+            for m in (p.mx, p.dw):
+                ctx = _ctx(L, m, 64, acc, n_seq=8, max_rows=40, engine=False if m is p.dw else None)
+                try:
+                    n1, l1 = ctx.forward_ragged([(s, 0, PROMPT[:2 + s % 6]) for s in range(8)], want_logits=True)
+                    n2, l2 = ctx.forward_batch([int(t) for t in n1[:2]], [2, 3], want_logits=True)
+                    n3, l3 = ctx.forward_batch([int(t) for t in n1], [2 + s % 6 + (s < 2) for s in range(8)], want_logits=True)
+                    res.append((n1, l1, n2, l2, n3, l3))
+                finally:
+                    ctx.close()
+            for i, (x, y) in enumerate(zip(*res)):
+                assert np.array_equal(np.asarray(x), np.asarray(y)), (mode, i)
+            a, b = _ctx(L, p.mx, 64, acc, max_rows=40), _ctx(L, p.dw, 64, acc, max_rows=40, engine=False)
+            try:
+                la0, lb0 = a.launch_count(), b.launch_count()
+                ga = p.mx.Transformer.forward_argmax(a, toks, 0, want_logits="all")
+                gb = p.dw.Transformer.forward_argmax(b, toks, 0, want_logits="all")
+                assert ga[0] == gb[0] and np.array_equal(ga[1], gb[1]), mode
+                assert np.isfinite(ga[1]).all()
+                extra = _tc_extra(p.args, 40, mode == "strict", 40)
+                assert (a.launch_count() - la0) - (b.launch_count() - lb0) == extra, mode
+                if mode == "fast":
+                    assert extra - 4 * p.args["n_layers"] == 2 * (p.args["vocab_size"] // 2048) - 1, "the LM head did not run in slices"
+                else:
+                    os_ = om.new_session(64)
+                    try:
+                        assert np.array_equal(os_.forward(toks, 0), ga[1])
+                    finally:
+                        os_.close()
+            finally:
+                a.close(); b.close()
+    finally:
+        om.close()
 
 
 def _acc(L, mode):
@@ -126,6 +213,21 @@ def test_quantizer_equals_the_c_statement(L, request, model):
         assert np.array_equal(codes, want_c), name
 
 
+@pytest.mark.parametrize("model", ["tiny", "tiny128", "wide", "tail16"])
+def test_quantizer_on_edge_and_tie_matrices(L, model):
+    check_case_matrices(L, "mxfp8", case_args(L, model))
+
+
+@pytest.mark.parametrize("vocab", [4096, 8192, 16384])
+def test_decoders_at_extreme_scales_through_the_lm_head(L, vocab):
+    args = dict(L.synth.TINY128, vocab_size=vocab)
+    p = Pair(L, args, MC.extreme_head("mxfp8", host_tensors(args, SEED)))
+    try:
+        check_extreme_head(L, p)
+    finally:
+        p.close()
+
+
 @pytest.mark.parametrize("name,row,col,bits", [("layers.1.feed_forward.w3.weight", 5, 17, 0x7F80),
                                                ("layers.0.attention.wk.weight", 40, 3, 0xFFC0),
                                                ("output.weight", 1000, 255, 0xFF80)])
@@ -147,58 +249,77 @@ def test_non_finite_weight_fails_finalize_with_its_index(L, name, row, col, bits
 
 # ---- identity: prompts ----------------------------------------------------------------------------------------------------
 def _tc_extra(args, S, strict, max_rows):
-    """the launches an MXFP8 prompt adds on the tensor-core route: one dequantization per GEMM"""
+    """the launches an MX prompt adds on the tensor-core route: one dequantization per GEMM, and an LM head in n row slices
+    runs n dequantizations and n GEMMs where the bf16 model runs one GEMM"""
     if not MS.forward_tc(args, S, strict, max_rows):
         return 0
     w = MS.widths(args)
     d, q, kv, f, v = args["dim"], w["q_l"], w["kv_l"], w["ffn_l"], w["vocab_l"]
     elems = max((q + 2 * kv) * d, d * q, 2 * f * d, d * f, 128 * d)
     slice_rows = min(v, elems // d // 128 * 128)
-    head = -(-v // slice_rows) if v % 128 == 0 and S > 1 else 0
-    return 4 * args["n_layers"] + head
+    slices = -(-v // slice_rows) if v % 128 == 0 and S > 1 else 0
+    return 4 * args["n_layers"] + max(2 * slices - 1, 0)
 
 
-@pytest.mark.parametrize("model", ["tiny", "tiny128", "wide", "tail16"])
+@pytest.mark.parametrize("model", ["tiny", "tiny128", "wide", "tail16", "tiny128_8k"])
 @pytest.mark.parametrize("mode", ["strict", "fast"])
 def test_prompt_logits_and_caches(L, request, model, mode):
     p = request.getfixturevalue(model)
-    acc, seq = _acc(L, mode), 64
+    # tiny128_8k: prompts past one 128-row tile (S = 129: two M tiles in the layer GEMMs, one full tile in the LM head;
+    # 130 and 300: an LM head of 129 and 299 rows, two and three tiles, in 2048-row slices), each followed by decode steps
+    sizes, rows = ((129, 130, 300), 300) if model == "tiny128_8k" else ((1, 7, 40), 40)
+    acc, seq = _acc(L, mode), max(64, rows + 8)
     rng = np.random.default_rng(3)
-    for S in (1, 7, 40):
+    for S in sizes:
         toks = rng.integers(0, p.args["vocab_size"], S).astype(np.int32)
         # the bf16 session on the kernel chain too, so that launch counts compare (the engine's bits are the chain's)
-        a, b = _ctx(L, p.mx, seq, acc, max_rows=40), _ctx(L, p.dw, seq, acc, max_rows=40, engine=False)
+        a, b = _ctx(L, p.mx, seq, acc, max_rows=rows), _ctx(L, p.dw, seq, acc, max_rows=rows, engine=False)
         try:
             la, lb = a.launch_count(), b.launch_count()
             ga = p.mx.Transformer.Forward(a, L.ml.Tensor(toks, L.ml.DT_INT32), 0).RawData
             gb = p.dw.Transformer.Forward(b, L.ml.Tensor(toks, L.ml.DT_INT32), 0).RawData
             assert np.array_equal(ga, gb), (S, np.abs(ga - gb).max())
             _caches_equal(p.args, a, b, S)
-            extra = _tc_extra(p.args, S, mode == "strict", 40)
+            extra = _tc_extra(p.args, S, mode == "strict", rows)
             assert (a.launch_count() - la) - (b.launch_count() - lb) == extra, S
-            if model == "tiny128" and mode == "fast" and S == 40:
+            if model.startswith("tiny128") and mode == "fast" and S >= 40:
                 assert extra > 0, "the tensor-core route was not taken"
+            if model == "tiny128_8k":
+                t = int(np.argmax(ga[-1]))
+                for j in range(3):
+                    ta, da = p.mx.Transformer.forward_argmax(a, np.array([t], np.int32), S + j, want_logits="last")
+                    tb, db = p.dw.Transformer.forward_argmax(b, np.array([t], np.int32), S + j, want_logits="last")
+                    assert ta == tb and np.array_equal(da, db), (S, j)
+                    t = ta
+                _caches_equal(p.args, a, b, S + 3)
         finally:
             a.close(); b.close()
 
 
 def test_chunked_prefill(L, tiny128):
+    """the second plan's last chunk runs 263 rows from position 37: its GEMMs and its sliced LM head cross the 128-row tile
+    edges at an offset.  Each plan ends with a decode step."""
     p = tiny128
-    for mode in ("strict", "fast"):
-        a, b = _ctx(L, p.mx, 64, _acc(L, mode), max_rows=40), _ctx(L, p.dw, 64, _acc(L, mode), max_rows=40)
-        try:
-            out = []
-            for ctx, m in ((a, p.mx), (b, p.dw)):
-                ctx.allow_chunked_prefill()
-                toks = np.arange(3, 3 + 45, dtype=np.int32)
-                lg = []
-                for s0, s1 in ((0, 5), (5, 38), (38, 45)):
-                    lg.append(m.Transformer.Forward(ctx, L.ml.Tensor(toks[s0:s1], L.ml.DT_INT32), s0).RawData)
-                out.append(np.concatenate(lg))
-            assert np.array_equal(out[0], out[1]), mode
-            _caches_equal(p.args, a, b, 45)
-        finally:
-            a.close(); b.close()
+    for chunks in (((0, 5), (5, 38), (38, 45)), ((0, 5), (5, 37), (37, 300))):
+        end, rows = chunks[-1][1], max(s1 - s0 for s0, s1 in chunks)
+        for mode in ("strict", "fast"):
+            a, b = _ctx(L, p.mx, end + 8, _acc(L, mode), max_rows=rows), _ctx(L, p.dw, end + 8, _acc(L, mode), max_rows=rows)
+            try:
+                out = []
+                for ctx, m in ((a, p.mx), (b, p.dw)):
+                    ctx.allow_chunked_prefill()
+                    toks = np.arange(3, 3 + end, dtype=np.int32)
+                    lg = []
+                    for s0, s1 in chunks:
+                        lg.append(m.Transformer.Forward(ctx, L.ml.Tensor(toks[s0:s1], L.ml.DT_INT32), s0).RawData)
+                    nxt = np.array([int(np.argmax(lg[-1][-1]))], np.int32)
+                    t, d = m.Transformer.forward_argmax(ctx, nxt, end, want_logits="last")
+                    out.append((np.concatenate(lg), t, d))
+                assert np.array_equal(out[0][0], out[1][0]), (chunks, mode)
+                assert out[0][1] == out[1][1] and np.array_equal(out[0][2], out[1][2]), (chunks, mode)
+                _caches_equal(p.args, a, b, end + 1)
+            finally:
+                a.close(); b.close()
 
 
 # ---- identity: decode ---------------------------------------------------------------------------------------------------
@@ -476,7 +597,7 @@ def test_weight_format_errors_and_weight_info(L, tiny128):
 def test_8b_mxfp8_equals_its_dequantized_model(L):
     """synthetic 8B: the LM head's and layer 0's codes against the C statement; then an MXFP8 model against the bf16 model of
     its D(W), built tensor by tensor from the library's own codes (both fit in 80 GB): FAST 8-token prompt and 32 decode
-    steps, STRICT 8 + 10 with the first and last layer's caches"""
+    steps, STRICT 8 + 10 with the first and last layer's caches, and a FAST 2048-token prompt"""
     args = dict(L.synth.LLAMA31_8B)
     mx = L.model.LoadSyntheticModel(args, weight_format="mxfp8")
     dw = None
@@ -519,6 +640,20 @@ def test_8b_mxfp8_equals_its_dequantized_model(L):
                                                   getattr(b, rd)(layer).RawData[:len(prompt) + n]), (layer, rd)
             finally:
                 a.close(); b.close()
+        # the benchmark's prefill2048 workload: a FAST prompt of 2048 tokens on the tensor cores, every layer GEMM over 16 M
+        # tiles of the dequantized scratch; its last row, and the first and last layer's caches at every position
+        S = 2048
+        toks = np.random.default_rng(0).integers(0, 128000, size=S).astype(np.int32)
+        a, b = _ctx(L, mx, S, _acc(L, "fast"), max_rows=S), _ctx(L, dw, S, _acc(L, "fast"), max_rows=S, engine=False)
+        try:
+            ta, lga = mx.Transformer.forward_argmax(a, toks, 0, want_logits="last")
+            tb, lgb = dw.Transformer.forward_argmax(b, toks, 0, want_logits="last")
+            assert ta == tb and np.array_equal(lga, lgb), "prefill2048"
+            for layer in (0, args["n_layers"] - 1):
+                for rd in ("CacheK", "CacheV"):
+                    assert np.array_equal(getattr(a, rd)(layer).RawData[:S], getattr(b, rd)(layer).RawData[:S]), (layer, rd)
+        finally:
+            a.close(); b.close()
     finally:
         mx.Free()
         if dw is not None:

@@ -10,8 +10,9 @@ The intervals are single values on a large share of elements at these widths (th
 widths they are several ulps wide and the checks would say little, so they run on the small shapes.
 
 Routes: the FAST tensor-core prompt path (enqueue_forward_tc) on TINY, TINY128 and every catalogue shape whose prompts
-take it, an MXFP8 prompt whose LM head runs in row slices, and the batch engine's tensor-core form (LNB_BATCH_TC=1).  The
-probes themselves are first checked bit for bit on the STRICT routes, where every stage can be recomputed exactly."""
+take it, MXFP8 and MXFP4 prompts whose LM head runs in row slices, and the batch engine's tensor-core form
+(LNB_BATCH_TC=1).  The probes themselves are first checked bit for bit on the STRICT routes, where every stage can be
+recomputed exactly."""
 import time
 
 import numpy as np
@@ -82,10 +83,13 @@ class Model:
         self.gm = L.model.LoadModelFromTensors(args, self.tensors, weight_format=weight_format)
         self.cis = O.rope_table(args["head_dim"], args["max_seq_len"], args["rope_theta"], bool(args["use_scaled_rope"]))[1]
         self.silu = O.silu_table_bf16()
-        # the weights the stages read: D(W) for an MXFP8 model (the bf16 model of its dequantized weights)
+        # the weights the stages read: D(W) for an MXFP8 or MXFP4 model (the bf16 model of its dequantized weights)
         self.w = self.tensors
         if weight_format == "mxfp8":
             from tests.test_gpu_mxfp8 import dequantized
+            self.w = dequantized(args, self.tensors)
+        elif weight_format == "mxfp4":
+            from tests.test_gpu_mxfp4 import dequantized
             self.w = dequantized(args, self.tensors)
 
     def lw(self, l, name):
@@ -348,21 +352,32 @@ def test_tensor_core_prompt_stage_by_stage(L, sms, name, S, start):
     _prefill_stages(L, m, S, start, "prefill")
 
 
-def test_mxfp8_prompt_with_a_sliced_lm_head_stage_by_stage(L, sms):
-    """an MXFP8 FAST prompt of 40 rows whose LM head is dequantized and run in row slices (TINY128 with a vocabulary of
-    8192: the largest layer matrix, w1|w3, holds 2048 rows of dim; `wide` slices too, but its FFN is off the 128-wide tiles,
-    so its prompts stay on the kernel chain): every stage against D(W), the bf16 values of the dequantized weights"""
+def _sliced_head_prompt(L, sms, fmt, S):
     a = dict(_shape("tiny128", sms), vocab_size=8192)
-    dim, S = a["dim"], 40
+    dim = a["dim"]
     assert forward_tc(a, S, False, S)
     w_elems = max([(a["n_heads"] + 2 * a["n_kv_heads"]) * a["head_dim"] * dim, dim * a["n_heads"] * a["head_dim"],
                    2 * a["ffn_dim"] * dim, dim * a["ffn_dim"], 128 * dim])
     assert a["vocab_size"] > w_elems // dim, "the LM head must run in row slices"
-    m = Model(L, a, weight_format="mxfp8")
+    m = Model(L, a, weight_format=fmt)
     try:
-        _prefill_stages(L, m, S, 0, "mxfp8 prefill")
+        _prefill_stages(L, m, S, 0, f"{fmt} prefill")
     finally:
         m.close()
+
+
+def test_mxfp8_prompt_with_a_sliced_lm_head_stage_by_stage(L, sms):
+    """an MXFP8 FAST prompt of 40 rows whose LM head is dequantized and run in row slices (TINY128 with a vocabulary of
+    8192: the largest layer matrix, w1|w3, holds 2048 rows of dim; `wide` slices too, but its FFN is off the 128-wide tiles,
+    so its prompts stay on the kernel chain): every stage against D(W), the bf16 values of the dequantized weights"""
+    _sliced_head_prompt(L, sms, "mxfp8", 40)
+
+
+@pytest.mark.parametrize("fmt,S", [("mxfp8", 300), ("mxfp4", 40), ("mxfp4", 300)])
+def test_mx_prompt_with_a_sliced_lm_head_stage_by_stage(L, sms, fmt, S):
+    """the test above for MXFP4, and for prompts of 300 rows: three M tiles in every GEMM over the dequantized scratch,
+    and a sliced LM head of 299 rows"""
+    _sliced_head_prompt(L, sms, fmt, S)
 
 
 # ---- 3. the batch engine's tensor-core form ------------------------------------------------------------------------------------

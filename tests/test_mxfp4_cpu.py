@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from oracle_sampling import sample_ref as SR
+from tests import mx_cases as MC
 
 MIDS4 = (1, 3, 5, 7, 10, 14, 20)     # 4 x the midpoints 0.25, 0.75, 1.25, 1.75, 2.5, 3.5, 5 of the E2M1 grid
 
@@ -63,10 +64,7 @@ def restate_dequant(code: int, X: int) -> int:
     return sign | ((e - 1 + X + 127) << 7) | (m << 6)
 
 
-def bf16(x: float) -> int:
-    b = int(np.array([x], np.float32).view(np.uint32)[0])
-    assert b & 0xFFFF == 0, x
-    return b >> 16
+bf16 = MC.bf16
 
 
 def bf16_matrix(rng, rows, cols, scale=1.0):
@@ -96,20 +94,16 @@ def test_random_blocks_match_restatement(cols):
 def test_scale_on_both_sides_of_f_64(e):
     for f, dx in ((63, 2), (64, 2), (65, 1), (127, 1), (0, 2)):
         amax = (1 + f / 128) * 2.0 ** e
-        w = np.array([[bf16(amax)] + [bf16(amax / 4)] * 31], np.uint16)
+        w = np.array([MC.mxfp4_f64_row(e, f)], np.uint16)
         codes, scales = _check(w)
         assert int(scales[0, 0]) - 127 == e - dx, (e, f)
         assert amax <= 6.0 * 2.0 ** (e - dx) < 2 * amax  # the smallest X that does not clip the block maximum
 
 
 def test_every_tie_rounds_to_the_even_code():
-    ties = {0.25: 0, 0.75: 2, 1.25: 2, 1.75: 4, 2.5: 4, 3.5: 6, 5.0: 6}
-    for X in (-100, -6, -1, 0, 3, 90):
-        row = [bf16(6.0 * 2.0 ** X)]                    # amax = 6 * 2^X: f = 64, so X = e - 2 exactly
-        for t in ties:
-            row += [bf16(t * 2.0 ** X), bf16(-t * 2.0 ** X)]
-        row += [0] * (32 - len(row))
-        w = np.array([row], np.uint16)
+    ties = MC.TIES4
+    for X in MC.TIE4_X:
+        w = np.array([MC.mxfp4_tie_row(X)], np.uint16)  # amax = 6 * 2^X: f = 64, so X = e - 2 exactly
         codes, scales = _check(w)
         assert int(scales[0, 0]) - 127 == X
         nib = [(codes[0, c // 2] >> (4 * (c & 1))) & 15 for c in range(32)]
@@ -119,7 +113,7 @@ def test_every_tie_rounds_to_the_even_code():
 
 
 def test_upper_clamp_saturates_to_six():
-    w = np.array([[0x7F7F, 0xFF7F, 0x7F00, 0x7E00] + [0x3F80] * 28], np.uint16)   # +-max bf16, 2^127, 2^125
+    w = np.array([MC.mxfp4_upper_clamp_row()], np.uint16)   # +-max bf16, 2^127, 2^125
     codes, scales = _check(w)
     assert int(scales[0, 0]) - 127 == 125
     assert codes[0, 0] == 0xF7                          # +6 (low nibble), -6 (high nibble)
@@ -127,15 +121,19 @@ def test_upper_clamp_saturates_to_six():
 
 
 def test_lower_clamp_subnormal_zero_and_negative_zero():
-    tiny = [0x0080, 0x8100, 0x00C0] + [0x0080] * 29      # amax 2^-125 (E = 2): X = -127 -> -125
-    sub = [0x0040, 0x8001, 0x0020, 0x0000] + [0x0001] * 28   # subnormal amax: -125
-    zero = [0x0000, 0x8000] * 16                        # zero block with -0
-    neg = [0x8000 | bf16(0.125)] + [bf16(4.0)] * 31       # a negative weight that rounds to 0 keeps its sign
-    w = np.array([tiny, sub, zero, neg], np.uint16)
+    # amax 2^-125 (E = 2): X = -127 -> -125; a subnormal amax: -125; a zero block with -0; a negative weight that rounds
+    # to 0 keeps its sign
+    w = np.array(MC.mxfp4_lower_rows(), np.uint16)
     codes, scales = _check(w)
     assert list(scales[:3, 0].astype(int) - 127) == [-125, -125, -125]
     assert codes[2, 0] == 0x80                          # +0, -0
     assert codes[3, 0] & 15 == 0x8
+
+
+@pytest.mark.parametrize("cols", [208, 256])
+def test_case_blocks_match_restatement(cols):
+    _check(MC.matrix("mxfp4", 48, cols, shift=5))
+    _check(np.vstack(MC.mxfp4_extreme_blocks()))
 
 
 def test_non_finite_weights_are_refused():

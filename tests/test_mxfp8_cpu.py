@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 
 from oracle_sampling import sample_ref as SR
+from tests import mx_cases as MC
 
 
 # ---- the integer restatement -----------------------------------------------------------------------------------------
@@ -84,45 +85,16 @@ def _random_rows(rng, rows, cols):
     return np.where(rng.random((rows, 1)) < 0.5, w, narrow).astype(np.uint16)
 
 
-def _tie_rows():
-    # X = 0 (256 is the block maximum): the midpoints between neighbouring codes of every binade, and of the subnormals
-    vals = []
-    for e in range(-6, 9):
-        for n in range(8, 15 if e == 8 else 16):
-            vals.append((n + 0.5) * 2.0 ** (e - 3))
-    vals += [(n + 0.5) * 2.0 ** -9 for n in range(0, 8)]
-    vals = [v for v in vals if v < 448]
-    rows = []
-    for i in range(0, len(vals), 31):
-        chunk = vals[i:i + 31]
-        row = [256.0] + chunk + [0.0] * (31 - len(chunk))
-        rows.append(row)
-        rows.append([-v for v in row])
-    return _bf16(np.array(rows, np.float32))
-
-
-def _edge_rows():
-    f = lambda xs: list(_bf16(np.array(xs, np.float32)))   # noqa: E731
-    sat = f([511.0, 448.0, 449.0, 455.0, 456.0, 460.0, 464.0, 472.0, 480.0, 500.0, 447.0, 440.0, 432.0, 416.0, 444.0, 452.0])
-    sat += [x | 0x8000 for x in sat]
-    small = f([1.0] + [2.0 ** -k for k in range(6, 17)] + [3 * 2.0 ** -12, 5 * 2.0 ** -13, 7 * 2.0 ** -12, 2.0 ** -15 * 1.5] +
-              [9 * 2.0 ** -13, 1.0 / 3, 0.1, 2.0 ** -14 * 1.75] + [0.0] * 12)
-    clamp = [0x0001, 0x0002, 0x007F, 0x0080, 0x0081, 0x00FF, 0x0100, 0x0180, 0x0200, 0x0280, 0x0300, 0x0301,
-             0x8001, 0x807F, 0x8080, 0x8300] + [0x0000] * 14 + [0x0380, 0x03FF]     # amax < 2^-109: X = -117
-    big = [0x7F7F, 0xFF7F, 0x7F00, 0x7E80, 0x3F80, 0x0001, 0x8001, 0x0080] + [0x7F7F - i for i in range(24)]
-    zero = [0x0000] * 32
-    negz = [0x8000] * 16 + [0x0000] * 16
-    return np.array([sat, small, clamp, big, zero, negz], np.uint16)
-
-
 def _cases():
     rng = np.random.default_rng(9)
     return {
         "random": _random_rows(rng, 24, 96),
         "random_tail16": _random_rows(rng, 16, 80),      # cols % 32 == 16: a 16-wide last block
-        "ties": _tie_rows(),
-        "edges": _edge_rows(),
-        "edges_tail16": np.ascontiguousarray(_edge_rows()[:, :48]),
+        "ties": MC.mxfp8_tie_rows(),
+        "edges": MC.mxfp8_edge_rows(),
+        "edges_tail16": np.ascontiguousarray(MC.mxfp8_edge_rows()[:, :48]),
+        "extremes": np.vstack(MC.mxfp8_extreme_blocks()),
+        "case_matrix_tail16": MC.matrix("mxfp8", 40, 208, shift=3),
     }
 
 
@@ -142,7 +114,7 @@ def test_c_statement_matches_integer_restatement(name):
 
 
 def test_edge_cases_cover_what_they_claim():
-    codes, scales = SR.mxfp8_quantize(_edge_rows())
+    codes, scales = SR.mxfp8_quantize(MC.mxfp8_edge_rows())
     X = scales.astype(int) - 127
     assert (codes[0] & 0x7F == 0x7E).sum() >= 20                     # saturation to 448
     assert ((codes[1] & 0x7F) < 8).sum() > 10 and (codes[1] & 0x7F == 0).sum() > 0   # E4M3 subnormals and underflow
@@ -150,7 +122,7 @@ def test_edge_cases_cover_what_they_claim():
     assert X[3, 0] == 119                                            # the largest finite bf16
     assert (codes[4] == 0).all() and X[4, 0] == -117                 # zero block
     assert (codes[5, :16] == 0x80).all()                             # -0 stays -0
-    tc, _ = SR.mxfp8_quantize(_tie_rows())
+    tc, _ = SR.mxfp8_quantize(MC.mxfp8_tie_rows())
     assert ((tc[:, 1:] & 1) == 0).all()                              # every midpoint went to the even neighbour
     assert len(set((tc & 0x7F).ravel().tolist())) > 50               # ... over the whole code space
 
@@ -198,7 +170,7 @@ def test_non_finite_weights_are_refused(bad):
 
 
 def test_broken_rules_are_caught():
-    ties, edges = _tie_rows(), _edge_rows()
+    ties, edges = MC.mxfp8_tie_rows(), MC.mxfp8_edge_rows()
     c, _ = SR.mxfp8_quantize(ties)
     bc, _ = restate_quantize(ties, half_up=True)
     assert not np.array_equal(c, bc)
