@@ -123,11 +123,39 @@ extern "C" int lnb_nccl_unique_id(void* out128) {
 
 // ------------------------------------------------------------------------------------------
 // model
+// The STRICT decode engine's packed copy of a matrix (wpack.cuh), built by the first STRICT engine session (ensure_wpack).
+// Sessions need a finalized model and a finalized model takes no more weights, so a packed copy can never fall behind the
+// bf16 matrix it was built from.
+struct WPack {
+  uint8_t* data = nullptr;
+  uint8_t* units = nullptr;
+  int kt = 0;
+  int64_t read_bytes = 0;        // bytes the engine reads per pass (packed units, raw units, unit table)
+  int64_t packed_units = 0, n_units = 0;
+};
+// One linear matrix of this rank's shard, N x K in the device layout (8-row panels): bf16 panels, or after an MX finalize
+// its codes (mxfp8.cuh, mxfp4.cuh) and their scales.  Every helper that knows how the format lays out bytes is here.
+struct Linear {
+  void* w = nullptr;             // bf16 panels or MX codes
+  uint8_t* s = nullptr;          // MX scales; NULL for bf16
+  int fmt = LNB_WEIGHTS_BF16;
+  int N = 0, K = 0;
+  WPack pack;                    // w1|w3 and the LM head only
+  size_t code_bytes() const {
+    return fmt == LNB_WEIGHTS_MXFP4 ? (size_t)N * K / 2 : fmt == LNB_WEIGHTS_MXFP8 ? (size_t)N * K : (size_t)N * K * 2;
+  }
+  size_t scale_bytes() const { return fmt == LNB_WEIGHTS_BF16 ? 0 : (size_t)(N / 8) * mx_nbp(K) * 8; }
+  size_t bytes() const { return code_bytes() + scale_bytes(); }
+  Linear rows(int n0, int n) const {   // rows [n0, n0 + n), n0 a multiple of 8 (whole panels), without the packed copy
+    const Linear head{w, s, fmt, n0, K};
+    return {static_cast<uint8_t*>(w) + head.code_bytes(), s ? s + head.scale_bytes() : nullptr, fmt, n, K};
+  }
+  uint16_t* bf16() const { return fmt == LNB_WEIGHTS_BF16 ? static_cast<uint16_t*>(w) : nullptr; }
+  uint8_t* codes() const { return fmt == LNB_WEIGHTS_BF16 ? nullptr : static_cast<uint8_t*>(w); }
+};
 struct LayerW {
-  // the four projection matrices: bf16 panels, or after an MXFP8 finalize their E4M3 codes (mxfp8.cuh), whose scales are
-  // then in sqkv / so / s13 / s2 (NULL for bf16)
-  uint16_t *attn_norm = nullptr, *wqkv = nullptr, *wo = nullptr, *ffn_norm = nullptr, *w13 = nullptr, *w2 = nullptr;
-  uint8_t *sqkv = nullptr, *so = nullptr, *s13 = nullptr, *s2 = nullptr;
+  uint16_t *attn_norm = nullptr, *ffn_norm = nullptr;
+  Linear qkv, o, w13, w2;        // the stacked wq|wk|wv, wo, the interleaved w1|w3, w2
   unsigned have = 0;  // bit per checkpoint tensor (9)
 };
 enum { T_ATTN_NORM = 0, T_WQ, T_WK, T_WV, T_WO, T_FFN_NORM, T_W1, T_W2, T_W3, T_EMBD, T_NORM, T_OUTPUT };
@@ -136,9 +164,9 @@ struct lnb_model {
   lnb_model_args a;
   int device = 0, tp_rank = 0, tp_size = 1;
   int q_dim = 0, kv_dim = 0, q_l = 0, kv_l = 0, ffn_l = 0, vocab_l = 0;
-  uint16_t *tok_embd = nullptr, *norm = nullptr, *output = nullptr;
-  uint8_t* output_s = nullptr;     // MXFP8 scales of the LM head (output then holds its codes)
-  int wfmt = LNB_WEIGHTS_BF16;     // lnb_model_set_weight_format; the linear weights are in this format once finalized
+  uint16_t *tok_embd = nullptr, *norm = nullptr;
+  Linear output;                   // the LM head
+  int wfmt = LNB_WEIGHTS_BF16;     // lnb_model_set_weight_format: lnb_model_finalize quantizes the linear weights to it
   bool have_embd = false, have_norm = false, have_output = false, finalized = false;
   std::vector<LayerW> layers;
   float* cis = nullptr;
@@ -149,19 +177,7 @@ struct lnb_model {
   void* staging = nullptr;
   size_t staging_bytes = 0;
   int sm_count = 132;
-  // the STRICT decode engine's packed copies of w1|w3 (per layer) and the LM head (wpack.cuh), built by the first STRICT
-  // engine session (ensure_wpack).  Sessions need a finalized model and a finalized model takes no more weights, so a
-  // packed copy can never fall behind the bf16 matrix it was built from.
-  struct WPack {
-    uint8_t* data = nullptr;
-    uint8_t* units = nullptr;
-    int kt = 0;
-    int64_t read_bytes = 0;        // bytes the engine reads per pass (packed units, raw units, unit table)
-    int64_t packed_units = 0, n_units = 0;
-  };
-  std::vector<WPack> wp_w13;
-  WPack wp_out;
-  void* wpack_mem = nullptr;
+  void* wpack_mem = nullptr;       // the packed copies of every layer's w13 and of the LM head (ensure_wpack)
   int wpack_state = 0;             // 0 = not built, 1 = built, -1 = the engine streams bf16 (wpack_why says why)
   std::string wpack_why;
   std::mutex wpack_mu;
@@ -200,7 +216,8 @@ static void full_shape(const lnb_model* m, int kind, int64_t* rows, int64_t* col
 
 // where a checkpoint tensor lands in the HBM layout of this rank
 struct Placement {
-  uint16_t* dst;
+  uint16_t* dst;       // where upload writes: the bf16 tensor, or the bf16 panels of lin
+  Linear* lin;         // the linear matrix the tensor is part of (NULL for the embedding and the norms)
   int64_t row0, col0;  // window of the full tensor owned by this rank
   int rows, cols;      // window size
   bool panel_major;
@@ -219,16 +236,36 @@ static Placement placement(lnb_model* m, int kind, int layer) {
     case T_FFN_NORM: p.dst = L->ffn_norm; p.rows = 1; p.cols = a.dim; p.panel_major = false; break;
     case T_NORM: p.dst = m->norm; p.rows = 1; p.cols = a.dim; p.panel_major = false; break;
     case T_EMBD: p.dst = m->tok_embd; p.rows = a.vocab_size; p.cols = a.dim; p.panel_major = false; break;
-    case T_WQ: p.dst = L->wqkv; p.row0 = (int64_t)r * m->q_l; p.rows = m->q_l; p.cols = a.dim; break;
-    case T_WK: p.dst = L->wqkv; p.row0 = (int64_t)r * m->kv_l; p.rows = m->kv_l; p.cols = a.dim; p.dpanel0 = m->q_l / 8; break;
-    case T_WV: p.dst = L->wqkv; p.row0 = (int64_t)r * m->kv_l; p.rows = m->kv_l; p.cols = a.dim; p.dpanel0 = (m->q_l + m->kv_l) / 8; break;
-    case T_WO: p.dst = L->wo; p.col0 = (int64_t)r * m->q_l; p.rows = a.dim; p.cols = m->q_l; break;
-    case T_W1: p.dst = L->w13; p.row0 = (int64_t)r * m->ffn_l; p.rows = m->ffn_l; p.cols = a.dim; p.dpanel0 = 0; p.dpanel_stride = 2; break;
-    case T_W3: p.dst = L->w13; p.row0 = (int64_t)r * m->ffn_l; p.rows = m->ffn_l; p.cols = a.dim; p.dpanel0 = 2; p.dpanel_stride = 2; break;
-    case T_W2: p.dst = L->w2; p.col0 = (int64_t)r * m->ffn_l; p.rows = a.dim; p.cols = m->ffn_l; break;
-    case T_OUTPUT: p.dst = m->output; p.row0 = (int64_t)r * m->vocab_l; p.rows = m->vocab_l; p.cols = a.dim; break;
+    case T_WQ: p.lin = &L->qkv; p.row0 = (int64_t)r * m->q_l; p.rows = m->q_l; p.cols = a.dim; break;
+    case T_WK: p.lin = &L->qkv; p.row0 = (int64_t)r * m->kv_l; p.rows = m->kv_l; p.cols = a.dim; p.dpanel0 = m->q_l / 8; break;
+    case T_WV: p.lin = &L->qkv; p.row0 = (int64_t)r * m->kv_l; p.rows = m->kv_l; p.cols = a.dim; p.dpanel0 = (m->q_l + m->kv_l) / 8; break;
+    case T_WO: p.lin = &L->o; p.col0 = (int64_t)r * m->q_l; p.rows = a.dim; p.cols = m->q_l; break;
+    case T_W1: p.lin = &L->w13; p.row0 = (int64_t)r * m->ffn_l; p.rows = m->ffn_l; p.cols = a.dim; p.dpanel0 = 0; p.dpanel_stride = 2; break;
+    case T_W3: p.lin = &L->w13; p.row0 = (int64_t)r * m->ffn_l; p.rows = m->ffn_l; p.cols = a.dim; p.dpanel0 = 2; p.dpanel_stride = 2; break;
+    case T_W2: p.lin = &L->w2; p.col0 = (int64_t)r * m->ffn_l; p.rows = a.dim; p.cols = m->ffn_l; break;
+    case T_OUTPUT: p.lin = &m->output; p.row0 = (int64_t)r * m->vocab_l; p.rows = m->vocab_l; p.cols = a.dim; break;
   }
+  if (p.lin) p.dst = p.lin->bf16();
   return p;
+}
+
+// one linear matrix of the device layout, with the layer and the checkpoint tensor kind it comes from
+struct LinMat {
+  Linear* lin;
+  int layer;   // -1: the LM head
+  int kind;    // T_WQ (the stacked wq|wk|wv), T_WO, T_W1 (the interleaved w1|w3), T_W2, T_OUTPUT
+};
+static std::vector<LinMat> linear_mats(lnb_model* m) {
+  std::vector<LinMat> v;
+  for (int l = 0; l < m->a.n_layers; l++) {
+    LayerW& L = m->layers[l];
+    v.push_back({&L.qkv, l, T_WQ});
+    v.push_back({&L.o, l, T_WO});
+    v.push_back({&L.w13, l, T_W1});
+    v.push_back({&L.w2, l, T_W2});
+  }
+  v.push_back({&m->output, -1, T_OUTPUT});
+  return v;
 }
 
 static void mark_present(lnb_model* m, int kind, int layer) {
@@ -297,19 +334,17 @@ extern "C" int lnb_model_create(const lnb_model_args* args, int device, int tp_r
   cudaDeviceGetAttribute(&m->sm_count, cudaDevAttrMultiProcessorCount, device);
   m->layers.resize(a.n_layers);
   auto alloc16 = [&](uint16_t** p, size_t elems) -> cudaError_t { return cudaMalloc((void**)p, elems * 2); };
-  cudaError_t e = cudaSuccess;
-  e = alloc16(&m->tok_embd, (size_t)a.vocab_size * a.dim);
+  cudaError_t e = alloc16(&m->tok_embd, (size_t)a.vocab_size * a.dim);
   if (e == cudaSuccess) e = alloc16(&m->norm, a.dim);
-  if (e == cudaSuccess) e = alloc16(&m->output, (size_t)vocab_l * a.dim);
-  for (int l = 0; l < a.n_layers && e == cudaSuccess; l++) {
-    LayerW& L = m->layers[l];
-    e = alloc16(&L.attn_norm, a.dim);
+  for (LayerW& L : m->layers) {
+    L.qkv.N = q_l + 2 * kv_l; L.o.N = a.dim; L.w13.N = 2 * ffn_l; L.w2.N = a.dim;
+    L.qkv.K = a.dim; L.o.K = q_l; L.w13.K = a.dim; L.w2.K = ffn_l;
+    if (e == cudaSuccess) e = alloc16(&L.attn_norm, a.dim);
     if (e == cudaSuccess) e = alloc16(&L.ffn_norm, a.dim);
-    if (e == cudaSuccess) e = alloc16(&L.wqkv, (size_t)(q_l + 2 * kv_l) * a.dim);
-    if (e == cudaSuccess) e = alloc16(&L.wo, (size_t)a.dim * q_l);
-    if (e == cudaSuccess) e = alloc16(&L.w13, (size_t)2 * ffn_l * a.dim);
-    if (e == cudaSuccess) e = alloc16(&L.w2, (size_t)a.dim * ffn_l);
   }
+  m->output.N = vocab_l; m->output.K = a.dim;
+  for (const LinMat& x : linear_mats(m))
+    if (e == cudaSuccess) e = cudaMalloc(&x.lin->w, x.lin->bytes());
   if (e == cudaSuccess) e = cudaMalloc((void**)&m->silu_tab, 65536 * 2);
   if (e != cudaSuccess) {
     lnb_model_destroy(m);
@@ -332,11 +367,9 @@ extern "C" int lnb_model_destroy(lnb_model* m) {
   cudaSetDevice(m->device);
   cudaDeviceSynchronize();
   if (m->comm) g_nccl.CommDestroy(m->comm);
-  cudaFree(m->tok_embd); cudaFree(m->norm); cudaFree(m->output); cudaFree(m->output_s);
-  for (auto& L : m->layers) {
-    cudaFree(L.attn_norm); cudaFree(L.ffn_norm); cudaFree(L.wqkv); cudaFree(L.wo); cudaFree(L.w13); cudaFree(L.w2);
-    cudaFree(L.sqkv); cudaFree(L.so); cudaFree(L.s13); cudaFree(L.s2);
-  }
+  cudaFree(m->tok_embd); cudaFree(m->norm);
+  for (auto& L : m->layers) { cudaFree(L.attn_norm); cudaFree(L.ffn_norm); }
+  for (const LinMat& x : linear_mats(m)) { cudaFree(x.lin->w); cudaFree(x.lin->s); }
   cudaFree(m->cis); cudaFree(m->silu_tab); cudaFree(m->staging); cudaFree(m->wpack_mem);
   delete m;
   return 0;
@@ -800,33 +833,6 @@ extern "C" int lnb_model_set_weight_format(lnb_model* m, int fmt) {
   m->wfmt = fmt;
   return 0;
 }
-// one linear matrix of the device layout: its bf16 panels / codes, its scales, its shape
-struct LinMat {
-  uint16_t** w;
-  uint8_t** s;
-  int N, K;
-  int layer;   // -1: the LM head
-  int kind;    // T_WQ (the stacked wq|wk|wv), T_WO, T_W1 (the interleaved w1|w3), T_W2, T_OUTPUT
-};
-static std::vector<LinMat> linear_mats(lnb_model* m) {
-  std::vector<LinMat> v;
-  const int d = m->a.dim;
-  for (int l = 0; l < m->a.n_layers; l++) {
-    LayerW& L = m->layers[l];
-    v.push_back({&L.wqkv, &L.sqkv, m->q_l + 2 * m->kv_l, d, l, T_WQ});
-    v.push_back({&L.wo, &L.so, d, m->q_l, l, T_WO});
-    v.push_back({&L.w13, &L.s13, 2 * m->ffn_l, d, l, T_W1});
-    v.push_back({&L.w2, &L.s2, d, m->ffn_l, l, T_W2});
-  }
-  v.push_back({&m->output, &m->output_s, m->vocab_l, d, -1, T_OUTPUT});
-  return v;
-}
-static size_t mx_scale_bytes(int N, int K) { return (size_t)(N / 8) * mx_nbp(K) * 8; }
-// the bytes of the codes (bf16: of the panels) of N rows
-static size_t code_bytes(int fmt, int N, int K) {
-  return fmt == LNB_WEIGHTS_MXFP4 ? (size_t)N * K / 2 : fmt == LNB_WEIGHTS_MXFP8 ? (size_t)N * K : (size_t)N * K * 2;
-}
-static size_t mat_bytes(int fmt, int N, int K) { return code_bytes(fmt, N, K) + (fmt == LNB_WEIGHTS_BF16 ? 0 : mx_scale_bytes(N, K)); }
 // the checkpoint tensor and row of device row d of a matrix (inverse of placement + panel_dest_row)
 static void checkpoint_row(const lnb_model* m, const LinMat& x, int64_t d, const char** name, int64_t* row) {
   static const char* kn[] = {"attention.wq.weight", "attention.wk.weight", "attention.wv.weight", "attention.wo.weight",
@@ -848,23 +854,23 @@ static void checkpoint_row(const lnb_model* m, const LinMat& x, int64_t d, const
 // held until every matrix has passed, so a refused weight leaves the bf16 model as it was.
 static int quantize_model(lnb_model* m, int fmt) {
   std::vector<LinMat> mats = linear_mats(m);
-  std::vector<uint8_t*> codes(mats.size(), nullptr), scales(mats.size(), nullptr);
+  std::vector<Linear> q;   // the quantized matrices
+  size_t total = 0;
+  for (const LinMat& x : mats) { q.push_back({nullptr, nullptr, fmt, x.lin->N, x.lin->K}); total += q.back().bytes(); }
   unsigned long long* flags = nullptr;
   auto drop = [&]() {
-    for (size_t i = 0; i < mats.size(); i++) { cudaFree(codes[i]); cudaFree(scales[i]); }
+    for (Linear& x : q) { cudaFree(x.w); cudaFree(x.s); }
     cudaFree(flags);
   };
-  size_t total = 0;
-  for (const LinMat& x : mats) total += mat_bytes(fmt, x.N, x.K);
   cudaError_t e = cudaMalloc((void**)&flags, mats.size() * 8);
   if (e == cudaSuccess) e = cudaMemset(flags, 0xff, mats.size() * 8);
   for (size_t i = 0; i < mats.size() && e == cudaSuccess; i++) {
-    e = cudaMalloc((void**)&codes[i], code_bytes(fmt, mats[i].N, mats[i].K));
-    if (e == cudaSuccess) e = cudaMalloc((void**)&scales[i], mx_scale_bytes(mats[i].N, mats[i].K));
-    if (e == cudaSuccess) e = cudaMemset(scales[i], 0, mx_scale_bytes(mats[i].N, mats[i].K));
+    e = cudaMalloc(&q[i].w, q[i].code_bytes());
+    if (e == cudaSuccess) e = cudaMalloc((void**)&q[i].s, q[i].scale_bytes());
+    if (e == cudaSuccess) e = cudaMemset(q[i].s, 0, q[i].scale_bytes());
     if (e == cudaSuccess) {
       (fmt == LNB_WEIGHTS_MXFP4 ? mxfp4_quantize_kernel : mxfp8_quantize_kernel)<<<m->sm_count * 8, 256>>>(
-          *mats[i].w, mats[i].N, mats[i].K, codes[i], scales[i], flags + i);
+          mats[i].lin->bf16(), q[i].N, q[i].K, q[i].codes(), q[i].s, flags + i);
       e = cudaGetLastError();
     }
   }
@@ -880,8 +886,8 @@ static int quantize_model(lnb_model* m, int fmt) {
     if (h[i] == ~0ull) continue;
     const char* name;
     int64_t row;
-    checkpoint_row(m, mats[i], (int64_t)(h[i] / (unsigned long long)mats[i].K), &name, &row);
-    const long long col = (long long)(h[i] % (unsigned long long)mats[i].K);
+    checkpoint_row(m, mats[i], (int64_t)(h[i] / (unsigned long long)q[i].K), &name, &row);
+    const long long col = (long long)(h[i] % (unsigned long long)q[i].K);
     drop();
     if (mats[i].layer < 0)
       return fail(LNB_EINVAL, "%s: tensor \"%s\" has a non-finite weight at row %lld, column %lld", wfmt_name(fmt), name, (long long)row, col);
@@ -889,9 +895,8 @@ static int quantize_model(lnb_model* m, int fmt) {
                 name, (long long)row, col);
   }
   for (size_t i = 0; i < mats.size(); i++) {
-    cudaFree(*mats[i].w);
-    *mats[i].w = reinterpret_cast<uint16_t*>(codes[i]);
-    *mats[i].s = scales[i];
+    cudaFree(mats[i].lin->w);
+    *mats[i].lin = q[i];
   }
   cudaFree(flags);
   return 0;
@@ -901,23 +906,21 @@ static int quantize_model(lnb_model* m, int fmt) {
 static int mx_read(lnb_model* m, int fmt, const char* name, uint8_t* codes, uint8_t* scales) {
   if (!m || !name) return fail(LNB_EINVAL, "NULL argument");
   if (!m->finalized) return fail(LNB_ESTATE, "model is not finalized");
-  if (m->wfmt != fmt) return fail(LNB_ESTATE, m->wfmt == LNB_WEIGHTS_BF16 ? "the model's weights are bf16" : "the model's weights are %s",
-                                  wfmt_name(m->wfmt));
+  const int mfmt = m->output.fmt;   // every linear matrix has the same format
+  if (mfmt != fmt) return fail(LNB_ESTATE, mfmt == LNB_WEIGHTS_BF16 ? "the model's weights are bf16" : "the model's weights are %s",
+                               wfmt_name(mfmt));
   int kind, layer;
   if (parse_name(m, name, &kind, &layer)) return fail(LNB_EINVAL, "unknown tensor name \"%s\"", name);
   if (kind == T_EMBD || kind == T_NORM || kind == T_ATTN_NORM || kind == T_FFN_NORM)
     return fail(LNB_EINVAL, "tensor \"%s\" is not a linear weight: it stays bf16", name);
   CU(cudaSetDevice(m->device));
   const Placement p = placement(m, kind, layer);
-  const LinMat* x = nullptr;
-  std::vector<LinMat> mats = linear_mats(m);
-  for (const LinMat& c : mats)
-    if (c.layer == layer && *c.w == p.dst) x = &c;
-  const int K = x->K, nbp = mx_nbp(K), nb = (K + 31) / 32;
-  const int rb = (int)code_bytes(fmt, 1, K), cpc = rb / (K / 8);   // code bytes of one row, of one chunk row (8 or 4)
-  std::vector<uint8_t> hc(code_bytes(fmt, x->N, K)), hs(mx_scale_bytes(x->N, K));
-  CU(cudaMemcpy(hc.data(), *x->w, hc.size(), cudaMemcpyDeviceToHost));
-  CU(cudaMemcpy(hs.data(), *x->s, hs.size(), cudaMemcpyDeviceToHost));
+  const Linear& x = *p.lin;
+  const int K = x.K, nbp = mx_nbp(K), nb = (K + 31) / 32;
+  const int rb = (int)(x.code_bytes() / x.N), cpc = rb / (K / 8);   // code bytes of one row, of one chunk row (8 or 4)
+  std::vector<uint8_t> hc(x.code_bytes()), hs(x.scale_bytes());
+  CU(cudaMemcpy(hc.data(), x.w, hc.size(), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(hs.data(), x.s, hs.size(), cudaMemcpyDeviceToHost));
   for (int64_t r = 0; r < p.rows; r++) {
     const int64_t d = p.dpanel_stride == 2 ? (r >> 2) * 8 + (p.dpanel0 ? 4 : 0) + (r & 3) : (int64_t)p.dpanel0 * 8 + r;
     const int64_t dp = d / 8, rr = d % 8;
@@ -936,11 +939,10 @@ extern "C" int lnb_model_mxfp4_read(lnb_model* m, const char* name, uint8_t* cod
 }
 extern "C" int lnb_model_weight_info(lnb_model* m, int* fmt, int64_t* device_bytes, int64_t* step_bytes) {
   if (!m) return fail(LNB_EINVAL, "model is NULL");
-  const int f = m->finalized ? m->wfmt : LNB_WEIGHTS_BF16;
   int64_t lin = 0;
-  for (const LinMat& x : linear_mats(m)) lin += (int64_t)mat_bytes(f, x.N, x.K);
+  for (const LinMat& x : linear_mats(m)) lin += (int64_t)x.lin->bytes();
   const int64_t norms = (int64_t)(2 * m->a.n_layers + 1) * m->a.dim * 2;
-  if (fmt) *fmt = f;
+  if (fmt) *fmt = m->output.fmt;
   if (device_bytes) *device_bytes = lin + norms + (int64_t)m->a.vocab_size * m->a.dim * 2;
   if (step_bytes) *step_bytes = lin + norms + (int64_t)m->a.dim * 2;   // every matrix and norm once, one embedding row
   return 0;
@@ -1155,14 +1157,14 @@ static int launch_gemv_fmt(const Launcher& L, int mode, GemvParams p, int M_tota
   }
   return 0;
 }
-// wfmt: the model's weight format (LNB_WEIGHTS_*); for MXFP8 and MXFP4, p.W points at the matrix's codes and Ws at its scales
+// x W^T for the matrix W (p.W, p.N and p.K come from it); the one place a weight format picks the kernels' F
 template <int PRO, int EPI>
-static int launch_gemv(const Launcher& L, int mode, GemvParams p, int M_total, int mb_rows = 0, const uint8_t* Ws = nullptr,
-                       int wfmt = LNB_WEIGHTS_BF16) {
+static int launch_gemv(const Launcher& L, int mode, GemvParams p, const Linear& W, int M_total, int mb_rows = 0) {
+  p.W = static_cast<const uint16_t*>(W.w); p.N = W.N; p.K = W.K;   // MX: the codes, the kernel's second argument the scales
   if (p.N % 16 || p.K % 8) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 16 and K %d of 8", p.N, p.K);  // 16: panel pairs
   if ((EPI == EPI_QKV_ROPE || EPI == EPI_SWIGLU) && p.N % 32) return fail(LNB_EINVAL, "gemv: N %d must be a multiple of 32", p.N);
-  if (wfmt == LNB_WEIGHTS_MXFP8) return launch_gemv_fmt<PRO, EPI, WF_MXFP8>(L, mode, p, M_total, mb_rows, Ws);
-  if (wfmt == LNB_WEIGHTS_MXFP4) return launch_gemv_fmt<PRO, EPI, WF_MXFP4>(L, mode, p, M_total, mb_rows, Ws);
+  if (W.fmt == LNB_WEIGHTS_MXFP8) return launch_gemv_fmt<PRO, EPI, WF_MXFP8>(L, mode, p, M_total, mb_rows, W.s);
+  if (W.fmt == LNB_WEIGHTS_MXFP4) return launch_gemv_fmt<PRO, EPI, WF_MXFP4>(L, mode, p, M_total, mb_rows, W.s);
   return launch_gemv_fmt<PRO, EPI, WF_BF16>(L, mode, p, M_total, mb_rows, nullptr);
 }
 
@@ -1541,10 +1543,11 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
     A.add(&s->m8, (size_t)s->mpad * m->ffn_l * 2);
     A.add(&s->qkv_raw, (size_t)max_rows * (m->q_l + 2 * m->kv_l) * 2);
     A.add(&s->gu, (size_t)max_rows * 2 * m->ffn_l * 2);
-    if (m->wfmt != LNB_WEIGHTS_BF16) {
-      for (const LinMat& x : linear_mats(m)) s->wdq_elems = std::max(s->wdq_elems, x.layer < 0 ? (size_t)TC_BN * x.K : (size_t)x.N * x.K);
-      A.add(&s->wdq, s->wdq_elems * 2);
-    }
+    // the dequantized panels an MX matrix's GEMM reads (the LM head's GEMMs take row slices: it needs one 128-row tile)
+    for (const LinMat& x : linear_mats(m))
+      if (x.lin->fmt != LNB_WEIGHTS_BF16)
+        s->wdq_elems = std::max(s->wdq_elems, x.layer < 0 ? (size_t)TC_BN * x.lin->K : (size_t)x.lin->N * x.lin->K);
+    if (s->wdq_elems) A.add(&s->wdq, s->wdq_elems * 2);
   }
   const size_t in_words = row_map_words(max_rows);
   A.add(&s->d_rag, in_words * 4);
@@ -1770,14 +1773,14 @@ static bool engine_probe(lnb_session* s) {
   if (s->eng_state) return s->eng_state > 0;
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
-  auto no = [&](const char* why) { s->eng_state = -1; s->eng_why = why; return false; };
+  auto no = [&](const std::string& why) { s->eng_state = -1; s->eng_why = why; return false; };
   // Default: the engine is meant for where launch count or the serial order dominates -- LNB_ACC_STRICT at every N and
   // every host-driven loop; in LNB_ACC_FAST it competes with the kernel chain.  It is the default except for single-GPU
   // FAST sessions; LNB_ENGINE=1 / 0 forces it on / off.
   const char* e = getenv("LNB_ENGINE");
   if (e && !strcmp(e, "0")) return no("LNB_ENGINE=0");
-  if (m->wfmt == LNB_WEIGHTS_MXFP8) return no("MXFP8 weights: the decode and batch engines stream bf16 panels");
-  if (m->wfmt == LNB_WEIGHTS_MXFP4) return no("MXFP4 weights: the decode and batch engines stream bf16 panels");
+  if (m->output.fmt != LNB_WEIGHTS_BF16)   // every linear matrix has the same format
+    return no(std::string(wfmt_name(m->output.fmt)) + " weights: the decode and batch engines stream bf16 panels");
   // single-sequence steps of single-GPU FAST sessions stay on the kernel chain by default (the batch engine does not care)
   s->eng_single_default = (e && !strcmp(e, "1")) || !(s->mode == LNB_ACC_FAST && m->tp_size == 1);
   const int kmax = std::max(a.dim, std::max(m->q_l, m->ffn_l));
@@ -1864,25 +1867,23 @@ static bool ensure_wpack(lnb_model* m) {
   const lnb_model_args& a = m->a;
   const int G = m->sm_count, L = a.n_layers;
   auto no = [&](const std::string& why) { m->wpack_state = -1; m->wpack_why = why; return false; };
-  if (m->wfmt == LNB_WEIGHTS_MXFP8) return no("MXFP8 weights: the packed copies are built from bf16 panels");
-  if (m->wfmt == LNB_WEIGHTS_MXFP4) return no("MXFP4 weights: the packed copies are built from bf16 panels");
-  struct Mat { const uint16_t* W; int N; lnb_model::WPack* wp; };
-  std::vector<Mat> mats;
-  m->wp_w13.assign(L, lnb_model::WPack{});
-  for (int l = 0; l < L; l++) mats.push_back({m->layers[l].w13, 2 * m->ffn_l, &m->wp_w13[l]});
-  mats.push_back({m->output, m->vocab_l, &m->wp_out});
+  if (m->output.fmt != LNB_WEIGHTS_BF16)
+    return no(std::string(wfmt_name(m->output.fmt)) + " weights: the packed copies are built from bf16 panels");
+  std::vector<Linear*> mats;
+  for (int l = 0; l < L; l++) mats.push_back(&m->layers[l].w13);
+  mats.push_back(&m->output);
   const int K = a.dim;
   size_t total = 0;
   std::vector<size_t> off_data, off_units;
-  for (Mat& x : mats) {
-    const int kt = eng_kt(LNB_ACC_STRICT, x.N, K, G);
+  for (Linear* x : mats) {
+    const int kt = eng_kt(LNB_ACC_STRICT, x->N, K, G);
     if (K % 32 || kt % 32) return no("packed weights need K and the k-tile to be multiples of 32");
-    x.wp->kt = kt;
-    x.wp->n_units = (int64_t)(x.N / 8) * ((K + kt - 1) / kt);
+    x->pack.kt = kt;
+    x->pack.n_units = (int64_t)(x->N / 8) * ((K + kt - 1) / kt);
     off_data.push_back(total);
-    total += (size_t)x.N / 8 * K * 12;
+    total += (size_t)x->N / 8 * K * 12;
     off_units.push_back(total);
-    total = (total + x.wp->n_units + 255) & ~(size_t)255;
+    total = (total + x->pack.n_units + 255) & ~(size_t)255;
   }
   unsigned long long* ctr = nullptr;
   if (cudaMalloc(&m->wpack_mem, total) != cudaSuccess || cudaMalloc((void**)&ctr, mats.size() * 16) != cudaSuccess) {
@@ -1895,10 +1896,10 @@ static bool ensure_wpack(lnb_model* m) {
   }
   cudaMemset(ctr, 0, mats.size() * 16);
   for (size_t i = 0; i < mats.size(); i++) {
-    lnb_model::WPack& wp = *mats[i].wp;
+    WPack& wp = mats[i]->pack;
     wp.data = static_cast<uint8_t*>(m->wpack_mem) + off_data[i];
     wp.units = static_cast<uint8_t*>(m->wpack_mem) + off_units[i];
-    wpack_encode_kernel<<<G * 8, 256>>>(mats[i].W, mats[i].N / 8, K, wp.kt, wp.data, wp.units, ctr + 2 * i);
+    wpack_encode_kernel<<<G * 8, 256>>>(mats[i]->bf16(), mats[i]->N / 8, K, wp.kt, wp.data, wp.units, ctr + 2 * i);
   }
   std::vector<unsigned long long> h(mats.size() * 2);
   cudaError_t e = cudaGetLastError();
@@ -1910,8 +1911,8 @@ static bool ensure_wpack(lnb_model* m) {
     return no(std::string("packing the weights failed: ") + cudaGetErrorString(e));
   }
   for (size_t i = 0; i < mats.size(); i++) {
-    mats[i].wp->read_bytes = (int64_t)h[2 * i];
-    mats[i].wp->packed_units = (int64_t)h[2 * i + 1];
+    mats[i]->pack.read_bytes = (int64_t)h[2 * i];
+    mats[i]->pack.packed_units = (int64_t)h[2 * i + 1];
   }
   m->wpack_state = 1;
   return true;
@@ -1922,11 +1923,12 @@ extern "C" int lnb_model_wpack_read(lnb_model* m, int layer, uint8_t* data, uint
   if (layer < -1 || layer >= m->a.n_layers) return fail(LNB_EINVAL, "layer %d out of range", layer);
   CU(cudaSetDevice(m->device));
   if (!ensure_wpack(m)) { g_err = m->wpack_why; return 0; }
-  const lnb_model::WPack& wp = layer < 0 ? m->wp_out : m->wp_w13[layer];
-  const int64_t N = layer < 0 ? m->vocab_l : 2 * (int64_t)m->ffn_l, K = m->a.dim;
+  const Linear& x = layer < 0 ? m->output : m->layers[layer].w13;
+  const WPack& wp = x.pack;
+  const int64_t N = x.N, K = x.K;
   if (data) CU(cudaMemcpy(data, wp.data, (size_t)(N / 8) * K * 12, cudaMemcpyDeviceToHost));
   if (units) CU(cudaMemcpy(units, wp.units, (size_t)wp.n_units, cudaMemcpyDeviceToHost));
-  if (src) CU(cudaMemcpy(src, layer < 0 ? m->output : m->layers[layer].w13, (size_t)N * K * 2, cudaMemcpyDeviceToHost));
+  if (src) CU(cudaMemcpy(src, x.bf16(), x.bytes(), cudaMemcpyDeviceToHost));
   if (info) { info[0] = wp.kt; info[1] = wp.n_units; info[2] = wp.packed_units; info[3] = wp.read_bytes; info[4] = N; }
   return 1;
 }
@@ -1944,11 +1946,15 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
   std::vector<EnginePhase> ph;
   // which phase of the step wrote a tagged vector last (consumers wait for exactly that phase's tag)
   int w_x = -1, w_h1 = -1, w_qkv = -1, w_o = -1, w_m = -1;
-  auto gemv = [&](int pro, int epi, const uint16_t* W, int N, int K, const uint16_t* x, const uint16_t* norm_w, uint16_t* out, int ldo,
+  const bool tp = m->tp_size > 1;
+  // STRICT streams the packed copies of w1|w3 and the LM head (the FAST engine's KS = 8 chains read bf16 only)
+  const bool wpack = mode == LNB_ACC_STRICT && ensure_wpack(m);
+  auto gemv = [&](int pro, int epi, const Linear& W, const uint16_t* x, const uint16_t* norm_w, uint16_t* out, int ldo,
                   const uint16_t* res) {
     EnginePhase e{};
-    e.type = EP_GEMV; e.pro = pro; e.epi = epi; e.W = W; e.N = N; e.K = K; e.kt = eng_kt(mode, N, K, G); e.x = x; e.ldx = K;
-    e.norm_w = norm_w; e.out_bf16 = out; e.ldo = ldo; e.res = res;
+    e.type = EP_GEMV; e.pro = pro; e.epi = epi; e.W = W.bf16(); e.N = W.N; e.K = W.K; e.kt = eng_kt(mode, W.N, W.K, G); e.x = x;
+    e.ldx = W.K; e.norm_w = norm_w; e.out_bf16 = out; e.ldo = ldo; e.res = res;
+    if (wpack && W.pack.data && W.pack.kt == e.kt) { e.Wp = W.pack.data; e.Wu = W.pack.units; }
     return e;
   };
   auto input = [&](EnginePhase& e, const uint32_t* vec, int writer) {   // tagged input of the phase being appended
@@ -1957,16 +1963,10 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
   auto resid = [&](EnginePhase& e, const uint32_t* vec, int writer) {
     if (full && writer >= 0) { e.res_t = vec; e.res_delta = (int)ph.size() - writer; }
   };
-  const bool tp = m->tp_size > 1;
-  // STRICT streams the packed copies of w1|w3 and the LM head (the FAST engine's KS = 8 chains read bf16 only)
-  const bool wpack = mode == LNB_ACC_STRICT && ensure_wpack(m);
-  auto packed = [&](EnginePhase& e, const lnb_model::WPack& wp) {
-    if (wpack && wp.kt == e.kt) { e.Wp = wp.data; e.Wu = wp.units; }
-  };
   for (int l = 0; l < n_layers; l++) {
     LayerW& W = m->layers[l];
     if (full || kind == 0) {  // attn_norm -> wq|wk|wv -> RoPE -> KV append
-      EnginePhase e = gemv(PRO_RMSNORM, EPI_QKV_ROPE, W.wqkv, m->q_l + 2 * m->kv_l, a.dim, s->x, W.attn_norm, s->q, m->q_l, nullptr);
+      EnginePhase e = gemv(PRO_RMSNORM, EPI_QKV_ROPE, W.qkv, s->x, W.attn_norm, s->q, m->q_l, nullptr);
       e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->ck[l] + cache_off; e.cache_v = s->cv[l] + cache_off;
       if (full && l == 0) e.flags |= EF_X_TOKEN;
       else input(e, s->x_t, w_x);
@@ -1982,7 +1982,7 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
       ph.push_back(e);
     }
     if (full || kind == 1) {  // wo + residual
-      EnginePhase e = gemv(PRO_PLAIN, (tp && full) ? EPI_P2P : EPI_RESID, W.wo, a.dim, m->q_l, s->o, nullptr, s->h1, a.dim, s->x);
+      EnginePhase e = gemv(PRO_PLAIN, (tp && full) ? EPI_P2P : EPI_RESID, W.o, s->o, nullptr, s->h1, a.dim, s->x);
       input(e, s->o_t, w_o);
       if (full && !tp) {
         if (l == 0) e.flags |= EF_RES_TOKEN; else resid(e, s->x_t, w_x);
@@ -1998,14 +1998,13 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
       }
     }
     if (full || kind == 2) {  // ffn_norm -> w1|w3 -> SiLU * up
-      EnginePhase e = gemv(PRO_RMSNORM, EPI_SWIGLU, W.w13, 2 * m->ffn_l, a.dim, s->h1, W.ffn_norm, s->mbuf, m->ffn_l, nullptr);
-      packed(e, m->wp_w13[l]);
+      EnginePhase e = gemv(PRO_RMSNORM, EPI_SWIGLU, W.w13, s->h1, W.ffn_norm, s->mbuf, m->ffn_l, nullptr);
       input(e, s->h1_t, w_h1);
       if (full) { e.out_t = s->m_t; w_m = (int)ph.size(); }
       ph.push_back(e);
     }
     if (full || kind == 3) {  // w2 + residual
-      EnginePhase e = gemv(PRO_PLAIN, (tp && full) ? EPI_P2P : EPI_RESID, W.w2, a.dim, m->ffn_l, s->mbuf, nullptr, s->x, a.dim, s->h1);
+      EnginePhase e = gemv(PRO_PLAIN, (tp && full) ? EPI_P2P : EPI_RESID, W.w2, s->mbuf, nullptr, s->x, a.dim, s->h1);
       input(e, s->m_t, w_m);
       if (full && !tp) { resid(e, s->h1_t, w_h1); e.out_t = s->x_t; w_x = (int)ph.size(); }
       ph.push_back(e);
@@ -2021,8 +2020,7 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
   if (full || kind == 4) {
     const int reps = kind == 4 ? 4 : 1;
     for (int i = 0; i < reps; i++) {
-      EnginePhase e = gemv(PRO_RMSNORM, EPI_LOGITS, m->output, m->vocab_l, a.dim, s->x, m->norm, nullptr, m->vocab_l, nullptr);
-      packed(e, m->wp_out);
+      EnginePhase e = gemv(PRO_RMSNORM, EPI_LOGITS, m->output, s->x, m->norm, nullptr, m->vocab_l, nullptr);
       e.out_f32 = const_cast<float*>(logits_out); e.n_offset = m->tp_rank * m->vocab_l;
       if (full && n_layers > 0) input(e, s->x_t, w_x);
       if (full) e.flags |= EF_GRID_SYNC;
@@ -2147,10 +2145,11 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
   const bool tp = m->tp_size > 1;
   const bool tc = s->batch_tc != 0;
   std::vector<BatchPhase> ph;
-  auto gemv = [&](int pro, int epi, const uint16_t* W, int N, int K, const uint16_t* x, const uint16_t* norm_w, uint16_t* out, int ldo,
+  auto gemv = [&](int pro, int epi, const Linear& W, const uint16_t* x, const uint16_t* norm_w, uint16_t* out, int ldo,
                   const uint16_t* res) {
+    const int N = W.N, K = W.K;
     BatchPhase e{};
-    e.type = BP_GEMV; e.pro = pro; e.epi = epi; e.W = W; e.N = N; e.K = K; e.kt = eng_kt(mode, N, K, G); e.x = x;
+    e.type = BP_GEMV; e.pro = pro; e.epi = epi; e.W = W.bf16(); e.N = N; e.K = K; e.kt = eng_kt(mode, N, K, G); e.x = x;
     e.norm_w = norm_w; e.out = out; e.ldo = ldo; e.res = res;
     if (tc) {
       // tensor-core form: 128-row tiles; the k-tile grows as the CTA's share of the rows shrinks (about 32 KB per stage,
@@ -2178,7 +2177,7 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
     LayerW& W = m->layers[l];
     ph.push_back(scale(s->bx, l == 0, W.attn_norm));
     {
-      BatchPhase e = gemv(PRO_RMSNORM, EPI_QKV_ROPE, W.wqkv, m->q_l + 2 * m->kv_l, a.dim, s->bx, W.attn_norm, s->bq, m->q_l, nullptr);
+      BatchPhase e = gemv(PRO_RMSNORM, EPI_QKV_ROPE, W.qkv, s->bx, W.attn_norm, s->bq, m->q_l, nullptr);
       e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->ck[l]; e.cache_v = s->cv[l];
       ph.push_back(e);
     }
@@ -2187,16 +2186,16 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
       e.type = BP_SDPA; e.x = s->bq; e.out = s->bo; e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->ck[l]; e.cache_v = s->cv[l];
       ph.push_back(e);
     }
-    ph.push_back(gemv(PRO_PLAIN, tp ? EPI_P2P : EPI_RESID, W.wo, a.dim, m->q_l, s->bo, nullptr, s->bh1, a.dim, s->bx));
+    ph.push_back(gemv(PRO_PLAIN, tp ? EPI_P2P : EPI_RESID, W.o, s->bo, nullptr, s->bh1, a.dim, s->bx));
     if (tp) ph.push_back(reduce(s->bx, s->bh1));
     ph.push_back(scale(s->bh1, false, W.ffn_norm));
-    ph.push_back(gemv(PRO_RMSNORM, EPI_SWIGLU, W.w13, 2 * m->ffn_l, a.dim, s->bh1, W.ffn_norm, s->bm, m->ffn_l, nullptr));
-    ph.push_back(gemv(PRO_PLAIN, tp ? EPI_P2P : EPI_RESID, W.w2, a.dim, m->ffn_l, s->bm, nullptr, s->bx, a.dim, s->bh1));
+    ph.push_back(gemv(PRO_RMSNORM, EPI_SWIGLU, W.w13, s->bh1, W.ffn_norm, s->bm, m->ffn_l, nullptr));
+    ph.push_back(gemv(PRO_PLAIN, tp ? EPI_P2P : EPI_RESID, W.w2, s->bm, nullptr, s->bx, a.dim, s->bh1));
     if (tp) ph.push_back(reduce(s->bh1, s->bx));
   }
   ph.push_back(scale(s->bx, n_layers == 0, m->norm));
   {
-    BatchPhase e = gemv(PRO_RMSNORM, EPI_LOGITS, m->output, m->vocab_l, a.dim, s->bx, m->norm, nullptr, m->vocab_l, nullptr);
+    BatchPhase e = gemv(PRO_RMSNORM, EPI_LOGITS, m->output, s->bx, m->norm, nullptr, m->vocab_l, nullptr);
     e.out_f32 = const_cast<float*>(logits_out); e.n_offset = m->tp_rank * m->vocab_l;
     ph.push_back(e);
   }
@@ -2374,9 +2373,9 @@ static int per_row_head(const Launcher& L, lnb_session* s, const Rows& R) {
   if (strict && (rc = launch_rms_scale(L, x, a.dim, s->rs, n, a.dim, a.norm_eps))) return rc;
   GemvParams p{};
   p.rscale = strict ? s->rs : nullptr;
-  p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
+  p.x = x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
   p.out_f32 = s->logits; p.ldo = m->vocab_l; p.n_offset = m->tp_rank * m->vocab_l; p.st = nullptr; p.argmax_row = -1;
-  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, n, R.mb_rows, m->output_s, m->wfmt))) return rc;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, m->output, n, R.mb_rows))) return rc;
   if ((rc = gather_logits(s, 0, n))) return rc;
   const float* lg = (m->tp_size > 1) ? s->logits_full : s->logits;
   return launch_kernel(L, argmax_f32_kernel, dim3(n), dim3(256), 0, lg, a.vocab_size, s->d_next_arr);
@@ -2435,22 +2434,22 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
     return launch_rms_scale(L, xin, a.dim, s->rs, rows, a.dim, a.norm_eps);
   };
   // wo / w2 + residual: out = res + x W^T; tensor-parallel ranks sum their partials first (peer all-reduce or NCCL)
-  auto proj_resid = [&](const uint16_t* W, const uint8_t* Ws, int K, const uint16_t* x, const uint16_t* res, uint16_t* out) -> int {
+  auto proj_resid = [&](const Linear& W, const uint16_t* x, const uint16_t* res, uint16_t* out) -> int {
     GemvParams p{};
-    p.W = W; p.N = a.dim; p.K = K; p.x = x; p.ldx = K; p.ldo = a.dim;
+    p.x = x; p.ldx = W.K; p.ldo = a.dim;
     if (m->tp_size == 1) {
       p.out_bf16 = out; p.res = res;
-      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, S, mb_rows, Ws, m->wfmt);
+      return launch_gemv<PRO_PLAIN, EPI_RESID>(L, mode, p, W, S, mb_rows);
     }
     int rc2;
     if (s->p2p_ready) {
       p.p2p = s->p2p; p.st = s->st;
-      if ((rc2 = launch_gemv<PRO_PLAIN, EPI_P2P>(L, mode, p, S))) return rc2;
+      if ((rc2 = launch_gemv<PRO_PLAIN, EPI_P2P>(L, mode, p, W, S))) return rc2;
       return launch_kernel(L, p2p_reduce_resid_kernel, dim3(std::min(16, (S * a.dim + 255) / 256)), dim3(256), 0, s->p2p, s->st, res, out,
                            S * a.dim);
     }
     p.out_f32 = s->part;
-    if ((rc2 = launch_gemv<PRO_PLAIN, EPI_F32RAW>(L, mode, p, S))) return rc2;
+    if ((rc2 = launch_gemv<PRO_PLAIN, EPI_F32RAW>(L, mode, p, W, S))) return rc2;
     NC(g_nccl.AllReduce(s->part, s->part, (size_t)S * a.dim, ncclFloat32_, ncclSum_, m->comm, s->stream));
     return launch_kernel(L, resid_from_f32_kernel, dim3(std::min(kWaveSMs, (S * a.dim + 255) / 256)), dim3(256), 0, (const float*)s->part,
                          res, out, (int64_t)S * a.dim);
@@ -2461,25 +2460,24 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
     {  // attn_norm -> wq|wk|wv -> RoPE -> KV append            (:222, :297-403)
       GemvParams p{};
       p.rscale = strict ? s->rs : nullptr;
-      p.W = W.wqkv; p.N = m->q_l + 2 * m->kv_l; p.K = a.dim;
       p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm; p.eps = a.norm_eps;
       p.out_bf16 = s->q; p.ldo = m->q_l;
       p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
       p.cache_k = s->ck[l] + R.cache_off; p.cache_v = s->cv[l] + R.cache_off; p.cis = m->cis; p.pos_ptr = &s->st->pos;
       p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = R.seq_stride;
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, S, mb_rows, W.sqkv, m->wfmt))) return rc;
+      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, W.qkv, S, mb_rows))) return rc;
     }
     if ((rc = launch_attention(L, s, l, R, s->o, 0))) return rc;
-    if ((rc = proj_resid(W.wo, W.so, m->q_l, s->o, s->x, s->h1))) return rc;            // wo + residual (:522, :232)
+    if ((rc = proj_resid(W.o, s->o, s->x, s->h1))) return rc;      // wo + residual (:522, :232)
     if ((rc = strict_scale(s->h1, S))) return rc;
     {  // ffn_norm -> w1|w3 -> SiLU * up                             (:237, :601-614)
       GemvParams p{};
       p.rscale = strict ? s->rs : nullptr;
-      p.W = W.w13; p.N = 2 * m->ffn_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm; p.eps = a.norm_eps;
+      p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm; p.eps = a.norm_eps;
       p.out_bf16 = s->mbuf; p.ldo = m->ffn_l; p.silu_tab = m->silu_tab;
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, S, mb_rows, W.s13, m->wfmt))) return rc;
+      if ((rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, mode, p, W.w13, S, mb_rows))) return rc;
     }
-    if ((rc = proj_resid(W.w2, W.s2, m->ffn_l, s->mbuf, s->h1, s->x))) return rc;        // w2 + residual (:619, :248)
+    if ((rc = proj_resid(W.w2, s->mbuf, s->h1, s->x))) return rc;  // w2 + residual (:619, :248)
   }
   if (R.head == HEAD_PER_ROW) return per_row_head(L, s, R);
   // output_norm -> output -> f32 logits (+ greedy argmax of the last row)   (:166-175; inference.go:207-216)
@@ -2488,14 +2486,13 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
   if ((rc = strict_scale(s->x + (size_t)row0 * a.dim, rows))) return rc;
   GemvParams p{};
   p.rscale = strict ? s->rs : nullptr;
-  p.W = m->output; p.N = m->vocab_l; p.K = a.dim;
   p.x = s->x + (size_t)row0 * a.dim; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
   p.out_f32 = R.head != HEAD_NONE ? s->logits : nullptr; p.ldo = m->vocab_l;
   p.n_offset = m->tp_rank * m->vocab_l;
   p.st = s->st; p.argmax_row = rows - 1; p.m_off = 0;
   p.publish = (m->tp_size == 1) ? 1 : 0;
   p.advance = R.advance ? 1 : 0; p.tok_out = s->d_tok_out;
-  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, rows, 0, m->output_s, m->wfmt))) return rc;
+  if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, mode, p, m->output, rows))) return rc;
   if (m->tp_size > 1) {
     if (s->p2p_ready) rc = launch_kernel(L, p2p_argmax_kernel, dim3(1), dim3(32), 0, s->p2p, s->st, R.advance ? 1 : 0, s->d_tok_out);
     else rc = reduce_argmax_publish(L, s, R.advance);
@@ -2519,18 +2516,19 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
     return rc;
   const int n_layers = active_layers(s);
   const int ew_grid = m->sm_count * 8;
-  // the bf16 panels a GEMM reads: the matrix itself, or (MXFP8, MXFP4) rows [0, N) dequantized into the session's scratch
-  auto tc_w = [&](GemmTcParams& g, const uint16_t* W, const uint8_t* Ws, int N, int K) -> int {
-    g.W = Ws ? s->wdq : W;
-    if (!Ws) return 0;
-    return launch_kernel(L, m->wfmt == LNB_WEIGHTS_MXFP4 ? mxfp4_dequant_kernel : mxfp8_dequant_kernel, dim3(ew_grid), dim3(256), 0,
-                         reinterpret_cast<const uint8_t*>(W), Ws, N, K, s->wdq);
+  // the matrix operand of a GEMM (g.W, g.N, g.K): the bf16 panels of W, or (MXFP8, MXFP4) W dequantized into the session's scratch
+  auto tc_w = [&](GemmTcParams& g, const Linear& W) -> int {
+    g.N = W.N; g.K = W.K;
+    if (W.fmt == LNB_WEIGHTS_BF16) { g.W = W.bf16(); return 0; }
+    g.W = s->wdq;
+    return launch_kernel(L, W.fmt == LNB_WEIGHTS_MXFP4 ? mxfp4_dequant_kernel : mxfp8_dequant_kernel, dim3(ew_grid), dim3(256), 0,
+                         (const uint8_t*)W.codes(), (const uint8_t*)W.s, W.N, W.K, s->wdq);
   };
   // wo / w2 + residual: out = res + X W^T; tensor-parallel ranks sum their partials over NCCL first
-  auto proj_resid = [&](const uint16_t* X8, const uint16_t* W, const uint8_t* Ws, int K, const uint16_t* res, uint16_t* out) -> int {
+  auto proj_resid = [&](const uint16_t* X8, const Linear& W, const uint16_t* res, uint16_t* out) -> int {
     GemmTcParams g{};
-    g.X8 = X8; g.M = S; g.N = a.dim; g.K = K; g.ldo = a.dim;
-    if (int rc2 = tc_w(g, W, Ws, a.dim, K)) return rc2;
+    g.X8 = X8; g.M = S; g.ldo = a.dim;
+    if (int rc2 = tc_w(g, W)) return rc2;
     if (m->tp_size == 1) {
       g.out_bf16 = out; g.res = res;
       return launch_gemm_tc<TC_EPI_RESID>(L, g);
@@ -2547,8 +2545,8 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
       return rc;
     {
       GemmTcParams g{};
-      g.X8 = s->xn8; g.M = S; g.N = qkv_n; g.K = a.dim; g.out_bf16 = s->qkv_raw; g.ldo = qkv_n;
-      if ((rc = tc_w(g, W.wqkv, W.sqkv, qkv_n, a.dim))) return rc;
+      g.X8 = s->xn8; g.M = S; g.out_bf16 = s->qkv_raw; g.ldo = qkv_n;
+      if ((rc = tc_w(g, W.qkv))) return rc;
       if ((rc = launch_gemm_tc<TC_EPI_BF16>(L, g))) return rc;
     }
     if ((rc = launch_kernel(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
@@ -2556,18 +2554,18 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
                             R.pos_arr, R.row_seq, (long long)s->seq_len * m->kv_l)))
       return rc;
     if ((rc = launch_attention(L, s, l, R, s->o8, 1))) return rc;
-    if ((rc = proj_resid(s->o8, W.wo, W.so, m->q_l, s->x, s->h1))) return rc;
+    if ((rc = proj_resid(s->o8, W.o, s->x, s->h1))) return rc;
     if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->h1, a.dim, (const uint16_t*)W.ffn_norm,
                             s->xn8, S, a.dim, a.norm_eps)))
       return rc;
     {
       GemmTcParams g{};
       // SwiGLU in the epilogue: the hidden activations go straight into the X8 operand of the w2 GEMM
-      g.X8 = s->xn8; g.M = S; g.N = 2 * m->ffn_l; g.K = a.dim; g.out_bf16 = s->m8; g.ldo = m->ffn_l; g.silu_tab = m->silu_tab;
-      if ((rc = tc_w(g, W.w13, W.s13, 2 * m->ffn_l, a.dim))) return rc;
+      g.X8 = s->xn8; g.M = S; g.out_bf16 = s->m8; g.ldo = m->ffn_l; g.silu_tab = m->silu_tab;
+      if ((rc = tc_w(g, W.w13))) return rc;
       if ((rc = launch_gemm_tc<TC_EPI_SWIGLU>(L, g))) return rc;
     }
-    if ((rc = proj_resid(s->m8, W.w2, W.s2, m->ffn_l, s->h1, s->x))) return rc;
+    if ((rc = proj_resid(s->m8, W.w2, s->h1, s->x))) return rc;
   }
   // LM head: all rows on the tensor cores when asked for (and the vocabulary shard tiles), then the
   // last row through the GEMV, which also owns the greedy argmax (identical to the decode path)
@@ -2577,30 +2575,27 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
                             a.dim, a.norm_eps)))
       return rc;
     GemmTcParams g{};
-    g.X8 = s->xn8; g.W = m->output; g.M = S - 1; g.N = m->vocab_l; g.K = a.dim; g.out_f32 = s->logits; g.ldo = m->vocab_l;
+    g.X8 = s->xn8; g.M = S - 1; g.ldo = m->vocab_l;
     // MXFP8, MXFP4: the LM head in row slices that fit the scratch (whole 128-row tiles), each dequantized before its GEMM
-    const int slice = m->output_s ? (int)std::min<size_t>(m->vocab_l, s->wdq_elems / a.dim / TC_BN * TC_BN) : m->vocab_l;
+    const int slice = m->output.s ? (int)std::min<size_t>(m->vocab_l, s->wdq_elems / a.dim / TC_BN * TC_BN) : m->vocab_l;
     for (int n0 = 0; S > 1 && n0 < m->vocab_l; n0 += slice) {
-      g.N = std::min(slice, m->vocab_l - n0);
       g.out_f32 = s->logits + n0;
-      const uint16_t* codes = reinterpret_cast<const uint16_t*>(reinterpret_cast<const uint8_t*>(m->output) + code_bytes(m->wfmt, n0, a.dim));
-      if (m->output_s && (rc = tc_w(g, codes, m->output_s + (size_t)(n0 / 8) * mx_nbp(a.dim) * 8, g.N, a.dim))) return rc;
+      if ((rc = tc_w(g, m->output.rows(n0, std::min(slice, m->vocab_l - n0))))) return rc;
       if ((rc = launch_gemm_tc<TC_EPI_F32TRUNC>(L, g))) return rc;
     }
   } else if (R.head == HEAD_ALL && S > 1) {
     GemvParams p{};
-    p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
+    p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
     p.out_f32 = s->logits; p.ldo = m->vocab_l; p.st = nullptr; p.argmax_row = -1;
-    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, S - 1, 0, m->output_s, m->wfmt))) return rc;
+    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, m->output, S - 1))) return rc;
   }
   {
     GemvParams p{};
-    p.W = m->output; p.N = m->vocab_l; p.K = a.dim;
     p.x = s->x + (size_t)(S - 1) * a.dim; p.ldx = a.dim; p.norm_w = m->norm; p.eps = a.norm_eps;
     p.out_f32 = R.head != HEAD_NONE ? s->logits + (R.head == HEAD_ALL ? (size_t)(S - 1) * m->vocab_l : 0) : nullptr;
     p.ldo = m->vocab_l; p.n_offset = m->tp_rank * m->vocab_l;
     p.st = s->st; p.argmax_row = 0; p.publish = (m->tp_size == 1) ? 1 : 0; p.advance = 0; p.tok_out = s->d_tok_out;
-    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1, 0, m->output_s, m->wfmt))) return rc;
+    if ((rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, m->output, 1))) return rc;
     if (m->tp_size > 1) {
       if ((rc = reduce_argmax_publish(L, s, false))) return rc;
       if (R.head != HEAD_NONE && R.gather && (rc = gather_logits(s, 0, R.head_rows))) return rc;
@@ -3605,6 +3600,11 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   CU(cudaSetDevice(m->device));
+  auto mat = [&](int l) -> const Linear& {   // the matrix this kind times in layer l
+    if (kind == 4) return m->output;
+    const LayerW& W = m->layers[l];
+    return kind == 0 ? W.qkv : kind == 1 ? W.o : kind == 2 ? W.w13 : W.w2;
+  };
   if (engine_ok(s)) {
     // the projection as the decode step runs it: a phase of the persistent engine (balanced static row split, weights
     // prefetched across the grid barrier).  One launch walks all layers' copies `reps` times; time per phase.
@@ -3621,23 +3621,13 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
     float ms = 0.f;
     CU(cudaEventElapsedTime(&ms, s->ev0, s->ev1));
     const int n = s->n_phases * reps;
-    int64_t bytes = 0;
-    switch (kind) {
-      case 0: bytes = (int64_t)(m->q_l + 2 * m->kv_l) * a.dim * 2; break;
-      case 1: bytes = (int64_t)a.dim * m->q_l * 2; break;
-      case 2: bytes = (int64_t)2 * m->ffn_l * a.dim * 2; break;
-      case 3: bytes = (int64_t)a.dim * m->ffn_l * 2; break;
-      default: bytes = (int64_t)m->vocab_l * a.dim * 2; break;
-    }
-    // packed phases read what their units hold: the mean over the phases of the sweep
+    int64_t bytes = (int64_t)mat(0).bytes();
+    // packed phases read what their units hold: the mean over the phases of the sweep (one per layer, the LM head's repeated)
     std::vector<EnginePhase> hp(s->n_phases);
     CU(cudaMemcpy(hp.data(), s->d_phases, hp.size() * sizeof(EnginePhase), cudaMemcpyDeviceToHost));
     if (!hp.empty() && hp[0].Wp) {
       int64_t sum = 0;
-      for (int i = 0; i < s->n_phases; i++) {
-        const lnb_model::WPack& wp = (kind == 4) ? m->wp_out : m->wp_w13[i];
-        sum += hp[i].Wp ? wp.read_bytes : bytes;
-      }
+      for (int i = 0; i < s->n_phases; i++) sum += hp[i].Wp ? mat(i).pack.read_bytes : bytes;
       bytes = sum / s->n_phases;
     }
     if (ms_per_launch) *ms_per_launch = ms / (float)n;
@@ -3655,37 +3645,37 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
     const int nl = (kind == 4) ? 4 : a.n_layers;  // the LM head is one 1 GB matrix: repeat it
     for (int l = 0; l < nl && !rc; l++) {
       LayerW& W = m->layers[kind == 4 ? 0 : l];
+      const Linear& w = mat(l);
       GemvParams p{};
       p.eps = a.norm_eps;
       p.rscale = (s->mode == LNB_ACC_STRICT) ? s->rs : nullptr;
-      const uint8_t* ws = kind == 0 ? W.sqkv : kind == 1 ? W.so : kind == 2 ? W.s13 : kind == 3 ? W.s2 : m->output_s;
       switch (kind) {
         case 0:
-          p.W = W.wqkv; p.N = m->q_l + 2 * m->kv_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm;
+          p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm;
           p.out_bf16 = s->q; p.ldo = m->q_l; p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
           p.cache_k = s->ck[l]; p.cache_v = s->cv[l]; p.cis = m->cis; p.pos_ptr = &s->st->pos;
-          rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, s->mode, p, 1, 0, ws, m->wfmt);
+          rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, s->mode, p, w, 1);
           break;
         case 1:
-          p.W = W.wo; p.N = a.dim; p.K = m->q_l; p.x = s->o; p.ldx = m->q_l; p.ldo = a.dim; p.out_bf16 = s->h1; p.res = s->x;
-          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1, 0, ws, m->wfmt);
+          p.x = s->o; p.ldx = m->q_l; p.ldo = a.dim; p.out_bf16 = s->h1; p.res = s->x;
+          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, w, 1);
           break;
         case 2:
-          p.W = W.w13; p.N = 2 * m->ffn_l; p.K = a.dim; p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm;
+          p.x = s->h1; p.ldx = a.dim; p.norm_w = W.ffn_norm;
           p.out_bf16 = s->mbuf; p.ldo = m->ffn_l; p.silu_tab = m->silu_tab;
-          rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, s->mode, p, 1, 0, ws, m->wfmt);
+          rc = launch_gemv<PRO_RMSNORM, EPI_SWIGLU>(L, s->mode, p, w, 1);
           break;
         case 3:
-          p.W = W.w2; p.N = a.dim; p.K = m->ffn_l; p.x = s->mbuf; p.ldx = m->ffn_l; p.ldo = a.dim; p.out_bf16 = s->h1; p.res = s->x;
-          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, 1, 0, ws, m->wfmt);
+          p.x = s->mbuf; p.ldx = m->ffn_l; p.ldo = a.dim; p.out_bf16 = s->h1; p.res = s->x;
+          rc = launch_gemv<PRO_PLAIN, EPI_RESID>(L, s->mode, p, w, 1);
           break;
         case 4:
-          p.W = m->output; p.N = m->vocab_l; p.K = a.dim; p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.ldo = m->vocab_l;
+          p.x = s->x; p.ldx = a.dim; p.norm_w = m->norm; p.ldo = m->vocab_l;
           p.st = nullptr; p.argmax_row = -1;
-          rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, 1, 0, ws, m->wfmt);
+          rc = launch_gemv<PRO_RMSNORM, EPI_LOGITS>(L, s->mode, p, w, 1);
           break;
       }
-      bytes = (int64_t)mat_bytes(m->wfmt, p.N, p.K);
+      bytes = (int64_t)w.bytes();
       n_launch++;
     }
     return rc;
@@ -3936,10 +3926,11 @@ extern "C" int lnb_op_linear_bf16(const uint16_t* x, const uint16_t* w, uint16_t
   } else {
     OPBUF(dwp, wb);
     retile_kernel<<<grid_for((int64_t)N * K / 8), 256>>>(dw.as<uint16_t>(), K, 0, 0, N, K, dwp.as<uint16_t>(), 0, 1);
+    const Linear w_panels{dwp.p, nullptr, LNB_WEIGHTS_BF16, N, K};
     GemvParams p{};
-    p.W = dwp.as<uint16_t>(); p.N = N; p.K = K; p.x = dx.as<uint16_t>(); p.ldx = K; p.out_bf16 = dout.as<uint16_t>(); p.ldo = N;
+    p.x = dx.as<uint16_t>(); p.ldx = K; p.out_bf16 = dout.as<uint16_t>(); p.ldo = N;
     Launcher L{nullptr, LAUNCH_PLAIN, nullptr};
-    int rc = launch_gemv<PRO_PLAIN, EPI_BF16>(L, acc_mode, p, S);
+    int rc = launch_gemv<PRO_PLAIN, EPI_BF16>(L, acc_mode, p, w_panels, S);
     if (rc) return rc;
     rc = op_finish();
     if (rc) return rc;
