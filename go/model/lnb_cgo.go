@@ -112,6 +112,14 @@ func newDeviceSession(dm *deviceModel, inferenceArgs common.InferenceArgs, maxRo
 	return ds, lnbErr(C.lnb_session_create(dm.h, C.int(inferenceArgs.SequenceLength), C.int(maxRows), C.int(accMode), &ds.h))
 }
 
+// newDeviceSessionKV: newDeviceSession with n_seq sequences and the KV cache in format kvFormat (C.LNB_KV_BF16 or
+// C.LNB_KV_MXFP8, lnb_session_create_kv)
+func newDeviceSessionKV(dm *deviceModel, inferenceArgs common.InferenceArgs, nSeq, maxRows, accMode, kvFormat int) (*deviceSession, error) {
+	ds := &deviceSession{}
+	return ds, lnbErr(C.lnb_session_create_kv(dm.h, C.int(inferenceArgs.SequenceLength), C.int(nSeq), C.int(maxRows), C.int(accMode),
+		C.int(kvFormat), &ds.h))
+}
+
 // deviceLogits is what Forward returns when the logits stay in HBM (lnb_forward_device): ml.Tensor carries it instead of
 // S x vocab floats; Slice keeps it and ml.Argmax on such a tensor calls argmaxRows (4 bytes per row over PCIe), anything
 // that touches RawData calls read.  Valid until the session's next forward.

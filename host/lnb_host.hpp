@@ -405,6 +405,12 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
         maxRows_(std::max(maxRows, nSeq)) {
     check(lnb_session_create_batch(t.handle(), SequenceLength, nSeq, maxRows, accMode, &h_));
   }
+  // the same with the KV cache in format kvFormat (LNB_KV_BF16 or LNB_KV_MXFP8, lnb_session_create_kv; nSeq 1..8)
+  InferenceContext(LlamaTransformer& t, int sequenceLength, int accMode, int maxRows, int nSeq, int kvFormat)
+      : SequenceLength(sequenceLength > 0 ? sequenceLength : t.args.max_seq_len), vocab_(t.args.vocab_size),
+        maxRows_(nSeq > 1 ? std::max(maxRows, nSeq) : maxRows) {
+    check(lnb_session_create_kv(t.handle(), SequenceLength, nSeq, maxRows, accMode, kvFormat, &h_));
+  }
   ~InferenceContext() { lnb_session_destroy(h_); }
   void SetActiveSequence(int seq) { check(lnb_session_set_active_sequence(h_, seq)); }
   // sequence seq samples its next tokens with *a (nullptr or Temperature 0: greedy); the token outputs below then carry them

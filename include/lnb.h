@@ -255,6 +255,33 @@ int lnb_forward(lnb_session* s, const int32_t* tokens, int S, int start_pos,
  * caches from HBM.  n_seq * seq_len positions of caches must fit the GPU, or creation is LNB_ENOMEM. */
 int lnb_session_create_batch(lnb_model* m, int seq_len, int n_seq, int max_rows, int acc_mode, lnb_session** out);
 int lnb_session_set_active_sequence(lnb_session* s, int seq);
+
+/* MXFP8 KV cache (DESIGN §9j).  lnb_session_create_kv with LNB_KV_BF16 is lnb_session_create (n_seq 1) or
+ * lnb_session_create_batch (n_seq 2..8).  With LNB_KV_MXFP8 every K row (after RoPE and its bf16 truncation) and V row the
+ * session stores (the rows SetSlice stores, llamatransformer.go:402-403) is kept as 8-bit blocks: 32 consecutive elements
+ * of one KV head's row (the last block of a head head_dim % 32 wide when that is nonzero) share one E8M0 scale X + 127
+ * with X = floor(log2(max |finite element|)) - 8 clamped to [-117, 119] (-117 for a zero block); each element is the E4M3
+ * code of e * 2^-X, round to nearest even, saturated to 448.  A NaN element stores the NaN code 0x7f and reads back as NaN;
+ * +-inf saturates to +-448 * 2^X.  Every finite d = e4m3(code) * 2^X is a bf16 value, and attention reads d for every key,
+ * the rows the current call wrote included: every call returns the bits the bf16 session returns when each cache row is
+ * replaced by its d.  A position takes 2 * n_layers * (kv_l + 4 * n_kv rounded up to 16) bytes (8B: 2 112 per layer, bf16
+ * 4 096); LNB_ENOMEM gives the bytes of this size.
+ * Routing: every attention row of an MXFP8 session runs on the streamed kernels (S = 1 steps, prompts, chunked prefill,
+ * batched, ragged and speculative rows, and FAST prompts of >= 32 rows, whose projections stay on the tensor cores); a
+ * layer launches one more kernel (the cache writer) than the bf16 route.  The decode and batch engines read bf16 caches:
+ * lnb_session_decode_engine returns 0 with "MXFP8 KV cache: ..." in lnb_last_error (also under LNB_ENGINE=1), and every
+ * step runs the kernel chain.  lnb_session_copy_sequences copies the codes and scales; lnb_session_read(LNB_BUF_CACHE_K /
+ * _V) returns the decoded bf16 rows in the bf16 layout.
+ * LNB_EINVAL with nothing allocated: an unknown format, an MXFP8 cache on a shape the streamed kernels do not serve
+ * (head_dim > 128 or n_heads / n_kv_heads > 8) or with tp_size > 1, n_seq outside 1..8. */
+enum { LNB_KV_BF16 = 0, LNB_KV_MXFP8 = 1 };
+int lnb_session_create_kv(lnb_model* m, int seq_len, int n_seq, int max_rows, int acc_mode, int kv_format, lnb_session** out);
+/* fmt = the session's cache format; cache_bytes = the bytes its K and V caches hold in HBM.  Either may be NULL. */
+int lnb_session_kv_info(lnb_session* s, int* fmt, int64_t* cache_bytes);
+/* the raw blocks of positions [pos0, pos0 + n) of sequence seq, layer `layer`, K (which = LNB_BUF_CACHE_K) or V
+ * (LNB_BUF_CACHE_V) of an MXFP8 session: codes [n][kv_l] and scales [n][n_kv][ceil(head_dim / 32)], heads in checkpoint
+ * order (either may be NULL).  Synchronises the session's stream. */
+int lnb_session_kv_read(lnb_session* s, int seq, int layer, int which, int pos0, int n, uint8_t* codes, uint8_t* scales);
 int lnb_forward_batch(lnb_session* s, const int32_t* tokens, const int32_t* positions, int n,
                       float* logits /* NULL or [n, vocab] */,
                       int32_t* argmax_out /* [n]: next token (greedy unless the sequence samples) */);
@@ -585,6 +612,10 @@ int lnb_op_penalize_f32(const float* logits, int rows, int vocab, const lnb_pena
                         const int32_t* pos_next, float* out);
 /* ml.Fwd_Get_Rows (operations_impl.go:142-173) */
 int lnb_op_get_rows_bf16(const uint16_t* emb, const int32_t* tokens, uint16_t* out, int S, int vocab, int dim);
+/* the MXFP8 KV cache's block rule (see lnb_session_create_kv), run by the cache writer's device code on host rows
+ * [n][n_kv * head_dim] bf16 (head_dim a multiple of 8, at most 128): codes [n][n_kv * head_dim], scales
+ * [n][n_kv][ceil(head_dim / 32)] and the decoded rows deq [n][n_kv * head_dim] bf16 (deq may be NULL) */
+int lnb_op_kv_quantize_bf16(const uint16_t* rows, int n, int head_dim, int n_kv, uint8_t* codes, uint8_t* scales, uint16_t* deq);
 
 #ifdef __cplusplus
 }

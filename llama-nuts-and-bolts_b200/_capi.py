@@ -11,6 +11,7 @@ LNB_ACC_STRICT, LNB_ACC_FAST = 0, 1
 LNB_BUF_RESIDUAL, LNB_BUF_CACHE_K, LNB_BUF_CACHE_V, LNB_BUF_LOGITS = 0, 1, 2, 3
 LNB_BUF_Q, LNB_BUF_ATTN, LNB_BUF_POST_ATTN, LNB_BUF_NORMED, LNB_BUF_FFN = 4, 5, 6, 7, 8
 LNB_WEIGHTS_BF16, LNB_WEIGHTS_MXFP8, LNB_WEIGHTS_MXFP4 = 0, 1, 2
+LNB_KV_BF16, LNB_KV_MXFP8 = 0, 1
 
 
 class LnbError(RuntimeError):
@@ -87,6 +88,9 @@ SIGNATURES = {
     "lnb_decode_run": (C.c_int, [vp, C.c_int32, C.c_int, C.c_int, C.c_int, i32p, f32p]),
     "lnb_session_create_batch": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
     "lnb_session_set_active_sequence": (C.c_int, [vp, C.c_int]),
+    "lnb_session_create_kv": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp)]),
+    "lnb_session_kv_info": (C.c_int, [vp, C.POINTER(C.c_int), i64p]),
+    "lnb_session_kv_read": (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     "lnb_forward_batch": (C.c_int, [vp, i32p, i32p, C.c_int, f32p, i32p]),
     "lnb_session_p2p_export": (C.c_int, [vp, vp]),
     "lnb_session_p2p_import": (C.c_int, [vp, vp, C.c_int]),
@@ -151,6 +155,7 @@ SIGNATURES = {
     "lnb_op_logprobs_f32": (C.c_int, [f32p, C.c_int, C.c_int, i32p, C.c_int, vp]),
     "lnb_op_penalize_f32": (C.c_int, [f32p, C.c_int, C.c_int, C.POINTER(PenaltiesC), i32p, C.c_int, i32p, f32p]),
     "lnb_op_get_rows_bf16": (C.c_int, [u16p, i32p, u16p, C.c_int, C.c_int, C.c_int]),
+    "lnb_op_kv_quantize_bf16": (C.c_int, [u16p, C.c_int, C.c_int, C.c_int, vp, vp, u16p]),
 }
 
 if not os.path.exists(LIB_PATH):

@@ -29,6 +29,7 @@
 #include "penalty.cuh"
 #include "grammar.cuh"
 #include "seqcopy.cuh"
+#include "kvcache.cuh"
 #include "pth.hpp"
 #include "tokenizer.hpp"
 #include "regex.hpp"
@@ -1070,23 +1071,26 @@ static void ss_plan(SsScratch& x, int T, int max_rows, int n_heads, int hd, size
 }
 // STRICT output chains: the d-range of one CTA (more CTAs per KV head; each chain still runs t = 0..p in order)
 static int ss_dsplit(int hd) { return hd % 32 == 0 ? 4 : hd % 16 == 0 ? 2 : 1; }
-// all `rows` rows of P (P.q, P.out, positions and caches set by the caller)
+// all `rows` rows of P (P.q, P.out, positions and caches set by the caller) over a cache of format KVF
+template <int KVF>
 static int launch_stream_attn(const Launcher& L, StreamAttn P, int rows, int n_kv, const SsScratch& x) {
   const int dsplit = P.strict ? ss_dsplit(P.hd) : 1;
-  const size_t s_scores = ss_scores_smem(P.hd, P.n_rep), s_out = ss_out_smem(P.hd, P.n_rep, dsplit);
+  const size_t s_scores = ss_scores_smem(P.hd, P.n_rep, KVF), s_out = ss_out_smem(P.hd, P.n_rep, dsplit, KVF);
   // the largest shape ss_shape_ok admits (head_dim 128, n_rep 8, FAST); the kernel's static shared memory comes on top
-  if (int rc = smem_opt_in<ss_out_kernel>((int)ss_out_smem(128, 8, 1))) return rc;
+  if (int rc = smem_opt_in<ss_out_kernel<KVF>>((int)ss_out_smem(128, 8, 1, KVF))) return rc;
+  if (KVF == KVF_MXFP8)
+    if (int rc = smem_opt_in<ss_scores_kernel<KVF>>((int)ss_scores_smem(128, 8, KVF))) return rc;
   P.sc = x.sc; P.zpart = x.z; P.opart = x.op; P.t_stride = x.t_stride; P.n_chunks = x.n_chunks;
   for (int r0 = 0; r0 < rows; r0 += x.rows) {
     const int n = std::min(x.rows, rows - r0);
     P.row0 = r0;
     int rc;
-    if ((rc = launch_kernel(L, ss_scores_kernel, dim3(n_kv, n, x.n_chunks), dim3(SS_KT), s_scores, P))) return rc;
+    if ((rc = launch_kernel(L, ss_scores_kernel<KVF>, dim3(n_kv, n, x.n_chunks), dim3(SS_KT), s_scores, P))) return rc;
     if (P.strict) {
       if ((rc = launch_kernel(L, ss_zsum_kernel, dim3(P.n_heads, n), dim3(128), 0, P))) return rc;
-      if ((rc = launch_kernel(L, ss_out_kernel, dim3(n_kv * dsplit, n), dim3(P.n_rep * P.hd / dsplit), s_out, P, dsplit))) return rc;
+      if ((rc = launch_kernel(L, ss_out_kernel<KVF>, dim3(n_kv * dsplit, n), dim3(P.n_rep * P.hd / dsplit), s_out, P, dsplit))) return rc;
     } else {
-      if ((rc = launch_kernel(L, ss_out_kernel, dim3(n_kv, n, x.n_chunks), dim3(P.n_rep * P.hd), s_out, P, 1))) return rc;
+      if ((rc = launch_kernel(L, ss_out_kernel<KVF>, dim3(n_kv, n, x.n_chunks), dim3(P.n_rep * P.hd), s_out, P, 1))) return rc;
       if ((rc = launch_kernel(L, ss_combine_kernel, dim3(P.n_heads, n), dim3(P.hd), 0, P))) return rc;
     }
   }
@@ -1347,6 +1351,10 @@ struct lnb_session {
   size_t logits_rows = 0;
   float* logits_full = nullptr;  // tp>1: gathered [rows, vocab]
   std::vector<uint16_t*> ck, cv;
+  // cache format (lnb_session_create_kv): LNB_KV_BF16, or LNB_KV_MXFP8 with ck / cv holding the records of kvcache.cuh;
+  // kv_pos: cache elements per position (bf16: kv_l values; MXFP8: the record's bytes)
+  int kv_fmt = LNB_KV_BF16;
+  int kv_pos = 0;
   LnbDevState* st = nullptr;
   int32_t* d_tok_out = nullptr;
   // pinned staging, one allocation (at h_tok) carved into two views: a call's token ids or row map on their way to d_rag
@@ -1478,16 +1486,27 @@ static unsigned long long p2p_timeout_ns() {
   return ms > 0 ? (unsigned long long)ms * 1000000ull : 0ull;
 }
 
-static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, lnb_session** out);
+static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, int kv_fmt, lnb_session** out);
 extern "C" int lnb_session_create(lnb_model* m, int seq_len, int max_rows, int acc_mode, lnb_session** out) {
-  return session_create_impl(m, seq_len, max_rows, acc_mode, 1, out);
+  return session_create_impl(m, seq_len, max_rows, acc_mode, 1, LNB_KV_BF16, out);
 }
 extern "C" int lnb_session_create_batch(lnb_model* m, int seq_len, int n_seq, int max_rows, int acc_mode, lnb_session** out) {
   if (n_seq < 1 || n_seq > 8) return fail(LNB_EINVAL, "n_seq must be 1..8");
-  return session_create_impl(m, seq_len, max_rows < n_seq ? n_seq : max_rows, acc_mode, n_seq, out);
+  return session_create_impl(m, seq_len, max_rows < n_seq ? n_seq : max_rows, acc_mode, n_seq, LNB_KV_BF16, out);
 }
-static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, lnb_session** out) {
+extern "C" int lnb_session_create_kv(lnb_model* m, int seq_len, int n_seq, int max_rows, int acc_mode, int kv_format, lnb_session** out) {
+  if (n_seq < 1 || n_seq > 8) return fail(LNB_EINVAL, "n_seq must be 1..8");
+  if (n_seq == 1) return session_create_impl(m, seq_len, max_rows, acc_mode, 1, kv_format, out);
+  return session_create_impl(m, seq_len, max_rows < n_seq ? n_seq : max_rows, acc_mode, n_seq, kv_format, out);
+}
+static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, int kv_fmt, lnb_session** out) {
   if (!m || !out) return fail(LNB_EINVAL, "NULL argument");
+  if (kv_fmt != LNB_KV_BF16 && kv_fmt != LNB_KV_MXFP8) return fail(LNB_EINVAL, "unknown KV cache format %d", kv_fmt);
+  const bool kv_mx = kv_fmt == LNB_KV_MXFP8;
+  if (kv_mx && !ss_shape_ok(m->a.head_dim, m->a.n_heads / m->a.n_kv_heads))
+    return fail(LNB_EINVAL, "MXFP8 KV cache: attention runs on the streamed kernels, which serve head_dim <= 128 and n_rep <= 8 "
+                "(head_dim %d, n_rep %d)", m->a.head_dim, m->a.n_heads / m->a.n_kv_heads);
+  if (kv_mx && m->tp_size > 1) return fail(LNB_EINVAL, "MXFP8 KV cache: not built for tensor parallelism (tp_size %d)", m->tp_size);
   if (!m->finalized) return fail(LNB_ESTATE, "model is not finalized");
   if (seq_len <= 0 || max_rows <= 0) return fail(LNB_EINVAL, "seq_len and max_rows must be positive");
   if (seq_len > m->cis_rows) return fail(LNB_EINVAL, "seq_len %d exceeds the RoPE table (%d rows)", seq_len, m->cis_rows);
@@ -1517,14 +1536,16 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
     }
   }
   s->stream_attn = stream_attn;
+  s->kv_fmt = kv_fmt;
+  s->kv_pos = kv_mx ? kv_row_bytes(m->kv_l, m->kv_l / a.head_dim) : m->kv_l;
   s->samp_rows = n_seq;
   s->lp_rows = std::max(max_rows, 8);
   cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
   AllocBatch A;
-  if (stream_attn || (!s->sdpa_smem_decode && ss_shape_ok(a.head_dim, a.n_heads / a.n_kv_heads))) {
-    // streamed rows: every row of a long session, or the n_seq rows of a batched step
+  if (stream_attn || kv_mx || (!s->sdpa_smem_decode && ss_shape_ok(a.head_dim, a.n_heads / a.n_kv_heads))) {
+    // streamed rows: every row of a long session or of an MXFP8-cache session, or the n_seq rows of a batched step
     size_t sc_b, z_b, op_b;
-    ss_plan(s->ss, seq_len, stream_attn ? max_rows : n_seq, m->q_l / a.head_dim, a.head_dim, &sc_b, &z_b, &op_b);
+    ss_plan(s->ss, seq_len, stream_attn || kv_mx ? max_rows : n_seq, m->q_l / a.head_dim, a.head_dim, &sc_b, &z_b, &op_b);
     A.add(&s->ss.sc, sc_b);
     A.add(&s->ss.z, z_b);
     A.add(&s->ss.op, op_b);
@@ -1548,6 +1569,8 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
       if (x.lin->fmt != LNB_WEIGHTS_BF16)
         s->wdq_elems = std::max(s->wdq_elems, x.layer < 0 ? (size_t)TC_BN * x.lin->K : (size_t)x.lin->N * x.lin->K);
     if (s->wdq_elems) A.add(&s->wdq, s->wdq_elems * 2);
+  } else if (kv_mx) {
+    A.add(&s->qkv_raw, (size_t)max_rows * (m->q_l + 2 * m->kv_l) * 2);   // the projection rows the cache writer reads
   }
   const size_t in_words = row_map_words(max_rows);
   A.add(&s->d_rag, in_words * 4);
@@ -1555,7 +1578,7 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
   A.add(&s->d_tok_out, (size_t)seq_len * 4);
   s->ck.assign(a.n_layers, nullptr);
   s->cv.assign(a.n_layers, nullptr);
-  const size_t cbytes = (size_t)n_seq * seq_len * m->kv_l * 2;
+  const size_t cbytes = (size_t)n_seq * seq_len * (kv_mx ? (size_t)s->kv_pos : (size_t)m->kv_l * 2);
   A.add(&s->d_next_arr, 8 * 4);
   for (int l = 0; l < a.n_layers; l++) {
     A.add(&s->ck[l], cbytes, 0);  // ml.Zeros, inferencecontext.go:31-43
@@ -1779,6 +1802,7 @@ static bool engine_probe(lnb_session* s) {
   // FAST sessions; LNB_ENGINE=1 / 0 forces it on / off.
   const char* e = getenv("LNB_ENGINE");
   if (e && !strcmp(e, "0")) return no("LNB_ENGINE=0");
+  if (s->kv_fmt == LNB_KV_MXFP8) return no("MXFP8 KV cache: the decode and batch engines read bf16 caches");
   if (m->output.fmt != LNB_WEIGHTS_BF16)   // every linear matrix has the same format
     return no(std::string(wfmt_name(m->output.fmt)) + " weights: the decode and batch engines stream bf16 panels");
   // single-sequence steps of single-GPU FAST sessions stay on the kernel chain by default (the batch engine does not care)
@@ -2283,7 +2307,7 @@ struct Rows {
 static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int logits_rows, bool advance, bool gather) {
   Rows R{};
   R.kind = ROWS_SINGLE; R.S = S; R.tokens = tokens;
-  R.cache_off = (size_t)s->active_seq * s->seq_len * s->m->kv_l;
+  R.cache_off = (size_t)s->active_seq * s->seq_len * s->kv_pos;
   R.head = logits_rows == 0 ? HEAD_NONE : logits_rows == 1 ? HEAD_LAST : HEAD_ALL;
   R.head_rows = logits_rows > 1 ? S : 1;
   R.advance = advance; R.gather = gather;
@@ -2295,7 +2319,7 @@ static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int 
 static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, const CtlSum& u) {
   Rows R{};
   R.kind = ROWS_RAGGED; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
-  R.seq_stride = (long long)s->seq_len * s->m->kv_l;
+  R.seq_stride = (long long)s->seq_len * s->kv_pos;
   R.mb_rows = 8;
   R.seg_last = s->d_rag + 3 * rows;
   R.head = HEAD_PER_ROW; R.head_rows = n_segs;
@@ -2308,10 +2332,21 @@ static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, const CtlSum
 static Rows rows_spec(const lnb_session* s, int rows, const CtlSum& u) {
   Rows R{};
   R.kind = ROWS_SPEC; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
-  R.seq_stride = (long long)s->seq_len * s->m->kv_l;
+  R.seq_stride = (long long)s->seq_len * s->kv_pos;
   R.head = HEAD_PER_ROW; R.head_rows = rows;
   R.record = u.pen; R.grammar = u.gram;
   return R;
+}
+
+// MXFP8 cache writer of layer l for the rows R: q and k rotated from the projection rows in qkv_raw, q to s->q, k and v
+// quantized into their records (kvcache.cuh)
+static int launch_kv_writer(const Launcher& L, lnb_session* s, int l, const Rows& R) {
+  const lnb_model* m = s->m;
+  const int hd = m->a.head_dim, tasks = R.S * 2 * (m->kv_l / hd) * ((hd + 31) / 32);
+  const int grid = std::min(m->sm_count * 8, std::max((tasks + 7) / 8, (R.S * m->q_l / 2 + 255) / 256));
+  return launch_kernel(L, kvq_rope_store_kernel, dim3(grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, m->q_l + 2 * m->kv_l, s->q,
+                       m->q_l, m->kv_l, hd, (uint8_t*)s->ck[l] + R.cache_off, (uint8_t*)s->cv[l] + R.cache_off, (const float*)m->cis,
+                       (const int32_t*)&s->st->pos, R.S, R.pos_arr, R.row_seq, R.seq_stride);
 }
 
 // Attention of layer l for the rows R (queries in s->q), written to out: plain rows, or the X8 operand of the tensor-core
@@ -2321,7 +2356,10 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
   const lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   const int S = R.S, n_rep = a.n_heads / a.n_kv_heads, n_q = m->q_l / a.head_dim, n_kv = m->kv_l / a.head_dim;
-  const uint16_t *ck = s->ck[l] + R.cache_off, *cv = s->cv[l] + R.cache_off;
+  const bool kv_mx = s->kv_fmt == LNB_KV_MXFP8;
+  // MXFP8: R.cache_off counts bytes
+  const uint16_t *ck = kv_mx ? (const uint16_t*)((const uint8_t*)s->ck[l] + R.cache_off) : s->ck[l] + R.cache_off;
+  const uint16_t *cv = kv_mx ? (const uint16_t*)((const uint8_t*)s->cv[l] + R.cache_off) : s->cv[l] + R.cache_off;
   const int32_t* pos_ptr = &s->st->pos;
   const float scale = attn_scale_bf16(a.head_dim);
   const int strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
@@ -2331,15 +2369,16 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
   auto streamed = [&]() {
     StreamAttn P{};
     P.q = s->q; P.ldq = m->q_l;
-    P.cache_k = ck; P.cache_v = cv; P.kv_dim = m->kv_l;
+    P.cache_k = ck; P.cache_v = cv; P.kv_dim = s->kv_pos;
     P.row_cache_stride = R.seq_stride; P.row_seq = R.row_seq; P.pos_arr = R.pos_arr;
     P.n_rep = n_rep; P.hd = a.head_dim; P.n_heads = n_q;
     P.pos_ptr = pos_ptr; P.pos_step = 1;
     P.out = out; P.ldo = m->q_l; P.out_x8 = out_x8;
     P.scale = scale; P.strict = strict;
-    return launch_stream_attn(L, P, S, n_kv, s->ss);
+    if (kv_mx) return launch_stream_attn<KVF_MXFP8>(L, P, S, n_kv, s->ss);
+    return launch_stream_attn<KVF_BF16>(L, P, S, n_kv, s->ss);
   };
-  if (R.kind == ROWS_RAGGED) return streamed();
+  if (R.kind == ROWS_RAGGED || kv_mx) return streamed();
   if (!out_x8 && (S == 1 || spec) && s->sdpa_smem_decode)
     return launch_kernel(L, sdpa_decode_kernel, dim3(n_kv, S), dim3(128 * n_rep), s->sdpa_decode_smem, (const uint16_t*)s->q, ck, cv,
                          m->kv_l, n_rep, a.head_dim, out, pos_ptr, s->seq_len, strict, scale, R.pos_arr,
@@ -2463,9 +2502,15 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
       p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm; p.eps = a.norm_eps;
       p.out_bf16 = s->q; p.ldo = m->q_l;
       p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
-      p.cache_k = s->ck[l] + R.cache_off; p.cache_v = s->cv[l] + R.cache_off; p.cis = m->cis; p.pos_ptr = &s->st->pos;
-      p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = R.seq_stride;
-      if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, W.qkv, S, mb_rows))) return rc;
+      if (s->kv_fmt == LNB_KV_MXFP8) {   // the projection's bf16 rows, then RoPE and the cache writer (kvcache.cuh)
+        p.out_bf16 = s->qkv_raw; p.ldo = W.qkv.N;
+        if ((rc = launch_gemv<PRO_RMSNORM, EPI_BF16>(L, mode, p, W.qkv, S, mb_rows))) return rc;
+        if ((rc = launch_kv_writer(L, s, l, R))) return rc;
+      } else {
+        p.cache_k = s->ck[l] + R.cache_off; p.cache_v = s->cv[l] + R.cache_off; p.cis = m->cis; p.pos_ptr = &s->st->pos;
+        p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = R.seq_stride;
+        if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, W.qkv, S, mb_rows))) return rc;
+      }
     }
     if ((rc = launch_attention(L, s, l, R, s->o, 0))) return rc;
     if ((rc = proj_resid(W.o, s->o, s->x, s->h1))) return rc;      // wo + residual (:522, :232)
@@ -2549,10 +2594,11 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
       if ((rc = tc_w(g, W.qkv))) return rc;
       if ((rc = launch_gemm_tc<TC_EPI_BF16>(L, g))) return rc;
     }
-    if ((rc = launch_kernel(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
+    if (s->kv_fmt == LNB_KV_MXFP8) rc = launch_kv_writer(L, s, l, R);
+    else rc = launch_kernel(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
                             a.head_dim, s->ck[l] + R.cache_off, s->cv[l] + R.cache_off, (const float*)m->cis, (const int32_t*)&s->st->pos, S,
-                            R.pos_arr, R.row_seq, (long long)s->seq_len * m->kv_l)))
-      return rc;
+                            R.pos_arr, R.row_seq, (long long)s->seq_len * m->kv_l);
+    if (rc) return rc;
     if ((rc = launch_attention(L, s, l, R, s->o8, 1))) return rc;
     if ((rc = proj_resid(s->o8, W.o, s->x, s->h1))) return rc;
     if ((rc = launch_kernel(L, rmsnorm_x8_kernel, dim3(Mpad), dim3(256), 0, (const uint16_t*)s->h1, a.dim, (const uint16_t*)W.ffn_norm,
@@ -3262,7 +3308,9 @@ extern "C" int lnb_session_copy_sequences(lnb_session* s, int n, const int32_t* 
   if ((m->kv_l * 2) % 16) return fail(LNB_EINVAL, "cache rows of %d bytes are not a multiple of 16", m->kv_l * 2);
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(m->device));
-  const long long row16 = (long long)m->kv_l * 2 / 16, rec16 = (long long)sizeof(LpRecord) / 16, np = pos1 - pos0;
+  // (MXFP8 records are whole 16-byte vectors, kvcache.cuh)
+  const long long row16 = s->kv_fmt == LNB_KV_MXFP8 ? (long long)s->kv_pos / 16 : (long long)m->kv_l * 2 / 16;
+  const long long rec16 = (long long)sizeof(LpRecord) / 16, np = pos1 - pos0;
   SeqCopyJob J{};
   J.n = n;
   for (int i = 0; i < n; i++) { J.src[i] = src[i]; J.dst[i] = dst[i]; }
@@ -3596,6 +3644,7 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
 extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, float* ms_per_launch, int64_t* bytes_per_launch,
                                         int* launches) {
   if (!s || reps <= 0 || kind < 0 || kind > 4) return fail(LNB_EINVAL, "bad argument");
+  if (s->kv_fmt != LNB_KV_BF16) return fail(LNB_EINVAL, "MXFP8 KV cache: the projection benchmark writes bf16 cache rows");
   std::lock_guard<std::mutex> lk(s->mu);
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
@@ -3757,6 +3806,65 @@ static int read_rows(lnb_session* s, const uint16_t* src, int layout, int width,
   return 0;
 }
 
+// lnb_session_read(LNB_BUF_CACHE_K / _V) of an MXFP8 session: the first nbytes of the active sequence's rows, decoded to bf16
+// in chunks of at most kKvReadRows rows through a small device buffer
+static const int kKvReadRows = 4096;
+static int read_kv_decoded(lnb_session* s, int which, int layer, void* host, int64_t nbytes) {
+  const lnb_model* m = s->m;
+  const int64_t row_b = (int64_t)m->kv_l * 2, avail = (int64_t)s->seq_len * row_b;
+  if (nbytes < 0 || nbytes > avail) return fail(LNB_EINVAL, "buffer %d holds %lld bytes, %lld requested", which, (long long)avail, (long long)nbytes);
+  if (nbytes == 0) return 0;
+  const int64_t rows = (nbytes + row_b - 1) / row_b, chunk = std::min<int64_t>(rows, kKvReadRows);
+  CU(cudaStreamSynchronize(s->stream));
+  uint16_t* d = nullptr;
+  if (cudaMalloc((void**)&d, (size_t)(chunk * row_b)) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(LNB_ENOMEM, "cudaMalloc(%lld) for the decoded cache rows", (long long)(chunk * row_b));
+  }
+  const uint8_t* rec = (const uint8_t*)(which == LNB_BUF_CACHE_K ? s->ck[layer] : s->cv[layer]) + (size_t)s->active_seq * s->seq_len * s->kv_pos;
+  cudaError_t e = cudaSuccess;
+  for (int64_t r0 = 0; r0 < rows && e == cudaSuccess; r0 += chunk) {
+    const int64_t n = std::min(chunk, rows - r0), off = r0 * row_b;
+    kv_dequant_kernel<<<m->sm_count * 4, 256, 0, s->stream>>>(rec + (size_t)r0 * s->kv_pos, s->kv_pos, m->kv_l, m->a.head_dim, n, d);
+    e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync((uint8_t*)host + off, d, (size_t)std::min(n * row_b, nbytes - off), cudaMemcpyDeviceToHost, s->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
+  }
+  cudaFree(d);
+  if (e != cudaSuccess) return fail(LNB_ECUDA, "decoding the cache rows: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+extern "C" int lnb_session_kv_info(lnb_session* s, int* fmt, int64_t* cache_bytes) {
+  if (!s) return fail(LNB_EINVAL, "session is NULL");
+  if (fmt) *fmt = s->kv_fmt;
+  if (cache_bytes)
+    *cache_bytes = (int64_t)2 * s->m->a.n_layers * s->n_seq * s->seq_len * (s->kv_fmt == LNB_KV_MXFP8 ? s->kv_pos : s->kv_pos * 2);
+  return 0;
+}
+
+extern "C" int lnb_session_kv_read(lnb_session* s, int seq, int layer, int which, int pos0, int n, uint8_t* codes, uint8_t* scales) {
+  if (!s) return fail(LNB_EINVAL, "session is NULL");
+  const lnb_model* m = s->m;
+  if (s->kv_fmt != LNB_KV_MXFP8) return fail(LNB_EINVAL, "the session's KV cache is not MXFP8");
+  if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
+  if (layer < 0 || layer >= m->a.n_layers) return fail(LNB_EINVAL, "bad layer %d", layer);
+  if (which != LNB_BUF_CACHE_K && which != LNB_BUF_CACHE_V) return fail(LNB_EINVAL, "which must be LNB_BUF_CACHE_K or _V");
+  if (pos0 < 0 || n < 1 || pos0 + n > s->seq_len) return fail(LNB_EINVAL, "positions [%d, %d) outside [0, %d)", pos0, pos0 + n, s->seq_len);
+  CU(cudaSetDevice(m->device));
+  CU(cudaStreamSynchronize(s->stream));
+  const int n_kv = m->kv_l / m->a.head_dim, nb = (m->a.head_dim + 31) / 32, rowb = s->kv_pos;
+  const uint8_t* rec = (const uint8_t*)(which == LNB_BUF_CACHE_K ? s->ck[layer] : s->cv[layer]) + ((size_t)seq * s->seq_len + pos0) * rowb;
+  if (codes) CU(cudaMemcpy2D(codes, m->kv_l, rec, rowb, m->kv_l, n, cudaMemcpyDeviceToHost));
+  if (scales) {
+    std::vector<uint8_t> slots((size_t)n * n_kv * 4);
+    CU(cudaMemcpy2D(slots.data(), (size_t)n_kv * 4, rec + m->kv_l, rowb, (size_t)n_kv * 4, n, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < (size_t)n * n_kv; i++)
+      for (int b = 0; b < nb; b++) scales[i * nb + b] = slots[i * 4 + b];
+  }
+  return 0;
+}
+
 extern "C" int lnb_session_read(lnb_session* s, int which, int layer, void* host, int64_t nbytes) {
   if (!s || !host) return fail(LNB_EINVAL, "NULL argument");
   lnb_model* m = s->m;
@@ -3817,6 +3925,7 @@ extern "C" int lnb_session_read(lnb_session* s, int which, int layer, void* host
     case LNB_BUF_CACHE_K:
     case LNB_BUF_CACHE_V:
       if (layer < 0 || layer >= m->a.n_layers) return fail(LNB_EINVAL, "bad layer %d", layer);
+      if (s->kv_fmt == LNB_KV_MXFP8) return read_kv_decoded(s, which, layer, host, nbytes);
       src = (which == LNB_BUF_CACHE_K ? s->ck[layer] : s->cv[layer]) + (size_t)s->active_seq * s->seq_len * m->kv_l;
       avail = (int64_t)s->seq_len * m->kv_l * 2;
       break;
@@ -4067,7 +4176,7 @@ extern "C" int lnb_op_attention_bf16(const uint16_t* q, const uint16_t* cache_k,
     P.out = dout.as<uint16_t>(); P.ldo = n_heads * hd;
     P.scale = f;
     P.strict = acc_mode == LNB_ACC_STRICT ? 1 : 0;
-    int rc2 = launch_stream_attn(Launcher{nullptr, LAUNCH_PLAIN, nullptr}, P, S, n_kv, x);
+    int rc2 = launch_stream_attn<KVF_BF16>(Launcher{nullptr, LAUNCH_PLAIN, nullptr}, P, S, n_kv, x);
     if (!rc2) rc2 = op_finish();
     if (rc2) return rc2;
     D2H(out, dout, qb);
@@ -4120,6 +4229,22 @@ static int silu_table_device(uint16_t** out) {
     tab_dev = dev;
   }
   *out = tab;
+  return 0;
+}
+
+extern "C" int lnb_op_kv_quantize_bf16(const uint16_t* rows, int n, int head_dim, int n_kv, uint8_t* codes, uint8_t* scales, uint16_t* deq) {
+  OpScope scope_;
+  if (!rows || !codes || !scales) return fail(LNB_EINVAL, "NULL argument");
+  if (n < 1 || n_kv < 1 || head_dim < 8 || head_dim > 128 || head_dim % 8) return fail(LNB_EINVAL, "bad shape n %d head_dim %d n_kv %d", n, head_dim, n_kv);
+  const int nb = (head_dim + 31) / 32;
+  const size_t e = (size_t)n * n_kv * head_dim, sb = (size_t)n * n_kv * nb;
+  OPBUF(dx, e * 2); OPBUF(dc, e); OPBUF(ds, sb); OPBUF(dd, e * 2);
+  H2D(dx, rows, e * 2);
+  kvq_rows_kernel<<<grid_for((int64_t)n * n_kv * nb * 32), 256>>>(dx.as<uint16_t>(), n, head_dim, n_kv, dc.as<uint8_t>(), ds.as<uint8_t>(),
+                                                                  dd.as<uint16_t>());
+  if (int rc = op_finish()) return rc;
+  D2H(codes, dc, e); D2H(scales, ds, sb);
+  if (deq) D2H(deq, dd, e * 2);
   return 0;
 }
 

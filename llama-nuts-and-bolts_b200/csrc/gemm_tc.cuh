@@ -230,6 +230,13 @@ __global__ void __launch_bounds__(256) rmsnorm_x8_kernel(const uint16_t* __restr
   }
 }
 
+// RoPE of one pair: w holds columns (2i, 2i+1) as bf16 (low half first), fc = cis[pos][i]; the rotated pair, same packing
+// (the MXFP8 cache writer, kvcache.cuh, rotates its K rows with it too)
+LNB_DEVINL uint32_t rope_pair(uint32_t w, float2 fc) {
+  const double a = (double)bf_lo(w), b = (double)bf_hi(w), c = (double)fc.x, d = (double)fc.y;
+  return (uint32_t)f2bf((float)(a * c - b * d)) | ((uint32_t)f2bf((float)(a * d + b * c)) << 16);
+}
+
 // After the fused wq|wk|wv GEMM of the prefill path: RoPE on q and k (f64 intermediates, see
 // gemv.cuh EPI_QKV_ROPE), q -> q_out [S, q_dim], k -> cacheK[pos0+s], v -> cacheV[pos0+s]
 // (llamatransformer.go:374-403).  One thread per (row, pair of columns).  Ragged calls (rows of several sequences):
@@ -252,8 +259,7 @@ __global__ void rope_kv_kernel(const uint16_t* __restrict__ qkv, int ld, uint16_
       const int nn = (n < q_dim) ? n : n - q_dim;
       const int ii = (nn % head_dim) >> 1;
       const float2 fc = *reinterpret_cast<const float2*>(cis + ((size_t)pos * (head_dim / 2) + ii) * 2);
-      const double a = (double)bf_lo(w), b = (double)bf_hi(w), c = (double)fc.x, d = (double)fc.y;
-      const uint32_t o = (uint32_t)f2bf((float)(a * c - b * d)) | ((uint32_t)f2bf((float)(a * d + b * c)) << 16);
+      const uint32_t o = rope_pair(w, fc);
       if (n < q_dim) *reinterpret_cast<uint32_t*>(q_out + (size_t)s * q_dim + n) = o;
       else *reinterpret_cast<uint32_t*>(cache_k + cb + (size_t)pos * kv_dim + nn) = o;
     } else {

@@ -49,6 +49,13 @@ LNB_DEVINL uint32_t e4m3x2(float hi, float lo) {
   asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
   return r;
 }
+// The block rule shared by the weight quantizer and the KV cache writer (kvcache.cuh): X from the largest bf16 magnitude
+// field amax (bits & 0x7fff) of the block, and 2^-X, the factor each element is multiplied by before e4m3x2
+LNB_DEVINL int mx_block_x(uint32_t amax) {
+  const int E = (int)(amax >> 7);                                   // bf16 exponent field of amax (0: zero or subnormal)
+  return E == 0 ? -117 : max(-117, min(119, E - 127 - 8));
+}
+LNB_DEVINL float mx_inv_scale(int X) { return __uint_as_float((uint32_t)(127 - X) << 23); }   // X in [-117, 119]: normal
 
 // One pass over a bf16 panel-major matrix W[N, K]: one thread per (panel, block, row).  Writes the codes and scales
 // above; a non-finite weight lowers *flag (preset to ~0) to row * K + col of the first one, in the matrix's row order.
@@ -78,10 +85,9 @@ __global__ void mxfp8_quantize_kernel(const uint16_t* __restrict__ W, int N, int
           amax = max(amax, mag);
         }
     }
-    const int E = (int)(amax >> 7);                                   // bf16 exponent field of amax (0: zero or subnormal)
-    const int X = E == 0 ? -117 : max(-117, min(119, E - 127 - 8));
+    const int X = mx_block_x(amax);
     scales[(p * nbp + b) * 8 + r] = (uint8_t)(X + 127);
-    const float inv = __uint_as_float((uint32_t)(127 - X) << 23);     // 2^-X, X in [-117, 119]: a normal f32
+    const float inv = mx_inv_scale(X);
 #pragma unroll
     for (int q = 0; q < 4; q++) {
       if (q >= nc) break;

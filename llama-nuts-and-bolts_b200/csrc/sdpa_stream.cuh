@@ -22,8 +22,12 @@
 // So STRICT is bit-identical to sdpa_kernel's strict form; FAST has the order above (DESIGN §3).  No float atomics.
 // PDL: every kernel waits (griddepcontrol.wait) before its first global access, so nothing is read or written while an
 // earlier kernel of the stream may still run.
+// MXFP8 caches (KVF = KVF_MXFP8, kvcache.cuh): ss_scores_kernel and ss_out_kernel copy each tile's codes (8-byte pieces)
+// and its keys' 4-byte scale slots with cp.async, decode them into the bf16 tile the bf16 form copies, and then run the
+// bf16 form's arithmetic unchanged.  cache_k / cache_v then point at the records, kv_dim is the record's byte size and
+// row_cache_stride counts bytes.
 #pragma once
-#include "gemm_tc.cuh"
+#include "kvcache.cuh"
 
 namespace lnb {
 
@@ -77,9 +81,39 @@ LNB_DEVINL void ss_cp_commit() { asm volatile("cp.async.commit_group;" ::: "memo
 template <int N>
 LNB_DEVINL void ss_cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
-// dyn smem = SS_KT * (hd + 8) * 2 + n_rep * hd * 4
-inline size_t ss_scores_smem(int hd, int n_rep) { return (size_t)SS_KT * (hd + 8) * 2 + (size_t)n_rep * hd * 4; }
+// dyn smem = SS_KT * (hd + 8) * 2 + n_rep * hd * 4 (MXFP8: + the tile's codes and scale slots, SS_KT * (hd + 4))
+inline size_t ss_scores_smem(int hd, int n_rep, int kvf) {
+  return (size_t)SS_KT * (hd + 8) * 2 + (size_t)n_rep * hd * 4 + (kvf == KVF_MXFP8 ? (size_t)SS_KT * (hd + 4) : 0);
+}
+LNB_DEVINL void ss_cp8(void* smem_dst, const void* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+LNB_DEVINL void ss_cp4(void* smem_dst, const void* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+// MXFP8: issue the copies of keys [k0, k0 + n) of head h (records at rec, rowb bytes apart; codes of the head's columns
+// [c0, c0 + w)) into codes [n][w] and slots [n]
+LNB_DEVINL void ss_issue_fp8(const uint8_t* rec, int rowb, int kv_l, int h, int hd, int c0, int w, int k0, int n, uint8_t* codes,
+                             uint32_t* slots, int tid, int nthr) {
+  const int cpr = w / 8;
+  for (int i = tid; i < n * cpr; i += nthr) {
+    const int t = i / cpr, cc = i % cpr;
+    ss_cp8(codes + (size_t)t * w + cc * 8, rec + (size_t)(k0 + t) * rowb + h * hd + c0 + cc * 8);
+  }
+  for (int t = tid; t < n; t += nthr) ss_cp4(slots + t, rec + (size_t)(k0 + t) * rowb + kv_l + h * 4);
+}
+// MXFP8: decode the copied codes [n][w] (columns [c0, c0 + w) of the head) into the bf16 tile [n][ld]
+LNB_DEVINL void ss_decode_fp8(const uint8_t* codes, const uint32_t* slots, int c0, int w, int n, uint16_t* out, int ld, int tid, int nthr) {
+  const int cpr = w / 8;
+  for (int i = tid; i < n * cpr; i += nthr) {
+    const int t = i / cpr, cc = i % cpr;
+    const uint32_t e8m0 = (slots[t] >> (8 * ((c0 + cc * 8) >> 5))) & 0xffu;
+    *reinterpret_cast<uint4*>(out + (size_t)t * ld + cc * 8) =
+        kv_decode8(*reinterpret_cast<const uint2*>(codes + (size_t)t * w + cc * 8), mx_scale(e8m0));
+  }
+}
 
+template <int KVF>
 __global__ void __launch_bounds__(SS_KT) ss_scores_kernel(const StreamAttn P) {
   pdl_launch_dependents();
   pdl_wait();
@@ -94,7 +128,10 @@ __global__ void __launch_bounds__(SS_KT) ss_scores_kernel(const StreamAttn P) {
   const int hd = P.hd, n_rep = P.n_rep, ks = hd + 8, cpr = hd / 8;
   uint16_t* sK = reinterpret_cast<uint16_t*>(sm);                     // [SS_KT][hd + 8]
   float* sQ = reinterpret_cast<float*>(sK + (size_t)SS_KT * ks);      // [n_rep][hd]
+  uint32_t* sSl = reinterpret_cast<uint32_t*>(sQ + (size_t)n_rep * hd);  // MXFP8: [SS_KT] scale slots, then [SS_KT][hd] codes
+  uint8_t* sC = reinterpret_cast<uint8_t*>(sSl + SS_KT);
   const uint16_t* kb = P.cache_k + ss_cache_base(P, r) + (size_t)h * hd;
+  const uint8_t* kr8 = reinterpret_cast<const uint8_t*>(P.cache_k) + ss_cache_base(P, r);
   for (int i = tid; i < n_rep * hd; i += SS_KT) sQ[i] = bf2f(P.q[(size_t)r * P.ldq + (size_t)h * n_rep * hd + i]);
   double z[8];
 #pragma unroll
@@ -102,13 +139,21 @@ __global__ void __launch_bounds__(SS_KT) ss_scores_kernel(const StreamAttn P) {
   for (int k0 = t0; k0 < t1; k0 += SS_KT) {
     const int n = min(SS_KT, t1 - k0);
     __syncthreads();
-    for (int i = tid; i < n * cpr; i += SS_KT) {
-      const int t = i / cpr, cc = i % cpr;
-      ss_cp16(sK + (size_t)t * ks + cc * 8, kb + (size_t)(k0 + t) * P.kv_dim + cc * 8);
+    if constexpr (KVF == KVF_MXFP8) {
+      ss_issue_fp8(kr8, P.kv_dim, P.n_heads / n_rep * hd, h, hd, 0, hd, k0, n, sC, sSl, tid, SS_KT);
+    } else {
+      for (int i = tid; i < n * cpr; i += SS_KT) {
+        const int t = i / cpr, cc = i % cpr;
+        ss_cp16(sK + (size_t)t * ks + cc * 8, kb + (size_t)(k0 + t) * P.kv_dim + cc * 8);
+      }
     }
     ss_cp_commit();
     ss_cp_wait<0>();
     __syncthreads();
+    if constexpr (KVF == KVF_MXFP8) {
+      ss_decode_fp8(sC, sSl, 0, hd, n, sK, ks, tid, SS_KT);
+      __syncthreads();
+    }
     if (tid < n) {
       const uint16_t* kr = sK + (size_t)tid * ks;
       float acc[8];
@@ -191,12 +236,15 @@ __global__ void __launch_bounds__(128) ss_zsum_kernel(const StreamAttn P) {
 }
 
 // dyn smem = 2 stages x (SS_VT x dw V columns + n_rep x SS_VT bf16 scores) + n_rep x SS_VT f32 p
-inline size_t ss_out_smem(int hd, int n_rep, int dsplit) {
+// (MXFP8: + 2 stages of the tile's codes and scale slots, SS_VT x (dw + 4) each)
+inline size_t ss_out_smem(int hd, int n_rep, int dsplit, int kvf) {
   const int dw = hd / dsplit;
-  return (size_t)2 * ((size_t)SS_VT * dw * 2 + (size_t)n_rep * SS_VT * 2) + (size_t)n_rep * SS_VT * 4;
+  return (size_t)2 * ((size_t)SS_VT * dw * 2 + (size_t)n_rep * SS_VT * 2) + (size_t)n_rep * SS_VT * 4 +
+         (kvf == KVF_MXFP8 ? (size_t)2 * SS_VT * (dw + 4) : 0);
 }
 
 // block = n_rep * (hd / dsplit): thread = (query head hh of the group, column d of the CTA's d-range)
+template <int KVF>
 __global__ void __launch_bounds__(1024) ss_out_kernel(const StreamAttn P, int dsplit) {
   pdl_launch_dependents();
   pdl_wait();
@@ -215,6 +263,8 @@ __global__ void __launch_bounds__(1024) ss_out_kernel(const StreamAttn P, int ds
   uint16_t* sV = reinterpret_cast<uint16_t*>(sm);                       // [2][SS_VT][dw]
   uint16_t* sS = sV + (size_t)2 * SS_VT * dw;                           // [2][n_rep][SS_VT] raw bf16 (score or p)
   float* sP = reinterpret_cast<float*>(sS + (size_t)2 * n_rep * SS_VT); // [n_rep][SS_VT]
+  uint32_t* sSl = reinterpret_cast<uint32_t*>(sP + (size_t)n_rep * SS_VT);   // MXFP8: [2][SS_VT] scale slots, [2][SS_VT][dw] codes
+  uint8_t* sC = reinterpret_cast<uint8_t*>(sSl + 2 * SS_VT);
   const int hh = tid / dw, dd = tid % dw;
   if (!P.strict && tid < n_rep) {   // Z: the chunk partials in chunk order
     const double* zp = P.zpart + ((size_t)rl * P.n_heads + h * n_rep + tid) * P.n_chunks;
@@ -224,12 +274,18 @@ __global__ void __launch_bounds__(1024) ss_out_kernel(const StreamAttn P, int ds
     sZ[tid] = z;
   }
   const uint16_t* vb = P.cache_v + ss_cache_base(P, r) + (size_t)h * P.hd + (size_t)g * dw;
+  const uint8_t* vr8 = reinterpret_cast<const uint8_t*>(P.cache_v) + ss_cache_base(P, r);
   auto issue = [&](int k0, int stage) {
     const int n = min(SS_VT, t1 - k0);
-    uint16_t* v = sV + (size_t)stage * SS_VT * dw;
-    for (int i = tid; i < n * cpr; i += nthr) {
-      const int t = i / cpr, cc = i % cpr;
-      ss_cp16(v + (size_t)t * dw + cc * 8, vb + (size_t)(k0 + t) * P.kv_dim + cc * 8);
+    if constexpr (KVF == KVF_MXFP8) {
+      ss_issue_fp8(vr8, P.kv_dim, P.n_heads / n_rep * P.hd, h, P.hd, g * dw, dw, k0, n, sC + (size_t)stage * SS_VT * dw,
+                   sSl + stage * SS_VT, tid, nthr);
+    } else {
+      uint16_t* v = sV + (size_t)stage * SS_VT * dw;
+      for (int i = tid; i < n * cpr; i += nthr) {
+        const int t = i / cpr, cc = i % cpr;
+        ss_cp16(v + (size_t)t * dw + cc * 8, vb + (size_t)(k0 + t) * P.kv_dim + cc * 8);
+      }
     }
     uint16_t* s = sS + (size_t)stage * n_rep * SS_VT;
     const int n8 = (n + 7) / 8;   // whole 16-byte pieces (t_stride is a multiple of SS_VT: never past the row)
@@ -251,6 +307,8 @@ __global__ void __launch_bounds__(1024) ss_out_kernel(const StreamAttn P, int ds
       ss_cp_wait<0>();
     }
     __syncthreads();
+    if constexpr (KVF == KVF_MXFP8)
+      ss_decode_fp8(sC + (size_t)stage * SS_VT * dw, sSl + stage * SS_VT, g * dw, dw, n, sV + (size_t)stage * SS_VT * dw, dw, tid, nthr);
     const uint16_t* s = sS + (size_t)stage * n_rep * SS_VT;
     for (int i = tid; i < n_rep * n; i += nthr) {
       const int j = i / n, t = i % n;

@@ -188,8 +188,10 @@ DEFAULT_STEP_TOKENS = 64
 
 class InferenceEngine:
     def __init__(self, model: "model_mod.Model", inferenceArgs: "model_mod.InferenceArgs", logFn=None,
-                 acc_mode: int = model_mod.LNB_ACC_FAST, max_rows: int = 8):
+                 acc_mode: int = model_mod.LNB_ACC_FAST, max_rows: int = 8, kv_format: str = "bf16"):
+        """kv_format: the cache format of every context the engine creates ("bf16" or "mxfp8", DESIGN §9j)"""
         self.model = model
+        self.kv_format = kv_format
         self.inferenceArgs = inferenceArgs
         self.logFn = logFn
         self.acc_mode = acc_mode
@@ -198,7 +200,7 @@ class InferenceEngine:
 
     def CreateInferenceContext(self) -> "model_mod.InferenceContext":  # inference.go:256-258
         ctx = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
-                                         max_rows=self.max_rows, acc_mode=self.acc_mode)
+                                         max_rows=self.max_rows, acc_mode=self.acc_mode, kv_format=self.kv_format)
         if self.context_hook is not None:
             self.context_hook(ctx)
         return ctx

@@ -333,8 +333,13 @@ def _token_logprobs(recs) -> list:
 class InferenceContext:
     """model.InferenceContext (inferencecontext.go:8-46): the KV cache (here: in HBM)."""
 
+    KV_FORMATS = {"bf16": _capi.LNB_KV_BF16, "mxfp8": _capi.LNB_KV_MXFP8}
+
     def __init__(self, transformer: LlamaTransformer, inferenceArgs: InferenceArgs, logFn=None,
-                 max_rows: int = 8, acc_mode: int = LNB_ACC_FAST, n_seq: int = 1):
+                 max_rows: int = 8, acc_mode: int = LNB_ACC_FAST, n_seq: int = 1, kv_format: str = "bf16"):
+        """kv_format: "bf16", or "mxfp8" for the MXFP8 KV cache (lnb_session_create_kv, DESIGN §9j)"""
+        if kv_format not in self.KV_FORMATS:
+            raise ValueError(f"kv_format must be one of {sorted(self.KV_FORMATS)}, not {kv_format!r}")
         self.transformer = transformer
         self.SequenceLength = inferenceArgs.SequenceLength if inferenceArgs.SequenceLength > 0 \
             else transformer.args.MaxSequenceLength
@@ -342,8 +347,12 @@ class InferenceContext:
         self.acc_mode = acc_mode
         self.max_rows = max_rows
         self.n_seq = n_seq
+        self.kv_format = kv_format
         h = C.c_void_p()
-        if n_seq > 1:   # n_seq reference InferenceContexts that share the weights (batched decode)
+        if kv_format != "bf16":
+            check(lib.lnb_session_create_kv(transformer.h, self.SequenceLength, n_seq, max_rows, acc_mode,
+                                            self.KV_FORMATS[kv_format], C.byref(h)))
+        elif n_seq > 1:   # n_seq reference InferenceContexts that share the weights (batched decode)
             check(lib.lnb_session_create_batch(transformer.h, self.SequenceLength, n_seq, max_rows, acc_mode, C.byref(h)))
         else:
             check(lib.lnb_session_create(transformer.h, self.SequenceLength, max_rows, acc_mode, C.byref(h)))
@@ -369,6 +378,24 @@ class InferenceContext:
         out = np.empty((self.SequenceLength, kv_l, a.HeadDim), np.uint16)
         check(lib.lnb_session_read(self.h, which, layer, out.ctypes.data_as(C.c_void_p), out.nbytes))
         return ml.Tensor(out, ml.DT_BF16)
+
+    def kv_info(self) -> tuple[str, int]:
+        """(the cache format, the bytes its K and V caches hold in HBM)"""
+        fmt, nbytes = C.c_int(), C.c_int64()
+        check(lib.lnb_session_kv_info(self.h, C.byref(fmt), C.byref(nbytes)))
+        return {v: k for k, v in self.KV_FORMATS.items()}[fmt.value], nbytes.value
+
+    def kv_read(self, seq: int, layer: int, which: str, pos0: int, n: int) -> tuple[np.ndarray, np.ndarray]:
+        """the raw MXFP8 blocks of positions [pos0, pos0 + n) of K (which="k") or V ("v"): (codes [n, kv_l] u8, scales
+        [n, n_kv, ceil(head_dim / 32)] u8), heads in checkpoint order"""
+        a, tp = self.transformer.args, self.transformer.tp_size
+        n_kv = a.N_KVHeads // tp
+        codes = np.empty((n, n_kv * a.HeadDim), np.uint8)
+        scales = np.empty((n, n_kv, (a.HeadDim + 31) // 32), np.uint8)
+        w = {"k": _capi.LNB_BUF_CACHE_K, "v": _capi.LNB_BUF_CACHE_V}[which]
+        check(lib.lnb_session_kv_read(self.h, seq, layer, w, pos0, n, codes.ctypes.data_as(C.c_void_p),
+                                      scales.ctypes.data_as(C.c_void_p)))
+        return codes, scales
 
     def residual(self, rows: int) -> np.ndarray:
         out = np.empty((rows, self.transformer.args.Dim), np.uint16)

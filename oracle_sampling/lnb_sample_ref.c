@@ -673,6 +673,23 @@ void orc_mxfp8_dequantize(const uint8_t* codes, const uint8_t* scales, int rows,
     }
 }
 
+/* MXFP8 KV cache (DESIGN.md §9j; the device form is csrc/kvcache.cuh): rows [n][n_kv * head_dim] bf16 -> codes
+ * [n][n_kv * head_dim], scales [n][n_kv][ceil(head_dim / 32)] and (deq != NULL) e4m3(code) * 2^X as bf16 bits.  The rule of
+ * orc_mxfp8_quantize on the matrix of head rows [n * n_kv][head_dim], except that K and V rows cannot be refused: the block
+ * maximum is taken over the finite elements, a NaN element stores the NaN code 0x7F (decoded 0x7FC0) and +-inf saturates
+ * to +-448 (0x7E with the sign). */
+void orc_kv_mxfp8_quantize(const uint16_t* rows, int n, int head_dim, int n_kv, uint8_t* codes, uint8_t* scales, uint16_t* deq) {
+  const int64_t ne = (int64_t)n * n_kv * head_dim;
+  if (ne <= 0) return;
+  uint16_t* fin = (uint16_t*)malloc((size_t)ne * 2);
+  for (int64_t i = 0; i < ne; i++) fin[i] = (rows[i] & 0x7f80) == 0x7f80 ? (uint16_t)(rows[i] & 0x8000) : rows[i];
+  orc_mxfp8_quantize(fin, n * n_kv, head_dim, codes, scales);
+  free(fin);
+  for (int64_t i = 0; i < ne; i++)
+    if ((rows[i] & 0x7f80) == 0x7f80) codes[i] = (rows[i] & 0x7f) ? 0x7F : (uint8_t)(((rows[i] >> 8) & 0x80) | 0x7E);
+  if (deq) orc_mxfp8_dequantize(codes, scales, n * n_kv, head_dim, deq);
+}
+
 /* MXFP4 linear weights (DESIGN.md §9i): the MXFP8 blocks, one E2M1 code per weight, packed two a byte with the even
  * column in the low nibble: codes [rows][cols / 2], scales [rows][ceil(cols / 32)].  X = e - 2 if the 7-bit mantissa field
  * f of the bf16 block maximum is <= 64, else e - 1 (e its unbiased exponent), clamped to [-125, 125]; -125 for a zero or

@@ -88,6 +88,8 @@ def lib():
         L.orc_mxfp8_quantize.argtypes = [_u16p, C.c_int, C.c_int, _u8p, _u8p]
         L.orc_mxfp8_dequantize.restype = None
         L.orc_mxfp8_dequantize.argtypes = [_u8p, _u8p, C.c_int, C.c_int, _u16p]
+        L.orc_kv_mxfp8_quantize.restype = None
+        L.orc_kv_mxfp8_quantize.argtypes = [_u16p, C.c_int, C.c_int, C.c_int, _u8p, _u8p, _u16p]
         L.orc_mxfp4_quantize.restype = C.c_int64
         L.orc_mxfp4_quantize.argtypes = [_u16p, C.c_int, C.c_int, _u8p, _u8p]
         L.orc_mxfp4_dequantize.restype = None
@@ -365,6 +367,21 @@ def mxfp8_dequantize(codes, scales) -> np.ndarray:
     lib().orc_mxfp8_dequantize(codes.ctypes.data_as(u8), scales.ctypes.data_as(u8), rows, cols,
                                out.ctypes.data_as(C.POINTER(C.c_uint16)))
     return out
+
+
+def kv_mxfp8_quantize(rows, head_dim: int) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """orc_kv_mxfp8_quantize of K or V rows (uint16 bits [n, n_kv * head_dim]): (codes [n, n_kv * head_dim] u8, scales
+    [n, n_kv, ceil(head_dim / 32)] u8, decoded rows [n, n_kv * head_dim] bf16 bits)"""
+    rows = np.ascontiguousarray(rows, np.uint16)
+    n, kv = rows.shape
+    n_kv = kv // head_dim
+    codes = np.empty((n, kv), np.uint8)
+    scales = np.empty((n, n_kv, (head_dim + 31) // 32), np.uint8)
+    deq = np.empty((n, kv), np.uint16)
+    u8 = C.POINTER(C.c_uint8)
+    lib().orc_kv_mxfp8_quantize(rows.ctypes.data_as(C.POINTER(C.c_uint16)), n, head_dim, n_kv, codes.ctypes.data_as(u8),
+                                scales.ctypes.data_as(u8), deq.ctypes.data_as(C.POINTER(C.c_uint16)))
+    return codes, scales, deq
 
 
 def mxfp4_quantize(w) -> tuple[np.ndarray, np.ndarray]:
