@@ -384,7 +384,8 @@ class InferenceEngine:
             raise ml.MlError(f"NumReturn {beams.NumReturn} must be in [1, NumBeams = {B}]")
         prompt = [int(t) for t in promptTokens]
         infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
-                                                max_rows=max(self.max_rows, B), acc_mode=self.acc_mode, n_seq=B)
+                                                max_rows=max(self.max_rows, B), acc_mode=self.acc_mode, n_seq=B,
+                                                kv_format=self.kv_format)
         if self.context_hook is not None:
             self.context_hook(infContext)
         try:
@@ -521,7 +522,8 @@ class InferenceEngine:
             raise ml.MlError(f"step_tokens {step_tokens} must be at least slots {slots} (every decoding sequence gets a row)")
         prompts = [[int(t) for t in p] for p in prompts]
         infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
-                                                max_rows=max(self.max_rows, step_tokens), acc_mode=self.acc_mode, n_seq=slots)
+                                                max_rows=max(self.max_rows, step_tokens), acc_mode=self.acc_mode, n_seq=slots,
+                                                kv_format=self.kv_format)
         if self.context_hook is not None:
             self.context_hook(infContext)
         try:
@@ -638,7 +640,8 @@ class InferenceEngine:
                 yield 0, state, tok
             return
         infContext = model_mod.InferenceContext(self.model.Transformer, self.inferenceArgs, self.logFn,
-                                                max_rows=max(self.max_rows, n), acc_mode=self.acc_mode, n_seq=n)
+                                                max_rows=max(self.max_rows, n), acc_mode=self.acc_mode, n_seq=n,
+                                                kv_format=self.kv_format)
         if self.context_hook is not None:
             self.context_hook(infContext)
         try:

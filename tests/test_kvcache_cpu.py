@@ -114,10 +114,12 @@ def test_broken_rules_are_caught():
 class RefSession:
     """orc_forward_order's sequence of oracle ops, with every K and V row the forward stores replaced by its decoded MXFP8
     blocks when kv_mx: what an MXFP8-cache session must compute.  order: O.ORDER_REF (STRICT) or O.ORDER_FAST_STREAM (the
-    FAST order of the kernel chain with streamed attention, which every row of an MXFP8 session takes)"""
+    FAST order of the kernel chain with streamed attention, which every row of an MXFP8 session takes).  decode: rows
+    [n, kv_l], head_dim -> the decoded rows stored in their place (default: the C statement's)"""
 
-    def __init__(self, args: dict, tensors: dict, seq_len: int, kv_mx: bool, order=O.ORDER_REF):
+    def __init__(self, args: dict, tensors: dict, seq_len: int, kv_mx: bool, order=O.ORDER_REF, decode=None):
         self.a, self.t, self.seq_len, self.kv_mx = args, tensors, seq_len, kv_mx
+        self.decode = decode or (lambda rows, hd: SR.kv_mxfp8_quantize(rows, hd)[2])
         self.ks, self.parts, self.attn = order
         kvd = args["n_kv_heads"] * args["head_dim"]
         self.ck = [np.zeros((seq_len, kvd), np.uint16) for _ in range(args["n_layers"])]
@@ -158,7 +160,7 @@ class RefSession:
             k2 = O.rope_apply(np.ascontiguousarray(k.reshape(S, nkv, hd)), self.cis, start_pos).reshape(S, nkv * hd)
             self.pre_k[l][start_pos:T], self.pre_v[l][start_pos:T] = k2, v
             if self.kv_mx:
-                k2, v = SR.kv_mxfp8_quantize(k2, hd)[2], SR.kv_mxfp8_quantize(v, hd)[2]
+                k2, v = self.decode(k2, hd), self.decode(v, hd)
             self.ck[l][start_pos:T], self.cv[l][start_pos:T] = k2, v
             ck, cv = self.ck[l].reshape(self.seq_len, nkv, hd), self.cv[l].reshape(self.seq_len, nkv, hd)
             if self.attn == O.ATTN_REF:
