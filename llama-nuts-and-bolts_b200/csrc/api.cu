@@ -1306,6 +1306,26 @@ struct AllocBatch {
   }
 };
 
+// A session's K and V caches (lnb_session_create_kv): per layer, [n_seq][seq_len] positions of pos_bytes each, holding
+// kv_l bf16 values (LNB_KV_BF16) or a record of kvcache.cuh (LNB_KV_MXFP8).  Every address into the caches is made here.
+struct KvCache {
+  int fmt = LNB_KV_BF16, n_seq = 0, seq_len = 0, pos_bytes = 0;   // pos_bytes: kv_l * 2, or kv_row_bytes(kv_l, n_kv)
+  std::vector<uint8_t*> mem;       // [n_layers][K, V], each cache_bytes()
+  // The kernels count cache offsets in bf16 elements, or in bytes for MXFP8 records: pos_stride() of those units per
+  // position (StreamAttn.kv_dim), seq_stride() per sequence (the stride a row map's row_seq is scaled by).
+  int pos_stride() const { return fmt == LNB_KV_MXFP8 ? pos_bytes : pos_bytes / 2; }
+  long long seq_stride() const { return (long long)seq_len * pos_stride(); }
+  long long row16() const { return pos_bytes / 16; }   // 16-byte vectors per position (seqcopy_kernel)
+  size_t cache_bytes() const { return (size_t)n_seq * seq_len * pos_bytes; }   // one layer's K, or its V
+  size_t bytes() const { return mem.size() * cache_bytes(); }
+  // layer l's K (v = 0) or V (v = 1) cache from position pos of sequence seq
+  uint8_t* rec(int l, int v, int seq, int pos = 0) const { return mem[2 * l + v] + ((size_t)seq * seq_len + pos) * pos_bytes; }
+  uint16_t* at(int l, int v, int seq) const { return reinterpret_cast<uint16_t*>(rec(l, v, seq)); }   // as the kernels take it
+  uint16_t* bf16(int l, int v, int seq) const { return fmt == LNB_KV_BF16 ? at(l, v, seq) : nullptr; }   // bf16-only routes
+  void alloc(AllocBatch& A) { for (uint8_t*& p : mem) A.add(&p, cache_bytes(), 0); }   // ml.Zeros, inferencecontext.go:31-43
+  void release() { for (uint8_t* p : mem) cudaFree(p); }
+};
+
 // the generation controls of one sequence of a session
 struct SeqCtl {
   bool samp = false;               // draws with its sampler parameters (lnb_session_set_sampling)
@@ -1350,11 +1370,7 @@ struct lnb_session {
   float* logits = nullptr;
   size_t logits_rows = 0;
   float* logits_full = nullptr;  // tp>1: gathered [rows, vocab]
-  std::vector<uint16_t*> ck, cv;
-  // cache format (lnb_session_create_kv): LNB_KV_BF16, or LNB_KV_MXFP8 with ck / cv holding the records of kvcache.cuh;
-  // kv_pos: cache elements per position (bf16: kv_l values; MXFP8: the record's bytes)
-  int kv_fmt = LNB_KV_BF16;
-  int kv_pos = 0;
+  KvCache kv;
   LnbDevState* st = nullptr;
   int32_t* d_tok_out = nullptr;
   // pinned staging, one allocation (at h_tok) carved into two views: a call's token ids or row map on their way to d_rag
@@ -1486,7 +1502,7 @@ static unsigned long long p2p_timeout_ns() {
   return ms > 0 ? (unsigned long long)ms * 1000000ull : 0ull;
 }
 
-static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, int kv_fmt, lnb_session** out);
+static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, int kv_format, lnb_session** out);
 extern "C" int lnb_session_create(lnb_model* m, int seq_len, int max_rows, int acc_mode, lnb_session** out) {
   return session_create_impl(m, seq_len, max_rows, acc_mode, 1, LNB_KV_BF16, out);
 }
@@ -1499,10 +1515,10 @@ extern "C" int lnb_session_create_kv(lnb_model* m, int seq_len, int n_seq, int m
   if (n_seq == 1) return session_create_impl(m, seq_len, max_rows, acc_mode, 1, kv_format, out);
   return session_create_impl(m, seq_len, max_rows < n_seq ? n_seq : max_rows, acc_mode, n_seq, kv_format, out);
 }
-static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, int kv_fmt, lnb_session** out) {
+static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_mode, int n_seq, int kv_format, lnb_session** out) {
   if (!m || !out) return fail(LNB_EINVAL, "NULL argument");
-  if (kv_fmt != LNB_KV_BF16 && kv_fmt != LNB_KV_MXFP8) return fail(LNB_EINVAL, "unknown KV cache format %d", kv_fmt);
-  const bool kv_mx = kv_fmt == LNB_KV_MXFP8;
+  if (kv_format != LNB_KV_BF16 && kv_format != LNB_KV_MXFP8) return fail(LNB_EINVAL, "unknown KV cache format %d", kv_format);
+  const bool kv_mx = kv_format == LNB_KV_MXFP8;
   if (kv_mx && !ss_shape_ok(m->a.head_dim, m->a.n_heads / m->a.n_kv_heads))
     return fail(LNB_EINVAL, "MXFP8 KV cache: attention runs on the streamed kernels, which serve head_dim <= 128 and n_rep <= 8 "
                 "(head_dim %d, n_rep %d)", m->a.head_dim, m->a.n_heads / m->a.n_kv_heads);
@@ -1536,8 +1552,8 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
     }
   }
   s->stream_attn = stream_attn;
-  s->kv_fmt = kv_fmt;
-  s->kv_pos = kv_mx ? kv_row_bytes(m->kv_l, m->kv_l / a.head_dim) : m->kv_l;
+  s->kv = KvCache{kv_format, n_seq, seq_len, kv_mx ? kv_row_bytes(m->kv_l, m->kv_l / a.head_dim) : m->kv_l * 2,
+                  std::vector<uint8_t*>(2 * a.n_layers)};
   s->samp_rows = n_seq;
   s->lp_rows = std::max(max_rows, 8);
   cudaError_t e = cudaStreamCreateWithFlags(&s->stream, cudaStreamNonBlocking);
@@ -1576,17 +1592,11 @@ static int session_create_impl(lnb_model* m, int seq_len, int max_rows, int acc_
   A.add(&s->d_rag, in_words * 4);
   A.add(&s->st, sizeof(LnbDevState), 0);
   A.add(&s->d_tok_out, (size_t)seq_len * 4);
-  s->ck.assign(a.n_layers, nullptr);
-  s->cv.assign(a.n_layers, nullptr);
-  const size_t cbytes = (size_t)n_seq * seq_len * (kv_mx ? (size_t)s->kv_pos : (size_t)m->kv_l * 2);
   A.add(&s->d_next_arr, 8 * 4);
-  for (int l = 0; l < a.n_layers; l++) {
-    A.add(&s->ck[l], cbytes, 0);  // ml.Zeros, inferencecontext.go:31-43
-    A.add(&s->cv[l], cbytes, 0);
-  }
+  s->kv.alloc(A);
   A.add_host(&s->h_tok, (in_words + seq_len + 8) * 4);
   A.add_host(&s->h_err, 64);
-  int rc = e == cudaSuccess ? A.commit(s->stream, "session allocation", "KV cache", (size_t)2 * a.n_layers * cbytes) : 0;
+  int rc = e == cudaSuccess ? A.commit(s->stream, "session allocation", "KV cache", s->kv.bytes()) : 0;
   if (rc == 0 && e == cudaSuccess) {
     s->h_out = s->h_tok + in_words;
     *s->h_err = 0;
@@ -1626,8 +1636,7 @@ extern "C" int lnb_session_destroy(lnb_session* s) {
   cudaFree(s->d_gst); cudaFree(s->d_gslot);
   for (int q = 0; q < 8; q++)
     if (s->ctl[q].gram) grammar_release(s->ctl[q].gram);
-  for (auto p : s->ck) cudaFree(p);
-  for (auto p : s->cv) cudaFree(p);
+  s->kv.release();
   if (s->h_tok) cudaFreeHost(s->h_tok);
   if (s->h_err) cudaFreeHost(s->h_err);
   if (s->h_logits_pin) cudaFreeHost(s->h_logits_pin);
@@ -1802,7 +1811,7 @@ static bool engine_probe(lnb_session* s) {
   // FAST sessions; LNB_ENGINE=1 / 0 forces it on / off.
   const char* e = getenv("LNB_ENGINE");
   if (e && !strcmp(e, "0")) return no("LNB_ENGINE=0");
-  if (s->kv_fmt == LNB_KV_MXFP8) return no("MXFP8 KV cache: the decode and batch engines read bf16 caches");
+  if (s->kv.fmt == LNB_KV_MXFP8) return no("MXFP8 KV cache: the decode and batch engines read bf16 caches");
   if (m->output.fmt != LNB_WEIGHTS_BF16)   // every linear matrix has the same format
     return no(std::string(wfmt_name(m->output.fmt)) + " weights: the decode and batch engines stream bf16 panels");
   // single-sequence steps of single-GPU FAST sessions stay on the kernel chain by default (the batch engine does not care)
@@ -1965,7 +1974,6 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
       s->eng_key_logits == logits_out)
     return 0;
   const int G = m->sm_count, mode = s->mode;
-  const size_t cache_off = (size_t)s->active_seq * s->seq_len * m->kv_l;
   const bool full = kind < 0;
   std::vector<EnginePhase> ph;
   // which phase of the step wrote a tagged vector last (consumers wait for exactly that phase's tag)
@@ -1991,7 +1999,7 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
     LayerW& W = m->layers[l];
     if (full || kind == 0) {  // attn_norm -> wq|wk|wv -> RoPE -> KV append
       EnginePhase e = gemv(PRO_RMSNORM, EPI_QKV_ROPE, W.qkv, s->x, W.attn_norm, s->q, m->q_l, nullptr);
-      e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->ck[l] + cache_off; e.cache_v = s->cv[l] + cache_off;
+      e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->kv.bf16(l, 0, s->active_seq); e.cache_v = s->kv.bf16(l, 1, s->active_seq);
       if (full && l == 0) e.flags |= EF_X_TOKEN;
       else input(e, s->x_t, w_x);
       if (full) { e.out_t = s->qkv_t; w_qkv = (int)ph.size(); }
@@ -2000,7 +2008,7 @@ static int engine_build(lnb_session* s, int kind, const float* logits_out) {
     if (full) {
       EnginePhase e{};
       e.type = EP_SDPA; e.kv_dim = m->kv_l; e.q_dim = m->q_l;
-      e.cache_k = s->ck[l] + cache_off; e.cache_v = s->cv[l] + cache_off;
+      e.cache_k = s->kv.bf16(l, 0, s->active_seq); e.cache_v = s->kv.bf16(l, 1, s->active_seq);
       input(e, s->qkv_t, w_qkv);
       e.out_t = s->o_t; w_o = (int)ph.size();
       ph.push_back(e);
@@ -2202,12 +2210,12 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
     ph.push_back(scale(s->bx, l == 0, W.attn_norm));
     {
       BatchPhase e = gemv(PRO_RMSNORM, EPI_QKV_ROPE, W.qkv, s->bx, W.attn_norm, s->bq, m->q_l, nullptr);
-      e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->ck[l]; e.cache_v = s->cv[l];
+      e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->kv.bf16(l, 0, 0); e.cache_v = s->kv.bf16(l, 1, 0);
       ph.push_back(e);
     }
     {
       BatchPhase e{};
-      e.type = BP_SDPA; e.x = s->bq; e.out = s->bo; e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->ck[l]; e.cache_v = s->cv[l];
+      e.type = BP_SDPA; e.x = s->bq; e.out = s->bo; e.q_dim = m->q_l; e.kv_dim = m->kv_l; e.cache_k = s->kv.bf16(l, 0, 0); e.cache_v = s->kv.bf16(l, 1, 0);
       ph.push_back(e);
     }
     ph.push_back(gemv(PRO_PLAIN, tp ? EPI_P2P : EPI_RESID, W.o, s->bo, nullptr, s->bh1, a.dim, s->bx));
@@ -2246,7 +2254,7 @@ static int batch_engine_launch(lnb_session* s, int n, const int32_t* tokens, con
   P.emb = m->tok_embd; P.dim = a.dim; P.head_dim = a.head_dim; P.n_rep = a.n_heads / a.n_kv_heads; P.seq_len = s->seq_len;
   P.cis = m->cis; P.silu_tab = m->silu_tab; P.eps = a.norm_eps; P.attn_scale = attn_scale_bf16(a.head_dim);
   P.strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
-  P.tokens = tokens; P.pos_arr = pos_arr; P.row_seq = row_seq; P.cache_seq_stride = (long long)s->seq_len * m->kv_l;
+  P.tokens = tokens; P.pos_arr = pos_arr; P.row_seq = row_seq; P.cache_seq_stride = s->kv.seq_stride();
   P.rscale = s->rs; P.keys = s->d_bkeys; P.next_arr = s->d_next_arr; P.bar_ctr = s->d_bar;
   P.p2p = s->p2p; P.tp = m->tp_size;
   P.timeout_ns = p2p_timeout_ns();
@@ -2280,7 +2288,7 @@ static int enqueue_decode_engine(lnb_session* s, int32_t token, int start_pos, i
 
 // The rows of one forward: where row r's token, position and KV cache come from, and what the LM head makes of them.
 // rows_single, rows_ragged and rows_spec are the only places that decide this; the forward builders read it from here.
-// Rows of several sequences always carry row_seq; without it every row is on the cache at cache_off.
+// Rows of several sequences always carry row_seq; without it every row is on the cache of sequence seq.
 enum RowsKind { ROWS_SINGLE, ROWS_RAGGED, ROWS_SPEC };
 // what the LM head produces: the last row's greedy token with no logits kept, the last row's or every row's (NONE, LAST,
 // ALL); or, for output rows that each end their own sequence, the logits and a greedy token in d_next_arr per row (PER_ROW)
@@ -2291,8 +2299,7 @@ struct Rows {
   const int32_t* tokens;    // device token id of each row, or NULL: st->next_token (a device-driven decode step)
   const int32_t* pos_arr;   // device position of each row, or NULL: st->pos + r
   const int32_t* row_seq;   // ragged, speculative, batched: the sequence of each row
-  size_t cache_off;         // elements to the cache every row addresses (the active sequence's), or 0
-  long long seq_stride;     // rows on several caches: elements between consecutive sequences' caches, else 0
+  int seq;                  // without row_seq: the sequence every row is on (the active one)
   int mb_rows;              // launch_gemv's mb_rows: ragged 8, else 0
   const int32_t* seg_last;  // ragged: the last row of each segment
   RowsHead head;
@@ -2306,8 +2313,7 @@ struct Rows {
 // kept, 0 = none, 1 = the last row, S = all rows.
 static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int logits_rows, bool advance, bool gather) {
   Rows R{};
-  R.kind = ROWS_SINGLE; R.S = S; R.tokens = tokens;
-  R.cache_off = (size_t)s->active_seq * s->seq_len * s->kv_pos;
+  R.kind = ROWS_SINGLE; R.S = S; R.tokens = tokens; R.seq = s->active_seq;
   R.head = logits_rows == 0 ? HEAD_NONE : logits_rows == 1 ? HEAD_LAST : HEAD_ALL;
   R.head_rows = logits_rows > 1 ? S : 1;
   R.advance = advance; R.gather = gather;
@@ -2319,7 +2325,6 @@ static Rows rows_single(const lnb_session* s, int S, const int32_t* tokens, int 
 static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, const CtlSum& u) {
   Rows R{};
   R.kind = ROWS_RAGGED; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
-  R.seq_stride = (long long)s->seq_len * s->kv_pos;
   R.mb_rows = 8;
   R.seg_last = s->d_rag + 3 * rows;
   R.head = HEAD_PER_ROW; R.head_rows = n_segs;
@@ -2332,7 +2337,6 @@ static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, const CtlSum
 static Rows rows_spec(const lnb_session* s, int rows, const CtlSum& u) {
   Rows R{};
   R.kind = ROWS_SPEC; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
-  R.seq_stride = (long long)s->seq_len * s->kv_pos;
   R.head = HEAD_PER_ROW; R.head_rows = rows;
   R.record = u.pen; R.grammar = u.gram;
   return R;
@@ -2345,8 +2349,8 @@ static int launch_kv_writer(const Launcher& L, lnb_session* s, int l, const Rows
   const int hd = m->a.head_dim, tasks = R.S * 2 * (m->kv_l / hd) * ((hd + 31) / 32);
   const int grid = std::min(m->sm_count * 8, std::max((tasks + 7) / 8, (R.S * m->q_l / 2 + 255) / 256));
   return launch_kernel(L, kvq_rope_store_kernel, dim3(grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, m->q_l + 2 * m->kv_l, s->q,
-                       m->q_l, m->kv_l, hd, (uint8_t*)s->ck[l] + R.cache_off, (uint8_t*)s->cv[l] + R.cache_off, (const float*)m->cis,
-                       (const int32_t*)&s->st->pos, R.S, R.pos_arr, R.row_seq, R.seq_stride);
+                       m->q_l, m->kv_l, hd, s->kv.rec(l, 0, R.seq), s->kv.rec(l, 1, R.seq), (const float*)m->cis,
+                       (const int32_t*)&s->st->pos, R.S, R.pos_arr, R.row_seq, s->kv.seq_stride());
 }
 
 // Attention of layer l for the rows R (queries in s->q), written to out: plain rows, or the X8 operand of the tensor-core
@@ -2356,10 +2360,7 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
   const lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   const int S = R.S, n_rep = a.n_heads / a.n_kv_heads, n_q = m->q_l / a.head_dim, n_kv = m->kv_l / a.head_dim;
-  const bool kv_mx = s->kv_fmt == LNB_KV_MXFP8;
-  // MXFP8: R.cache_off counts bytes
-  const uint16_t *ck = kv_mx ? (const uint16_t*)((const uint8_t*)s->ck[l] + R.cache_off) : s->ck[l] + R.cache_off;
-  const uint16_t *cv = kv_mx ? (const uint16_t*)((const uint8_t*)s->cv[l] + R.cache_off) : s->cv[l] + R.cache_off;
+  const KvCache& kv = s->kv;
   const int32_t* pos_ptr = &s->st->pos;
   const float scale = attn_scale_bf16(a.head_dim);
   const int strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
@@ -2369,20 +2370,21 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
   auto streamed = [&]() {
     StreamAttn P{};
     P.q = s->q; P.ldq = m->q_l;
-    P.cache_k = ck; P.cache_v = cv; P.kv_dim = s->kv_pos;
-    P.row_cache_stride = R.seq_stride; P.row_seq = R.row_seq; P.pos_arr = R.pos_arr;
+    P.cache_k = kv.at(l, 0, R.seq); P.cache_v = kv.at(l, 1, R.seq); P.kv_dim = kv.pos_stride();
+    P.row_cache_stride = kv.seq_stride(); P.row_seq = R.row_seq; P.pos_arr = R.pos_arr;
     P.n_rep = n_rep; P.hd = a.head_dim; P.n_heads = n_q;
     P.pos_ptr = pos_ptr; P.pos_step = 1;
     P.out = out; P.ldo = m->q_l; P.out_x8 = out_x8;
     P.scale = scale; P.strict = strict;
-    if (kv_mx) return launch_stream_attn<KVF_MXFP8>(L, P, S, n_kv, s->ss);
+    if (kv.fmt == LNB_KV_MXFP8) return launch_stream_attn<KVF_MXFP8>(L, P, S, n_kv, s->ss);
     return launch_stream_attn<KVF_BF16>(L, P, S, n_kv, s->ss);
   };
-  if (R.kind == ROWS_RAGGED || kv_mx) return streamed();
+  if (R.kind == ROWS_RAGGED || kv.fmt == LNB_KV_MXFP8) return streamed();
+  const uint16_t *ck = kv.bf16(l, 0, R.seq), *cv = kv.bf16(l, 1, R.seq);   // the kernels below read bf16 caches only
   if (!out_x8 && (S == 1 || spec) && s->sdpa_smem_decode)
     return launch_kernel(L, sdpa_decode_kernel, dim3(n_kv, S), dim3(128 * n_rep), s->sdpa_decode_smem, (const uint16_t*)s->q, ck, cv,
-                         m->kv_l, n_rep, a.head_dim, out, pos_ptr, s->seq_len, strict, scale, R.pos_arr,
-                         (long long)s->seq_len * m->kv_l, m->q_l, (const LnbDevState*)s->st, R.row_seq);
+                         m->kv_l, n_rep, a.head_dim, out, pos_ptr, s->seq_len, strict, scale, R.pos_arr, kv.seq_stride(), m->q_l,
+                         (const LnbDevState*)s->st, R.row_seq);
   if (out_x8 && a.head_dim == SP_HD) {
     const double* exp_tab = sdpa_tc_enabled() ? exp_table_device() : nullptr;
     if (exp_tab)
@@ -2502,13 +2504,13 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
       p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm; p.eps = a.norm_eps;
       p.out_bf16 = s->q; p.ldo = m->q_l;
       p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
-      if (s->kv_fmt == LNB_KV_MXFP8) {   // the projection's bf16 rows, then RoPE and the cache writer (kvcache.cuh)
+      if (s->kv.fmt == LNB_KV_MXFP8) {   // the projection's bf16 rows, then RoPE and the cache writer (kvcache.cuh)
         p.out_bf16 = s->qkv_raw; p.ldo = W.qkv.N;
         if ((rc = launch_gemv<PRO_RMSNORM, EPI_BF16>(L, mode, p, W.qkv, S, mb_rows))) return rc;
         if ((rc = launch_kv_writer(L, s, l, R))) return rc;
       } else {
-        p.cache_k = s->ck[l] + R.cache_off; p.cache_v = s->cv[l] + R.cache_off; p.cis = m->cis; p.pos_ptr = &s->st->pos;
-        p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = R.seq_stride;
+        p.cache_k = s->kv.bf16(l, 0, R.seq); p.cache_v = s->kv.bf16(l, 1, R.seq); p.cis = m->cis; p.pos_ptr = &s->st->pos;
+        p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = s->kv.seq_stride();
         if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, W.qkv, S, mb_rows))) return rc;
       }
     }
@@ -2594,10 +2596,10 @@ static int enqueue_forward_tc(lnb_session* s, const Rows& R) {
       if ((rc = tc_w(g, W.qkv))) return rc;
       if ((rc = launch_gemm_tc<TC_EPI_BF16>(L, g))) return rc;
     }
-    if (s->kv_fmt == LNB_KV_MXFP8) rc = launch_kv_writer(L, s, l, R);
+    if (s->kv.fmt == LNB_KV_MXFP8) rc = launch_kv_writer(L, s, l, R);
     else rc = launch_kernel(L, rope_kv_kernel, dim3(ew_grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, qkv_n, s->q, m->q_l, m->kv_l,
-                            a.head_dim, s->ck[l] + R.cache_off, s->cv[l] + R.cache_off, (const float*)m->cis, (const int32_t*)&s->st->pos, S,
-                            R.pos_arr, R.row_seq, (long long)s->seq_len * m->kv_l);
+                            a.head_dim, s->kv.bf16(l, 0, R.seq), s->kv.bf16(l, 1, R.seq), (const float*)m->cis, (const int32_t*)&s->st->pos, S,
+                            R.pos_arr, R.row_seq, s->kv.seq_stride());
     if (rc) return rc;
     if ((rc = launch_attention(L, s, l, R, s->o8, 1))) return rc;
     if ((rc = proj_resid(s->o8, W.o, s->x, s->h1))) return rc;
@@ -3304,22 +3306,20 @@ extern "C" int lnb_session_copy_sequences(lnb_session* s, int n, const int32_t* 
   const int L = m->a.n_layers;
   if (L > SC_MAX_LAYERS) return fail(LNB_EINVAL, "copying sequences serves up to %d layers (this model has %d)", SC_MAX_LAYERS, L);
   static_assert(sizeof(LpRecord) % 16 == 0, "records move as 16-byte vectors");
-  // cache rows move as 16-byte vectors too: kv_l * 2 bytes must be a multiple of 16 (model creation makes kv_l a multiple of 32)
-  if ((m->kv_l * 2) % 16) return fail(LNB_EINVAL, "cache rows of %d bytes are not a multiple of 16", m->kv_l * 2);
+  // cache rows move as 16-byte vectors too (model creation makes kv_l a multiple of 32; MXFP8 records are padded to 16 bytes)
+  if (s->kv.pos_bytes % 16) return fail(LNB_EINVAL, "cache rows of %d bytes are not a multiple of 16", s->kv.pos_bytes);
   std::lock_guard<std::mutex> lk(s->mu);
   CU(cudaSetDevice(m->device));
-  // (MXFP8 records are whole 16-byte vectors, kvcache.cuh)
-  const long long row16 = s->kv_fmt == LNB_KV_MXFP8 ? (long long)s->kv_pos / 16 : (long long)m->kv_l * 2 / 16;
   const long long rec16 = (long long)sizeof(LpRecord) / 16, np = pos1 - pos0;
   SeqCopyJob J{};
   J.n = n;
   for (int i = 0; i < n; i++) { J.src[i] = src[i]; J.dst[i] = dst[i]; }
   J.n_kv = 2 * L;
-  J.kv_stride = (long long)s->seq_len * row16; J.kv_len = np * row16;
+  J.kv_stride = s->seq_len * s->kv.row16(); J.kv_len = np * s->kv.row16();
   J.kv_tiles = (J.kv_len + SC_TILE - 1) / SC_TILE;
   for (int l = 0; l < L; l++) {
-    J.kv[l] = reinterpret_cast<uint4*>(s->ck[l]) + pos0 * row16;
-    J.kv[L + l] = reinterpret_cast<uint4*>(s->cv[l]) + pos0 * row16;
+    J.kv[l] = reinterpret_cast<uint4*>(s->kv.rec(l, 0, 0, pos0));
+    J.kv[L + l] = reinterpret_cast<uint4*>(s->kv.rec(l, 1, 0, pos0));
   }
   if (s->d_lp_rec) {
     J.rec = reinterpret_cast<uint4*>(s->d_lp_rec + pos0);
@@ -3644,7 +3644,7 @@ extern "C" int lnb_decode_run(lnb_session* s, int32_t first_token, int start_pos
 extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, float* ms_per_launch, int64_t* bytes_per_launch,
                                         int* launches) {
   if (!s || reps <= 0 || kind < 0 || kind > 4) return fail(LNB_EINVAL, "bad argument");
-  if (s->kv_fmt != LNB_KV_BF16) return fail(LNB_EINVAL, "MXFP8 KV cache: the projection benchmark writes bf16 cache rows");
+  if (s->kv.fmt != LNB_KV_BF16) return fail(LNB_EINVAL, "MXFP8 KV cache: the projection benchmark writes bf16 cache rows");
   std::lock_guard<std::mutex> lk(s->mu);
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
@@ -3702,7 +3702,7 @@ extern "C" int lnb_session_bench_kernel(lnb_session* s, int kind, int reps, floa
         case 0:
           p.x = s->x; p.ldx = a.dim; p.norm_w = W.attn_norm;
           p.out_bf16 = s->q; p.ldo = m->q_l; p.q_dim = m->q_l; p.kv_dim = m->kv_l; p.head_dim = a.head_dim;
-          p.cache_k = s->ck[l]; p.cache_v = s->cv[l]; p.cis = m->cis; p.pos_ptr = &s->st->pos;
+          p.cache_k = s->kv.bf16(l, 0, 0); p.cache_v = s->kv.bf16(l, 1, 0); p.cis = m->cis; p.pos_ptr = &s->st->pos;
           rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, s->mode, p, w, 1);
           break;
         case 1:
@@ -3821,11 +3821,11 @@ static int read_kv_decoded(lnb_session* s, int which, int layer, void* host, int
     cudaGetLastError();
     return fail(LNB_ENOMEM, "cudaMalloc(%lld) for the decoded cache rows", (long long)(chunk * row_b));
   }
-  const uint8_t* rec = (const uint8_t*)(which == LNB_BUF_CACHE_K ? s->ck[layer] : s->cv[layer]) + (size_t)s->active_seq * s->seq_len * s->kv_pos;
   cudaError_t e = cudaSuccess;
   for (int64_t r0 = 0; r0 < rows && e == cudaSuccess; r0 += chunk) {
     const int64_t n = std::min(chunk, rows - r0), off = r0 * row_b;
-    kv_dequant_kernel<<<m->sm_count * 4, 256, 0, s->stream>>>(rec + (size_t)r0 * s->kv_pos, s->kv_pos, m->kv_l, m->a.head_dim, n, d);
+    kv_dequant_kernel<<<m->sm_count * 4, 256, 0, s->stream>>>(s->kv.rec(layer, which == LNB_BUF_CACHE_V, s->active_seq, (int)r0),
+                                                              s->kv.pos_bytes, m->kv_l, m->a.head_dim, n, d);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpyAsync((uint8_t*)host + off, d, (size_t)std::min(n * row_b, nbytes - off), cudaMemcpyDeviceToHost, s->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(s->stream);
@@ -3837,24 +3837,23 @@ static int read_kv_decoded(lnb_session* s, int which, int layer, void* host, int
 
 extern "C" int lnb_session_kv_info(lnb_session* s, int* fmt, int64_t* cache_bytes) {
   if (!s) return fail(LNB_EINVAL, "session is NULL");
-  if (fmt) *fmt = s->kv_fmt;
-  if (cache_bytes)
-    *cache_bytes = (int64_t)2 * s->m->a.n_layers * s->n_seq * s->seq_len * (s->kv_fmt == LNB_KV_MXFP8 ? s->kv_pos : s->kv_pos * 2);
+  if (fmt) *fmt = s->kv.fmt;
+  if (cache_bytes) *cache_bytes = (int64_t)s->kv.bytes();
   return 0;
 }
 
 extern "C" int lnb_session_kv_read(lnb_session* s, int seq, int layer, int which, int pos0, int n, uint8_t* codes, uint8_t* scales) {
   if (!s) return fail(LNB_EINVAL, "session is NULL");
   const lnb_model* m = s->m;
-  if (s->kv_fmt != LNB_KV_MXFP8) return fail(LNB_EINVAL, "the session's KV cache is not MXFP8");
+  if (s->kv.fmt != LNB_KV_MXFP8) return fail(LNB_EINVAL, "the session's KV cache is not MXFP8");
   if (seq < 0 || seq >= s->n_seq) return fail(LNB_EINVAL, "sequence %d out of range (session has %d)", seq, s->n_seq);
   if (layer < 0 || layer >= m->a.n_layers) return fail(LNB_EINVAL, "bad layer %d", layer);
   if (which != LNB_BUF_CACHE_K && which != LNB_BUF_CACHE_V) return fail(LNB_EINVAL, "which must be LNB_BUF_CACHE_K or _V");
   if (pos0 < 0 || n < 1 || pos0 + n > s->seq_len) return fail(LNB_EINVAL, "positions [%d, %d) outside [0, %d)", pos0, pos0 + n, s->seq_len);
   CU(cudaSetDevice(m->device));
   CU(cudaStreamSynchronize(s->stream));
-  const int n_kv = m->kv_l / m->a.head_dim, nb = (m->a.head_dim + 31) / 32, rowb = s->kv_pos;
-  const uint8_t* rec = (const uint8_t*)(which == LNB_BUF_CACHE_K ? s->ck[layer] : s->cv[layer]) + ((size_t)seq * s->seq_len + pos0) * rowb;
+  const int n_kv = m->kv_l / m->a.head_dim, nb = (m->a.head_dim + 31) / 32, rowb = s->kv.pos_bytes;
+  const uint8_t* rec = s->kv.rec(layer, which == LNB_BUF_CACHE_V, seq, pos0);
   if (codes) CU(cudaMemcpy2D(codes, m->kv_l, rec, rowb, m->kv_l, n, cudaMemcpyDeviceToHost));
   if (scales) {
     std::vector<uint8_t> slots((size_t)n * n_kv * 4);
@@ -3925,9 +3924,9 @@ extern "C" int lnb_session_read(lnb_session* s, int which, int layer, void* host
     case LNB_BUF_CACHE_K:
     case LNB_BUF_CACHE_V:
       if (layer < 0 || layer >= m->a.n_layers) return fail(LNB_EINVAL, "bad layer %d", layer);
-      if (s->kv_fmt == LNB_KV_MXFP8) return read_kv_decoded(s, which, layer, host, nbytes);
-      src = (which == LNB_BUF_CACHE_K ? s->ck[layer] : s->cv[layer]) + (size_t)s->active_seq * s->seq_len * m->kv_l;
-      avail = (int64_t)s->seq_len * m->kv_l * 2;
+      if (s->kv.fmt == LNB_KV_MXFP8) return read_kv_decoded(s, which, layer, host, nbytes);
+      src = s->kv.bf16(layer, which == LNB_BUF_CACHE_V, s->active_seq);
+      avail = (int64_t)s->seq_len * s->kv.pos_bytes;
       break;
     case LNB_BUF_LOGITS: src = s->logits; avail = (int64_t)s->logits_rows * m->vocab_l * 4; break;
     default: return fail(LNB_EINVAL, "bad buffer id %d", which);
