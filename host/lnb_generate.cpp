@@ -7,7 +7,8 @@
 // temp=T [top_k=K] [top_p=P] [seed=S]: seeded sampling instead of the greedy argmax (lnb_session_set_sampling); prompt b of a
 // batch samples with seed S + b.
 // spec=K: speculative decoding -- each call verifies the last token plus up to K prompt-lookup drafts in one pass over the
-// weights (lnb_forward_speculative); the generated ids are the same as without it.  Not with slots=.
+// weights (lnb_forward_speculative); the generated ids are the same as without it.  Not with slots=.  branches=B (with spec=K):
+// each call verifies a tree of up to K prompt-lookup nodes holding the top B continuations (lnb_forward_speculative_tree).
 // rep=R freq=F pres=P [last_n=N]: repetition, frequency and presence penalties over the generated tokens (the last N positions;
 // 0, the default: all) before the sampler or the greedy pick (lnb_session_set_penalties).
 // regex=PATTERN (with <modelDir>/tokenizer.model): every generated token keeps the text a prefix of a string of
@@ -176,6 +177,7 @@ int main(int argc, char** argv) {
       if (!strncmp(argv[i], "len_pen=", 8)) beam_args.LengthPenalty = atof(argv[i] + 8);
       if (!strncmp(argv[i], "early_stop=", 11)) beam_args.EarlyStopping = atoi(argv[i] + 11) != 0;
       if (!strncmp(argv[i], "spec=", 5)) spec.MaxDraft = atoi(argv[i] + 5);
+      if (!strncmp(argv[i], "branches=", 9)) spec.Branches = atoi(argv[i] + 9);
       if (!strncmp(argv[i], "batch=", 6)) batch = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "slots=", 6)) slots = atoi(argv[i] + 6);
       if (!strncmp(argv[i], "prompt=", 7)) prompt_text = argv[i] + 7;

@@ -341,11 +341,14 @@ struct PenaltyArgs {
   }
 };
 
-// EXTENSION: speculative decoding (lnb_forward_speculative) with prompt-lookup drafts of up to MaxDraft tokens
+// EXTENSION: speculative decoding (lnb_forward_speculative) with prompt-lookup drafts of up to MaxDraft tokens.  Branches > 1:
+// trees of up to MaxDraft nodes holding the top Branches continuations (PromptLookupTree, lnb_forward_speculative_tree); not
+// with penalties, a grammar or logprobs
 struct SpeculativeArgs {
   int MaxDraft = 0;
   int NgramMax = 3;
   int NgramMin = 1;
+  int Branches = 1;
 };
 
 // Prompt-lookup drafter (the Python mirror's prompt_lookup_drafts), a pure function of the history h[0..L) whose last token
@@ -362,6 +365,47 @@ inline std::vector<int32_t> PromptLookupDrafts(const std::vector<int32_t>& h, in
     }
   }
   return {};
+}
+
+// Tree drafter (the Python mirror's prompt_lookup_tree), a pure function of the history: up to `branches` distinct
+// continuations h[j+n .. min(j+n+maxNodes, L)), for n = ngramMax down to ngramMin and within one n the matches from the most
+// recent; merged into a trie under the root (row 0), numbered breadth first (a depth's nodes in the order of the first
+// continuation that reaches them) and cut to maxNodes.  tokens[i] / parents[i]: node i is row i + 1 under row parents[i].
+// branches = 1 gives PromptLookupDrafts as a chain.
+inline void PromptLookupTree(const std::vector<int32_t>& h, int maxNodes, int branches, int ngramMax, int ngramMin,
+                             std::vector<int32_t>& tokens, std::vector<int32_t>& parents) {
+  tokens.clear();
+  parents.clear();
+  const int L = (int)h.size();
+  if (maxNodes <= 0 || branches <= 0) return;
+  std::vector<std::vector<int32_t>> conts;
+  for (int n = ngramMax; n >= std::max(ngramMin, 1) && (int)conts.size() < branches; n--) {
+    if (L < n + 1) continue;
+    for (int j = L - n - 1; j >= 0 && (int)conts.size() < branches; j--) {
+      if (!std::equal(h.begin() + j, h.begin() + j + n, h.begin() + (L - n))) continue;
+      std::vector<int32_t> c(h.begin() + j + n, h.begin() + std::min(j + n + maxNodes, L));
+      if (std::find(conts.begin(), conts.end(), c) == conts.end()) conts.push_back(c);
+    }
+  }
+  // trie nodes as (depth, rank of the first continuation reaching it, that continuation): breadth first, then rank
+  std::vector<std::pair<std::pair<int, int>, std::vector<int32_t>>> nodes;
+  for (int r = 0; r < (int)conts.size(); r++)
+    for (int d = 1; d <= (int)conts[r].size(); d++) {
+      std::vector<int32_t> key(conts[r].begin(), conts[r].begin() + d);
+      bool seen = false;
+      for (const auto& nd : nodes) seen |= nd.second == key;
+      if (!seen) nodes.push_back({{d, r}, key});
+    }
+  std::stable_sort(nodes.begin(), nodes.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  if ((int)nodes.size() > maxNodes) nodes.resize((size_t)maxNodes);
+  for (size_t i = 0; i < nodes.size(); i++) {
+    const std::vector<int32_t>& key = nodes[i].second;
+    int par = 0;
+    for (size_t k = 0; k < i; k++)
+      if (nodes[k].second.size() + 1 == key.size() && std::equal(key.begin(), key.end() - 1, nodes[k].second.begin())) par = (int)k + 1;
+    tokens.push_back(key.back());
+    parents.push_back(par);
+  }
 }
 
 // EXTENSION: regex-constrained generation (lnb_grammar_create, DESIGN.md §9g).  The tokens a sequence emits after the
@@ -487,6 +531,30 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
                                   accepted.data()));
     return next;
   }
+  // EXTENSION (tree verification, lnb_forward_speculative_tree): segment tokens = the sequence's last emitted token + the
+  // nodes, parents[s][j] the parent row of row j (parents[s][0] is not read).  -> next token of every row; accepted[i] = the
+  // depth segment i reaches, paths[i] = its accepted rows, segment-local, root first (segment i emits their next tokens)
+  std::vector<int32_t> ForwardSpeculativeTree(const std::vector<Segment>& segs, const std::vector<std::vector<int32_t>>& parents,
+                                              std::vector<int32_t>& accepted, std::vector<std::vector<int32_t>>& paths) {
+    std::vector<int32_t> seq, start, n_nodes, flat, par;
+    for (size_t k = 0; k < segs.size(); k++) {
+      const Segment& s = segs[k];
+      if (parents[k].size() != s.tokens.size()) throw Error("a tree segment needs one parent entry per row");
+      seq.push_back(s.seq);
+      start.push_back(s.startPos);
+      n_nodes.push_back((int32_t)s.tokens.size() - 1);
+      flat.insert(flat.end(), s.tokens.begin(), s.tokens.end());
+      par.insert(par.end(), parents[k].begin(), parents[k].end());
+    }
+    std::vector<int32_t> next(flat.size(), -1), path(flat.size(), -1);
+    accepted.assign(segs.size(), 0);
+    check(lnb_forward_speculative_tree(h_, (int)segs.size(), seq.data(), start.data(), n_nodes.data(), par.data(), flat.data(), nullptr,
+                                       next.data(), accepted.data(), path.data()));
+    paths.assign(segs.size(), {});
+    for (size_t k = 0, w = 0, r0 = 0; k < segs.size(); r0 += segs[k].tokens.size(), k++)
+      for (int d = 0; d <= accepted[k]; d++) paths[k].push_back(path[w++] - (int32_t)r0);
+    return next;
+  }
   // EXTENSION (lnb_session_copy_sequences): positions [pos0, pos1) of sequence dst[i] get what sequence src[i] held there
   // before the call (K and V of every layer, the penalty history, the logprob records); the sources are read as a snapshot
   void CopySequences(const std::vector<int32_t>& src, const std::vector<int32_t>& dst, int pos0, int pos1) {
@@ -542,6 +610,14 @@ class InferenceContext {  // inferencecontext.go:8-46 (KV cache in HBM)
 namespace inference {  // ---- src/inference ------------------------------------------------------------------
 enum GenerationState { GSInProgress = 0, GSFinishedByReachingEOS = 1, GSFinishedByReachingSeqLen = 2 };
 
+// speculative trees (Branches > 1) key nothing by position: not with penalties, a grammar or logprobs (keyed)
+inline void CheckSpeculativeTree(const model::SpeculativeArgs* spec, bool keyed) {
+  if (spec && spec->Branches < 1) throw Error("SpeculativeArgs.Branches must be >= 1");
+  if (spec && spec->Branches > 1 && keyed)
+    throw Error("speculative trees (Branches > 1) with penalties, a grammar or logprobs are not built: their records are keyed by "
+                "position, which sibling drafts share");
+}
+
 // The speculative loop of the Python mirror's _generate_speculative: hists[i] = the tokens of sequence i so far, its last one
 // emitted and fed next (at position size - 1); every live sequence gets a row per call, the rest of min(8, maxRows) rows go to
 // prompt-lookup drafts in sequence order, no row past position SequenceLength - 2; the accepted tokens are emitted one at a
@@ -552,21 +628,33 @@ inline void GenerateSpeculative(model::InferenceContext& infContext, const model
                                 std::vector<std::vector<lnb_logprob>>* logprobsOut = nullptr) {
   const int seqLen = infContext.SequenceLength;
   const int budget = std::min(8, infContext.MaxRows());
+  const bool tree = spec.Branches > 1;
   if ((int)live.size() > budget) throw Error("more live sequences than rows in a speculative call");
   while (!live.empty()) {
     int left = budget - (int)live.size();
     std::vector<model::InferenceContext::Segment> segs;
+    std::vector<std::vector<int32_t>> parents;
     for (int i : live) {
       const int pos = (int)hists[i].size() - 1;
-      std::vector<int32_t> toks{hists[i].back()};
-      const std::vector<int32_t> d =
-          model::PromptLookupDrafts(hists[i], std::min({spec.MaxDraft, left, seqLen - 2 - pos}), spec.NgramMax, spec.NgramMin);
+      const int k = std::min({spec.MaxDraft, left, seqLen - 2 - pos});
+      std::vector<int32_t> toks{hists[i].back()}, d, par{-1};
+      if (tree) model::PromptLookupTree(hists[i], k, spec.Branches, spec.NgramMax, spec.NgramMin, d, par);
+      else d = model::PromptLookupDrafts(hists[i], k, spec.NgramMax, spec.NgramMin);
+      if (tree) par.insert(par.begin(), -1);
       left -= (int)d.size();
       toks.insert(toks.end(), d.begin(), d.end());
       segs.push_back({i, pos, toks});
+      parents.push_back(par);
     }
     std::vector<int32_t> accepted;
-    const std::vector<int32_t> next = infContext.ForwardSpeculative(segs, accepted);
+    std::vector<std::vector<int32_t>> paths;
+    const std::vector<int32_t> next =
+        tree ? infContext.ForwardSpeculativeTree(segs, parents, accepted, paths) : infContext.ForwardSpeculative(segs, accepted);
+    if (!tree)
+      for (int32_t a : accepted) {
+        paths.emplace_back();
+        for (int d = 0; d <= a; d++) paths.back().push_back(d);
+      }
     std::vector<int> still;
     int r0 = 0;
     for (size_t k = 0; k < segs.size(); k++) {
@@ -575,7 +663,7 @@ inline void GenerateSpeculative(model::InferenceContext& infContext, const model
       std::vector<lnb_logprob> recs;   // the records of the accepted positions
       if (logprobsOut) recs = infContext.ReadLogprobs(i, segs[k].startPos + 1, accepted[k] + 1);
       for (int j = 0; j <= accepted[k] && !finished; j++) {
-        const int32_t tok = next[r0 + j];
+        const int32_t tok = next[r0 + paths[k][(size_t)j]];
         const int curPos = segs[k].startPos + 1 + j;
         hists[i].push_back(tok);
         if (logprobsOut) (*logprobsOut)[(size_t)i].push_back(recs[(size_t)j]);
@@ -604,6 +692,7 @@ inline void GenerateTokens(model::LlamaTransformer& transformer, const model::Vo
   // the prefill call carries the whole prompt: size the session's row buffers for it
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max<int>(8, (int)promptTokens.size()));
   if (penalties && penalties->Neutral()) penalties = nullptr;
+  CheckSpeculativeTree(speculative, penalties || grammar || logprobs >= 0);
   const bool samples = (sampling && sampling->Samples()) || penalties || grammar;
   if (sampling && sampling->Samples()) infContext.SetSampling(0, sampling);   // the sampled token instead of Slice + ml.Argmax
   if (penalties) infContext.SetPenalties(0, penalties, (int)promptTokens.size());
@@ -662,6 +751,7 @@ inline void GenerateTokensBatch(model::LlamaTransformer& transformer, const mode
                                 const model::PenaltyArgs* penalties = nullptr, const model::Grammar* grammar = nullptr) {
   const int n = (int)prompts.size();
   if (n < 1) throw Error("empty prompt batch");
+  CheckSpeculativeTree(speculative, (penalties && !penalties->Neutral()) || grammar || logprobs >= 0);
   model::InferenceContext infContext(transformer, sequenceLength, accMode, std::max(8, n), n);
   if (penalties)
     for (int i = 0; i < n; i++) infContext.SetPenalties(i, penalties, (int)prompts[i].size());

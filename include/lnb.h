@@ -347,6 +347,29 @@ int lnb_forward_ragged(lnb_session* s, int n_segs, const int32_t* seq, const int
 int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t* seq, const int32_t* start_pos, const int32_t* n_draft,
                             const int32_t* tokens, float* logits, int32_t* next_out, int32_t* n_accepted);
 
+/* EXTENSION: tree speculative verification.  Segment i = sequence seq[i]: row 0 feeds the sequence's last emitted token at
+ * position start_pos[i]; rows 1 .. n_nodes[i] are draft nodes, row j with parent[j] in [0, j) (per segment, row indices
+ * local to the segment), token tokens[j], depth(j) = depth(parent[j]) + 1 and position start_pos[i] + depth(j).
+ * Row j sees the cache keys [0, start_pos[i]) and the rows of its path root .. j, and nothing else.
+ * tokens and parent: segment after segment, 1 + n_nodes[i] entries each (the root's parent entry is not read).
+ * next_out[r] = the next token of row r (greedy, or sampled with p_next = its position + 1).  Acceptance: from the root,
+ * move to the child of the current node that carries the node's next token; n_accepted[i] = the depth reached, and
+ * path_out gets the accepted path's rows (call-global indices), root first: n_accepted[i] + 1 entries per segment, segment
+ * after segment.  The emitted tokens of segment i are next_out along its path.  logits: NULL or host [rows, vocab].
+ *   valid: lnb_forward_speculative's rules (total rows <= min(8, max_rows), start_pos[i] + n_nodes[i] < seq_len), parent[j]
+ *   in [0, j), siblings with distinct tokens, tp_size == 1, and no branching tree on a sequence with penalties, a grammar
+ *   or logprobs on (their records are keyed by position, which siblings share: not built).  Anything else is LNB_EINVAL
+ *   with nothing enqueued.  next_out / n_accepted / path_out may be NULL.
+ *   Every row j has the bits of the last row of lnb_forward_speculative over its path (root .. j as a chain) on the same
+ *   session state, in both modes and on every route.  Row j writes its K and V at slot start_pos + j (rotated at its
+ *   position); before the call returns, stream-ordered, ONE launch moves the accepted path's rows to positions
+ *   start_pos .. start_pos + a in every layer, so the cache then holds what the chain call over the accepted path leaves.
+ *   Rows above start_pos + a are stale, as in lnb_forward_speculative.  A call whose every tree is a chain
+ *   (parent[j] = j - 1) is lnb_forward_speculative: the same bits and launches. */
+int lnb_forward_speculative_tree(lnb_session* s, int n_segs, const int32_t* seq, const int32_t* start_pos, const int32_t* n_nodes,
+                                 const int32_t* parent, const int32_t* tokens, float* logits, int32_t* next_out, int32_t* n_accepted,
+                                 int32_t* path_out);
+
 /* Device-resident greedy decode: runs n_steps consecutive S=1 forwards starting with
  * `first_token` at position start_pos, feeding each argmax back on the device (no host
  * sync inside), optionally as CUDA-graph replays.  tokens_out[n_steps]; ms_out = device

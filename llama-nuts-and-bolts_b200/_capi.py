@@ -100,6 +100,7 @@ SIGNATURES = {
     "lnb_session_set_chunked_prefill": (C.c_int, [vp, C.c_int]),
     "lnb_forward_ragged": (C.c_int, [vp, C.c_int, i32p, i32p, i32p, i32p, f32p, i32p]),
     "lnb_forward_speculative": (C.c_int, [vp, C.c_int, i32p, i32p, i32p, i32p, f32p, i32p, i32p]),
+    "lnb_forward_speculative_tree": (C.c_int, [vp, C.c_int, i32p, i32p, i32p, i32p, i32p, f32p, i32p, i32p, i32p]),
     "lnb_session_set_sampling": (C.c_int, [vp, C.c_int, C.POINTER(SamplingC)]),
     "lnb_session_set_logprobs": (C.c_int, [vp, C.c_int, C.c_int]),
     "lnb_session_set_penalties": (C.c_int, [vp, C.c_int, C.POINTER(PenaltiesC)]),

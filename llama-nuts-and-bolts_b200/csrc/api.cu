@@ -1252,8 +1252,9 @@ __global__ void publish_kernel(LnbDevState* st, int advance, int32_t* tok_out) {
   }
 }
 
-// words of a call's row map [tokens | row_seq | row_pos | last row of each segment]: `rows` words each, <= 8 segments
-static size_t row_map_words(int max_rows) { return (size_t)max_rows * 3 + 8; }
+// words of a call's row map [tokens | row_seq | row_pos | last row of each segment | tree words]: `rows` words each, <= 8
+// segments (the tree words of a speculative tree call start at 3 * rows + 8)
+static size_t row_map_words(int max_rows) { return (size_t)max_rows * 4 + 8; }
 
 // a compiled grammar (grammar.cuh, lnb_grammar_create): its device tables, and the sequences of sessions that use it
 struct lnb_grammar {
@@ -2246,7 +2247,9 @@ static int batch_engine_build(lnb_session* s, const float* logits_out) {
   return 0;
 }
 // n rows: token tokens[m] at position pos_arr[m] on the cache of sequence row_seq[m], already on the device
-static int batch_engine_launch(lnb_session* s, int n, const int32_t* tokens, const int32_t* pos_arr, const int32_t* row_seq) {
+// (row_tree: the words of speculative tree rows, or NULL)
+static int batch_engine_launch(lnb_session* s, int n, const int32_t* tokens, const int32_t* pos_arr, const int32_t* row_seq,
+                               const int32_t* row_tree) {
   lnb_model* m = s->m;
   const lnb_model_args& a = m->a;
   BatchParams P{};
@@ -2254,7 +2257,7 @@ static int batch_engine_launch(lnb_session* s, int n, const int32_t* tokens, con
   P.emb = m->tok_embd; P.dim = a.dim; P.head_dim = a.head_dim; P.n_rep = a.n_heads / a.n_kv_heads; P.seq_len = s->seq_len;
   P.cis = m->cis; P.silu_tab = m->silu_tab; P.eps = a.norm_eps; P.attn_scale = attn_scale_bf16(a.head_dim);
   P.strict = s->mode == LNB_ACC_STRICT ? 1 : 0;
-  P.tokens = tokens; P.pos_arr = pos_arr; P.row_seq = row_seq; P.cache_seq_stride = s->kv.seq_stride();
+  P.tokens = tokens; P.pos_arr = pos_arr; P.row_seq = row_seq; P.row_tree = row_tree; P.cache_seq_stride = s->kv.seq_stride();
   P.rscale = s->rs; P.keys = s->d_bkeys; P.next_arr = s->d_next_arr; P.bar_ctr = s->d_bar;
   P.p2p = s->p2p; P.tp = m->tp_size;
   P.timeout_ns = p2p_timeout_ns();
@@ -2299,6 +2302,7 @@ struct Rows {
   const int32_t* tokens;    // device token id of each row, or NULL: st->next_token (a device-driven decode step)
   const int32_t* pos_arr;   // device position of each row, or NULL: st->pos + r
   const int32_t* row_seq;   // ragged, speculative, batched: the sequence of each row
+  const int32_t* row_tree;  // speculative tree: the slot and ancestor mask of each row (common.cuh KeyMap); else NULL
   int seq;                  // without row_seq: the sequence every row is on (the active one)
   int mb_rows;              // launch_gemv's mb_rows: ragged 8, else 0
   const int32_t* seg_last;  // ragged: the last row of each segment
@@ -2334,9 +2338,10 @@ static Rows rows_ragged(const lnb_session* s, int rows, int n_segs, const CtlSum
 // a speculative verification call or a batched step (segments of one row): the row map in d_rag, [tokens | row_seq | row_pos]
 // of `rows` words each; consecutive rows of a segment are consecutive positions of one sequence, and EVERY row is an output
 // row (a verified row's next token is compared with the following draft), so the LM head runs over all of them
-static Rows rows_spec(const lnb_session* s, int rows, const CtlSum& u) {
+static Rows rows_spec(const lnb_session* s, int rows, const CtlSum& u, bool tree) {
   Rows R{};
   R.kind = ROWS_SPEC; R.S = rows; R.tokens = s->d_rag; R.row_seq = s->d_rag + rows; R.pos_arr = s->d_rag + 2 * rows;
+  R.row_tree = tree ? s->d_rag + 3 * rows + 8 : nullptr;
   R.head = HEAD_PER_ROW; R.head_rows = rows;
   R.record = u.pen; R.grammar = u.gram;
   return R;
@@ -2350,7 +2355,7 @@ static int launch_kv_writer(const Launcher& L, lnb_session* s, int l, const Rows
   const int grid = std::min(m->sm_count * 8, std::max((tasks + 7) / 8, (R.S * m->q_l / 2 + 255) / 256));
   return launch_kernel(L, kvq_rope_store_kernel, dim3(grid), dim3(256), 0, (const uint16_t*)s->qkv_raw, m->q_l + 2 * m->kv_l, s->q,
                        m->q_l, m->kv_l, hd, s->kv.rec(l, 0, R.seq), s->kv.rec(l, 1, R.seq), (const float*)m->cis,
-                       (const int32_t*)&s->st->pos, R.S, R.pos_arr, R.row_seq, s->kv.seq_stride());
+                       (const int32_t*)&s->st->pos, R.S, R.pos_arr, R.row_seq, s->kv.seq_stride(), R.row_tree);
 }
 
 // Attention of layer l for the rows R (queries in s->q), written to out: plain rows, or the X8 operand of the tensor-core
@@ -2371,7 +2376,7 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
     StreamAttn P{};
     P.q = s->q; P.ldq = m->q_l;
     P.cache_k = kv.at(l, 0, R.seq); P.cache_v = kv.at(l, 1, R.seq); P.kv_dim = kv.pos_stride();
-    P.row_cache_stride = kv.seq_stride(); P.row_seq = R.row_seq; P.pos_arr = R.pos_arr;
+    P.row_cache_stride = kv.seq_stride(); P.row_seq = R.row_seq; P.row_tree = R.row_tree; P.pos_arr = R.pos_arr;
     P.n_rep = n_rep; P.hd = a.head_dim; P.n_heads = n_q;
     P.pos_ptr = pos_ptr; P.pos_step = 1;
     P.out = out; P.ldo = m->q_l; P.out_x8 = out_x8;
@@ -2384,7 +2389,7 @@ static int launch_attention(const Launcher& L, lnb_session* s, int l, const Rows
   if (!out_x8 && (S == 1 || spec) && s->sdpa_smem_decode)
     return launch_kernel(L, sdpa_decode_kernel, dim3(n_kv, S), dim3(128 * n_rep), s->sdpa_decode_smem, (const uint16_t*)s->q, ck, cv,
                          m->kv_l, n_rep, a.head_dim, out, pos_ptr, s->seq_len, strict, scale, R.pos_arr, kv.seq_stride(), m->q_l,
-                         (const LnbDevState*)s->st, R.row_seq);
+                         (const LnbDevState*)s->st, R.row_seq, R.row_tree);
   if (out_x8 && a.head_dim == SP_HD) {
     const double* exp_tab = sdpa_tc_enabled() ? exp_table_device() : nullptr;
     if (exp_tab)
@@ -2510,7 +2515,7 @@ static int enqueue_forward(lnb_session* s, const Rows& R) {
         if ((rc = launch_kv_writer(L, s, l, R))) return rc;
       } else {
         p.cache_k = s->kv.bf16(l, 0, R.seq); p.cache_v = s->kv.bf16(l, 1, R.seq); p.cis = m->cis; p.pos_ptr = &s->st->pos;
-        p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.cache_seq_stride = s->kv.seq_stride();
+        p.pos_arr = R.pos_arr; p.row_seq = R.row_seq; p.row_tree = R.row_tree; p.cache_seq_stride = s->kv.seq_stride();
         if ((rc = launch_gemv<PRO_RMSNORM, EPI_QKV_ROPE>(L, mode, p, W.qkv, S, mb_rows))) return rc;
       }
     }
@@ -3392,18 +3397,25 @@ static int segments_check(const lnb_session* s, const Segments& g, const int32_t
   return 0;
 }
 // the row map in d_rag, [tokens | row_seq | row_pos | last row of each segment]: one pinned staging copy (the host words stay
-// in s->h_tok for the rest of the call)
-static int stage_row_map(lnb_session* s, const Segments& g, const int32_t* tokens, int rows) {
+// in s->h_tok for the rest of the call).  A speculative tree call passes each row's depth and tree word: row r then sits at
+// position start_pos + depth[r], and the tree words follow at 3 * rows + 8.
+static int stage_row_map(lnb_session* s, const Segments& g, const int32_t* tokens, int rows, const int32_t* depth = nullptr,
+                         const int32_t* tree = nullptr) {
   int32_t* h = s->h_tok;
   memcpy(h, tokens, (size_t)rows * 4);
   for (int i = 0, r = 0; i < g.n; i++) {
     for (int k = 0; k < g.rows(i); k++, r++) {
       h[rows + r] = g.seq[i];
-      h[2 * rows + r] = g.start_pos[i] + k;
+      h[2 * rows + r] = g.start_pos[i] + (depth ? depth[r] : k);
     }
     h[3 * rows + i] = r - 1;
   }
-  CU(cudaMemcpyAsync(s->d_rag, h, (size_t)(3 * rows + g.n) * 4, cudaMemcpyHostToDevice, s->stream));
+  size_t words = (size_t)3 * rows + g.n;
+  if (tree) {
+    memcpy(h + 3 * rows + 8, tree, (size_t)rows * 4);
+    words = (size_t)4 * rows + 8;
+  }
+  CU(cudaMemcpyAsync(s->d_rag, h, words * 4, cudaMemcpyHostToDevice, s->stream));
   return 0;
 }
 
@@ -3452,8 +3464,10 @@ static int samp_grow(lnb_session* s, int rows) {
 }
 
 // The forward of a call whose every row is an output row, its segments checked (segments_check): speculative calls of >= 2
-// rows and batched steps.  The greedy (or drawn) token of row r lands in s->h_out[r] when want_tokens.
-static int forward_segments(lnb_session* s, const Segments& g, const int32_t* tokens, int rows, float* logits, bool want_tokens) {
+// rows and batched steps.  The greedy (or drawn) token of row r lands in s->h_out[r] when want_tokens.  depth / tree: a
+// speculative tree call's row depths and tree words (stage_row_map), else NULL.
+static int forward_segments(lnb_session* s, const Segments& g, const int32_t* tokens, int rows, float* logits, bool want_tokens,
+                            const int32_t* depth = nullptr, const int32_t* tree = nullptr) {
   // the batch engine for >= 2 rows (single-sequence sessions included: engine_capable already holds every position below
   // the engine's limit, eng_sdpa_smem), and for one row on a session of several sequences
   const bool eng = batch_engine_usable(s) && (rows >= 2 || s->n_seq >= 2);
@@ -3464,16 +3478,17 @@ static int forward_segments(lnb_session* s, const Segments& g, const int32_t* to
   if (u.processed && (rc = samp_grow(s, rows))) return rc;
   if ((rc = ensure_logits(s, (size_t)rows))) return rc;
   s->kept_rows = 0;   // a logits handle is valid until the session's next forward
-  if ((rc = stage_row_map(s, g, tokens, rows))) return rc;
+  if ((rc = stage_row_map(s, g, tokens, rows, depth, tree))) return rc;
+  const Rows R = rows_spec(s, rows, u, tree != nullptr);
   if (eng) {
     // ONE launch of the batch engine: every weight matrix streamed once for all rows
-    if ((rc = launch_record(s, rows_spec(s, rows, u)))) return rc;
+    if ((rc = launch_record(s, R))) return rc;
     if ((rc = batch_engine_build(s, (logits || u.processed || u.lp) ? s->logits : nullptr))) return rc;
-    if ((rc = batch_engine_launch(s, rows, s->d_rag, s->d_rag + 2 * rows, s->d_rag + rows))) return rc;
+    if ((rc = batch_engine_launch(s, rows, R.tokens, R.pos_arr, R.row_seq, R.row_tree))) return rc;
     if (logits && (rc = gather_logits(s, 0, rows))) return rc;
   } else {
     if ((rc = set_state(s, 0, rows, -1, false))) return rc;
-    if ((rc = enqueue_forward(s, rows_spec(s, rows, u)))) return rc;
+    if ((rc = enqueue_forward(s, R))) return rc;
   }
   const int32_t *row_seq = s->h_tok + rows, *row_pos = s->h_tok + 2 * rows;
   int32_t p_next[8];
@@ -3532,6 +3547,100 @@ extern "C" int lnb_forward_speculative(lnb_session* s, int n_segs, const int32_t
     while (acc < n_draft[i] && s->h_out[r0 + acc] == tokens[r0 + acc + 1]) acc++;
     if (n_accepted) n_accepted[i] = acc;
   }
+  if (next_out) memcpy(next_out, s->h_out, (size_t)rows * 4);
+  return 0;
+}
+
+// Tree verification (DESIGN.md §9c): the checks, then a call of chains only is lnb_forward_speculative itself; otherwise
+// ONE forward over the tree rows (slot start + j, position start + depth, keys through the ancestor mask), the walk on the
+// host, and ONE seqcopy_kernel launch that moves the accepted path's K and V rows to positions start .. start + a.
+extern "C" int lnb_forward_speculative_tree(lnb_session* s, int n_segs, const int32_t* seq, const int32_t* start_pos,
+                                            const int32_t* n_nodes, const int32_t* parent, const int32_t* tokens, float* logits,
+                                            int32_t* next_out, int32_t* n_accepted, int32_t* path_out) {
+  if (!s || !seq || !start_pos || !n_nodes || !parent || !tokens) return fail(LNB_EINVAL, "NULL argument");
+  lnb_model* m = s->m;
+  if (m->tp_size > 1) return fail(LNB_EINVAL, "lnb_forward_speculative_tree is not built for tensor parallelism (tp_size %d)", m->tp_size);
+  const Segments g{n_segs, seq, start_pos, n_nodes, 1};
+  int rows, rc;
+  if ((rc = segments_check(s, g, tokens, std::min(8, s->max_rows), &rows))) return rc;
+  int32_t depth[8], tree[8];
+  bool chains = true;
+  for (int i = 0, r0 = 0; i < n_segs; r0 += 1 + n_nodes[i], i++) {
+    const int n = 1 + n_nodes[i];
+    uint32_t mask[8];
+    depth[r0] = 0; mask[0] = 1u;
+    bool chain = true;
+    for (int j = 1; j < n; j++) {
+      const int pj = parent[r0 + j];
+      if (pj < 0 || pj >= j) return fail(LNB_EINVAL, "segment %d: parent[%d] = %d outside [0, %d)", i, j, pj, j);
+      for (int k = 1; k < j; k++)
+        if (parent[r0 + k] == pj && tokens[r0 + k] == tokens[r0 + j])
+          return fail(LNB_EINVAL, "segment %d: rows %d and %d are siblings with the same token %d", i, k, j, tokens[r0 + j]);
+      depth[r0 + j] = depth[r0 + pj] + 1;
+      mask[j] = mask[pj] | (1u << j);
+      chain &= pj == j - 1;
+    }
+    if (!chain) {
+      const SeqCtl& c = s->ctl[seq[i]];
+      if (c.pen || c.gram || c.lp_top >= 0)
+        return fail(LNB_EINVAL, "segment %d: sequence %d has penalties, a grammar or logprobs on, whose records are keyed by position; "
+                    "a branching tree puts siblings at one position, so this combination is not built", i, seq[i]);
+    }
+    chains &= chain;
+    for (int j = 0; j < n; j++) tree[r0 + j] = (int32_t)((uint32_t)(start_pos[i] + j) | (mask[j] << TREE_SLOT_BITS));
+  }
+  if (chains) {
+    // a tree of chains is lnb_forward_speculative: the same bits and launches; its accepted path is rows 0 .. a
+    int32_t acc[8];
+    if ((rc = lnb_forward_speculative(s, n_segs, seq, start_pos, n_nodes, tokens, logits, next_out, acc))) return rc;
+    for (int i = 0, r0 = 0, w = 0; i < n_segs; r0 += 1 + n_nodes[i], i++) {
+      if (n_accepted) n_accepted[i] = acc[i];
+      for (int d = 0; path_out && d <= acc[i]; d++) path_out[w++] = r0 + d;
+    }
+    return 0;
+  }
+  const int L = m->a.n_layers;
+  if (L > SC_MAX_LAYERS) return fail(LNB_EINVAL, "tree verification serves up to %d layers (this model has %d)", SC_MAX_LAYERS, L);
+  if (s->kv.pos_bytes % 16) return fail(LNB_EINVAL, "cache rows of %d bytes are not a multiple of 16", s->kv.pos_bytes);
+  std::lock_guard<std::mutex> lk(s->mu);
+  CU(cudaSetDevice(m->device));
+  if ((rc = forward_segments(s, g, tokens, rows, logits, true, depth, tree))) return rc;
+  // the walk: from the root, to the child that carries the node's next token (siblings are distinct: at most one); the
+  // path's K and V rows move from their slots to the positions start .. start + a, every layer, one snapshot launch
+  SeqCopyJob J{};
+  int np = 0;
+  for (int i = 0, r0 = 0, w = 0; i < n_segs; r0 += 1 + n_nodes[i], i++) {
+    const int n = 1 + n_nodes[i];
+    int u = 0, a = 0;
+    if (path_out) path_out[w++] = r0;
+    for (;;) {
+      int next = -1;
+      for (int j = u + 1; j < n && next < 0; j++)
+        if (parent[r0 + j] == u && tokens[r0 + j] == s->h_out[r0 + u]) next = j;
+      if (next < 0) break;
+      u = next;
+      a++;
+      if (path_out) path_out[w++] = r0 + u;
+      if (u != a) {
+        const int base = seq[i] * s->seq_len + start_pos[i];
+        J.src[np] = base + u;
+        J.dst[np] = base + a;
+        np++;
+      }
+    }
+    if (n_accepted) n_accepted[i] = a;
+  }
+  J.n = np;
+  J.n_kv = 2 * L;
+  J.kv_stride = s->kv.row16(); J.kv_len = s->kv.row16();
+  J.kv_tiles = (J.kv_len + SC_TILE - 1) / SC_TILE;
+  for (int l = 0; l < L; l++) {
+    J.kv[l] = reinterpret_cast<uint4*>(s->kv.rec(l, 0, 0));
+    J.kv[L + l] = reinterpret_cast<uint4*>(s->kv.rec(l, 1, 0));
+  }
+  if ((rc = launch_kernel(Launcher{s->stream, LAUNCH_PDL, &s->launches}, seqcopy_kernel, dim3((unsigned)(J.n_kv * J.kv_tiles)),
+                          dim3(SC_THREADS), 0, J)))
+    return rc;
   if (next_out) memcpy(next_out, s->h_out, (size_t)rows * 4);
   return 0;
 }

@@ -78,6 +78,35 @@ LNB_DEVINL void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint6
 LNB_DEVINL void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 LNB_DEVINL void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
+// ---- rows of a speculative tree (lnb_forward_speculative_tree, DESIGN.md §9c) ----------
+// A tree call's row map carries one word per row: the cache slot the row's K and V go to (low 24 bits) and its ancestor
+// mask (high 8 bits: the segment-local rows of its path root .. itself; ancestors precede their descendants, so the set
+// bits in ascending order ARE the path).  A row at position pos of a segment starting at base = pos + 1 - popc(mask)
+// sees logical keys 0 .. pos: key t < base is slot t, key base + d is slot base + (the d-th set bit of the mask).  Every
+// summation runs over logical keys, so a tree row computes what the chain row over its path computes.  Rows of every
+// other call carry no words (row_tree NULL): slot = position, and KeyMap's identity costs no load.
+constexpr int TREE_SLOT_BITS = 24;
+LNB_HDINL int tree_slot(int32_t w) { return w & ((1 << TREE_SLOT_BITS) - 1); }
+struct KeyMap {
+  int base = 0x7fffffff;
+  uint32_t mask = 0;
+  LNB_DEVINL int operator()(int t) const {
+    if (t < base) return t;
+    uint32_t m = mask;
+    for (int d = t - base; d > 0; d--) m &= m - 1;   // drop the lower set bits: the path's first d rows
+    return base + __ffs(m) - 1;
+  }
+};
+// the key map of row r at position pos (call only after the row map may be read: pdl_wait)
+LNB_DEVINL KeyMap key_map(const int32_t* row_tree, int r, int pos) {
+  KeyMap k;
+  if (row_tree) {
+    k.mask = (uint32_t)__ldcg(row_tree + r) >> TREE_SLOT_BITS;
+    k.base = pos + 1 - __popc(k.mask);
+  }
+  return k;
+}
+
 // ---- named barrier among a subset of the CTA -------------------------------------------
 LNB_DEVINL void named_bar_sync(int id, int nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");

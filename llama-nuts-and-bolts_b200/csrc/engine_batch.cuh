@@ -75,6 +75,7 @@ struct BatchParams {
   const int32_t* tokens;    // [n] input token of every sequence
   const int32_t* pos_arr;   // [n] position it is fed at
   const int32_t* row_seq;   // [n] sequence of every row (its KV cache)
+  const int32_t* row_tree;  // [n] speculative tree rows: slot and ancestor mask of every row (common.cuh KeyMap); else NULL
   long long cache_seq_stride;
   float* rscale;            // [8] RMSNorm scales of the running norm
   unsigned long long* keys; // [8] greedy-argmax keys (cleared by the host before the launch)
@@ -198,7 +199,7 @@ LNB_DEVINL void bt_epilogue(const GemvParams& p, int epi, const float (&v)[8], i
     if (lane < 8 && key != LNB_ARGMAX_EMPTY) atomicMax(&p.amax_keys_row[m], key);
   } else if (epi == EPI_QKV_ROPE) {
     if (valid) {
-      const int pos = p.pos_arr[m];
+      const int pos = p.pos_arr[m], slot = p.row_tree ? tree_slot(p.row_tree[m]) : pos;   // RoPE at pos, stored at slot
       uint16_t* ck = p.cache_k + be_cache_base(p.row_seq, m, p.cache_seq_stride);
       uint16_t* cv = p.cache_v + be_cache_base(p.row_seq, m, p.cache_seq_stride);
       uint32_t o[4];
@@ -216,12 +217,12 @@ LNB_DEVINL void bt_epilogue(const GemvParams& p, int epi, const float (&v)[8], i
           const float re = (float)(a * cc - b * dd), im = (float)(a * dd + b * cc);
           o[i] = (__float_as_uint(re) >> 16) | (__float_as_uint(im) & 0xffff0000u);
         }
-        uint16_t* dst = (n0 < p.q_dim) ? p.out_bf16 + cm_idx(m, n0) : ck + (size_t)pos * p.kv_dim + nn0;          // SetSlice :402
+        uint16_t* dst = (n0 < p.q_dim) ? p.out_bf16 + cm_idx(m, n0) : ck + (size_t)slot * p.kv_dim + nn0;         // SetSlice :402
         *reinterpret_cast<uint4*>(dst) = make_uint4(o[0], o[1], o[2], o[3]);
       } else {
 #pragma unroll
         for (int i = 0; i < 4; i++) o[i] = (__float_as_uint(v[2 * i]) >> 16) | (__float_as_uint(v[2 * i + 1]) & 0xffff0000u);
-        *reinterpret_cast<uint4*>(cv + (size_t)pos * p.kv_dim + (n0 - p.q_dim - p.kv_dim)) = make_uint4(o[0], o[1], o[2], o[3]);   // :403
+        *reinterpret_cast<uint4*>(cv + (size_t)slot * p.kv_dim + (n0 - p.q_dim - p.kv_dim)) = make_uint4(o[0], o[1], o[2], o[3]);  // :403
       }
     }
   } else if (epi == EPI_SWIGLU) {
@@ -462,7 +463,7 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
             g.out_bf16 = E->out; g.out_f32 = E->out_f32; g.ldo = E->ldo; g.res = E->res; g.cm = 1;
             g.q_dim = E->q_dim; g.kv_dim = E->kv_dim; g.head_dim = P.head_dim;
             g.cache_k = E->cache_k; g.cache_v = E->cache_v; g.pos_arr = P.pos_arr; g.cache_seq_stride = P.cache_seq_stride;
-            g.row_seq = P.row_seq;
+            g.row_seq = P.row_seq; g.row_tree = P.row_tree;
             g.cis = P.cis; g.silu_tab = P.silu_tab;
             g.n_offset = E->n_offset; g.st = nullptr; g.argmax_row = -1; g.amax_keys_row = P.keys;
             g.pos_ptr = P.pos_arr; g.m_off = 0;
@@ -593,7 +594,7 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
           g.out_bf16 = E->out; g.out_f32 = E->out_f32; g.ldo = E->ldo; g.res = E->res; g.cm = 1;
           g.q_dim = E->q_dim; g.kv_dim = E->kv_dim; g.head_dim = P.head_dim;
           g.cache_k = E->cache_k; g.cache_v = E->cache_v; g.pos_arr = P.pos_arr; g.cache_seq_stride = P.cache_seq_stride;
-          g.row_seq = P.row_seq;
+          g.row_seq = P.row_seq; g.row_tree = P.row_tree;
           g.cis = P.cis; g.silu_tab = P.silu_tab;
           g.n_offset = E->n_offset; g.st = nullptr; g.argmax_row = -1; g.amax_keys_row = P.keys;
           g.pos_ptr = P.pos_arr; g.m_off = 0;
@@ -756,12 +757,14 @@ __global__ void __launch_bounds__(ENG_THREADS, 1) batch_engine_kernel(const Batc
       for (int item = bid; item < n_qh * n; item += G) {
         const int H = item % n_qh, m = item / n_qh, h = H / n_rep;
         const int T = P.pos_arr[m] + 1;   // keys 0 .. pos: earlier rows of the same sequence appended theirs in the QKV phase
+        const KeyMap km = key_map(P.row_tree, m, T - 1);   // tree rows: key t from slot km(t)
         const uint16_t* ck = E->cache_k + be_cache_base(P.row_seq, m, P.cache_seq_stride);
         const uint16_t* cv = E->cache_v + be_cache_base(P.row_seq, m, P.cache_seq_stride);
         for (int i = c; i < T * cpr; i += ENG_NCONS) {
           const int t = i / cpr, cc = i % cpr;
-          *reinterpret_cast<uint4*>(sK + (size_t)t * kstride + cc * 8) = ldcg_u4(ck + (size_t)t * E->kv_dim + (size_t)h * hd + cc * 8);
-          *reinterpret_cast<uint4*>(sV + (size_t)t * hd + cc * 8) = ldcg_u4(cv + (size_t)t * E->kv_dim + (size_t)h * hd + cc * 8);
+          const size_t kt = (size_t)km(t) * E->kv_dim + (size_t)h * hd + cc * 8;
+          *reinterpret_cast<uint4*>(sK + (size_t)t * kstride + cc * 8) = ldcg_u4(ck + kt);
+          *reinterpret_cast<uint4*>(sV + (size_t)t * hd + cc * 8) = ldcg_u4(cv + kt);
         }
         for (int d = c; d < hd; d += ENG_NCONS) sQ[d] = bf2f(ldcg_u16(E->x + cm_idx(m, H * hd + d)));
         named_bar_sync(1, ENG_NCONS);

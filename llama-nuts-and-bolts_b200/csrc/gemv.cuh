@@ -70,6 +70,7 @@ struct GemvParams {
   const int32_t* pos_arr;  // batched decode (one row per independent sequence): position of row m; NULL -> *pos_ptr + m
   long long cache_seq_stride;  // elements between the caches of consecutive sequences (batched decode)
   const int32_t* row_seq;  // rows of several sequences: row m's sequence (cache at + row_seq[m] * cache_seq_stride); NULL: cache_k
+  const int32_t* row_tree; // with pos_arr, speculative tree rows: K and V of row m go to slot tree_slot(row_tree[m]); NULL: pos
   const float* cis;        // [rows][head_dim/2][2]
   // EPI_SWIGLU
   const uint16_t* silu_tab;
@@ -194,7 +195,13 @@ LNB_DEVINL void gemv_epilogue(const GemvParams& p, float v, int n, int em, bool 
     const float other = __shfl_xor_sync(0xffffffffu, mine, 1);
     if (valid) {
       const int row = p.m_off + em;
-      const int pos = p.pos_arr ? p.pos_arr[row] : *p.pos_ptr + row;
+      int pos, slot;   // RoPE at the position, the cache row at the slot
+      if (p.pos_arr) {
+        pos = p.pos_arr[row];
+        slot = p.row_tree ? tree_slot(p.row_tree[row]) : pos;
+      } else {
+        pos = slot = *p.pos_ptr + row;
+      }
       const size_t cb = p.row_seq ? (size_t)p.row_seq[row] * (size_t)p.cache_seq_stride : 0;
       uint16_t* ck = p.cache_k + cb;
       uint16_t* cv = p.cache_v + cb;
@@ -213,10 +220,10 @@ LNB_DEVINL void gemv_epilogue(const GemvParams& p, float v, int n, int em, bool 
         }
         if (p.out_t) p.out_t[n] = p.tag_hi | f2bf(o);                   // engine: q, and this step's k row for the attention phase
         if (n < p.q_dim) { if (!p.out_t) p.out_bf16[p.cm ? cm_idx(p.m_off + em, n) : (size_t)em * p.ldo + n] = f2bf(o); }
-        else ck[(size_t)pos * p.kv_dim + nn] = f2bf(o);                  // SetSlice :402
+        else ck[(size_t)slot * p.kv_dim + nn] = f2bf(o);                 // SetSlice :402
       } else {
         if (p.out_t) p.out_t[n] = p.tag_hi | f2bf(mine);
-        cv[(size_t)pos * p.kv_dim + (n - p.q_dim - p.kv_dim)] = f2bf(mine);         // :403
+        cv[(size_t)slot * p.kv_dim + (n - p.q_dim - p.kv_dim)] = f2bf(mine);        // :403
       }
     }
   } else if (EPI == EPI_SWIGLU) {

@@ -195,7 +195,8 @@ __global__ void __launch_bounds__(1024) sdpa_decode_kernel(const uint16_t* __res
                                                            uint16_t* __restrict__ out, const int32_t* __restrict__ pos_ptr,
                                                            int T_max, int strict, float scale_bf16_as_f32,
                                                            const int32_t* __restrict__ pos_arr, long long cache_seq_stride, int ldq,
-                                                           const LnbDevState* __restrict__ st, const int32_t* __restrict__ row_seq) {
+                                                           const LnbDevState* __restrict__ st, const int32_t* __restrict__ row_seq,
+                                                           const int32_t* __restrict__ row_tree) {
   extern __shared__ __align__(16) uint8_t sm[];
   const int kstride = hd + 8;
   uint16_t* sK = reinterpret_cast<uint16_t*>(sm);                       // [T_max][hd + 8]
@@ -236,10 +237,12 @@ __global__ void __launch_bounds__(1024) sdpa_decode_kernel(const uint16_t* __res
   const int pos = __ldcg(pos_ptr);
   const int T = pos + 1;
   const int lo = min(safe, T);
+  const KeyMap km = key_map(row_tree, blockIdx.y, pos);   // tree rows: key t from slot km(t) (row_tree implies pos_arr)
   for (int i = tid; i < (T - lo) * cpr; i += nthr) {
     const int t = lo + i / cpr, c = i % cpr;
-    cp_async16(sK + (size_t)t * kstride + c * 8, cache_k + (size_t)t * kv_dim + (size_t)h * hd + c * 8);
-    cp_async16(sV + (size_t)t * hd + c * 8, cache_v + (size_t)t * kv_dim + (size_t)h * hd + c * 8);
+    const size_t kt = (size_t)km(t) * kv_dim + (size_t)h * hd + c * 8;
+    cp_async16(sK + (size_t)t * kstride + c * 8, cache_k + kt);
+    cp_async16(sV + (size_t)t * hd + c * 8, cache_v + kt);
   }
   for (int i = tid; i < n_rep * hd; i += nthr) sQ[i] = bf2f(q[(size_t)(h * n_rep) * hd + i]);
   cp_async_wait_all();

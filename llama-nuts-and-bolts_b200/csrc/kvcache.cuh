@@ -55,12 +55,14 @@ LNB_DEVINL uint32_t kvq_block(uint32_t v, bool valid, uint8_t* code, uint8_t* sc
 
 // The cache writer of a quantized session, after the wq|wk|wv projection wrote its bf16 rows to qkv ([S][ld], columns
 // q | k | v): q rotated -> q_out [S][q_dim] (rope_kv_kernel's arithmetic), k rotated and v quantized into the record of
-// (row_seq[s], row_pos[s]) or (the cache at `cache`, pos0 + s).  Threads of the first loop own q pairs; warps of the
+// (row_seq[s], row_pos[s]) or (the cache at `cache`, pos0 + s); a speculative tree row rotates at its position and stores
+// at its slot (row_tree, common.cuh).  Threads of the first loop own q pairs; warps of the
 // second own (row, K or V, KV head, block).  Waits for the projection before any global access (PDL).
 __global__ void kvq_rope_store_kernel(const uint16_t* __restrict__ qkv, int ld, uint16_t* __restrict__ q_out, int q_dim, int kv_dim,
                                       int head_dim, uint8_t* __restrict__ cache_k, uint8_t* __restrict__ cache_v,
                                       const float* __restrict__ cis, const int32_t* __restrict__ pos_ptr, int S,
-                                      const int32_t* __restrict__ row_pos, const int32_t* __restrict__ row_seq, long long seq_stride) {
+                                      const int32_t* __restrict__ row_pos, const int32_t* __restrict__ row_seq, long long seq_stride,
+                                      const int32_t* __restrict__ row_tree) {
   pdl_launch_dependents();
   pdl_wait();
   const int pos0 = row_pos ? 0 : *pos_ptr;
@@ -90,7 +92,8 @@ __global__ void kvq_rope_store_kernel(const uint16_t* __restrict__ qkv, int ld, 
         v = (lane & 1) ? o >> 16 : o & 0xffffu;
       }
     }
-    uint8_t* rec = (which ? cache_v : cache_k) + (row_seq ? (size_t)row_seq[s] * (size_t)seq_stride : 0) + (size_t)pos * rowb;
+    const int slot = row_tree ? tree_slot(row_tree[s]) : pos;
+    uint8_t* rec = (which ? cache_v : cache_k) + (row_seq ? (size_t)row_seq[s] * (size_t)seq_stride : 0) + (size_t)slot * rowb;
     kvq_block(v, valid, rec + h * head_dim + b * 32, rec + kv_dim + h * 4 + b, lane);
   }
 }

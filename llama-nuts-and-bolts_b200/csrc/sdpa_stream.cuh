@@ -6,7 +6,8 @@
 // (cache + row_seq[r] * row_cache_stride: batched, ragged and speculative calls, where rows of one sequence follow each
 // other; cache without a row map) and its own position p_r (pos_arr[r], or base + pos_step * r: S = 1
 // decode, a prompt or chunked prefill under the [S,T] mask, or pos_step = 0 for the op's unmasked form) and sees keys
-// 0..p_r.  The arithmetic is sdpa_kernel's (llamatransformer.go:459-514):
+// 0..p_r (a speculative tree row reads key t from slot KeyMap(t) of its row_tree word, common.cuh).  The arithmetic is
+// sdpa_kernel's (llamatransformer.go:459-514):
 //   sc_t = t( t(sum_seq_d q_d k_td) / t(sqrt(hd)) );  e_t = exp_f64(sc_t);  p_t = t(f32(e_t / Z));  o_d = t(sum_t p_t v_td)
 // Because sc_t is a bf16 value, e_t is recomputed from the 2-byte score wherever it is needed instead of being kept
 // as 8 bytes.  Three launches per group of rows, all reading and writing a per-session scratch:
@@ -44,6 +45,7 @@ struct StreamAttn {
   int kv_dim;
   long long row_cache_stride;   // elements between the caches of consecutive sequences
   const int32_t* row_seq;       // rows of several sequences: row r reads the cache of sequence row_seq[r]; NULL: cache_k
+  const int32_t* row_tree;      // speculative tree rows: row r's slot and ancestor mask (common.cuh KeyMap); NULL: key t = slot t
   int n_rep, hd, n_heads;       // n_heads: query heads of this rank
   const int32_t* pos_arr;       // per-row positions, or NULL:
   const int32_t* pos_ptr;       //   p_r = (pos_ptr ? *pos_ptr : pos_fixed) + pos_step * r
@@ -64,6 +66,7 @@ LNB_DEVINL int ss_keys(const StreamAttn& P, int r) {   // keys row r sees (call 
   const int p = P.pos_arr ? __ldcg(P.pos_arr + r) : (P.pos_ptr ? __ldcg(P.pos_ptr) : P.pos_fixed) + P.pos_step * r;
   return p + 1;
 }
+LNB_DEVINL KeyMap ss_key_map(const StreamAttn& P, int r, int T) { return key_map(P.row_tree, r, T - 1); }   // (after pdl_wait)
 LNB_DEVINL size_t ss_cache_base(const StreamAttn& P, int r) {   // (call only after pdl_wait)
   return P.row_seq ? (size_t)__ldcg(P.row_seq + r) * (size_t)P.row_cache_stride : 0;
 }
@@ -91,16 +94,16 @@ LNB_DEVINL void ss_cp8(void* smem_dst, const void* gsrc) {
 LNB_DEVINL void ss_cp4(void* smem_dst, const void* gsrc) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
 }
-// MXFP8: issue the copies of keys [k0, k0 + n) of head h (records at rec, rowb bytes apart; codes of the head's columns
-// [c0, c0 + w)) into codes [n][w] and slots [n]
-LNB_DEVINL void ss_issue_fp8(const uint8_t* rec, int rowb, int kv_l, int h, int hd, int c0, int w, int k0, int n, uint8_t* codes,
-                             uint32_t* slots, int tid, int nthr) {
+// MXFP8: issue the copies of keys [k0, k0 + n) of head h (key t in the record at slot km(t) of rec, rowb bytes apart; codes
+// of the head's columns [c0, c0 + w)) into codes [n][w] and slots [n]
+LNB_DEVINL void ss_issue_fp8(const uint8_t* rec, int rowb, int kv_l, int h, int hd, int c0, int w, int k0, int n, const KeyMap& km,
+                             uint8_t* codes, uint32_t* slots, int tid, int nthr) {
   const int cpr = w / 8;
   for (int i = tid; i < n * cpr; i += nthr) {
     const int t = i / cpr, cc = i % cpr;
-    ss_cp8(codes + (size_t)t * w + cc * 8, rec + (size_t)(k0 + t) * rowb + h * hd + c0 + cc * 8);
+    ss_cp8(codes + (size_t)t * w + cc * 8, rec + (size_t)km(k0 + t) * rowb + h * hd + c0 + cc * 8);
   }
-  for (int t = tid; t < n; t += nthr) ss_cp4(slots + t, rec + (size_t)(k0 + t) * rowb + kv_l + h * 4);
+  for (int t = tid; t < n; t += nthr) ss_cp4(slots + t, rec + (size_t)km(k0 + t) * rowb + kv_l + h * 4);
 }
 // MXFP8: decode the copied codes [n][w] (columns [c0, c0 + w) of the head) into the bf16 tile [n][ld]
 LNB_DEVINL void ss_decode_fp8(const uint8_t* codes, const uint32_t* slots, int c0, int w, int n, uint16_t* out, int ld, int tid, int nthr) {
@@ -125,6 +128,7 @@ __global__ void __launch_bounds__(SS_KT) ss_scores_kernel(const StreamAttn P) {
   const int t0 = c * SS_CH;
   if (t0 >= T) return;
   const int t1 = min(T, t0 + SS_CH);
+  const KeyMap km = ss_key_map(P, r, T);
   const int hd = P.hd, n_rep = P.n_rep, ks = hd + 8, cpr = hd / 8;
   uint16_t* sK = reinterpret_cast<uint16_t*>(sm);                     // [SS_KT][hd + 8]
   float* sQ = reinterpret_cast<float*>(sK + (size_t)SS_KT * ks);      // [n_rep][hd]
@@ -140,11 +144,11 @@ __global__ void __launch_bounds__(SS_KT) ss_scores_kernel(const StreamAttn P) {
     const int n = min(SS_KT, t1 - k0);
     __syncthreads();
     if constexpr (KVF == KVF_MXFP8) {
-      ss_issue_fp8(kr8, P.kv_dim, P.n_heads / n_rep * hd, h, hd, 0, hd, k0, n, sC, sSl, tid, SS_KT);
+      ss_issue_fp8(kr8, P.kv_dim, P.n_heads / n_rep * hd, h, hd, 0, hd, k0, n, km, sC, sSl, tid, SS_KT);
     } else {
       for (int i = tid; i < n * cpr; i += SS_KT) {
         const int t = i / cpr, cc = i % cpr;
-        ss_cp16(sK + (size_t)t * ks + cc * 8, kb + (size_t)(k0 + t) * P.kv_dim + cc * 8);
+        ss_cp16(sK + (size_t)t * ks + cc * 8, kb + (size_t)km(k0 + t) * P.kv_dim + cc * 8);
       }
     }
     ss_cp_commit();
@@ -260,6 +264,7 @@ __global__ void __launch_bounds__(1024) ss_out_kernel(const StreamAttn P, int ds
     if (t0 >= T) return;
     t1 = min(T, t0 + SS_CH);
   }
+  const KeyMap km = ss_key_map(P, r, T);
   uint16_t* sV = reinterpret_cast<uint16_t*>(sm);                       // [2][SS_VT][dw]
   uint16_t* sS = sV + (size_t)2 * SS_VT * dw;                           // [2][n_rep][SS_VT] raw bf16 (score or p)
   float* sP = reinterpret_cast<float*>(sS + (size_t)2 * n_rep * SS_VT); // [n_rep][SS_VT]
@@ -278,13 +283,13 @@ __global__ void __launch_bounds__(1024) ss_out_kernel(const StreamAttn P, int ds
   auto issue = [&](int k0, int stage) {
     const int n = min(SS_VT, t1 - k0);
     if constexpr (KVF == KVF_MXFP8) {
-      ss_issue_fp8(vr8, P.kv_dim, P.n_heads / n_rep * P.hd, h, P.hd, g * dw, dw, k0, n, sC + (size_t)stage * SS_VT * dw,
+      ss_issue_fp8(vr8, P.kv_dim, P.n_heads / n_rep * P.hd, h, P.hd, g * dw, dw, k0, n, km, sC + (size_t)stage * SS_VT * dw,
                    sSl + stage * SS_VT, tid, nthr);
     } else {
       uint16_t* v = sV + (size_t)stage * SS_VT * dw;
       for (int i = tid; i < n * cpr; i += nthr) {
         const int t = i / cpr, cc = i % cpr;
-        ss_cp16(v + (size_t)t * dw + cc * 8, vb + (size_t)(k0 + t) * P.kv_dim + cc * 8);
+        ss_cp16(v + (size_t)t * dw + cc * 8, vb + (size_t)km(k0 + t) * P.kv_dim + cc * 8);
       }
     }
     uint16_t* s = sS + (size_t)stage * n_rep * SS_VT;

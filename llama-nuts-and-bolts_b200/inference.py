@@ -23,10 +23,14 @@ PenaltyArgs = model_mod.PenaltyArgs
 class SpeculativeArgs:
     """EXTENSION: speculative decoding (lnb_forward_speculative).  Each call feeds a sequence's last token plus up to MaxDraft
     tokens drafted by prompt lookup (prompt_lookup_drafts, n-grams of NgramMax down to NgramMin tokens) and keeps the drafts
-    the model agrees with.  Every verified row has the bits of the plain step, so the generated stream is the plain one."""
+    the model agrees with.  Every verified row has the bits of the plain step, so the generated stream is the plain one.
+    Branches > 1: each call verifies a tree of up to MaxDraft nodes holding the top Branches distinct continuations
+    (prompt_lookup_tree, lnb_forward_speculative_tree) and keeps its longest path the model agrees with; not with
+    penalties, a grammar or logprobs.  Branches = 1 issues exactly the chain calls."""
     MaxDraft: int
     NgramMax: int = 3
     NgramMin: int = 1
+    Branches: int = 1
 
 
 @dataclass
@@ -132,6 +136,48 @@ def prompt_lookup_drafts(history, max_draft: int, ngram_max: int = 3, ngram_min:
     return []
 
 
+def prompt_lookup_tree(history, max_nodes: int, branches: int = 1, ngram_max: int = 3,
+                       ngram_min: int = 1) -> tuple[list[int], list[int]]:
+    """Tree drafter, a pure function of the token history h[0..L) (h[L-1] is the token about to be fed): up to `branches`
+    distinct continuations, for n = ngram_max down to ngram_min and within one n the matches j (j + n < L,
+    h[j..j+n) == h[L-n..L)) from the most recent, each h[j+n .. min(j+n+max_nodes, L)).  They are merged into a trie under
+    the root (row 0, the fed token); its nodes are numbered breadth first, a depth's nodes in the order of the first
+    continuation that reaches them, so every parent precedes its children, and the first max_nodes nodes are kept.
+    Returns (tokens, parents) of the kept nodes: node i is row i + 1, under row parents[i].  branches = 1 gives
+    prompt_lookup_drafts as a chain."""
+    h = [int(t) for t in np.asarray(history, np.int64).reshape(-1)]
+    L = len(h)
+    if max_nodes <= 0 or branches <= 0:
+        return [], []
+    conts = []
+    for n in range(ngram_max, max(ngram_min, 1) - 1, -1):
+        if L < n + 1:
+            continue
+        suffix = h[L - n:]
+        for j in range(L - n - 1, -1, -1):
+            if h[j:j + n] == suffix:
+                c = h[j + n:min(j + n + max_nodes, L)]
+                if c not in conts:
+                    conts.append(c)
+                    if len(conts) == branches:
+                        break
+        if len(conts) == branches:
+            break
+    # the trie: key = the token path from the root; a node's rank = the first continuation that reaches it
+    nodes = {}
+    for rank, c in enumerate(conts):
+        for d in range(1, len(c) + 1):
+            nodes.setdefault(tuple(c[:d]), rank)
+    order = sorted(nodes, key=lambda k: (len(k), nodes[k]))[:max_nodes]
+    row = {(): 0}
+    tokens, parents = [], []
+    for k in order:
+        row[k] = len(tokens) + 1
+        tokens.append(k[-1])
+        parents.append(row[k[:-1]])
+    return tokens, parents
+
+
 def _sampling_for(sampling, i: int):
     """prompt i of a batch or continuous run samples with Seed + i: its stream is GenerateTokens(prompts[i]) with that seed"""
     if sampling is None or sampling.Temperature == 0:
@@ -169,13 +215,17 @@ def _set_penalties(infContext, seq: int, penalties: "PenaltyArgs | None", prompt
         infContext.set_penalties(seq, penalties, prompt_len)
 
 
-def _check_speculative(speculative, use_reference_api: bool = False):
+def _check_speculative(speculative, use_reference_api: bool = False, keyed: bool = False):
+    """keyed: the run has penalties, a grammar or logprobs on, whose records are keyed by position (no trees)"""
     if speculative is None:
         return
     if use_reference_api:
         raise ml.MlError("use_reference_api=True runs the reference's Forward -> Slice -> ml.Argmax calls; it cannot verify drafts")
-    if speculative.MaxDraft < 0 or not 1 <= speculative.NgramMin <= speculative.NgramMax:
-        raise ml.MlError(f"SpeculativeArgs {speculative}: MaxDraft must be >= 0 and 1 <= NgramMin <= NgramMax")
+    if speculative.MaxDraft < 0 or not 1 <= speculative.NgramMin <= speculative.NgramMax or speculative.Branches < 1:
+        raise ml.MlError(f"SpeculativeArgs {speculative}: MaxDraft must be >= 0, 1 <= NgramMin <= NgramMax and Branches >= 1")
+    if speculative.Branches > 1 and keyed:
+        raise ml.MlError("speculative trees (Branches > 1) with penalties, a grammar or logprobs are not built: their records "
+                         "are keyed by position, which sibling drafts share")
 
 # Row budget of one GenerateTokensContinuous step.  FAST ragged steps of >= 32 rows run on the tensor cores (one pass over
 # the weights); steps of 9..31 rows run the GEMV chain, which streams the weights once per 8 rows (up to 4 passes), and
@@ -303,7 +353,7 @@ class InferenceEngine:
             raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax of the raw logits; it cannot apply penalties")
         if grammar is not None and use_reference_api:
             raise ml.MlError("use_reference_api=True ends in the greedy ml.Argmax of the raw logits; it cannot apply a grammar")
-        _check_speculative(speculative, use_reference_api)
+        _check_speculative(speculative, use_reference_api, penalties is not None or grammar is not None or logprobs is not None)
         infContext = self.CreateInferenceContext()
         try:
             if sampling is not None:
@@ -446,16 +496,17 @@ class InferenceEngine:
 
     def _generate_speculative(self, infContext, hists, live, speculative: "SpeculativeArgs", step_times: list | None = None,
                               spec_stats: list | None = None, lp_out: list | None = None):
-        """The speculative loop on a given context (anything with SequenceLength, max_rows and forward_speculative).
-        hists[i]: the tokens of sequence i so far, its last one emitted and not yet fed (it is fed at position
-        len(hists[i]) - 1); live: the sequences still generating, each gets a row in every call.  The rows left of the
-        budget min(8, max_rows) go to drafts in sequence order, clamped so that no row passes position SequenceLength - 2
-        (the last position the plain loop feeds).  Yields (sequence, state, token) per emitted token, a segment's accepted
-        tokens in order; hists grow with them.  lp_out (or None): per sequence, the list that gets the logprob record of each
-        emitted token (the records of the accepted positions)."""
+        """The speculative loop on a given context (anything with SequenceLength, max_rows and forward_speculative, or
+        forward_speculative_tree when Branches > 1).  hists[i]: the tokens of sequence i so far, its last one emitted and not
+        yet fed (it is fed at position len(hists[i]) - 1); live: the sequences still generating, each gets a row in every
+        call.  The rows left of the budget min(8, max_rows) go to drafts (tree nodes) in sequence order, clamped so that no
+        row passes position (tree: slot) SequenceLength - 2 (the last position the plain loop feeds).  Yields (sequence,
+        state, token) per emitted token, a segment's accepted tokens in order; hists grow with them.  lp_out (or None): per
+        sequence, the list that gets the logprob record of each emitted token (the records of the accepted positions)."""
         seqLen = infContext.SequenceLength
         stop = self.model.Vocabulary.StopTokenIds
         budget = min(SPEC_MAX_ROWS, infContext.max_rows)
+        tree = speculative.Branches > 1
         live = list(live)
         if len(live) > budget:
             raise ml.MlError(f"{len(live)} sequences do not fit the row budget {budget} of a speculative call")
@@ -466,21 +517,30 @@ class InferenceEngine:
                 h = hists[i]
                 pos = len(h) - 1
                 k = min(speculative.MaxDraft, left, seqLen - 2 - pos)
-                drafts = prompt_lookup_drafts(h, k, speculative.NgramMax, speculative.NgramMin)
+                if tree:
+                    drafts, parents = prompt_lookup_tree(h, k, speculative.Branches, speculative.NgramMax, speculative.NgramMin)
+                    segs.append((i, pos, [h[-1]] + drafts, [-1] + parents))
+                else:
+                    drafts = prompt_lookup_drafts(h, k, speculative.NgramMax, speculative.NgramMin)
+                    segs.append((i, pos, [h[-1]] + drafts))
                 left -= len(drafts)
-                segs.append((i, pos, [h[-1]] + drafts))
             t0 = time.perf_counter()
-            nxt, acc, _ = infContext.forward_speculative(segs)
+            if tree:
+                nxt, acc, paths, _ = infContext.forward_speculative_tree(segs)
+            else:
+                nxt, acc, _ = infContext.forward_speculative(segs)
+                paths = [list(range(int(a) + 1)) for a in acc]
             if step_times is not None:
                 step_times.append(time.perf_counter() - t0)
             if spec_stats is not None:
-                spec_stats.append((sum(len(t) for _, _, t in segs), int(sum(int(a) for a in acc))))
+                spec_stats.append((sum(len(sg[2]) for sg in segs), int(sum(int(a) for a in acc))))
             still, r0 = [], 0
-            for (i, pos, toks), a in zip(segs, acc):
+            for sg, a, path in zip(segs, acc, paths):
+                i, pos, toks = sg[0], sg[1], sg[2]
                 finished = False
                 recs = infContext.read_logprobs(i, pos + 1, int(a) + 1) if lp_out is not None else None
-                for j in range(int(a) + 1):            # the next tokens of rows 0 .. a, one at a time (:218-248)
-                    tok, curPos = int(nxt[r0 + j]), pos + 1 + j
+                for j in range(int(a) + 1):            # the next tokens of the path's rows, one at a time (:218-248)
+                    tok, curPos = int(nxt[r0 + path[j]]), pos + 1 + j
                     hists[i].append(tok)
                     if recs is not None:
                         lp_out[i].append(recs[j])
@@ -625,7 +685,7 @@ class InferenceEngine:
         are the same.  spec_stats as in GenerateTokens; logprobs / logprobs_out as in GenerateTokens, logprobs_out gets one
         list per prompt; penalties as in GenerateTokens, for every sequence; grammar: one model.Grammar for every
         sequence or one per prompt (None entries: unconstrained)."""
-        _check_speculative(speculative)
+        _check_speculative(speculative, False, penalties is not None or grammar is not None or logprobs is not None)
         n = len(prompts)
         if n < 1:
             raise ml.MlError("empty prompt batch")

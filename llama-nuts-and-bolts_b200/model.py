@@ -468,6 +468,38 @@ class InferenceContext:
                                           ptr(nxt, _capi.i32p), ptr(acc, _capi.i32p)))
         return nxt, acc, logits
 
+    def forward_speculative_tree(self, segments, want_logits: bool = False):
+        """EXTENSION (tree speculative verification, lnb_forward_speculative_tree): ONE forward over segments
+        (seq, start_pos, tokens, parent): tokens[0] is the sequence's last emitted token (the root, parent[0] is not read),
+        node j > 0 carries tokens[j] under parent[j] in [0, j), at position start_pos + its depth.  Returns (next token of
+        every row [rows], accepted depth of every segment [n_segs], the accepted path of every segment as segment-local
+        rows, root first, logits [rows, vocab] or None); segment i emits the next tokens of its path's rows."""
+        n = len(segments)
+        seq = np.array([s for s, _, _, _ in segments], np.int32)
+        start = np.array([p for _, p, _, _ in segments], np.int32)
+        toks = [np.asarray(t, np.int32).reshape(-1) for _, _, t, _ in segments]
+        n_nodes = np.array([len(t) - 1 for t in toks], np.int32)
+        flat = np.ascontiguousarray(np.concatenate(toks) if toks else np.zeros(0, np.int32), np.int32)
+        par = np.ascontiguousarray(np.concatenate([np.asarray(q, np.int32).reshape(-1) for _, _, _, q in segments])
+                                   if segments else np.zeros(0, np.int32), np.int32)
+        rows = flat.shape[0]
+        if par.shape[0] != rows:
+            raise ml.MlError(f"forward_speculative_tree: {par.shape[0]} parent entries for {rows} rows")
+        nxt = np.empty(rows, np.int32)
+        acc = np.empty(n, np.int32)
+        path = np.empty(rows, np.int32)
+        logits = np.empty((rows, self.transformer.args.VocabSize), np.float32) if want_logits else None
+        check(lib.lnb_forward_speculative_tree(self.h, n, ptr(seq, _capi.i32p), ptr(start, _capi.i32p),
+                                               ptr(n_nodes, _capi.i32p), ptr(par, _capi.i32p), ptr(flat, _capi.i32p),
+                                               ptr(logits, _capi.f32p) if want_logits else None, ptr(nxt, _capi.i32p),
+                                               ptr(acc, _capi.i32p), ptr(path, _capi.i32p)))
+        paths, w, r0 = [], 0, 0
+        for i in range(n):
+            paths.append([int(r) - r0 for r in path[w:w + acc[i] + 1]])
+            w += int(acc[i]) + 1
+            r0 += len(toks[i])
+        return nxt, acc, paths, logits
+
     def set_sampling(self, seq: int, args: "SamplingArgs | None"):
         """EXTENSION: sequence `seq` samples its next tokens with `args` (None or Temperature 0: greedy) from its next
         forward on; every token output of forward_argmax / forward_batch / forward_ragged / decode_run then carries the
